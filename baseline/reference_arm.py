@@ -1,10 +1,11 @@
 """The reference's own SuperPoint + LightGlue path for ``bench.py --impl reference`` (CPU) and the ``gpu_reference`` leg
-(eager PyTorch on the same B200, batch 1 - the bar BASELINE.md section 3 names).
+(eager PyTorch on the same GPU, batch 1 - the bar BASELINE.md section 3 names).
 
 Nothing of this repository's kernels, oracle or engine is on this path: the two model files are the reference's vendored
 ``thirdparty/SuperGluePretrainedNetwork/models/superpoint.py`` and ``thirdparty/LightGlue/lightglue/lightglue.py``, copied
-byte for byte into ``baseline/_ref/`` by :func:`stage` (run by ``__graft_entry__.build()`` in the authoring container, where
-``/root/reference`` exists; the directory is git-ignored and travels to the GPU box with the snapshot).  The reference
+byte for byte into the git-ignored ``baseline/_ref/`` by :func:`stage` from a checkout of the reference (they are the
+reference's files, not this project's, so they are not committed).  Without them ``bench.py --impl reference`` times the
+oracle port instead and says so in its JSON line.  The reference
 package itself cannot be imported or pip-installed here (h5py, kornia, rasterio, pydegensac, pycolmap are absent from the
 image and the wheelhouse), so the thin plugin adapters around the models are restated below, each citing the lines it
 follows; the models run unmodified with DIM's defaults (fp32 weights, ``flash=True``, ``mp=False``, cuDNN defaults).
@@ -23,7 +24,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REF_DIR = os.path.join(HERE, "_ref")
-SRC = "/root/reference/src/deep_image_matching/thirdparty/"
+SRC = "src/deep_image_matching/thirdparty/"  # inside a checkout of the reference
 FILES = {
     "superpoint.py": SRC + "SuperGluePretrainedNetwork/models/superpoint.py",
     "superpoint_v1.pth": SRC + "SuperGluePretrainedNetwork/models/weights/superpoint_v1.pth",
@@ -33,12 +34,12 @@ SP_CONF = {"name": "superpoint", "nms_radius": 3, "keypoint_threshold": 0.0005, 
            "fix_sampling": False}  # config.py:93-99 over SuperPointExtractor._default_conf (extractors/superpoint.py:84-91)
 
 
-def stage() -> bool:
-    """Copy the reference's model files into baseline/_ref/ (authoring container only). True if the arm is available."""
-    if os.path.isdir("/root/reference"):
+def stage(reference_root: str) -> bool:
+    """Copy the reference's model files from the checkout at `reference_root` into baseline/_ref/. True if the arm is available."""
+    if os.path.isdir(reference_root):
         os.makedirs(REF_DIR, exist_ok=True)
-        for name, src in FILES.items():
-            dst = os.path.join(REF_DIR, name)
+        for name, rel in FILES.items():
+            src, dst = os.path.join(reference_root, rel), os.path.join(REF_DIR, name)
             if not os.path.exists(dst) or os.path.getsize(dst) != os.path.getsize(src):
                 shutil.copyfile(src, dst)
     return available()
@@ -64,7 +65,7 @@ class ReferenceSPLG:
 
         import torch
         if not available():
-            raise FileNotFoundError("baseline/_ref/ is not staged (run __graft_entry__.build() where /root/reference exists)")
+            raise FileNotFoundError("baseline/_ref/ is not staged (baseline.reference_arm.stage(<checkout of the reference>))")
         self.torch, self.device = torch, torch.device(device)
         with warnings.catch_warnings():
             warnings.simplefilter("ignore")

@@ -1,13 +1,17 @@
 #!/usr/bin/env python
 """bench.py - headline benchmark: image-pairs/sec, SuperPoint+LightGlue, 1024x1024 synthetic, 2048 kpts
-(BASELINE.json configs[1]) on N B200s of one node.
+(BASELINE.json configs[1]) on N H100s of one node.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--pairs P] [--precision exact|fast]
+                  [--dump-outputs DIR]
 
 A step = one pass of the hot path over one batch of P independent synthetic pairs per rank: SuperPoint on the 2P
 images, LightGlue on the P pairs (independent-pair accounting of BASELINE.md: 2 extractions + 1 match per pair).
 `value` times the device-resident path (images already in HBM); `e2e` times the C-ABI call with HOST buffers
 (H2D of the images and D2H of the match tables inside the timed region).  Rank 0 prints ONE JSON line.
+--dump-outputs DIR writes what the last timed step computed (the six device-resident outputs of the pipe) as DIR/<name>.npy
+in float64, with the slots past each valid prefix (n_matches[p] matches, n_kpts[i] keypoints) set to zero; the inputs are seeded,
+so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -45,7 +49,7 @@ def lg_group_gflop(n=KPTS, d=D):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -81,7 +85,7 @@ def peaks():
         j = json.load(open(p))
         return {"tflops": j.get("bf16_tflops_sustained", j.get("bf16_tflops")), "hbm_gbs": j.get("hbm_gbs"),
                 "source": "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)"}
-    return {"tflops": 1400.0, "hbm_gbs": 6650.0, "source": "fallback of B200_PROFILING.md (sustained ~1.4 PFLOP/s)"}
+    return {"tflops": 989.0, "hbm_gbs": 3350.0, "source": "NVIDIA H100 SXM data sheet (dense FP16, 700 W card): not a measured rate"}
 
 
 def make_batches(P, nbatch, rank):
@@ -201,7 +205,7 @@ def run_reference(args, rank, world):
 
 def gpu_reference_pairs_per_s(n_pairs=12, fixed=True):
     """The "reference GPU" bar of BASELINE.md section 3: the reference's vendored PyTorch SuperPoint + LightGlue modules,
-    unmodified, eager at batch 1 on the same B200 with DIM's defaults (fp32 weights, flash=True -> fp16 SDPA, cuDNN defaults),
+    unmodified, eager at batch 1 on the same GPU with DIM's defaults (fp32 weights, flash=True -> fp16 SDPA, cuDNN defaults),
     driven per pair exactly like the serial loop of image_matching.py:413-494 (host image in, fp16 h5 round trip, host matches out)."""
     import torch
     from baseline import reference_arm as ra
@@ -470,7 +474,7 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--pairs", type=int, default=37, help="pairs per rank per step (37: every tile count is a multiple of the 148 SMs)")
+    ap.add_argument("--pairs", type=int, default=33, help="pairs per rank per step (33: every tile count is a multiple of the 132 SMs)")
     ap.add_argument("--precision", default="exact", choices=["exact", "fast"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-budget", type=float, default=0.0, help="seconds of CPU work for the CPU arms (default: 150 reference arm, 25 baseline leg)")
@@ -482,6 +486,8 @@ def main():
                          "nn = cfg5 (8192 x 256-d brute-force NN over sequential pairs), tiled = cfg3 (ALIKED 4 tiles / image + LightGlue 4096^2)")
     ap.add_argument("--images", type=int, default=0, help="images of the secondary modes (default 100 / 200 / 8)")
     ap.add_argument("--lg-mode", default="fixed", choices=["fixed", "adaptive"])
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float64, zero past the valid prefix; mode pairs)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
@@ -516,6 +522,22 @@ def main():
 
     matches_t = torch.as_tensor(_DevArr(outs["matches"], (P, cap, 2), "<i8"), device="cuda")
     counts_t = torch.as_tensor(_DevArr(outs["n_matches"], (P,), "<i4"), device="cuda")
+    # what a caller of the device-resident path receives (dimb_pipe_outputs_dev): about 5 MB as float64 at the default size
+    dump_views = {"matches": matches_t, "mscores": torch.as_tensor(_DevArr(outs["mscores"], (P, cap), "<f4"), device="cuda"),
+                  "n_matches": counts_t, "stop": torch.as_tensor(_DevArr(outs["stop"], (P,), "<i4"), device="cuda"),
+                  "n_kpts": torch.as_tensor(_DevArr(outs["n_kpts"], (2 * P,), "<i4"), device="cuda"),
+                  "kpts": torch.as_tensor(_DevArr(outs["kpts"], (2 * P, cap, 2), "<f4"), device="cuda")}
+
+    def dump_outputs(dirname):
+        """The arrays of dump_views as float64; entries past the valid prefix hold whatever earlier steps left there: zeroed."""
+        os.makedirs(dirname, exist_ok=True)
+        arrs = {name: t.cpu().numpy().astype(np.float64) for name, t in dump_views.items()}
+        slot = np.arange(cap)
+        arrs["matches"][slot[None, :] >= arrs["n_matches"][:, None]] = 0
+        arrs["mscores"][slot[None, :] >= arrs["n_matches"][:, None]] = 0
+        arrs["kpts"][slot[None, :] >= arrs["n_kpts"][:, None]] = 0
+        for name, a in arrs.items():
+            np.save(os.path.join(dirname, name + ".npy"), a)
     gathered = [torch.zeros_like(matches_t) for _ in range(world)] if (world > 1 and rank == 0) else None
     gathered_n = [torch.zeros_like(counts_t) for _ in range(world)] if (world > 1 and rank == 0) else None
 
@@ -549,6 +571,8 @@ def main():
         step_dev(i)
     e1.record()
     barrier()
+    if args.dump_outputs and rank == 0:  # before anything else runs the pipe again
+        dump_outputs(args.dump_outputs)
     launches = ctx.launches - l0
     ms = torch.tensor([e0.elapsed_time(e1)], device="cuda")
     per_rank_ms = [float(ms) / args.steps]
@@ -614,7 +638,7 @@ def main():
         "config": {"workload": "cfg2: superpoint+lightglue 1024x1024 2048 kpts, independent pairs (2 extractions + 1 match)",
                    "pairs_per_step_per_gpu": P, "lg_mode": "fixed-work (depth=-1,width=-1: all 9 layers, no pruning)",
                    "precision": args.precision, "weights": "superpoint_v1 + seeded LightGlue-architecture weights",
-                   "l2": "working set per step (>5 GB of activations) exceeds the 126 MB L2; inputs rotate over 3 batches"},
+                   "l2": "working set per step (>5 GB of activations) exceeds the 50 MB L2; inputs rotate over 3 batches"},
         "e2e": {"value": e2e_value, "unit": "pairs/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                 "api": "dimb_pipe_match_image_pairs (host float32 images in, host match tables out, pinned host memory)",
                 "timing": "host clock around the blocking C-ABI calls (each returns after its D2H copy completed), max over ranks",
@@ -648,14 +672,7 @@ def main():
         for g in groups.values():
             g["share"] = g["ms_per_step"] / total
         dom = max((n for n in groups if groups[n]["tflops_algorithmic"]), key=lambda n: groups[n]["ms_per_step"])
-        traffic, traffic_src = None, None  # DRAM bytes per launch of the dominant kernel: ncu --set full capture of THIS build
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")))
-            if dom in tj and "dram_bytes_per_image" in tj[dom]:
-                traffic = tj[dom]["dram_bytes_per_image"] * B
-                traffic_src = tj[dom].get("source")
-        except Exception:
-            pass
+        traffic, traffic_src = None, None  # DRAM bytes per launch of the dominant kernel: not measured
         result["roofline"] = {"bound": "tensor", "kernel": dom, "achieved": groups[dom]["tflops_algorithmic"], "peak": pk["tflops"],
                               "unit": "TFLOP/s", "frac": groups[dom]["tflops_algorithmic"] / pk["tflops"], "traffic": traffic, "traffic_source": traffic_src,
                               "executed_tflops": (3 if args.precision == "exact" else 1) * groups[dom]["tflops_algorithmic"],
@@ -700,9 +717,8 @@ def main():
                 result["fast_secondary"] = {
                     "value": P * 10 / (f0.elapsed_time(f1) / 1e3), "unit": "pairs/s (1 GPU)", "dtype": "f16 MMA, f32 accumulate",
                     "within_tolerance": False,
-                    "note": "same kernels with the lo planes dropped - what the reference's own TF32 / fp16 GPU path amounts to; against the "
-                            "fp32 oracle: 99.7-99.9 % identical keypoints, 99.9-100 % identical matches, |dscore| up to 9e-3 "
-                            "(tests/test_fast_mode.py, profiles/r1_fast_mode_report.json)"}
+                    "note": "same kernels with the lo planes dropped - what the reference's own TF32 / fp16 GPU path amounts to; "
+                            "its agreement with the fp32 oracle is checked by tests/test_fast_mode.py"}
             except Exception as e:
                 result["fast_secondary"] = {"error": str(e)[:200]}
             finally:
@@ -716,7 +732,7 @@ def main():
                                                        "one image / one pair per call as image_matching.py:413-494 does"}
             except Exception as e:
                 result["e2e"]["plugin_loop"] = {"error": str(e)[:200]}
-            # ---------------- "reference GPU" bar: the reference's torch modules, eager, batch 1, same B200
+            # ---------------- "reference GPU" bar: the reference's torch modules, eager, batch 1, same GPU
             try:
                 from baseline import reference_arm as ra
                 if ra.available():

@@ -155,7 +155,7 @@ _selftest = None
 
 
 def load_selftest_library():
-    """libdimb200_selftest.so: the production GEMM template behind a C = A B^T entry plus the UMMA descriptor probes.
+    """libdimb200_selftest.so: the production GEMM template behind a C = A B^T entry and the host drive of the RANSAC arithmetic.
     Test / tool infrastructure - the product library exports none of it.  Its context is its own (dimb_ctx_create of
     THIS library); never mix handles of the two libraries."""
     global _selftest
@@ -172,22 +172,19 @@ def load_selftest_library():
         lib.dimb_last_error.restype = C.c_char_p
         lib.dimb_ctx_set_precision.argtypes = [vp, ip]
         lib.dimb_selftest_gemm.argtypes = [vp, vp, vp, vp, ip, ip, ip, ip]
-        lib.dimb_probe_rowshift.argtypes = [vp, vp, vp, vp, ip, ip, ip, ip]
-        lib.dimb_probe_rowshift64.argtypes = [vp, vp, vp, vp, ip, ip, ip]
-        lib.dimb_probe_tmem_a.argtypes = [vp, vp, vp, vp]
         lib.dimb_gv_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_uint, vp, vp]
         _selftest = lib
     return _selftest
 
 
 class SelfTest:
-    """Context of the self-test library (tests/test_gpu_parity.py::test_tensor_core_gemm, tools/probe_umma_rowshift.py)."""
+    """Context of the self-test library (tests/test_gpu_parity.py::test_tensor_core_gemm)."""
 
     def __init__(self, device: int = 0):
         self.lib = load_selftest_library()
         h = C.c_void_p()
         if self.lib.dimb_ctx_create(device, C.byref(h)) != OK:
-            raise DimbError("selftest: dimb_ctx_create failed (a B200 is required)")
+            raise DimbError("selftest: dimb_ctx_create failed (an H100 is required)")
         self.h = h
 
     def check(self, rc, what):
@@ -228,7 +225,7 @@ class Context:
         rc = self.lib.dimb_ctx_create(device, C.byref(h))
         if rc != OK:
             raise DimbError(f"dimb_ctx_create(device={device}) failed with code {rc}: a CUDA device of compute "
-                            "capability 10.x (B200, sm_100a) is required; there is no CPU fallback")
+                            "capability 9.x (H100, sm_90a) is required; there is no CPU fallback")
         self.h = h
         self.device = device
         if precision is not None:

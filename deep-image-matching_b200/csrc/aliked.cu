@@ -131,164 +131,6 @@ __global__ void __launch_bounds__(128) al_conv3x3_kernel(const float* __restrict
   }
 }
 
-// ------------------------------------------------------------------ 3x3 conv of blocks 1-2 on the tensor cores
-// The 3 / 16 / 32-channel layers at full and half resolution are 6 of the network's 10.5 GMAC and were its slowest part on the CUDA
-// cores (0.75 ms of 2.3 per tile).  Here each is an im2col GEMM per 8 x 16-pixel tile: A = [128 pixels x K], K = Cin * 9 (index ci*9 +
-// tap, the weight order) padded to 32-wide blocks, written by the CTA's threads as fp16 hi / lo planes into SWIZZLE_64B K-major tiles
-// (the operand layout of gemm.cuh CONV 2 / conv_pair.cuh) from a shared-memory halo patch; B = the layer's weights, packed on the host
-// into the same layout and copied into shared memory once per CTA; D = [128 x Cout] fp32 in TMEM from three MMAs per 16-deep k-step
-// (hi.hi + hi.lo + lo.hi: fp32-class, the EXACT arithmetic of every other tensor-core layer).  The epilogue applies the folded BatchNorm,
-// residual and SELU and stores planar fp32 (thread = pixel: coalesced along x).  Persistent CTAs, one tile at a time (patch -> im2col ->
-// MMA -> drain); two CTAs per SM overlap each other's phases where shared memory allows.
-template <int CIN>
-struct AlTc {
-  static constexpr int K = CIN * 9, KB = (K + 31) / 32;  // 32-wide K blocks (64-byte rows)
-  static constexpr int kABlock = 128 * 64;                // one plane of one K block of the A tile
-  static constexpr int kPatch = 10 * 18 * CIN;            // floats of the (8+2) x (16+2) halo patch
-};
-constexpr int kAlTcThreads = 256;
-
-// packs [Cout][Cin*9] fp32 weights -> [KB][plane][Cout rows x 64 B] fp16, 16-byte chunks XOR-swizzled by (row >> 1) & 3
-static void al_pack_tc_weights(const float* w, int cout, int cin, std::vector<__half>& out) {
-  const int K = cin * 9, KB = (K + 31) / 32;
-  out.assign(static_cast<size_t>(KB) * 2 * cout * 32, __float2half_rn(0.f));
-  for (int kb = 0; kb < KB; ++kb)
-    for (int r = 0; r < cout; ++r)
-      for (int kk = 0; kk < 32; ++kk) {
-        const int k = kb * 32 + kk;
-        if (k >= K) continue;
-        const float v = w[static_cast<size_t>(r) * K + k];
-        const __half h = __float2half_rn(v), l = __float2half_rn(v - __half2float(h));
-        const int chunk = (kk >> 3) ^ ((r >> 1) & 3);
-        const size_t o = (static_cast<size_t>(kb) * 2 * cout + r) * 32 + chunk * 8 + (kk & 7);
-        out[o] = h;
-        out[o + static_cast<size_t>(cout) * 32] = l;
-      }
-}
-
-// chunks [HALF * NCH / 2, (HALF + 1) * NCH / 2) of one im2col row: 8 consecutive K values each (k = ci * 9 + tap -> patch[ci][ty][tx]), split
-// into fp16 hi / lo and stored as one 16-byte piece per plane at the SWIZZLE_64B position of the chunk
-template <int CIN, int HALF>
-__device__ __forceinline__ void al_im2col_part(const float* __restrict__ pb /*patch + py * 18 + px*/, uint8_t* __restrict__ rowA, uint32_t sw) {
-  using G = AlTc<CIN>;
-  constexpr int NCH = (G::K + 7) / 8, C0 = HALF * (NCH / 2), C1 = HALF ? NCH : NCH / 2;
-#pragma unroll
-  for (int ch = C0; ch < C1; ++ch) {
-    __half2 h[4], l[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int k0 = ch * 8 + 2 * j, k1 = k0 + 1;
-      const float a = k0 < G::K ? pb[(k0 / 9) * 180 + ((k0 % 9) / 3) * 18 + (k0 % 9) % 3] : 0.f;
-      const float b = k1 < G::K ? pb[(k1 / 9) * 180 + ((k1 % 9) / 3) * 18 + (k1 % 9) % 3] : 0.f;
-      split2_f32(a, b, h[j], l[j]);
-    }
-    const uint32_t off = static_cast<uint32_t>(ch >> 2) * 2u * G::kABlock + (((static_cast<uint32_t>(ch) & 3u) ^ sw) << 4);
-    *reinterpret_cast<uint4*>(rowA + off) = *reinterpret_cast<uint4*>(h);
-    *reinterpret_cast<uint4*>(rowA + off + G::kABlock) = *reinterpret_cast<uint4*>(l);
-  }
-}
-
-template <int CIN, int COUT>
-__global__ void __launch_bounds__(kAlTcThreads) al_conv3x3_tc_kernel(const float* __restrict__ in, int H, int W, const __half* __restrict__ wtc,
-                                                                     const float* __restrict__ alpha, const float* __restrict__ beta,
-                                                                     const float* __restrict__ resid, float* __restrict__ out, int act,
-                                                                     int tiles_x, int n_tiles) {
-  using namespace tc05;
-  using G = AlTc<CIN>;
-  constexpr int KB = G::KB, kWBlock = COUT * 64;  // bytes of one plane of one K block of the weights
-  extern __shared__ uint8_t altc_raw[];
-  uint8_t* sm = altc_raw + ((1024u - (smem_u32(altc_raw) & 1023u)) & 1023u);
-  uint8_t* sA = sm;                                   // [KB][plane][128 x 64 B]
-  uint8_t* sW = sA + KB * 2 * G::kABlock;             // [KB][plane][COUT x 64 B]
-  float* patch = reinterpret_cast<float*>(sW + KB * 2 * kWBlock);  // [CIN][10][18]
-  uint64_t* bar = reinterpret_cast<uint64_t*>(patch + G::kPatch);
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bar + 1);
-  const int tid = threadIdx.x, warp = tid >> 5;
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) tmem_alloc(tmem_ptr, 32);
-  for (int i = tid; i < KB * 2 * kWBlock / 16; i += kAlTcThreads) reinterpret_cast<uint4*>(sW)[i] = reinterpret_cast<const uint4*>(wtc)[i];
-  // K columns beyond Cin * 9 of the last block stay zero for the whole kernel
-  for (int i = tid; i < KB * 2 * G::kABlock / 16; i += kAlTcThreads) reinterpret_cast<uint4*>(sA)[i] = make_uint4(0u, 0u, 0u, 0u);
-  fence_proxy_async_smem();
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = *tmem_ptr;
-  const size_t P = static_cast<size_t>(H) * W;
-  constexpr uint32_t idesc = make_idesc_f16(COUT);
-  uint32_t phase = 0;
-  for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-    const int y0 = (t / tiles_x) * 8, x0 = (t % tiles_x) * 16;
-    for (int e = tid; e < G::kPatch; e += kAlTcThreads) {
-      const int c = e / 180, rem = e - c * 180, yy = rem / 18, xx = rem - yy * 18;
-      const int gy = y0 + yy - 1, gx = x0 + xx - 1;
-      patch[e] = (gy >= 0 && gy < H && gx >= 0 && gx < W) ? in[c * P + static_cast<size_t>(gy) * W + gx] : 0.f;
-    }
-    __syncthreads();
-    {  // im2col: thread = (pixel, half of the 16-byte K chunks); K index = ci * 9 + tap.  Every index below is a compile-time constant
-       // of the fully unrolled loops (the first cut computed k / 9, k % 9 at run time: 44 instructions per element, tensor pipe 2 %)
-      const int r = tid & 127;
-      const float* pb = patch + (r >> 4) * 18 + (r & 15);
-      const uint32_t sw = (static_cast<uint32_t>(r) >> 1) & 3u;
-      uint8_t* rowA = sA + static_cast<uint32_t>(r) * 64u;
-      if (tid < 128) al_im2col_part<CIN, 0>(pb, rowA, sw);
-      else al_im2col_part<CIN, 1>(pb, rowA, sw);
-    }
-    fence_proxy_async_smem();
-    __syncthreads();
-    if (warp == 4) {  // one elected lane issues the tile's MMAs
-      tc_fence_after_sync();
-      if (elect_one()) {
-#pragma unroll
-        for (int kb = 0; kb < KB; ++kb) {
-          const uint32_t a = smem_u32(sA + kb * 2 * G::kABlock), b = smem_u32(sW + kb * 2 * kWBlock);
-          const uint64_t ah = make_sdesc(a, 512, kLayoutSw64), al = make_sdesc(a + G::kABlock, 512, kLayoutSw64);
-          const uint64_t bh = make_sdesc(b, 512, kLayoutSw64), bl = make_sdesc(b + kWBlock, 512, kLayoutSw64);
-#pragma unroll
-          for (int k16 = 0; k16 < 2; ++k16) {
-            if (kb * 32 + k16 * 16 >= G::K) break;  // a 16-deep step that is all padding
-            mma_f16_ss(tmem, sdesc_advance_k(ah, k16), sdesc_advance_k(bh, k16), idesc, (kb | k16) != 0);
-            mma_f16_ss(tmem, sdesc_advance_k(ah, k16), sdesc_advance_k(bl, k16), idesc, 1);
-            mma_f16_ss(tmem, sdesc_advance_k(al, k16), sdesc_advance_k(bh, k16), idesc, 1);
-          }
-        }
-        mma_commit(bar);
-      }
-      __syncwarp();
-    }
-    if (warp < 4) {  // drain: thread = pixel = TMEM lane
-      mbar_wait(bar, phase);
-      tc_fence_after_sync();
-      float v[32];
-      if (COUT == 32) tmem_ld32(tmem + (static_cast<uint32_t>(warp * 32) << 16), v);
-      else tmem_ld16(tmem + (static_cast<uint32_t>(warp * 32) << 16), v);
-      tmem_ld_wait();
-      tc_fence_before_sync();
-      const int r = tid, y = y0 + (r >> 4), x = x0 + (r & 15);
-      if (y < H && x < W) {
-        const size_t o = static_cast<size_t>(y) * W + x;
-#pragma unroll
-        for (int co = 0; co < COUT; ++co) {
-          float q = v[co] * alpha[co] + beta[co];
-          if (resid) q += resid[co * P + o];
-          out[co * P + o] = act_f(q, act);
-        }
-      }
-    }
-    phase ^= 1;
-    __syncthreads();  // TMEM drained, patch and A tile free: next tile
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem, 32);
-  }
-}
-
 // 1x1 conv: out[co][p] = act(sum_ci w[co][ci] in[ci][p] + b[co]); thread per pixel, 16 output channels per blockIdx.y
 __global__ void __launch_bounds__(256) al_conv1x1_kernel(const float* __restrict__ in, int Cin, size_t P, const float* __restrict__ w,
                                                          const float* __restrict__ bias, float* __restrict__ out, int Cout, int act) {
@@ -720,7 +562,6 @@ __global__ void __launch_bounds__(1024) al_threshold_kernel(const float* __restr
 struct BnConv {
   float *w = nullptr, *alpha = nullptr, *beta = nullptr;
   int cin = 0, cout = 0;
-  __half* wtc = nullptr;  // blocks 1-2: the weights as the B operand of al_conv3x3_tc_kernel, laid out exactly as they sit in shared memory
 };
 
 }  // namespace
@@ -793,12 +634,6 @@ int make_bnconv(dimb_ctx* ctx, BnConv& c, const float*& p, int cout, int cin, bo
     DIMB_TRY(up_f32(ctx, &c.w, wt.data(), wt.size()));
   } else {
     DIMB_TRY(up_f32(ctx, &c.w, p, static_cast<size_t>(cout) * cin * 9));
-    if ((cin == 3 || cin == 16 || cin == 32) && (cout == 16 || cout == 32)) {  // blocks 1-2: also as the tensor-core B operand
-      std::vector<__half> pk;
-      al_pack_tc_weights(p, cout, cin, pk);
-      DIMB_TRY(dimb_alloc_t(ctx, &c.wtc, pk.size(), false));
-      DIMB_CUDA_OK(ctx, cudaMemcpy(c.wtc, pk.data(), pk.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    }
   }
   p += static_cast<size_t>(cout) * cin * 9;
   const float *g = p, *b = p + cout, *m = p + 2 * cout, *v = p + 3 * cout;
@@ -814,29 +649,8 @@ int make_bnconv(dimb_ctx* ctx, BnConv& c, const float*& p, int cout, int cin, bo
   return DIMB_OK;
 }
 
-template <int CIN, int COUT>
-int conv3_tc(dimb_ctx* ctx, cudaStream_t st, const float* in, int H, int W, const __half* wtc, const float* alpha, const float* beta,
-             const float* resid, float* out, int act) {
-  using G = AlTc<CIN>;
-  const int smem = G::KB * 2 * (G::kABlock + COUT * 64) + G::kPatch * 4 + 64 + 1024;
-  auto kern = al_conv3x3_tc_kernel<CIN, COUT>;
-  DIMB_TRY(dimb_func_smem(ctx, kern, smem));
-  const int tiles_x = ceil_div(W, 16), n_tiles = tiles_x * ceil_div(H, 8);
-  const int per_sm = smem > 113 * 1024 ? 1 : 2;
-  const int grid = std::min(n_tiles, ctx->num_sms * per_sm);
-  kern<<<grid, kAlTcThreads, smem, st>>>(in, H, W, wtc, alpha, beta, resid, out, act, tiles_x, n_tiles);
-  DIMB_LAUNCH_CHECK(ctx);
-  return DIMB_OK;
-}
-
 int conv3(dimb_ctx* ctx, cudaStream_t st, const float* in, int cin, int H, int W, const float* w, const float* alpha, const float* beta,
-          const float* resid, float* out, int cout, int act, const __half* wtc = nullptr) {
-  if (wtc && alpha && beta && ctx->use_tc && ctx->al_tc) {  // blocks 1-2 on the tensor cores (al_conv3x3_tc_kernel); DIMB_AL_TC=0: CUDA cores
-    if (cin == 3 && cout == 16) return conv3_tc<3, 16>(ctx, st, in, H, W, wtc, alpha, beta, resid, out, act);
-    if (cin == 16 && cout == 16) return conv3_tc<16, 16>(ctx, st, in, H, W, wtc, alpha, beta, resid, out, act);
-    if (cin == 16 && cout == 32) return conv3_tc<16, 32>(ctx, st, in, H, W, wtc, alpha, beta, resid, out, act);
-    if (cin == 32 && cout == 32) return conv3_tc<32, 32>(ctx, st, in, H, W, wtc, alpha, beta, resid, out, act);
-  }
+          const float* resid, float* out, int cout, int act) {
   if (static_cast<size_t>(H) * W <= 64 * 64) {  // low-resolution maps: small tiles so that the grid still fills the SMs
     dim3 grid(ceil_div(W, 16), ceil_div(H, 8), ceil_div(cout, 8));
     al_conv3x3_kernel<8, 1><<<grid, 128, 0, st>>>(in, cin, H, W, w, alpha, beta, resid, out, cout, act);
@@ -1039,16 +853,16 @@ int dimb_aliked_extract_dev(dimb_aliked* al, const float* image, int H, int W, i
     al_pad_kernel<<<dim3(ceil_div(Wp, 128), Hp, 3), 128, 0, st>>>(image, H, W, channels, al->pad, Hp, Wp, top, left);
     DIMB_LAUNCH_CHECK(ctx);
     // block1
-    DIMB_TRY(conv3(ctx, st, al->pad, 3, Hp, Wp, al->b1c1.w, al->b1c1.alpha, al->b1c1.beta, nullptr, al->t1a, 16, 1, al->b1c1.wtc));
-    DIMB_TRY(conv3(ctx, st, al->t1a, 16, Hp, Wp, al->b1c2.w, al->b1c2.alpha, al->b1c2.beta, nullptr, al->x1, 16, 1, al->b1c2.wtc));
+    DIMB_TRY(conv3(ctx, st, al->pad, 3, Hp, Wp, al->b1c1.w, al->b1c1.alpha, al->b1c1.beta, nullptr, al->t1a, 16, 1));
+    DIMB_TRY(conv3(ctx, st, al->t1a, 16, Hp, Wp, al->b1c2.w, al->b1c2.alpha, al->b1c2.beta, nullptr, al->x1, 16, 1));
   }
   {
     ProfScope prof(ctx, st, "al.block2");  // ResBlock, regular convs
     al_avgpool_kernel<<<static_cast<unsigned>((P / 4 * 16 + 255) / 256), 256, 0, st>>>(al->x1, 16, Hp, Wp, 2, al->p2);
     DIMB_LAUNCH_CHECK(ctx);
-    DIMB_TRY(conv3(ctx, st, al->p2, 16, H2, W2, al->b2c1.w, al->b2c1.alpha, al->b2c1.beta, nullptr, al->t2a, 32, 1, al->b2c1.wtc));
+    DIMB_TRY(conv3(ctx, st, al->p2, 16, H2, W2, al->b2c1.w, al->b2c1.alpha, al->b2c1.beta, nullptr, al->t2a, 32, 1));
     DIMB_TRY(conv1(ctx, st, al->p2, 16, P / 4, al->b2dw, al->b2db, al->sc2, 32, 0));
-    DIMB_TRY(conv3(ctx, st, al->t2a, 32, H2, W2, al->b2c2.w, al->b2c2.alpha, al->b2c2.beta, al->sc2, al->x2, 32, 1, al->b2c2.wtc));
+    DIMB_TRY(conv3(ctx, st, al->t2a, 32, H2, W2, al->b2c2.w, al->b2c2.alpha, al->b2c2.beta, al->sc2, al->x2, 32, 1));
   }
   {
     ProfScope prof(ctx, st, "al.block3");  // deformable

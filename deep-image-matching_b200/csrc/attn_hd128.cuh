@@ -2,26 +2,16 @@
 // LightGlue path (lightglue_generic.cu).  Attention is 93 % of LighterGlue's arithmetic (19.3 of 20.7 GMAC per 2048 x 2048 pair); the
 // linears stay on the plain fp32 kernels.
 //
-// Same scheme as lg_attn5_kernel (lg_kernels.cuh): S = Q K^T one 64-key block ahead in TMEM, online softmax with lazy rescaling by the
-// thread that owns the query row (= TMEM lane), P written back as fp16 hi / lo words into the TMEM columns its scores came from, O += P V
-// with the A operand read from tensor memory, O resident in TMEM for the whole key loop.  Differences forced by the wider head:
-//   * head dim padded to 128 (zero columns): Q / K tiles are two SWIZZLE_128B atoms side by side (8 k-steps for S), V^T tile = 128 rows
-//     (N = 128 for P V), O = 128 TMEM columns;
-//   * ONE query tile (128 rows) per CTA: Q 64 KB + two K / V^T stages of 64 KB = 192 KB of shared memory in EXACT mode;
-//   * TMEM: two 64-column S / P slots + O = 256 columns.  S(j+1) overwrites the slot of P(j-1) only after P V(j-1), which the same thread
-//     issued earlier (MMAs retire in issue order) - no "slot free" barrier.
-// Inputs are packed by gx_pack_rows_kernel / gx_pack_vt_kernel from the fp32 activations of the generic path; the result is written as
-// fp32 rows.  EXACT mode = fp16 hi / lo planes, three MMAs per product (fp32-class); FAST = hi plane only.
+// The kernel is attention.cuh's with the head dim padded to 128 (zero columns): Q / K tiles are two SWIZZLE_128B atoms side by side,
+// the V^T tile has 128 rows.  Inputs are packed by gx_pack_rows_kernel / gx_pack_vt_kernel from the fp32 activations of the generic
+// path; the result is written as fp32 rows.  EXACT mode = fp16 hi / lo planes, three MMAs per product (fp32-class); FAST = hi plane only.
 #pragma once
+#include "attention.cuh"
 #include "common.cuh"
-#include "tc05.cuh"
 
 namespace {
 
 constexpr int kXHd = 128;   // padded head dim
-constexpr int kXBlk = 64;   // keys per block
-constexpr int kXTile = 128; // queries per CTA
-constexpr int kXStages = 2;
 
 struct AttnXArgs {
   int nq, nk;       // live queries / keys
@@ -66,261 +56,42 @@ __global__ void gx_pack_vt_kernel(const float* __restrict__ src, int ld, int n, 
   }
 }
 
-// grid (ceil(nq / 128), H); 192 threads: warps 0-3 softmax (thread = query row), warp 4 TMA producer, warp 5 MMA issuer
+struct AttnOutX {  // O rows of one head -> fp32 [nq][ldo], head h at columns h * hd; padding columns >= hd dropped
+  float* out;
+  int ldo, hd;
+  __device__ void operator()(int row, int col, float x, float y) const {
+    float* dst = out + static_cast<size_t>(row) * ldo + col;
+    if (col < hd) dst[0] = x;
+    if (col + 1 < hd) dst[1] = y;
+  }
+};
+
+// grid (ceil(nq / 128), H)
 template <bool SPLIT>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(kAttnThreads, 1)
 gx_attn_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
                   const __grid_constant__ CUtensorMap tmKh, const __grid_constant__ CUtensorMap tmKl,
                   const __grid_constant__ CUtensorMap tmVh, const __grid_constant__ CUtensorMap tmVl, AttnXArgs a) {
-  using namespace tc05;
-  const int head = blockIdx.y, qbase = blockIdx.x * kXTile, NP = a.NP, nq = a.nq, nk = a.nk;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  if (qbase >= nq) return;
-  if (nk == 0) {  // Attention.forward: empty key set -> zeros (lightglue.py:103-104)
-    if (warp < 4 && qbase + tid < nq)
-      for (int c = 0; c < a.hd; ++c) a.out[static_cast<size_t>(qbase + tid) * a.ldo + head * a.hd + c] = 0.f;
-    return;
-  }
-  constexpr int kPl = SPLIT ? 2 : 1, KST = kXStages;
-  constexpr int kAtomQ = kXTile * 128, kQB = 2 * kAtomQ;  // Q plane: two [128 x 64] atoms
-  constexpr int kAtomK = kXBlk * 128, kKB = 2 * kAtomK;   // K plane of a stage: two [64 x 64] atoms
-  constexpr int kVB = kXHd * 128;                         // V^T plane of a stage: [128 dims x 64 keys]
-  extern __shared__ uint8_t smx_raw[];
-  uint8_t* smx = smx_raw + ((1024u - (smem_u32(smx_raw) & 1023u)) & 1023u);
-  uint8_t* sQ = smx;                          // [plane]
-  uint8_t* sK = sQ + kPl * kQB;               // [stage][plane]
-  uint8_t* sV = sK + KST * kPl * kKB;         // [stage][plane]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + KST * kPl * kVB);
-  uint64_t *bQ = bars, *kFull = bQ + 1, *kEmpty = kFull + KST, *vFull = kEmpty + KST, *vEmpty = vFull + KST, *bS = vEmpty + KST /*[2]*/,
-           *pReady = bS + 2, *bO = pReady + 1;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bO + 1);
-  if (tid == 0) {
-    mbar_init(bQ, 1);
-    mbar_init(pReady, kXTile);
-    mbar_init(bO, 1);
-    for (int i = 0; i < KST; ++i) {
-      mbar_init(&kFull[i], 1);
-      mbar_init(&kEmpty[i], 1);
-      mbar_init(&vFull[i], 1);
-      mbar_init(&vEmpty[i], 1);
-    }
-    mbar_init(&bS[0], 1);
-    mbar_init(&bS[1], 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) tmem_alloc(tmem_ptr, 256);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr;  // slots at +0 / +64, O at +128
-  const int krow = head * NP, vrow = head * kXHd;
-  const int nblk = (nk + kXBlk - 1) / kXBlk;
-
-  if (warp == 4) {  // ---------------- TMA producer (whole warp waits, one elected lane issues)
-    if (elect_one()) {
-      const int qrow = head * NP + qbase;
-      mbar_expect_tx(bQ, kPl * kQB);
-      for (int at = 0; at < 2; ++at) {
-        tma_load_2d(sQ + at * kAtomQ, &tmQh, bQ, at * 64, qrow);
-        if (SPLIT) tma_load_2d(sQ + kQB + at * kAtomQ, &tmQl, bQ, at * 64, qrow);
-      }
-    }
-    __syncwarp();
-    for (int j = 0; j < nblk; ++j) {
-      const int s = j % KST;
-      const uint32_t ph = (j / KST) & 1;
-      mbar_wait(&kEmpty[s], ph ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&kFull[s], kPl * kKB);
-        for (int at = 0; at < 2; ++at) {
-          tma_load_2d(sK + s * kPl * kKB + at * kAtomK, &tmKh, &kFull[s], at * 64, krow + j * kXBlk);
-          if (SPLIT) tma_load_2d(sK + s * kPl * kKB + kKB + at * kAtomK, &tmKl, &kFull[s], at * 64, krow + j * kXBlk);
-        }
-      }
-      __syncwarp();
-      mbar_wait(&vEmpty[s], ph ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&vFull[s], kPl * kVB);
-        tma_load_2d(sV + s * kPl * kVB, &tmVh, &vFull[s], j * kXBlk, vrow);
-        if (SPLIT) tma_load_2d(sV + s * kPl * kVB + kVB, &tmVl, &vFull[s], j * kXBlk, vrow);
-      }
-      __syncwarp();
-    }
-  } else if (warp == 5) {  // ---------------- MMA issuer: the whole warp waits, one elected lane issues
-    constexpr uint32_t idescS = make_idesc_f16(kXBlk), idescO = make_idesc_f16(kXHd);
-    const uint32_t q = smem_u32(sQ);
-    const uint32_t dO = tmem_base + 128;
-    auto issue_S = [&](int j) {
-      const int s = j % KST;
-      const uint32_t d = tmem_base + (j & 1) * 64;
-      const uint32_t k = smem_u32(sK + s * kPl * kKB);
-      if (elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {  // 128 padded dims = 2 atoms x 4 k-steps
-          const uint64_t qh = sdesc_advance_k(make_sdesc_sw128(q + (kk >> 2) * kAtomQ), kk & 3);
-          const uint64_t kh = sdesc_advance_k(make_sdesc_sw128(k + (kk >> 2) * kAtomK), kk & 3);
-          mma_f16_ss(d, qh, kh, idescS, kk != 0);
-          if (SPLIT) {
-            const uint64_t ql = sdesc_advance_k(make_sdesc_sw128(q + kQB + (kk >> 2) * kAtomQ), kk & 3);
-            const uint64_t kl = sdesc_advance_k(make_sdesc_sw128(k + kKB + (kk >> 2) * kAtomK), kk & 3);
-            mma_f16_ss(d, qh, kl, idescS, 1);
-            mma_f16_ss(d, ql, kh, idescS, 1);
-          }
-        }
-        mma_commit(&bS[j & 1]);
-        mma_commit(&kEmpty[s]);
-      }
-      __syncwarp();
-    };
-    mbar_wait(bQ, 0);
-    mbar_wait(&kFull[0], 0);
-    tc_fence_after_sync();
-    issue_S(0);
-    for (int j = 0; j < nblk; ++j) {
-      if (j + 1 < nblk) {  // next block's scores into the slot of P(j-1): P V(j-1) was issued one iteration ago
-        mbar_wait(&kFull[(j + 1) % KST], ((j + 1) / KST) & 1);
-        tc_fence_after_sync();
-        issue_S(j + 1);
-      }
-      const int sb = j % KST;
-      mbar_wait(&vFull[sb], (j / KST) & 1);
-      mbar_wait(pReady, j & 1);
-      tc_fence_after_sync();
-      const uint32_t vv = smem_u32(sV + sb * kPl * kVB);
-      const uint64_t v_h = make_sdesc_sw128(vv), v_l = make_sdesc_sw128(vv + kVB);
-      const uint32_t tP = tmem_base + (j & 1) * 64;  // hi words in columns [0, 32), lo words in [32, 64); 8 columns per 16 keys
-      if (elect_one()) {
-#pragma unroll
-        for (int k16 = 0; k16 < 4; ++k16) {
-          mma_f16_ts(dO, tP + k16 * 8, sdesc_advance_k(v_h, k16), idescO, (j | k16) != 0);
-          if (SPLIT) {
-            mma_f16_ts(dO, tP + k16 * 8, sdesc_advance_k(v_l, k16), idescO, 1);
-            mma_f16_ts(dO, tP + 32 + k16 * 8, sdesc_advance_k(v_h, k16), idescO, 1);
-          }
-        }
-        mma_commit(bO);
-        mma_commit(&vEmpty[sb]);
-      }
-      __syncwarp();
-    }
-  } else {  // ---------------- softmax warpgroup: thread = query row = TMEM lane
-    const int r = tid;
-    const uint32_t lane_off = static_cast<uint32_t>(warp * 32) << 16;
-    const uint32_t tS0 = tmem_base + lane_off, tO = tS0 + 128;
-    float m_run = -INFINITY, l_run = 0.f;
-    const float c2 = a.scale * 1.4426950408889634f;  // softmax(scale * s) via exp2
-    for (int j = 0; j < nblk; ++j) {
-      const int slot = j & 1;
-      mbar_wait(&bS[slot], (j >> 1) & 1);
-      tc_fence_after_sync();
-      float s[kXBlk];
-      tmem_ld32(tS0 + slot * 64, s);
-      tmem_ld32(tS0 + slot * 64 + 32, s + 32);
-      tmem_ld_wait();
-      const int key0 = j * kXBlk;
-      if (key0 + kXBlk > nk) {
-#pragma unroll
-        for (int c = 0; c < kXBlk; ++c)
-          if (key0 + c >= nk) s[c] = -INFINITY;
-      }
-      float mx[4] = {s[0], s[1], s[2], s[3]};
-#pragma unroll
-      for (int c = 4; c < kXBlk; c += 4) {
-        mx[0] = fmaxf(mx[0], s[c]);
-        mx[1] = fmaxf(mx[1], s[c + 1]);
-        mx[2] = fmaxf(mx[2], s[c + 2]);
-        mx[3] = fmaxf(mx[3], s[c + 3]);
-      }
-      const float m_blk = fmaxf(m_run, fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])));
-      const bool grow = (m_blk - m_run) * c2 > a.lazy;      // always true on the first block (m_run = -inf)
-      const float m_new = grow ? m_blk : m_run;
-      const float alpha = grow ? fast_exp2((m_run - m_new) * c2) : 1.f;  // 0 on the first block
-      const float mc = m_new * c2;
-      float2 ps[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
-      const float2 c22 = make_float2(c2, c2), mc2 = make_float2(-mc, -mc);
-#pragma unroll
-      for (int c = 0; c < kXBlk; c += 4) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {  // packed fp32 pairs: one FFMA2 + two MUFU + one FADD2 per two scores (same values, same summation order)
-          const float2 x = ffma2(make_float2(s[c + 2 * e], s[c + 2 * e + 1]), c22, mc2);
-          s[c + 2 * e] = fast_exp2(x.x);
-          s[c + 2 * e + 1] = fast_exp2(x.y);
-          ps[e] = fadd2(ps[e], make_float2(s[c + 2 * e], s[c + 2 * e + 1]));
-        }
-      }
-      l_run = l_run * alpha + ((ps[0].x + ps[0].y) + (ps[1].x + ps[1].y));
-      m_run = m_new;
-      {
-        __half2 ph[32], pl[32];
-#pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          const float2 p = make_float2(s[2 * c], s[2 * c + 1]);
-          ph[c] = __floats2half2_rn(p.x, p.y);
-          const float2 d = fsub2(p, __half22float2(ph[c]));  // exact residual (same values as split2_f32, one FADD2)
-          pl[c] = __floats2half2_rn(d.x, d.y);
-        }
-        tmem_st32(tS0 + slot * 64, reinterpret_cast<const float*>(ph));
-        if (SPLIT) tmem_st32(tS0 + slot * 64 + 32, reinterpret_cast<const float*>(pl));
-      }
-      if (j > 0) {
-        mbar_wait(bO, (j - 1) & 1);  // P V of the previous block retired: O is ours until P(j) is posted
-        tc_fence_after_sync();
-        if (__any_sync(0xffffffffu, alpha != 1.f)) {  // a row maximum moved: rescale the warp's O rows in TMEM
-          float o[32];
-#pragma unroll
-          for (int h = 0; h < kXHd / 32; ++h) {
-            tmem_ld32(tO + h * 32, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int d = 0; d < 32; ++d) o[d] *= alpha;
-            tmem_st32(tO + h * 32, o);
-          }
-        }
-      }
-      tmem_st_wait();
-      tc_fence_before_sync();
-      mbar_arrive(pReady);
-    }
-    mbar_wait(bO, (nblk - 1) & 1);
-    tc_fence_after_sync();
-    const int qi = qbase + r;
-    const float inv = 1.f / l_run;
-#pragma unroll
-    for (int h = 0; h < kXHd / 32; ++h) {
-      float o[32];
-      tmem_ld32(tO + h * 32, o);
-      tmem_ld_wait();
-      if (qi < nq) {
-        float* dst = a.out + static_cast<size_t>(qi) * a.ldo + head * a.hd + h * 32;
-#pragma unroll
-        for (int d = 0; d < 32; ++d)
-          if (h * 32 + d < a.hd) dst[d] = o[d] * inv;
-      }
-    }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 256);
-  }
+  const int head = blockIdx.y, qbase = blockIdx.x * kAttnTile;
+  if (qbase >= a.nq) return;
+  const AttnOutX out{a.out + static_cast<size_t>(qbase) * a.ldo + head * a.hd, a.ldo, a.hd};
+  attn_tile<kXHd, SPLIT>(&tmQh, &tmQl, &tmKh, &tmKl, &tmVh, &tmVl, head * a.NP + qbase, head * a.NP, head * kXHd, a.nq - qbase, a.nk,
+                         a.scale, a.lazy, out);
 }
-
-constexpr int kXSmemPlane = 2 * kXTile * 128 + kXStages * (2 * kXBlk * 128 + kXHd * 128);  // Q + stages x (K + V^T), per operand plane
 
 inline int launch_attn_hd128(dimb_ctx* ctx, cudaStream_t st, const CUtensorMap* Q /*[2] hi,lo, box 128 rows*/,
                              const CUtensorMap* K /*[2], box 64 rows*/, const CUtensorMap* V /*[2] V^T, box 128 rows*/, int heads,
                              const AttnXArgs& a, bool exact) {
   if (a.nq <= 0) return DIMB_OK;
-  dim3 grid((a.nq + kXTile - 1) / kXTile, heads);
+  dim3 grid((a.nq + kAttnTile - 1) / kAttnTile, heads);
   if (exact) {
-    const int smem = 2 * kXSmemPlane + 256 + 1024;
+    constexpr int smem = AttnGeom<kXHd, true>::kSmem;
     DIMB_TRY(dimb_func_smem(ctx, gx_attn_tc_kernel<true>, smem));
-    gx_attn_tc_kernel<true><<<grid, 192, smem, st>>>(Q[0], Q[1], K[0], K[1], V[0], V[1], a);
+    gx_attn_tc_kernel<true><<<grid, kAttnThreads, smem, st>>>(Q[0], Q[1], K[0], K[1], V[0], V[1], a);
   } else {
-    const int smem = kXSmemPlane + 256 + 1024;
+    constexpr int smem = AttnGeom<kXHd, false>::kSmem;
     DIMB_TRY(dimb_func_smem(ctx, gx_attn_tc_kernel<false>, smem));
-    gx_attn_tc_kernel<false><<<grid, 192, smem, st>>>(Q[0], Q[0], K[0], K[0], V[0], V[0], a);
+    gx_attn_tc_kernel<false><<<grid, kAttnThreads, smem, st>>>(Q[0], Q[0], K[0], K[0], V[0], V[0], a);
   }
   DIMB_LAUNCH_CHECK(ctx);
   return DIMB_OK;

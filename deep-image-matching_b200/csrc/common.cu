@@ -115,7 +115,7 @@ int dimb_tmap_2d(dimb_ctx* ctx, CUtensorMap* out, const __half* base, uint64_t r
   return DIMB_OK;
 }
 
-// 2-D map with boxes of 32 halfs (64-byte rows) x box_rows and SWIZZLE_64B: weights of the half-K-block convolution (gemm.cuh CONV 2)
+// 2-D map with boxes of 32 halfs (64-byte rows) x box_rows and SWIZZLE_64B: operands of the 32-wide K blocks (gemm.cuh CONV 3)
 int dimb_tmap_2d_sw64(dimb_ctx* ctx, CUtensorMap* out, const __half* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
   PFN_encodeTiled enc = get_encode(ctx);
   if (!enc) return DIMB_ERR_CUDA;
@@ -128,25 +128,6 @@ int dimb_tmap_2d_sw64(dimb_ctx* ctx, CUtensorMap* out, const __half* base, uint6
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     dimb_set_error(ctx, "cuTensorMapEncodeTiled(2d, 64B swizzle) failed: code " + std::to_string(int(r)));
-    return DIMB_ERR_CUDA;
-  }
-  return DIMB_OK;
-}
-
-// NHWC map with boxes of 32 channels (64-byte rows) x box_w x box_h and SWIZZLE_64B: halo boxes of gemm.cuh CONV 2
-int dimb_tmap_nhwc_sw64(dimb_ctx* ctx, CUtensorMap* out, const __half* base, uint64_t n, uint64_t h, uint64_t w, uint64_t c,
-                        uint32_t box_h, uint32_t box_w) {
-  PFN_encodeTiled enc = get_encode(ctx);
-  if (!enc) return DIMB_ERR_CUDA;
-  cuuint64_t dims[4] = {c, w, h, n};
-  cuuint64_t strides[3] = {c * sizeof(__half), w * c * sizeof(__half), h * w * c * sizeof(__half)};
-  cuuint32_t box[4] = {32, box_w, box_h, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    dimb_set_error(ctx, "cuTensorMapEncodeTiled(nhwc, 64B swizzle) failed: code " + std::to_string(int(r)));
     return DIMB_ERR_CUDA;
   }
   return DIMB_OK;
@@ -239,7 +220,7 @@ int dimb_read_dev(dimb_ctx* ctx, void* dst, const void* d_src, size_t bytes) {
   return DIMB_OK;
 }
 
-const char* dimb_version(void) { return "dimb200 0.1.0 (sm_100a)"; }
+const char* dimb_version(void) { return "dimb200 0.1.0 (sm_90a)"; }
 
 int dimb_ctx_create(int device, dimb_ctx** out) {
   if (!out) return DIMB_ERR_ARG;
@@ -253,33 +234,21 @@ int dimb_ctx_create(int device, dimb_ctx** out) {
     delete ctx;
     return DIMB_ERR_CUDA;
   }
-  if (prop.major != 10) {  // sm_100a cubins only: no compatibility path
+  if (prop.major != 9) {  // sm_90a cubins only: no compatibility path
     delete ctx;
     return DIMB_ERR_UNSUPPORTED;
   }
   ctx->num_sms = prop.multiProcessorCount;
   const char* e = getenv("DIMB_TC");
   if (e && e[0] == '0') ctx->use_tc = 0;
-  const char* pr = getenv("DIMB_PAIR");
-  if (pr) ctx->use_pair = pr[0] == '2' ? 2 : pr[0] == '1';
-  const char* fu = getenv("DIMB_FUSE1A");
-  if (fu) ctx->use_fuse1a = fu[0] == '2' ? 2 : fu[0] == '1';
-  const char* hl = getenv("DIMB_HALO");
-  if (hl) ctx->use_halo = hl[0] == '1';
   const char* lz = getenv("DIMB_ATTN_LAZY");
   if (lz) ctx->attn_lazy = static_cast<float>(atof(lz));
-  const char* at = getenv("DIMB_AL_TC");
-  if (at) ctx->al_tc = at[0] == '1';
-  const char* ff = getenv("DIMB_FUSE_FFN");
-  if (ff) ctx->fuse_ffn = ff[0] == '1';
   const char* k3 = getenv("DIMB_K32");
   if (k3) ctx->k32 = k3[0] == '1';
   const char* b2 = getenv("DIMB_BN256");
   if (b2) ctx->bn256 = b2[0] == '1';
   const char* nv = getenv("DIMB_NMS");
   if (nv && atoi(nv) == 1) ctx->nms_ver = 1;
-  const char* av = getenv("DIMB_ATTN");
-  if (av && atoi(av) >= 3 && atoi(av) <= 7) ctx->attn_ver = atoi(av);
   const char* p = getenv("DIMB_PRECISION");
   if (p && !strcmp(p, "fast")) ctx->precision = DIMB_PRECISION_FAST;
   *out = ctx;

@@ -16,18 +16,12 @@
 // ---------------------------------------------------------------- errors
 struct dimb_ctx {
   int device = 0;
-  int num_sms = 148;
-  int use_tc = 1;        // 1 = tcgen05 tensor path, 0 = SIMT CUDA-core debug path (DIMB_TC=0)
-  int use_pair = 2;      // Cin = Cout = 64 convolutions on CTA pairs (cta_group::2, conv_pair.cuh): 2 = pooled layers + conv2a (8 epilogue warps) (default), 1 = pooled layers only, 0 = single-CTA kernel (DIMB_PAIR)
-  int use_fuse1a = 2;    // conv1a inside the CTA-pair conv1b kernel (no 268 MB / image round trip): 2 = as an im2col MMA (default), 1 = SIMT producer warps, 0 = separate kernels (DIMB_FUSE1A)
-  int use_halo = 1;      // Cin = Cout = 64 convolutions on the single-halo-box kernel (gemm.cuh CONV 2); DIMB_HALO=0 -> three dx boxes (CONV 1)
+  int num_sms = 132;
+  int use_tc = 1;        // 1 = wgmma tensor path, 0 = SIMT CUDA-core debug path (DIMB_TC=0)
   int precision = DIMB_PRECISION_EXACT;
-  int al_tc = 0;          // ALIKED blocks 1-2 as tensor-core im2col GEMMs (al_conv3x3_tc_kernel): parity-equal, not yet faster than the fp32 kernels; DIMB_AL_TC=1
-  int fuse_ffn = 0;       // LightGlue FFN0 + LayerNorm + GELU in one kernel (EpiFfnLn, gemm.cuh kFullRow); DIMB_FUSE_FFN=1
-  int k32 = 0;            // 32-wide K stages (four 48 KB stages) for the 128 x 256 LightGlue tiles (gemm.cuh CONV 3); DIMB_K32=1
-  int bn256 = 1;          // LightGlue q/k projection and FFN0 on 128 x 256 output tiles (DIMB_BN256=0 -> 128 x 128)
+  int k32 = 0;            // 32-wide K stages (half-size stages) for the 128 x 256 LightGlue tiles (gemm.cuh CONV 3); DIMB_K32=1
+  int bn256 = 0;          // LightGlue q/k projection and FFN0 on 128 x 256 output tiles (DIMB_BN256=1); default 128 x 128: spill-free
   int nms_ver = 2;        // simple_nms kernel: 2 = bit-mask kernel (sp_nms2_kernel), 1 = first cut (DIMB_NMS)
-  int attn_ver = 7;       // tensor-core attention kernel: 7 = P in tensor memory + lazily consumed P V barriers (default), 5 = without the lazy barriers, 6 = 5 with two softmax threads per row, 4 / 3 = P through shared memory (DIMB_ATTN)
   float attn_lazy = 8.f;  // lazy-rescale threshold of the attention kernel in log2 units (DIMB_ATTN_LAZY; 0 = rescale on every new maximum)
   std::string last_error;
   std::vector<void*> allocs;            // device memory owned by the context itself
@@ -138,7 +132,5 @@ int dimb_tmap_2d(dimb_ctx* ctx, CUtensorMap* out, const __half* base, uint64_t r
                  uint32_t box_rows);
 // 4D fp16 NHWC activation [n][h][w][c], box = [1][box_h][box_w][64], SWIZZLE_128B, OOB -> 0 (conv zero padding).
 int dimb_tmap_2d_sw64(dimb_ctx* ctx, CUtensorMap* out, const __half* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows);
-int dimb_tmap_nhwc_sw64(dimb_ctx* ctx, CUtensorMap* out, const __half* base, uint64_t n, uint64_t h, uint64_t w, uint64_t c,
-                        uint32_t box_h, uint32_t box_w);
 int dimb_tmap_nhwc(dimb_ctx* ctx, CUtensorMap* out, const __half* base, uint64_t n, uint64_t h, uint64_t w, uint64_t c,
                    uint32_t box_h, uint32_t box_w);

@@ -6,18 +6,21 @@
 //   tap is the NHWC activation tile shifted by (dy-1, dx-1), fetched by a 4D TMA whose out-of-bounds
 //   fill implements the zero padding.
 //
-// Structure (sm_100a): 320 threads = 8 epilogue warps + 1 TMA producer warp + 1 MMA-issuer warp.
-//   producer : cp.async.bulk.tensor -> 128B-swizzled smem stages, mbarrier full/empty ring
-//   issuer   : one thread issues tcgen05.mma (M=128, N=BN, K=16) into an fp32 TMEM accumulator;
-//              EXACT mode issues hi*hi + hi*lo + lo*hi per k-step (fp16 split operands)
-//   epilogue : tcgen05.ld 32 columns at a time, thread r owns output row r -> fused epilogue functor
+// Structure (sm_90a): 384 threads = 2 consumer warpgroups + 1 producer warpgroup (one warp of it issues the TMA copies).
+//   setmaxnreg moves registers from the producer warpgroup (40 per thread) to the consumers (232): a 128 x 256 tile keeps
+//   128 fp32 accumulators per consumer thread plus the epilogue's working set without spilling.
+//   producer : cp.async.bulk.tensor -> swizzled smem stages, mbarrier full/empty ring
+//   consumers: warpgroup g issues wgmma (M = 64 rows 64g..64g+63 of the 128-row tile, N = BN, K = 16) into fp32
+//              registers; EXACT mode issues hi*hi + hi*lo + lo*hi per k-step (fp16 split operands).  After the
+//              last k-step the warpgroup stages its accumulator through shared memory, 64 columns at a time, so that
+//              thread r owns output row r and 32 consecutive columns -> fused epilogue functor
 //
 // A SIMT twin (simt_gemm_kernel) evaluates the same contraction on CUDA cores with the same
 // epilogue functors; it is a debug/bisect aid (DIMB_TC=0), never the default.  The kernel is persistent:
-// one CTA per SM, double-buffered TMEM accumulators (see below).
+// one CTA per SM; the producer fills the stages of the next tile while the consumers run the epilogue.
 #pragma once
 #include "common.cuh"
-#include "tc05.cuh"
+#include "sm90.cuh"
 
 struct TileCoord {
   int m0;         // GEMM: first global row of this 128-row tile
@@ -26,7 +29,7 @@ struct TileCoord {
 };
 
 struct GemmArgs {
-  int num_kb;      // B tiles per output tile: K / 64 (CONV 2: 9 taps x Cin / 32 half blocks)
+  int num_kb;      // B tiles per output tile: K / 64 (CONV 3: K / 32)
   int k_total;     // total K for the SIMT twin; 0 = num_kb * 64
   int M;           // GEMM: valid rows of A
   int N;           // valid rows of B (output columns)
@@ -38,39 +41,36 @@ struct GemmArgs {
 };
 
 constexpr int kTileM = 128;
-// Per-warp shared scratch of the epilogue: a 32 x 32 fp32 chunk used to turn the TMEM ownership "lane = row" into "8 lanes = one
-// row segment" so that global accesses are coalesced.  Rows are 128 B with the eight 16-byte chunks XOR-swizzled by (row & 7):
-// conflict-free for both the row-wise writes and the transposed reads without padding - 4 KB per warp instead of 4.5 KB, which is
-// what lets the K = 256 weight panel (128 KB) stay resident next to two A stages even with eight epilogue warps (EpiQK).
+constexpr int kGemmThreads = 12 * 32;  // warps 0-7: two consumer warpgroups, warps 8-11: producer warpgroup (warp 8 issues)
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;  // 128 x 40 + 256 x 232 <= 64 K registers of the SM
+// Per-warp shared scratch of the epilogue functors: a 32 x 32 fp32 chunk used to turn "lane = row" into "8 lanes = one row segment"
+// so that global accesses are coalesced.  Rows are 128 B with the eight 16-byte chunks XOR-swizzled by (row & 7): conflict-free for
+// both the row-wise writes and the transposed reads without padding.
 constexpr int kScratchPitch = 32;
 constexpr int kScratchFloats = 32 * kScratchPitch;
-// Epilogue warps per CTA come from the functor (Epi::kEpiWarps): 4 (one per TMEM lane quarter) or 8 (two per
-// quarter, each taking every other 32-column chunk) for epilogues heavy enough to out-last the MMAs of a tile.
+// Accumulator staging of one consumer warpgroup: [64 rows][64 columns] fp32, rows padded by 4 floats (the float4 row reads of 8
+// consecutive lanes hit 8 distinct 16-byte bank groups).  Once every warp holds its 32 x 32 chunk in registers the same bytes are the
+// four warps' functor scratch (4 x 4 KB <= 17 KB).
+constexpr int kStgCols = 64, kStgPitch = kStgCols + 4;
+constexpr int kStgFloats = 64 * kStgPitch;
+constexpr int kStgBytes = 2 * kStgFloats * 4;
+static_assert(4 * kScratchFloats <= kStgFloats, "functor scratch must fit in the staging buffer of a warpgroup");
 // CONV modes of the kernel templates (int CONV):
 //   0  plain GEMM
 //   1  3x3 conv, tile = 8 rows x 16 pixels, one (8+2) x 16-pixel box of 64 channels per dx (three boxes per channel block);
 //      the three dy taps are the same stage at descriptor offsets of one box row (2048 B)
-//   2  3x3 conv, tile = 16 rows x 8 pixels, ONE (16+2) x (8+2)-pixel halo box of 32 channels (64-byte rows, SWIZZLE_64B)
-//      per half channel block; all nine taps are descriptor start offsets (dy * 10 + dx) * 64 B into that box and the MMA's
-//      8-row groups are the image rows, 10 * 64 B apart.  tcgen05 derives the swizzle phase from absolute shared-memory
-//      address bits (probed: tools/probe_umma_rowshift.py), so neither the row shift nor the non-power-of-two group stride
-//      needs anything beyond the descriptor fields.  A third of the activation fill traffic of mode 1, and small enough
-//      (23 KB per stage, hi+lo) to keep three stages next to the resident weights of the Cin = Cout = 64 layers.
-//   3  plain GEMM with 32-wide K blocks (64-byte rows, SWIZZLE_64B): half-size pipeline stages.  For the 128 x 256 tiles a 64-wide
-//      K stage is 96 KB (hi+lo A and B) and only two fit: the refill of a stage starts only when all of its 12 MMAs have retired and
-//      takes longer than the other stage lasts.  Four 48 KB stages keep the same bytes in flight but start refills twice as early.
+//   3  plain GEMM with 32-wide K blocks (64-byte rows, SWIZZLE_64B): half-size pipeline stages, so that more of them fit next to
+//      the 128 x 256 tiles
 constexpr int kConvTH = 8, kConvTW = 16;    // mode 1 tile
-constexpr int kHaloTH = 16, kHaloTW = 8;    // mode 2 tile
-constexpr int kHaloRows = (kHaloTH + 2) * (kHaloTW + 2);  // 180 smem rows per halo box
 template <int CONV>
 struct ConvTile {
-  static constexpr int TH = CONV == 2 ? kHaloTH : kConvTH, TW = CONV == 2 ? kHaloTW : kConvTW;
+  static constexpr int TH = kConvTH, TW = kConvTW;
 };
 
 template <int CONV>
 __device__ __forceinline__ TileCoord make_tile_coord(const GemmArgs& g, int t) {
   TileCoord tc;
-  if (CONV == 1 || CONV == 2) {
+  if (CONV == 1) {
     int per_img = g.tiles_x * g.tiles_y;
     tc.b = t / per_img;
     int rem = t - tc.b * per_img;
@@ -88,8 +88,6 @@ __device__ __forceinline__ TileCoord make_tile_coord(const GemmArgs& g, int t) {
 
 // ------------------------------------------------------------------ persistent tensor-core kernel
 // One CTA per SM loops over output tiles:
-//   * the accumulator is double-buffered in TMEM (2 x BN columns): the epilogue of tile i overlaps the MMAs of
-//     tile i+1, and barrier init / TMEM allocation / pipeline fill are paid once per CTA, not once per tile;
 //   * A and B have separate smem rings.  CONV mode fetches the activation tile ONCE per (dx, channel block) as
 //     a (8+2) x 16 pixel box and runs the three dy taps out of it by advancing the smem descriptor by one box row
 //     (16 px * 128 B = 2048 B, swizzle-atom aligned): 3 A loads per channel block instead of 9;
@@ -104,40 +102,35 @@ struct PersCfg {
 template <int BN, bool SPLIT, int CONV>
 struct PersGeom {
   static constexpr int kPl = SPLIT ? 2 : 1;
-  static constexpr int kRowB = (CONV == 2 || CONV == 3) ? 64 : 128;  // bytes per shared-memory operand row (K block of 32 / 64 halfs)
-  static constexpr int kABoxTx = CONV == 2 ? kHaloRows * 64 : CONV == 1 ? (kConvTH + 2) * kConvTW * 128 : kTileM * kRowB;  // bytes a TMA box delivers
+  static constexpr int kRowB = CONV == 3 ? 64 : 128;  // bytes per shared-memory operand row (K block of 32 / 64 halfs)
+  static constexpr int kABoxTx = CONV == 1 ? (kConvTH + 2) * kConvTW * 128 : kTileM * kRowB;  // bytes a TMA box delivers
   static constexpr int kABox = (kABoxTx + 1023) / 1024 * 1024;  // plane pitch inside a stage (swizzle-atom aligned)
   static constexpr int kATx = kPl * kABoxTx;
   static constexpr int kAStage = kPl * kABox;
   static constexpr int kBPlane = BN * kRowB;
   static constexpr int kBTile = kPl * kBPlane;
-  static constexpr int kBudget = 232448 - 1024 - 1024;
+  static constexpr int kBudget = 232448 - 1024 - 1024 - kStgBytes;
 };
 
 template <int BN, bool SPLIT, int CONV, bool RESB, class Epi>
-__global__ void __launch_bounds__((Epi::kEpiWarps + 2) * 32, 1)
+__global__ void __launch_bounds__(kGemmThreads, 1)
 tc_gemm_pers_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                     const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, GemmArgs g, Epi epi,
                     int m_tiles, int n_tiles, int SA, int SB) {
   using G = PersGeom<BN, SPLIT, CONV>;
-  using namespace tc05;
-  // EXACT mode issues 2 MMAs per k-step instead of 3: A_hi x [B_hi ; B_lo] as ONE N = 2*BN instruction (the two
-  // weight planes are adjacent in the stage, i.e. a single 2*BN-row K-major tile) writing two accumulators
-  // [A_hi B_hi | A_hi B_lo], then A_lo x B_hi into the first; the epilogue adds the halves.  Fewer, larger
-  // instructions keep the single issuing thread ahead of the tensor pipe for the N = 64 layers.
-  constexpr bool STACK = SPLIT && BN <= 128;
-  constexpr int ACC_COLS = STACK ? 2 * BN : BN;
-  constexpr int kEpiWarps = Epi::kEpiWarps;
+  using namespace sm90;
+  static_assert(BN % kStgCols == 0, "BN must be a multiple of the staging width");
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment by OFFSET from the __shared__ array (not by integer-casting the pointer): the compiler keeps the shared
   // address space and emits LDS / STS instead of generic LD / ST for every access derived from it
-  uint8_t* smem = smem_raw + ((1024u - (tc05::smem_u32(smem_raw) & 1023u)) & 1023u);
-  constexpr bool HALO = CONV == 2;
-  constexpr bool ISCONV = CONV == 1 || CONV == 2;  // CONV 3 is a GEMM
-  constexpr bool K32 = CONV == 2 || CONV == 3;
+  uint8_t* smem = smem_raw + ((1024u - (sm90::smem_u32(smem_raw) & 1023u)) & 1023u);
+  constexpr bool ISCONV = CONV == 1;
+  constexpr bool K32 = CONV == 3;
   constexpr int KB_COLS = K32 ? 32 : 64;  // K elements per B tile / A stage
   constexpr int KSTEPS = K32 ? 2 : 4;     // 16-deep MMA steps per K block
-  const int nkb = g.num_kb;  // GEMM: K/64.  CONV 1: 9 * cin_blocks.  CONV 2: 9 * 2 * cin_blocks
+  constexpr uint32_t kLayout = K32 ? kLayoutSw64 : kLayoutSw128;
+  constexpr uint32_t kSbo = 8 * G::kRowB;
+  const int nkb = g.num_kb;  // GEMM: K/64 (CONV 3: K/32).  CONV 1: 9 * cin_blocks
   uint8_t* sA = smem;
   uint8_t* sB = sA + SA * G::kAStage;
   const int nb_slots = RESB ? nkb : SB;
@@ -145,39 +138,28 @@ tc_gemm_pers_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_const
   uint64_t* emptyA = fullA + SA;
   uint64_t* fullB = emptyA + SA;
   uint64_t* emptyB = fullB + nb_slots;
-  uint64_t* tfull = emptyB + nb_slots;   // [2]
-  uint64_t* tempty = tfull + 2;          // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tempty + 2);
-  float* scratch = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(fullA) + 1024);  // [4 warps][32 x 36]
+  float* staging = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(fullA) + 1024);  // [2 warpgroups][kStgFloats]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int s = 0; s < SA; ++s) {
       mbar_init(&fullA[s], 1);
-      mbar_init(&emptyA[s], 1);
+      mbar_init(&emptyA[s], 8);  // one arrival per consumer warp
     }
     for (int s = 0; s < nb_slots; ++s) {
       mbar_init(&fullB[s], 1);
-      mbar_init(&emptyB[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull[a], 1);
-      mbar_init(&tempty[a], kEpiWarps * 32);
+      mbar_init(&emptyB[s], 8);
     }
     fence_barrier_init();
   }
-  if (warp == kEpiWarps + 1) tmem_alloc(tmem_ptr, 2 * ACC_COLS);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr;
   const int total = m_tiles * n_tiles;
   const int cinb = ISCONV ? g.cin_blocks : 1;
   // A stages per output tile and B tiles (taps) consumed out of each stage
-  const int outer_n = HALO ? 2 * cinb : ISCONV ? 3 * cinb : nkb;
-  constexpr int inner_n = HALO ? 9 : ISCONV ? 3 : 1;
+  const int outer_n = ISCONV ? 3 * cinb : nkb;
+  constexpr int inner_n = ISCONV ? 3 : 1;
   // B tile index of tap step `in` of A stage `o`: weights are [Cout][tap * Cin + c]
-  auto kb_of = [&](int o, int in) { return HALO ? in * (2 * cinb) + o : ISCONV ? ((in * 3 + o / cinb) * cinb + (o % cinb)) : o; };
+  auto kb_of = [&](int o, int in) { return ISCONV ? ((in * 3 + o / cinb) * cinb + (o % cinb)) : o; };
 
   auto tile_coord = [&](int w, int& n0) {
     const int mt = w / n_tiles, nt = w - mt * n_tiles;
@@ -188,20 +170,9 @@ tc_gemm_pers_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_const
     return tc;
   };
 
-  // Tile sequence of this CTA.  Default: tiles blockIdx.x, + gridDim.x, ... of the (m, n) grid.  kFullRow: the CTA takes whole rows of
-  // n-tiles (m-tile u = blockIdx.x + k gridDim.x, then n = 0, 1) so that tile parity = accumulator buffer = column half.
-  auto tile_at = [&](int i, int& w) -> bool {
-    if constexpr (Epi::kFullRow) {
-      const int u = static_cast<int>(blockIdx.x) + (i >> 1) * static_cast<int>(gridDim.x);
-      w = u * 2 + (i & 1);
-      return u < m_tiles;
-    } else {
-      w = static_cast<int>(blockIdx.x) + i * static_cast<int>(gridDim.x);
-      return w < total;
-    }
-  };
-  if (warp == kEpiWarps) {
-    {  // ---------------- TMA producer: the whole warp walks the schedule and waits, one elected lane issues the copies
+  if (warp >= 8) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == 8) {  // ---------------- TMA producer: the whole warp walks the schedule and waits, one elected lane issues the copies
       if (elect_one()) {
         tma_prefetch_desc(&tmAh);
         tma_prefetch_desc(&tmBh);
@@ -221,23 +192,20 @@ tc_gemm_pers_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_const
       }
       __syncwarp();
       uint32_t itA = 0, itB = 0;
-      for (int ti = 0, w; tile_at(ti, w); ++ti) {
+      for (int w = blockIdx.x; w < total; w += gridDim.x) {
         int n0;
         const TileCoord tc = tile_coord(w, n0);
         if (!epi.tile_active(tc)) continue;
         const int b_off = epi.b_row_offset(tc);
         const int outer = outer_n;
         if (elect_one()) {  // pull the A operand of the tile this CTA processes two iterations from now into L2
-          const int wp = w + 2 * static_cast<int>(gridDim.x);  // kFullRow: the m-tile after next of this CTA (same column half)
+          const int wp = w + 2 * static_cast<int>(gridDim.x);
           if (wp < total) {
             int n0p;
             const TileCoord tp = tile_coord(wp, n0p);
             if ((ISCONV || n0p == 0) && epi.tile_active(tp)) {
               for (int o = 0; o < outer; ++o) {
-                if (HALO) {
-                  tma_prefetch_4d(&tmAh, o * 32, tp.x0 - 1, tp.y0 - 1, tp.b);
-                  if (SPLIT) tma_prefetch_4d(&tmAl, o * 32, tp.x0 - 1, tp.y0 - 1, tp.b);
-                } else if (ISCONV) {
+                if (ISCONV) {
                   const int dx = o / cinb, cb = o - dx * cinb;
                   if (dx != 1) continue;  // the three dx boxes overlap: the centre one plus neighbours' halos cover them
                   tma_prefetch_4d(&tmAh, cb * 64, tp.x0 - 1, tp.y0 - 1, tp.b);
@@ -258,19 +226,16 @@ tc_gemm_pers_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_const
           mbar_wait(&emptyA[s], ((itA / SA) & 1) ^ 1);
           uint8_t* st = sA + s * G::kAStage;
           if (elect_one()) {
-          mbar_expect_tx(&fullA[s], G::kATx);
-          if (HALO) {
-            tma_load_4d(st, &tmAh, &fullA[s], o * 32, tc.x0 - 1, tc.y0 - 1, tc.b);
-            if (SPLIT) tma_load_4d(st + G::kABox, &tmAl, &fullA[s], o * 32, tc.x0 - 1, tc.y0 - 1, tc.b);
-          } else if (ISCONV) {
-            const int dx = o / cinb, cb = o - dx * cinb;
-            tma_load_4d(st, &tmAh, &fullA[s], cb * 64, tc.x0 + dx - 1, tc.y0 - 1, tc.b);
-            if (SPLIT) tma_load_4d(st + G::kABox, &tmAl, &fullA[s], cb * 64, tc.x0 + dx - 1, tc.y0 - 1, tc.b);
-          } else {
-            tma_load_2d(st, &tmAh, &fullA[s], o * KB_COLS, tc.m0);
-            if (SPLIT) tma_load_2d(st + G::kABox, &tmAl, &fullA[s], o * KB_COLS, tc.m0);
+            mbar_expect_tx(&fullA[s], G::kATx);
+            if (ISCONV) {
+              const int dx = o / cinb, cb = o - dx * cinb;
+              tma_load_4d(st, &tmAh, &fullA[s], cb * 64, tc.x0 + dx - 1, tc.y0 - 1, tc.b);
+              if (SPLIT) tma_load_4d(st + G::kABox, &tmAl, &fullA[s], cb * 64, tc.x0 + dx - 1, tc.y0 - 1, tc.b);
+            } else {
+              tma_load_2d(st, &tmAh, &fullA[s], o * KB_COLS, tc.m0);
+              if (SPLIT) tma_load_2d(st + G::kABox, &tmAl, &fullA[s], o * KB_COLS, tc.m0);
+            }
           }
-          }  // elect_one
           __syncwarp();
           ++itA;
           if (!RESB) {
@@ -291,155 +256,88 @@ tc_gemm_pers_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_const
         }
       }
     }
-  } else if (warp == kEpiWarps + 1) {
-    {  // ---------------- MMA issuer: the whole warp walks the schedule (uniform control flow), one elected lane issues
-      constexpr uint32_t idesc = make_idesc_f16(BN);
-      constexpr uint32_t idesc2 = make_idesc_f16(STACK ? 2 * BN : BN);
-      uint32_t itA = 0, itB = 0, tcount = 0;
-      bool resb_ready = false;
-      for (int ti = 0, w; tile_at(ti, w); ++ti) {
-        int n0;
-        const TileCoord tc = tile_coord(w, n0);
-        if (!epi.tile_active(tc)) continue;
-        const uint32_t acc = tcount & 1;
-        mbar_wait(&tempty[acc], ((tcount >> 1) & 1) ^ 1);  // epilogue has drained this accumulator
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + acc * ACC_COLS;
-        const int outer = outer_n;
-        uint32_t accumulate = 0;
-        for (int o = 0; o < outer; ++o) {
-          const int s = itA % SA;
-          mbar_wait(&fullA[s], (itA / SA) & 1);
-          tc_fence_after_sync();
-          const uint32_t a_base = smem_u32(sA + s * G::kAStage);
-          // mode 2: the descriptors of a stage differ from tap to tap only in the start-address field - build them once
-          uint64_t a0h = 0, a0l = 0;
-          if (HALO) {
-            a0h = make_sdesc(a_base, (kHaloTW + 2) * 64, kLayoutSw64);
-            a0l = make_sdesc(a_base + G::kABox, (kHaloTW + 2) * 64, kLayoutSw64);
-          }
-#pragma unroll
-          for (int dy = 0; dy < inner_n; ++dy) {  // mode 2: dy enumerates the nine taps
-            const int kb = kb_of(o, dy);
-            uint32_t b_base;
-            int sb = 0;
-            if (RESB) {
-              if (!resb_ready) {
-                mbar_wait(&fullB[kb], 0);
-                tc_fence_after_sync();
-              }
-              b_base = smem_u32(sB + kb * G::kBTile);
-            } else {
-              sb = itB % SB;
-              mbar_wait(&fullB[sb], (itB / SB) & 1);
-              tc_fence_after_sync();
-              b_base = smem_u32(sB + sb * G::kBTile);
-            }
-            uint64_t a_h, a_l, b_h, b_l;
-            if (HALO) {  // tap (ty, tx): start at halo row ty * 10 + tx; image rows (8-row groups) are 10 * 64 B apart
-              const uint64_t tap16 = static_cast<uint64_t>(((dy / 3) * (kHaloTW + 2) + dy % 3) * 4);  // byte offset >> 4
-              a_h = a0h + tap16, a_l = a0l + tap16;
-              b_h = make_sdesc(b_base, 512, kLayoutSw64), b_l = b_h + (G::kBPlane >> 4);
-            } else if (K32) {  // GEMM with 64-byte rows: 8-row groups 512 B apart, both operands SWIZZLE_64B
-              a_h = make_sdesc(a_base, 512, kLayoutSw64), a_l = make_sdesc(a_base + G::kABox, 512, kLayoutSw64);
-              b_h = make_sdesc(b_base, 512, kLayoutSw64), b_l = b_h + (G::kBPlane >> 4);
-            } else {
-              const uint32_t a_tap = a_base + (ISCONV ? dy * (kConvTW * 128) : 0);
-              a_h = make_sdesc_sw128(a_tap), a_l = make_sdesc_sw128(a_tap + G::kABox);
-              b_h = make_sdesc_sw128(b_base), b_l = make_sdesc_sw128(b_base + G::kBPlane);
-            }
-            if (elect_one()) {
-#pragma unroll
-            for (int k16 = 0; k16 < KSTEPS; ++k16) {
-              if (STACK) {
-                mma_f16_ss(d_tmem, sdesc_advance_k(a_h, k16), sdesc_advance_k(b_h, k16), idesc2, k16 ? 1u : accumulate);  // [Ah Bh | Ah Bl]
-                mma_f16_ss(d_tmem, sdesc_advance_k(a_l, k16), sdesc_advance_k(b_h, k16), idesc, 1);           // += Al Bh
-              } else {
-                mma_f16_ss(d_tmem, sdesc_advance_k(a_h, k16), sdesc_advance_k(b_h, k16), idesc, k16 ? 1u : accumulate);
-                if (SPLIT) {
-                  mma_f16_ss(d_tmem, sdesc_advance_k(a_h, k16), sdesc_advance_k(b_l, k16), idesc, 1);
-                  mma_f16_ss(d_tmem, sdesc_advance_k(a_l, k16), sdesc_advance_k(b_h, k16), idesc, 1);
-                }
-              }
-            }
-            if (!RESB) mma_commit(&emptyB[sb]);
-            }  // elect_one
-            __syncwarp();
-            accumulate = 1;  // every lane tracks the schedule state: any lane may be elected next time
-            if (!RESB) ++itB;
-          }
-          if (elect_one()) mma_commit(&emptyA[s]);
-          __syncwarp();
-          ++itA;
-        }
-        resb_ready = true;  // every resident tile has been waited for once
-        if (elect_one()) mma_commit(&tfull[acc]);
-        __syncwarp();
-        ++tcount;
-      }
-      if (RESB && !resb_ready)  // no active tile: still drain the resident-weight loads before the CTA exits
-        for (int kb = 0; kb < nkb; ++kb) mbar_wait(&fullB[kb], 0);
-    }
-  } else {  // ---------------- epilogue warps: lane quarter q = warp % 4 (TMEM access rule), column group warp / 4
-    uint32_t tcount = 0;
-    const int q = warp & 3, cg = warp >> 2;
-    const int r = q * 32 + lane;
-    constexpr int kGroups = kEpiWarps / 4;
-    if constexpr (Epi::kFullRow) {
-      // Whole-row epilogue (row-wise reductions over all 2 * BN output columns, e.g. LayerNorm): both accumulators of an m-tile are
-      // complete before the functor runs; it releases column half h (tempty[h]) as soon as it has finished with it, so the MMAs of
-      // the next m-tile's first half overlap the second half of this epilogue.
-      for (int ui = 0, w; tile_at(2 * ui, w); ++ui) {
-        int n0;
-        const TileCoord tc = tile_coord(w, n0);
-        if (!epi.tile_active(tc)) continue;
-        mbar_wait(&tfull[0], tcount & 1);
-        mbar_wait(&tfull[1], tcount & 1);
-        tc_fence_after_sync();
-        epi.full_row(tc, r, cg, tmem_base + (static_cast<uint32_t>(q * 32) << 16), scratch + warp * kScratchFloats, tempty);
-        ++tcount;
-      }
-    } else
+  } else {  // ---------------- consumer warpgroup wg: rows 64 wg .. 64 wg + 63 of every tile
+    setmaxnreg_inc<kConsumerRegs>();
+    const int wg = warp >> 2, w4 = warp & 3;
+    // A rows of this warpgroup start 64 rows into the stage: 8 swizzle atoms of 8 rows, atom-aligned
+    const uint32_t a_wg = static_cast<uint32_t>(wg * 64 * G::kRowB);
+    float* stg = staging + wg * kStgFloats;
+    uint32_t itA = 0, itB = 0;
+    bool resb_ready = false;
+    float acc[BN / 2];
     for (int w = blockIdx.x; w < total; w += gridDim.x) {
       int n0;
       const TileCoord tc = tile_coord(w, n0);
       if (!epi.tile_active(tc)) continue;
-      const uint32_t acc = tcount & 1;
-      mbar_wait(&tfull[acc], (tcount >> 1) & 1);
-      tc_fence_after_sync();
-      bool released = false;
-#pragma unroll 1
-      for (int c0 = cg * 32; c0 < BN; c0 += 32 * kGroups) {
-        float v[32];
-        tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * ACC_COLS + c0, v);
-        if (STACK) {
-          float v2[32];
-          tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * ACC_COLS + BN + c0, v2);
-          tmem_ld_wait();
+      const int outer = outer_n;
+      for (int o = 0; o < outer; ++o) {
+        const int s = itA % SA;
+        mbar_wait(&fullA[s], (itA / SA) & 1);
+        const uint32_t a_base = smem_u32(sA + s * G::kAStage) + a_wg;
+        int sb0 = 0;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += v2[j];
-        } else {
-          tmem_ld_wait();
+        for (int dy = 0; dy < inner_n; ++dy) {
+          const int kb = kb_of(o, dy);
+          uint32_t b_base;
+          if (RESB) {
+            if (!resb_ready) mbar_wait(&fullB[kb], 0);
+            b_base = smem_u32(sB + kb * G::kBTile);
+          } else {
+            const int sb = (itB + dy) % SB;
+            if (dy == 0) sb0 = sb;
+            mbar_wait(&fullB[sb], ((itB + dy) / SB) & 1);
+            b_base = smem_u32(sB + sb * G::kBTile);
+          }
+          const uint32_t a_tap = a_base + (ISCONV ? dy * (kConvTW * 128) : 0);
+          const uint64_t a_h = make_sdesc(a_tap, kSbo, kLayout), a_l = make_sdesc(a_tap + G::kABox, kSbo, kLayout);
+          const uint64_t b_h = make_sdesc(b_base, kSbo, kLayout), b_l = make_sdesc(b_base + G::kBPlane, kSbo, kLayout);
+          wgmma_fence();
+#pragma unroll
+          for (int k16 = 0; k16 < KSTEPS; ++k16) {
+            Wgmma<BN>::ss(acc, sdesc_advance_k(a_h, k16), sdesc_advance_k(b_h, k16), (o | dy | k16) != 0);
+            if (SPLIT) {
+              Wgmma<BN>::ss(acc, sdesc_advance_k(a_h, k16), sdesc_advance_k(b_l, k16), 1);
+              Wgmma<BN>::ss(acc, sdesc_advance_k(a_l, k16), sdesc_advance_k(b_h, k16), 1);
+            }
+          }
         }
-        if (c0 + 32 * kGroups >= BN) {  // last TMEM read of this thread for this tile: release the accumulator early
-          tc_fence_before_sync();
-          mbar_arrive(&tempty[acc]);
-          released = true;
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        if (lane == 0) {  // this warp is done with the stage and its B tiles
+          mbar_arrive(&emptyA[s]);
+          if (!RESB)
+            for (int dy = 0; dy < inner_n; ++dy) mbar_arrive(&emptyB[(sb0 + dy) % SB]);
         }
-        epi(tc, r, n0 + c0, v, scratch + warp * kScratchFloats);
+        ++itA;
+        if (!RESB) itB += inner_n;
       }
-      if (!released) {  // BN smaller than the column-group stride: this warp had no chunk
-        tc_fence_before_sync();
-        mbar_arrive(&tempty[acc]);
+      resb_ready = true;  // every resident tile has been waited for once
+      // epilogue: accumulator -> staging (64 columns at a time) -> thread r = row of the tile, 32 consecutive columns
+      const int rr = 32 * (w4 & 1) + lane, cq = 32 * (w4 >> 1);
+#pragma unroll
+      for (int c0 = 0; c0 < BN; c0 += kStgCols) {
+        const int lr = 16 * w4 + (lane >> 2);
+#pragma unroll
+        for (int i = c0 / 8; i < (c0 + kStgCols) / 8; ++i) {
+          const int col = 8 * i - c0 + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(stg + lr * kStgPitch + col) = make_float2(acc[4 * i], acc[4 * i + 1]);
+          *reinterpret_cast<float2*>(stg + (lr + 8) * kStgPitch + col) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+        }
+        named_bar_sync(1 + wg, 128);
+        float v[32];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const float4 x = *reinterpret_cast<const float4*>(stg + rr * kStgPitch + cq + 4 * q);
+          v[4 * q] = x.x, v[4 * q + 1] = x.y, v[4 * q + 2] = x.z, v[4 * q + 3] = x.w;
+        }
+        named_bar_sync(1 + wg, 128);
+        epi(tc, 64 * wg + rr, n0 + c0 + cq, v, stg + w4 * kScratchFloats);
+        named_bar_sync(1 + wg, 128);
       }
-      ++tcount;
     }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == kEpiWarps + 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 2 * ACC_COLS);
+    if (RESB && !resb_ready)  // no active tile: still drain the resident-weight loads before the CTA exits
+      for (int kb = 0; kb < nkb; ++kb) mbar_wait(&fullB[kb], 0);
   }
 }
 
@@ -447,7 +345,7 @@ tc_gemm_pers_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_const
 template <int CONV>
 __device__ __forceinline__ float simt_load_a(const GemmArgs& g, const TileCoord& tc, int row, int k) {
   size_t off;
-  if (CONV) {
+  if (CONV == 1) {
     const int cin = g.cin_blocks * 64;
     const int tap = k / cin, c = k - tap * cin;
     const int dy = tap / 3, dx = tap - dy * 3;
@@ -467,7 +365,7 @@ __device__ __forceinline__ float simt_load_a(const GemmArgs& g, const TileCoord&
 template <int CONV, class Epi>
 __global__ void __launch_bounds__(128) simt_gemm_kernel(GemmArgs g, Epi epi) {
   TileCoord tc = make_tile_coord<CONV>(g, blockIdx.x);
-  if (!CONV) tc.m0 = epi.m0_of(blockIdx.x);
+  if (CONV != 1) tc.m0 = epi.m0_of(blockIdx.x);
   tc.n0 = blockIdx.y * 32;
   if (!epi.tile_active(tc)) return;
   const int b_off = epi.b_row_offset(tc);
@@ -517,34 +415,36 @@ int launch_pers(dimb_ctx* ctx, cudaStream_t st, const TcOperands& ops, const Gem
                 const PersCfg& cfg, int grid) {
   auto kern = tc_gemm_pers_kernel<BN, SPLIT, CONV, RESB, Epi>;
   DIMB_TRY(dimb_func_smem(ctx, kern, cfg.smem_bytes));
-  kern<<<grid, (Epi::kEpiWarps + 2) * 32, cfg.smem_bytes, st>>>(ops.Ah, ops.Al, ops.Bh, ops.Bl, g, epi, m_tiles, n_tiles, cfg.sa, cfg.sb);
+  kern<<<grid, kGemmThreads, cfg.smem_bytes, st>>>(ops.Ah, ops.Al, ops.Bh, ops.Bl, g, epi, m_tiles, n_tiles, cfg.sa, cfg.sb);
   DIMB_LAUNCH_CHECK(ctx);
   return DIMB_OK;
 }
 
 // ring depths from the 227 KB shared-memory budget; resb: keep all nkb B tiles resident
 template <int BN, bool SPLIT, int CONV>
-PersCfg pers_config(int nkb, bool resb, int scratch_bytes) {
+PersCfg pers_config(int nkb, bool resb) {
   using G = PersGeom<BN, SPLIT, CONV>;
   PersCfg c{};
   c.nkb_total = nkb;
-  int budget = G::kBudget - scratch_bytes;
+  int budget = G::kBudget;
   if (resb) {
     budget -= nkb * G::kBTile;
     c.sb = 0;
     c.sa = budget / G::kAStage;
   } else {
     // conv consumes 3 B tiles per A stage: give B the deeper ring
-    const int unit = G::kAStage + ((CONV == 1 || CONV == 2) ? 2 : 1) * G::kBTile;
+    const int per = CONV == 1 ? 3 : 1;
+    const int unit = G::kAStage + per * G::kBTile;
     int n = budget / unit;
     if (n < 1) n = 1;
     c.sa = n;
-    c.sb = ((CONV == 1 || CONV == 2) ? 2 : 1) * n;
+    c.sb = per * n;
     while (c.sa * G::kAStage + (c.sb + 1) * G::kBTile <= budget) ++c.sb;
+    while ((c.sa + 1) * G::kAStage + c.sb * G::kBTile <= budget) ++c.sa;
   }
   if (c.sa > 8) c.sa = 8;
   if (c.sb > 12) c.sb = 12;
-  c.smem_bytes = c.sa * G::kAStage + (resb ? nkb : c.sb) * G::kBTile + 1024 + 1024 + scratch_bytes;
+  c.smem_bytes = c.sa * G::kAStage + (resb ? nkb : c.sb) * G::kBTile + 1024 + 1024 + kStgBytes;
   return c;
 }
 
@@ -552,20 +452,19 @@ template <int BN, bool SPLIT, int CONV, class Epi>
 int launch_pers_auto(dimb_ctx* ctx, cudaStream_t st, const TcOperands& ops, const GemmArgs& g, const Epi& epi, int m_tiles, int n_pad) {
   using G = PersGeom<BN, SPLIT, CONV>;
   const int n_tiles = n_pad / BN;
-  const int scratch = Epi::kUsesScratch ? Epi::kEpiWarps * kScratchFloats * 4 : 0;
   // resident weights only where a CTA keeps seeing the same B panel (its tiles share the n-tile: the persistent
   // stride = grid size must be a multiple of n_tiles) and >= 2 A stages still fit
   const int total = m_tiles * n_tiles, grid = total < ctx->num_sms ? total : ctx->num_sms;
-  const bool fits = Epi::kConstB && (G::kBudget - scratch - g.num_kb * G::kBTile) >= 2 * G::kAStage;
+  const bool fits = Epi::kConstB && (G::kBudget - g.num_kb * G::kBTile) >= 2 * G::kAStage;
   // a grid that is a multiple of n_tiles pins every CTA to one B panel; when the SM count is not such a multiple (the brute-force
   // matcher: 32 panels of 256 descriptors), giving up a few SMs is far cheaper than re-streaming B from L2 for every tile
   int rgrid = grid;
   if (fits && grid % n_tiles != 0 && n_tiles <= grid) rgrid = grid / n_tiles * n_tiles;
   const bool resb = fits && (rgrid % n_tiles == 0) && rgrid * 8 >= grid * 7;
   if (resb)
-    return launch_pers<BN, SPLIT, CONV, true, Epi>(ctx, st, ops, g, epi, m_tiles, n_tiles, pers_config<BN, SPLIT, CONV>(g.num_kb, true, scratch),
+    return launch_pers<BN, SPLIT, CONV, true, Epi>(ctx, st, ops, g, epi, m_tiles, n_tiles, pers_config<BN, SPLIT, CONV>(g.num_kb, true),
                                                    rgrid);
-  return launch_pers<BN, SPLIT, CONV, false, Epi>(ctx, st, ops, g, epi, m_tiles, n_tiles, pers_config<BN, SPLIT, CONV>(g.num_kb, false, scratch),
+  return launch_pers<BN, SPLIT, CONV, false, Epi>(ctx, st, ops, g, epi, m_tiles, n_tiles, pers_config<BN, SPLIT, CONV>(g.num_kb, false),
                                                   grid);
 }
 
@@ -595,10 +494,7 @@ int launch_gemm(dimb_ctx* ctx, cudaStream_t st, const TcOperands& ops, GemmArgs 
 // Optional hooks (defaults in EpiBase): m0_of(t) maps the tile index to its first A row; b_row_offset(tc) shifts
 // the B rows a tile multiplies with (stacked per-layer weights, or "the other image" for similarity matrices).
 struct EpiBase {
-  static constexpr bool kUsesScratch = true;  // needs the per-warp transpose scratch (false: pass-through)
-  static constexpr int kEpiWarps = 4;         // 4, or 8 for epilogues that out-last the MMAs of a tile
   static constexpr bool kConstB = true;       // b_row_offset() == 0 for every tile (B panel may stay resident)
-  static constexpr bool kFullRow = false;     // true: the CTA owns whole output rows (n_tiles == 2, both accumulators) - see EpiFfnLn
   __device__ int m0_of(int t) const { return t * kTileM; }
   __device__ int b_row_offset(const TileCoord&) const { return 0; }
   __device__ bool tile_active(const TileCoord&) const { return true; }

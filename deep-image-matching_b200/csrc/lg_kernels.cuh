@@ -1,8 +1,9 @@
 // lg_kernels.cuh - the tensor-core building blocks of a 256-dim / 4-head x 64 attentional matcher, shared by LightGlue
 // (lightglue.cu) and SuperGlue (superglue.cu, same attention shape: models/superglue.py:96-152): the GEMM epilogues that produce the
 // attention operands (q / k head-split with optional rotary, V^T), the message / residual epilogues on the [x | message] concat
-// buffer, the final projection / similarity epilogues, and the warp-specialised flash-attention kernel (S and O in TMEM).
+// buffer, the final projection / similarity epilogues, and the launch of the flash-attention kernel (attention.cuh).
 #pragma once
+#include "attention.cuh"
 #include "gemm.cuh"
 
 namespace {
@@ -25,7 +26,6 @@ struct LgRows {  // device-side liveness of a 128-row tile
 // ------------------------------------------------------------------ GEMM epilogues
 // Self-attention q,k: columns [q(4x64) | k(4x64)] (weights re-packed at load), rotary applied; cross: [qk(4x64)].
 struct EpiQK : EpiBase {
-  static constexpr int kEpiWarps = 8;  // rotary + head split make this the longest epilogue relative to K = 256
   LgRows rows;
   const float* bias;           // [512] or [256]
   const float *cs, *sn;        // [R][32] rotary tables (unused for cross)
@@ -138,84 +138,9 @@ __device__ __forceinline__ float lg_gelu(float y) {
   const float ax = fabsf(y) * 0.70710678118654752440f;
   const float tt = __frcp_rn(fmaf(0.3275911f, ax, 1.f));
   const float poly = tt * fmaf(tt, fmaf(tt, fmaf(tt, fmaf(tt, 1.061405429f, -1.453152027f), 1.421413741f), -0.284496736f), 0.254829592f);
-  const float er = 1.f - poly * tc05::fast_exp2(-ax * ax * 1.4426950408889634f);
+  const float er = 1.f - poly * sm90::fast_exp2(-ax * ax * 1.4426950408889634f);
   return 0.5f * y * (1.f + copysignf(er, y));
 }
-
-// FFN0 + LayerNorm(512) + GELU in one kernel (lightglue.py:146-159 ffn[0..2]): the CTA owns 128 rows x all 512 hidden columns
-// (two 256-column accumulators = all of TMEM, gemm.cuh kFullRow), so the pre-LayerNorm activations - 310 MB written and read back
-// per launch by the two-kernel form - never leave the SM.  Per row (thread = TMEM lane): two-pass mean / variance straight from
-// TMEM (both warps of a lane quarter compute them redundantly - no exchange), then normalise, GELU, hi/lo split and the coalesced
-// store of the FFN3 operand, 32 columns at a time; column half h is handed back to the MMA issuer as soon as it is drained.
-struct EpiFfnLn : EpiBase {
-  static constexpr int kEpiWarps = 8;
-  static constexpr bool kFullRow = true;
-  LgRows rows;
-  const float *bias, *gamma, *beta;  // [512]
-  __half *hi, *lo;                   // [R][512]
-  __device__ bool tile_active(const TileCoord& tc) const { return rows.active(tc.m0); }
-  __device__ void operator()(const TileCoord&, int, int, float (&)[32], float*) const {}  // (SIMT twin only; not used)
-  __device__ void full_row(const TileCoord& tc, int r, int cg, uint32_t trow, float* sc, uint64_t* tempty) const {
-    using namespace tc05;
-    float sum[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 1
-    for (int c = 0; c < 512; c += 32) {
-      float v[32];
-      tmem_ld32(trow + c, v);
-      tmem_ld_wait();
-      add_bias32(v, bias, c);
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) sum[0] += v[j], sum[1] += v[j + 1], sum[2] += v[j + 2], sum[3] += v[j + 3];
-    }
-    const float mean = ((sum[0] + sum[1]) + (sum[2] + sum[3])) / 512.f;
-    float q2[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 1
-    for (int c = 0; c < 512; c += 32) {
-      float v[32];
-      tmem_ld32(trow + c, v);
-      tmem_ld_wait();
-      add_bias32(v, bias, c);
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const float a = v[j] - mean, b = v[j + 1] - mean, cc = v[j + 2] - mean, d = v[j + 3] - mean;
-        q2[0] = fmaf(a, a, q2[0]), q2[1] = fmaf(b, b, q2[1]), q2[2] = fmaf(cc, cc, q2[2]), q2[3] = fmaf(d, d, q2[3]);
-      }
-    }
-    const float rstd = 1.f / sqrtf(((q2[0] + q2[1]) + (q2[2] + q2[3])) / 512.f + 1e-5f);
-    const int lane = r & 31;
-#pragma unroll 1
-    for (int c = cg * 32; c < 512; c += 64) {
-      float v[32];
-      tmem_ld32(trow + c, v);
-      tmem_ld_wait();
-      if (c + 64 >= 256 && c < 256) {  // last read of column half 0 by this warp
-        tc_fence_before_sync();
-        mbar_arrive(&tempty[0]);
-      } else if (c + 64 >= 512) {
-        tc_fence_before_sync();
-        mbar_arrive(&tempty[1]);
-      }
-      add_bias32(v, bias, c);
-      const float4* g4 = reinterpret_cast<const float4*>(gamma + c);
-      const float4* b4 = reinterpret_cast<const float4*>(beta + c);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float4 g = __ldg(g4 + j), b = __ldg(b4 + j);
-        v[4 * j] = lg_gelu(fmaf((v[4 * j] - mean) * rstd, g.x, b.x));
-        v[4 * j + 1] = lg_gelu(fmaf((v[4 * j + 1] - mean) * rstd, g.y, b.y));
-        v[4 * j + 2] = lg_gelu(fmaf((v[4 * j + 2] - mean) * rstd, g.z, b.z));
-        v[4 * j + 3] = lg_gelu(fmaf((v[4 * j + 3] - mean) * rstd, g.w, b.w));
-      }
-      float4 f[8];
-      warp_transpose32(v, sc, f);
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        const size_t off = static_cast<size_t>(tc.m0 + (r & ~31) + it * 4 + (lane >> 3)) * 512 + c + (lane & 7) * 4;
-        store_split4(hi + off, lo ? lo + off : nullptr, f[it]);
-      }
-    }
-  }
-};
 
 // x = (residual ? x : 0) + acc + bias -> fp32 master and fp16 hi/lo (first half of the concat buffer)
 struct EpiLgResidual : EpiBase {
@@ -308,1157 +233,45 @@ struct AttnArgs {
   float lazy;         // O / l are rescaled only when a row maximum grows by more than 2^lazy over the reference it was scaled by
 };
 
-// ------------------------------------------------------------------ flash attention v3 (default)
-// 11 warps: two softmax warpgroups (one 128-row query tile each, thread = query row = TMEM lane), one TMA producer
-// warp, one MMA-issuer warp per warpgroup (a single thread cannot issue both tiles' 48 MMAs per key block fast enough).  All hand-offs are mbarriers (no CTA-wide or named barriers in the loop):
-//   issuer : S(j+1) = Q K^T one block ahead into the other TMEM S buffer; O += P(j) V as soon as P(j) is posted
-//   softmax: S(j) -> registers -> (sFree) ; online max ; O rescaled IN TMEM only when a row maximum moved
-//            (tcgen05.ld/st of the warp's own lanes) ; P(j) = exp2(..) hi/lo -> swizzled smem -> (pReady)
-// O lives in TMEM for the whole key loop (the P V MMAs accumulate), so the per-block cost on the CUDA cores is
-// the softmax itself.
+struct AttnOutLg {  // O rows of (side, head) -> fp16 hi / lo planes of the context buffer [R][256], head h at columns 64 h
+  __half *h, *l;
+  __device__ void operator()(int row, int col, float x, float y) const {
+    __half2 hi, lo;
+    split2_f32(x, y, hi, lo);
+    *reinterpret_cast<__half2*>(h + static_cast<size_t>(row) * kD + col) = hi;
+    if (l) *reinterpret_cast<__half2*>(l + static_cast<size_t>(row) * kD + col) = lo;
+  }
+};
+
+// grid (NP / 128, heads, sides): one 128-row query tile of one head of one side per CTA
 template <bool SPLIT>
-__global__ void __launch_bounds__(352, 1)
-lg_attn3_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
-                const __grid_constant__ CUtensorMap tmKh, const __grid_constant__ CUtensorMap tmKl,
-                const __grid_constant__ CUtensorMap tmVh, const __grid_constant__ CUtensorMap tmVl, AttnArgs a) {
-  using namespace tc05;
-  const int side = blockIdx.z, head = blockIdx.y, qbase = blockIdx.x * 2 * kTileM, NP = a.rows.NP;
+__global__ void __launch_bounds__(kAttnThreads, 1)
+lg_attn_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
+               const __grid_constant__ CUtensorMap tmKh, const __grid_constant__ CUtensorMap tmKl,
+               const __grid_constant__ CUtensorMap tmVh, const __grid_constant__ CUtensorMap tmVl, AttnArgs a) {
+  const int side = blockIdx.z, head = blockIdx.y, qbase = blockIdx.x * kAttnTile, NP = a.rows.NP;
   const int ks = a.cross ? (side ^ 1) : side;
   if (a.rows.stopped[side >> 1] != 0) return;
   const int nq = a.rows.n_act[side], nk = a.rows.n_act[ks];
   if (qbase >= nq) return;
-  const int tid = threadIdx.x, warp = tid >> 5, wg = warp >> 2;
-  const int nwg = (qbase + kTileM < nq) ? 2 : 1;
-  if (nk == 0) {  // Attention.forward: empty key set -> zeros (lightglue.py:103-104)
-    if (wg < nwg) {
-      const size_t orow = static_cast<size_t>(side) * NP + qbase + tid;
-      float z[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) z[j] = 0.f;
-      for (int c = 0; c < kHd; c += 32)
-        store_split32(a.ctx_h + orow * kD + head * kHd + c, a.ctx_l ? a.ctx_l + orow * kD + head * kHd + c : nullptr, z);
-    }
-    return;
-  }
-  constexpr int kPl = SPLIT ? 2 : 1;
-  constexpr int kQB = kTileM * 128, kKB = kBlkK * 128, kVB = kHd * 128, kPB = kTileM * 128;
-  extern __shared__ __align__(1024) uint8_t smem3[];
-  uint8_t* sQ = smem3;                       // [wg][plane]
-  uint8_t* sK = sQ + 2 * kPl * kQB;          // [buf][plane]
-  uint8_t* sV = sK + 2 * kPl * kKB;          // [buf][plane]
-  uint8_t* sP = sV + 2 * kPl * kVB;          // [wg][plane]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * kPl * kPB);
-  uint64_t *bQ = bars, *kFull = bars + 2, *kEmpty = bars + 4, *vFull = bars + 6, *vEmpty = bars + 8, *bS = bars + 10 /*[wg][buf]*/,
-           *sFree = bars + 14 /*[wg][buf]*/, *pReady = bars + 18, *bO = bars + 20;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 22);
-  if (tid == 0) {
-    if (smem_u32(smem3) & 1023u) {
-      printf("dimb200: attention smem base not 1024B aligned\n");
-      __trap();
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bQ[i], 1);
-      mbar_init(&kFull[i], 1);
-      mbar_init(&kEmpty[i], nwg);
-      mbar_init(&vFull[i], 1);
-      mbar_init(&vEmpty[i], nwg);
-      mbar_init(&pReady[i], kTileM);
-      mbar_init(&bO[i], 1);
-    }
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(&bS[i], 1);
-      mbar_init(&sFree[i], kTileM);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 0) tmem_alloc(tmem_ptr, 512);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr;
-  const int krow = (ks * kHeads + head) * NP;
-  const int vrow = (ks * kHeads + head) * kHd;
-  const int nblk = (nk + kBlkK - 1) / kBlkK;
-
-  if (warp == 8) {
-    {  // ---------------- TMA producer (whole warp waits, one elected lane issues)
-      if (elect_one()) {
-        for (int w = 0; w < nwg; ++w) {
-          const int qrow = (side * kHeads + head) * NP + qbase + w * kTileM;
-          mbar_expect_tx(&bQ[w], kPl * kQB);
-          tma_load_2d(sQ + w * kPl * kQB, &tmQh, &bQ[w], 0, qrow);
-          if (SPLIT) tma_load_2d(sQ + w * kPl * kQB + kQB, &tmQl, &bQ[w], 0, qrow);
-        }
-      }
-      __syncwarp();
-      for (int j = 0; j < nblk; ++j) {
-        const int s = j & 1;
-        const uint32_t ph = (j >> 1) & 1;
-        mbar_wait(&kEmpty[s], ph ^ 1);
-        if (elect_one()) {
-          mbar_expect_tx(&kFull[s], kPl * kKB);
-          tma_load_2d(sK + s * kPl * kKB, &tmKh, &kFull[s], 0, krow + j * kBlkK);
-          if (SPLIT) tma_load_2d(sK + s * kPl * kKB + kKB, &tmKl, &kFull[s], 0, krow + j * kBlkK);
-        }
-        __syncwarp();
-        mbar_wait(&vEmpty[s], ph ^ 1);
-        if (elect_one()) {
-          mbar_expect_tx(&vFull[s], kPl * kVB);
-          tma_load_2d(sV + s * kPl * kVB, &tmVh, &vFull[s], j * kBlkK, vrow);
-          if (SPLIT) tma_load_2d(sV + s * kPl * kVB + kVB, &tmVl, &vFull[s], j * kBlkK, vrow);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp >= 9) {
-    const int w = warp - 9;  // ---------------- MMA issuer of warpgroup w: the whole warp waits, one elected lane issues (tc05.cuh)
-    if (w < nwg) {
-      constexpr uint32_t idesc = make_idesc_f16(64);
-      const uint32_t q = smem_u32(sQ + w * kPl * kQB);
-      const uint64_t qh = make_sdesc_sw128(q), ql = make_sdesc_sw128(q + kQB);
-      const uint32_t pp = smem_u32(sP + w * kPl * kPB);
-      const uint64_t p_h = make_sdesc_sw128(pp), p_l = make_sdesc_sw128(pp + kPB);
-      const uint32_t dO = tmem_base + w * 192 + 128;
-      auto issue_S = [&](int j) {
-        const int s = j & 1;
-        const uint32_t d = tmem_base + w * 192 + s * 64;
-        const uint32_t k = smem_u32(sK + s * kPl * kKB);
-        const uint64_t kh = make_sdesc_sw128(k), kl = make_sdesc_sw128(k + kKB);
-        if (elect_one()) {
-#pragma unroll
-          for (int k16 = 0; k16 < 4; ++k16) {
-            mma_f16_ss(d, sdesc_advance_k(qh, k16), sdesc_advance_k(kh, k16), idesc, k16 != 0);
-            if (SPLIT) {
-              mma_f16_ss(d, sdesc_advance_k(qh, k16), sdesc_advance_k(kl, k16), idesc, 1);
-              mma_f16_ss(d, sdesc_advance_k(ql, k16), sdesc_advance_k(kh, k16), idesc, 1);
-            }
-          }
-          mma_commit(&bS[w * 2 + s]);
-          mma_commit(&kEmpty[s]);
-        }
-        __syncwarp();
-      };
-      mbar_wait(&bQ[w], 0);
-      mbar_wait(&kFull[0], 0);
-      tc_fence_after_sync();
-      issue_S(0);
-      for (int j = 0; j < nblk; ++j) {
-        if (j + 1 < nblk) {  // next block's scores, one block ahead of the softmax
-          const int s1 = (j + 1) & 1;
-          mbar_wait(&kFull[s1], ((j + 1) >> 1) & 1);
-          if (j >= 1) mbar_wait(&sFree[w * 2 + s1], ((j - 1) >> 1) & 1);
-          tc_fence_after_sync();
-          issue_S(j + 1);
-        }
-        const int sb = j & 1;
-        mbar_wait(&vFull[sb], (j >> 1) & 1);
-        mbar_wait(&pReady[w], j & 1);
-        tc_fence_after_sync();
-        const uint32_t vv = smem_u32(sV + sb * kPl * kVB);
-        const uint64_t v_h = make_sdesc_sw128(vv), v_l = make_sdesc_sw128(vv + kVB);
-        if (elect_one()) {
-#pragma unroll
-          for (int k16 = 0; k16 < 4; ++k16) {
-            mma_f16_ss(dO, sdesc_advance_k(p_h, k16), sdesc_advance_k(v_h, k16), idesc, (j | k16) != 0);
-            if (SPLIT) {
-              mma_f16_ss(dO, sdesc_advance_k(p_h, k16), sdesc_advance_k(v_l, k16), idesc, 1);
-              mma_f16_ss(dO, sdesc_advance_k(p_l, k16), sdesc_advance_k(v_h, k16), idesc, 1);
-            }
-          }
-          mma_commit(&bO[w]);
-          mma_commit(&vEmpty[sb]);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (wg < nwg) {  // ---------------- softmax warpgroups
-    const int r = tid & 127, w4 = warp & 3;
-    const uint32_t lane_off = static_cast<uint32_t>(w4 * 32) << 16;
-    const uint32_t tS0 = tmem_base + wg * 192 + lane_off, tO = tmem_base + wg * 192 + 128 + lane_off;
-    uint8_t* myP = sP + wg * kPl * kPB;
-    float m_run = -INFINITY, l_run = 0.f;
-    const float c2 = a.scale * 1.4426950408889634f;  // softmax(scale * s) via exp2
-    for (int j = 0; j < nblk; ++j) {
-      const int sb = j & 1;
-      mbar_wait(&bS[wg * 2 + sb], (j >> 1) & 1);
-      tc_fence_after_sync();
-      float s[kBlkK];
-      tmem_ld32(tS0 + sb * 64, s);
-      tmem_ld32(tS0 + sb * 64 + 32, s + 32);
-      tmem_ld_wait();
-      tc_fence_before_sync();
-      mbar_arrive(&sFree[wg * 2 + sb]);  // scores are in registers: the issuer may overwrite this buffer
-      const int key0 = j * kBlkK;
-      if (key0 + kBlkK > nk) {
-#pragma unroll
-        for (int c = 0; c < kBlkK; ++c)
-          if (key0 + c >= nk) s[c] = -INFINITY;
-      }
-      float mx[4] = {s[0], s[1], s[2], s[3]};
-#pragma unroll
-      for (int c = 4; c < kBlkK; c += 4) {
-        mx[0] = fmaxf(mx[0], s[c]);
-        mx[1] = fmaxf(mx[1], s[c + 1]);
-        mx[2] = fmaxf(mx[2], s[c + 2]);
-        mx[3] = fmaxf(mx[3], s[c + 3]);
-      }
-      // Lazy rescaling: softmax is invariant to the reference subtracted in the exponent, so the running reference m_run only has
-      // to stay within 2^lazy of the true maximum (P <= 2^lazy, far inside fp16 / fp32 range; the hi/lo split keeps its RELATIVE
-      // precision).  After the first few key blocks the maximum rarely grows by that much, so the O rescale - a TMEM round trip
-      // in the critical path of every block (85 % of the blocks of a 2048-key row otherwise) - almost never runs.
-      const float m_blk = fmaxf(m_run, fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])));
-      const bool grow = (m_blk - m_run) * c2 > a.lazy;      // always true on the first block (m_run = -inf)
-      const float m_new = grow ? m_blk : m_run;
-      const float alpha = grow ? fast_exp2((m_run - m_new) * c2) : 1.f;  // 0 on the first block
-      const float mc = m_new * c2;
-      float ps[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int c = 0; c < kBlkK; c += 4) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          s[c + e] = fast_exp2(fmaf(s[c + e], c2, -mc));
-          ps[e] += s[c + e];
-        }
-      }
-      l_run = l_run * alpha + ((ps[0] + ps[1]) + (ps[2] + ps[3]));
-      m_run = m_new;
-      if (j > 0) {
-        mbar_wait(&bO[wg], (j - 1) & 1);  // P V of the previous block retired: P smem and O are ours again
-        tc_fence_after_sync();
-        if (__any_sync(0xffffffffu, alpha != 1.f)) {  // a row maximum moved: rescale the warp's O rows in TMEM
-          float o[32];
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            tmem_ld32(tO + h * 32, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int d = 0; d < 32; ++d) o[d] *= alpha;
-            tmem_st32(tO + h * 32, o);
-          }
-          tmem_st_wait();
-        }
-      }
-#pragma unroll
-      for (int c8 = 0; c8 < 8; ++c8) {
-        __half2 h[4], l[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) split2_f32(s[c8 * 8 + 2 * e], s[c8 * 8 + 2 * e + 1], h[e], l[e]);
-        const uint32_t off = static_cast<uint32_t>(r * 128 + (((c8 ^ r) & 7) << 4));
-        *reinterpret_cast<uint4*>(myP + off) = *reinterpret_cast<uint4*>(h);
-        if (SPLIT) *reinterpret_cast<uint4*>(myP + kPB + off) = *reinterpret_cast<uint4*>(l);
-      }
-      fence_proxy_async_smem();
-      tc_fence_before_sync();
-      mbar_arrive(&pReady[wg]);
-    }
-    mbar_wait(&bO[wg], (nblk - 1) & 1);
-    tc_fence_after_sync();
-    const int q = qbase + wg * kTileM + r;
-    const float inv = 1.f / l_run;
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float o[32];
-      tmem_ld32(tO + h * 32, o);
-      tmem_ld_wait();
-      if (q < nq) {
-#pragma unroll
-        for (int d = 0; d < 32; ++d) o[d] *= inv;
-        const size_t off = (static_cast<size_t>(side) * NP + q) * kD + head * kHd + h * 32;
-        store_split32(a.ctx_h + off, a.ctx_l ? a.ctx_l + off : nullptr, o);
-      }
-    }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
-  }
+  const size_t obase = (static_cast<size_t>(side) * NP + qbase) * kD + head * kHd;
+  const AttnOutLg out{a.ctx_h + obase, a.ctx_l ? a.ctx_l + obase : nullptr};
+  attn_tile<kHd, SPLIT>(&tmQh, &tmQl, &tmKh, &tmKl, &tmVh, &tmVl, (side * kHeads + head) * NP + qbase, (ks * kHeads + head) * NP,
+                        (ks * kHeads + head) * kHd, nq - qbase, nk, a.scale, a.lazy, out);
 }
 
-// ------------------------------------------------------------------ flash attention v4 (default): two softmax threads per query row
-// Same tiles, TMA rings and barriers as v3, but the softmax of a 128-row query tile is done by EIGHT warps: warps w and w + 4 own the
-// same TMEM lanes, and thread half h owns key columns [32h, 32h + 32) of every 64-key block - with its own running reference, its
-// own row sum and its own O accumulator in TMEM (O_h += P[:, 32h:32h+32] V[32h:32h+32, :], i.e. the two k-halves of the P V product
-// go to different accumulators).  The two partial softmaxes are merged once, after the last key block (split-KV inside the CTA).
-// v3 ran one 64-element dependency chain per warp and key block with two such warps per scheduler (issue slots 39 % busy, tensor
-// pipe 45 %); four half-length chains per scheduler hide each other's MUFU / TMEM / barrier latency.
-// TMEM per tile: S0 | S1 | O_0 | O_1 (4 x 64 columns); 19 warps: 16 softmax, 1 TMA producer, 2 MMA issuers.
-template <bool SPLIT>
-__global__ void __launch_bounds__(608, 1)
-lg_attn4_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
-                const __grid_constant__ CUtensorMap tmKh, const __grid_constant__ CUtensorMap tmKl,
-                const __grid_constant__ CUtensorMap tmVh, const __grid_constant__ CUtensorMap tmVl, AttnArgs a) {
-  using namespace tc05;
-  const int side = blockIdx.z, head = blockIdx.y, qbase = blockIdx.x * 2 * kTileM, NP = a.rows.NP;
-  const int ks = a.cross ? (side ^ 1) : side;
-  if (a.rows.stopped[side >> 1] != 0) return;
-  const int nq = a.rows.n_act[side], nk = a.rows.n_act[ks];
-  if (qbase >= nq) return;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int tile = warp >> 3, half = (warp >> 2) & 1, w4 = warp & 3;  // softmax warps only (warp < 16)
-  const int ntile = (qbase + kTileM < nq) ? 2 : 1;
-  if (nk == 0) {  // Attention.forward: empty key set -> zeros (lightglue.py:103-104)
-    if (warp < 16 && tile < ntile) {
-      const size_t orow = static_cast<size_t>(side) * NP + qbase + tile * kTileM + w4 * 32 + lane;
-      float z[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) z[j] = 0.f;
-      store_split32(a.ctx_h + orow * kD + head * kHd + half * 32, a.ctx_l ? a.ctx_l + orow * kD + head * kHd + half * 32 : nullptr, z);
-    }
-    return;
-  }
-  constexpr int kPl = SPLIT ? 2 : 1;
-  constexpr int kQB = kTileM * 128, kKB = kBlkK * 128, kVB = kHd * 128, kPB = kTileM * 128;
-  extern __shared__ __align__(1024) uint8_t smem3[];
-  uint8_t* sQ = smem3;                       // [tile][plane]
-  uint8_t* sK = sQ + 2 * kPl * kQB;          // [buf][plane]
-  uint8_t* sV = sK + 2 * kPl * kKB;          // [buf][plane]
-  uint8_t* sP = sV + 2 * kPl * kVB;          // [tile][plane]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * kPl * kPB);
-  uint64_t *bQ = bars, *kFull = bars + 2, *kEmpty = bars + 4, *vFull = bars + 6, *vEmpty = bars + 8, *bS = bars + 10 /*[tile][buf]*/,
-           *sFree = bars + 14 /*[tile][buf]*/, *pReady = bars + 18, *bO = bars + 20;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 22);
-  if (tid == 0) {
-    if (smem_u32(smem3) & 1023u) {
-      printf("dimb200: attention smem base not 1024B aligned\n");
-      __trap();
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bQ[i], 1);
-      mbar_init(&kFull[i], 1);
-      mbar_init(&kEmpty[i], ntile);
-      mbar_init(&vFull[i], 1);
-      mbar_init(&vEmpty[i], ntile);
-      mbar_init(&pReady[i], 2 * kTileM);
-      mbar_init(&bO[i], 1);
-    }
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(&bS[i], 1);
-      mbar_init(&sFree[i], 2 * kTileM);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 0) tmem_alloc(tmem_ptr, 512);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr;
-  const int krow = (ks * kHeads + head) * NP;
-  const int vrow = (ks * kHeads + head) * kHd;
-  const int nblk = (nk + kBlkK - 1) / kBlkK;
-
-  if (warp == 16) {  // ---------------- TMA producer (whole warp waits, one elected lane issues)
-    if (elect_one()) {
-      for (int w = 0; w < ntile; ++w) {
-        const int qrow = (side * kHeads + head) * NP + qbase + w * kTileM;
-        mbar_expect_tx(&bQ[w], kPl * kQB);
-        tma_load_2d(sQ + w * kPl * kQB, &tmQh, &bQ[w], 0, qrow);
-        if (SPLIT) tma_load_2d(sQ + w * kPl * kQB + kQB, &tmQl, &bQ[w], 0, qrow);
-      }
-    }
-    __syncwarp();
-    for (int j = 0; j < nblk; ++j) {
-      const int s = j & 1;
-      const uint32_t ph = (j >> 1) & 1;
-      mbar_wait(&kEmpty[s], ph ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&kFull[s], kPl * kKB);
-        tma_load_2d(sK + s * kPl * kKB, &tmKh, &kFull[s], 0, krow + j * kBlkK);
-        if (SPLIT) tma_load_2d(sK + s * kPl * kKB + kKB, &tmKl, &kFull[s], 0, krow + j * kBlkK);
-      }
-      __syncwarp();
-      mbar_wait(&vEmpty[s], ph ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&vFull[s], kPl * kVB);
-        tma_load_2d(sV + s * kPl * kVB, &tmVh, &vFull[s], j * kBlkK, vrow);
-        if (SPLIT) tma_load_2d(sV + s * kPl * kVB + kVB, &tmVl, &vFull[s], j * kBlkK, vrow);
-      }
-      __syncwarp();
-    }
-  } else if (warp >= 17) {
-    const int w = warp - 17;  // ---------------- MMA issuer of tile w: the whole warp waits, one elected lane issues (tc05.cuh)
-    if (w < ntile) {
-      constexpr uint32_t idesc = make_idesc_f16(64);
-      const uint32_t q = smem_u32(sQ + w * kPl * kQB);
-      const uint64_t qh = make_sdesc_sw128(q), ql = make_sdesc_sw128(q + kQB);
-      const uint32_t pp = smem_u32(sP + w * kPl * kPB);
-      const uint64_t p_h = make_sdesc_sw128(pp), p_l = make_sdesc_sw128(pp + kPB);
-      const uint32_t dO = tmem_base + w * 256 + 128;
-      auto issue_S = [&](int j) {
-        const int s = j & 1;
-        const uint32_t d = tmem_base + w * 256 + s * 64;
-        const uint32_t k = smem_u32(sK + s * kPl * kKB);
-        const uint64_t kh = make_sdesc_sw128(k), kl = make_sdesc_sw128(k + kKB);
-        if (elect_one()) {
-#pragma unroll
-          for (int k16 = 0; k16 < 4; ++k16) {
-            mma_f16_ss(d, sdesc_advance_k(qh, k16), sdesc_advance_k(kh, k16), idesc, k16 != 0);
-            if (SPLIT) {
-              mma_f16_ss(d, sdesc_advance_k(qh, k16), sdesc_advance_k(kl, k16), idesc, 1);
-              mma_f16_ss(d, sdesc_advance_k(ql, k16), sdesc_advance_k(kh, k16), idesc, 1);
-            }
-          }
-          mma_commit(&bS[w * 2 + s]);
-          mma_commit(&kEmpty[s]);
-        }
-        __syncwarp();
-      };
-      mbar_wait(&bQ[w], 0);
-      mbar_wait(&kFull[0], 0);
-      tc_fence_after_sync();
-      issue_S(0);
-      for (int j = 0; j < nblk; ++j) {
-        if (j + 1 < nblk) {  // next block's scores, one block ahead of the softmax
-          const int s1 = (j + 1) & 1;
-          mbar_wait(&kFull[s1], ((j + 1) >> 1) & 1);
-          if (j >= 1) mbar_wait(&sFree[w * 2 + s1], ((j - 1) >> 1) & 1);
-          tc_fence_after_sync();
-          issue_S(j + 1);
-        }
-        const int sb = j & 1;
-        mbar_wait(&vFull[sb], (j >> 1) & 1);
-        mbar_wait(&pReady[w], j & 1);
-        tc_fence_after_sync();
-        const uint32_t vv = smem_u32(sV + sb * kPl * kVB);
-        const uint64_t v_h = make_sdesc_sw128(vv), v_l = make_sdesc_sw128(vv + kVB);
-        if (elect_one()) {
-#pragma unroll
-          for (int k16 = 0; k16 < 4; ++k16) {  // keys 0-31 of the block accumulate into O_0, keys 32-63 into O_1
-            const uint32_t d = dO + (k16 >> 1) * 64;
-            mma_f16_ss(d, sdesc_advance_k(p_h, k16), sdesc_advance_k(v_h, k16), idesc, (j | (k16 & 1)) != 0);
-            if (SPLIT) {
-              mma_f16_ss(d, sdesc_advance_k(p_h, k16), sdesc_advance_k(v_l, k16), idesc, 1);
-              mma_f16_ss(d, sdesc_advance_k(p_l, k16), sdesc_advance_k(v_h, k16), idesc, 1);
-            }
-          }
-          mma_commit(&bO[w]);
-          mma_commit(&vEmpty[sb]);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp < 16 && tile < ntile) {  // ---------------- softmax: 8 warps per query tile
-    const int r = w4 * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(w4 * 32) << 16;
-    const uint32_t tS0 = tmem_base + tile * 256 + half * 32 + lane_off;
-    const uint32_t tO = tmem_base + tile * 256 + 128 + lane_off;  // O_0 at +0, O_1 at +64
-    const uint32_t tOmine = tO + half * 64;
-    uint8_t* myP = sP + tile * kPl * kPB;
-    float m_run = -INFINITY, l_run = 0.f;
-    const float c2 = a.scale * 1.4426950408889634f;  // softmax(scale * s) via exp2
-    for (int j = 0; j < nblk; ++j) {
-      const int sb = j & 1;
-      mbar_wait(&bS[tile * 2 + sb], (j >> 1) & 1);
-      tc_fence_after_sync();
-      float s[32];
-      tmem_ld32(tS0 + sb * 64, s);
-      tmem_ld_wait();
-      tc_fence_before_sync();
-      mbar_arrive(&sFree[tile * 2 + sb]);  // scores are in registers: the issuer may overwrite this buffer
-      const int key0 = j * kBlkK + half * 32;
-      if (key0 + 32 > nk) {
-#pragma unroll
-        for (int c = 0; c < 32; ++c)
-          if (key0 + c >= nk) s[c] = -INFINITY;
-      }
-      float mx[4] = {s[0], s[1], s[2], s[3]};
-#pragma unroll
-      for (int c = 4; c < 32; c += 4) {
-        mx[0] = fmaxf(mx[0], s[c]);
-        mx[1] = fmaxf(mx[1], s[c + 1]);
-        mx[2] = fmaxf(mx[2], s[c + 2]);
-        mx[3] = fmaxf(mx[3], s[c + 3]);
-      }
-      // Lazy rescaling as in v3.  A half whose columns are all beyond nk keeps m_run = -inf (grow is false on NaN) and must not
-      // form inf - inf in the exponent: its reference is taken as 0, every P is exp2(-inf) = 0.
-      const float m_blk = fmaxf(m_run, fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])));
-      const bool grow = (m_blk - m_run) * c2 > a.lazy;      // true on the first block with a live key (m_run = -inf)
-      const float m_new = grow ? m_blk : m_run;
-      const float alpha = grow ? fast_exp2((m_run - m_new) * c2) : 1.f;  // 0 on that first block
-      const float mc = (m_new == -INFINITY) ? 0.f : m_new * c2;
-      float2 ps[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
-      const float2 c22 = make_float2(c2, c2), mc2 = make_float2(-mc, -mc);
-#pragma unroll
-      for (int c = 0; c < 32; c += 4) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {  // packed fp32 pairs: one FFMA2 + two MUFU + one FADD2 per two scores
-          const float2 x = ffma2(make_float2(s[c + 2 * e], s[c + 2 * e + 1]), c22, mc2);
-          s[c + 2 * e] = fast_exp2(x.x);
-          s[c + 2 * e + 1] = fast_exp2(x.y);
-          ps[e] = fadd2(ps[e], make_float2(s[c + 2 * e], s[c + 2 * e + 1]));
-        }
-      }
-      l_run = l_run * alpha + ((ps[0].x + ps[0].y) + (ps[1].x + ps[1].y));
-      m_run = m_new;
-      if (j > 0) {
-        mbar_wait(&bO[tile], (j - 1) & 1);  // P V of the previous block retired: P smem and O are ours again
-        tc_fence_after_sync();
-        if (__any_sync(0xffffffffu, alpha != 1.f)) {  // a row maximum moved: rescale the warp's rows of its own O accumulator
-          float o[16];  // 16-column steps: the 32 P values of this block stay in registers next to it
-#pragma unroll
-          for (int h = 0; h < 4; ++h) {
-            tmem_ld16(tOmine + h * 16, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int d = 0; d < 16; ++d) o[d] *= alpha;
-            tmem_st16(tOmine + h * 16, o);
-          }
-          tmem_st_wait();
-        }
-      }
-#pragma unroll
-      for (int c4 = 0; c4 < 4; ++c4) {
-        __half2 h[4], l[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float2 p = make_float2(s[c4 * 8 + 2 * e], s[c4 * 8 + 2 * e + 1]);
-          h[e] = __floats2half2_rn(p.x, p.y);
-          const float2 d = fsub2(p, __half22float2(h[e]));  // exact residual (same values as split2_f32, one FADD2)
-          l[e] = __floats2half2_rn(d.x, d.y);
-        }
-        const int c8 = half * 4 + c4;
-        const uint32_t off = static_cast<uint32_t>(r * 128 + (((c8 ^ r) & 7) << 4));
-        *reinterpret_cast<uint4*>(myP + off) = *reinterpret_cast<uint4*>(h);
-        if (SPLIT) *reinterpret_cast<uint4*>(myP + kPB + off) = *reinterpret_cast<uint4*>(l);
-      }
-      fence_proxy_async_smem();
-      tc_fence_before_sync();
-      mbar_arrive(&pReady[tile]);
-    }
-    mbar_wait(&bO[tile], (nblk - 1) & 1);
-    tc_fence_after_sync();
-    // merge the two halves: the P tile is free now, use it to exchange (reference, row sum)
-    float2* stat = reinterpret_cast<float2*>(myP);
-    stat[half * kTileM + r] = make_float2(m_run, l_run);
-    asm volatile("bar.sync %0, %1;" ::"r"(1 + tile), "r"(2 * kTileM) : "memory");
-    const float2 other = stat[(half ^ 1) * kTileM + r];
-    const float m_all = fmaxf(m_run, other.x);  // finite: block 0 has a live key in half 0
-    const float w_me = fast_exp2((m_run - m_all) * c2), w_ot = fast_exp2((other.x - m_all) * c2);
-    const float inv = 1.f / (l_run * w_me + other.y * w_ot);
-    const float w0 = (half ? w_ot : w_me) * inv, w1 = (half ? w_me : w_ot) * inv;
-    const int q = qbase + tile * kTileM + r;
-    float o0[32], o1[32];  // this thread finishes output dims [32 half, 32 half + 32)
-    tmem_ld32(tO + half * 32, o0);
-    tmem_ld32(tO + 64 + half * 32, o1);
-    tmem_ld_wait();
-    if (q < nq) {
-#pragma unroll
-      for (int d = 0; d < 32; ++d) o0[d] = o0[d] * w0 + o1[d] * w1;
-      const size_t off = (static_cast<size_t>(side) * NP + q) * kD + head * kHd + half * 32;
-      store_split32(a.ctx_h + off, a.ctx_l ? a.ctx_l + off : nullptr, o0);
-    }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// ------------------------------------------------------------------ flash attention v5: P stays in tensor memory
-// v3 / v4 are bound by the shared-memory pipe, not by the tensor pipe (ncu: l1tex 82 %, tensor 55 %): per 64-key block and query
-// tile the MMAs read 72 KB (Q K^T) + 72 KB (P V) of operands, the softmax threads write 32 KB of P and TMA fills 16 KB - 192 KB
-// = 1536 cycles of a 128 B/clk pipe against 768 tensor cycles.  Here P never touches shared memory: the softmax thread stores its
-// row of P (fp16 hi words | lo words) with tcgen05.st into the TMEM columns its scores came from, and the P V product reads the A
-// operand from tensor memory (tcgen05.mma [d], [a_tmem], b_desc - probed, tools/probe_tmem_a.py).  What is left on the shared-
-// memory pipe is 72 KB (Q K^T) + 24 KB (the V^T operand) + 16 KB of fill = 112 KB per block and tile.
-//   TMEM per query tile: S/P ring of three 64-column slots + O (64 columns) = 256 columns; two tiles = all 512.
-//   S(j+1) goes to slot (j+1) % 3 while the softmax owns slot j % 3 and P V(j-1) may still read slot (j-1) % 3; the MMAs of one
-//   issuer retire in issue order, so no "slot free" barrier is needed (v3's sFree is gone).
-//   The shared memory P used to occupy now holds a four-deep K / V^T ring.
-//   DEFER (v7): the softmax thread waits for "P V(j-1) retired" only when it has to rescale O (rare under lazy rescaling); otherwise it
-//   posts P(j) at once and consumes that barrier phase one block later - phases are still consumed one by one and in order, so the
-//   parity wait stays unambiguous - and P V(j) queues right behind P V(j-1) instead of a barrier round trip later.
-constexpr int kAttn5Stages = 4;
-template <bool SPLIT, bool DEFER = false>
-__global__ void __launch_bounds__(352, 1)
-lg_attn5_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
-                const __grid_constant__ CUtensorMap tmKh, const __grid_constant__ CUtensorMap tmKl,
-                const __grid_constant__ CUtensorMap tmVh, const __grid_constant__ CUtensorMap tmVl, AttnArgs a) {
-  using namespace tc05;
-  const int side = blockIdx.z, head = blockIdx.y, qbase = blockIdx.x * 2 * kTileM, NP = a.rows.NP;
-  const int ks = a.cross ? (side ^ 1) : side;
-  if (a.rows.stopped[side >> 1] != 0) return;
-  const int nq = a.rows.n_act[side], nk = a.rows.n_act[ks];
-  if (qbase >= nq) return;
-  const int tid = threadIdx.x, warp = tid >> 5, wg = warp >> 2;
-  const int nwg = (qbase + kTileM < nq) ? 2 : 1;
-  if (nk == 0) {  // Attention.forward: empty key set -> zeros (lightglue.py:103-104)
-    if (wg < nwg) {
-      const size_t orow = static_cast<size_t>(side) * NP + qbase + tid;
-      float z[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) z[j] = 0.f;
-      for (int c = 0; c < kHd; c += 32)
-        store_split32(a.ctx_h + orow * kD + head * kHd + c, a.ctx_l ? a.ctx_l + orow * kD + head * kHd + c : nullptr, z);
-    }
-    return;
-  }
-  constexpr int kPl = SPLIT ? 2 : 1, KST = kAttn5Stages;
-  constexpr int kQB = kTileM * 128, kKB = kBlkK * 128, kVB = kHd * 128;
-  extern __shared__ __align__(1024) uint8_t smem5[];
-  uint8_t* sQ = smem5;                       // [wg][plane]
-  uint8_t* sK = sQ + 2 * kPl * kQB;          // [stage][plane]
-  uint8_t* sV = sK + KST * kPl * kKB;        // [stage][plane]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + KST * kPl * kVB);
-  uint64_t *bQ = bars, *kFull = bQ + 2, *kEmpty = kFull + KST, *vFull = kEmpty + KST, *vEmpty = vFull + KST,
-           *bS = vEmpty + KST /*[wg][3]*/, *pReady = bS + 6, *bO = pReady + 2 /*[wg][2]: P V of even / odd blocks*/;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bO + 4);
-  if (tid == 0) {
-    if (smem_u32(smem5) & 1023u) {
-      printf("dimb200: attention smem base not 1024B aligned\n");
-      __trap();
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bQ[i], 1);
-      mbar_init(&pReady[i], kTileM);
-      mbar_init(&bO[2 * i], 1);
-      mbar_init(&bO[2 * i + 1], 1);
-    }
-    for (int i = 0; i < KST; ++i) {
-      mbar_init(&kFull[i], 1);
-      mbar_init(&kEmpty[i], nwg);
-      mbar_init(&vFull[i], 1);
-      mbar_init(&vEmpty[i], nwg);
-    }
-    for (int i = 0; i < 6; ++i) mbar_init(&bS[i], 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) tmem_alloc(tmem_ptr, 512);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr;
-  const int krow = (ks * kHeads + head) * NP;
-  const int vrow = (ks * kHeads + head) * kHd;
-  const int nblk = (nk + kBlkK - 1) / kBlkK;
-
-  if (warp == 8) {
-    {  // ---------------- TMA producer (whole warp waits, one elected lane issues)
-      if (elect_one()) {
-        for (int w = 0; w < nwg; ++w) {
-          const int qrow = (side * kHeads + head) * NP + qbase + w * kTileM;
-          mbar_expect_tx(&bQ[w], kPl * kQB);
-          tma_load_2d(sQ + w * kPl * kQB, &tmQh, &bQ[w], 0, qrow);
-          if (SPLIT) tma_load_2d(sQ + w * kPl * kQB + kQB, &tmQl, &bQ[w], 0, qrow);
-        }
-      }
-      __syncwarp();
-      for (int j = 0; j < nblk; ++j) {
-        const int s = j % KST;
-        const uint32_t ph = (j / KST) & 1;
-        mbar_wait(&kEmpty[s], ph ^ 1);
-        if (elect_one()) {
-          mbar_expect_tx(&kFull[s], kPl * kKB);
-          tma_load_2d(sK + s * kPl * kKB, &tmKh, &kFull[s], 0, krow + j * kBlkK);
-          if (SPLIT) tma_load_2d(sK + s * kPl * kKB + kKB, &tmKl, &kFull[s], 0, krow + j * kBlkK);
-        }
-        __syncwarp();
-        mbar_wait(&vEmpty[s], ph ^ 1);
-        if (elect_one()) {
-          mbar_expect_tx(&vFull[s], kPl * kVB);
-          tma_load_2d(sV + s * kPl * kVB, &tmVh, &vFull[s], j * kBlkK, vrow);
-          if (SPLIT) tma_load_2d(sV + s * kPl * kVB + kVB, &tmVl, &vFull[s], j * kBlkK, vrow);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp >= 9) {
-    const int w = warp - 9;  // ---------------- MMA issuer of query tile w: the whole warp waits, one elected lane issues
-    if (w < nwg) {
-      constexpr uint32_t idesc = make_idesc_f16(64);
-      const uint32_t q = smem_u32(sQ + w * kPl * kQB);
-      const uint64_t qh = make_sdesc_sw128(q), ql = make_sdesc_sw128(q + kQB);
-      const uint32_t tW = tmem_base + w * 256, dO = tW + 192;
-      auto issue_S = [&](int j) {
-        const int s = j % KST;
-        const uint32_t d = tW + (j % 3) * 64;
-        const uint32_t k = smem_u32(sK + s * kPl * kKB);
-        const uint64_t kh = make_sdesc_sw128(k), kl = make_sdesc_sw128(k + kKB);
-        if (elect_one()) {
-#pragma unroll
-          for (int k16 = 0; k16 < 4; ++k16) {
-            mma_f16_ss(d, sdesc_advance_k(qh, k16), sdesc_advance_k(kh, k16), idesc, k16 != 0);
-            if (SPLIT) {
-              mma_f16_ss(d, sdesc_advance_k(qh, k16), sdesc_advance_k(kl, k16), idesc, 1);
-              mma_f16_ss(d, sdesc_advance_k(ql, k16), sdesc_advance_k(kh, k16), idesc, 1);
-            }
-          }
-          mma_commit(&bS[w * 3 + j % 3]);
-          mma_commit(&kEmpty[s]);
-        }
-        __syncwarp();
-      };
-      mbar_wait(&bQ[w], 0);
-      mbar_wait(&kFull[0], 0);
-      tc_fence_after_sync();
-      issue_S(0);
-      for (int j = 0; j < nblk; ++j) {
-        if (j + 1 < nblk) {  // next block's scores, one block ahead of the softmax (slot (j+1) % 3: last read by P V(j-2), already issued)
-          mbar_wait(&kFull[(j + 1) % KST], ((j + 1) / KST) & 1);
-          tc_fence_after_sync();
-          issue_S(j + 1);
-        }
-        const int sb = j % KST;
-        mbar_wait(&vFull[sb], (j / KST) & 1);
-        mbar_wait(&pReady[w], j & 1);
-        tc_fence_after_sync();
-        const uint32_t vv = smem_u32(sV + sb * kPl * kVB);
-        const uint64_t v_h = make_sdesc_sw128(vv), v_l = make_sdesc_sw128(vv + kVB);
-        const uint32_t tP = tW + (j % 3) * 64;  // hi words in columns [0, 32), lo words in [32, 64); 8 columns per 16 keys
-        if (elect_one()) {
-#pragma unroll
-          for (int k16 = 0; k16 < 4; ++k16) {
-            mma_f16_ts(dO, tP + k16 * 8, sdesc_advance_k(v_h, k16), idesc, (j | k16) != 0);
-            if (SPLIT) {
-              mma_f16_ts(dO, tP + k16 * 8, sdesc_advance_k(v_l, k16), idesc, 1);
-              mma_f16_ts(dO, tP + 32 + k16 * 8, sdesc_advance_k(v_h, k16), idesc, 1);
-            }
-          }
-          mma_commit(&bO[2 * w + (j & 1)]);
-          mma_commit(&vEmpty[sb]);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (wg < nwg) {  // ---------------- softmax warpgroups: thread = query row = TMEM lane
-    const int r = tid & 127, w4 = warp & 3;
-    const uint32_t lane_off = static_cast<uint32_t>(w4 * 32) << 16;
-    const uint32_t tS0 = tmem_base + wg * 256 + lane_off, tO = tS0 + 192;
-    float m_run = -INFINITY, l_run = 0.f;
-    // "P V(b) retired" = phase b >> 1 of barrier bO[wg][b & 1].  A parity wait can tell a phase only from its neighbour, so phases are
-    // consumed in order and a barrier may never run two phases ahead of its consumer: P V(b + 2) completes the next phase of the same
-    // barrier and cannot be issued before this thread posts P(b + 2) - which it does only after consuming block b.
-    int consumed[2] = {0, 0};
-    auto consume = [&](int b) {
-      const int p = b & 1;
-      if (consumed[p] <= (b >> 1)) {
-        mbar_wait(&bO[2 * wg + p], consumed[p] & 1);
-        ++consumed[p];
-      }
-    };
-    const float c2 = a.scale * 1.4426950408889634f;  // softmax(scale * s) via exp2
-    for (int j = 0; j < nblk; ++j) {
-      const int slot = j % 3;
-      mbar_wait(&bS[wg * 3 + slot], (j / 3) & 1);
-      tc_fence_after_sync();
-      float s[kBlkK];
-      tmem_ld32(tS0 + slot * 64, s);
-      tmem_ld32(tS0 + slot * 64 + 32, s + 32);
-      tmem_ld_wait();
-      const int key0 = j * kBlkK;
-      if (key0 + kBlkK > nk) {
-#pragma unroll
-        for (int c = 0; c < kBlkK; ++c)
-          if (key0 + c >= nk) s[c] = -INFINITY;
-      }
-      float mx[4] = {s[0], s[1], s[2], s[3]};
-#pragma unroll
-      for (int c = 4; c < kBlkK; c += 4) {
-        mx[0] = fmaxf(mx[0], s[c]);
-        mx[1] = fmaxf(mx[1], s[c + 1]);
-        mx[2] = fmaxf(mx[2], s[c + 2]);
-        mx[3] = fmaxf(mx[3], s[c + 3]);
-      }
-      // lazy rescaling as in v3: the running reference only has to stay within 2^lazy of the true maximum
-      const float m_blk = fmaxf(m_run, fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])));
-      const bool grow = (m_blk - m_run) * c2 > a.lazy;      // always true on the first block (m_run = -inf)
-      const float m_new = grow ? m_blk : m_run;
-      const float alpha = grow ? fast_exp2((m_run - m_new) * c2) : 1.f;  // 0 on the first block
-      const float mc = m_new * c2;
-      float2 ps[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
-      const float2 c22 = make_float2(c2, c2), mc2 = make_float2(-mc, -mc);
-#pragma unroll
-      for (int c = 0; c < kBlkK; c += 4) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {  // packed fp32 pairs: one FFMA2 + two MUFU + one FADD2 per two scores (same values, same summation order)
-          const float2 x = ffma2(make_float2(s[c + 2 * e], s[c + 2 * e + 1]), c22, mc2);
-          s[c + 2 * e] = fast_exp2(x.x);
-          s[c + 2 * e + 1] = fast_exp2(x.y);
-          ps[e] = fadd2(ps[e], make_float2(s[c + 2 * e], s[c + 2 * e + 1]));
-        }
-      }
-      l_run = l_run * alpha + ((ps[0].x + ps[0].y) + (ps[1].x + ps[1].y));
-      m_run = m_new;
-      // P(j) -> this row's TMEM slot (the scores are in registers; P V(j-1) reads another slot)
-      {
-        __half2 ph[32], pl[32];
-#pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          const float2 p = make_float2(s[2 * c], s[2 * c + 1]);
-          ph[c] = __floats2half2_rn(p.x, p.y);
-          const float2 d = fsub2(p, __half22float2(ph[c]));  // exact residual (same values as split2_f32, one FADD2)
-          pl[c] = __floats2half2_rn(d.x, d.y);
-        }
-        tmem_st32(tS0 + slot * 64, reinterpret_cast<const float*>(ph));
-        if (SPLIT) tmem_st32(tS0 + slot * 64 + 32, reinterpret_cast<const float*>(pl));
-      }
-      if (j > 0) {
-        const bool resc = __any_sync(0xffffffffu, alpha != 1.f);  // a row maximum moved: the warp's O rows have to be rescaled in TMEM
-        if (j >= 2) consume(j - 2);          // long retired: never blocks
-        if (!DEFER || resc) consume(j - 1);  // O is touched only when a row maximum moved (DEFER); v5 always waits
-        if (resc) {
-          tc_fence_after_sync();
-          float o[32];
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            tmem_ld32(tO + h * 32, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int d = 0; d < 32; ++d) o[d] *= alpha;
-            tmem_st32(tO + h * 32, o);
-          }
-        }
-      }
-      tmem_st_wait();
-      tc_fence_before_sync();
-      mbar_arrive(&pReady[wg]);
-    }
-    if (nblk >= 2) consume(nblk - 2);
-    consume(nblk - 1);  // the last P V retired: O is final
-    tc_fence_after_sync();
-    const int q = qbase + wg * kTileM + r;
-    const float inv = 1.f / l_run;
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float o[32];
-      tmem_ld32(tO + h * 32, o);
-      tmem_ld_wait();
-      if (q < nq) {
-#pragma unroll
-        for (int d = 0; d < 32; ++d) o[d] *= inv;
-        const size_t off = (static_cast<size_t>(side) * NP + q) * kD + head * kHd + h * 32;
-        store_split32(a.ctx_h + off, a.ctx_l ? a.ctx_l + off : nullptr, o);
-      }
-    }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// ------------------------------------------------------------------ flash attention v6: v5 (P in tensor memory) with v4's two softmax threads per row
-// With P out of shared memory the tensor pipe is no longer starved by the operand fetch (v5: tensor 63 %, shared-memory pipe 63 %)
-// but by the softmax dependency chain of the two warpgroups (issue slots 46 %, two softmax warps per scheduler).  v6 runs that chain on
-// 16 warps: warps w and w + 4 of a query tile own the same TMEM lanes, thread half h owns key columns [32h, 32h + 32) of every 64-key
-// block - its own running reference, row sum and O accumulator (O_h += P[:, 32h:32h+32] V[32h:32h+32, :]); merged once at the end.
-//   TMEM per tile: S0 | S1 | O_0 | O_1 (4 x 64 columns).  A half writes its P into the 32 columns its scores came from: hi words
-//   (16 columns) then lo words (16 columns) - no cross-half hazard, and the A operand of k-step u of half h is columns
-//   32h + 8u (hi) / 32h + 16 + 8u (lo).  S(j+1) overwrites the slot of P(j-1) only after P V(j-1) - issued earlier by the same
-//   thread, and MMAs retire in issue order - so the two-slot ring needs no "slot free" barrier.
-template <bool SPLIT>
-__global__ void __launch_bounds__(608, 1)
-lg_attn6_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
-                const __grid_constant__ CUtensorMap tmKh, const __grid_constant__ CUtensorMap tmKl,
-                const __grid_constant__ CUtensorMap tmVh, const __grid_constant__ CUtensorMap tmVl, AttnArgs a) {
-  using namespace tc05;
-  const int side = blockIdx.z, head = blockIdx.y, qbase = blockIdx.x * 2 * kTileM, NP = a.rows.NP;
-  const int ks = a.cross ? (side ^ 1) : side;
-  if (a.rows.stopped[side >> 1] != 0) return;
-  const int nq = a.rows.n_act[side], nk = a.rows.n_act[ks];
-  if (qbase >= nq) return;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int tile = warp >> 3, half = (warp >> 2) & 1, w4 = warp & 3;  // softmax warps only (warp < 16)
-  const int ntile = (qbase + kTileM < nq) ? 2 : 1;
-  if (nk == 0) {  // Attention.forward: empty key set -> zeros (lightglue.py:103-104)
-    if (warp < 16 && tile < ntile) {
-      const size_t orow = static_cast<size_t>(side) * NP + qbase + tile * kTileM + w4 * 32 + lane;
-      float z[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) z[j] = 0.f;
-      store_split32(a.ctx_h + orow * kD + head * kHd + half * 32, a.ctx_l ? a.ctx_l + orow * kD + head * kHd + half * 32 : nullptr, z);
-    }
-    return;
-  }
-  constexpr int kPl = SPLIT ? 2 : 1, KST = kAttn5Stages;
-  constexpr int kQB = kTileM * 128, kKB = kBlkK * 128, kVB = kHd * 128;
-  extern __shared__ __align__(1024) uint8_t smem6[];
-  uint8_t* sQ = smem6;                       // [tile][plane]
-  uint8_t* sK = sQ + 2 * kPl * kQB;          // [stage][plane]
-  uint8_t* sV = sK + KST * kPl * kKB;        // [stage][plane]
-  float2* stat = reinterpret_cast<float2*>(sV + KST * kPl * kVB);  // [tile][half][128] (reference, row sum) for the final merge
-  uint64_t* bars = reinterpret_cast<uint64_t*>(stat + 2 * 2 * kTileM);
-  uint64_t *bQ = bars, *kFull = bQ + 2, *kEmpty = kFull + KST, *vFull = kEmpty + KST, *vEmpty = vFull + KST,
-           *bS = vEmpty + KST /*[tile][2]*/, *pReady = bS + 4, *bO = pReady + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bO + 2);
-  if (tid == 0) {
-    if (smem_u32(smem6) & 1023u) {
-      printf("dimb200: attention smem base not 1024B aligned\n");
-      __trap();
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bQ[i], 1);
-      mbar_init(&pReady[i], 2 * kTileM);
-      mbar_init(&bO[i], 1);
-    }
-    for (int i = 0; i < KST; ++i) {
-      mbar_init(&kFull[i], 1);
-      mbar_init(&kEmpty[i], ntile);
-      mbar_init(&vFull[i], 1);
-      mbar_init(&vEmpty[i], ntile);
-    }
-    for (int i = 0; i < 4; ++i) mbar_init(&bS[i], 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) tmem_alloc(tmem_ptr, 512);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr;
-  const int krow = (ks * kHeads + head) * NP;
-  const int vrow = (ks * kHeads + head) * kHd;
-  const int nblk = (nk + kBlkK - 1) / kBlkK;
-
-  if (warp == 16) {  // ---------------- TMA producer (whole warp waits, one elected lane issues)
-    if (elect_one()) {
-      for (int w = 0; w < ntile; ++w) {
-        const int qrow = (side * kHeads + head) * NP + qbase + w * kTileM;
-        mbar_expect_tx(&bQ[w], kPl * kQB);
-        tma_load_2d(sQ + w * kPl * kQB, &tmQh, &bQ[w], 0, qrow);
-        if (SPLIT) tma_load_2d(sQ + w * kPl * kQB + kQB, &tmQl, &bQ[w], 0, qrow);
-      }
-    }
-    __syncwarp();
-    for (int j = 0; j < nblk; ++j) {
-      const int s = j % KST;
-      const uint32_t ph = (j / KST) & 1;
-      mbar_wait(&kEmpty[s], ph ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&kFull[s], kPl * kKB);
-        tma_load_2d(sK + s * kPl * kKB, &tmKh, &kFull[s], 0, krow + j * kBlkK);
-        if (SPLIT) tma_load_2d(sK + s * kPl * kKB + kKB, &tmKl, &kFull[s], 0, krow + j * kBlkK);
-      }
-      __syncwarp();
-      mbar_wait(&vEmpty[s], ph ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&vFull[s], kPl * kVB);
-        tma_load_2d(sV + s * kPl * kVB, &tmVh, &vFull[s], j * kBlkK, vrow);
-        if (SPLIT) tma_load_2d(sV + s * kPl * kVB + kVB, &tmVl, &vFull[s], j * kBlkK, vrow);
-      }
-      __syncwarp();
-    }
-  } else if (warp >= 17) {
-    const int w = warp - 17;  // ---------------- MMA issuer of tile w: the whole warp waits, one elected lane issues (tc05.cuh)
-    if (w < ntile) {
-      constexpr uint32_t idesc = make_idesc_f16(64);
-      const uint32_t q = smem_u32(sQ + w * kPl * kQB);
-      const uint64_t qh = make_sdesc_sw128(q), ql = make_sdesc_sw128(q + kQB);
-      const uint32_t tW = tmem_base + w * 256, dO = tW + 128;
-      auto issue_S = [&](int j) {
-        const int s = j % KST;
-        const uint32_t d = tW + (j & 1) * 64;
-        const uint32_t k = smem_u32(sK + s * kPl * kKB);
-        const uint64_t kh = make_sdesc_sw128(k), kl = make_sdesc_sw128(k + kKB);
-        if (elect_one()) {
-#pragma unroll
-          for (int k16 = 0; k16 < 4; ++k16) {
-            mma_f16_ss(d, sdesc_advance_k(qh, k16), sdesc_advance_k(kh, k16), idesc, k16 != 0);
-            if (SPLIT) {
-              mma_f16_ss(d, sdesc_advance_k(qh, k16), sdesc_advance_k(kl, k16), idesc, 1);
-              mma_f16_ss(d, sdesc_advance_k(ql, k16), sdesc_advance_k(kh, k16), idesc, 1);
-            }
-          }
-          mma_commit(&bS[w * 2 + (j & 1)]);
-          mma_commit(&kEmpty[s]);
-        }
-        __syncwarp();
-      };
-      mbar_wait(&bQ[w], 0);
-      mbar_wait(&kFull[0], 0);
-      tc_fence_after_sync();
-      issue_S(0);
-      for (int j = 0; j < nblk; ++j) {
-        if (j + 1 < nblk) {  // next block's scores into the slot of P(j-1): P V(j-1) was issued one iteration ago
-          mbar_wait(&kFull[(j + 1) % KST], ((j + 1) / KST) & 1);
-          tc_fence_after_sync();
-          issue_S(j + 1);
-        }
-        const int sb = j % KST;
-        mbar_wait(&vFull[sb], (j / KST) & 1);
-        mbar_wait(&pReady[w], j & 1);
-        tc_fence_after_sync();
-        const uint32_t vv = smem_u32(sV + sb * kPl * kVB);
-        const uint64_t v_h = make_sdesc_sw128(vv), v_l = make_sdesc_sw128(vv + kVB);
-        const uint32_t tP = tW + (j & 1) * 64;
-        if (elect_one()) {
-#pragma unroll
-          for (int k16 = 0; k16 < 4; ++k16) {  // keys 0-31 of the block accumulate into O_0, keys 32-63 into O_1
-            const uint32_t d = dO + (k16 >> 1) * 64;
-            const uint32_t ah = tP + (k16 >> 1) * 32 + (k16 & 1) * 8, al = ah + 16;
-            mma_f16_ts(d, ah, sdesc_advance_k(v_h, k16), idesc, (j | (k16 & 1)) != 0);
-            if (SPLIT) {
-              mma_f16_ts(d, ah, sdesc_advance_k(v_l, k16), idesc, 1);
-              mma_f16_ts(d, al, sdesc_advance_k(v_h, k16), idesc, 1);
-            }
-          }
-          mma_commit(&bO[w]);
-          mma_commit(&vEmpty[sb]);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp < 16 && tile < ntile) {  // ---------------- softmax: 8 warps per query tile
-    const int r = w4 * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(w4 * 32) << 16;
-    const uint32_t tS0 = tmem_base + tile * 256 + half * 32 + lane_off;
-    const uint32_t tO = tmem_base + tile * 256 + 128 + lane_off;  // O_0 at +0, O_1 at +64
-    const uint32_t tOmine = tO + half * 64;
-    float m_run = -INFINITY, l_run = 0.f;
-    const float c2 = a.scale * 1.4426950408889634f;  // softmax(scale * s) via exp2
-    for (int j = 0; j < nblk; ++j) {
-      const int sb = j & 1;
-      mbar_wait(&bS[tile * 2 + sb], (j >> 1) & 1);
-      tc_fence_after_sync();
-      float s[32];
-      tmem_ld32(tS0 + sb * 64, s);
-      tmem_ld_wait();
-      const int key0 = j * kBlkK + half * 32;
-      if (key0 + 32 > nk) {
-#pragma unroll
-        for (int c = 0; c < 32; ++c)
-          if (key0 + c >= nk) s[c] = -INFINITY;
-      }
-      float mx[4] = {s[0], s[1], s[2], s[3]};
-#pragma unroll
-      for (int c = 4; c < 32; c += 4) {
-        mx[0] = fmaxf(mx[0], s[c]);
-        mx[1] = fmaxf(mx[1], s[c + 1]);
-        mx[2] = fmaxf(mx[2], s[c + 2]);
-        mx[3] = fmaxf(mx[3], s[c + 3]);
-      }
-      // Lazy rescaling as in v3 / v4 (a half whose columns are all beyond nk keeps m_run = -inf and takes 0 as its reference)
-      const float m_blk = fmaxf(m_run, fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])));
-      const bool grow = (m_blk - m_run) * c2 > a.lazy;      // true on the first block with a live key (m_run = -inf)
-      const float m_new = grow ? m_blk : m_run;
-      const float alpha = grow ? fast_exp2((m_run - m_new) * c2) : 1.f;  // 0 on that first block
-      const float mc = (m_new == -INFINITY) ? 0.f : m_new * c2;
-      float2 ps[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
-      const float2 c22 = make_float2(c2, c2), mc2 = make_float2(-mc, -mc);
-#pragma unroll
-      for (int c = 0; c < 32; c += 4) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {  // packed fp32 pairs: one FFMA2 + two MUFU + one FADD2 per two scores
-          const float2 x = ffma2(make_float2(s[c + 2 * e], s[c + 2 * e + 1]), c22, mc2);
-          s[c + 2 * e] = fast_exp2(x.x);
-          s[c + 2 * e + 1] = fast_exp2(x.y);
-          ps[e] = fadd2(ps[e], make_float2(s[c + 2 * e], s[c + 2 * e + 1]));
-        }
-      }
-      l_run = l_run * alpha + ((ps[0].x + ps[0].y) + (ps[1].x + ps[1].y));
-      m_run = m_new;
-      {  // P(j) -> the 32 TMEM columns this thread's scores came from: 16 hi words, then 16 lo words
-        __half2 ph[16], pl[16];
-#pragma unroll
-        for (int c = 0; c < 16; ++c) {
-          const float2 p = make_float2(s[2 * c], s[2 * c + 1]);
-          ph[c] = __floats2half2_rn(p.x, p.y);
-          const float2 d = fsub2(p, __half22float2(ph[c]));  // exact residual (same values as split2_f32, one FADD2)
-          pl[c] = __floats2half2_rn(d.x, d.y);
-        }
-        tmem_st16(tS0 + sb * 64, reinterpret_cast<const float*>(ph));
-        if (SPLIT) tmem_st16(tS0 + sb * 64 + 16, reinterpret_cast<const float*>(pl));
-      }
-      if (j > 0) {
-        mbar_wait(&bO[tile], (j - 1) & 1);  // P V of the previous block retired: O is ours until P(j) is posted
-        tc_fence_after_sync();
-        if (__any_sync(0xffffffffu, alpha != 1.f)) {  // a row maximum moved: rescale the warp's rows of its own O accumulator
-          float o[16];
-#pragma unroll
-          for (int h = 0; h < 4; ++h) {
-            tmem_ld16(tOmine + h * 16, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int d = 0; d < 16; ++d) o[d] *= alpha;
-            tmem_st16(tOmine + h * 16, o);
-          }
-        }
-      }
-      tmem_st_wait();
-      tc_fence_before_sync();
-      mbar_arrive(&pReady[tile]);
-    }
-    mbar_wait(&bO[tile], (nblk - 1) & 1);
-    tc_fence_after_sync();
-    // merge the two halves: exchange (reference, row sum) through shared memory
-    float2* st2 = stat + tile * 2 * kTileM;
-    st2[half * kTileM + r] = make_float2(m_run, l_run);
-    asm volatile("bar.sync %0, %1;" ::"r"(1 + tile), "r"(2 * kTileM) : "memory");
-    const float2 other = st2[(half ^ 1) * kTileM + r];
-    const float m_all = fmaxf(m_run, other.x);  // finite: block 0 has a live key in half 0
-    const float w_me = fast_exp2((m_run - m_all) * c2), w_ot = fast_exp2((other.x - m_all) * c2);
-    const float inv = 1.f / (l_run * w_me + other.y * w_ot);
-    const float w0 = (half ? w_ot : w_me) * inv, w1 = (half ? w_me : w_ot) * inv;
-    const int q = qbase + tile * kTileM + r;
-    float o0[32], o1[32];  // this thread finishes output dims [32 half, 32 half + 32)
-    tmem_ld32(tO + half * 32, o0);
-    tmem_ld32(tO + 64 + half * 32, o1);
-    tmem_ld_wait();
-    if (q < nq) {
-#pragma unroll
-      for (int d = 0; d < 32; ++d) o0[d] = o0[d] * w0 + o1[d] * w1;
-      const size_t off = (static_cast<size_t>(side) * NP + q) * kD + head * kHd + half * 32;
-      store_split32(a.ctx_h + off, a.ctx_l ? a.ctx_l + off : nullptr, o0);
-    }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// Launch of the tensor-core attention (DIMB_ATTN selects 3 / 4 / 5 / 6).
+// Launch of the tensor-core attention (grid.y = heads, grid.z = sides; grid.x is set here: one CTA per 128-row query tile).
 inline int launch_lg_attention(dimb_ctx* ctx, cudaStream_t st, dim3 grid, const CUtensorMap* Q, const CUtensorMap* K, const CUtensorMap* V,
                                const AttnArgs& a, bool exact) {
-  constexpr int smem1 = (2 * kTileM * 128 + 2 * kBlkK * 128 + 2 * kHd * 128 + 2 * kTileM * 128) + 256;
-  constexpr int smem5 = 2 * kTileM * 128 + kAttn5Stages * (kBlkK + kHd) * 128;  // per operand plane; + 256 B of barriers
-  if (ctx->attn_ver == 7) {
-    if (exact) {
-      DIMB_TRY(dimb_func_smem(ctx, (lg_attn5_kernel<true, true>), 2 * smem5 + 256));
-      lg_attn5_kernel<true, true><<<grid, 352, 2 * smem5 + 256, st>>>(Q[0], Q[1], K[0], K[1], V[0], V[1], a);
-    } else {
-      DIMB_TRY(dimb_func_smem(ctx, (lg_attn5_kernel<false, true>), smem5 + 256));
-      lg_attn5_kernel<false, true><<<grid, 352, smem5 + 256, st>>>(Q[0], Q[1], K[0], K[1], V[0], V[1], a);
-    }
-  } else if (ctx->attn_ver == 6) {
-    constexpr int smem6 = 2 * 2 * kTileM * 8 + 256;  // merge statistics + barriers
-    if (exact) {
-      DIMB_TRY(dimb_func_smem(ctx, lg_attn6_kernel<true>, 2 * smem5 + smem6));
-      lg_attn6_kernel<true><<<grid, 608, 2 * smem5 + smem6, st>>>(Q[0], Q[1], K[0], K[1], V[0], V[1], a);
-    } else {
-      DIMB_TRY(dimb_func_smem(ctx, lg_attn6_kernel<false>, smem5 + smem6));
-      lg_attn6_kernel<false><<<grid, 608, smem5 + smem6, st>>>(Q[0], Q[1], K[0], K[1], V[0], V[1], a);
-    }
-  } else if (ctx->attn_ver == 5) {
-    if (exact) {
-      DIMB_TRY(dimb_func_smem(ctx, (lg_attn5_kernel<true, false>), 2 * smem5 + 256));
-      lg_attn5_kernel<true, false><<<grid, 352, 2 * smem5 + 256, st>>>(Q[0], Q[1], K[0], K[1], V[0], V[1], a);
-    } else {
-      DIMB_TRY(dimb_func_smem(ctx, (lg_attn5_kernel<false, false>), smem5 + 256));
-      lg_attn5_kernel<false, false><<<grid, 352, smem5 + 256, st>>>(Q[0], Q[1], K[0], K[1], V[0], V[1], a);
-    }
-  } else if (ctx->attn_ver == 3) {
-    if (exact) {
-      DIMB_TRY(dimb_func_smem(ctx, lg_attn3_kernel<true>, 2 * smem1 - 256));
-      lg_attn3_kernel<true><<<grid, 352, 2 * smem1 - 256, st>>>(Q[0], Q[1], K[0], K[1], V[0], V[1], a);
-    } else {
-      DIMB_TRY(dimb_func_smem(ctx, lg_attn3_kernel<false>, smem1));
-      lg_attn3_kernel<false><<<grid, 352, smem1, st>>>(Q[0], Q[1], K[0], K[1], V[0], V[1], a);
-    }
+  grid.x = ceil_div(a.rows.NP, kAttnTile);
+  if (exact) {
+    constexpr int smem = AttnGeom<kHd, true>::kSmem;
+    DIMB_TRY(dimb_func_smem(ctx, lg_attn_kernel<true>, smem));
+    lg_attn_kernel<true><<<grid, kAttnThreads, smem, st>>>(Q[0], Q[1], K[0], K[1], V[0], V[1], a);
   } else {
-    if (exact) {
-      DIMB_TRY(dimb_func_smem(ctx, lg_attn4_kernel<true>, 2 * smem1 - 256));
-      lg_attn4_kernel<true><<<grid, 608, 2 * smem1 - 256, st>>>(Q[0], Q[1], K[0], K[1], V[0], V[1], a);
-    } else {
-      DIMB_TRY(dimb_func_smem(ctx, lg_attn4_kernel<false>, smem1));
-      lg_attn4_kernel<false><<<grid, 608, smem1, st>>>(Q[0], Q[1], K[0], K[1], V[0], V[1], a);
-    }
+    constexpr int smem = AttnGeom<kHd, false>::kSmem;
+    DIMB_TRY(dimb_func_smem(ctx, lg_attn_kernel<false>, smem));
+    lg_attn_kernel<false><<<grid, kAttnThreads, smem, st>>>(Q[0], Q[0], K[0], K[0], V[0], V[0], a);
   }
   return DIMB_OK;
 }

@@ -985,31 +985,6 @@ int dimb_lg_match_dev(dimb_lg* lg, int P, const dimb_feats_dev* f0, const dimb_f
         e.col_off = d;
         DIMB_TRY(lg_gemm(lg, st, lg->m_ctx, lg->ctxh, lg->ctxl, d, outp, e, m_tiles, "lg.out_proj"));
       }
-      if (ctx->fuse_ffn && ctx->use_tc && f0.has256) {  // FFN0 + LayerNorm + GELU in one kernel (EpiFfnLn): no fp32 hidden state in HBM
-        EpiFfnLn e;
-        e.rows = rows;
-        e.bias = f0.bias;
-        e.gamma = blk ? ly.g_c : ly.g_s;
-        e.beta = blk ? ly.b_c : ly.b_s;
-        e.hi = lg->h2h;
-        e.lo = exact ? lg->h2l : nullptr;
-        TcOperands ops;
-        ops.Ah = lg->m_x[cur][0];
-        ops.Al = lg->m_x[cur][1];
-        ops.Bh = f0.tmh256;
-        ops.Bl = f0.tml256;
-        GemmArgs g{};
-        g.num_kb = 2 * d / 64;
-        g.M = lg->R;
-        g.N = 2 * d;
-        ProfScope prof_f(ctx, st, "lg.ffn0+ln_gelu");
-        const int grid = m_tiles < ctx->num_sms ? m_tiles : ctx->num_sms;
-        const int scratch = EpiFfnLn::kEpiWarps * kScratchFloats * 4;
-        if (exact)
-          DIMB_TRY((launch_pers<256, true, 0, false, EpiFfnLn>(ctx, st, ops, g, e, m_tiles, 2, pers_config<256, true, 0>(g.num_kb, false, scratch), grid)));
-        else
-          DIMB_TRY((launch_pers<256, false, 0, false, EpiFfnLn>(ctx, st, ops, g, e, m_tiles, 2, pers_config<256, false, 0>(g.num_kb, false, scratch), grid)));
-      } else {
       {
         EpiLgF32 e;
         e.rows = rows;
@@ -1023,7 +998,6 @@ int dimb_lg_match_dev(dimb_lg* lg, int P, const dimb_feats_dev* f0, const dimb_f
         lg_ln_gelu_kernel<<<ceil_div(R * 32, 256), 256, 0, st>>>(rows, lg->h1, blk ? ly.g_c : ly.g_s, blk ? ly.b_c : ly.b_s, lg->h2h,
                                                                   exact ? lg->h2l : nullptr, R);
         DIMB_LAUNCH_CHECK(ctx);
-      }
       }
       {
         EpiLgResidual e;

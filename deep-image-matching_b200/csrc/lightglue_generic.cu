@@ -2,7 +2,7 @@
 // checkpoint the reference ships (thirdparty/accelerated_features/modules/lighterglue.py:12-27: descriptor_dim 96,
 // one head, 6 layers, input_dim 64; matcher plugin src/deep_image_matching/matchers/lighterglue.py:78-262).
 // Same algorithm as lightglue.cu (thirdparty/LightGlue/lightglue/lightglue.py:24-610) in plain fp32 on the CUDA cores:
-// the tensor-core kernels of lightglue.cu are specialised for head dim 64 / model dim 256 (TMEM and shared-memory budgets of
+// the tensor-core kernels of lightglue.cu are specialised for head dim 64 / model dim 256 (registers and shared-memory budgets of
 // the attention kernel), this file trades speed for generality.  Control flow (early stop, pruning) is decided on the host
 // from per-token confidences copied back once per layer - exactly the synchronisation points of the reference
 // (lightglue.py:499,503).  One pair at a time.
@@ -217,16 +217,16 @@ int lgx_create(dimb_ctx* ctx, const float* weights, size_t n_floats, const dimb_
   // head dims 65..128 (LighterGlue: 96): attention on the tensor cores (attn_hd128.cuh); DIMB_TC=0 keeps the fp32 kernel
   g->tc_attn = hd > 64 && hd <= kXHd;
   if (g->tc_attn) {
-    g->NPp = (g->NP + kXTile - 1) / kXTile * kXTile;
+    g->NPp = (g->NP + kAttnTile - 1) / kAttnTile * kAttnTile;
     const size_t rows = static_cast<size_t>(h) * g->NPp, nel = rows * kXHd;
     for (int s = 0; s < 2; ++s)
       for (int pl = 0; pl < 2; ++pl) {
         DIMB_TRY(dimb_alloc_t(ctx, &g->qp[s][pl], nel));  // zero-initialised: pad rows / columns stay finite
         DIMB_TRY(dimb_alloc_t(ctx, &g->kp[s][pl], nel));
         DIMB_TRY(dimb_alloc_t(ctx, &g->vt[s][pl], nel));
-        DIMB_TRY(dimb_tmap_2d(ctx, &g->mQ128[s][pl], g->qp[s][pl], rows, kXHd, kXHd, kXTile));
-        DIMB_TRY(dimb_tmap_2d(ctx, &g->mQ64[s][pl], g->qp[s][pl], rows, kXHd, kXHd, kXBlk));
-        DIMB_TRY(dimb_tmap_2d(ctx, &g->mK64[s][pl], g->kp[s][pl], rows, kXHd, kXHd, kXBlk));
+        DIMB_TRY(dimb_tmap_2d(ctx, &g->mQ128[s][pl], g->qp[s][pl], rows, kXHd, kXHd, kAttnTile));
+        DIMB_TRY(dimb_tmap_2d(ctx, &g->mQ64[s][pl], g->qp[s][pl], rows, kXHd, kXHd, kAttnBlk));
+        DIMB_TRY(dimb_tmap_2d(ctx, &g->mK64[s][pl], g->kp[s][pl], rows, kXHd, kXHd, kAttnBlk));
         DIMB_TRY(dimb_tmap_2d(ctx, &g->mVt[s][pl], g->vt[s][pl], static_cast<uint64_t>(h) * kXHd, g->NPp, g->NPp, kXHd));
       }
   }

@@ -3,7 +3,7 @@
 //
 // The reference materialises the full n0 x n1 distance matrix (torch.cdist, 268 MB at 8192^2) and runs
 // min / topk over it.  Here the distance tile never leaves the SM: the tensor-core GEMM of gemm.cuh
-// produces a 128 x 128 tile of dot products in TMEM and its epilogue turns it into distances
+// produces a 128 x 128 tile of dot products in registers and its epilogue turns it into distances
 // (|a|^2 + |b|^2 - 2ab, clamped, sqrt) and a per-row running (best, second best, argbest) over each
 // 32-column chunk; a small merge kernel reduces the chunk partials.  The column statistics needed by the
 // mutual / symmetric modes are the same kernel with the operands swapped.
@@ -14,13 +14,11 @@
 
 namespace {
 
-// K = D is small (256): a 128 x 256 output tile halves the A re-reads per FLOP compared with 128 x 128 (the kernel is bound by
-// L2 -> shared-memory operand traffic, not by the tensor pipe)
-constexpr int kNnBN = 256;
+// 128 x 128 output tiles: with register accumulators a 128 x 256 tile leaves the running top-2 epilogue too few registers
+// (it spills), so the wider tile's halved A re-reads are not worth it
+constexpr int kNnBN = 128;
 
 struct EpiNNTop2 : EpiBase {
-  static constexpr bool kUsesScratch = false;
-  static constexpr int kEpiWarps = 8;  // running top-2 per element: the epilogue is as long as the K = 256 MMAs of a tile
   const float *na, *nb;  // squared norms of A rows / B rows
   float *pd1, *pd2;      // [rows][chunks] best / second best SQUARED distance of each 32-column chunk
   int* pi1;              // [rows][chunks] argbest

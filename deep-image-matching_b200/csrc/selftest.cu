@@ -1,5 +1,5 @@
 // selftest.cu - dimb_selftest_gemm: C = A * B^T through the production tensor-core GEMM (or its SIMT twin),
-// used by tests/ to validate the tcgen05/TMA plumbing in isolation from the model code.
+// used by tests/ to validate the wgmma/TMA plumbing in isolation from the model code.
 #include <vector>
 
 #include "gemm.cuh"
@@ -83,295 +83,6 @@ extern "C" int dimb_selftest_gemm(dimb_ctx* ctx, const float* A, const float* B,
     cudaMemcpy(C, dC, sizeof(float) * M * N, cudaMemcpyDeviceToHost);
   } while (0);
   for (void* p : tmp) cudaFree(p);
-  return rc;
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Hardware probe (not used by the product path): how does tcgen05.mma address a SWIZZLE_128B K-major A operand whose start
-// is NOT 1024-byte aligned, and with a stride between the 8-row groups that is not 1024 bytes?  The answer decides whether a
-// 3x3 convolution can read all nine taps from ONE halo box in shared memory (DESIGN.md section 8, item 1b).
-//   A: [rows_a][64] fp16 (one swizzle atom wide), loaded by TMA into a 1024-aligned box; B: [64][64].
-//   MMA row r (0..127) is read at  start + (r / 8) * sbo_bytes + (r % 8) * 128,  start = box + shift_rows * 128.
-//   Expected result if the swizzle phase follows absolute shared-memory address bits:  C[r] = A[src(r)] . B^T  with
-//   src(r) = shift_rows + (r / 8) * (sbo_bytes / 128) + r % 8.
-namespace {
-__global__ void __launch_bounds__(128) probe_rowshift_kernel(const __grid_constant__ CUtensorMap mA, const __grid_constant__ CUtensorMap mB,
-                                                             float* __restrict__ C, int rows_a, int shift_rows, int sbo_bytes,
-                                                             int use_base_offset) {
-  using namespace tc05;
-  extern __shared__ __align__(1024) uint8_t psm[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(psm) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* sA = base;                     // rows_a * 128 B (<= 32 KB)
-  uint8_t* sB = base + 32768;             // 64 * 128 B
-  uint64_t* bar = reinterpret_cast<uint64_t*>(base + 32768 + 8192);
-  uint32_t* tptr = reinterpret_cast<uint32_t*>(bar + 2);
-  const int t = threadIdx.x;
-  if (t == 0) {
-    mbar_init(&bar[0], 1);
-    mbar_init(&bar[1], 1);
-    fence_barrier_init();
-  }
-  if (t < 32) tmem_alloc(tptr, 64);
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = *tptr;
-  if (t == 0) {
-    mbar_expect_tx(&bar[0], static_cast<uint32_t>(rows_a * 128 + 64 * 128));
-    tma_load_2d(sA, &mA, &bar[0], 0, 0);
-    tma_load_2d(sB, &mB, &bar[0], 0, 0);
-    mbar_wait(&bar[0], 0);
-    tc_fence_after_sync();
-    const uint32_t a_addr = smem_u32(sA) + static_cast<uint32_t>(shift_rows) * 128u;
-    uint64_t ad = 0;
-    ad |= static_cast<uint64_t>((a_addr & 0x3FFFFu) >> 4);
-    ad |= static_cast<uint64_t>(1) << 16;
-    ad |= static_cast<uint64_t>(static_cast<uint32_t>(sbo_bytes) >> 4) << 32;
-    ad |= static_cast<uint64_t>(1) << 46;
-    if (use_base_offset) ad |= static_cast<uint64_t>((a_addr >> 7) & 7u) << 49;
-    ad |= static_cast<uint64_t>(2) << 61;
-    const uint64_t bd = make_sdesc_sw128(smem_u32(sB));
-    constexpr uint32_t idesc = make_idesc_f16(64);
-    for (int k16 = 0; k16 < 4; ++k16) mma_f16_ss(tmem, sdesc_advance_k(ad, k16), sdesc_advance_k(bd, k16), idesc, k16 > 0);
-    mma_commit(&bar[1]);
-  }
-  mbar_wait(&bar[1], 0);
-  tc_fence_after_sync();
-  float v[32];
-  for (int h = 0; h < 2; ++h) {
-    tmem_ld32(tmem + (static_cast<uint32_t>((t >> 5) * 32) << 16) + h * 32, v);
-    tmem_ld_wait();
-    for (int j = 0; j < 32; ++j) C[t * 64 + h * 32 + j] = v[j];
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (t < 32) tmem_dealloc(tmem, 64);
-}
-}  // namespace
-
-// A [rows_a][64], B [64][64] host fp32 with fp16-representable values; C [128][64] host fp32.
-extern "C" int dimb_probe_rowshift(dimb_ctx* ctx, const float* A, const float* B, float* C, int rows_a, int shift_rows, int sbo_bytes,
-                                   int use_base_offset) {
-  if (!ctx || !A || !B || !C || rows_a < 128 || rows_a > 256 || shift_rows < 0 || sbo_bytes < 1024 || sbo_bytes % 128) return DIMB_ERR_ARG;
-  if (shift_rows + 15 * (sbo_bytes / 128) + 8 > rows_a) return DIMB_ERR_ARG;
-  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-  std::vector<__half> ha(static_cast<size_t>(rows_a) * 64), hb(64 * 64);
-  for (size_t i = 0; i < ha.size(); ++i) ha[i] = __float2half_rn(A[i]);
-  for (size_t i = 0; i < hb.size(); ++i) hb[i] = __float2half_rn(B[i]);
-  __half *dA = nullptr, *dB = nullptr;
-  float* dC = nullptr;
-  int rc = DIMB_OK;
-  do {
-    if (cudaMalloc(&dA, ha.size() * 2) != cudaSuccess || cudaMalloc(&dB, hb.size() * 2) != cudaSuccess ||
-        cudaMalloc(&dC, 128 * 64 * 4) != cudaSuccess) {
-      rc = DIMB_ERR_OOM;
-      break;
-    }
-    cudaMemcpy(dA, ha.data(), ha.size() * 2, cudaMemcpyHostToDevice);
-    cudaMemcpy(dB, hb.data(), hb.size() * 2, cudaMemcpyHostToDevice);
-    CUtensorMap mA, mB;
-    if ((rc = dimb_tmap_2d(ctx, &mA, dA, rows_a, 64, 64, rows_a))) break;
-    if ((rc = dimb_tmap_2d(ctx, &mB, dB, 64, 64, 64, 64))) break;
-    const int smem = 32768 + 8192 + 64 + 1024;
-    cudaFuncSetAttribute(probe_rowshift_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    probe_rowshift_kernel<<<1, 128, smem>>>(mA, mB, dC, rows_a, shift_rows, sbo_bytes, use_base_offset);
-    const cudaError_t ce = cudaDeviceSynchronize();
-    if (ce != cudaSuccess) {
-      dimb_set_error(ctx, std::string("dimb_probe_rowshift: ") + cudaGetErrorString(ce));
-      rc = DIMB_ERR_CUDA;
-      break;
-    }
-    cudaMemcpy(C, dC, 128 * 64 * 4, cudaMemcpyDeviceToHost);
-  } while (false);
-  cudaFree(dA);
-  cudaFree(dB);
-  cudaFree(dC);
-  return rc;
-}
-
-// Same probe for SWIZZLE_64B operands with 32-half (64-byte) rows: the half-K-block stage that would let one halo box and the
-// resident Cin = Cout = 64 weights share the 227 KB (DESIGN.md section 8).  B is the 32 x 32 identity (N = 32, K = 32).
-namespace {
-__global__ void __launch_bounds__(128) probe_rowshift64_kernel(const __grid_constant__ CUtensorMap mA, const __grid_constant__ CUtensorMap mB,
-                                                               float* __restrict__ C, int rows_a, int shift_rows, int sbo_bytes) {
-  using namespace tc05;
-  extern __shared__ __align__(1024) uint8_t psm[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(psm) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* sA = base;                     // rows_a * 64 B (<= 16 KB)
-  uint8_t* sB = base + 16384;             // 32 * 64 B
-  uint64_t* bar = reinterpret_cast<uint64_t*>(base + 16384 + 2048);
-  uint32_t* tptr = reinterpret_cast<uint32_t*>(bar + 2);
-  const int t = threadIdx.x;
-  if (t == 0) {
-    mbar_init(&bar[0], 1);
-    mbar_init(&bar[1], 1);
-    fence_barrier_init();
-  }
-  if (t < 32) tmem_alloc(tptr, 32);
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = *tptr;
-  if (t == 0) {
-    mbar_expect_tx(&bar[0], static_cast<uint32_t>(rows_a * 64 + 32 * 64));
-    tma_load_2d(sA, &mA, &bar[0], 0, 0);
-    tma_load_2d(sB, &mB, &bar[0], 0, 0);
-    mbar_wait(&bar[0], 0);
-    tc_fence_after_sync();
-    auto desc = [](uint32_t addr, uint32_t sbo) {
-      uint64_t d = 0;
-      d |= static_cast<uint64_t>((addr & 0x3FFFFu) >> 4);
-      d |= static_cast<uint64_t>(1) << 16;
-      d |= static_cast<uint64_t>(sbo >> 4) << 32;
-      d |= static_cast<uint64_t>(1) << 46;
-      d |= static_cast<uint64_t>(4) << 61;  // SWIZZLE_64B
-      return d;
-    };
-    const uint64_t ad = desc(smem_u32(sA) + static_cast<uint32_t>(shift_rows) * 64u, static_cast<uint32_t>(sbo_bytes));
-    const uint64_t bd = desc(smem_u32(sB), 512u);
-    constexpr uint32_t idesc = make_idesc_f16(32);
-    for (int k16 = 0; k16 < 2; ++k16) mma_f16_ss(tmem, sdesc_advance_k(ad, k16), sdesc_advance_k(bd, k16), idesc, k16 > 0);
-    mma_commit(&bar[1]);
-  }
-  mbar_wait(&bar[1], 0);
-  tc_fence_after_sync();
-  float v[32];
-  tmem_ld32(tmem + (static_cast<uint32_t>((t >> 5) * 32) << 16), v);
-  tmem_ld_wait();
-  for (int j = 0; j < 32; ++j) C[t * 32 + j] = v[j];
-  tc_fence_before_sync();
-  __syncthreads();
-  if (t < 32) tmem_dealloc(tmem, 32);
-}
-}  // namespace
-
-// A [rows_a][32], B [32][32] host fp32 (fp16-representable); C [128][32].
-extern "C" int dimb_probe_rowshift64(dimb_ctx* ctx, const float* A, const float* B, float* C, int rows_a, int shift_rows, int sbo_bytes) {
-  if (!ctx || !A || !B || !C || rows_a < 128 || rows_a > 256 || shift_rows < 0 || sbo_bytes < 512 || sbo_bytes % 64) return DIMB_ERR_ARG;
-  if (shift_rows + 15 * (sbo_bytes / 64) + 8 > rows_a) return DIMB_ERR_ARG;
-  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-  std::vector<__half> ha(static_cast<size_t>(rows_a) * 32), hb(32 * 32);
-  for (size_t i = 0; i < ha.size(); ++i) ha[i] = __float2half_rn(A[i]);
-  for (size_t i = 0; i < hb.size(); ++i) hb[i] = __float2half_rn(B[i]);
-  __half *dA = nullptr, *dB = nullptr;
-  float* dC = nullptr;
-  int rc = DIMB_OK;
-  do {
-    if (cudaMalloc(&dA, ha.size() * 2) != cudaSuccess || cudaMalloc(&dB, hb.size() * 2) != cudaSuccess ||
-        cudaMalloc(&dC, 128 * 32 * 4) != cudaSuccess) {
-      rc = DIMB_ERR_OOM;
-      break;
-    }
-    cudaMemcpy(dA, ha.data(), ha.size() * 2, cudaMemcpyHostToDevice);
-    cudaMemcpy(dB, hb.data(), hb.size() * 2, cudaMemcpyHostToDevice);
-    CUtensorMap mA, mB;
-    if ((rc = dimb_tmap_2d_sw64(ctx, &mA, dA, rows_a, 32, 32, rows_a))) break;
-    if ((rc = dimb_tmap_2d_sw64(ctx, &mB, dB, 32, 32, 32, 32))) break;
-    const int smem = 16384 + 2048 + 64 + 1024;
-    probe_rowshift64_kernel<<<1, 128, smem>>>(mA, mB, dC, rows_a, shift_rows, sbo_bytes);
-    const cudaError_t ce = cudaDeviceSynchronize();
-    if (ce != cudaSuccess) {
-      dimb_set_error(ctx, std::string("dimb_probe_rowshift64: ") + cudaGetErrorString(ce));
-      rc = DIMB_ERR_CUDA;
-      break;
-    }
-    cudaMemcpy(C, dC, 128 * 32 * 4, cudaMemcpyDeviceToHost);
-  } while (false);
-  cudaFree(dA);
-  cudaFree(dB);
-  cudaFree(dC);
-  return rc;
-}
-
-// Probe of the TMEM-resident A operand (tcgen05.mma [d], [a_tmem], b_desc): thread r writes row r of A as 32 packed half2 words
-// (word c = elements 2c, 2c + 1) into TMEM columns [64, 96) with tcgen05.st.32x32b; B [64][64] comes from shared memory (SWIZZLE_128B,
-// K-major); four 16-deep MMAs read A at column offsets 0 / 8 / 16 / 24.  C [128][64] = A B^T if the layout assumption holds.
-// Basis of the attention kernel that keeps P in tensor memory (lg_attn5_kernel).
-namespace {
-__global__ void __launch_bounds__(128) probe_tmem_a_kernel(const __half* __restrict__ A, const __grid_constant__ CUtensorMap mB,
-                                                           float* __restrict__ C) {
-  using namespace tc05;
-  extern __shared__ __align__(1024) uint8_t psm[];
-  uint8_t* base = psm + ((1024u - (smem_u32(psm) & 1023u)) & 1023u);
-  uint8_t* sB = base;  // 64 * 128 B
-  uint64_t* bar = reinterpret_cast<uint64_t*>(base + 8192);
-  uint32_t* tptr = reinterpret_cast<uint32_t*>(bar + 2);
-  const int t = threadIdx.x;
-  if (t == 0) {
-    mbar_init(&bar[0], 1);
-    mbar_init(&bar[1], 1);
-    fence_barrier_init();
-  }
-  if (t < 32) tmem_alloc(tptr, 128);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = *tptr;
-  {
-    float w[32];
-    const uint32_t* src = reinterpret_cast<const uint32_t*>(A + t * 64);
-    for (int c = 0; c < 32; ++c) w[c] = __uint_as_float(src[c]);
-    tmem_st32(tmem + (static_cast<uint32_t>((t >> 5) * 32) << 16) + 64, w);
-    tmem_st_wait();
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  if (t == 0) {
-    mbar_expect_tx(&bar[0], 64 * 128);
-    tma_load_2d(sB, &mB, &bar[0], 0, 0);
-    mbar_wait(&bar[0], 0);
-    tc_fence_after_sync();
-    const uint64_t bd = make_sdesc_sw128(smem_u32(sB));
-    constexpr uint32_t idesc = make_idesc_f16(64);
-    for (int k16 = 0; k16 < 4; ++k16) mma_f16_ts(tmem, tmem + 64 + k16 * 8, sdesc_advance_k(bd, k16), idesc, k16 > 0);
-    mma_commit(&bar[1]);
-  }
-  mbar_wait(&bar[1], 0);
-  tc_fence_after_sync();
-  float v[32];
-  for (int h = 0; h < 2; ++h) {
-    tmem_ld32(tmem + (static_cast<uint32_t>((t >> 5) * 32) << 16) + h * 32, v);
-    tmem_ld_wait();
-    for (int j = 0; j < 32; ++j) C[t * 64 + h * 32 + j] = v[j];
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (t < 32) tmem_dealloc(tmem, 128);
-}
-}  // namespace
-
-// A [128][64], B [64][64] host fp32 (fp16-representable values); C [128][64] host fp32 = A B^T through the TMEM-A MMA.
-extern "C" int dimb_probe_tmem_a(dimb_ctx* ctx, const float* A, const float* B, float* C) {
-  if (!ctx || !A || !B || !C) return DIMB_ERR_ARG;
-  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-  std::vector<__half> ha(128 * 64), hb(64 * 64);
-  for (size_t i = 0; i < ha.size(); ++i) ha[i] = __float2half_rn(A[i]);
-  for (size_t i = 0; i < hb.size(); ++i) hb[i] = __float2half_rn(B[i]);
-  __half *dA = nullptr, *dB = nullptr;
-  float* dC = nullptr;
-  int rc = DIMB_OK;
-  do {
-    if (cudaMalloc(&dA, ha.size() * 2) != cudaSuccess || cudaMalloc(&dB, hb.size() * 2) != cudaSuccess ||
-        cudaMalloc(&dC, 128 * 64 * 4) != cudaSuccess) {
-      rc = DIMB_ERR_OOM;
-      break;
-    }
-    cudaMemcpy(dA, ha.data(), ha.size() * 2, cudaMemcpyHostToDevice);
-    cudaMemcpy(dB, hb.data(), hb.size() * 2, cudaMemcpyHostToDevice);
-    CUtensorMap mB;
-    if ((rc = dimb_tmap_2d(ctx, &mB, dB, 64, 64, 64, 64))) break;
-    const int smem = 8192 + 64 + 1024;
-    probe_tmem_a_kernel<<<1, 128, smem>>>(dA, mB, dC);
-    const cudaError_t ce = cudaDeviceSynchronize();
-    if (ce != cudaSuccess) {
-      dimb_set_error(ctx, std::string("dimb_probe_tmem_a: ") + cudaGetErrorString(ce));
-      rc = DIMB_ERR_CUDA;
-      break;
-    }
-    cudaMemcpy(C, dC, 128 * 64 * 4, cudaMemcpyDeviceToHost);
-  } while (false);
-  cudaFree(dA);
-  cudaFree(dB);
-  cudaFree(dC);
   return rc;
 }
 

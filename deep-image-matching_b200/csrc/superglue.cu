@@ -7,7 +7,7 @@
 // shared building blocks of lg_kernels.cuh: per layer ONE q|k GEMM (EpiQK without rotary), the V^T GEMM, the flash-attention kernel
 // (self: keys of the same side, cross: keys and values of the other side), merge -> message half of the [x | message] buffer, MLP0
 // with the eval-mode BatchNorm folded in and a ReLU / hi-lo-split epilogue, MLP3 + residual; then final_proj and the score matrix as
-// tcgen05 GEMMs, and 100 log-space Sinkhorn sweeps over the L2-resident score matrix with the dustbin row / column kept virtual
+// wgmma GEMMs, and 100 log-space Sinkhorn sweeps over the L2-resident score matrix with the dustbin row / column kept virtual
 // (coalesced row and column passes).  Done once at create time: BatchNorm folding, and the reference's (dim, heads)-interleaved
 // channel order of `view(b, dim, heads, n)` (:111-113) permuted to head-major.  The keypoint encoder (3 -> 32 -> 64 -> 128 -> 256 -> 256,
 // 0.2 GMAC) stays on the plain fp32 kernels of generic_kernels.cuh; the whole plain-fp32 path remains as the debug twin (DIMB_TC=0).
@@ -272,7 +272,7 @@ int upload(dimb_ctx* ctx, SgLin& d, const HostLin& h) {
   return DIMB_OK;
 }
 
-// one GEMM over all 2 * NPt token rows: C = A [R][K] * W^T on the tcgen05 kernel of gemm.cuh with epilogue `epi`
+// one GEMM over all 2 * NPt token rows: C = A [R][K] * W^T on the wgmma kernel of gemm.cuh with epilogue `epi`
 template <class Epi>
 int sg_tc_gemm(dimb_sg* g, cudaStream_t st, const CUtensorMap* A, const __half* Ah, const __half* Al, int lda, const SgTcLin& w, int n_out,
                const Epi& epi, const char* tag) {

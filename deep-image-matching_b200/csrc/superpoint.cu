@@ -6,7 +6,7 @@
 // implicit GEMM whose A tile for one filter tap is a plain 4D TMA box (see gemm.cuh); weights are
 // [Cout][tap*Cin + c] fp16 hi/lo.  Pipeline per call (B images):
 //   sp_conv1a (CUDA cores, Cin=1)        -> a1   64@HxW
-//   conv1b  +ReLU+pool (tcgen05)         -> a1p  64@H/2
+//   conv1b  +ReLU+pool (wgmma)           -> a1p  64@H/2
 //   conv2a, conv2b+pool                  -> a2p  64@H/4
 //   conv3a, conv3b+pool                  -> a3p 128@H/8
 //   conv4a, conv4b                       -> feat 128@h x w
@@ -20,14 +20,13 @@
 
 #include "detect.cuh"
 #include "gemm.cuh"
-#include "conv_pair.cuh"
 
 namespace {
 
 // ------------------------------------------------------------------ epilogue: conv bias + ReLU (+2x2 max pool) -> NHWC hi/lo
-template <bool POOL, int TW = kConvTW>  // TW: pixels per tile row (16: CONV 1 tiles, 8: CONV 2 tiles)
+template <bool POOL>
 struct EpiConvRelu : EpiBase {
-  static constexpr bool kUsesScratch = false;
+  static constexpr int TW = kConvTW;  // pixels per tile row
   __half *hi, *lo;
   const float* bias;
   int H, W;      // conv resolution
@@ -65,7 +64,9 @@ struct EpiConvRelu : EpiBase {
 // bank, the compiler pulls them into uniform registers (LDCU) and every FMA takes its weight as a uniform-register operand -
 // no per-thread load instruction (the kernel is bound by the L1 / shared-memory pipe) - and, unlike a __constant__ symbol,
 // each launch carries the weights of its own handle (same SASS as the symbol version: 591 FFMA + 163 LDCU).
-using Conv1aW = pairconv::Conv1aWeights;  // float v[576 + 64]: the same weights feed the fused conv1a producers of conv_pair.cuh
+struct Conv1aW {
+  float v[576 + 64];
+};
 
 __global__ void __launch_bounds__(256, 3) sp_conv1a_kernel(const __grid_constant__ Conv1aW c_w, const float* __restrict__ img,
                                                            __half* __restrict__ hi, __half* __restrict__ lo, int H, int W) {
@@ -212,8 +213,6 @@ struct ConvLayer {
   float* bias = nullptr;                // [cout_pad]
   int cout_pad, k;
   CUtensorMap tmBh, tmBl;
-  CUtensorMap tmBh64, tmBl64;  // the same weights as 32-half (64-byte) K blocks, SWIZZLE_64B (Cin = 64 layers, gemm.cuh CONV 2)
-  CUtensorMap tmBh32;          // W_hi in boxes of 32 rows: the per-CTA half of the N = 64 operand of the CTA-pair kernel (conv_pair.cuh)
 };
 
 }  // namespace
@@ -224,8 +223,6 @@ struct dimb_sp {
   dimb_sp_conf conf;
   // weights
   Conv1aW w1a;  // conv1a weights, tap-major [9][64] + bias [64] (host copy: passed by value with every launch)
-  __half *w1h = nullptr, *w1l = nullptr;  // conv1a as a GEMM operand [64 cout][32 K] fp16 hi / lo: K = 9 taps, bias, zeros (conv1ab_mma_pair_kernel)
-  CUtensorMap tmW1h, tmW1l;               // boxes of 32 rows (the per-CTA half of N = 64), SWIZZLE_64B
   ConvLayer L[11];  // conv1b conv2a conv2b conv3a conv3b conv4a conv4b convPa convPb convDa convDb
   // workspace (sized for max_batch x max_height x max_width)
   float* img = nullptr;
@@ -274,11 +271,6 @@ int make_conv_layer(dimb_ctx* ctx, ConvLayer& L, const float* w, const float* b,
   DIMB_CUDA_OK(ctx, cudaMemcpy(L.bias, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice));
   DIMB_TRY(dimb_tmap_2d(ctx, &L.tmBh, L.wh, L.cout_pad, L.k, L.k, bn));
   DIMB_TRY(dimb_tmap_2d(ctx, &L.tmBl, L.wl, L.cout_pad, L.k, L.k, bn));
-  if (L.cin == 64 && L.k == 9 * 64) {
-    DIMB_TRY(dimb_tmap_2d_sw64(ctx, &L.tmBh64, L.wh, L.cout_pad, L.k, L.k, bn));
-    DIMB_TRY(dimb_tmap_2d_sw64(ctx, &L.tmBl64, L.wl, L.cout_pad, L.k, L.k, bn));
-    DIMB_TRY(dimb_tmap_2d_sw64(ctx, &L.tmBh32, L.wh, L.cout_pad, L.k, L.k, 32));
-  }
   return DIMB_OK;
 }
 
@@ -310,32 +302,6 @@ int run_conv3(dimb_sp* sp, cudaStream_t st, const ConvLayer& L, const __half* in
     epi.Wo = POOL ? W / 2 : W;
     epi.C = L.cout;
   };
-  if (L.cin == 64 && BN == 64 && ctx->use_halo) {
-    // gemm.cuh CONV 2: one (16+2) x (8+2)-pixel halo box per 32-channel half block, resident weights
-    DIMB_TRY(dimb_tmap_nhwc_sw64(ctx, &ops.Ah, inh, B, H, W, L.cin, kHaloTH + 2, kHaloTW + 2));
-    DIMB_TRY(dimb_tmap_nhwc_sw64(ctx, &ops.Al, inl, B, H, W, L.cin, kHaloTH + 2, kHaloTW + 2));
-    ops.Bh = L.tmBh64;
-    ops.Bl = L.tmBl64;
-    g.num_kb = 9 * 2 * g.cin_blocks;
-    g.tiles_x = ceil_div(W, kHaloTW);
-    g.tiles_y = ceil_div(H, kHaloTH);
-    EpiConvRelu<POOL, kHaloTW> epi;
-    fill(epi);
-    // CTA pairs (cta_group::2, conv_pair.cuh) for the pooled layers conv1b / conv2b: 474 / 478 vs 410 / 416 TFLOP/s algorithmic on the
-    // single-CTA kernel (same box).  conv2a - no pooling, four times the output bytes per tile - is faster on the single-CTA kernel
-    // (its longer epilogue holds BOTH accumulators of a pair back): 3.46 vs 4.17 ms per 74 images.
-    if (ctx->use_pair && POOL && exact && ctx->use_tc && L.cout == 64) {
-      ProfScope prof(ctx, st, tag);
-      const int rc = pairconv::launch_conv64_pair(ctx, st, ops.Ah, ops.Al, L.tmBh64, L.tmBl64, L.tmBh32, B, H, W, epi);
-      if (rc != DIMB_ERR_UNSUPPORTED) return rc;  // odd tile count: the single-CTA kernel below
-    }
-    if (ctx->use_pair == 2 && !POOL && exact && ctx->use_tc && L.cout == 64) {  // DIMB_PAIR=2: conv2a on CTA pairs with 8 epilogue warps
-      ProfScope prof(ctx, st, tag);
-      const int rc = pairconv::launch_conv64_pair<EpiConvRelu<POOL, kHaloTW>, 8>(ctx, st, ops.Ah, ops.Al, L.tmBh64, L.tmBl64, L.tmBh32, B, H, W, epi);
-      if (rc != DIMB_ERR_UNSUPPORTED) return rc;
-    }
-    return launch_gemm<BN, 2>(ctx, st, ops, g, epi, B * g.tiles_x * g.tiles_y, L.cout_pad, tag);
-  }
   // gemm.cuh CONV 1: one (8+2)-row halo box per dx serves the three dy taps
   const int box_h = kConvTH + 2;
   DIMB_TRY(dimb_tmap_nhwc(ctx, &ops.Ah, inh, B, H, W, L.cin, box_h, kConvTW));
@@ -411,19 +377,6 @@ int dimb_sp_create(dimb_ctx* ctx, const float* weights, size_t n_floats, const d
     float* t = sp->w1a.v;
     for (int i = 0; i < 576; ++i) t[(i % 9) * 64 + i / 9] = p[i];
     for (int i = 0; i < 64; ++i) t[576 + i] = p[576 + i];
-    std::vector<__half> wh(64 * 32, __float2half_rn(0.f)), wl(64 * 32, __float2half_rn(0.f));
-    for (int c = 0; c < 64; ++c)
-      for (int k = 0; k < 10; ++k) {
-        const float w = k < 9 ? p[c * 9 + k] : p[576 + c];
-        wh[c * 32 + k] = __float2half_rn(w);
-        wl[c * 32 + k] = __float2half_rn(w - __half2float(wh[c * 32 + k]));
-      }
-    DIMB_TRY(dimb_alloc_t(ctx, &sp->w1h, wh.size(), false));
-    DIMB_TRY(dimb_alloc_t(ctx, &sp->w1l, wl.size(), false));
-    DIMB_CUDA_OK(ctx, cudaMemcpy(sp->w1h, wh.data(), wh.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    DIMB_CUDA_OK(ctx, cudaMemcpy(sp->w1l, wl.data(), wl.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    DIMB_TRY(dimb_tmap_2d_sw64(ctx, &sp->tmW1h, sp->w1h, 64, 32, 32, 32));
-    DIMB_TRY(dimb_tmap_2d_sw64(ctx, &sp->tmW1l, sp->w1l, 64, 32, 32, 32));
   }
   p += 640;
   for (int i = 1; i < 12; ++i) {
@@ -492,20 +445,7 @@ int dimb_sp_extract_dev(dimb_sp* sp, const float* d_images, int B, int H, int W,
   sp->lastB = B;
   sp->lastH = H;
   sp->lastW = W;
-  bool fused1 = false;
-  if (ctx->use_fuse1a && ctx->use_pair && ctx->use_tc && exact) {  // conv1a computed inside conv1b's producer warps (conv_pair.cuh)
-    const ConvLayer& L = sp->L[L1B];
-    EpiConvRelu<true, kHaloTW> epi;
-    epi.hi = sp->a1ph, epi.lo = sp->a1pl, epi.bias = L.bias;
-    epi.H = H, epi.W = W, epi.Ho = H / 2, epi.Wo = W / 2, epi.C = L.cout;
-    ProfScope prof(ctx, st, "sp.conv1ab");
-    const int rc = ctx->use_fuse1a == 2
-                       ? pairconv::launch_conv1ab_mma_pair(ctx, st, d_images, sp->tmW1h, sp->tmW1l, L.tmBh64, L.tmBl64, L.tmBh32, B, H, W, epi)
-                       : pairconv::launch_conv1ab_pair(ctx, st, sp->w1a, d_images, L.tmBh64, L.tmBl64, L.tmBh32, B, H, W, epi);
-    if (rc == DIMB_OK) fused1 = true;
-    else if (rc != DIMB_ERR_UNSUPPORTED) return rc;
-  }
-  if (!fused1) {
+  {
     ProfScope prof(ctx, st, "sp.conv1a");
     constexpr int c1smem = 4096 + 2 * 256 * 128;
     DIMB_TRY(dimb_func_smem(ctx, sp_conv1a_kernel, c1smem));
@@ -513,7 +453,7 @@ int dimb_sp_extract_dev(dimb_sp* sp, const float* d_images, int B, int H, int W,
                                                                                            exact ? sp->a1l : nullptr, H, W);
     DIMB_LAUNCH_CHECK(ctx);
   }
-  if (!fused1) DIMB_TRY((run_conv3<64, true>(sp, st, sp->L[L1B], sp->a1h, sp->a1l, sp->a1ph, sp->a1pl, B, H, W, "sp.conv1b")));
+  DIMB_TRY((run_conv3<64, true>(sp, st, sp->L[L1B], sp->a1h, sp->a1l, sp->a1ph, sp->a1pl, B, H, W, "sp.conv1b")));
   DIMB_TRY((run_conv3<64, false>(sp, st, sp->L[L2A], sp->a1ph, sp->a1pl, sp->a2h, sp->a2l, B, H2, W2, "sp.conv2a")));
   DIMB_TRY((run_conv3<64, true>(sp, st, sp->L[L2B], sp->a2h, sp->a2l, sp->a2ph, sp->a2pl, B, H2, W2, "sp.conv2b")));
   DIMB_TRY((run_conv3<128, false>(sp, st, sp->L[L3A], sp->a2ph, sp->a2pl, sp->a3h, sp->a3l, B, H4, W4, "sp.conv3a")));

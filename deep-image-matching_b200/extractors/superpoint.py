@@ -1,7 +1,7 @@
 """SuperPointExtractor on libdimb200 - drop-in for the reference plugin
 (src/deep_image_matching/extractors/superpoint.py:64-146): same class name, class attributes, config keys
 and ``_extract`` contract (float32 (H,W) gray 0..255 in; dict of writable numpy arrays out: keypoints (N,2)
-x,y, scores (N,), descriptors (256,N)).  The model arithmetic runs in hand-written sm_100a kernels
+x,y, scores (N,), descriptors (256,N)).  The model arithmetic runs in hand-written sm_90a kernels
 (csrc/superpoint.cu) instead of the MagicLeap torch graph.
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-/* dimb200.h - C ABI of libdimb200.so: the B200-native (sm_100a) hot path of
+/* dimb200.h - C ABI of libdimb200.so: the H100-native (sm_90a) hot path of
  * 3DOM-FBK/deep-image-matching behind plain pointers and sizes.
  *
  * Each entry point replaces the body of one reference plugin method (paths are
@@ -54,7 +54,7 @@ int dimb_ctx_create(int device, dimb_ctx** out);
 void dimb_ctx_destroy(dimb_ctx* ctx);
 const char* dimb_last_error(dimb_ctx* ctx);
 int dimb_ctx_set_precision(dimb_ctx* ctx, int precision);
-/* 1 (default): tcgen05 tensor-core kernels.  0: CUDA-core SIMT kernels with the same epilogues
+/* 1 (default): wgmma tensor-core kernels.  0: CUDA-core SIMT kernels with the same epilogues
  * (debug aid to bisect a tensor-path problem; also selectable with env DIMB_TC=0). */
 int dimb_ctx_set_tensor_path(dimb_ctx* ctx, int use_tc);
 /* Number of kernels this library has launched on ctx (bench.py "gpu_launches"). */

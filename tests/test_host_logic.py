@@ -17,7 +17,7 @@ def test_library_exports_every_declared_symbol():
     assert declared >= set(_native.EXPORTS)
     for sym in declared:
         assert hasattr(lib, sym), sym
-    assert b"sm_100a" in lib.dimb_version()
+    assert b"sm_90a" in lib.dimb_version()
 
 
 def test_no_cpu_fallback():
