@@ -25,7 +25,7 @@ EXPORTS = [
     "dimb_lg_create", "dimb_lg_destroy", "dimb_lg_match", "dimb_lg_match_dev", "dimb_lg_debug_read",
     "dimb_nn_match", "dimb_nn_match_dev", "dimb_ctx_profile", "dimb_ctx_profile_read", "dimb_pipe_create", "dimb_pipe_destroy",
     "dimb_pipe_match_image_pairs", "dimb_pipe_match_image_pairs_u8", "dimb_pipe_match_image_pairs_dev", "dimb_pipe_outputs_dev", "dimb_pipe_features_dev", "dimb_sp_ctx",
-    "dimb_sg_weight_count", "dimb_sg_create", "dimb_sg_destroy", "dimb_sg_match",
+    "dimb_sg_weight_count", "dimb_sg_create", "dimb_sg_destroy", "dimb_sg_match", "dimb_sg_match_dev", "dimb_fstore_sg_feats_dev",
     "dimb_aliked_create", "dimb_aliked_destroy", "dimb_aliked_extract", "dimb_aliked_extract_dev", "dimb_aliked_debug_read",
     "dimb_fstore_create", "dimb_fstore_destroy", "dimb_fstore_put_dev", "dimb_fstore_put", "dimb_fstore_count", "dimb_fstore_get",
     "dimb_fstore_feats_dev", "dimb_fstore_block_dev", "dimb_gv_fundamental", "dimb_gv_fundamental_batch_dev",
@@ -49,12 +49,18 @@ class AlikedConf(C.Structure):
 
 class SgConf(C.Structure):
     _fields_ = [("n_layers", C.c_int), ("cross_mask", C.c_ulonglong), ("sinkhorn_iterations", C.c_int), ("match_threshold", C.c_float),
-                ("max_kpts", C.c_int)]
+                ("max_kpts", C.c_int), ("max_pairs", C.c_int)]
 
 
 class SgFeats(C.Structure):
     _fields_ = [("keypoints", C.c_void_p), ("descriptors", C.c_void_p), ("scores", C.c_void_p), ("n", C.c_int), ("desc_ld", C.c_int),
                 ("height", C.c_int), ("width", C.c_int)]
+
+
+class SgFeatsDev(C.Structure):
+    _fields_ = [("keypoints", C.c_void_p), ("descriptors", C.c_void_p), ("scores", C.c_void_p), ("n", C.c_void_p), ("n_cap", C.c_int),
+                ("desc_ld", C.c_int), ("f16", C.c_int), ("round_fp16", C.c_int), ("height", C.c_int), ("width", C.c_int),
+                ("size_dev", C.c_void_p)]
 
 
 class LgConf(C.Structure):
@@ -129,6 +135,7 @@ def load_library():
     lib.dimb_sg_destroy.argtypes = [vp]
     lib.dimb_sg_destroy.restype = None
     lib.dimb_sg_match.argtypes = [vp, C.POINTER(SgFeats), C.POINTER(SgFeats), vp, vp, C.POINTER(ip), ip]
+    lib.dimb_sg_match_dev.argtypes = [vp, ip, C.POINTER(SgFeatsDev), C.POINTER(SgFeatsDev), vp, vp, vp, ip, vp]
     lib.dimb_aliked_create.argtypes = [vp, vp, C.c_size_t, C.POINTER(AlikedConf), C.POINTER(vp)]
     lib.dimb_aliked_destroy.argtypes = [vp]
     lib.dimb_aliked_destroy.restype = None
@@ -144,6 +151,7 @@ def load_library():
     lib.dimb_fstore_count.argtypes = [vp, ip, C.POINTER(ip), vp]
     lib.dimb_fstore_get.argtypes = [vp, ip, vp, vp, vp, vp, C.POINTER(ip), vp, ip]
     lib.dimb_fstore_feats_dev.argtypes = [vp, ip, C.POINTER(FeatsDev)]
+    lib.dimb_fstore_sg_feats_dev.argtypes = [vp, ip, C.POINTER(SgFeatsDev)]
     lib.dimb_gv_fundamental.argtypes = [vp, vp, vp, ip, fp, ip, C.c_uint, vp, vp, C.POINTER(ip)]
     lib.dimb_gv_fundamental_batch_dev.argtypes = [vp, ip, vp, vp, vp, vp, ip, fp, ip, C.c_uint, vp, vp, vp, vp]
     lib.dimb_fstore_block_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(C.c_size_t), C.POINTER(ip), C.POINTER(ip)]
@@ -480,13 +488,13 @@ def superglue_weight_names(n_layers: int = 18) -> list:
 
 
 class SuperGlueNet:
-    """Handle on dimb_sg: SuperGlue matching of one pair per call."""
+    """Handle on dimb_sg: SuperGlue matching of one host pair per call (match) or of up to max_pairs device pairs (match_dev)."""
 
     def __init__(self, ctx: Context, weights: dict, gnn_layers=("self", "cross") * 9, sinkhorn_iterations=100, match_threshold=0.2,
-                 max_kpts=2048):
+                 max_kpts=2048, max_pairs=1):
         self.ctx = ctx
         mask = sum(1 << i for i, n in enumerate(gnn_layers) if n == "cross")
-        self.conf = SgConf(len(gnn_layers), mask, int(sinkhorn_iterations), float(match_threshold), int(max_kpts))
+        self.conf = SgConf(len(gnn_layers), mask, int(sinkhorn_iterations), float(match_threshold), int(max_kpts), int(max_pairs))
         blob = np.ascontiguousarray(np.concatenate([np.asarray(weights[n], np.float32).ravel() for n in superglue_weight_names(len(gnn_layers))]))
         h = C.c_void_p()
         ctx.check(ctx.lib.dimb_sg_create(ctx.h, _ptr(blob), blob.size, C.byref(self.conf), C.byref(h)), "dimb_sg_create")
@@ -510,6 +518,15 @@ class SuperGlueNet:
         n = C.c_int(0)
         self.ctx.check(self.ctx.lib.dimb_sg_match(self.h, C.byref(fs[0]), C.byref(fs[1]), _ptr(m), _ptr(sc), C.byref(n), cap), "dimb_sg_match")
         return {"matches": m[: n.value].copy(), "scores": sc[: n.value].copy()}
+
+    def match_dev(self, f0: list, f1: list, d_matches, d_mscores, d_n_matches, cap, stream=0):
+        """f0/f1: lists of SgFeatsDev (device pointers); outputs [P][cap][2] int64, [P][cap], [P] int32 device buffers (ints are
+        device addresses); asynchronous on `stream`."""
+        P = len(f0)
+        a0 = (SgFeatsDev * P)(*f0)
+        a1 = (SgFeatsDev * P)(*f1)
+        self.ctx.check(self.ctx.lib.dimb_sg_match_dev(self.h, P, a0, a1, d_matches, d_mscores, d_n_matches, cap, stream),
+                       "dimb_sg_match_dev")
 
     def __del__(self):
         try:
@@ -636,6 +653,12 @@ class FeatureStoreDev:
     def feats_dev(self, slot: int) -> FeatsDev:
         f = FeatsDev()
         self.ctx.check(self.ctx.lib.dimb_fstore_feats_dev(self.h, slot, C.byref(f)), "dimb_fstore_feats_dev")
+        return f
+
+    def sg_feats_dev(self, slot: int) -> SgFeatsDev:
+        """The slot as SuperGlue input (float16 keypoints, descriptors and scores, image_size from the slot header)."""
+        f = SgFeatsDev()
+        self.ctx.check(self.ctx.lib.dimb_fstore_sg_feats_dev(self.h, slot, C.byref(f)), "dimb_fstore_sg_feats_dev")
         return f
 
     def desc_ptr(self, slot: int) -> int:

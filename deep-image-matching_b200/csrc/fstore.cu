@@ -199,6 +199,21 @@ int dimb_fstore_feats_dev(dimb_fstore* fs, int slot, dimb_feats_dev* out) {
   return DIMB_OK;
 }
 
+int dimb_fstore_sg_feats_dev(dimb_fstore* fs, int slot, dimb_sg_feats_dev* out) {
+  if (!fs || slot < 0 || slot >= fs->n_slots || !out) return DIMB_ERR_ARG;
+  const SlotPtrs s = slot_ptrs(fs, slot);
+  *out = dimb_sg_feats_dev{};
+  out->keypoints = s.kpts;
+  out->descriptors = s.desc;
+  out->scores = s.scores;
+  out->n = s.hdr;
+  out->n_cap = fs->cap;
+  out->desc_ld = fs->cap;
+  out->f16 = 1;
+  out->size_dev = s.hdr + 1;
+  return DIMB_OK;
+}
+
 int dimb_fstore_block_dev(dimb_fstore* fs, void** d_base, size_t* slot_bytes, int* n_slots, int* cap) {
   if (!fs) return DIMB_ERR_ARG;
   if (d_base) *d_base = fs->base;

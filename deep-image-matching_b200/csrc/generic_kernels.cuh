@@ -9,11 +9,12 @@ namespace {
 // ------------------------------------------------------------------ kernels
 // C[m][n] = act((sum_k A[m*lda + k] * W[n*ldw + k] + bias[n]) * scale) (+ resid[m*ldr + n]), act = ReLU or identity; 64 x 64 tile, 256 threads, 4 x 4 outputs
 // per thread, K streamed through shared memory 16 at a time (k ascending per output: deterministic summation order).
-__global__ void __launch_bounds__(256) gx_linear_kernel(const float* __restrict__ A, int lda, const float* __restrict__ W, int ldw,
-                                                        const float* __restrict__ bias, float* __restrict__ C, int ldc, int M, int N, int K,
-                                                        float scale, const float* __restrict__ resid, int ldr, int relu) {
+// The tile body is shared with SuperGlue's batched keypoint encoder (one more grid dimension over the sides).
+__device__ __forceinline__ void gx_linear_tile(const float* __restrict__ A, int lda, const float* __restrict__ W, int ldw,
+                                               const float* __restrict__ bias, float* __restrict__ C, int ldc, int M, int N, int K,
+                                               float scale, const float* __restrict__ resid, int ldr, int relu, int m0) {
   __shared__ float sa[16][64 + 4], sb[16][64 + 4];
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4, m0 = blockIdx.y * 64, n0 = blockIdx.x * 64;
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4, n0 = blockIdx.x * 64;
   float acc[4][4] = {};
   for (int k0 = 0; k0 < K; k0 += 16) {
     for (int e = threadIdx.x; e < 64 * 16; e += 256) {
@@ -48,6 +49,11 @@ __global__ void __launch_bounds__(256) gx_linear_kernel(const float* __restrict_
       C[static_cast<size_t>(m) * ldc + n] = v;
     }
   }
+}
+__global__ void __launch_bounds__(256) gx_linear_kernel(const float* __restrict__ A, int lda, const float* __restrict__ W, int ldw,
+                                                        const float* __restrict__ bias, float* __restrict__ C, int ldc, int M, int N, int K,
+                                                        float scale, const float* __restrict__ resid, int ldr, int relu) {
+  gx_linear_tile(A, lda, W, ldw, bias, C, ldc, M, N, K, scale, resid, ldr, relu, blockIdx.y * 64);
 }
 
 // keypoint normalisation (lightglue.py:24-34) + Fourier encoding (:57-70): enc [2][N][hd] = cos / sin, each frequency twice

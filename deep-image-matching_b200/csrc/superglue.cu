@@ -3,14 +3,25 @@
 // (thirdparty/SuperGluePretrainedNetwork/models/superglue.py:51-305: keypoint encoder :73-84, attentional GNN :96-152,
 // log-space Sinkhorn :155-187, mutual-max matching :278-296).
 //
-// SuperGlue's attention shape is 256 / 4 heads x 64 - the shape of LightGlue's tensor-core kernels - so the 18 GNN layers run on the
-// shared building blocks of lg_kernels.cuh: per layer ONE q|k GEMM (EpiQK without rotary), the V^T GEMM, the flash-attention kernel
-// (self: keys of the same side, cross: keys and values of the other side), merge -> message half of the [x | message] buffer, MLP0
-// with the eval-mode BatchNorm folded in and a ReLU / hi-lo-split epilogue, MLP3 + residual; then final_proj and the score matrix as
-// wgmma GEMMs, and 100 log-space Sinkhorn sweeps over the L2-resident score matrix with the dustbin row / column kept virtual
-// (coalesced row and column passes).  Done once at create time: BatchNorm folding, and the reference's (dim, heads)-interleaved
-// channel order of `view(b, dim, heads, n)` (:111-113) permuted to head-major.  The keypoint encoder (3 -> 32 -> 64 -> 128 -> 256 -> 256,
-// 0.2 GMAC) stays on the plain fp32 kernels of generic_kernels.cuh; the whole plain-fp32 path remains as the debug twin (DIMB_TC=0).
+// One batched engine (dimb_sg_match_dev) serves P pairs = S = 2P sides per call with no host synchronisation; side s owns rows
+// [s * NPt, (s + 1) * NPt) of every token buffer (NPt = max_kpts rounded up to 128), as in lightglue.cu.  Keypoint counts, the
+// per-pair Sinkhorn constants and the outputs stay on the device:
+//   input    : one kernel over all sides reads float32 / float16 keypoints, descriptors and scores (optional fp16 rounding), writes
+//              the token-major descriptors and the keypoint encoder's input (normalised x, y, score); padded rows are zero
+//   encoder  : 3 -> 32 -> 64 -> 128 -> 256 -> 256 on the plain fp32 tile of generic_kernels.cuh, one launch per layer over all sides
+//              (0.2 GMAC per side), rows past n skipped
+//   GNN      : SuperGlue's attention shape is 256 / 4 heads x 64 - the shape of LightGlue's tensor-core kernels - so the 18 layers run
+//              on the shared building blocks of lg_kernels.cuh: per layer ONE q|k GEMM (EpiQK without rotary), the V^T GEMM, the
+//              flash-attention kernel (self: keys of the same side, cross: keys and values of the other side), merge -> message half of
+//              the [x | message] buffer, MLP0 with the eval-mode BatchNorm folded in and a ReLU / hi-lo-split epilogue, MLP3 + residual;
+//              then final_proj and the score block of every pair (and its transpose) as wgmma GEMMs
+//   Sinkhorn : 100 log-space sweeps with the dustbin row / column kept virtual; one launch per half step serves a wave of pairs
+//              whose two score blocks fit in L2 together, so each sweep reads L2 rather than HBM (DESIGN.md section 3)
+//   matches  : row / column max and first argmax of the log assignment, then one CTA per pair for the mutual check, the threshold
+//              and the ordered compaction into the [P][cap] tables of dimb_lg_match_dev
+// Done once at create time: BatchNorm folding, and the reference's (dim, heads)-interleaved channel order of `view(b, dim, heads, n)`
+// (:111-113) permuted to head-major.  dimb_sg_match stages one host pair and runs the same engine with P = 1; its plain fp32 twin of
+// the GNN and Sinkhorn (DIMB_TC=0) remains as the debug path of that host entry.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -21,6 +32,8 @@
 #include "lg_kernels.cuh"
 
 namespace {
+
+constexpr int kSgD = 256, kSgHeads = 4, kSgHd = 64;
 
 // ---------------------------------------------------------------- tensor-core path helpers
 // out = relu(acc + bias) -> fp16 hi/lo planes (MLP0 with the BatchNorm folded into weights and bias), live tiles only
@@ -44,47 +57,110 @@ struct EpiSgReluSplit : EpiBase {
   }
 };
 
-// FeaturesDict inputs -> device layouts: descriptors (D,n) -> token-major [n][ldd] (32 x 32 tile transpose), keypoints / scores ->
-// the keypoint encoder's input [n][3] = (normalised x, normalised y, score)  (normalize_keypoints, superglue.py:63-70)
-__global__ void sg_input_kernel(const float* __restrict__ desc, int ld, int n, const float* __restrict__ kpts, const float* __restrict__ scores,
-                                float cx, float cy, float sc, float* __restrict__ dst, int ldd, float* __restrict__ enc_in) {
-  __shared__ float tile[32][33];
-  const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32, tx = threadIdx.x, ty = threadIdx.y;
-  for (int k = ty; k < 32; k += 8) tile[k][tx] = (t0 + tx < n) ? desc[static_cast<size_t>(c0 + k) * ld + t0 + tx] : 0.f;
-  __syncthreads();
-  for (int k = ty; k < 32; k += 8)
-    if (t0 + k < n) dst[static_cast<size_t>(t0 + k) * ldd + c0 + tx] = tile[tx][k];
-  if (blockIdx.y == 0 && ty == 0 && t0 + tx < n) {
-    const int i = t0 + tx;
-    enc_in[3 * i] = (kpts[2 * i] - cx) / sc;
-    enc_in[3 * i + 1] = (kpts[2 * i + 1] - cy) / sc;
-    enc_in[3 * i + 2] = scores[i];
+// one side of the batched engine (dimb_sg_feats_dev, resolved)
+struct SgSideIn {
+  const void *kpts, *desc, *scores;
+  const int* n;
+  int n_cap, ld, f16, round_fp16, height, width;
+  const int* size_dev;
+};
+
+// element i of a float32 or float16 array, float32 values optionally rounded to fp16 (the features.h5 round trip)
+__device__ __forceinline__ float sg_ld(const void* p, size_t i, int f16, int r16) {
+  if (f16) return __half2float(static_cast<const __half*>(p)[i]);
+  const float v = static_cast<const float*>(p)[i];
+  return r16 ? __half2float(__float2half_rn(v)) : v;
+}
+
+// live keypoints of side `side`: 0 for both sides of a pair with an empty side (the "no keypoints" return, superglue.py:248-256),
+// so that no later kernel does any work for that pair
+__device__ __forceinline__ int sg_side_n(const SgSideIn* in, int side, int NPs) {
+  const SgSideIn &a = in[side], &b = in[side ^ 1];
+  const int na = min(min(*a.n, a.n_cap), NPs), nb = min(min(*b.n, b.n_cap), NPs);
+  return (na <= 0 || nb <= 0) ? 0 : na;
+}
+
+// grid (ceil(NPs / 32), S), block (32, 8).  FeaturesDict inputs of every side -> descriptors token-major in dst rows
+// [side * NPs, (side + 1) * NPs) (pitch ldd, 32 x 32 tile transpose) and the keypoint encoder's input enc_in [row][3] = (normalised x,
+// normalised y, score) (normalize_keypoints, superglue.py:63-70); padded rows are zero.  Block 0 of every side records the live
+// count, and for even sides the pair's Sinkhorn constants pc[p] = {norm = -log(m + n), log n, log m} (:177-181).
+__global__ void sg_input_kernel(const SgSideIn* __restrict__ in, int NPs, float* __restrict__ dst, int ldd, float* __restrict__ enc_in,
+                                int* __restrict__ n_act, int* __restrict__ stopped, float* __restrict__ pc) {
+  const int side = blockIdx.y, t0 = blockIdx.x * 32, tx = threadIdx.x, ty = threadIdx.y;
+  const SgSideIn si = in[side];
+  const int n = sg_side_n(in, side, NPs);
+  if (blockIdx.x == 0 && tx == 0 && ty == 0) {
+    n_act[side] = n;
+    if ((side & 1) == 0) {
+      const int nb = sg_side_n(in, side + 1, NPs);
+      float* c = pc + 4 * (side >> 1);
+      stopped[side >> 1] = 0;  // SuperGlue has no early exit
+      c[0] = static_cast<float>(-log(static_cast<double>(n) + static_cast<double>(nb)));
+      c[1] = static_cast<float>(log(static_cast<double>(nb)));
+      c[2] = static_cast<float>(log(static_cast<double>(n)));
+    }
   }
+  __shared__ float tile[32][33];
+  for (int c0 = 0; c0 < kSgD; c0 += 32) {
+    for (int k = ty; k < 32; k += 8) {
+      const int tok = t0 + tx;
+      tile[k][tx] = tok < n ? sg_ld(si.desc, static_cast<size_t>(c0 + k) * si.ld + tok, si.f16, si.round_fp16) : 0.f;
+    }
+    __syncthreads();
+    for (int k = ty; k < 32; k += 8)
+      if (t0 + k < NPs) dst[(static_cast<size_t>(side) * NPs + t0 + k) * ldd + c0 + tx] = tile[tx][k];
+    __syncthreads();
+  }
+  const int tok = t0 + tx;
+  if (ty != 0 || tok >= NPs) return;
+  float* e = enc_in + (static_cast<size_t>(side) * NPs + tok) * 3;
+  if (tok >= n) {
+    e[0] = e[1] = e[2] = 0.f;
+    return;
+  }
+  const int H = si.size_dev ? si.size_dev[0] : si.height, W = si.size_dev ? si.size_dev[1] : si.width;
+  const float cx = static_cast<float>(W) / 2.f, cy = static_cast<float>(H) / 2.f, sc = static_cast<float>(max(W, H)) * 0.7f;
+  e[0] = (sg_ld(si.kpts, 2 * static_cast<size_t>(tok), si.f16, si.round_fp16) - cx) / sc;
+  e[1] = (sg_ld(si.kpts, 2 * static_cast<size_t>(tok) + 1, si.f16, si.round_fp16) - cy) / sc;
+  e[2] = sg_ld(si.scores, tok, si.f16, si.round_fp16);
 }
 
-// encoder output (fp32 [n][ld]) -> token state of side `side`: fp32 master + fp16 hi/lo first half of the concat buffer
-__global__ void sg_pack_kernel(const float* __restrict__ src, int ld, int n, int row0, float* __restrict__ x32, __half* __restrict__ xh,
-                               __half* __restrict__ xl) {
-  const int i = blockIdx.x, c = threadIdx.x;  // 256 threads = channels
-  if (i >= n) return;
-  const float v = src[static_cast<size_t>(i) * ld + c];
-  const size_t row = static_cast<size_t>(row0) + i;
-  x32[row * 256 + c] = v;
+// one keypoint-encoder layer over all sides: grid (ceil(N / 64), ceil(NPs / 64), S); rows past n_act[side] are neither read nor written
+__global__ void __launch_bounds__(256) sg_enc_linear_kernel(const float* __restrict__ A, int lda, const float* __restrict__ W,
+                                                            const float* __restrict__ bias, float* __restrict__ C, int ldc, int N, int K,
+                                                            int NPs, const int* __restrict__ n_act, int relu, int resid) {
+  const int side = blockIdx.z, M = n_act[side], m0 = blockIdx.y * 64;
+  if (m0 >= M) return;
+  const size_t r0 = static_cast<size_t>(side) * NPs;
+  float* c = C + r0 * ldc;
+  gx_linear_tile(A + r0 * lda, lda, W, K, bias, c, ldc, M, N, K, 1.f, resid ? c : nullptr, ldc, relu, m0);
+}
+
+// fp32 token state -> fp16 hi/lo first half of the [x | message] concat buffer, one 256-thread block per row (padded rows included)
+__global__ void sg_pack_kernel(const float* __restrict__ x32, __half* __restrict__ xh, __half* __restrict__ xl) {
+  const size_t row = blockIdx.x;
+  const int c = threadIdx.x;
   __half h, l;
-  split_f32(v, h, l);
-  xh[row * 512 + c] = h;
-  if (xl) xl[row * 512 + c] = l;
+  split_f32(x32[row * kSgD + c], h, l);
+  xh[row * 2 * kSgD + c] = h;
+  if (xl) xl[row * 2 * kSgD + c] = l;
 }
 
-// Sinkhorn half steps on the m x n score block S (row pitch ld) with the dustbin row / column (value alpha, :175-177) kept virtual.
-// Row pass: u[i] = log_mu(i) - logsumexp_j(Z(i, j) + v[j]) for i = 0..m (row m = dustbin), j = 0..n.  Warp per row, coalesced.
-__global__ void sg_sink_rows_kernel(const float* __restrict__ S, int ld, int m, int n, const float* __restrict__ alpha_p, const float* __restrict__ v,
-                                    float* __restrict__ u, float norm, float log_bin) {
+// One Sinkhorn half step for the pairs p0 + blockIdx.y of a wave, on the m x n score block S_p (row pitch ld, pairs pstride apart)
+// with the dustbin row / column (value alpha, :175-177) kept virtual.  dir 0 = row pass over sim:
+// u[i] = log_mu(i) - logsumexp_j(Z(i, j) + v[j]) for i = 0..m (row m = dustbin), j = 0..n; dir 1 = the column pass, the same
+// computation over the TRANSPOSED block simT with u and v swapped.  Warp per row, coalesced, one online log-sum-exp pass.
+__global__ void sg_sink_rows_kernel(const float* __restrict__ S, int ld, size_t pstride, int p0, const int* __restrict__ n_act, int dir,
+                                    const float* __restrict__ alpha_p, const float* __restrict__ add, float* __restrict__ out, int vld,
+                                    const float* __restrict__ pc) {
+  const int p = p0 + blockIdx.y;
+  const int m = n_act[2 * p + dir], n = n_act[2 * p + 1 - dir];
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (i > m) return;
+  if (m == 0 || i > m) return;
   const float alpha = alpha_p[0];
-  const float* row = S + static_cast<size_t>(i) * ld;
-  float mx = -INFINITY, s = 0.f;  // online log-sum-exp: one pass over the row
+  const float* row = S + p * pstride + static_cast<size_t>(i) * ld;
+  const float* v = add + static_cast<size_t>(p) * vld;
+  float mx = -INFINITY, s = 0.f;
   for (int j = lane; j <= n; j += 32) {
     const float x = ((i < m && j < n) ? row[j] : alpha) + v[j];
     if (x > mx) {
@@ -101,11 +177,11 @@ __global__ void sg_sink_rows_kernel(const float* __restrict__ S, int ld, int m, 
     s = (mx == -INFINITY ? 0.f : s * expf(mx - nm)) + (om == -INFINITY ? 0.f : os * expf(om - nm));
     mx = nm;
   }
-  if (lane == 0) u[i] = ((i == m) ? norm + log_bin : norm) - (mx + logf(s));
+  const float norm = pc[4 * p], log_bin = pc[4 * p + 1 + dir];
+  if (lane == 0) out[static_cast<size_t>(p) * vld + i] = ((i == m) ? norm + log_bin : norm) - (mx + logf(s));
 }
-// The column sweep v[j] = log_nu(j) - logsumexp_i(Z(i, j) + u[i]) is the same kernel on the TRANSPOSED score block (g->simT).
 
-// couplings (:175-177): fill the dustbin row / column of the (m+1) x (n+1) matrix with alpha
+// couplings (:175-177): fill the dustbin row / column of the (m+1) x (n+1) matrix with alpha (plain fp32 twin)
 __global__ void sg_fill_bins_kernel(float* __restrict__ Z, int ld, int m, int n, const float* __restrict__ alpha) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const float a = alpha[0];
@@ -113,10 +189,10 @@ __global__ void sg_fill_bins_kernel(float* __restrict__ Z, int ld, int m, int n,
   if (i < m) Z[static_cast<size_t>(i) * ld + n] = a;
 }
 
-// One Sinkhorn half step (:158-165): out[i] = log_marg(i) - logsumexp_j(Z[i][j] + add[j]) over rows (dir 0) or columns (dir 1) of
-// the (m+1) x (n+1) couplings; log_marg = norm for the regular entries, norm + log(other count) for the dustbin.  Warp per line.
+// One Sinkhorn half step of the plain fp32 twin (:158-165) on the materialised (m+1) x (n+1) couplings: out[i] = log_marg(i) -
+// logsumexp_j(Z[i][j] + add[j]) over rows (dir 0) or columns (dir 1); log_marg = norm, norm + log(other count) for the dustbin.
 __global__ void sg_sinkhorn_kernel(const float* __restrict__ Z, int ld, int m1, int n1, int dir, const float* __restrict__ add,
-                                   float* __restrict__ out, float norm, float log_bin) {
+                                   float* __restrict__ out, const float* __restrict__ pc) {
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   const int cnt = dir == 0 ? m1 : n1, len = dir == 0 ? n1 : m1;
   if (i >= cnt) return;
@@ -128,20 +204,24 @@ __global__ void sg_sinkhorn_kernel(const float* __restrict__ Z, int ld, int m1, 
   for (int j = lane; j < len; j += 32) s += expf((dir == 0 ? Z[static_cast<size_t>(i) * ld + j] : Z[static_cast<size_t>(j) * ld + i]) + add[j] - mx);
 #pragma unroll
   for (int of = 16; of; of >>= 1) s += __shfl_xor_sync(0xffffffffu, s, of);
-  if (lane == 0) out[i] = ((i == cnt - 1) ? norm + log_bin : norm) - (mx + logf(s));
+  if (lane == 0) out[i] = ((i == cnt - 1) ? pc[0] + pc[1 + dir] : pc[0]) - (mx + logf(s));
 }
 
-// row (dir 0) / column (dir 1) maximum and first argmax of Z[i][j] + u[i] + v[j] - norm over the inner m x n block (:279-280)
-__global__ void sg_argmax_kernel(const float* __restrict__ Z, int ld, int m, int n, const float* __restrict__ u, const float* __restrict__ v,
-                                 float norm, int dir, float* __restrict__ best, int* __restrict__ arg) {
+// Row maximum and first argmax of Z[i][j] + u[i] + v[j] - norm over the inner m x n block of every pair (:279-280): warp per row,
+// grid (ceil(NPs * 32 / 256), P); results at [p * NPs + i].
+__global__ void sg_row_max_kernel(const float* __restrict__ Z, int ld, size_t pstride, const int* __restrict__ n_act, const float* __restrict__ u,
+                                  const float* __restrict__ v, int vld, const float* __restrict__ pc, int NPs, float* __restrict__ best,
+                                  int* __restrict__ arg) {
+  const int p = blockIdx.y, m = n_act[2 * p], n = n_act[2 * p + 1];
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  const int cnt = dir == 0 ? m : n, len = dir == 0 ? n : m;
-  if (i >= cnt) return;
+  if (i >= m) return;
+  const float* row = Z + p * pstride + static_cast<size_t>(i) * ld;
+  const float ui = u[static_cast<size_t>(p) * vld + i], norm = pc[4 * p];
+  const float* vp = v + static_cast<size_t>(p) * vld;
   float bv = -INFINITY;
   int bi = 0x7fffffff;
-  for (int j = lane; j < len; j += 32) {
-    const int r = dir == 0 ? i : j, c = dir == 0 ? j : i;
-    const float val = ((Z[static_cast<size_t>(r) * ld + c] + u[r]) + v[c]) - norm;
+  for (int j = lane; j < n; j += 32) {
+    const float val = ((row[j] + ui) + vp[j]) - norm;
     if (val > bv) bv = val, bi = j;
   }
 #pragma unroll
@@ -150,7 +230,84 @@ __global__ void sg_argmax_kernel(const float* __restrict__ Z, int ld, int m, int
     const int oi = __shfl_xor_sync(0xffffffffu, bi, of);
     if (ov > bv || (ov == bv && oi < bi)) bv = ov, bi = oi;
   }
-  if (lane == 0) best[i] = bv, arg[i] = bi;
+  if (lane == 0) best[static_cast<size_t>(p) * NPs + i] = bv, arg[static_cast<size_t>(p) * NPs + i] = bi;
+}
+
+// Column first argmax of the same values: block (32, 32) = 32 columns x 32 row strides (coalesced reads), grid (ceil(NPs / 32), P)
+__global__ void __launch_bounds__(1024) sg_col_arg_kernel(const float* __restrict__ Z, int ld, size_t pstride, const int* __restrict__ n_act,
+                                                          const float* __restrict__ u, const float* __restrict__ v, int vld,
+                                                          const float* __restrict__ pc, int NPs, int* __restrict__ arg) {
+  const int p = blockIdx.y, m = n_act[2 * p], n = n_act[2 * p + 1];
+  const int tx = threadIdx.x, ty = threadIdx.y, j = blockIdx.x * 32 + tx;
+  if (blockIdx.x * 32 >= n) return;  // block-uniform
+  __shared__ float rv[32][33];
+  __shared__ int ri[32][33];
+  float bv = -INFINITY;
+  int bi = 0x7fffffff;
+  if (j < n) {
+    const float* up = u + static_cast<size_t>(p) * vld;
+    const float vj = v[static_cast<size_t>(p) * vld + j], norm = pc[4 * p];
+    const float* col = Z + p * pstride + j;
+    for (int i = ty; i < m; i += 32) {
+      const float val = ((col[static_cast<size_t>(i) * ld] + up[i]) + vj) - norm;
+      if (val > bv) bv = val, bi = i;
+    }
+  }
+  rv[ty][tx] = bv;
+  ri[ty][tx] = bi;
+  __syncthreads();
+  if (ty == 0 && j < n) {
+    for (int k = 1; k < 32; ++k)
+      if (rv[k][tx] > bv || (rv[k][tx] == bv && ri[k][tx] < bi)) bv = rv[k][tx], bi = ri[k][tx];
+    arg[static_cast<size_t>(p) * NPs + j] = bi;
+  }
+}
+
+// Mutual check, exp(max0) > match_threshold and ordered compaction (:281-296, correspondence_matrix_from_matches0): one CTA per
+// pair; n_matches[p] is the full count, only the first cap rows are written.  Modelled on lg_matches_kernel.
+__global__ void __launch_bounds__(1024) sg_matches_kernel(const int* __restrict__ n_act, int NPs, const float* __restrict__ best,
+                                                          const int* __restrict__ arg0, const int* __restrict__ arg1, float th,
+                                                          long long* __restrict__ matches, float* __restrict__ mscores,
+                                                          int* __restrict__ n_matches, int cap) {
+  const int p = blockIdx.x, t = threadIdx.x;
+  const int m = n_act[2 * p], n = n_act[2 * p + 1];
+  const size_t r0 = static_cast<size_t>(p) * NPs;
+  __shared__ int wsum[32];
+  __shared__ int s_base;
+  if (t == 0) s_base = 0;
+  __syncthreads();
+  if (m > 0 && n > 0) {
+    for (int base = 0; base < m; base += blockDim.x) {
+      const int i = base + t;
+      bool valid = false;
+      int j = 0;
+      float sc = 0.f;
+      if (i < m) {
+        j = arg0[r0 + i];
+        sc = expf(best[r0 + i]);
+        valid = arg1[r0 + j] == i && sc > th;
+      }
+      const unsigned bal = __ballot_sync(0xffffffffu, valid);
+      if ((t & 31) == 0) wsum[t >> 5] = __popc(bal);
+      __syncthreads();
+      int before = s_base;
+      for (int wv = 0; wv < (t >> 5); ++wv) before += wsum[wv];
+      before += __popc(bal & ((1u << (t & 31)) - 1u));
+      if (valid && before < cap) {
+        matches[(static_cast<size_t>(p) * cap + before) * 2 + 0] = i;
+        matches[(static_cast<size_t>(p) * cap + before) * 2 + 1] = j;
+        mscores[static_cast<size_t>(p) * cap + before] = sc;
+      }
+      __syncthreads();
+      if (t == 0) {
+        int tot = 0;
+        for (int wv = 0; wv < 32; ++wv) tot += wsum[wv];
+        s_base += tot;
+      }
+      __syncthreads();
+    }
+  }
+  if (t == 0) n_matches[p] = s_base;
 }
 
 struct SgLin {
@@ -176,28 +333,35 @@ struct dimb_sg {
   dimb_ctx* ctx;
   std::vector<void*> mem;
   dimb_sg_conf conf;
-  int NP, L;
+  int NP, L, max_pairs;
   std::vector<int> cross;  // per GNN layer: 1 = cross, 0 = self
   SgLin kenc[5];
   std::vector<SgLayer> layers;
   SgLin final_proj;
   float* bin_score;
-  float *cat[2], *q[2], *k[2], *v[2], *att, *hid, *enc_a, *enc_b, *md[2], *Z, *u, *vv, *best0, *best1;
-  int *arg0, *arg1;
-  // ---- tensor-core path (sides are rows [s * NPt, (s + 1) * NPt) of every token buffer, NPt = NP rounded up to 128)
-  int NPt = 0;
+  // ---- batched engine (side s = rows [s * NPt, (s + 1) * NPt) of every token buffer, NPt = NP rounded up to 128)
+  int NPt = 0, vld = 0, wave = 1;  // vld: pitch of the per-pair u / v vectors; wave: pairs per Sinkhorn launch (L2-resident blocks)
   std::vector<SgTcLayer> tc;
   SgTcLin tc_final;
-  float* x32 = nullptr;
+  SgSideIn* side_in = nullptr;  // [2 * max_pairs]
+  float *x32 = nullptr, *enc_in = nullptr;
   __half *xh, *xl, *qh, *ql, *kh, *kl, *vth, *vtl, *ctxh, *ctxl, *h2h, *h2l, *mdh, *mdl;
-  float *sim = nullptr, *simT = nullptr;  // score block and its transpose (both sweeps of a Sinkhorn iteration read rows)
+  float *sim = nullptr, *simT = nullptr;  // [P][NPt][NPt] score blocks and their transposes (both sweeps of a Sinkhorn iteration read rows)
   int *n_act = nullptr, *stopped = nullptr;
+  float *pc = nullptr, *uu = nullptr, *vv = nullptr, *best0 = nullptr;  // pc [P][4] Sinkhorn constants, uu / vv [P][vld]
+  int *arg0 = nullptr, *arg1 = nullptr;                                 // best0 / arg0 / arg1 [P][NPt]
   CUtensorMap m_x[2], m_ctx[2], m_h2[2], m_md[2], m_q128[2], m_k64[2], m_vt[2];
+  // ---- host entry: staging of one host pair, output tables, plain fp32 twin of the GNN and Sinkhorn (DIMB_TC=0)
+  float *st_kp = nullptr, *st_sc = nullptr, *st_desc = nullptr;
+  int* st_n = nullptr;
+  int64_t* o_m = nullptr;
+  float* o_ms = nullptr;
+  int* o_nm = nullptr;
+  int o_cap = 0;
+  float *cat = nullptr, *q[2], *k[2], *v[2], *att, *hid, *md[2], *Z;
 };
 
 namespace {
-
-constexpr int kSgD = 256, kSgHeads = 4, kSgHd = 64;
 
 int sg_linear(dimb_sg* g, cudaStream_t st, const float* A, int lda, const SgLin& l, float* C, int ldc, int M, int relu, float scale = 1.f,
               const float* resid = nullptr, int ldr = 0) {
@@ -272,10 +436,10 @@ int upload(dimb_ctx* ctx, SgLin& d, const HostLin& h) {
   return DIMB_OK;
 }
 
-// one GEMM over all 2 * NPt token rows: C = A [R][K] * W^T on the wgmma kernel of gemm.cuh with epilogue `epi`
+// one GEMM over the token rows of all S sides: C = A [S * NPt][K] * W^T on the wgmma kernel of gemm.cuh with epilogue `epi`
 template <class Epi>
-int sg_tc_gemm(dimb_sg* g, cudaStream_t st, const CUtensorMap* A, const __half* Ah, const __half* Al, int lda, const SgTcLin& w, int n_out,
-               const Epi& epi, const char* tag) {
+int sg_tc_gemm(dimb_sg* g, cudaStream_t st, int S, const CUtensorMap* A, const __half* Ah, const __half* Al, int lda, const SgTcLin& w,
+               int n_out, const Epi& epi, const char* tag) {
   TcOperands ops;
   ops.Ah = A[0];
   ops.Al = A[1];
@@ -283,7 +447,7 @@ int sg_tc_gemm(dimb_sg* g, cudaStream_t st, const CUtensorMap* A, const __half* 
   ops.Bl = w.tml;
   GemmArgs ga{};
   ga.num_kb = w.k / 64;
-  ga.M = 2 * g->NPt;
+  ga.M = S * g->NPt;
   ga.N = n_out;
   ga.Ah = Ah;
   ga.Al = Al;
@@ -291,33 +455,48 @@ int sg_tc_gemm(dimb_sg* g, cudaStream_t st, const CUtensorMap* A, const __half* 
   ga.Bl = w.wl;
   ga.lda = lda;
   ga.ldb = w.k;
-  return launch_gemm<128, false>(g->ctx, st, ops, ga, epi, 2 * g->NPt / kTileM, n_out, tag);
+  return launch_gemm<128, false>(g->ctx, st, ops, ga, epi, S * g->NPt / kTileM, n_out, tag);
 }
 
-// keypoint-encoded descriptors (g->cat[s], fp32) -> 18 GNN layers, final projection and the m x n score block (g->sim) on the
-// tensor-core kernels.  Both sides advance together from the OLD descriptors, as the reference does (superglue.py:147-151).
-int sg_gnn_tc(dimb_sg* g, cudaStream_t st, const int n[2]) {
+// keypoint encoder of S sides (rows of NPs per side; enc_in written by sg_input_kernel): dst rows += MLP(enc_in) (:73-84).  Its fp32
+// scratch lives in the MLP hidden buffers h2h / h2l, which the GNN only uses afterwards.
+int sg_encoder(dimb_sg* g, cudaStream_t st, int S, int NPs, float* dst, int ldd) {
+  dimb_ctx* ctx = g->ctx;
+  ProfScope prof(ctx, st, "sg.encoder");
+  float *a = g->enc_in, *b = reinterpret_cast<float*>(g->h2h), *spare = reinterpret_cast<float*>(g->h2l);
+  int lda = 3;
+  for (int i = 0; i < 5; ++i) {
+    const SgLin& l = g->kenc[i];
+    const bool last = i == 4;  // no BN / ReLU; desc = desc + kenc(...)
+    dim3 grid(ceil_div(l.n, 64), ceil_div(NPs, 64), S);
+    sg_enc_linear_kernel<<<grid, 256, 0, st>>>(a, lda, l.w, l.b, last ? dst : b, last ? ldd : l.n, l.n, l.k, NPs, g->n_act, last ? 0 : 1,
+                                               last ? 1 : 0);
+    DIMB_LAUNCH_CHECK(ctx);
+    a = b;
+    std::swap(b, spare);
+    lda = l.n;
+  }
+  return DIMB_OK;
+}
+
+// encoded descriptors (g->x32 / g->xh / g->xl of S = 2P sides) -> 18 GNN layers, final projection and the score blocks of the P pairs
+// (g->sim and its transpose g->simT) on the tensor-core kernels.  Both sides advance together from the OLD descriptors, as the
+// reference does (superglue.py:147-151).  Live rows come from g->n_act (device).
+int sg_gnn_tc(dimb_sg* g, cudaStream_t st, int P) {
   dimb_ctx* ctx = g->ctx;
   const bool exact = ctx->precision == DIMB_PRECISION_EXACT;
-  const int NPt = g->NPt, d = kSgD, R = 2 * NPt;
-  const int zero = 0;
-  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(g->n_act, n, 2 * sizeof(int), cudaMemcpyHostToDevice, st));
-  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(g->stopped, &zero, sizeof(int), cudaMemcpyHostToDevice, st));
-  for (int s = 0; s < 2; ++s) {
-    sg_pack_kernel<<<n[s], 256, 0, st>>>(g->cat[s], 2 * d, n[s], s * NPt, g->x32, g->xh, exact ? g->xl : nullptr);
-    DIMB_LAUNCH_CHECK(ctx);
-  }
+  const int NPt = g->NPt, d = kSgD, S = 2 * P, R = S * NPt;
   const LgRows rows{g->n_act, g->stopped, NPt};
   for (int i = 0; i < g->L; ++i) {
     const SgTcLayer& ly = g->tc[i];
-    {  // q | k for every token of both sides (no rotary: EpiQK's cross flag only switches the rotation off)
+    {  // q | k for every token of every side (no rotary: EpiQK's cross flag only switches the rotation off)
       EpiQK e;
       e.rows = rows;
       e.bias = ly.qkv.bias;
       e.cs = e.sn = nullptr;
       e.qh = g->qh, e.ql = exact ? g->ql : nullptr, e.kh = g->kh, e.kl = exact ? g->kl : nullptr;
       e.cross = 1;
-      DIMB_TRY(sg_tc_gemm(g, st, g->m_x, g->xh, g->xl, 2 * d, ly.qkv, 2 * d, e, "sg.qk"));
+      DIMB_TRY(sg_tc_gemm(g, st, S, g->m_x, g->xh, g->xl, 2 * d, ly.qkv, 2 * d, e, "sg.qk"));
     }
     {  // V^T: weights as the A operand (rows 512..767 of the stacked projection), tokens as B
       EpiVT e;
@@ -342,7 +521,7 @@ int sg_gnn_tc(dimb_sg* g, cudaStream_t st, const int n[2]) {
       a.scale = 0.125f;
       a.lazy = ctx->attn_lazy;
       ProfScope prof(ctx, st, "sg.attention");
-      dim3 grid(ceil_div(NPt, 2 * kTileM), kHeads, 2);
+      dim3 grid(ceil_div(NPt, 2 * kTileM), kHeads, S);
       DIMB_TRY(launch_lg_attention(ctx, st, grid, g->m_q128, g->m_k64, g->m_vt, a, exact));
       DIMB_LAUNCH_CHECK(ctx);
     }
@@ -352,7 +531,7 @@ int sg_gnn_tc(dimb_sg* g, cudaStream_t st, const int n[2]) {
       e.hi = g->xh, e.lo = exact ? g->xl : nullptr;
       e.bias = ly.merge.bias;
       e.ldc = 2 * d, e.col_off = d;
-      DIMB_TRY(sg_tc_gemm(g, st, g->m_ctx, g->ctxh, g->ctxl, d, ly.merge, d, e, "sg.merge"));
+      DIMB_TRY(sg_tc_gemm(g, st, S, g->m_ctx, g->ctxh, g->ctxl, d, ly.merge, d, e, "sg.merge"));
     }
     {  // MLP0 (BatchNorm folded) + ReLU
       EpiSgReluSplit e;
@@ -360,7 +539,7 @@ int sg_gnn_tc(dimb_sg* g, cudaStream_t st, const int n[2]) {
       e.hi = g->h2h, e.lo = exact ? g->h2l : nullptr;
       e.bias = ly.mlp0.bias;
       e.ldc = 2 * d;
-      DIMB_TRY(sg_tc_gemm(g, st, g->m_x, g->xh, g->xl, 2 * d, ly.mlp0, 2 * d, e, "sg.mlp0"));
+      DIMB_TRY(sg_tc_gemm(g, st, S, g->m_x, g->xh, g->xl, 2 * d, ly.mlp0, 2 * d, e, "sg.mlp0"));
     }
     {  // x += MLP3(...)
       EpiLgResidual e;
@@ -369,7 +548,7 @@ int sg_gnn_tc(dimb_sg* g, cudaStream_t st, const int n[2]) {
       e.xh = g->xh, e.xl = exact ? g->xl : nullptr;
       e.bias = ly.mlp3.bias;
       e.residual = 1;
-      DIMB_TRY(sg_tc_gemm(g, st, g->m_h2, g->h2h, g->h2l, 2 * d, ly.mlp3, d, e, "sg.mlp3"));
+      DIMB_TRY(sg_tc_gemm(g, st, S, g->m_h2, g->h2h, g->h2l, 2 * d, ly.mlp3, d, e, "sg.mlp3"));
     }
   }
   {  // mdesc = final_proj(x) / 256^0.25 on each side, so that the score block is mdesc0 . mdesc1^T / sqrt(256) (:262-265)
@@ -378,7 +557,7 @@ int sg_gnn_tc(dimb_sg* g, cudaStream_t st, const int n[2]) {
     e.bias = g->tc_final.bias;
     e.ldc = d, e.col_off = 0, e.n_valid = d, e.m_valid = R;
     e.scale = 0.25f;
-    DIMB_TRY(sg_tc_gemm(g, st, g->m_x, g->xh, g->xl, 2 * d, g->tc_final, d, e, "sg.final_proj"));
+    DIMB_TRY(sg_tc_gemm(g, st, S, g->m_x, g->xh, g->xl, 2 * d, g->tc_final, d, e, "sg.final_proj"));
   }
   {
     EpiSim e;
@@ -393,12 +572,78 @@ int sg_gnn_tc(dimb_sg* g, cudaStream_t st, const int n[2]) {
     ga.M = R, ga.N = R;
     ga.Ah = g->mdh, ga.Al = g->mdl, ga.Bh = g->mdh, ga.Bl = g->mdl;
     ga.lda = d, ga.ldb = d;
-    DIMB_TRY((launch_gemm<128, false>(ctx, st, ops, ga, e, NPt / kTileM, NPt, "sg.scores")));
+    DIMB_TRY((launch_gemm<128, false>(ctx, st, ops, ga, e, P * (NPt / kTileM), NPt, "sg.scores")));
     e.sim = g->simT;  // the same products with the operand roles swapped: scores^T, so that the column sweeps of Sinkhorn read rows
     e.swap = 1;
-    DIMB_TRY((launch_gemm<128, false>(ctx, st, ops, ga, e, NPt / kTileM, NPt, "sg.scores")));
+    DIMB_TRY((launch_gemm<128, false>(ctx, st, ops, ga, e, P * (NPt / kTileM), NPt, "sg.scores")));
   }
   return DIMB_OK;
+}
+
+// row / column max and first argmax of the log assignment (score blocks Z of pitch ld, pairs pstride apart) and the match tables
+int sg_matches(dimb_sg* g, cudaStream_t st, int P, const float* Z, int ld, size_t pstride, int NPs, int64_t* d_matches, float* d_mscores,
+               int* d_n_matches, int cap) {
+  dimb_ctx* ctx = g->ctx;
+  ProfScope prof(ctx, st, "sg.matches");
+  sg_row_max_kernel<<<dim3(ceil_div(NPs * 32, 256), P), 256, 0, st>>>(Z, ld, pstride, g->n_act, g->uu, g->vv, g->vld, g->pc, NPs, g->best0,
+                                                                      g->arg0);
+  DIMB_LAUNCH_CHECK(ctx);
+  sg_col_arg_kernel<<<dim3(ceil_div(NPs, 32), P), dim3(32, 32), 0, st>>>(Z, ld, pstride, g->n_act, g->uu, g->vv, g->vld, g->pc, NPs, g->arg1);
+  DIMB_LAUNCH_CHECK(ctx);
+  sg_matches_kernel<<<P, 1024, 0, st>>>(g->n_act, NPs, g->best0, g->arg0, g->arg1, g->conf.match_threshold,
+                                        reinterpret_cast<long long*>(d_matches), d_mscores, d_n_matches, cap);
+  DIMB_LAUNCH_CHECK(ctx);
+  return DIMB_OK;
+}
+
+// DIMB_TC=0 debug path of the host entry: one pair (features staged in d[2], n[2] live counts known on the host) through the same
+// input kernel and encoder, then the plain fp32 GNN and Sinkhorn on the materialised couplings.
+int sg_match_plain(dimb_sg* g, cudaStream_t st, const SgSideIn* hin, const int n[2], int cap) {
+  dimb_ctx* ctx = g->ctx;
+  const int NP = g->NP, d = kSgD, m = n[0], nn = n[1];
+  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(g->side_in, hin, 2 * sizeof(SgSideIn), cudaMemcpyHostToDevice, st));
+  sg_input_kernel<<<dim3(ceil_div(NP, 32), 2), dim3(32, 8), 0, st>>>(g->side_in, NP, g->cat, 2 * d, g->enc_in, g->n_act, g->stopped, g->pc);
+  DIMB_LAUNCH_CHECK(ctx);
+  DIMB_TRY(sg_encoder(g, st, 2, NP, g->cat, 2 * d));
+  float* cat[2] = {g->cat, g->cat + static_cast<size_t>(NP) * 2 * d};
+  for (int i = 0; i < g->L; ++i) {  // AttentionalGNN (:132-152): deltas of both sides from the OLD descriptors
+    const SgLayer& ly = g->layers[i];
+    for (int s = 0; s < 2; ++s) {
+      const int src = g->cross[i] ? 1 - s : s;
+      DIMB_TRY(sg_linear(g, st, cat[s], 2 * d, ly.q, g->q[s], d, n[s], 0));
+      DIMB_TRY(sg_linear(g, st, cat[src], 2 * d, ly.k, g->k[s], d, n[src], 0));
+      DIMB_TRY(sg_linear(g, st, cat[src], 2 * d, ly.v, g->v[s], d, n[src], 0));
+    }
+    for (int s = 0; s < 2; ++s) {
+      const int src = g->cross[i] ? 1 - s : s;
+      dim3 grid(ceil_div(n[s], 8), kSgHeads);
+      gx_attention_kernel<64><<<grid, 256, 0, st>>>(g->q[s], g->k[s], g->v[s], n[s], n[src], d, kSgHd, g->att, d);
+      DIMB_LAUNCH_CHECK(ctx);
+      DIMB_TRY(sg_linear(g, st, g->att, d, ly.merge, cat[s] + d, 2 * d, n[s], 0));  // message -> right half of [x | message]
+    }
+    for (int s = 0; s < 2; ++s) {  // x += mlp([x | message])
+      DIMB_TRY(sg_linear(g, st, cat[s], 2 * d, ly.mlp0, g->hid, 2 * d, n[s], 1));
+      DIMB_TRY(sg_linear(g, st, g->hid, 2 * d, ly.mlp3, cat[s], 2 * d, n[s], 0, 1.f, cat[s], 2 * d));
+    }
+  }
+  for (int s = 0; s < 2; ++s) DIMB_TRY(sg_linear(g, st, cat[s], 2 * d, g->final_proj, g->md[s], d, n[s], 0));
+  const int ld = nn + 1;
+  {  // scores = mdesc0 . mdesc1^T / sqrt(256) into the top-left block of the couplings
+    dim3 grid(ceil_div(nn, 64), ceil_div(m, 64));
+    gx_linear_kernel<<<grid, 256, 0, st>>>(g->md[0], d, g->md[1], d, nullptr, g->Z, ld, m, nn, d, 1.f / 16.f, nullptr, 0, 0);
+    DIMB_LAUNCH_CHECK(ctx);
+  }
+  sg_fill_bins_kernel<<<ceil_div(std::max(m, nn) + 1, 256), 256, 0, st>>>(g->Z, ld, m, nn, g->bin_score);
+  DIMB_LAUNCH_CHECK(ctx);
+  DIMB_CUDA_OK(ctx, cudaMemsetAsync(g->uu, 0, g->vld * sizeof(float), st));
+  DIMB_CUDA_OK(ctx, cudaMemsetAsync(g->vv, 0, g->vld * sizeof(float), st));
+  for (int it = 0; it < g->conf.sinkhorn_iterations; ++it) {
+    sg_sinkhorn_kernel<<<ceil_div((m + 1) * 32, 256), 256, 0, st>>>(g->Z, ld, m + 1, nn + 1, 0, g->vv, g->uu, g->pc);
+    DIMB_LAUNCH_CHECK(ctx);
+    sg_sinkhorn_kernel<<<ceil_div((nn + 1) * 32, 256), 256, 0, st>>>(g->Z, ld, m + 1, nn + 1, 1, g->uu, g->vv, g->pc);
+    DIMB_LAUNCH_CHECK(ctx);
+  }
+  return sg_matches(g, st, 1, g->Z, ld, 0, NP, g->o_m, g->o_ms, g->o_nm, cap);
 }
 
 }  // namespace
@@ -417,7 +662,8 @@ size_t dimb_sg_weight_count(int n_layers) {
 int dimb_sg_create(dimb_ctx* ctx, const float* weights, size_t n_floats, const dimb_sg_conf* conf, dimb_sg** out) {
   if (!ctx || !weights || !conf || !out) return DIMB_ERR_ARG;
   *out = nullptr;
-  if (conf->n_layers < 1 || conf->n_layers > 64 || conf->max_kpts < 1 || conf->sinkhorn_iterations < 0) return DIMB_ERR_ARG;
+  if (conf->n_layers < 1 || conf->n_layers > 64 || conf->max_kpts < 1 || conf->sinkhorn_iterations < 0 || conf->max_pairs < 0)
+    return DIMB_ERR_ARG;
   if (n_floats != dimb_sg_weight_count(conf->n_layers)) {
     dimb_set_error(ctx, "dimb_sg_create: weight blob has " + std::to_string(n_floats) + " floats, expected " +
                             std::to_string(dimb_sg_weight_count(conf->n_layers)));
@@ -431,6 +677,7 @@ int dimb_sg_create(dimb_ctx* ctx, const float* weights, size_t n_floats, const d
   g->conf = *conf;
   g->L = conf->n_layers;
   g->NP = conf->max_kpts;
+  g->max_pairs = conf->max_pairs ? conf->max_pairs : 1;
   for (int i = 0; i < g->L; ++i) g->cross.push_back((conf->cross_mask >> i) & 1ull ? 1 : 0);
   const float* p = weights;
   const int ch[6] = {3, 32, 64, 128, 256, 256};
@@ -475,38 +722,50 @@ int dimb_sg_create(dimb_ctx* ctx, const float* weights, size_t n_floats, const d
   }
   DIMB_TRY(dimb_alloc_t(ctx, &g->bin_score, 1, false));
   DIMB_CUDA_OK(ctx, cudaMemcpy(g->bin_score, p, sizeof(float), cudaMemcpyHostToDevice));
-  const size_t NP = g->NP;
-  for (int s = 0; s < 2; ++s) {
-    DIMB_TRY(dimb_alloc_t(ctx, &g->cat[s], NP * 2 * kSgD));
-    DIMB_TRY(dimb_alloc_t(ctx, &g->q[s], NP * kSgD));
-    DIMB_TRY(dimb_alloc_t(ctx, &g->k[s], NP * kSgD));
-    DIMB_TRY(dimb_alloc_t(ctx, &g->v[s], NP * kSgD));
-    DIMB_TRY(dimb_alloc_t(ctx, &g->md[s], NP * kSgD));
+  const size_t NP = g->NP, PP = g->max_pairs, d = kSgD;
+  {  // host entry: staging of one pair, outputs, plain fp32 twin
+    DIMB_TRY(dimb_alloc_t(ctx, &g->st_kp, 2 * NP * 2));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->st_sc, 2 * NP));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->st_desc, 2 * d * NP));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->st_n, 2));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->o_nm, 1));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->cat, 2 * NP * 2 * d));
+    for (int s = 0; s < 2; ++s) {
+      DIMB_TRY(dimb_alloc_t(ctx, &g->q[s], NP * d));
+      DIMB_TRY(dimb_alloc_t(ctx, &g->k[s], NP * d));
+      DIMB_TRY(dimb_alloc_t(ctx, &g->v[s], NP * d));
+      DIMB_TRY(dimb_alloc_t(ctx, &g->md[s], NP * d));
+    }
+    DIMB_TRY(dimb_alloc_t(ctx, &g->att, NP * d));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->hid, NP * 2 * d));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->Z, (NP + 1) * (NP + 1)));
   }
-  DIMB_TRY(dimb_alloc_t(ctx, &g->att, NP * kSgD));
-  DIMB_TRY(dimb_alloc_t(ctx, &g->hid, NP * 2 * kSgD));
-  DIMB_TRY(dimb_alloc_t(ctx, &g->enc_a, NP * kSgD));
-  DIMB_TRY(dimb_alloc_t(ctx, &g->enc_b, NP * kSgD));
-  DIMB_TRY(dimb_alloc_t(ctx, &g->Z, (NP + 1) * (NP + 1)));
-  DIMB_TRY(dimb_alloc_t(ctx, &g->u, NP + 1));
-  DIMB_TRY(dimb_alloc_t(ctx, &g->vv, NP + 1));
-  DIMB_TRY(dimb_alloc_t(ctx, &g->best0, NP));
-  DIMB_TRY(dimb_alloc_t(ctx, &g->best1, NP));
-  DIMB_TRY(dimb_alloc_t(ctx, &g->arg0, NP));
-  DIMB_TRY(dimb_alloc_t(ctx, &g->arg1, NP));
-  {  // tensor-core path state
-    const size_t NPt = round_up(g->NP, 128), R = 2 * NPt, d = kSgD;
+  {  // batched engine
+    const size_t NPt = round_up(g->NP, 128), S = 2 * PP, R = S * NPt;
     g->NPt = static_cast<int>(NPt);
+    g->vld = static_cast<int>(NPt) + 1;
+    // Sinkhorn waves: as many pairs per launch as keep their sim + simT blocks (at capacity) within 3/4 of L2
+    int l2 = 0;
+    DIMB_CUDA_OK(ctx, cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, ctx->device));
+    g->wave = std::max<int>(1, static_cast<int>(static_cast<size_t>(l2) * 3 / 4 / (2 * NPt * NPt * sizeof(float))));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->side_in, S));
     DIMB_TRY(dimb_alloc_t(ctx, &g->x32, R * d));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->enc_in, R * 3));
     DIMB_TRY(dimb_alloc_t(ctx, &g->xh, R * 2 * d));
     DIMB_TRY(dimb_alloc_t(ctx, &g->xl, R * 2 * d));
     DIMB_TRY(dimb_alloc_t(ctx, &g->h2h, R * 2 * d));
     DIMB_TRY(dimb_alloc_t(ctx, &g->h2l, R * 2 * d));
     for (__half** b : {&g->qh, &g->ql, &g->kh, &g->kl, &g->vth, &g->vtl, &g->ctxh, &g->ctxl, &g->mdh, &g->mdl}) DIMB_TRY(dimb_alloc_t(ctx, b, R * d));
-    DIMB_TRY(dimb_alloc_t(ctx, &g->sim, NPt * NPt));
-    DIMB_TRY(dimb_alloc_t(ctx, &g->simT, NPt * NPt));
-    DIMB_TRY(dimb_alloc_t(ctx, &g->n_act, 2));
-    DIMB_TRY(dimb_alloc_t(ctx, &g->stopped, 1));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->sim, PP * NPt * NPt));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->simT, PP * NPt * NPt));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->n_act, S));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->stopped, PP));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->pc, 4 * PP));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->uu, PP * g->vld));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->vv, PP * g->vld));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->best0, PP * NPt));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->arg0, PP * NPt));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->arg1, PP * NPt));
     DIMB_TRY(dimb_tmap_2d(ctx, &g->m_x[0], g->xh, R, 2 * d, 2 * d, kTileM));
     DIMB_TRY(dimb_tmap_2d(ctx, &g->m_x[1], g->xl, R, 2 * d, 2 * d, kTileM));
     DIMB_TRY(dimb_tmap_2d(ctx, &g->m_h2[0], g->h2h, R, 2 * d, 2 * d, kTileM));
@@ -515,12 +774,12 @@ int dimb_sg_create(dimb_ctx* ctx, const float* weights, size_t n_floats, const d
     DIMB_TRY(dimb_tmap_2d(ctx, &g->m_ctx[1], g->ctxl, R, d, d, kTileM));
     DIMB_TRY(dimb_tmap_2d(ctx, &g->m_md[0], g->mdh, R, d, d, kTileM));
     DIMB_TRY(dimb_tmap_2d(ctx, &g->m_md[1], g->mdl, R, d, d, kTileM));
-    DIMB_TRY(dimb_tmap_2d(ctx, &g->m_q128[0], g->qh, 2 * kHeads * NPt, kHd, kHd, kTileM));
-    DIMB_TRY(dimb_tmap_2d(ctx, &g->m_q128[1], g->ql, 2 * kHeads * NPt, kHd, kHd, kTileM));
-    DIMB_TRY(dimb_tmap_2d(ctx, &g->m_k64[0], g->kh, 2 * kHeads * NPt, kHd, kHd, kBlkK));
-    DIMB_TRY(dimb_tmap_2d(ctx, &g->m_k64[1], g->kl, 2 * kHeads * NPt, kHd, kHd, kBlkK));
-    DIMB_TRY(dimb_tmap_2d(ctx, &g->m_vt[0], g->vth, 2 * kHeads * kHd, NPt, NPt, kHd));
-    DIMB_TRY(dimb_tmap_2d(ctx, &g->m_vt[1], g->vtl, 2 * kHeads * kHd, NPt, NPt, kHd));
+    DIMB_TRY(dimb_tmap_2d(ctx, &g->m_q128[0], g->qh, S * kHeads * NPt, kHd, kHd, kTileM));
+    DIMB_TRY(dimb_tmap_2d(ctx, &g->m_q128[1], g->ql, S * kHeads * NPt, kHd, kHd, kTileM));
+    DIMB_TRY(dimb_tmap_2d(ctx, &g->m_k64[0], g->kh, S * kHeads * NPt, kHd, kHd, kBlkK));
+    DIMB_TRY(dimb_tmap_2d(ctx, &g->m_k64[1], g->kl, S * kHeads * NPt, kHd, kHd, kBlkK));
+    DIMB_TRY(dimb_tmap_2d(ctx, &g->m_vt[0], g->vth, S * kHeads * kHd, NPt, NPt, kHd));
+    DIMB_TRY(dimb_tmap_2d(ctx, &g->m_vt[1], g->vtl, S * kHeads * kHd, NPt, NPt, kHd));
   }
   *out = guard.release();
   return DIMB_OK;
@@ -532,8 +791,66 @@ void dimb_sg_destroy(dimb_sg* g) {
   delete g;
 }
 
+int dimb_sg_match_dev(dimb_sg* g, int P, const dimb_sg_feats_dev* f0, const dimb_sg_feats_dev* f1, int64_t* d_matches, float* d_mscores,
+                      int* d_n_matches, int cap, void* stream) {
+  if (!g || !f0 || !f1 || !d_matches || !d_mscores || !d_n_matches || P < 1 || P > g->max_pairs || cap < 1) return DIMB_ERR_ARG;
+  dimb_ctx* ctx = g->ctx;
+  const int S = 2 * P, NPt = g->NPt;
+  std::vector<SgSideIn> hin(S);
+  for (int p = 0; p < P; ++p)
+    for (int sd = 0; sd < 2; ++sd) {
+      const dimb_sg_feats_dev& f = sd ? f1[p] : f0[p];
+      if (!f.keypoints || !f.descriptors || !f.scores || !f.n || f.n_cap < 0 || f.n_cap > g->NP) {
+        dimb_set_error(ctx, "dimb_sg_match_dev: pair " + std::to_string(p) + " side " + std::to_string(sd) +
+                                ": NULL keypoints / descriptors / scores / n, or n_cap above max_kpts");
+        return DIMB_ERR_ARG;
+      }
+      hin[2 * p + sd] = SgSideIn{f.keypoints, f.descriptors, f.scores, f.n, f.n_cap, f.desc_ld ? f.desc_ld : f.n_cap, f.f16, f.round_fp16,
+                                 f.height, f.width, f.size_dev};
+    }
+  if (!ctx->use_tc) {
+    dimb_set_error(ctx, "dimb_sg_match_dev: the device entry runs on the tensor-core path only (tensor path is off: DIMB_TC=0 or "
+                        "dimb_ctx_set_tensor_path); dimb_sg_match serves the fp32 debug path");
+    return DIMB_ERR_UNSUPPORTED;
+  }
+  OwnerScope own(ctx, &g->mem);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(g->side_in, hin.data(), S * sizeof(SgSideIn), cudaMemcpyHostToDevice, st));
+  {
+    ProfScope prof(ctx, st, "sg.input");
+    sg_input_kernel<<<dim3(NPt / 32, S), dim3(32, 8), 0, st>>>(g->side_in, NPt, g->x32, kSgD, g->enc_in, g->n_act, g->stopped, g->pc);
+    DIMB_LAUNCH_CHECK(ctx);
+  }
+  DIMB_TRY(sg_encoder(g, st, S, NPt, g->x32, kSgD));
+  {
+    ProfScope prof(ctx, st, "sg.input");
+    sg_pack_kernel<<<S * NPt, kSgD, 0, st>>>(g->x32, g->xh, ctx->precision == DIMB_PRECISION_EXACT ? g->xl : nullptr);
+    DIMB_LAUNCH_CHECK(ctx);
+  }
+  DIMB_TRY(sg_gnn_tc(g, st, P));
+  {  // wave by wave: all iterations of a wave run while its score blocks are L2-resident
+    ProfScope prof(ctx, st, "sg.sinkhorn");
+    const size_t ps = static_cast<size_t>(NPt) * NPt;
+    DIMB_CUDA_OK(ctx, cudaMemsetAsync(g->uu, 0, static_cast<size_t>(P) * g->vld * sizeof(float), st));
+    DIMB_CUDA_OK(ctx, cudaMemsetAsync(g->vv, 0, static_cast<size_t>(P) * g->vld * sizeof(float), st));
+    const dim3 blk(256);
+    const int gx = ceil_div((NPt + 1) * 32, 256);
+    for (int p0 = 0; p0 < P; p0 += g->wave) {
+      const int np = std::min(g->wave, P - p0);
+      for (int it = 0; it < g->conf.sinkhorn_iterations; ++it) {
+        sg_sink_rows_kernel<<<dim3(gx, np), blk, 0, st>>>(g->sim, NPt, ps, p0, g->n_act, 0, g->bin_score, g->vv, g->uu, g->vld, g->pc);
+        DIMB_LAUNCH_CHECK(ctx);
+        sg_sink_rows_kernel<<<dim3(gx, np), blk, 0, st>>>(g->simT, NPt, ps, p0, g->n_act, 1, g->bin_score, g->uu, g->vv, g->vld, g->pc);
+        DIMB_LAUNCH_CHECK(ctx);
+      }
+    }
+  }
+  return sg_matches(g, st, P, g->sim, NPt, static_cast<size_t>(NPt) * NPt, NPt, d_matches, d_mscores, d_n_matches, cap);
+}
+
 // One pair.  Outputs (host): matches [cap][2] int64 ascending in column 0 (correspondence_matrix_from_matches0, superglue.py:44-52),
-// mscores [cap] (matching_scores0 of the matched rows), n_matches.
+// mscores [cap] (matching_scores0 of the matched rows), n_matches.  Stages the pair and runs dimb_sg_match_dev with P = 1
+// (or, with the tensor path off, the plain fp32 twin).
 int dimb_sg_match(dimb_sg* g, const dimb_sg_feats* f0, const dimb_sg_feats* f1, int64_t* matches, float* mscores, int* n_matches, int cap) {
   if (!g || !f0 || !f1 || !matches || !mscores || !n_matches || cap < 1) return DIMB_ERR_ARG;
   dimb_ctx* ctx = g->ctx;
@@ -548,113 +865,39 @@ int dimb_sg_match(dimb_sg* g, const dimb_sg_feats* f0, const dimb_sg_feats* f1, 
     return DIMB_ERR_ARG;
   }
   if (n[0] == 0 || n[1] == 0) return DIMB_OK;  // "no keypoints" return of the reference (superglue.py:248-256): everything unmatched
+  if (g->o_cap < cap) {
+    dimb_free(ctx, g->o_m);
+    dimb_free(ctx, g->o_ms);
+    DIMB_TRY(dimb_alloc_t(ctx, &g->o_m, static_cast<size_t>(cap) * 2));
+    DIMB_TRY(dimb_alloc_t(ctx, &g->o_ms, static_cast<size_t>(cap)));
+    g->o_cap = cap;
+  }
+  dimb_sg_feats_dev df[2];
+  SgSideIn hin[2];
   for (int s = 0; s < 2; ++s) {
     const dimb_sg_feats& f = *F[s];
-    // descriptors arrive (D,N) like the FeaturesDict: copied as they are, transposed to token-major on the device together with the
-    // keypoint encoder's input (normalised x, normalised y, score)
-    const float cx = static_cast<float>(f.width) / 2.f, cy = static_cast<float>(f.height) / 2.f;
-    const float sc = static_cast<float>(std::max(f.width, f.height)) * 0.7f;
+    float* kp = g->st_kp + static_cast<size_t>(s) * NP * 2;
+    float* sc = g->st_sc + static_cast<size_t>(s) * NP;
+    float* de = g->st_desc + static_cast<size_t>(s) * d * NP;
     const int ld = f.desc_ld ? f.desc_ld : f.n;
-    float* st_desc = g->hid;  // staging: [256][n] fits the [NP][512] hidden buffer; keypoints / scores behind it
-    float* st_kp = g->att;
-    DIMB_CUDA_OK(ctx, cudaMemcpy2DAsync(st_desc, static_cast<size_t>(n[s]) * sizeof(float), f.descriptors, static_cast<size_t>(ld) * sizeof(float),
+    DIMB_CUDA_OK(ctx, cudaMemcpy2DAsync(de, static_cast<size_t>(NP) * sizeof(float), f.descriptors, static_cast<size_t>(ld) * sizeof(float),
                                         static_cast<size_t>(n[s]) * sizeof(float), d, cudaMemcpyHostToDevice, st));
-    DIMB_CUDA_OK(ctx, cudaMemcpyAsync(st_kp, f.keypoints, static_cast<size_t>(n[s]) * 2 * sizeof(float), cudaMemcpyHostToDevice, st));
-    DIMB_CUDA_OK(ctx, cudaMemcpyAsync(st_kp + 2 * static_cast<size_t>(NP), f.scores, static_cast<size_t>(n[s]) * sizeof(float), cudaMemcpyHostToDevice, st));
-    sg_input_kernel<<<dim3(ceil_div(n[s], 32), d / 32), dim3(32, 8), 0, st>>>(st_desc, n[s], n[s], st_kp, st_kp + 2 * static_cast<size_t>(NP), cx, cy, sc,
-                                                                              g->cat[s], 2 * d, g->enc_a);
-    DIMB_LAUNCH_CHECK(ctx);
-    float *a = g->enc_a, *b = g->enc_b;
-    int lda = 3;
-    for (int i = 0; i < 5; ++i) {
-      if (i < 4) {
-        DIMB_TRY(sg_linear(g, st, a, lda, g->kenc[i], b, g->kenc[i].n, n[s], 1));
-        std::swap(a, b);
-        lda = g->kenc[i].n;
-      } else {  // last layer: no BN / ReLU; desc = desc + kenc(...)
-        DIMB_TRY(sg_linear(g, st, a, lda, g->kenc[i], g->cat[s], 2 * d, n[s], 0, 1.f, g->cat[s], 2 * d));
-      }
-    }
-    // enc_a / enc_b and the staging buffers are reused by the other side: stream order is enough
+    DIMB_CUDA_OK(ctx, cudaMemcpyAsync(kp, f.keypoints, static_cast<size_t>(n[s]) * 2 * sizeof(float), cudaMemcpyHostToDevice, st));
+    DIMB_CUDA_OK(ctx, cudaMemcpyAsync(sc, f.scores, static_cast<size_t>(n[s]) * sizeof(float), cudaMemcpyHostToDevice, st));
+    df[s] = dimb_sg_feats_dev{kp, de, sc, g->st_n + s, n[s], NP, 0, 0, f.height, f.width, nullptr};
+    hin[s] = SgSideIn{kp, de, sc, g->st_n + s, n[s], NP, 0, 0, f.height, f.width, nullptr};
   }
-  const int m = n[0], nn = n[1];
-  const float norm = -std::log(static_cast<float>(m) + static_cast<float>(nn));
-  const float* Zs = g->Z;   // score block of the couplings and its row pitch (tensor path: the similarity buffer, virtual dustbins)
-  int ld = nn + 1;
-  if (ctx->use_tc) {
-    DIMB_TRY(sg_gnn_tc(g, st, n));
-    Zs = g->sim;
-    ld = g->NPt;
-    DIMB_CUDA_OK(ctx, cudaMemsetAsync(g->u, 0, (m + 1) * sizeof(float), st));
-    DIMB_CUDA_OK(ctx, cudaMemsetAsync(g->vv, 0, (nn + 1) * sizeof(float), st));
-    for (int it = 0; it < g->conf.sinkhorn_iterations; ++it) {
-      sg_sink_rows_kernel<<<ceil_div((m + 1) * 32, 256), 256, 0, st>>>(Zs, ld, m, nn, g->bin_score, g->vv, g->u, norm, std::log(static_cast<float>(nn)));
-      DIMB_LAUNCH_CHECK(ctx);
-      // column sweep = row sweep over the transposed block (coalesced, one warp per column)
-      sg_sink_rows_kernel<<<ceil_div((nn + 1) * 32, 256), 256, 0, st>>>(g->simT, ld, nn, m, g->bin_score, g->u, g->vv, norm, std::log(static_cast<float>(m)));
-      DIMB_LAUNCH_CHECK(ctx);
-    }
-  } else {
-  for (int i = 0; i < g->L; ++i) {  // AttentionalGNN (:132-152): deltas of both sides from the OLD descriptors
-    const SgLayer& ly = g->layers[i];
-    for (int s = 0; s < 2; ++s) {
-      const int src = g->cross[i] ? 1 - s : s;
-      DIMB_TRY(sg_linear(g, st, g->cat[s], 2 * d, ly.q, g->q[s], d, n[s], 0));
-      DIMB_TRY(sg_linear(g, st, g->cat[src], 2 * d, ly.k, g->k[s], d, n[src], 0));
-      DIMB_TRY(sg_linear(g, st, g->cat[src], 2 * d, ly.v, g->v[s], d, n[src], 0));
-    }
-    for (int s = 0; s < 2; ++s) {
-      const int src = g->cross[i] ? 1 - s : s;
-      dim3 grid(ceil_div(n[s], 8), kSgHeads);
-      gx_attention_kernel<64><<<grid, 256, 0, st>>>(g->q[s], g->k[s], g->v[s], n[s], n[src], d, kSgHd, g->att, d);
-      DIMB_LAUNCH_CHECK(ctx);
-      DIMB_TRY(sg_linear(g, st, g->att, d, ly.merge, g->cat[s] + d, 2 * d, n[s], 0));  // message -> right half of [x | message]
-    }
-    for (int s = 0; s < 2; ++s) {  // x += mlp([x | message])
-      DIMB_TRY(sg_linear(g, st, g->cat[s], 2 * d, ly.mlp0, g->hid, 2 * d, n[s], 1));
-      DIMB_TRY(sg_linear(g, st, g->hid, 2 * d, ly.mlp3, g->cat[s], 2 * d, n[s], 0, 1.f, g->cat[s], 2 * d));
-    }
-  }
-  for (int s = 0; s < 2; ++s) DIMB_TRY(sg_linear(g, st, g->cat[s], 2 * d, g->final_proj, g->md[s], d, n[s], 0));
-  {  // scores = mdesc0 . mdesc1^T / sqrt(256) into the top-left block of the couplings
-    dim3 grid(ceil_div(nn, 64), ceil_div(m, 64));
-    gx_linear_kernel<<<grid, 256, 0, st>>>(g->md[0], d, g->md[1], d, nullptr, g->Z, ld, m, nn, d, 1.f / 16.f, nullptr, 0, 0);
-    DIMB_LAUNCH_CHECK(ctx);
-  }
-  sg_fill_bins_kernel<<<ceil_div(std::max(m, nn) + 1, 256), 256, 0, st>>>(g->Z, ld, m, nn, g->bin_score);
-  DIMB_LAUNCH_CHECK(ctx);
-  DIMB_CUDA_OK(ctx, cudaMemsetAsync(g->u, 0, (m + 1) * sizeof(float), st));
-  DIMB_CUDA_OK(ctx, cudaMemsetAsync(g->vv, 0, (nn + 1) * sizeof(float), st));
-  for (int it = 0; it < g->conf.sinkhorn_iterations; ++it) {
-    sg_sinkhorn_kernel<<<ceil_div((m + 1) * 32, 256), 256, 0, st>>>(g->Z, ld, m + 1, nn + 1, 0, g->vv, g->u, norm, std::log(static_cast<float>(nn)));
-    DIMB_LAUNCH_CHECK(ctx);
-    sg_sinkhorn_kernel<<<ceil_div((nn + 1) * 32, 256), 256, 0, st>>>(g->Z, ld, m + 1, nn + 1, 1, g->u, g->vv, norm, std::log(static_cast<float>(m)));
-    DIMB_LAUNCH_CHECK(ctx);
-  }
-  }  // plain fp32 twin
-  sg_argmax_kernel<<<ceil_div(m * 32, 256), 256, 0, st>>>(Zs, ld, m, nn, g->u, g->vv, norm, 0, g->best0, g->arg0);
-  DIMB_LAUNCH_CHECK(ctx);
-  sg_argmax_kernel<<<ceil_div(nn * 32, 256), 256, 0, st>>>(Zs, ld, m, nn, g->u, g->vv, norm, 1, g->best1, g->arg1);
-  DIMB_LAUNCH_CHECK(ctx);
-  std::vector<float> b0(m);
-  std::vector<int> a0(m), a1(nn);
-  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(b0.data(), g->best0, m * sizeof(float), cudaMemcpyDeviceToHost, st));
-  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(a0.data(), g->arg0, m * sizeof(int), cudaMemcpyDeviceToHost, st));
-  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(a1.data(), g->arg1, nn * sizeof(int), cudaMemcpyDeviceToHost, st));
-  DIMB_CUDA_OK(ctx, cudaStreamSynchronize(st));
+  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(g->st_n, n, 2 * sizeof(int), cudaMemcpyHostToDevice, st));
+  if (ctx->use_tc)
+    DIMB_TRY(dimb_sg_match_dev(g, 1, &df[0], &df[1], g->o_m, g->o_ms, g->o_nm, cap, st));
+  else
+    DIMB_TRY(sg_match_plain(g, st, hin, n, cap));
   int cnt = 0;
-  for (int r = 0; r < m; ++r) {
-    const int c = a0[r];
-    if (a1[c] != r) continue;  // mutual
-    const float e = std::exp(b0[r]);
-    if (!(e > g->conf.match_threshold)) continue;
-    if (cnt < cap) {
-      matches[2 * cnt] = r;
-      matches[2 * cnt + 1] = c;
-      mscores[cnt] = e;
-    }
-    ++cnt;
-  }
+  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(&cnt, g->o_nm, sizeof(int), cudaMemcpyDeviceToHost, st));
+  DIMB_CUDA_OK(ctx, cudaStreamSynchronize(st));
+  const int rows = std::min(cnt, cap);
+  DIMB_CUDA_OK(ctx, cudaMemcpy(matches, g->o_m, static_cast<size_t>(rows) * 2 * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  DIMB_CUDA_OK(ctx, cudaMemcpy(mscores, g->o_ms, static_cast<size_t>(rows) * sizeof(float), cudaMemcpyDeviceToHost));
   *n_matches = cnt;
   if (cnt > cap) {
     dimb_set_error(ctx, "dimb_sg_match: more matches than cap");

@@ -7,7 +7,8 @@ match_pairs, image_matching.py:413-494, is the serial loop this replaces) run in
      ``store_slot``);
   2. ONE ``all_gather`` of the float16 feature blocks (NCCL over NVLink; ~1.07 MB per SuperPoint image) gives every rank all
      features (``all_gather_blocks``), then the pair list is dealt by longest-processing-time (``shard_pairs``) and each rank
-     matches its pairs out of its own HBM; the variable-length match tables are gathered to rank 0 (``gather_match_tables``)."""
+     matches its pairs (LightGlue or SuperGlue) out of its own HBM; the variable-length match tables are gathered to rank 0
+     (``gather_match_tables``)."""
 from __future__ import annotations
 
 import numpy as np
@@ -96,11 +97,14 @@ def gather_match_tables(local_ids, local_matches, n_pairs: int, dist=None, devic
 
 class ImageSetMatcher:
     """Two-phase multi-GPU matching of an image set (module docstring): SuperPoint on this rank's images into the device feature
-    store, one all_gather of the float16 feature blocks, LightGlue on this rank's share of the pair list, gather of the match
-    tables.  ``dist`` is ``torch.distributed`` (initialised, nccl) or None for a single process."""
+    store, one all_gather of the float16 feature blocks, LightGlue or SuperGlue on this rank's share of the pair list, gather of the
+    match tables.  ``dist`` is ``torch.distributed`` (initialised, nccl) or None for a single process.
+
+    ``matcher="superglue"``: ``lg_weights`` is the SuperGlue state dict and ``lg_conf`` its configuration (``sinkhorn_iterations``,
+    ``match_threshold``, ``gnn_layers``), and phase 2 runs the batched device SuperGlue on the store's slots."""
 
     def __init__(self, ctx, sp_weights: dict, lg_weights: dict, n_images: int, height: int, width: int, sp_conf: dict, lg_conf: dict,
-                 batch_images: int = 16, batch_pairs: int = 32, dist=None):
+                 batch_images: int = 16, batch_pairs: int = 32, dist=None, matcher: str = "lightglue"):
         import torch
 
         from . import _native
@@ -111,7 +115,13 @@ class ImageSetMatcher:
         self.cap = int(sp_conf["max_keypoints"])
         self.B, self.P = batch_images, batch_pairs
         self.sp = _native.SuperPointNet(ctx, sp_weights, max_batch=batch_images, max_height=height, max_width=width, **sp_conf)
-        self.lg = _native.LightGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=self.cap, **lg_conf)
+        if matcher not in ("lightglue", "superglue"):
+            raise ValueError(f'matcher must be "lightglue" or "superglue", got {matcher!r}')
+        self.matcher = matcher
+        if matcher == "superglue":
+            self.sg = _native.SuperGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=self.cap, **lg_conf)
+        else:
+            self.lg = _native.LightGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=self.cap, **lg_conf)
         self.ipr = images_per_rank(n_images, self.world)
         self.store = _native.FeatureStoreDev(ctx, self.world * self.ipr, self.cap, 256)
         dev = torch.device("cuda", ctx.device)
@@ -149,15 +159,20 @@ class ImageSetMatcher:
         self.exchanged_bytes = all_gather_blocks(self.store_t, self.n, self.dist)
 
     def match(self, pairs, pair_ids):
-        """Phase 2: LightGlue on `pairs` = [(i, j), ...] (this rank's share); returns {pair id: int64 (S,2)} after ONE device->host
-        copy per batch.  Features are read in place from the store (float16, no rounding left to do)."""
+        """Phase 2: LightGlue or SuperGlue on `pairs` = [(i, j), ...] (this rank's share); returns {pair id: int64 (S,2)} after ONE
+        device->host copy per batch.  Features are read in place from the store (float16, no rounding left to do)."""
         st = self.torch.cuda.current_stream().cuda_stream
         out = {}
         for b0 in range(0, len(pairs), self.P):
             chunk = pairs[b0:b0 + self.P]
-            f0 = [self.store.feats_dev(store_slot(i, self.n, self.world)) for i, _ in chunk]
-            f1 = [self.store.feats_dev(store_slot(j, self.n, self.world)) for _, j in chunk]
-            self.lg.match_dev(f0, f1, self.m.data_ptr(), self.ms.data_ptr(), self.nm.data_ptr(), self.sl.data_ptr(), self.cap, st)
+            if self.matcher == "superglue":
+                f0 = [self.store.sg_feats_dev(store_slot(i, self.n, self.world)) for i, _ in chunk]
+                f1 = [self.store.sg_feats_dev(store_slot(j, self.n, self.world)) for _, j in chunk]
+                self.sg.match_dev(f0, f1, self.m.data_ptr(), self.ms.data_ptr(), self.nm.data_ptr(), self.cap, st)
+            else:
+                f0 = [self.store.feats_dev(store_slot(i, self.n, self.world)) for i, _ in chunk]
+                f1 = [self.store.feats_dev(store_slot(j, self.n, self.world)) for _, j in chunk]
+                self.lg.match_dev(f0, f1, self.m.data_ptr(), self.ms.data_ptr(), self.nm.data_ptr(), self.sl.data_ptr(), self.cap, st)
             nm = self.nm[:len(chunk)].cpu().numpy()
             m = self.m[:len(chunk)].cpu().numpy()
             for k in range(len(chunk)):

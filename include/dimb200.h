@@ -277,7 +277,8 @@ int dimb_aliked_debug_read(dimb_aliked* al, int which, float* out, size_t n_floa
 /* ---------------------------------------------------------------------------------------------------------
  * SuperGlue matching.  Replaces SuperGlueMatcher._match_pairs (reference src/deep_image_matching/matchers/superglue.py:75-106,
  * adapter features_2_sg :8-41) and the model it drives (thirdparty/SuperGluePretrainedNetwork/models/superglue.py:51-305).
- * descriptor_dim 256, 4 heads, keypoint encoder [32,64,128,256].  First cut on the plain fp32 kernels (csrc/superglue.cu).
+ * descriptor_dim 256, 4 heads, keypoint encoder [32,64,128,256].  The GNN and the score matrix run on the wgmma kernels shared with
+ * LightGlue; the keypoint encoder, Sinkhorn and the mutual-max filter are batched CUDA-core kernels (csrc/superglue.cu).
  *
  * weights: fp32 blob in THIS order (names of the reference state_dict; BatchNorm = weight, bias, running_mean, running_var):
  *   kenc.encoder.{0,3,6,9}.{weight,bias} each followed by its BatchNorm kenc.encoder.{1,4,7,10}; kenc.encoder.12.{weight,bias};
@@ -291,6 +292,7 @@ typedef struct {
   int sinkhorn_iterations;        /* 100 (superglue.py:218; the plugin's own 20 never reaches the model, see matchers/superglue.py) */
   float match_threshold;          /* 0.2 */
   int max_kpts;                   /* workspace sizing */
+  int max_pairs;                  /* workspace sizing: pairs per dimb_sg_match_dev call (0 = 1) */
 } dimb_sg_conf;
 typedef struct {
   const float* keypoints;   /* (n,2) x,y */
@@ -305,6 +307,25 @@ void dimb_sg_destroy(dimb_sg* sg);
 /* One pair.  Out (host): matches [cap][2] int64 ascending in column 0, mscores [cap] (matching_scores0 of the matched rows). */
 int dimb_sg_match(dimb_sg* sg, const dimb_sg_feats* f0, const dimb_sg_feats* f1, int64_t* matches, float* mscores, int* n_matches,
                   int cap);
+/* Device counterpart of dimb_sg_feats: SuperGlue needs the scores, which dimb_feats_dev does not carry. */
+typedef struct {
+  const void* keypoints;    /* device (n_cap,2) x,y */
+  const void* descriptors;  /* device (256,n) rows of pitch desc_ld (0 = n_cap): the FeaturesDict / store layout */
+  const void* scores;       /* device (n_cap,); required (features_2_sg needs scores) */
+  const int* n;             /* device scalar, <= n_cap */
+  int n_cap, desc_ld;
+  int f16;                  /* 1: the three arrays are float16 (feature-store blocks) */
+  int round_fp16;           /* 1: round float32 inputs to fp16 first (the features.h5 round trip) */
+  int height, width;        /* image_size [H,W] */
+  const int* size_dev;      /* non-NULL: device int[2] [H,W], overrides height / width */
+} dimb_sg_feats_dev;
+/* P <= max_pairs pairs on device pointers, asynchronous on `stream` (never synchronises).  Outputs as dimb_lg_match_dev:
+ * d_matches [P][cap][2] int64 ascending in column 0, d_mscores [P][cap], d_n_matches [P] (the full count, also when it exceeds
+ * cap; only the first cap rows are written).  Needs the tensor-core path: DIMB_ERR_UNSUPPORTED with DIMB_TC=0. */
+int dimb_sg_match_dev(dimb_sg* sg, int P, const dimb_sg_feats_dev* f0, const dimb_sg_feats_dev* f1, int64_t* d_matches, float* d_mscores,
+                      int* d_n_matches, int cap, void* stream);
+/* The slot as SuperGlue device input: f16 = 1, scores from the slot's score block, size_dev = the slot header's [H,W]. */
+int dimb_fstore_sg_feats_dev(dimb_fstore* fs, int slot, dimb_sg_feats_dev* out);
 
 #ifdef __cplusplus
 }
