@@ -28,7 +28,7 @@ EXPORTS = [
     "dimb_sg_weight_count", "dimb_sg_create", "dimb_sg_destroy", "dimb_sg_match", "dimb_sg_match_dev", "dimb_fstore_sg_feats_dev",
     "dimb_aliked_create", "dimb_aliked_destroy", "dimb_aliked_extract", "dimb_aliked_extract_dev", "dimb_aliked_debug_read",
     "dimb_fstore_create", "dimb_fstore_destroy", "dimb_fstore_put_dev", "dimb_fstore_put", "dimb_fstore_count", "dimb_fstore_get",
-    "dimb_fstore_feats_dev", "dimb_fstore_block_dev", "dimb_gv_fundamental", "dimb_gv_fundamental_batch_dev",
+    "dimb_fstore_feats_dev", "dimb_fstore_block_dev", "dimb_gv_fundamental", "dimb_gv_fundamental_batch_dev", "dimb_gv_verify_dev",
 ]
 
 
@@ -78,6 +78,10 @@ class FeatsDev(C.Structure):
     _fields_ = [("keypoints", C.c_void_p), ("descriptors", C.c_void_p), ("n", C.c_void_p), ("n_cap", C.c_int),
                 ("desc_layout", C.c_int), ("desc_ld", C.c_int), ("size0", C.c_float), ("size1", C.c_float),
                 ("round_fp16", C.c_int), ("f16", C.c_int), ("size_dev", C.c_void_p)]
+
+
+class GvConf(C.Structure):
+    _fields_ = [("threshold", C.c_float), ("max_iters", C.c_int), ("min_inliers", C.c_int), ("min_inlier_ratio", C.c_float)]
 
 
 _lib = None
@@ -154,6 +158,8 @@ def load_library():
     lib.dimb_fstore_sg_feats_dev.argtypes = [vp, ip, C.POINTER(SgFeatsDev)]
     lib.dimb_gv_fundamental.argtypes = [vp, vp, vp, ip, fp, ip, C.c_uint, vp, vp, C.POINTER(ip)]
     lib.dimb_gv_fundamental_batch_dev.argtypes = [vp, ip, vp, vp, vp, vp, ip, fp, ip, C.c_uint, vp, vp, vp, vp]
+    lib.dimb_gv_verify_dev.argtypes = [vp, ip, C.POINTER(FeatsDev), C.POINTER(FeatsDev), vp, vp, ip, C.POINTER(C.c_uint),
+                                       C.POINTER(GvConf), vp, vp, vp, vp, vp, vp]
     lib.dimb_fstore_block_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(C.c_size_t), C.POINTER(ip), C.POINTER(ip)]
     _lib = lib
     return lib
@@ -297,6 +303,21 @@ class Context:
         self.check(self.lib.dimb_gv_fundamental(self.h, _ptr(k0), _ptr(k1), n, float(threshold), int(max_iters), int(seed) & 0xffffffff, _ptr(F),
                                                 _ptr(mask), C.byref(cnt)), "dimb_gv_fundamental")
         return (F.reshape(3, 3) if np.any(F) else None), mask[:n].astype(bool)
+
+    def gv_verify_dev(self, f0: list, f1: list, d_matches, d_n_matches, cap, seeds, threshold=1.0, max_iters=10000, min_inliers=0,
+                      min_inlier_ratio=0.0, d_verified=0, d_n_verified=0, d_F=0, d_mask=0, d_n_inliers=0, stream=0):
+        """Geometric verification of P match tables on the device (dimb_gv_verify_dev).  f0/f1: lists of FeatsDev (e.g.
+        FeatureStoreDev.feats_dev); d_matches [P][cap][2] int64 / d_n_matches [P] int32 as LightGlueNet.match_dev writes them; seeds:
+        one uint32 per pair (geometric_verification.gv_seed).  Outputs are device buffers (ints are device addresses): d_verified
+        [P][cap][2] int64, d_n_verified [P] int32, d_F [P][9] float32, d_mask [P][cap] uint8, d_n_inliers [P] int32.  Asynchronous
+        on `stream`."""
+        P = len(f0)
+        a0 = (FeatsDev * P)(*f0)
+        a1 = (FeatsDev * P)(*f1)
+        sd = (C.c_uint * P)(*[int(s) & 0xffffffff for s in seeds])
+        conf = GvConf(float(threshold), int(max_iters), int(min_inliers), float(min_inlier_ratio))
+        self.check(self.lib.dimb_gv_verify_dev(self.h, P, a0, a1, d_matches, d_n_matches, cap, sd, C.byref(conf), d_verified, d_n_verified,
+                                               d_F, d_mask, d_n_inliers, stream), "dimb_gv_verify_dev")
 
     def nn_match_dev(self, d_desc0: int, n0: int, d_desc1: int, n1: int, D: int, mode: str, th: float, d_idx: int, d_dist: int,
                      d_n: int, cap: int, f16: bool = False, ld0: int = 0, ld1: int = 0, stream: int = 0):

@@ -8,7 +8,12 @@
 // thread (gv_math.cuh); the best hypothesis is refitted twice by least squares on its inliers (local optimisation) and the final
 // inlier mask is written.  No adaptive stopping: every hypothesis runs in parallel, H = min(max_iters, 8192).
 // RANSAC is stochastic in the reference too (pydegensac's own RNG), so parity is statistical: tests compare inlier sets on data
-// with known geometry and against OpenCV on the same matches.
+// with known geometry and against OpenCV on the same matches.  Every reduction runs in a fixed order (integer atomics only), so a
+// pair's result is a function of its matches, its seed and the configuration alone: bitwise reproducible across calls and batches.
+//
+// dimb_gv_verify_dev adds what an image set needs after matching: keypoints straight from the float16 feature store, a seed per pair
+// (independent of the pair's position in the call), and in the last pass of the finalize kernel the ordered compaction of the inlier
+// rows of the match table plus the per-pair inlier gate.
 #include <memory>
 #include <vector>
 
@@ -18,16 +23,36 @@
 namespace {
 
 struct GvPair {
-  const float *k0, *k1;        // keypoints of image 0 / 1: (N,2) x,y
+  const void *k0, *k1;         // keypoints of image 0 / 1: (N,2) x,y, float32 or float16 (f16)
   const long long* matches;    // [n][2] indices into k0 / k1, or null: k0[i] <-> k1[i]
   const int* n_dev;            // device count (or null: n_host)
   int n_host, cap;
+  unsigned seed;               // RNG stream of this pair
+  int f16[2], round_fp16[2];   // per side: float16 keypoints / round float32 keypoints to fp16 first (the features.h5 round trip)
+};
+
+// Optional outputs of dimb_gv_verify_dev: the inlier rows of each match table in order, and the gated count.
+struct GvCompact {
+  long long* verified;  // [P][cap][2], or null: no compaction (the older entries)
+  int* n_verified;      // [P]
+  int min_inliers;
+  float min_ratio;
 };
 
 __device__ __forceinline__ int gv_count(const GvPair& p) { return min(p.n_dev ? *p.n_dev : p.n_host, p.cap); }
+__device__ __forceinline__ float gv_kpt(const void* k, long long i, int f16, int r16) {
+  if (f16) return __half2float(static_cast<const __half*>(k)[i]);
+  const float v = static_cast<const float*>(k)[i];
+  return r16 ? __half2float(__float2half_rn(v)) : v;
+}
 __device__ __forceinline__ void gv_point(const GvPair& p, int i, float& x0, float& y0, float& x1, float& y1) {
   const long long a = p.matches ? p.matches[2 * i] : i, b = p.matches ? p.matches[2 * i + 1] : i;
-  x0 = p.k0[2 * a], y0 = p.k0[2 * a + 1], x1 = p.k1[2 * b], y1 = p.k1[2 * b + 1];
+  x0 = gv_kpt(p.k0, 2 * a, p.f16[0], p.round_fp16[0]), y0 = gv_kpt(p.k0, 2 * a + 1, p.f16[0], p.round_fp16[0]);
+  x1 = gv_kpt(p.k1, 2 * b, p.f16[1], p.round_fp16[1]), y1 = gv_kpt(p.k1, 2 * b + 1, p.f16[1], p.round_fp16[1]);
+}
+// the gate of dimb_gv_verify_dev (float32 comparison of the ratio, as documented in dimb200.h)
+__device__ __forceinline__ bool gv_gate(int n_inl, int n_raw, const GvCompact& c) {
+  return n_inl >= c.min_inliers && static_cast<float>(n_inl) >= c.min_ratio * static_cast<float>(n_raw);
 }
 
 // one CTA per pair: centroid + mean distance of both point sets -> Hartley normalisations; packed coordinates [cap][4]
@@ -76,14 +101,14 @@ __global__ void gv_prepare_kernel(const GvPair* pairs, float* xy, gv::Norm* norm
 
 // grid (ceil(H / 128), P): one hypothesis per thread; best = max over (inliers << 32 | ~hyp) (ties -> lowest hypothesis index)
 __global__ void gv_hypotheses_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, unsigned long long* best, int cap, int H,
-                                     float thr2, unsigned seed) {
+                                     float thr2) {
   const int pi = blockIdx.y, h = blockIdx.x * blockDim.x + threadIdx.x;
   const GvPair p = pairs[pi];
   const int n = gv_count(p);
   if (n < 8 || h >= H) return;
   const float* pts = xy + static_cast<size_t>(pi) * cap * 4;
   int idx[8];
-  gv::sample8(seed + 0x9E37u * pi, h, n, idx);
+  gv::sample8(p.seed, h, n, idx);
   float k0[16], k1[16];
   int id8[8];
   for (int k = 0; k < 8; ++k) {
@@ -101,22 +126,34 @@ __global__ void gv_hypotheses_kernel(const GvPair* pairs, const float* xy, const
   atomicMax(&best[pi], (static_cast<unsigned long long>(cnt) << 32) | (0xffffffffu - static_cast<unsigned>(h)));
 }
 
-// one CTA per pair: best hypothesis -> two least-squares refits on its inliers -> mask, count, F
-__global__ void __launch_bounds__(256)
-gv_finalize_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, const unsigned long long* best, int cap, float thr2, unsigned seed,
-                   float* Fout, unsigned char* mask, int* n_inl) {
-  const int pi = blockIdx.x, t = threadIdx.x;
+// one CTA per pair: best hypothesis -> two least-squares refits on its inliers -> mask, count, F; with cmp.verified also the inlier
+// rows of the match table in order (ballot + warp prefix + block prefix per 256-row chunk) and the gated count
+constexpr int kFinThreads = 256, kFinWarps = kFinThreads / 32;
+
+__global__ void __launch_bounds__(kFinThreads)
+gv_finalize_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, const unsigned long long* best, int cap, float thr2,
+                   float* Fout, unsigned char* mask, int* n_inl, GvCompact cmp) {
+  const int pi = blockIdx.x, t = threadIdx.x, lane = t & 31, wid = t >> 5;
   const GvPair p = pairs[pi];
   const int n = gv_count(p);
   unsigned char* mk = mask + static_cast<size_t>(pi) * cap;
   float* Fo = Fout + 9 * pi;
+  long long* vo = cmp.verified ? cmp.verified + static_cast<size_t>(pi) * cap * 2 : nullptr;
   __shared__ float F[9];
   __shared__ float Nm[45];
+  __shared__ float part[kFinWarps][45];  // per-warp partials of the normal matrix, summed in warp order (no float atomics)
+  __shared__ int wcnt[kFinWarps];
   __shared__ int ok, cnt;
   if (n < 8 || (best[pi] >> 32) < 8) {  // fewer than 8 matches / no usable model: every match stays (reference :107-111 returns all ones)
-    for (int i = t; i < n; i += blockDim.x) mk[i] = 1;
+    for (int i = t; i < n; i += blockDim.x) {
+      mk[i] = 1;
+      if (vo) vo[2 * i] = p.matches[2 * i], vo[2 * i + 1] = p.matches[2 * i + 1];
+    }
     if (t < 9) Fo[t] = 0.f;
-    if (t == 0) n_inl[pi] = n;
+    if (t == 0) {
+      n_inl[pi] = n;
+      if (vo) cmp.n_verified[pi] = gv_gate(n, n, cmp) ? n : 0;
+    }
     return;
   }
   const gv::Norm n0 = norms[2 * pi], n1 = norms[2 * pi + 1];
@@ -125,7 +162,7 @@ gv_finalize_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, 
     const unsigned h = 0xffffffffu - static_cast<unsigned>(best[pi] & 0xffffffffu);
     int idx[8], id8[8];
     float k0[16], k1[16], f[9];
-    gv::sample8(seed + 0x9E37u * pi, h, n, idx);
+    gv::sample8(p.seed, h, n, idx);
     for (int k = 0; k < 8; ++k) {
       k0[2 * k] = pts[4 * idx[k]], k0[2 * k + 1] = pts[4 * idx[k] + 1], k1[2 * k] = pts[4 * idx[k] + 2], k1[2 * k + 1] = pts[4 * idx[k] + 3];
       id8[k] = k;
@@ -135,7 +172,6 @@ gv_finalize_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, 
   }
   __syncthreads();
   for (int round = 0; round < 2; ++round) {
-    if (t < 45) Nm[t] = 0.f;
     if (t == 0) cnt = 0;
     __syncthreads();
     float acc[45];
@@ -159,10 +195,17 @@ gv_finalize_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, 
     for (int k = 0; k < 45; ++k) {
       float v = acc[k];
       for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-      if ((t & 31) == 0) atomicAdd(&Nm[k], v);
+      if (lane == 0) part[wid][k] = v;
     }
     for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-    if ((t & 31) == 0) atomicAdd(&cnt, c);
+    if (lane == 0) atomicAdd(&cnt, c);
+    __syncthreads();
+    if (t < 45) {
+      float a = 0.f;
+#pragma unroll
+      for (int w = 0; w < kFinWarps; ++w) a += part[w][t];
+      Nm[t] = a;
+    }
     __syncthreads();
     if (t == 0) {
       ok = 0;
@@ -194,41 +237,49 @@ gv_finalize_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, 
       __syncthreads();
     }
   }
-  if (t == 0) cnt = 0;
-  __syncthreads();
-  int c = 0;
-  for (int i = t; i < n; i += blockDim.x) {
-    const unsigned char in = gv::sampson2(F, pts[4 * i], pts[4 * i + 1], pts[4 * i + 2], pts[4 * i + 3]) < thr2;
-    mk[i] = in;
-    c += in;
+  // last pass, in chunks of kFinThreads rows: mask; prefix of the inlier flags -> output row of each inlier (order kept)
+  int total = 0;
+  for (int base = 0; base < n; base += kFinThreads) {
+    const int i = base + t;
+    const bool in = i < n && gv::sampson2(F, pts[4 * i], pts[4 * i + 1], pts[4 * i + 2], pts[4 * i + 3]) < thr2;
+    if (i < n) mk[i] = in;
+    const unsigned bal = __ballot_sync(0xffffffffu, in);
+    if (lane == 0) wcnt[wid] = __popc(bal);
+    __syncthreads();
+    int off = total + __popc(bal & ((1u << lane) - 1u));
+    for (int w = 0; w < wid; ++w) off += wcnt[w];
+    if (in && vo) vo[2 * off] = p.matches[2 * i], vo[2 * off + 1] = p.matches[2 * i + 1];
+    for (int w = 0; w < kFinWarps; ++w) total += wcnt[w];
+    __syncthreads();  // wcnt is rewritten by the next chunk
   }
-  for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if ((t & 31) == 0) atomicAdd(&cnt, c);
-  __syncthreads();
   if (t < 9) Fo[t] = F[t];
-  if (t == 0) n_inl[pi] = cnt;
+  if (t == 0) {
+    n_inl[pi] = total;
+    if (vo) cmp.n_verified[pi] = gv_gate(total, n, cmp) ? total : 0;
+  }
 }
 
-int gv_run(dimb_ctx* ctx, cudaStream_t st, const std::vector<GvPair>& hp, int cap, float threshold, int max_iters, unsigned seed, float* d_F,
-           unsigned char* d_mask, int* d_ninl) {
+// slot0 .. slot0 + 3: the context scratch slots of the calling entry (40 for the float32 entries, 48 for dimb_gv_verify_dev)
+int gv_run(dimb_ctx* ctx, cudaStream_t st, const std::vector<GvPair>& hp, int cap, float threshold, int max_iters, float* d_F,
+           unsigned char* d_mask, int* d_ninl, const GvCompact& cmp, int slot0) {
   const int P = static_cast<int>(hp.size());
   GvPair* d_pairs;
   float* d_xy;
   gv::Norm* d_norm;
   unsigned long long* d_best;
-  DIMB_TRY(dimb_scratch(ctx, 40, P * sizeof(GvPair), reinterpret_cast<void**>(&d_pairs)));
-  DIMB_TRY(dimb_scratch(ctx, 41, static_cast<size_t>(P) * cap * 4 * sizeof(float), reinterpret_cast<void**>(&d_xy)));
-  DIMB_TRY(dimb_scratch(ctx, 42, 2 * P * sizeof(gv::Norm), reinterpret_cast<void**>(&d_norm)));
-  DIMB_TRY(dimb_scratch(ctx, 43, P * sizeof(unsigned long long), reinterpret_cast<void**>(&d_best)));
+  DIMB_TRY(dimb_scratch(ctx, slot0, P * sizeof(GvPair), reinterpret_cast<void**>(&d_pairs)));
+  DIMB_TRY(dimb_scratch(ctx, slot0 + 1, static_cast<size_t>(P) * cap * 4 * sizeof(float), reinterpret_cast<void**>(&d_xy)));
+  DIMB_TRY(dimb_scratch(ctx, slot0 + 2, 2 * P * sizeof(gv::Norm), reinterpret_cast<void**>(&d_norm)));
+  DIMB_TRY(dimb_scratch(ctx, slot0 + 3, P * sizeof(unsigned long long), reinterpret_cast<void**>(&d_best)));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_pairs, hp.data(), P * sizeof(GvPair), cudaMemcpyHostToDevice, st));
   const int H = std::max(64, std::min(max_iters, 8192));
   const float thr2 = threshold * threshold;
   ProfScope prof(ctx, st, "gv.ransac");
   gv_prepare_kernel<<<P, 256, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap);
   DIMB_LAUNCH_CHECK(ctx);
-  gv_hypotheses_kernel<<<dim3(ceil_div(H, 128), P), 128, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap, H, thr2, seed);
+  gv_hypotheses_kernel<<<dim3(ceil_div(H, 128), P), 128, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap, H, thr2);
   DIMB_LAUNCH_CHECK(ctx);
-  gv_finalize_kernel<<<P, 256, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap, thr2, seed, d_F, d_mask, d_ninl);
+  gv_finalize_kernel<<<P, kFinThreads, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap, thr2, d_F, d_mask, d_ninl, cmp);
   DIMB_LAUNCH_CHECK(ctx);
   return DIMB_OK;
 }
@@ -260,8 +311,8 @@ int dimb_gv_fundamental(dimb_ctx* ctx, const float* kpts0, const float* kpts1, i
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_k0, kpts0, static_cast<size_t>(n) * 2 * sizeof(float), cudaMemcpyHostToDevice, st));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_k1, kpts1, static_cast<size_t>(n) * 2 * sizeof(float), cudaMemcpyHostToDevice, st));
   std::vector<GvPair> hp(1);
-  hp[0] = GvPair{d_k0, d_k1, nullptr, nullptr, n, n};
-  DIMB_TRY(gv_run(ctx, st, hp, n, threshold, max_iters, seed, d_F, d_mask, d_n));
+  hp[0] = GvPair{d_k0, d_k1, nullptr, nullptr, n, n, seed, {0, 0}, {0, 0}};
+  DIMB_TRY(gv_run(ctx, st, hp, n, threshold, max_iters, d_F, d_mask, d_n, GvCompact{}, 40));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(F, d_F, 9 * sizeof(float), cudaMemcpyDeviceToHost, st));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(n_inliers, d_n, sizeof(int), cudaMemcpyDeviceToHost, st));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(mask, d_mask, n, cudaMemcpyDeviceToHost, st));
@@ -280,8 +331,31 @@ int dimb_gv_fundamental_batch_dev(dimb_ctx* ctx, int P, const float* const* d_kp
   DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
   std::vector<GvPair> hp(P);
   for (int p = 0; p < P; ++p)
-    hp[p] = GvPair{d_kpts0[p], d_kpts1[p], reinterpret_cast<const long long*>(d_matches) + static_cast<size_t>(p) * cap * 2, d_n_matches + p, 0, cap};
-  return gv_run(ctx, static_cast<cudaStream_t>(stream), hp, cap, threshold, max_iters, seed, d_F, d_mask, d_n_inliers);
+    hp[p] = GvPair{d_kpts0[p], d_kpts1[p], reinterpret_cast<const long long*>(d_matches) + static_cast<size_t>(p) * cap * 2, d_n_matches + p, 0, cap,
+                   seed + 0x9E37u * static_cast<unsigned>(p), {0, 0}, {0, 0}};
+  return gv_run(ctx, static_cast<cudaStream_t>(stream), hp, cap, threshold, max_iters, d_F, d_mask, d_n_inliers, GvCompact{}, 40);
+}
+
+// P pairs of an image set, asynchronous on `stream`: keypoints from dimb_feats_dev (feature-store slots or float32 extractor
+// outputs), one seed per pair, the inlier rows of each match table compacted in order and gated (contract in dimb200.h).
+int dimb_gv_verify_dev(dimb_ctx* ctx, int P, const dimb_feats_dev* f0, const dimb_feats_dev* f1, const int64_t* d_matches,
+                       const int* d_n_matches, int cap, const unsigned* seeds, const dimb_gv_conf* conf, int64_t* d_verified,
+                       int* d_n_verified, float* d_F, unsigned char* d_mask, int* d_n_inliers, void* stream) {
+  if (!ctx || P < 1 || !f0 || !f1 || !d_matches || !d_n_matches || cap < 1 || !seeds || !conf || !d_verified || !d_n_verified || !d_F ||
+      !d_mask || !d_n_inliers)
+    return DIMB_ERR_ARG;
+  if (!(conf->threshold > 0.f) || conf->min_inliers < 0 || !(conf->min_inlier_ratio >= 0.f && conf->min_inlier_ratio <= 1.f))
+    return DIMB_ERR_ARG;
+  for (int p = 0; p < P; ++p)
+    if (!f0[p].keypoints || !f1[p].keypoints) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  std::vector<GvPair> hp(P);
+  for (int p = 0; p < P; ++p)
+    hp[p] = GvPair{f0[p].keypoints, f1[p].keypoints, reinterpret_cast<const long long*>(d_matches) + static_cast<size_t>(p) * cap * 2,
+                   d_n_matches + p, 0, cap, seeds[p], {f0[p].f16 ? 1 : 0, f1[p].f16 ? 1 : 0},
+                   {f0[p].round_fp16 ? 1 : 0, f1[p].round_fp16 ? 1 : 0}};
+  const GvCompact cmp{reinterpret_cast<long long*>(d_verified), d_n_verified, conf->min_inliers, conf->min_inlier_ratio};
+  return gv_run(ctx, static_cast<cudaStream_t>(stream), hp, cap, conf->threshold, conf->max_iters, d_F, d_mask, d_n_inliers, cmp, 48);
 }
 
 }  // extern "C"

@@ -7,6 +7,8 @@ method name of the reference (PYDEGENSAC, MAGSAC, RANSAC, the OpenCV USAC family
 RANSAC with Sampson inliers and two least-squares refits (csrc/gv.cu), all hypotheses evaluated in parallel.  ``confidence`` is
 accepted and unused (there is no adaptive stopping: min(max_iters, 8192) hypotheses always run).  Like the reference's
 estimators the result is stochastic in the sense that it depends on the seed; parity is statistical (tests/test_geometry.py).
+For image sets, ``gv_seed(seed, pair_id)`` is the seed of each pair, so that a pair's result does not depend on how the pair list is
+batched or sharded (``sharded.ImageSetMatcher(verification=...)``).
 """
 from __future__ import annotations
 
@@ -16,15 +18,37 @@ METHODS = ("NONE", "PYDEGENSAC", "MAGSAC", "RANSAC", "LMEDS", "RHO", "USAC_DEFAU
            "USAC_ACCURATE", "USAC_PROSAC", "USAC_MAGSAC")
 
 
-def geometric_verification(kpts0: np.ndarray = None, kpts1: np.ndarray = None, method="pydegensac", threshold: float = 1, confidence: float = 0.9999,
-                           max_iters: int = 10000, quiet: bool = False, device: int = 0, seed: int = 0, **kwargs):
-    from . import _native
+def method_name(method) -> str:
+    """Upper-case name in METHODS of a method given as name, enum member or index; ValueError otherwise."""
     name = getattr(method, "name", method)
     if isinstance(name, int):
         name = METHODS[name] if 0 <= name < len(METHODS) else None
     if not isinstance(name, str) or name.upper() not in METHODS:
         raise ValueError(f"Invalid Geometry Verification method. It must be one of {list(METHODS)}")
+    return name.upper()
+
+
+def gv_seed(seed: int, pair_id: int) -> int:
+    """RNG seed (uint32) of pair `pair_id` of a pair list verified with base seed `seed`.
+
+    A pure function of the two integers (both taken modulo 2**32): a pair's verification result depends on its global id in the
+    pair list, never on the batch it was verified in or the rank that verified it.  The mix is the 32-bit "lowbias32" finaliser of
+    ``seed * 0x9E3779B1 + (pair_id + 1) * 0x85EBCA77`` (mod 2**32)."""
+    m = 0xFFFFFFFF
+    h = ((int(seed) & m) * 0x9E3779B1 + (((int(pair_id) & m) + 1) & m) * 0x85EBCA77) & m
+    h ^= h >> 16
+    h = (h * 0x7FEB352D) & m
+    h ^= h >> 15
+    h = (h * 0x846CA68B) & m
+    h ^= h >> 16
+    return h
+
+
+def geometric_verification(kpts0: np.ndarray = None, kpts1: np.ndarray = None, method="pydegensac", threshold: float = 1, confidence: float = 0.9999,
+                           max_iters: int = 10000, quiet: bool = False, device: int = 0, seed: int = 0, **kwargs):
+    from . import _native
+    name = method_name(method)
     n = len(kpts0)
-    if name.upper() == "NONE" or n < 8:
+    if name == "NONE" or n < 8:
         return None, np.ones(n, dtype=bool)
     return _native.Context.get(device).gv_fundamental(kpts0, kpts1, threshold, max_iters, seed)

@@ -8,7 +8,10 @@ match_pairs, image_matching.py:413-494, is the serial loop this replaces) run in
   2. ONE ``all_gather`` of the float16 feature blocks (NCCL over NVLink; ~1.07 MB per SuperPoint image) gives every rank all
      features (``all_gather_blocks``), then the pair list is dealt by longest-processing-time (``shard_pairs``) and each rank
      matches its pairs (LightGlue or SuperGlue) out of its own HBM; the variable-length match tables are gathered to rank 0
-     (``gather_match_tables``)."""
+     (``gather_match_tables``).
+With ``verification`` the matcher's tables of each pair batch go straight into the device geometric verification (fundamental-matrix
+RANSAC, ordered inlier compaction and the per-pair gate, one launch group per batch); raw tables, verified tables and F are gathered
+to rank 0 (``gather_verified``), and ``export_verified_to_colmap`` writes the COLMAP database from the store and those results."""
 from __future__ import annotations
 
 import numpy as np
@@ -95,16 +98,130 @@ def gather_match_tables(local_ids, local_matches, n_pairs: int, dist=None, devic
     return out
 
 
+def _gather_rows(local_ids, rows, n_pairs: int, dist, device):
+    """Gather {pair id -> float64 row of fixed width} to rank 0 (None elsewhere); pairs nobody sent stay None."""
+    import torch
+
+    world, rank = dist.get_world_size(), dist.get_rank()
+    width = rows.shape[1]
+    k = torch.tensor([len(local_ids)], dtype=torch.int64, device=device)
+    ks = [torch.zeros_like(k) for _ in range(world)]
+    dist.all_gather(ks, k)
+    kmax = max(1, int(max(int(c) for c in ks)))
+    buf = torch.zeros((kmax, 1 + width), dtype=torch.float64, device=device)
+    if len(local_ids):
+        buf[:len(local_ids), 0] = torch.as_tensor(np.asarray(local_ids, np.float64), device=device)
+        buf[:len(local_ids), 1:] = torch.as_tensor(np.asarray(rows, np.float64), device=device)
+    bufs = [torch.zeros_like(buf) for _ in range(world)]
+    dist.all_gather(bufs, buf)
+    if rank != 0:
+        return None
+    out = [None] * n_pairs
+    for r in range(world):
+        b = bufs[r].cpu().numpy()
+        for j in range(int(ks[r])):
+            out[int(b[j, 0])] = b[j, 1:].copy()
+    return out
+
+
+def gather_verified(local_ids, local_results, n_pairs: int, dist=None, device=None):
+    """Gather {pair id -> (raw (S,2), verified (V,2), F (3,3) float32 or None, n_inliers)} from all ranks to rank 0: the two tables
+    through ``gather_match_tables``, F and the count as one fixed-width float64 row per pair (exact for float32 and int32).
+    Returns the full list of 4-tuples on rank 0 (None elsewhere)."""
+    raw = gather_match_tables(local_ids, [r[0] for r in local_results], n_pairs, dist, device)
+    ver = gather_match_tables(local_ids, [r[1] for r in local_results], n_pairs, dist, device)
+    rows = np.zeros((len(local_ids), 11), np.float64)  # has_F, n_inliers, F row-major
+    for k, r in enumerate(local_results):
+        rows[k, 1] = r[3]
+        if r[2] is not None:
+            rows[k, 0] = 1.0
+            rows[k, 2:] = np.asarray(r[2], np.float32).ravel()
+    if dist is None or not dist.is_initialized() or dist.get_world_size() == 1:
+        full = [None] * n_pairs
+        for i, row in zip(local_ids, rows):
+            full[i] = row
+    else:
+        import torch
+        full = _gather_rows(local_ids, rows, n_pairs, dist, device if device is not None else torch.device("cpu"))
+        if full is None:
+            return None
+    out = [None] * n_pairs
+    for i in range(n_pairs):
+        if full[i] is not None:
+            F = full[i][2:].astype(np.float32).reshape(3, 3) if full[i][0] else None
+            out[i] = (raw[i], ver[i], F, int(full[i][1]))
+    return out
+
+
+def export_verified_to_colmap(store, n_images: int, world: int, pairs, results, database_path, image_names=None, **kwargs) -> dict:
+    """Write the COLMAP database of a verified image set through ``io_colmap.export_to_colmap`` (call on rank 0).
+
+    store: the device feature store (``FeatureStoreDev``; features read with ``get`` from slot ``store_slot(i, n_images, world)``,
+    in image order); pairs: [(i, j), ...]; results: per pair ``(raw, verified, F, n_inliers)`` as ``run_verified`` returns them.
+    Raw tables go to ``matches``; non-empty verified tables go to ``two_view_geometries`` with their F; pairs the gate rejected
+    (empty verified table) are left out of it.  Image i gets database id i + 1, and each pair is handed over oriented from the lower
+    to the higher id (columns swapped and F transposed for a pair (i, j) with i > j), so the stored F satisfies x_high^T F x_low = 0.
+    image_names: database names of the images (default ``image_{i}``); kwargs go to ``export_to_colmap``.  Returns {name: image_id}."""
+    from .io_colmap import export_to_colmap
+
+    names = list(image_names) if image_names is not None else [f"image_{i}" for i in range(n_images)]
+    if len(names) != n_images or len(set(names)) != n_images:
+        raise ValueError(f"image_names must hold {n_images} distinct names")
+    features = {names[i]: store.get(store_slot(i, n_images, world)) for i in range(n_images)}
+    raw_tables, verified, fundamental = {}, {}, {}
+    for (i, j), (raw, ver, F, _) in zip(pairs, results):
+        raw = np.asarray(raw, np.int64).reshape(-1, 2)
+        ver = np.asarray(ver, np.int64).reshape(-1, 2)
+        if i > j:  # orient low id -> high id: export_to_colmap would swap the columns but not transpose F
+            i, j, raw, ver = j, i, raw[:, ::-1], ver[:, ::-1]
+            F = None if F is None else np.asarray(F).T
+        key = (names[i], names[j])
+        raw_tables[key] = raw
+        if len(ver):
+            verified[key] = ver
+            if F is not None:
+                fundamental[key] = np.asarray(F, np.float64)
+    return export_to_colmap(features, verified, database_path, raw_matches=raw_tables, fundamental=fundamental, **kwargs)
+
+
+def verification_conf(verification) -> dict | None:
+    """The ``verification`` argument of ImageSetMatcher with its defaults filled in (None stays None).  Defaults: method
+    "pydegensac", threshold 1.0, max_iters 10000, seed 0 (those of geometric_verification), min_inliers_per_pair 15 and
+    min_inlier_ratio_per_pair 0.2 (MatcherBase's general defaults).  ``confidence`` is accepted and unused, as in
+    geometric_verification."""
+    if verification is None:
+        return None
+    from .geometric_verification import method_name
+    conf = {"method": "pydegensac", "threshold": 1.0, "max_iters": 10000, "seed": 0, "min_inliers_per_pair": 15,
+            "min_inlier_ratio_per_pair": 0.2, "confidence": 0.9999}
+    unknown = set(verification) - set(conf)
+    if unknown:
+        raise ValueError(f"unknown verification option(s) {sorted(unknown)}; expected some of {sorted(conf)}")
+    conf.update(verification)
+    conf["method"] = method_name(conf["method"])
+    if not float(conf["threshold"]) > 0 or int(conf["min_inliers_per_pair"]) < 0 or not 0 <= float(conf["min_inlier_ratio_per_pair"]) <= 1:
+        raise ValueError("verification needs threshold > 0, min_inliers_per_pair >= 0 and 0 <= min_inlier_ratio_per_pair <= 1")
+    return conf
+
+
 class ImageSetMatcher:
     """Two-phase multi-GPU matching of an image set (module docstring): SuperPoint on this rank's images into the device feature
     store, one all_gather of the float16 feature blocks, LightGlue or SuperGlue on this rank's share of the pair list, gather of the
     match tables.  ``dist`` is ``torch.distributed`` (initialised, nccl) or None for a single process.
 
     ``matcher="superglue"``: ``lg_weights`` is the SuperGlue state dict and ``lg_conf`` its configuration (``sinkhorn_iterations``,
-    ``match_threshold``, ``gnn_layers``), and phase 2 runs the batched device SuperGlue on the store's slots."""
+    ``match_threshold``, ``gnn_layers``), and phase 2 runs the batched device SuperGlue on the store's slots.
+
+    ``verification``: None (default) matches only (``run`` / ``match``).  A dict (keys and defaults in ``verification_conf``) enables
+    ``run_verified`` / ``match_verified``: every pair batch is verified on the device right after matching (dimb_gv_verify_dev on the
+    store's float16 keypoints, seed ``gv_seed(seed, pair id)``).  The gate: a pair keeps its verified table iff
+    ``n_inliers >= min_inliers_per_pair`` and ``float32(n_inliers) >= float32(min_inlier_ratio_per_pair) * float32(n_raw)``; a
+    rejected pair gets an empty verified table (its F and count are still reported).  Pairs with fewer than 8 raw matches keep
+    every match and have no F (as the reference's geometric_verification returns), then face the same gate.  Method "NONE":
+    verified = raw, F = None, nothing is launched."""
 
     def __init__(self, ctx, sp_weights: dict, lg_weights: dict, n_images: int, height: int, width: int, sp_conf: dict, lg_conf: dict,
-                 batch_images: int = 16, batch_pairs: int = 32, dist=None, matcher: str = "lightglue"):
+                 batch_images: int = 16, batch_pairs: int = 32, dist=None, matcher: str = "lightglue", verification: dict | None = None):
         import torch
 
         from . import _native
@@ -134,6 +251,15 @@ class ImageSetMatcher:
         self.ms = torch.zeros(batch_pairs, self.cap, device=dev)
         self.nm = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
         self.sl = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
+        self.gv = verification_conf(verification)
+        if self.gv is not None and self.gv["method"] != "NONE":  # verification outputs of one pair batch + pinned host copies
+            self.v = torch.zeros(batch_pairs, self.cap, 2, dtype=torch.int64, device=dev)
+            self.nv = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
+            self.F = torch.zeros(batch_pairs, 9, device=dev)
+            self.mask = torch.zeros(batch_pairs, self.cap, dtype=torch.uint8, device=dev)
+            self.ninl = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
+            self.host_out = {k: torch.zeros_like(t, device="cpu").pin_memory() for k, t in
+                      (("m", self.m), ("nm", self.nm), ("v", self.v), ("nv", self.nv), ("F", self.F), ("ninl", self.ninl))}
 
         class _DevArr:  # zero-copy torch view of the store's device allocation (for the NCCL all_gather)
             def __init__(self, ptr, shape):
@@ -158,6 +284,17 @@ class ImageSetMatcher:
         """The collective of the path: every rank's float16 feature blocks to every rank (NCCL all_gather over NVLink)."""
         self.exchanged_bytes = all_gather_blocks(self.store_t, self.n, self.dist)
 
+    def _match_batch(self, chunk, st):
+        """Enqueue the matcher on one pair batch (outputs in self.m / self.ms / self.nm)."""
+        if self.matcher == "superglue":
+            f0 = [self.store.sg_feats_dev(store_slot(i, self.n, self.world)) for i, _ in chunk]
+            f1 = [self.store.sg_feats_dev(store_slot(j, self.n, self.world)) for _, j in chunk]
+            self.sg.match_dev(f0, f1, self.m.data_ptr(), self.ms.data_ptr(), self.nm.data_ptr(), self.cap, st)
+        else:
+            f0 = [self.store.feats_dev(store_slot(i, self.n, self.world)) for i, _ in chunk]
+            f1 = [self.store.feats_dev(store_slot(j, self.n, self.world)) for _, j in chunk]
+            self.lg.match_dev(f0, f1, self.m.data_ptr(), self.ms.data_ptr(), self.nm.data_ptr(), self.sl.data_ptr(), self.cap, st)
+
     def match(self, pairs, pair_ids):
         """Phase 2: LightGlue or SuperGlue on `pairs` = [(i, j), ...] (this rank's share); returns {pair id: int64 (S,2)} after ONE
         device->host copy per batch.  Features are read in place from the store (float16, no rounding left to do)."""
@@ -165,18 +302,44 @@ class ImageSetMatcher:
         out = {}
         for b0 in range(0, len(pairs), self.P):
             chunk = pairs[b0:b0 + self.P]
-            if self.matcher == "superglue":
-                f0 = [self.store.sg_feats_dev(store_slot(i, self.n, self.world)) for i, _ in chunk]
-                f1 = [self.store.sg_feats_dev(store_slot(j, self.n, self.world)) for _, j in chunk]
-                self.sg.match_dev(f0, f1, self.m.data_ptr(), self.ms.data_ptr(), self.nm.data_ptr(), self.cap, st)
-            else:
-                f0 = [self.store.feats_dev(store_slot(i, self.n, self.world)) for i, _ in chunk]
-                f1 = [self.store.feats_dev(store_slot(j, self.n, self.world)) for _, j in chunk]
-                self.lg.match_dev(f0, f1, self.m.data_ptr(), self.ms.data_ptr(), self.nm.data_ptr(), self.sl.data_ptr(), self.cap, st)
+            self._match_batch(chunk, st)
             nm = self.nm[:len(chunk)].cpu().numpy()
             m = self.m[:len(chunk)].cpu().numpy()
             for k in range(len(chunk)):
                 out[pair_ids[b0 + k]] = m[k, :nm[k]].copy()
+        return out
+
+    def match_verified(self, pairs, pair_ids):
+        """Phase 2 with geometric verification: returns {pair id: (raw int64 (S,2), verified int64 (V,2), F (3,3) float32 or None,
+        n_inliers)}.  Per batch the matcher and dimb_gv_verify_dev are enqueued on the same stream and the results come back with
+        ONE synchronise."""
+        from .geometric_verification import gv_seed
+        if self.gv is None:
+            raise RuntimeError("ImageSetMatcher was built without verification")
+        if self.gv["method"] == "NONE":  # the reference skips the estimator: verified = raw, no F
+            return {k: (m, m.copy(), None, len(m)) for k, m in self.match(pairs, pair_ids).items()}
+        torch, st = self.torch, self.torch.cuda.current_stream()
+        g, h = self.gv, self.host_out
+        out = {}
+        for b0 in range(0, len(pairs), self.P):
+            chunk, ids = pairs[b0:b0 + self.P], pair_ids[b0:b0 + self.P]
+            self._match_batch(chunk, st.cuda_stream)
+            f0 = [self.store.feats_dev(store_slot(i, self.n, self.world)) for i, _ in chunk]
+            f1 = [self.store.feats_dev(store_slot(j, self.n, self.world)) for _, j in chunk]
+            self.ctx.gv_verify_dev(f0, f1, self.m.data_ptr(), self.nm.data_ptr(), self.cap, [gv_seed(g["seed"], k) for k in ids],
+                                   g["threshold"], g["max_iters"], g["min_inliers_per_pair"], g["min_inlier_ratio_per_pair"],
+                                   self.v.data_ptr(), self.nv.data_ptr(), self.F.data_ptr(), self.mask.data_ptr(), self.ninl.data_ptr(),
+                                   st.cuda_stream)
+            P = len(chunk)
+            for k in ("nm", "nv", "F", "ninl", "m", "v"):
+                h[k][:P].copy_(getattr(self, k)[:P], non_blocking=True)
+            st.synchronize()
+            nm, nv, F, ninl = h["nm"][:P].numpy(), h["nv"][:P].numpy(), h["F"][:P].numpy(), h["ninl"][:P].numpy()
+            m, v = h["m"].numpy(), h["v"].numpy()
+            for k in range(P):
+                n = min(int(nm[k]), self.cap)
+                out[ids[k]] = (m[k, :n].copy(), v[k, :int(nv[k])].copy(), F[k].reshape(3, 3).copy() if np.any(F[k]) else None,
+                               int(ninl[k]))
         return out
 
     def run(self, d_images, my_image_ids, pairs, costs=None):
@@ -187,3 +350,17 @@ class ImageSetMatcher:
         res = self.match([pairs[k] for k in mine], mine)
         return gather_match_tables(mine, [res[k] for k in mine], len(pairs), self.dist if self.world > 1 else None,
                                    self.torch.device("cuda", self.ctx.device) if self.world > 1 else None)
+
+    def run_verified(self, d_images, my_image_ids, pairs, costs=None):
+        """extract -> exchange -> match and verify my share -> gather to rank 0.  Returns, on rank 0, the list of
+        (raw, verified, F, n_inliers) per pair (None elsewhere); ``export_colmap`` turns it into a COLMAP database."""
+        self.extract(d_images, my_image_ids)
+        self.exchange()
+        mine = shard_pairs(len(pairs), self.world, self.rank, costs)
+        res = self.match_verified([pairs[k] for k in mine], mine)
+        return gather_verified(mine, [res[k] for k in mine], len(pairs), self.dist if self.world > 1 else None,
+                               self.torch.device("cuda", self.ctx.device) if self.world > 1 else None)
+
+    def export_colmap(self, pairs, results, database_path, image_names=None, **kwargs) -> dict:
+        """Rank 0: the COLMAP database of this image set (``export_verified_to_colmap`` on this matcher's feature store)."""
+        return export_verified_to_colmap(self.store, self.n, self.world, pairs, results, database_path, image_names, **kwargs)

@@ -218,6 +218,26 @@ int dimb_gv_fundamental(dimb_ctx* ctx, const float* kpts0, const float* kpts1, i
 int dimb_gv_fundamental_batch_dev(dimb_ctx* ctx, int P, const float* const* d_kpts0, const float* const* d_kpts1, const int64_t* d_matches,
                                   const int* d_n_matches, int cap, float threshold, int max_iters, unsigned seed, float* d_F,
                                   unsigned char* d_mask, int* d_n_inliers, void* stream);
+/* Verification of an image set's match tables (the step between _match_pairs and the COLMAP database).  Every GV entry is bitwise
+ * reproducible: a pair's mask, F and count depend on its matches, its seed and the configuration only. */
+typedef struct {
+  float threshold;          /* Sampson distance threshold in pixels, > 0 */
+  int max_iters;            /* hypotheses per pair = max(64, min(max_iters, 8192)) */
+  int min_inliers;          /* gate: a pair keeps its verified table iff n_inliers >= min_inliers ... */
+  float min_inlier_ratio;   /* ... and float(n_inliers) >= min_inlier_ratio * float(n_raw), in [0, 1] (0 / 0: every pair kept) */
+} dimb_gv_conf;
+/* P pairs, asynchronous on `stream`, never synchronises (once its scratch has grown to the call's size).  Keypoints come from
+ * f0[p] / f1[p], of which only keypoints, f16 and round_fp16 are read: feature-store slots or float32 extractor outputs.
+ * d_matches [P][cap][2] int64 + d_n_matches [P] in the layout of dimb_lg_match_dev / dimb_sg_match_dev (n_raw = min(d_n_matches[p],
+ * cap)).  seeds: HOST array [P], the RNG seed of each pair (independent of the pair's position in the call).  Outputs (device):
+ * d_verified [P][cap][2] int64 = the rows of d_matches whose mask is 1, in their original order; d_n_verified [P] = n_inliers, or 0
+ * when the gate rejects the pair; d_F [P][9] (x1^T F x0 = 0, zeros when no model); d_mask [P][cap]; d_n_inliers [P].  Pairs with
+ * fewer than 8 raw matches (or no model): mask all ones, F zeros, n_inliers = n_raw, then the gate.  DIMB_ERR_ARG, before any CUDA
+ * call, for a NULL ctx / f0 / f1 / seeds / conf / buffer / keypoint pointer, P < 1, cap < 1, threshold <= 0, min_inliers < 0 or
+ * min_inlier_ratio outside [0, 1].  CUDA-core kernels: runs with DIMB_TC=0 as well. */
+int dimb_gv_verify_dev(dimb_ctx* ctx, int P, const dimb_feats_dev* f0, const dimb_feats_dev* f1, const int64_t* d_matches,
+                       const int* d_n_matches, int cap, const unsigned* seeds, const dimb_gv_conf* conf, int64_t* d_verified,
+                       int* d_n_verified, float* d_F, unsigned char* d_mask, int* d_n_inliers, void* stream);
 
 /* ------------------------------------------------------------------ fused per-pair path
  * SuperPoint on both images of every pair followed by LightGlue, features kept in HBM in between (the
