@@ -29,6 +29,7 @@ EXPORTS = [
     "dimb_aliked_create", "dimb_aliked_destroy", "dimb_aliked_extract", "dimb_aliked_extract_dev", "dimb_aliked_debug_read",
     "dimb_fstore_create", "dimb_fstore_destroy", "dimb_fstore_put_dev", "dimb_fstore_put", "dimb_fstore_count", "dimb_fstore_get",
     "dimb_fstore_feats_dev", "dimb_fstore_block_dev", "dimb_gv_fundamental", "dimb_gv_fundamental_batch_dev", "dimb_gv_verify_dev",
+    "dimb_tile_grid", "dimb_tile_cut_dev", "dimb_tile_merge_dev", "dimb_tile_views_dev", "dimb_tile_match_merge_dev",
 ]
 
 
@@ -161,6 +162,11 @@ def load_library():
     lib.dimb_gv_verify_dev.argtypes = [vp, ip, C.POINTER(FeatsDev), C.POINTER(FeatsDev), vp, vp, ip, C.POINTER(C.c_uint),
                                        C.POINTER(GvConf), vp, vp, vp, vp, vp, vp]
     lib.dimb_fstore_block_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(C.c_size_t), C.POINTER(ip), C.POINTER(ip)]
+    lib.dimb_tile_grid.argtypes = [ip] * 6 + [vp]
+    lib.dimb_tile_cut_dev.argtypes = [vp, vp] + [ip] * 8 + [vp, vp]
+    lib.dimb_tile_merge_dev.argtypes = [vp, ip, vp] + [ip] * 6 + [vp, vp, vp, vp, ip, vp]
+    lib.dimb_tile_views_dev.argtypes = [vp, ip, vp, ip, vp, vp, vp, vp]
+    lib.dimb_tile_match_merge_dev.argtypes = [vp, ip, vp, vp, vp, vp, ip, vp, vp, ip, vp, vp, ip, vp]
     _lib = lib
     return lib
 
@@ -226,6 +232,24 @@ class SelfTest:
 
 def _ptr(a: np.ndarray):
     return a.ctypes.data_as(C.c_void_p)
+
+
+def _int_array(values):
+    a = np.ascontiguousarray(np.asarray(values, np.int64).astype(np.int32).reshape(-1))
+    return a, _ptr(a) if a.size else None
+
+
+def tile_grid(height: int, width: int, tile_h: int, tile_w: int, overlap_h: int, overlap_w: int) -> dict:
+    """The tile grid the library cuts (dimb_tile_grid, no GPU needed): n_rows, n_cols, pad_top, pad_left, stride_h, stride_w and
+    the (x, y) origin of every tile in the un-padded image (tiling.compute_tiles_by_size's geometry, row-major)."""
+    out = np.zeros(6, np.int32)
+    rc = load_library().dimb_tile_grid(int(height), int(width), int(tile_h), int(tile_w), int(overlap_h), int(overlap_w), _ptr(out))
+    if rc != OK:
+        raise ValueError(f"invalid tile geometry: image {height}x{width}, tile {tile_h}x{tile_w}, overlap {overlap_h}x{overlap_w} "
+                         "(need 0 <= overlap < tile and at most 2048 tiles)")
+    rows, cols, pt, pl, sh, sw = (int(v) for v in out)
+    origins = [(-pl + c * sw, -pt + r * sh) for r in range(rows) for c in range(cols)]
+    return {"n_rows": rows, "n_cols": cols, "pad_top": pt, "pad_left": pl, "stride_h": sh, "stride_w": sw, "origins": origins}
 
 
 class Context:
@@ -318,6 +342,21 @@ class Context:
         conf = GvConf(float(threshold), int(max_iters), int(min_inliers), float(min_inlier_ratio))
         self.check(self.lib.dimb_gv_verify_dev(self.h, P, a0, a1, d_matches, d_n_matches, cap, sd, C.byref(conf), d_verified, d_n_verified,
                                                d_F, d_mask, d_n_inliers, stream), "dimb_gv_verify_dev")
+
+    def tile_cut_dev(self, d_images, B, H, W, channels, tile_h, tile_w, overlap_h, overlap_w, d_tiles, stream=0):
+        """B float32 (H,W,channels) device images -> their tiles [B*T][tile_h][tile_w][channels] (dimb_tile_cut_dev; ints are device
+        addresses); asynchronous on `stream`."""
+        self.check(self.lib.dimb_tile_cut_dev(self.h, d_images, B, H, W, channels, tile_h, tile_w, overlap_h, overlap_w, d_tiles, stream),
+                   "dimb_tile_cut_dev")
+
+    def tile_match_merge_dev(self, pair_offsets, view0, view1, d_maps, map_ld, d_matches, d_n_matches, cap, d_out, d_n_out, cap2, stream=0):
+        """Tile-pair match tables -> de-duplicated image-pair tables in merged rows (dimb_tile_match_merge_dev).  pair_offsets: host
+        CSR [Q+1] over the tile pairs; view0 / view1: the map rows of both sides of every tile pair.  Asynchronous on `stream`."""
+        off, p_off = _int_array(pair_offsets)
+        v0, p0 = _int_array(view0)
+        v1, p1 = _int_array(view1)
+        self.check(self.lib.dimb_tile_match_merge_dev(self.h, len(off) - 1, p_off, p0, p1, d_maps, map_ld, d_matches, d_n_matches, cap, d_out,
+                                                      d_n_out, cap2, stream), "dimb_tile_match_merge_dev")
 
     def nn_match_dev(self, d_desc0: int, n0: int, d_desc1: int, n1: int, D: int, mode: str, th: float, d_idx: int, d_dist: int,
                      d_n: int, cap: int, f16: bool = False, ld0: int = 0, ld1: int = 0, stream: int = 0):
@@ -681,6 +720,20 @@ class FeatureStoreDev:
         f = SgFeatsDev()
         self.ctx.check(self.ctx.lib.dimb_fstore_sg_feats_dev(self.h, slot, C.byref(f)), "dimb_fstore_sg_feats_dev")
         return f
+
+    def tile_merge_dev(self, slots, H, W, tile_h, tile_w, overlap_h, overlap_w, d_kpts, d_scores, d_desc, d_counts, K, stream=0):
+        """Tile-feature merge of len(slots) images (dimb_tile_merge_dev): the extractor outputs of their T tiles each ([B*T][K] layouts)
+        -> one merged slot per image.  Asynchronous on `stream`."""
+        s, p = _int_array(slots)
+        self.ctx.check(self.ctx.lib.dimb_tile_merge_dev(self.h, len(s), p, H, W, tile_h, tile_w, overlap_h, overlap_w, d_kpts, d_scores, d_desc,
+                                                        d_counts, K, stream), "dimb_tile_merge_dev")
+
+    def tile_views_dev(self, src_slots, n_tiles, views: "FeatureStoreDev", dst_slots, d_map, stream=0):
+        """Tile views of the merged slots src_slots (dimb_tile_views_dev): view slot dst_slots[b] + t of `views`, map row of the same
+        index in d_map ([views.n_slots][views.cap] int32).  Asynchronous on `stream`."""
+        s, ps = _int_array(src_slots)
+        d, pd = _int_array(dst_slots)
+        self.ctx.check(self.ctx.lib.dimb_tile_views_dev(self.h, len(s), ps, n_tiles, views.h, pd, d_map, stream), "dimb_tile_views_dev")
 
     def desc_ptr(self, slot: int) -> int:
         """Device address of the slot's float16 (D, cap) descriptor block (for dimb_nn_match_dev, ld = cap)."""

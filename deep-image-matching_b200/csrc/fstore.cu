@@ -13,16 +13,9 @@
 #include <memory>
 #include <vector>
 
-#include "common.cuh"
+#include "fstore.cuh"
 
 namespace {
-constexpr int kHdrInts = 8;  // n, H, W, valid, 4 spare
-
-struct SlotPtrs {
-  int* hdr;
-  __half *kpts, *scores, *tile, *desc;
-};
-
 // float32 features (layouts of dimb_sp_extract_dev / dimb_aliked_extract_dev) -> one float16 block.  grid.x covers cap in 256s,
 // grid.y = D + 1: row y < D converts descriptor row y, row D converts keypoints / scores / tile_idx and writes the header.
 __global__ void fs_put_kernel(const float* __restrict__ kpts, const float* __restrict__ scores, const float* __restrict__ tile_idx,
@@ -52,21 +45,7 @@ __global__ void fs_put_kernel(const float* __restrict__ kpts, const float* __res
 }
 }  // namespace
 
-struct dimb_fstore {
-  std::vector<void*> mem;
-  dimb_ctx* ctx;
-  int n_slots, cap, D;
-  size_t slot_bytes, off_kpts, off_scores, off_tile, off_desc;
-  uint8_t* base = nullptr;
-  float *st_k = nullptr, *st_s = nullptr, *st_t = nullptr, *st_d = nullptr;  // staging of the host put
-  std::vector<uint8_t> host;  // staging of the host get
-};
-
-static SlotPtrs slot_ptrs(const dimb_fstore* fs, int slot) {
-  uint8_t* b = fs->base + static_cast<size_t>(slot) * fs->slot_bytes;
-  return {reinterpret_cast<int*>(b), reinterpret_cast<__half*>(b + fs->off_kpts), reinterpret_cast<__half*>(b + fs->off_scores),
-          reinterpret_cast<__half*>(b + fs->off_tile), reinterpret_cast<__half*>(b + fs->off_desc)};
-}
+static SlotPtrs slot_ptrs(const dimb_fstore* fs, int slot) { return fs_layout(fs).at(slot); }
 
 extern "C" {
 

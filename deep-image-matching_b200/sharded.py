@@ -11,7 +11,11 @@ match_pairs, image_matching.py:413-494, is the serial loop this replaces) run in
      (``gather_match_tables``).
 With ``verification`` the matcher's tables of each pair batch go straight into the device geometric verification (fundamental-matrix
 RANSAC, ordered inlier compaction and the per-pair gate, one launch group per batch); raw tables, verified tables and F are gathered
-to rank 0 (``gather_verified``), and ``export_verified_to_colmap`` writes the COLMAP database from the store and those results."""
+to rank 0 (``gather_verified``), and ``export_verified_to_colmap`` writes the COLMAP database from the store and those results.
+With ``tiling`` (the reference's tile_size / tile_overlap / tile_selection) high-resolution images are cut into tiles on the device,
+the extractor runs over tiles and every image's tile features are merged into its slot (ExtractorBase._extract_by_tile); after the
+exchange each rank splits the merged slots into per-tile views, matches the selected tile pairs out of the views and merges their
+tables into one table per image pair (MatcherBase._match_by_tile)."""
 from __future__ import annotations
 
 import numpy as np
@@ -204,6 +208,61 @@ def verification_conf(verification) -> dict | None:
     return conf
 
 
+TILE_SELECTIONS = ("grid", "exhaustive")
+
+
+def tiling_conf(tiling) -> dict | None:
+    """The ``tiling`` argument of ImageSetMatcher, validated (None stays None).  Keys as in the reference's configuration:
+    ``tile_size`` (x, y) or one int (required), ``tile_overlap`` int (default 0) and ``tile_selection`` "grid" (default) or
+    "exhaustive".  The returned dict adds ``tile_hw`` / ``overlap_hw``, the (H, W) order ``tiling._hw`` gives them.  Preselection is
+    not a configured mode here: pass its tile-pair lists to ``match`` / ``run`` as ``tile_pairs``."""
+    if tiling is None:
+        return None
+    from .tiling import _hw
+    unknown = set(tiling) - {"tile_size", "tile_overlap", "tile_selection"}
+    if unknown:
+        raise ValueError(f"unknown tiling option(s) {sorted(unknown)}; expected some of ['tile_overlap', 'tile_selection', 'tile_size']")
+    if "tile_size" not in tiling:
+        raise ValueError("tiling needs tile_size")
+    size, overlap = tiling["tile_size"], tiling.get("tile_overlap", 0)
+    sel = str(tiling.get("tile_selection", "grid")).lower()
+    ok_size = isinstance(size, int) or (isinstance(size, (tuple, list)) and len(size) == 2 and all(isinstance(v, int) for v in size))
+    if not ok_size or min(_hw(size)) < 1:
+        raise ValueError(f"tile_size must be a positive int or (x, y) of positive ints, got {size!r}")
+    if not isinstance(overlap, int) or not 0 <= overlap < min(_hw(size)):
+        raise ValueError(f"tile_overlap must be an int in [0, min(tile_size)), got {overlap!r}")
+    if sel not in TILE_SELECTIONS:
+        raise ValueError(f"tile_selection must be one of {TILE_SELECTIONS} (preselection: pass tile_pairs), got {tiling.get('tile_selection')!r}")
+    return {"tile_size": size if isinstance(size, int) else tuple(size), "tile_overlap": overlap, "tile_selection": sel,
+            "tile_hw": _hw(size), "overlap_hw": _hw(overlap)}
+
+
+def tile_pairs_for(selection: str, n_tiles: int) -> list:
+    """The tile pairs of one image pair under a configured selection (tiling.tile_selection for equally tiled images): "grid" pairs
+    tile t with tile t, "exhaustive" every (t0, t1), sorted."""
+    if selection == "grid":
+        return [(t, t) for t in range(n_tiles)]
+    if selection == "exhaustive":
+        return [(t0, t1) for t0 in range(n_tiles) for t1 in range(n_tiles)]
+    raise ValueError(f"tile_selection must be one of {TILE_SELECTIONS}, got {selection!r}")
+
+
+def pack_tile_batches(n_tile_pairs, batch_pairs: int) -> list:
+    """Consecutive image pairs packed into matcher batches of at most ``batch_pairs`` tile pairs, image pairs kept whole: a list of
+    (start, end) ranges of image pairs.  Raises ValueError when one image pair alone selects more than ``batch_pairs`` tile pairs."""
+    out, start, load = [], 0, 0
+    for k, n in enumerate(n_tile_pairs):
+        if n > batch_pairs:
+            raise ValueError(f"image pair {k} selects {n} tile pairs, more than batch_pairs={batch_pairs}")
+        if load + n > batch_pairs:
+            out.append((start, k))
+            start, load = k, 0
+        load += n
+    if start < len(n_tile_pairs):
+        out.append((start, len(n_tile_pairs)))
+    return out
+
+
 class ImageSetMatcher:
     """Two-phase multi-GPU matching of an image set (module docstring): SuperPoint on this rank's images into the device feature
     store, one all_gather of the float16 feature blocks, LightGlue or SuperGlue on this rank's share of the pair list, gather of the
@@ -218,48 +277,104 @@ class ImageSetMatcher:
     ``n_inliers >= min_inliers_per_pair`` and ``float32(n_inliers) >= float32(min_inlier_ratio_per_pair) * float32(n_raw)``; a
     rejected pair gets an empty verified table (its F and count are still reported).  Pairs with fewer than 8 raw matches keep
     every match and have no F (as the reference's geometric_verification returns), then face the same gate.  Method "NONE":
-    verified = raw, F = None, nothing is launched."""
+    verified = raw, F = None, nothing is launched.
+
+    ``extractor``: "superpoint" (default; gray images (k, H, W)) or "aliked" (RGB images (k, H, W, 3); ``sp_weights`` / ``sp_conf``
+    are the ALIKED weights and the ``AlikedNet`` configuration, one image or tile per extraction call, 128-d descriptors, LightGlue
+    built with input_dim 128).  ALIKED with SuperGlue is refused.
+
+    ``tiling``: None (default) or a dict checked by ``tiling_conf``.  With tiling, ``extract`` takes full-size images, cuts their tiles
+    on the device, runs the extractor over tiles (SuperPoint ``batch_images`` tiles per call, network sized for one tile, with
+    ``fix_sampling=True`` as the reference's tiling requires) and merges each image's tile features into its slot (store capacity
+    T * K).  ``exchange`` also builds the per-tile views of every image.  ``match`` / ``match_verified`` pack whole image pairs into
+    matcher batches of at most ``batch_pairs`` tile pairs, match the selected tile pairs out of the views and return one merged,
+    de-duplicated table per image pair in merged-slot rows; verification and ``export_colmap`` run on the merged slots.  ``tile_pairs``
+    (per image pair, a list of (t0, t1)) overrides the configured selection, e.g. with PRESELECTION lists computed on the host by
+    ``tiling.preselection_matches`` + ``tiling.tile_selection``."""
 
     def __init__(self, ctx, sp_weights: dict, lg_weights: dict, n_images: int, height: int, width: int, sp_conf: dict, lg_conf: dict,
-                 batch_images: int = 16, batch_pairs: int = 32, dist=None, matcher: str = "lightglue", verification: dict | None = None):
+                 batch_images: int = 16, batch_pairs: int = 32, dist=None, matcher: str = "lightglue", verification: dict | None = None,
+                 tiling: dict | None = None, extractor: str = "superpoint"):
         import torch
 
         from . import _native
+        if matcher not in ("lightglue", "superglue"):
+            raise ValueError(f'matcher must be "lightglue" or "superglue", got {matcher!r}')
+        if extractor not in ("superpoint", "aliked"):
+            raise ValueError(f'extractor must be "superpoint" or "aliked", got {extractor!r}')
+        if extractor == "aliked" and matcher == "superglue":
+            raise ValueError("SuperGlue matches SuperPoint features only; use matcher=\"lightglue\" with ALIKED")
+        self.tiling = tiling_conf(tiling)
+        if self.tiling is not None and extractor == "superpoint":
+            if "fix_sampling" in sp_conf and not sp_conf["fix_sampling"]:
+                raise ValueError("tiled SuperPoint extraction runs with fix_sampling=True (the reference's rule); fix_sampling=False was given")
+            sp_conf = {**sp_conf, "fix_sampling": True}
+        if extractor == "aliked":
+            lg_conf = {"input_dim": 128, **lg_conf}
+            if lg_conf["input_dim"] != 128:
+                raise ValueError(f"LightGlue on ALIKED features needs input_dim=128, got {lg_conf['input_dim']}")
         self.torch, self.dist, self.ctx = torch, dist, ctx
         self.world = dist.get_world_size() if dist is not None and dist.is_initialized() else 1
         self.rank = dist.get_rank() if self.world > 1 else 0
         self.n, self.H, self.W = n_images, height, width
-        self.cap = int(sp_conf["max_keypoints"])
+        self.extractor = extractor
+        self.cap = int(sp_conf["max_keypoints"]) if extractor == "superpoint" else int(sp_conf.get("max_num_keypoints", 4000))
+        if self.cap < 1:
+            raise ValueError(f"the image-set matcher needs a positive keypoint limit per extraction, got {self.cap}")
+        self.D = 256 if extractor == "superpoint" else 128
         self.B, self.P = batch_images, batch_pairs
-        self.sp = _native.SuperPointNet(ctx, sp_weights, max_batch=batch_images, max_height=height, max_width=width, **sp_conf)
-        if matcher not in ("lightglue", "superglue"):
-            raise ValueError(f'matcher must be "lightglue" or "superglue", got {matcher!r}')
+        eh, ew = (height, width)
+        if self.tiling is not None:
+            eh, ew = self.tiling["tile_hw"]
+            self.grid = _native.tile_grid(height, width, eh, ew, *self.tiling["overlap_hw"])
+            self.T = len(self.grid["origins"])
+        if extractor == "superpoint":
+            self.sp = _native.SuperPointNet(ctx, sp_weights, max_batch=batch_images, max_height=eh, max_width=ew, **sp_conf)
+        else:
+            self.al = _native.AlikedNet(ctx, sp_weights, max_height=eh, max_width=ew, **sp_conf)
         self.matcher = matcher
         if matcher == "superglue":
             self.sg = _native.SuperGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=self.cap, **lg_conf)
         else:
             self.lg = _native.LightGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=self.cap, **lg_conf)
         self.ipr = images_per_rank(n_images, self.world)
-        self.store = _native.FeatureStoreDev(ctx, self.world * self.ipr, self.cap, 256)
+        store_cap = self.cap if self.tiling is None else self.T * self.cap
+        self.store = _native.FeatureStoreDev(ctx, self.world * self.ipr, store_cap, self.D)
         dev = torch.device("cuda", ctx.device)
-        # extraction outputs of one batch (float32, library layouts) and match outputs of one pair batch
-        self.kp = torch.zeros(batch_images, self.cap, 2, device=dev)
-        self.sc = torch.zeros(batch_images, self.cap, device=dev)
-        self.de = torch.zeros(batch_images, 256, self.cap, device=dev)
-        self.cnt = torch.zeros(batch_images, dtype=torch.int32, device=dev)
+        # extraction outputs of one batch (float32, library layouts) and match outputs of one pair batch; tiled: the tiles of G images
+        n_ext = batch_images
+        if self.tiling is not None:
+            self.G = max(1, batch_images // self.T)
+            n_ext = self.G * self.T
+            self.C = 1 if extractor == "superpoint" else 3
+            self.tiles = torch.zeros(n_ext, eh, ew, self.C, device=dev)
+        self.kp = torch.zeros(n_ext, self.cap, 2, device=dev)
+        self.sc = torch.zeros(n_ext, self.cap, device=dev)
+        self.de = torch.zeros(n_ext, self.D, self.cap, device=dev)
+        self.cnt = torch.zeros(n_ext, dtype=torch.int32, device=dev)
         self.m = torch.zeros(batch_pairs, self.cap, 2, dtype=torch.int64, device=dev)
         self.ms = torch.zeros(batch_pairs, self.cap, device=dev)
         self.nm = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
         self.sl = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
+        gv_cap = self.cap
+        if self.tiling is not None:
+            # per-tile views of every image (slot i * T + t) with their row maps, and the merged tables of one batch: an image pair
+            # has at most min(batch_pairs, T * T) distinct tile pairs of at most K rows each, so cap2 holds every merged table whole
+            self.views = _native.FeatureStoreDev(ctx, n_images * self.T, self.cap, self.D)
+            self.vmap = torch.zeros(n_images * self.T, self.views.cap, dtype=torch.int32, device=dev)
+            self.cap2 = gv_cap = min(batch_pairs, self.T * self.T) * self.cap
+            self.mm = torch.zeros(batch_pairs, self.cap2, 2, dtype=torch.int64, device=dev)
+            self.nmm = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
         self.gv = verification_conf(verification)
         if self.gv is not None and self.gv["method"] != "NONE":  # verification outputs of one pair batch + pinned host copies
-            self.v = torch.zeros(batch_pairs, self.cap, 2, dtype=torch.int64, device=dev)
+            self.v = torch.zeros(batch_pairs, gv_cap, 2, dtype=torch.int64, device=dev)
             self.nv = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
             self.F = torch.zeros(batch_pairs, 9, device=dev)
-            self.mask = torch.zeros(batch_pairs, self.cap, dtype=torch.uint8, device=dev)
+            self.mask = torch.zeros(batch_pairs, gv_cap, dtype=torch.uint8, device=dev)
             self.ninl = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
-            self.host_out = {k: torch.zeros_like(t, device="cpu").pin_memory() for k, t in
-                      (("m", self.m), ("nm", self.nm), ("v", self.v), ("nv", self.nv), ("F", self.F), ("ninl", self.ninl))}
+            if self.tiling is None:
+                self.host_out = {k: torch.zeros_like(t, device="cpu").pin_memory() for k, t in
+                                 (("m", self.m), ("nm", self.nm), ("v", self.v), ("nv", self.nv), ("F", self.F), ("ninl", self.ninl))}
 
         class _DevArr:  # zero-copy torch view of the store's device allocation (for the NCCL all_gather)
             def __init__(self, ptr, shape):
@@ -269,8 +384,18 @@ class ImageSetMatcher:
         self.exchanged_bytes = 0
 
     def extract(self, d_images, image_ids):
-        """Phase 1: d_images = float32 CUDA tensor (k, H, W) holding this rank's images `image_ids` (gray 0..255)."""
+        """Phase 1: d_images = float32 CUDA tensor holding this rank's images `image_ids`, 0..255: (k, H, W) gray for SuperPoint,
+        (k, H, W, 3) RGB for ALIKED.  With tiling the images are full size and are cut into tiles on the device."""
         st = self.torch.cuda.current_stream().cuda_stream
+        if self.tiling is not None:
+            return self._extract_tiled(d_images, image_ids, st)
+        if self.extractor == "aliked":
+            for k, i in enumerate(image_ids):
+                self.al.extract_dev(d_images[k].data_ptr(), self.H, self.W, 3, self.kp.data_ptr(), self.sc.data_ptr(), self.de.data_ptr(),
+                                    self.cnt.data_ptr(), self.cap, st)
+                self.store.put_dev(store_slot(i, self.n, self.world), self.kp.data_ptr(), self.sc.data_ptr(), self.de.data_ptr(), self.cap,
+                                   self.cnt.data_ptr(), self.H, self.W, None, st)
+            return
         for b0 in range(0, len(image_ids), self.B):
             ids = image_ids[b0:b0 + self.B]
             nb = len(ids)
@@ -280,26 +405,99 @@ class ImageSetMatcher:
                 self.store.put_dev(store_slot(i, self.n, self.world), self.kp[k].data_ptr(), self.sc[k].data_ptr(), self.de[k].data_ptr(),
                                    self.cap, self.cnt[k:k + 1].data_ptr(), self.H, self.W, None, st)
 
+    def _extract_tiled(self, d_images, image_ids, st):
+        """Groups of G images: tile cut, the extractor over their G * T tiles, one tile merge into their slots."""
+        (th, tw), (oh, ow), T, K = self.tiling["tile_hw"], self.tiling["overlap_hw"], self.T, self.cap
+        for g0 in range(0, len(image_ids), self.G):
+            ids = image_ids[g0:g0 + self.G]
+            nt = len(ids) * T
+            self.ctx.tile_cut_dev(d_images[g0:g0 + len(ids)].data_ptr(), len(ids), self.H, self.W, self.C, th, tw, oh, ow,
+                                  self.tiles.data_ptr(), st)
+            if self.extractor == "superpoint":
+                for t0 in range(0, nt, self.B):
+                    k = min(self.B, nt - t0)
+                    self.sp.extract_dev(self.tiles[t0].data_ptr(), k, th, tw, self.kp[t0].data_ptr(), self.sc[t0].data_ptr(),
+                                        self.de[t0].data_ptr(), self.cnt[t0:].data_ptr(), K, st)
+            else:
+                for t in range(nt):
+                    self.al.extract_dev(self.tiles[t].data_ptr(), th, tw, 3, self.kp[t].data_ptr(), self.sc[t].data_ptr(), self.de[t].data_ptr(),
+                                        self.cnt[t:].data_ptr(), K, st)
+            self.store.tile_merge_dev([store_slot(i, self.n, self.world) for i in ids], self.H, self.W, th, tw, oh, ow, self.kp.data_ptr(),
+                                      self.sc.data_ptr(), self.de.data_ptr(), self.cnt.data_ptr(), K, st)
+
     def exchange(self):
-        """The collective of the path: every rank's float16 feature blocks to every rank (NCCL all_gather over NVLink)."""
+        """The collective of the path: every rank's float16 feature blocks to every rank (NCCL all_gather over NVLink).  With tiling,
+        every rank then builds the per-tile views of all images from the merged slots."""
         self.exchanged_bytes = all_gather_blocks(self.store_t, self.n, self.dist)
+        if self.tiling is not None:
+            st = self.torch.cuda.current_stream().cuda_stream
+            step = max(1, 65535 // self.T)
+            for b0 in range(0, self.n, step):
+                ids = range(b0, min(self.n, b0 + step))
+                self.store.tile_views_dev([store_slot(i, self.n, self.world) for i in ids], self.T, self.views, [i * self.T for i in ids],
+                                          self.vmap.data_ptr(), st)
+
+    def _match_slots(self, store, s0, s1, st):
+        """Enqueue the matcher on slot pairs (s0[k], s1[k]) of `store` (outputs in self.m / self.ms / self.nm)."""
+        if self.matcher == "superglue":
+            self.sg.match_dev([store.sg_feats_dev(s) for s in s0], [store.sg_feats_dev(s) for s in s1], self.m.data_ptr(), self.ms.data_ptr(),
+                              self.nm.data_ptr(), self.cap, st)
+        else:
+            self.lg.match_dev([store.feats_dev(s) for s in s0], [store.feats_dev(s) for s in s1], self.m.data_ptr(), self.ms.data_ptr(),
+                              self.nm.data_ptr(), self.sl.data_ptr(), self.cap, st)
 
     def _match_batch(self, chunk, st):
         """Enqueue the matcher on one pair batch (outputs in self.m / self.ms / self.nm)."""
-        if self.matcher == "superglue":
-            f0 = [self.store.sg_feats_dev(store_slot(i, self.n, self.world)) for i, _ in chunk]
-            f1 = [self.store.sg_feats_dev(store_slot(j, self.n, self.world)) for _, j in chunk]
-            self.sg.match_dev(f0, f1, self.m.data_ptr(), self.ms.data_ptr(), self.nm.data_ptr(), self.cap, st)
-        else:
-            f0 = [self.store.feats_dev(store_slot(i, self.n, self.world)) for i, _ in chunk]
-            f1 = [self.store.feats_dev(store_slot(j, self.n, self.world)) for _, j in chunk]
-            self.lg.match_dev(f0, f1, self.m.data_ptr(), self.ms.data_ptr(), self.nm.data_ptr(), self.sl.data_ptr(), self.cap, st)
+        self._match_slots(self.store, [store_slot(i, self.n, self.world) for i, _ in chunk],
+                          [store_slot(j, self.n, self.world) for _, j in chunk], st)
 
-    def match(self, pairs, pair_ids):
+    def _tile_pair_lists(self, pairs, tile_pairs):
+        if tile_pairs is None:
+            return [tile_pairs_for(self.tiling["tile_selection"], self.T)] * len(pairs)
+        if len(tile_pairs) != len(pairs):
+            raise ValueError(f"tile_pairs must hold one list per image pair: {len(tile_pairs)} lists for {len(pairs)} pairs")
+        lists = []
+        for lst in tile_pairs:
+            lst = [(int(a), int(b)) for a, b in lst]
+            if any(not (0 <= a < self.T and 0 <= b < self.T) for a, b in lst):
+                raise ValueError(f"tile indices must lie in [0, {self.T})")
+            lists.append(lst)
+        return lists
+
+    def _match_tiled_batch(self, chunk, lists, st):
+        """Enqueue the matcher on the selected tile pairs of the image pairs `chunk` (views i * T + t) and the tile-pair match merge
+        (outputs in self.mm / self.nmm)."""
+        T = self.T
+        v0 = [i * T + a for (i, _), lst in zip(chunk, lists) for a, _ in lst]
+        v1 = [j * T + b for (_, j), lst in zip(chunk, lists) for _, b in lst]
+        if v0:
+            self._match_slots(self.views, v0, v1, st)
+        offsets = np.concatenate([[0], np.cumsum([len(lst) for lst in lists])])
+        self.ctx.tile_match_merge_dev(offsets, v0, v1, self.vmap.data_ptr(), self.views.cap, self.m.data_ptr(), self.nm.data_ptr(), self.cap,
+                                      self.mm.data_ptr(), self.nmm.data_ptr(), self.cap2, st)
+
+    def _read_tables(self, m, nm, Q):
+        """Host copies of the first Q tables of m [P][cap][2] with counts nm (the first copy synchronises)."""
+        n = np.minimum(nm[:Q].cpu().numpy(), m.shape[1])
+        rows = int(n.max(initial=0))
+        h = m[:Q, :rows].cpu().numpy()
+        return [h[k, :n[k]].copy() for k in range(Q)]
+
+    def match(self, pairs, pair_ids, tile_pairs=None):
         """Phase 2: LightGlue or SuperGlue on `pairs` = [(i, j), ...] (this rank's share); returns {pair id: int64 (S,2)} after ONE
-        device->host copy per batch.  Features are read in place from the store (float16, no rounding left to do)."""
+        device->host copy per batch.  Features are read in place from the store (float16, no rounding left to do).  Tiled: the tables
+        are the merged image-pair tables; `tile_pairs` optionally gives each pair's list of (t0, t1)."""
         st = self.torch.cuda.current_stream().cuda_stream
         out = {}
+        if self.tiling is not None:
+            lists = self._tile_pair_lists(pairs, tile_pairs)
+            for s, e in pack_tile_batches([len(lst) for lst in lists], self.P):
+                self._match_tiled_batch(pairs[s:e], lists[s:e], st)
+                for k, m in enumerate(self._read_tables(self.mm, self.nmm, e - s)):
+                    out[pair_ids[s + k]] = m
+            return out
+        if tile_pairs is not None:
+            raise ValueError("tile_pairs needs an ImageSetMatcher built with tiling")
         for b0 in range(0, len(pairs), self.P):
             chunk = pairs[b0:b0 + self.P]
             self._match_batch(chunk, st)
@@ -309,15 +507,19 @@ class ImageSetMatcher:
                 out[pair_ids[b0 + k]] = m[k, :nm[k]].copy()
         return out
 
-    def match_verified(self, pairs, pair_ids):
+    def match_verified(self, pairs, pair_ids, tile_pairs=None):
         """Phase 2 with geometric verification: returns {pair id: (raw int64 (S,2), verified int64 (V,2), F (3,3) float32 or None,
         n_inliers)}.  Per batch the matcher and dimb_gv_verify_dev are enqueued on the same stream and the results come back with
-        ONE synchronise."""
+        ONE synchronise.  Tiled: the merged tables are verified against the merged slots."""
         from .geometric_verification import gv_seed
         if self.gv is None:
             raise RuntimeError("ImageSetMatcher was built without verification")
         if self.gv["method"] == "NONE":  # the reference skips the estimator: verified = raw, no F
-            return {k: (m, m.copy(), None, len(m)) for k, m in self.match(pairs, pair_ids).items()}
+            return {k: (m, m.copy(), None, len(m)) for k, m in self.match(pairs, pair_ids, tile_pairs).items()}
+        if self.tiling is not None:
+            return self._match_verified_tiled(pairs, pair_ids, tile_pairs)
+        if tile_pairs is not None:
+            raise ValueError("tile_pairs needs an ImageSetMatcher built with tiling")
         torch, st = self.torch, self.torch.cuda.current_stream()
         g, h = self.gv, self.host_out
         out = {}
@@ -342,22 +544,45 @@ class ImageSetMatcher:
                                int(ninl[k]))
         return out
 
-    def run(self, d_images, my_image_ids, pairs, costs=None):
-        """extract -> exchange -> match my share -> gather to rank 0.  Returns the list of match tables on rank 0 (None elsewhere)."""
+    def _match_verified_tiled(self, pairs, pair_ids, tile_pairs):
+        from .geometric_verification import gv_seed
+        st, g = self.torch.cuda.current_stream(), self.gv
+        lists = self._tile_pair_lists(pairs, tile_pairs)
+        out = {}
+        for s, e in pack_tile_batches([len(lst) for lst in lists], self.P):
+            chunk, ids = pairs[s:e], pair_ids[s:e]
+            self._match_tiled_batch(chunk, lists[s:e], st.cuda_stream)
+            f0 = [self.store.feats_dev(store_slot(i, self.n, self.world)) for i, _ in chunk]
+            f1 = [self.store.feats_dev(store_slot(j, self.n, self.world)) for _, j in chunk]
+            self.ctx.gv_verify_dev(f0, f1, self.mm.data_ptr(), self.nmm.data_ptr(), self.cap2, [gv_seed(g["seed"], k) for k in ids],
+                                   g["threshold"], g["max_iters"], g["min_inliers_per_pair"], g["min_inlier_ratio_per_pair"],
+                                   self.v.data_ptr(), self.nv.data_ptr(), self.F.data_ptr(), self.mask.data_ptr(), self.ninl.data_ptr(),
+                                   st.cuda_stream)
+            Q = e - s
+            raw = self._read_tables(self.mm, self.nmm, Q)
+            ver = self._read_tables(self.v, self.nv, Q)
+            F, ninl = self.F[:Q].cpu().numpy(), self.ninl[:Q].cpu().numpy()
+            for k in range(Q):
+                out[ids[k]] = (raw[k], ver[k], F[k].reshape(3, 3).copy() if np.any(F[k]) else None, int(ninl[k]))
+        return out
+
+    def run(self, d_images, my_image_ids, pairs, costs=None, tile_pairs=None):
+        """extract -> exchange -> match my share -> gather to rank 0.  Returns the list of match tables on rank 0 (None elsewhere).
+        tile_pairs (tiled only): per pair of `pairs`, its list of (t0, t1)."""
         self.extract(d_images, my_image_ids)
         self.exchange()
         mine = shard_pairs(len(pairs), self.world, self.rank, costs)
-        res = self.match([pairs[k] for k in mine], mine)
+        res = self.match([pairs[k] for k in mine], mine, None if tile_pairs is None else [tile_pairs[k] for k in mine])
         return gather_match_tables(mine, [res[k] for k in mine], len(pairs), self.dist if self.world > 1 else None,
                                    self.torch.device("cuda", self.ctx.device) if self.world > 1 else None)
 
-    def run_verified(self, d_images, my_image_ids, pairs, costs=None):
+    def run_verified(self, d_images, my_image_ids, pairs, costs=None, tile_pairs=None):
         """extract -> exchange -> match and verify my share -> gather to rank 0.  Returns, on rank 0, the list of
         (raw, verified, F, n_inliers) per pair (None elsewhere); ``export_colmap`` turns it into a COLMAP database."""
         self.extract(d_images, my_image_ids)
         self.exchange()
         mine = shard_pairs(len(pairs), self.world, self.rank, costs)
-        res = self.match_verified([pairs[k] for k in mine], mine)
+        res = self.match_verified([pairs[k] for k in mine], mine, None if tile_pairs is None else [tile_pairs[k] for k in mine])
         return gather_verified(mine, [res[k] for k in mine], len(pairs), self.dist if self.world > 1 else None,
                                self.torch.device("cuda", self.ctx.device) if self.world > 1 else None)
 

@@ -239,6 +239,50 @@ int dimb_gv_verify_dev(dimb_ctx* ctx, int P, const dimb_feats_dev* f0, const dim
                        const int* d_n_matches, int cap, const unsigned* seeds, const dimb_gv_conf* conf, int64_t* d_verified,
                        int* d_n_verified, float* d_F, unsigned char* d_mask, int* d_n_inliers, void* stream);
 
+/* ------------------------------------------------------------------ tiled image sets
+ * Device counterparts of ExtractorBase._extract_by_tile (extractors/extractor_base.py:279-390) and MatcherBase._match_by_tile
+ * (matchers/matcher_base.py:362-485).  Every entry is asynchronous on `stream` and never synchronises (once its context scratch has
+ * grown to the call's size), is bitwise reproducible and independent of how images or pairs are batched, and returns DIMB_ERR_ARG
+ * before any CUDA call for a NULL pointer or an out-of-range size.  CUDA-core kernels: they run with DIMB_TC=0 as well.
+ * Profile groups: tile.cut, tile.merge, tile.views, tile.match_merge.
+ *
+ * Tile geometry (utils/tiling.py Tiler.compute_tiles_by_size): tile_h x tile_w windows stepped by (tile - overlap), on the image
+ * zero-padded by kornia's compute_padding called WITHOUT the stride (quirk A.7: the padding makes (size - tile) % tile == 0, the
+ * odd pixel at the bottom / right; with an overlap the last `overlap` padded pixels are never covered).  Tiles are numbered
+ * row-major; tile t = row * n_cols + col has its origin at (x, y) = (-pad_left + col * stride_w, -pad_top + row * stride_h) in the
+ * un-padded image.  At most 2048 tiles (tile_idx is stored as float16).
+ * Host only (no CUDA call): out[6] = {n_rows, n_cols, pad_top, pad_left, stride_h, stride_w}. */
+int dimb_tile_grid(int height, int width, int tile_h, int tile_w, int overlap_h, int overlap_w, int* out);
+/* d_images: B float32 images [B][H][W][channels], channels 1 (gray) or 3 (RGB).  d_tiles: [B * T][tile_h][tile_w][channels], the
+ * T tiles of image 0 first; pixels in the padding are 0.  B * T <= 65535. */
+int dimb_tile_cut_dev(dimb_ctx* ctx, const float* d_images, int B, int height, int width, int channels, int tile_h, int tile_w, int overlap_h,
+                      int overlap_w, float* d_tiles, void* stream);
+/* Tile-feature merge of B images into the store slots slots[b] (host array).  Input: the float32 extractor outputs of the T tiles
+ * of every image in the layouts of dimb_sp_extract_dev / dimb_aliked_extract_dev with capacity K per tile: d_kpts [B*T][K][2],
+ * d_scores [B*T][K], d_desc [B*T][D][K], d_counts [B*T] (device; rows = min(count, K)).  Per tile t in order: keypoints shifted by
+ * the tile origin (float32 add), kept iff 2 <= x < W - 2 and 2 <= y < H - 2, concatenated; then np.unique(kpts, axis=0,
+ * return_index=True): sorted by (x, y), the first of exact duplicates in concatenation order kept.  Descriptors, scores and
+ * tile_idx = t follow; the slot gets the float16 cast of dimb_fstore_put_dev and the header n = merged count, [H, W] of the full
+ * image.  DIMB_ERR_CAPACITY when the store's capacity is below T * K. */
+int dimb_tile_merge_dev(dimb_fstore* fs, int B, const int* slots, int height, int width, int tile_h, int tile_w, int overlap_h, int overlap_w,
+                        const float* d_kpts, const float* d_scores, const float* d_desc, const int* d_counts, int K, void* stream);
+/* Tile views (matcher_base.py:1380-1391 get_features_by_tile) of B merged slots src_slots[b]: view slot dst_slots[b] + t of `dst`
+ * receives the merged rows with tile_idx == t in merged order, and row dst_slot of d_map ([dst n_slots][dst cap] int32) maps each view
+ * row to its merged row.  The view header carries the FULL image's [H, W] (quirk A.3), so dimb_fstore_feats_dev /
+ * dimb_fstore_sg_feats_dev of a view slot feed dimb_lg_match_dev / dimb_sg_match_dev unchanged.  A tile left without rows gives
+ * n = 0.  Views hold at most dst's capacity rows (a tile never contributes more than the extractor's K).  Both stores share the
+ * context and the descriptor size; B * n_tiles <= 65535. */
+int dimb_tile_views_dev(dimb_fstore* src, int B, const int* src_slots, int n_tiles, dimb_fstore* dst, const int* dst_slots, int* d_map,
+                        void* stream);
+/* Tile-pair match merge of Q image pairs.  Host CSR: image pair q owns the tile pairs p in [pair_offsets[q], pair_offsets[q+1]);
+ * tile pair p matched view rows view0[p] (side 0) and view1[p] (side 1) of d_maps (rows of map_ld ints, as dimb_tile_views_dev writes
+ * them).  d_matches [P][cap][2] int64 + d_n_matches [P] in the layout of dimb_lg_match_dev / dimb_sg_match_dev (rows = min(n, cap)).
+ * Per image pair: both columns remapped to merged rows, concatenated, np.unique(axis=0) (sorted by (idx0, idx1), duplicates
+ * dropped).  Out (device): d_out [Q][cap2][2] int64 and d_n_out [Q], the full count also when it exceeds cap2 (only the first cap2
+ * rows are written).  An image pair without tile pairs gets 0. */
+int dimb_tile_match_merge_dev(dimb_ctx* ctx, int Q, const int* pair_offsets, const int* view0, const int* view1, const int* d_maps, int map_ld,
+                              const int64_t* d_matches, const int* d_n_matches, int cap, int64_t* d_out, int* d_n_out, int cap2, void* stream);
+
 /* ------------------------------------------------------------------ fused per-pair path
  * SuperPoint on both images of every pair followed by LightGlue, features kept in HBM in between (the
  * reference's features.h5 round trip, ImageMatcher.extract_features -> match_pairs, image_matching.py:413-494,
