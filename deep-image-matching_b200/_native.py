@@ -30,6 +30,7 @@ EXPORTS = [
     "dimb_fstore_create", "dimb_fstore_destroy", "dimb_fstore_put_dev", "dimb_fstore_put", "dimb_fstore_count", "dimb_fstore_get",
     "dimb_fstore_feats_dev", "dimb_fstore_block_dev", "dimb_gv_fundamental", "dimb_gv_fundamental_batch_dev", "dimb_gv_verify_dev",
     "dimb_tile_grid", "dimb_tile_cut_dev", "dimb_tile_merge_dev", "dimb_tile_views_dev", "dimb_tile_match_merge_dev",
+    "dimb_resize_area_tab", "dimb_resize_area_dev", "dimb_kpts_extent_dev", "dimb_tile_preselect_dev",
 ]
 
 
@@ -78,7 +79,7 @@ class Feats(C.Structure):
 class FeatsDev(C.Structure):
     _fields_ = [("keypoints", C.c_void_p), ("descriptors", C.c_void_p), ("n", C.c_void_p), ("n_cap", C.c_int),
                 ("desc_layout", C.c_int), ("desc_ld", C.c_int), ("size0", C.c_float), ("size1", C.c_float),
-                ("round_fp16", C.c_int), ("f16", C.c_int), ("size_dev", C.c_void_p)]
+                ("round_fp16", C.c_int), ("f16", C.c_int), ("size_dev", C.c_void_p), ("size_f32_dev", C.c_void_p)]
 
 
 class GvConf(C.Structure):
@@ -167,6 +168,11 @@ def load_library():
     lib.dimb_tile_merge_dev.argtypes = [vp, ip, vp] + [ip] * 6 + [vp, vp, vp, vp, ip, vp]
     lib.dimb_tile_views_dev.argtypes = [vp, ip, vp, ip, vp, vp, vp, vp]
     lib.dimb_tile_match_merge_dev.argtypes = [vp, ip, vp, vp, vp, vp, ip, vp, vp, ip, vp, vp, ip, vp]
+    lib.dimb_resize_area_tab.argtypes = [ip, ip, vp, vp, vp, ip, C.POINTER(ip)]
+    lib.dimb_resize_area_dev.argtypes = [vp, vp, ip, ip, ip, vp, ip, ip, vp]
+    lib.dimb_kpts_extent_dev.argtypes = [vp, ip, vp, ip, vp, vp, vp]
+    lib.dimb_tile_preselect_dev.argtypes = [vp, ip, C.POINTER(FeatsDev), C.POINTER(FeatsDev), vp, vp, ip] + [ip] * 6 + \
+        [C.c_double, C.c_double, ip, vp, vp, vp]
     _lib = lib
     return lib
 
@@ -250,6 +256,16 @@ def tile_grid(height: int, width: int, tile_h: int, tile_w: int, overlap_h: int,
     rows, cols, pt, pl, sh, sw = (int(v) for v in out)
     origins = [(-pl + c * sw, -pt + r * sh) for r in range(rows) for c in range(cols)]
     return {"n_rows": rows, "n_cols": cols, "pad_top": pt, "pad_left": pl, "stride_h": sh, "stride_w": sw, "origins": origins}
+
+
+def resize_area_tab(ssize: int, dsize: int):
+    """The INTER_AREA table of one axis that dimb_resize_area_dev uses (dimb_resize_area_tab, no GPU needed): (d_idx int32, s_idx
+    int32, alpha float32), one entry per (destination, source) contribution in OpenCV's order."""
+    lib, cap, n = load_library(), 2 * max(int(ssize), 1), C.c_int()
+    di, si, al = np.zeros(cap, np.int32), np.zeros(cap, np.int32), np.zeros(cap, np.float32)
+    if lib.dimb_resize_area_tab(int(ssize), int(dsize), _ptr(di), _ptr(si), _ptr(al), cap, C.byref(n)) != OK:
+        raise ValueError(f"INTER_AREA downscaling needs 1 <= dsize <= ssize, got ssize {ssize}, dsize {dsize}")
+    return di[:n.value].copy(), si[:n.value].copy(), al[:n.value].copy()
 
 
 class Context:
@@ -357,6 +373,28 @@ class Context:
         v1, p1 = _int_array(view1)
         self.check(self.lib.dimb_tile_match_merge_dev(self.h, len(off) - 1, p_off, p0, p1, d_maps, map_ld, d_matches, d_n_matches, cap, d_out,
                                                       d_n_out, cap2, stream), "dimb_tile_match_merge_dev")
+
+    def resize_area_dev(self, d_src, B, H, W, d_dst, H2, W2, stream=0):
+        """cv2.resize(INTER_AREA) of B float32 gray device images [B][H][W] -> [B][H2][W2], downscaling only (dimb_resize_area_dev);
+        asynchronous on `stream`."""
+        self.check(self.lib.dimb_resize_area_dev(self.h, d_src, B, H, W, d_dst, H2, W2, stream), "dimb_resize_area_dev")
+
+    def kpts_extent_dev(self, B, d_kpts, kpt_ld, d_counts, d_size_out, stream=0):
+        """Own-extent normalisation size (1 + max) - min per axis of B keypoint sets [B][kpt_ld][2] -> d_size_out [B][2] float32
+        (dimb_kpts_extent_dev; FeatsDev.size_f32_dev takes one row); asynchronous on `stream`."""
+        self.check(self.lib.dimb_kpts_extent_dev(self.h, B, d_kpts, kpt_ld, d_counts, d_size_out, stream), "dimb_kpts_extent_dev")
+
+    def tile_preselect_dev(self, f0: list, f1: list, d_matches, d_n_matches, cap, H, W, tile_h, tile_w, overlap_h, overlap_w, scale0, scale1,
+                           min_matches_per_tile, d_counts, d_flags, stream=0):
+        """PRESELECTION's box count for len(f0) image pairs (dimb_tile_preselect_dev): low-resolution match tables [Q][cap][2] int64 over
+        the keypoints of f0[q] / f1[q] (FeatsDev) -> d_counts [Q][T*T] int32 and d_flags [Q][T*T] uint8 (count > min_matches_per_tile).
+        Asynchronous on `stream`."""
+        Q = len(f0)
+        a0 = (FeatsDev * Q)(*f0)
+        a1 = (FeatsDev * Q)(*f1)
+        self.check(self.lib.dimb_tile_preselect_dev(self.h, Q, a0, a1, d_matches, d_n_matches, cap, H, W, tile_h, tile_w, overlap_h, overlap_w,
+                                                    float(scale0), float(scale1), int(min_matches_per_tile), d_counts, d_flags, stream),
+                   "dimb_tile_preselect_dev")
 
     def nn_match_dev(self, d_desc0: int, n0: int, d_desc1: int, n1: int, D: int, mode: str, th: float, d_idx: int, d_dist: int,
                      d_n: int, cap: int, f16: bool = False, ld0: int = 0, ld1: int = 0, stream: int = 0):

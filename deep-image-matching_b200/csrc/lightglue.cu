@@ -38,6 +38,7 @@ struct SideIn {
   int round_fp16;
   int f16;              // keypoints / descriptors are __half arrays (feature store blocks)
   const int* size_dev;  // device [H, W] (overrides size0 / size1)
+  const float* size_f32;  // device float[2] (overrides size_dev / size0 / size1)
 };
 
 __device__ __forceinline__ float maybe_round(float v, int r16) { return r16 ? __half2float(__float2half_rn(v)) : v; }
@@ -95,7 +96,8 @@ __global__ void lg_prep_kernel(const SideIn* __restrict__ in, const float* __res
     __syncthreads();
   }
   // normalize_keypoints (lightglue.py:24-34) + LearnableFourierPositionalEncoding (:57-70)
-  const float sz0 = si.size_dev ? static_cast<float>(si.size_dev[0]) : si.size0, sz1 = si.size_dev ? static_cast<float>(si.size_dev[1]) : si.size1;
+  float sz0 = si.size_dev ? static_cast<float>(si.size_dev[0]) : si.size0, sz1 = si.size_dev ? static_cast<float>(si.size_dev[1]) : si.size1;
+  if (si.size_f32) sz0 = si.size_f32[0], sz1 = si.size_f32[1];
   const float shift0 = sz0 / 2.f, shift1 = sz1 / 2.f, scale = fmaxf(sz0, sz1) / 2.f;
   for (int k = ty; k < 32; k += 8) {
     const int tok = t0 + k;
@@ -865,6 +867,7 @@ int dimb_lg_match_dev(dimb_lg* lg, int P, const dimb_feats_dev* f0, const dimb_f
       s.round_fp16 = f.round_fp16;
       s.f16 = f.f16;
       s.size_dev = f.size_dev;
+      s.size_f32 = f.size_f32_dev;
       if (f.n_cap > NP) {
         dimb_set_error(ctx, "dimb_lg_match: more keypoints than max_kpts given at create time");
         return DIMB_ERR_ARG;

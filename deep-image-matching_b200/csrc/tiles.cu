@@ -13,6 +13,8 @@
 // where every record finds its output slot by binary search in the partner run.  Every source index is distinct, so the order is
 // total and the result does not depend on the launch configuration or on which other segments share the launch.
 #include <algorithm>
+#include <cmath>
+#include <cstring>
 #include <vector>
 
 #include "fstore.cuh"
@@ -23,6 +25,8 @@ constexpr int kMaxTiles = 2048;        // tile_idx is stored as float16: integer
 constexpr int kChunk = 1024;           // records per shared-memory sort
 constexpr int kScanThreads = 1024;     // threads of the one-CTA-per-segment scans
 constexpr int kSlotKeysA = 64, kSlotKeysB = 65, kSlotParams = 66, kSlotSrc = 67, kSlotCount = 68;  // context scratch slots
+constexpr int kSlotResizeTab = 69, kSlotPreSides = 70;
+constexpr int kCvFloatLanes = 4;        // float32 lanes of OpenCV's 128-bit baseline SIMD (ResizeAreaFastVec_SIMD_32f)
 constexpr unsigned long long kNoKey = ~0ull;
 constexpr int kBorder = 2;             // border_thr of extractor_base.py:335
 
@@ -319,6 +323,156 @@ struct MatchEmit {
   __device__ void count(int q, int c) const { n[q] = c; }
 };
 
+// ---------------------------------------------------------------------------------------------------------------- preselection
+// OpenCV's computeResizeAreaTab (imgproc/src/resize.cpp) for one axis, cn = 1: every weight in double, stored as float.
+void area_tab(int ssize, int dsize, std::vector<int>* di, std::vector<int>* si, std::vector<float>* alpha) {
+  const double scale = 1.0 / (static_cast<double>(dsize) / ssize);
+  auto push = [&](int d, int s, float a) { di->push_back(d), si->push_back(s), alpha->push_back(a); };
+  for (int dx = 0; dx < dsize; ++dx) {
+    const double fsx1 = dx * scale, fsx2 = fsx1 + scale;
+    const double cell = std::min(scale, ssize - fsx1);
+    int sx1 = static_cast<int>(std::ceil(fsx1)), sx2 = static_cast<int>(std::floor(fsx2));
+    sx2 = std::min(sx2, ssize - 1);
+    sx1 = std::min(sx1, sx2);
+    if (sx1 - fsx1 > 1e-3) push(dx, sx1 - 1, static_cast<float>((sx1 - fsx1) / cell));
+    for (int sx = sx1; sx < sx2; ++sx) push(dx, sx, static_cast<float>(1.0 / cell));
+    if (fsx2 - sx2 > 1e-3) push(dx, sx2, static_cast<float>(std::min(std::min(fsx2 - sx2, 1.), cell) / cell));
+  }
+}
+
+// cv::resize's is_area_fast: the factor 1 / (dsize / ssize) is an integer within DBL_EPSILON (0 otherwise).
+int area_fast_factor(int ssize, int dsize) {
+  const double scale = 1.0 / (static_cast<double>(dsize) / ssize);
+  const int i = static_cast<int>(std::lround(scale));
+  return std::abs(scale - i) < 2.220446049250313e-16 ? i : 0;
+}
+
+struct AreaTab {  // per axis: the entries of output index d are [ofs[d], ofs[d + 1]) of src / alpha, in OpenCV's order
+  const int *xofs, *xsrc, *yofs, *ysrc;
+  const float *xa, *ya;
+};
+
+// resizeArea_: per output pixel, the rows of the y-table in order; buf = sum of S * alpha in x-table order from 0; the first row sets
+// sum = beta * buf, the others add beta * buf.  Every product and sum is rounded on its own, as OpenCV's scalar code does.
+__global__ void resize_area_kernel(const float* __restrict__ src, float* __restrict__ dst, int H, int W, int H2, int W2, AreaTab t) {
+  const int dx = blockIdx.x * blockDim.x + threadIdx.x, dy = blockIdx.y, b = blockIdx.z;
+  if (dx >= W2) return;
+  const float* img = src + static_cast<size_t>(b) * H * W;
+  const int x0 = t.xofs[dx], x1 = t.xofs[dx + 1], j0 = t.yofs[dy], j1 = t.yofs[dy + 1];
+  float sum = 0.f;
+  for (int j = j0; j < j1; ++j) {
+    const float* row = img + static_cast<size_t>(t.ysrc[j]) * W;
+    float buf = 0.f;
+    for (int k = x0; k < x1; ++k) buf = __fadd_rn(buf, __fmul_rn(row[t.xsrc[k]], t.xa[k]));
+    const float v = __fmul_rn(t.ya[j], buf);
+    sum = j == j0 ? v : __fadd_rn(sum, v);
+  }
+  dst[(static_cast<size_t>(b) * H2 + dy) * W2 + dx] = sum;
+}
+
+// resizeAreaFast_ for integer factors (fy, fx): the block row-major, sum += ((a + b) + c) + d per four pixels, then sum * (1.f / area).
+// For 2 x 2 OpenCV's vector loop (ResizeAreaFastVec_SIMD_32f) covers the columns dx < vec_end and computes ((a + b) + (c + d)) * 0.25f;
+// the scalar loop above takes the rest of the row.
+__global__ void resize_area_fast_kernel(const float* __restrict__ src, float* __restrict__ dst, int H, int W, int H2, int W2, int fy, int fx,
+                                        int vec_end) {
+  const int dx = blockIdx.x * blockDim.x + threadIdx.x, dy = blockIdx.y, b = blockIdx.z;
+  if (dx >= W2) return;
+  const float* S = src + (static_cast<size_t>(b) * H + static_cast<size_t>(dy) * fy) * W + static_cast<size_t>(dx) * fx;
+  const int area = fy * fx;
+  auto at = [&](int k) { return S[static_cast<size_t>(k / fx) * W + k % fx]; };
+  if (dx < vec_end) {
+    dst[(static_cast<size_t>(b) * H2 + dy) * W2 + dx] = __fmul_rn(__fadd_rn(__fadd_rn(at(0), at(1)), __fadd_rn(at(2), at(3))), 0.25f);
+    return;
+  }
+  float sum = 0.f;
+  int k = 0;
+  for (; k <= area - 4; k += 4) sum = __fadd_rn(sum, __fadd_rn(__fadd_rn(__fadd_rn(at(k), at(k + 1)), at(k + 2)), at(k + 3)));
+  for (; k < area; ++k) sum = __fadd_rn(sum, at(k));
+  dst[(static_cast<size_t>(b) * H2 + dy) * W2 + dx] = __fmul_rn(sum, __fdiv_rn(1.f, static_cast<float>(area)));
+}
+
+// One CTA per image: size = (1 + max) - min per axis over its keypoints, {1, 1} without keypoints (min / max are exact in any order).
+__global__ void __launch_bounds__(256) kpts_extent_kernel(const float* __restrict__ kpts, int ld, const int* __restrict__ counts,
+                                                          float* __restrict__ out) {
+  __shared__ float red[4][8];
+  const int b = blockIdx.x, n = min(max(counts[b], 0), ld);
+  const float2* k = reinterpret_cast<const float2*>(kpts) + static_cast<size_t>(b) * ld;
+  float mn0 = INFINITY, mn1 = INFINITY, mx0 = -INFINITY, mx1 = -INFINITY;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float2 p = k[i];
+    mn0 = fminf(mn0, p.x), mx0 = fmaxf(mx0, p.x), mn1 = fminf(mn1, p.y), mx1 = fmaxf(mx1, p.y);
+  }
+  for (int o = 16; o; o >>= 1) {
+    mn0 = fminf(mn0, __shfl_xor_sync(0xffffffffu, mn0, o)), mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, o));
+    mn1 = fminf(mn1, __shfl_xor_sync(0xffffffffu, mn1, o)), mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, o));
+  }
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  if (lane == 0) red[0][w] = mn0, red[1][w] = mx0, red[2][w] = mn1, red[3][w] = mx1;
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  for (int i = 1; i < 8; ++i) mn0 = fminf(mn0, red[0][i]), mx0 = fmaxf(mx0, red[1][i]), mn1 = fminf(mn1, red[2][i]), mx1 = fmaxf(mx1, red[3][i]);
+  out[2 * b] = n ? __fsub_rn(__fadd_rn(1.f, mx0), mn0) : 1.f;
+  out[2 * b + 1] = n ? __fsub_rn(__fadd_rn(1.f, mx1), mn1) : 1.f;
+}
+
+struct PreSide {  // keypoints of one side of one pair (dimb_feats_dev's keypoints / f16 / round_fp16)
+  const void* kpts;
+  int f16, round_fp16;
+};
+
+__device__ __forceinline__ float pre_kpt(const PreSide& s, int64_t i) {
+  if (s.f16) return __half2float(static_cast<const __half*>(s.kpts)[i]);
+  const float v = static_cast<const float*>(s.kpts)[i];
+  return s.round_fp16 ? __half2float(__float2half_rn(v)) : v;
+}
+
+// The tiles along one axis whose open interval (origin, origin + size) holds v: a float estimate widened by one on both sides, then
+// the exact test on every candidate (origins are integers below 2^21, exact in float).
+__device__ __forceinline__ void axis_cover(float v, int pad, int step, int size, int n, int& lo, int& hi) {
+  const float u = v + static_cast<float>(pad);
+  lo = max(0, static_cast<int>(floorf((u - static_cast<float>(size)) / static_cast<float>(step))) - 1);
+  hi = min(n - 1, static_cast<int>(floorf(u / static_cast<float>(step))) + 1);
+}
+
+__device__ __forceinline__ bool in_open(float v, int o, int size) { return v > static_cast<float>(o) && v < static_cast<float>(o + size); }
+
+// grid (cap / 128, Q): one thread per match row; +1 for every (t0, t1) whose boxes both hold the row's full-resolution points.
+__global__ void tile_preselect_count_kernel(const PreSide* __restrict__ sides, const int64_t* __restrict__ matches, const int* __restrict__ n_matches,
+                                            int cap, Grid g, float sc0, float sc1, int* __restrict__ counts) {
+  const int q = blockIdx.y, r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= min(n_matches[q], cap)) return;
+  const int64_t* m = matches + (static_cast<size_t>(q) * cap + r) * 2;
+  const PreSide s0 = sides[2 * q], s1 = sides[2 * q + 1];
+  const float x0 = __fdiv_rn(pre_kpt(s0, 2 * m[0]), sc0), y0 = __fdiv_rn(pre_kpt(s0, 2 * m[0] + 1), sc0);
+  const float x1 = __fdiv_rn(pre_kpt(s1, 2 * m[1]), sc1), y1 = __fdiv_rn(pre_kpt(s1, 2 * m[1] + 1), sc1);
+  constexpr float kFar = 4194304.f;  // 2^22: beyond every box (image and tile sides are below 2^20 / 2^14), and keeps the estimates in int
+  if (!(fabsf(x0) < kFar && fabsf(y0) < kFar && fabsf(x1) < kFar && fabsf(y1) < kFar)) return;
+  const int T = g.tiles();
+  int* c = counts + static_cast<size_t>(q) * T * T;
+  int r0lo, r0hi, c0lo, c0hi, r1lo, r1hi, c1lo, c1hi;
+  axis_cover(y0, g.pad_top, g.sy, g.th, g.rows, r0lo, r0hi);
+  axis_cover(x0, g.pad_left, g.sx, g.tw, g.cols, c0lo, c0hi);
+  axis_cover(y1, g.pad_top, g.sy, g.th, g.rows, r1lo, r1hi);
+  axis_cover(x1, g.pad_left, g.sx, g.tw, g.cols, c1lo, c1hi);
+  for (int ra = r0lo; ra <= r0hi; ++ra) {
+    if (!in_open(y0, -g.pad_top + ra * g.sy, g.th)) continue;
+    for (int ca = c0lo; ca <= c0hi; ++ca) {
+      if (!in_open(x0, -g.pad_left + ca * g.sx, g.tw)) continue;
+      const int t0 = ra * g.cols + ca;
+      for (int rb = r1lo; rb <= r1hi; ++rb) {
+        if (!in_open(y1, -g.pad_top + rb * g.sy, g.th)) continue;
+        for (int cb = c1lo; cb <= c1hi; ++cb)
+          if (in_open(x1, -g.pad_left + cb * g.sx, g.tw)) atomicAdd(c + static_cast<size_t>(t0) * T + rb * g.cols + cb, 1);
+      }
+    }
+  }
+}
+
+__global__ void tile_preselect_flag_kernel(const int* __restrict__ counts, size_t n, int min_matches, unsigned char* __restrict__ flags) {
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    flags[i] = counts[i] > min_matches;
+}
+
 }  // namespace
 
 extern "C" {
@@ -442,6 +596,112 @@ int dimb_tile_match_merge_dev(dimb_ctx* ctx, int Q, const int* pair_offsets, con
     DIMB_TRY(seg_sort(ctx, st, ra, rb, Q, Li, &sorted));
   }
   seg_unique_kernel<<<Q, kScanThreads, 0, st>>>(Li > 0 ? sorted : ra, Li, MatchEmit{d_out, d_n_out, cap2});
+  DIMB_LAUNCH_CHECK(ctx);
+  return DIMB_OK;
+}
+
+int dimb_resize_area_tab(int ssize, int dsize, int* d_idx, int* s_idx, float* alpha, int cap, int* n) {
+  if (!n || ssize < 1 || dsize < 1 || dsize > ssize || cap < 0 || (cap > 0 && (!d_idx || !s_idx || !alpha))) return DIMB_ERR_ARG;
+  std::vector<int> di, si;
+  std::vector<float> a;
+  area_tab(ssize, dsize, &di, &si, &a);
+  *n = static_cast<int>(di.size());
+  if (*n > cap) return DIMB_ERR_CAPACITY;
+  std::copy(di.begin(), di.end(), d_idx);
+  std::copy(si.begin(), si.end(), s_idx);
+  std::copy(a.begin(), a.end(), alpha);
+  return DIMB_OK;
+}
+
+int dimb_resize_area_dev(dimb_ctx* ctx, const float* d_src, int B, int height, int width, float* d_dst, int height2, int width2, void* stream) {
+  if (!ctx || !d_src || !d_dst || B < 1 || B > 65535 || height < 1 || width < 1 || height > (1 << 20) || width > (1 << 20) || height2 < 1 ||
+      width2 < 1 || height2 > height || width2 > width || height2 > 65535)
+    return DIMB_ERR_ARG;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (height2 == height && width2 == width) {
+    ProfScope prof(ctx, st, "tile.resize");
+    DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_dst, d_src, static_cast<size_t>(B) * height * width * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return DIMB_OK;
+  }
+  const dim3 grid(ceil_div(width2, 128), height2, B);
+  const int fy = area_fast_factor(height, height2), fx = area_fast_factor(width, width2);
+  if (fy && fx) {
+    // OpenCV's baseline build vectorises float rows 128 bits (4 lanes) wide; only 2 x 2 has a vector loop
+    const int vec_end = fy == 2 && fx == 2 ? width2 / kCvFloatLanes * kCvFloatLanes : 0;
+    ProfScope prof(ctx, st, "tile.resize");
+    resize_area_fast_kernel<<<grid, 128, 0, st>>>(d_src, d_dst, height, width, height2, width2, fy, fx, vec_end);
+    DIMB_LAUNCH_CHECK(ctx);
+    return DIMB_OK;
+  }
+  // one upload: x offsets [W2 + 1], x sources, y offsets [H2 + 1], y sources, then the x and y weights (float bits)
+  std::vector<int> xd, xs, yd, ys;
+  std::vector<float> xa, ya;
+  area_tab(width, width2, &xd, &xs, &xa);
+  area_tab(height, height2, &yd, &ys, &ya);
+  auto offsets = [](const std::vector<int>& d, int n) {
+    std::vector<int> o(n + 1, 0);
+    for (int v : d) ++o[v + 1];
+    for (int i = 0; i < n; ++i) o[i + 1] += o[i];
+    return o;
+  };
+  std::vector<int> hp = offsets(xd, width2);
+  const size_t o_xs = hp.size();
+  hp.insert(hp.end(), xs.begin(), xs.end());
+  const size_t o_yofs = hp.size();
+  const std::vector<int> yo = offsets(yd, height2);
+  hp.insert(hp.end(), yo.begin(), yo.end());
+  const size_t o_ys = hp.size();
+  hp.insert(hp.end(), ys.begin(), ys.end());
+  const size_t o_xa = hp.size();
+  hp.resize(o_xa + xa.size() + ya.size());
+  std::memcpy(hp.data() + o_xa, xa.data(), xa.size() * sizeof(float));
+  std::memcpy(hp.data() + o_xa + xa.size(), ya.data(), ya.size() * sizeof(float));
+  int* d_tab;
+  DIMB_TRY(dimb_scratch(ctx, kSlotResizeTab, hp.size() * sizeof(int), reinterpret_cast<void**>(&d_tab)));
+  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_tab, hp.data(), hp.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  const AreaTab t{d_tab, d_tab + o_xs, d_tab + o_yofs, d_tab + o_ys, reinterpret_cast<const float*>(d_tab + o_xa),
+                  reinterpret_cast<const float*>(d_tab + o_xa + xa.size())};
+  ProfScope prof(ctx, st, "tile.resize");
+  resize_area_kernel<<<grid, 128, 0, st>>>(d_src, d_dst, height, width, height2, width2, t);
+  DIMB_LAUNCH_CHECK(ctx);
+  return DIMB_OK;
+}
+
+int dimb_kpts_extent_dev(dimb_ctx* ctx, int B, const float* d_kpts, int kpt_ld, const int* d_counts, float* d_size_out, void* stream) {
+  if (!ctx || !d_kpts || !d_counts || !d_size_out || B < 1 || kpt_ld < 1) return DIMB_ERR_ARG;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope prof(ctx, st, "tile.extent");
+  kpts_extent_kernel<<<B, 256, 0, st>>>(d_kpts, kpt_ld, d_counts, d_size_out);
+  DIMB_LAUNCH_CHECK(ctx);
+  return DIMB_OK;
+}
+
+int dimb_tile_preselect_dev(dimb_ctx* ctx, int Q, const dimb_feats_dev* f0, const dimb_feats_dev* f1, const int64_t* d_matches,
+                            const int* d_n_matches, int cap, int height, int width, int tile_h, int tile_w, int overlap_h, int overlap_w,
+                            double scale0, double scale1, int min_matches_per_tile, int* d_counts, unsigned char* d_flags, void* stream) {
+  Grid g;
+  if (!ctx || !f0 || !f1 || !d_matches || !d_n_matches || !d_counts || !d_flags || Q < 1 || Q > 65535 || cap < 1 ||
+      !make_grid(height, width, tile_h, tile_w, overlap_h, overlap_w, &g) || min_matches_per_tile < 0)
+    return DIMB_ERR_ARG;
+  const float sc0 = static_cast<float>(scale0), sc1 = static_cast<float>(scale1);  // numpy: float32 array / Python float in float32
+  if (!(std::isfinite(sc0) && sc0 > 0.f && std::isfinite(sc1) && sc1 > 0.f)) return DIMB_ERR_ARG;
+  std::vector<PreSide> hp(2 * Q);
+  for (int q = 0; q < Q; ++q) {
+    if (!f0[q].keypoints || !f1[q].keypoints) return DIMB_ERR_ARG;
+    hp[2 * q] = PreSide{f0[q].keypoints, f0[q].f16, f0[q].round_fp16};
+    hp[2 * q + 1] = PreSide{f1[q].keypoints, f1[q].f16, f1[q].round_fp16};
+  }
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t n = static_cast<size_t>(Q) * g.tiles() * g.tiles();
+  PreSide* d_sides;
+  DIMB_TRY(dimb_scratch(ctx, kSlotPreSides, hp.size() * sizeof(PreSide), reinterpret_cast<void**>(&d_sides)));
+  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_sides, hp.data(), hp.size() * sizeof(PreSide), cudaMemcpyHostToDevice, st));
+  ProfScope prof(ctx, st, "tile.preselect");
+  DIMB_CUDA_OK(ctx, cudaMemsetAsync(d_counts, 0, n * sizeof(int), st));
+  tile_preselect_count_kernel<<<dim3(ceil_div(cap, 128), Q), 128, 0, st>>>(d_sides, d_matches, d_n_matches, cap, g, sc0, sc1, d_counts);
+  DIMB_LAUNCH_CHECK(ctx);
+  tile_preselect_flag_kernel<<<static_cast<int>(std::min<size_t>((n + 255) / 256, 4096)), 256, 0, st>>>(d_counts, n, min_matches_per_tile,
+                                                                                                    d_flags);
   DIMB_LAUNCH_CHECK(ctx);
   return DIMB_OK;
 }

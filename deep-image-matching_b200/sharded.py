@@ -208,20 +208,23 @@ def verification_conf(verification) -> dict | None:
     return conf
 
 
-TILE_SELECTIONS = ("grid", "exhaustive")
+TILE_SELECTIONS = ("grid", "exhaustive", "preselection")
+TILING_KEYS = ("min_matches_per_tile", "tile_overlap", "tile_preselection_size", "tile_selection", "tile_size")
 
 
 def tiling_conf(tiling) -> dict | None:
     """The ``tiling`` argument of ImageSetMatcher, validated (None stays None).  Keys as in the reference's configuration:
-    ``tile_size`` (x, y) or one int (required), ``tile_overlap`` int (default 0) and ``tile_selection`` "grid" (default) or
-    "exhaustive".  The returned dict adds ``tile_hw`` / ``overlap_hw``, the (H, W) order ``tiling._hw`` gives them.  Preselection is
-    not a configured mode here: pass its tile-pair lists to ``match`` / ``run`` as ``tile_pairs``."""
+    ``tile_size`` (x, y) or one int (required), ``tile_overlap`` int (default 0) and ``tile_selection`` "grid" (default),
+    "exhaustive" or "preselection".  Preselection also needs ``tile_preselection_size`` (positive int: the longest side of the
+    down-sampled images, no default) and takes ``min_matches_per_tile`` (int >= 0, default 5, tiling.tile_selection's); grid and
+    exhaustive accept and ignore both.  The returned dict adds ``tile_hw`` / ``overlap_hw``, the (H, W) order ``tiling._hw`` gives
+    them."""
     if tiling is None:
         return None
     from .tiling import _hw
-    unknown = set(tiling) - {"tile_size", "tile_overlap", "tile_selection"}
+    unknown = set(tiling) - set(TILING_KEYS)
     if unknown:
-        raise ValueError(f"unknown tiling option(s) {sorted(unknown)}; expected some of ['tile_overlap', 'tile_selection', 'tile_size']")
+        raise ValueError(f"unknown tiling option(s) {sorted(unknown)}; expected some of {list(TILING_KEYS)}")
     if "tile_size" not in tiling:
         raise ValueError("tiling needs tile_size")
     size, overlap = tiling["tile_size"], tiling.get("tile_overlap", 0)
@@ -232,9 +235,17 @@ def tiling_conf(tiling) -> dict | None:
     if not isinstance(overlap, int) or not 0 <= overlap < min(_hw(size)):
         raise ValueError(f"tile_overlap must be an int in [0, min(tile_size)), got {overlap!r}")
     if sel not in TILE_SELECTIONS:
-        raise ValueError(f"tile_selection must be one of {TILE_SELECTIONS} (preselection: pass tile_pairs), got {tiling.get('tile_selection')!r}")
-    return {"tile_size": size if isinstance(size, int) else tuple(size), "tile_overlap": overlap, "tile_selection": sel,
-            "tile_hw": _hw(size), "overlap_hw": _hw(overlap)}
+        raise ValueError(f"tile_selection must be one of {TILE_SELECTIONS}, got {tiling.get('tile_selection')!r}")
+    out = {"tile_size": size if isinstance(size, int) else tuple(size), "tile_overlap": overlap, "tile_selection": sel,
+           "tile_hw": _hw(size), "overlap_hw": _hw(overlap)}
+    if sel == "preselection":
+        pre, mm = tiling.get("tile_preselection_size"), tiling.get("min_matches_per_tile", 5)
+        if isinstance(pre, bool) or not isinstance(pre, int) or pre < 1:
+            raise ValueError(f"tile_selection \"preselection\" needs tile_preselection_size, a positive int, got {pre!r}")
+        if isinstance(mm, bool) or not isinstance(mm, int) or mm < 0:
+            raise ValueError(f"min_matches_per_tile must be an int >= 0, got {mm!r}")
+        out.update(tile_preselection_size=pre, min_matches_per_tile=mm)
+    return out
 
 
 def tile_pairs_for(selection: str, n_tiles: int) -> list:
@@ -289,12 +300,20 @@ class ImageSetMatcher:
     T * K).  ``exchange`` also builds the per-tile views of every image.  ``match`` / ``match_verified`` pack whole image pairs into
     matcher batches of at most ``batch_pairs`` tile pairs, match the selected tile pairs out of the views and return one merged,
     de-duplicated table per image pair in merged-slot rows; verification and ``export_colmap`` run on the merged slots.  ``tile_pairs``
-    (per image pair, a list of (t0, t1)) overrides the configured selection, e.g. with PRESELECTION lists computed on the host by
-    ``tiling.preselection_matches`` + ``tiling.tile_selection``."""
+    (per image pair, a list of (t0, t1)) overrides the configured selection.
+
+    ``tile_selection: "preselection"`` computes every pair's list on the device, equal to ``tiling.preselection_matches`` +
+    ``tiling.tile_selection``: ``extract`` also down-samples each image once (INTER_AREA, longest side ``tile_preselection_size``)
+    and runs SuperPoint (``tiling.SP_PRESELECTION_CONF``) into float32 per-slot buffers (about 4.2 MB per image, all-gathered by
+    ``exchange``); ``match`` runs LightGlue (``tiling.LG_PRESELECTION_CONF``, keypoints normalised by their own extent) on the
+    low-resolution features of each pair batch and keeps the tile pairs with more than ``min_matches_per_tile`` matches inside both
+    boxes.  ``preselection_weights``: the weights of that LightGlue (default ``lg_weights``; required with SuperGlue).  SuperPoint
+    only: ALIKED with preselection is refused.  The per-pair flags of one ``match`` call take T^2 bytes per pair on the device and
+    on the host (``_preselect``), which matters only at hundreds of tiles per image."""
 
     def __init__(self, ctx, sp_weights: dict, lg_weights: dict, n_images: int, height: int, width: int, sp_conf: dict, lg_conf: dict,
                  batch_images: int = 16, batch_pairs: int = 32, dist=None, matcher: str = "lightglue", verification: dict | None = None,
-                 tiling: dict | None = None, extractor: str = "superpoint"):
+                 tiling: dict | None = None, extractor: str = "superpoint", preselection_weights: dict | None = None):
         import torch
 
         from . import _native
@@ -305,6 +324,21 @@ class ImageSetMatcher:
         if extractor == "aliked" and matcher == "superglue":
             raise ValueError("SuperGlue matches SuperPoint features only; use matcher=\"lightglue\" with ALIKED")
         self.tiling = tiling_conf(tiling)
+        self.presel = self.tiling is not None and self.tiling["tile_selection"] == "preselection"
+        if self.presel:
+            if extractor == "aliked":
+                raise ValueError("tile preselection runs on gray images and is available with extractor=\"superpoint\" only; "
+                                 "pass tile_pairs with ALIKED")
+            if self.tiling["tile_preselection_size"] > max(height, width):
+                raise ValueError(f"tile_preselection_size {self.tiling['tile_preselection_size']} exceeds the image's longest side "
+                                 f"{max(height, width)}: preselection only downscales")
+            if matcher == "superglue" and preselection_weights is None:
+                raise ValueError("tile preselection with matcher=\"superglue\" needs preselection_weights (SuperPoint-LightGlue weights)")
+            # the down-sampled size exactly as tiling.preselection_matches computes it
+            self.pre_scale = self.tiling["tile_preselection_size"] / max(height, width)
+            self.pre_w, self.pre_h = (int(round(x * self.pre_scale)) for x in (width, height))
+            if min(self.pre_h, self.pre_w) < 1:
+                raise ValueError(f"tile_preselection_size {self.tiling['tile_preselection_size']} down-samples a {height}x{width} image to nothing")
         if self.tiling is not None and extractor == "superpoint":
             if "fix_sampling" in sp_conf and not sp_conf["fix_sampling"]:
                 raise ValueError("tiled SuperPoint extraction runs with fix_sampling=True (the reference's rule); fix_sampling=False was given")
@@ -365,6 +399,28 @@ class ImageSetMatcher:
             self.cap2 = gv_cap = min(batch_pairs, self.T * self.T) * self.cap
             self.mm = torch.zeros(batch_pairs, self.cap2, 2, dtype=torch.int64, device=dev)
             self.nmm = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
+        if self.presel:
+            # PRESELECTION (matcher_base.py:1055-1089) on the device: the networks of matcher_base.py:143-159, float32 low-resolution
+            # features per store slot (they never pass through features.h5 in the reference: no float16 cast), their own-extent size
+            # for LightGlue without image_size, and the outputs of one pair batch
+            from .tiling import LG_PRESELECTION_CONF, SP_PRESELECTION_CONF
+            K = self.pre_k = SP_PRESELECTION_CONF["max_keypoints"]
+            S = self.world * self.ipr
+            self.sp_pre = _native.SuperPointNet(ctx, sp_weights, max_batch=batch_images, max_height=self.pre_h, max_width=self.pre_w,
+                                                **SP_PRESELECTION_CONF)
+            self.lg_pre = _native.LightGlueNet(ctx, lg_weights if preselection_weights is None else preselection_weights,
+                                               max_pairs=batch_pairs, max_kpts=K, **LG_PRESELECTION_CONF)
+            self.low = torch.zeros(batch_images, self.pre_h, self.pre_w, device=dev)
+            self.pre_sc = torch.zeros(batch_images, K, device=dev)  # written by the extractor, not read by preselection
+            self.pre_kp = torch.zeros(S, K, 2, device=dev)
+            self.pre_de = torch.zeros(S, 256, K, device=dev)
+            self.pre_n = torch.zeros(S, dtype=torch.int32, device=dev)
+            self.pre_size = torch.zeros(S, 2, device=dev)
+            self.pre_m = torch.zeros(batch_pairs, K, 2, dtype=torch.int64, device=dev)
+            self.pre_ms = torch.zeros(batch_pairs, K, device=dev)
+            self.pre_nm = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
+            self.pre_sl = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
+            self.pre_cnt = torch.zeros(batch_pairs, self.T * self.T, dtype=torch.int32, device=dev)
         self.gv = verification_conf(verification)
         if self.gv is not None and self.gv["method"] != "NONE":  # verification outputs of one pair batch + pinned host copies
             self.v = torch.zeros(batch_pairs, gv_cap, 2, dtype=torch.int64, device=dev)
@@ -388,6 +444,8 @@ class ImageSetMatcher:
         (k, H, W, 3) RGB for ALIKED.  With tiling the images are full size and are cut into tiles on the device."""
         st = self.torch.cuda.current_stream().cuda_stream
         if self.tiling is not None:
+            if self.presel:
+                self._extract_preselection(d_images, image_ids, st)
             return self._extract_tiled(d_images, image_ids, st)
         if self.extractor == "aliked":
             for k, i in enumerate(image_ids):
@@ -404,6 +462,26 @@ class ImageSetMatcher:
             for k, i in enumerate(ids):
                 self.store.put_dev(store_slot(i, self.n, self.world), self.kp[k].data_ptr(), self.sc[k].data_ptr(), self.de[k].data_ptr(),
                                    self.cap, self.cnt[k:k + 1].data_ptr(), self.H, self.W, None, st)
+
+    def _extract_preselection(self, d_images, image_ids, st):
+        """PRESELECTION's low-resolution extraction, once per image: INTER_AREA down-sampling, SuperPoint into the image's slot rows of
+        the float32 preselection buffers, and the own extent of its keypoints."""
+        K = self.pre_k
+        for b0 in range(0, len(image_ids), self.B):
+            ids = image_ids[b0:b0 + self.B]
+            self.ctx.resize_area_dev(d_images[b0:b0 + len(ids)].data_ptr(), len(ids), self.H, self.W, self.low.data_ptr(), self.pre_h,
+                                     self.pre_w, st)
+            slots = [store_slot(i, self.n, self.world) for i in ids]
+            k = 0
+            while k < len(ids):  # the extractor writes consecutive rows: one call per run of consecutive slots
+                e = k + 1
+                while e < len(ids) and slots[e] == slots[k] + (e - k):
+                    e += 1
+                s = slots[k]
+                self.sp_pre.extract_dev(self.low[k].data_ptr(), e - k, self.pre_h, self.pre_w, self.pre_kp[s].data_ptr(), self.pre_sc[k].data_ptr(),
+                                        self.pre_de[s].data_ptr(), self.pre_n[s:].data_ptr(), K, st)
+                self.ctx.kpts_extent_dev(e - k, self.pre_kp[s].data_ptr(), K, self.pre_n[s:].data_ptr(), self.pre_size[s].data_ptr(), st)
+                k = e
 
     def _extract_tiled(self, d_images, image_ids, st):
         """Groups of G images: tile cut, the extractor over their G * T tiles, one tile merge into their slots."""
@@ -429,6 +507,9 @@ class ImageSetMatcher:
         """The collective of the path: every rank's float16 feature blocks to every rank (NCCL all_gather over NVLink).  With tiling,
         every rank then builds the per-tile views of all images from the merged slots."""
         self.exchanged_bytes = all_gather_blocks(self.store_t, self.n, self.dist)
+        if self.presel:  # the low-resolution features of every image, for the preselection of any pair
+            for t in (self.pre_kp, self.pre_de, self.pre_n, self.pre_size):
+                self.exchanged_bytes += all_gather_blocks(t.view(self.torch.uint8).view(t.shape[0], -1), self.n, self.dist)
         if self.tiling is not None:
             st = self.torch.cuda.current_stream().cuda_stream
             step = max(1, 65535 // self.T)
@@ -451,8 +532,37 @@ class ImageSetMatcher:
         self._match_slots(self.store, [store_slot(i, self.n, self.world) for i, _ in chunk],
                           [store_slot(j, self.n, self.world) for _, j in chunk], st)
 
+    def _pre_feats(self, slot):
+        """The float32 low-resolution features of a slot as LightGlue input, normalised by their own extent."""
+        from . import _native
+        K = self.pre_k
+        return _native.FeatsDev(self.pre_kp[slot].data_ptr(), self.pre_de[slot].data_ptr(), self.pre_n[slot:].data_ptr(), K, 0, K, 0.0, 0.0,
+                                0, 0, None, self.pre_size[slot].data_ptr())
+
+    def _preselect(self, pairs):
+        """PRESELECTION tile-pair lists of `pairs` (tiling.preselection_matches + tiling.tile_selection): per batch of batch_pairs,
+        LightGlue on the low-resolution slots and the tile box count, then ONE device->host copy of every pair's flags.  Row-major
+        flags give the lists sorted.  Memory: the flags take len(pairs) * T^2 bytes on the device and again on the host, and the
+        counts of one batch (allocated with the matcher) batch_pairs * T^2 int32; at T in the tens that is kilobytes per pair, but at
+        hundreds of tiles per image it reaches megabytes per pair, so a very large pair list is better matched in several calls."""
+        st = self.torch.cuda.current_stream().cuda_stream
+        T, K = self.T, self.pre_k
+        (th, tw), (oh, ow) = self.tiling["tile_hw"], self.tiling["overlap_hw"]
+        flags = self.torch.zeros(max(len(pairs), 1), T * T, dtype=self.torch.uint8, device=self.pre_cnt.device)
+        for b0 in range(0, len(pairs), self.P):
+            chunk = pairs[b0:b0 + self.P]
+            f0 = [self._pre_feats(store_slot(i, self.n, self.world)) for i, _ in chunk]
+            f1 = [self._pre_feats(store_slot(j, self.n, self.world)) for _, j in chunk]
+            self.lg_pre.match_dev(f0, f1, self.pre_m.data_ptr(), self.pre_ms.data_ptr(), self.pre_nm.data_ptr(), self.pre_sl.data_ptr(), K, st)
+            self.ctx.tile_preselect_dev(f0, f1, self.pre_m.data_ptr(), self.pre_nm.data_ptr(), K, self.H, self.W, th, tw, oh, ow, self.pre_scale,
+                                        self.pre_scale, self.tiling["min_matches_per_tile"], self.pre_cnt.data_ptr(), flags[b0].data_ptr(), st)
+        fl = flags[:len(pairs)].cpu().numpy().reshape(-1, T, T)
+        return [[(int(a), int(b)) for a, b in zip(*np.nonzero(f))] for f in fl]
+
     def _tile_pair_lists(self, pairs, tile_pairs):
         if tile_pairs is None:
+            if self.presel:
+                return self._preselect(pairs)
             return [tile_pairs_for(self.tiling["tile_selection"], self.T)] * len(pairs)
         if len(tile_pairs) != len(pairs):
             raise ValueError(f"tile_pairs must hold one list per image pair: {len(tile_pairs)} lists for {len(pairs)} pairs")

@@ -6,6 +6,8 @@ Only the geometry is restated (it is pure numpy in the reference too, apart from
 PRESELECTION mode runs on the down-sampled images - SuperPoint (hloc wrapper: ``fix_sampling=True``, ``nms_radius 5``,
 ``max_keypoints 4000``, ``keypoint_threshold 0.005``) and LightGlue (``depth 0.9 / width 0.95 / filter 0.3``, keypoints
 normalised by their own extent because ``sp2lg`` passes no ``image_size``) ``matcher_base.py:143-159`` - run on libdimb200.
+This host flow is the reference restated; ``ImageSetMatcher(tiling={..., "tile_selection": "preselection"})`` computes the same
+lists on the device (``dimb_resize_area_dev``, ``dimb_kpts_extent_dev``, ``dimb_tile_preselect_dev``).
 
 Reproduced quirk (SURVEY A.7): ``kornia.contrib.compute_padding`` is called without the stride (tiling.py:124), so the
 padding assumes stride == window while the tiles are cut with stride ``window - overlap``: with an overlap the last

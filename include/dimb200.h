@@ -153,6 +153,8 @@ typedef struct {
   int round_fp16;           /* 1: round keypoints/descriptors to fp16 first, as the features.h5 round trip does */
   int f16;                  /* 1: keypoints and descriptors ARE float16 arrays (device feature store blocks); round_fp16 is moot */
   const int* size_dev;      /* non-NULL: device int[2] holding image_size ([H,W]); overrides size0 / size1 */
+  const float* size_f32_dev; /* non-NULL: device float[2] used as the normalisation size as is (e.g. dimb_kpts_extent_dev's
+                                own-extent size); overrides size0 / size1 / size_dev */
 } dimb_feats_dev;
 
 /* Device-resident variant, asynchronous on `stream`; d_matches [P][cap][2] int64, d_mscores [P][cap],
@@ -282,6 +284,41 @@ int dimb_tile_views_dev(dimb_fstore* src, int B, const int* src_slots, int n_til
  * rows are written).  An image pair without tile pairs gets 0. */
 int dimb_tile_match_merge_dev(dimb_ctx* ctx, int Q, const int* pair_offsets, const int* view0, const int* view1, const int* d_maps, int map_ld,
                               const int64_t* d_matches, const int* d_n_matches, int cap, int64_t* d_out, int* d_n_out, int cap2, void* stream);
+
+/* Tile preselection (matcher_base.py:1055-1148): the low-resolution SuperPoint + LightGlue pass that picks the tile pairs worth
+ * matching.  Same conventions as the entries above; profile groups tile.resize, tile.extent, tile.preselect.
+ *
+ * cv2.resize(img, (W2, H2), interpolation=INTER_AREA) for downscaling, OpenCV's resizeArea_ / computeResizeAreaTab: per axis
+ * scale = 1 / (dsize / ssize) in double; destination index d covers [d * scale, d * scale + scale) with a leading partial weight, full
+ * weights 1 / cellWidth and a trailing partial weight, all computed in double and stored as float.  Host only (no CUDA call): the
+ * table of one axis, entries in OpenCV's order, d_idx / s_idx / alpha of at most cap entries; *n = the entry count (<= 2 * ssize).
+ * DIMB_ERR_CAPACITY (n filled) when cap is too small; DIMB_ERR_ARG unless 1 <= dsize <= ssize. */
+int dimb_resize_area_tab(int ssize, int dsize, int* d_idx, int* s_idx, float* alpha, int cap, int* n);
+/* B float32 gray images d_src [B][H][W] -> d_dst [B][H2][W2], bitwise the value cv2.resize(INTER_AREA) gives: per output pixel,
+ * over the contributing source rows in table order, buf = sum of S[sx] * alpha in x-table order from 0, then sum = beta * buf for
+ * the first row and sum += beta * buf for the others, every product and sum rounded separately (no FMA).  H2 == H and W2 == W is a
+ * copy.  When both factors H / H2 and W / W2 are integers (within DBL_EPSILON, OpenCV's is_area_fast) OpenCV sums the
+ * sy x sx block row-major, four pixels at a time (sum += ((a + b) + c) + d), and scales by float(1 / area); that order is used too.
+ * The 2 x 2 block also has OpenCV's vector loop, ((a + b) + (c + d)) * 0.25f, over the first floor(W2 / 4) * 4 columns of each row,
+ * with the scalar order for the rest: parity is with OpenCV's 128-bit baseline SIMD width (4 float lanes).  Upscaling (OpenCV
+ * switches to a bilinear variant there) is refused: DIMB_ERR_ARG for H2 > H or W2 > W.  B, H2 <= 65535. */
+int dimb_resize_area_dev(dimb_ctx* ctx, const float* d_src, int B, int height, int width, float* d_dst, int height2, int width2,
+                         void* stream);
+/* normalize_keypoints' own-extent size for LightGlue without image_size (lightglue.py:26-27): per image b, over its
+ * min(d_counts[b], kpt_ld) keypoints of d_kpts [B][kpt_ld][2] float32, d_size_out[b] = {(1 + max x) - min x, (1 + max y) - min y}
+ * in float32, as dimb_lg_match computes it on the host; {1, 1} for an image without keypoints.  Feed it to dimb_lg_match_dev
+ * through dimb_feats_dev.size_f32_dev. */
+int dimb_kpts_extent_dev(dimb_ctx* ctx, int B, const float* d_kpts, int kpt_ld, const int* d_counts, float* d_size_out, void* stream);
+/* The box-count loop of tile_selection's PRESELECTION for Q image pairs of equally sized images (height x width, tiled as
+ * dimb_tile_grid).  Pair q: the low-resolution match table d_matches[q] ([Q][cap][2] int64, rows = min(d_n_matches[q], cap), as
+ * dimb_lg_match_dev writes it) indexes the keypoints of f0[q] / f1[q] (host arrays of Q; keypoints, f16 and round_fp16 are read).
+ * Each matched keypoint maps back to full resolution as kpt / float(scale) (float32 division) and counts for tile pair (t0, t1) iff it
+ * lies strictly inside both boxes: ox < x < ox + tile_w and oy < y < oy + tile_h.  Out (device): d_counts [Q][T*T] int32, the
+ * count per tile pair t0 * T + t1; d_flags [Q][T*T] uint8 = count > min_matches_per_tile.  Integer counts: exact in any order.
+ * DIMB_ERR_ARG for a bad geometry, scales that are not finite and positive, or min_matches_per_tile < 0. */
+int dimb_tile_preselect_dev(dimb_ctx* ctx, int Q, const dimb_feats_dev* f0, const dimb_feats_dev* f1, const int64_t* d_matches,
+                            const int* d_n_matches, int cap, int height, int width, int tile_h, int tile_w, int overlap_h, int overlap_w,
+                            double scale0, double scale1, int min_matches_per_tile, int* d_counts, unsigned char* d_flags, void* stream);
 
 /* ------------------------------------------------------------------ fused per-pair path
  * SuperPoint on both images of every pair followed by LightGlue, features kept in HBM in between (the
