@@ -66,29 +66,30 @@ def all_gather_blocks(store_tensor, n_images: int, dist=None):
     return (world - 1) * mine.numel()
 
 
-def gather_match_tables(local_ids, local_matches, n_pairs: int, dist=None, device=None):
-    """Gather {pair id -> int64 (S,2)} from all ranks to rank 0 (counts all_gather + padded all_gather).
-    Returns the full list on rank 0 (None elsewhere)."""
+def _gather_arrays(local_ids, arrays, n_pairs: int, width: int, dtype, dist, device):
+    """Gather {pair id -> `dtype` array of `width` columns and any number of rows} from all ranks to rank 0: one all_gather of every
+    rank's (pair count, most rows), one of the padded arrays, each row of the padded buffer being (pair id, rows, values...).
+    Returns the list by pair id on rank 0, pairs nobody sent left None (None elsewhere)."""
     import torch
 
+    arrays = [np.asarray(a, dtype).reshape(-1, width) for a in arrays]
     if dist is None or not dist.is_initialized() or dist.get_world_size() == 1:
         out = [None] * n_pairs
-        for i, m in zip(local_ids, local_matches):
-            out[i] = np.asarray(m, np.int64).reshape(-1, 2)
+        for i, a in zip(local_ids, arrays):
+            out[i] = a
         return out
     world, rank = dist.get_world_size(), dist.get_rank()
     dev = device if device is not None else torch.device("cpu")
-    k = len(local_ids)
-    cnt = torch.tensor([k, max([len(m) for m in local_matches], default=0)], dtype=torch.int64, device=dev)
+    cnt = torch.tensor([len(arrays), max([len(a) for a in arrays], default=0)], dtype=torch.int64, device=dev)
     cnts = [torch.zeros_like(cnt) for _ in range(world)]
     dist.all_gather(cnts, cnt)
-    kmax, smax = int(max(c[0] for c in cnts)), int(max(c[1] for c in cnts))
-    buf = torch.full((max(kmax, 1), 2 + 2 * max(smax, 1)), -1, dtype=torch.int64, device=dev)
-    for j, (i, m) in enumerate(zip(local_ids, local_matches)):
-        m = torch.as_tensor(np.asarray(m, np.int64).reshape(-1, 2), device=dev)
-        buf[j, 0], buf[j, 1] = i, m.shape[0]
-        if m.shape[0]:
-            buf[j, 2:2 + 2 * m.shape[0]] = m.reshape(-1)
+    cnts = torch.stack(cnts).cpu().numpy()
+    kmax, smax = cnts.max(axis=0)
+    buf = np.zeros((max(kmax, 1), 2 + width * max(smax, 1)), dtype)
+    for j, (i, a) in enumerate(zip(local_ids, arrays)):
+        buf[j, :2] = i, len(a)
+        buf[j, 2:2 + a.size] = a.ravel()
+    buf = torch.as_tensor(buf, device=dev)
     bufs = [torch.zeros_like(buf) for _ in range(world)]
     dist.all_gather(bufs, buf)
     if rank != 0:
@@ -96,64 +97,38 @@ def gather_match_tables(local_ids, local_matches, n_pairs: int, dist=None, devic
     out = [None] * n_pairs
     for r in range(world):
         b = bufs[r].cpu().numpy()
-        for j in range(int(cnts[r][0])):
+        for j in range(cnts[r, 0]):
             i, s = int(b[j, 0]), int(b[j, 1])
-            out[i] = b[j, 2:2 + 2 * s].reshape(-1, 2).copy()
+            out[i] = b[j, 2:2 + width * s].reshape(-1, width).copy()
     return out
 
 
-def _gather_rows(local_ids, rows, n_pairs: int, dist, device):
-    """Gather {pair id -> float64 row of fixed width} to rank 0 (None elsewhere); pairs nobody sent stay None."""
-    import torch
-
-    world, rank = dist.get_world_size(), dist.get_rank()
-    width = rows.shape[1]
-    k = torch.tensor([len(local_ids)], dtype=torch.int64, device=device)
-    ks = [torch.zeros_like(k) for _ in range(world)]
-    dist.all_gather(ks, k)
-    kmax = max(1, int(max(int(c) for c in ks)))
-    buf = torch.zeros((kmax, 1 + width), dtype=torch.float64, device=device)
-    if len(local_ids):
-        buf[:len(local_ids), 0] = torch.as_tensor(np.asarray(local_ids, np.float64), device=device)
-        buf[:len(local_ids), 1:] = torch.as_tensor(np.asarray(rows, np.float64), device=device)
-    bufs = [torch.zeros_like(buf) for _ in range(world)]
-    dist.all_gather(bufs, buf)
-    if rank != 0:
-        return None
-    out = [None] * n_pairs
-    for r in range(world):
-        b = bufs[r].cpu().numpy()
-        for j in range(int(ks[r])):
-            out[int(b[j, 0])] = b[j, 1:].copy()
-    return out
+def gather_match_tables(local_ids, local_matches, n_pairs: int, dist=None, device=None):
+    """Gather {pair id -> int64 (S,2)} from all ranks to rank 0 (counts all_gather + padded all_gather).
+    Returns the full list on rank 0 (None elsewhere)."""
+    return _gather_arrays(local_ids, local_matches, n_pairs, 2, np.int64, dist, device)
 
 
 def gather_verified(local_ids, local_results, n_pairs: int, dist=None, device=None):
-    """Gather {pair id -> (raw (S,2), verified (V,2), F (3,3) float32 or None, n_inliers)} from all ranks to rank 0: the two tables
-    through ``gather_match_tables``, F and the count as one fixed-width float64 row per pair (exact for float32 and int32).
+    """Gather {pair id -> (raw (S,2), verified (V,2), F (3,3) float32 or None, n_inliers)} from all ranks to rank 0: the two int64
+    tables, and F and the count as one fixed-width float64 row per pair (exact for float32 and int32).
     Returns the full list of 4-tuples on rank 0 (None elsewhere)."""
-    raw = gather_match_tables(local_ids, [r[0] for r in local_results], n_pairs, dist, device)
-    ver = gather_match_tables(local_ids, [r[1] for r in local_results], n_pairs, dist, device)
+    raw = _gather_arrays(local_ids, [r[0] for r in local_results], n_pairs, 2, np.int64, dist, device)
+    ver = _gather_arrays(local_ids, [r[1] for r in local_results], n_pairs, 2, np.int64, dist, device)
     rows = np.zeros((len(local_ids), 11), np.float64)  # has_F, n_inliers, F row-major
     for k, r in enumerate(local_results):
         rows[k, 1] = r[3]
         if r[2] is not None:
             rows[k, 0] = 1.0
             rows[k, 2:] = np.asarray(r[2], np.float32).ravel()
-    if dist is None or not dist.is_initialized() or dist.get_world_size() == 1:
-        full = [None] * n_pairs
-        for i, row in zip(local_ids, rows):
-            full[i] = row
-    else:
-        import torch
-        full = _gather_rows(local_ids, rows, n_pairs, dist, device if device is not None else torch.device("cpu"))
-        if full is None:
-            return None
+    full = _gather_arrays(local_ids, rows, n_pairs, 11, np.float64, dist, device)
+    if full is None:
+        return None
     out = [None] * n_pairs
-    for i in range(n_pairs):
-        if full[i] is not None:
-            F = full[i][2:].astype(np.float32).reshape(3, 3) if full[i][0] else None
-            out[i] = (raw[i], ver[i], F, int(full[i][1]))
+    for i, row in enumerate(full):
+        if row is not None:
+            row = row[0]
+            out[i] = (raw[i], ver[i], row[2:].astype(np.float32).reshape(3, 3) if row[0] else None, int(row[1]))
     return out
 
 
@@ -275,9 +250,13 @@ def pack_tile_batches(n_tile_pairs, batch_pairs: int) -> list:
 
 
 class ImageSetMatcher:
-    """Two-phase multi-GPU matching of an image set (module docstring): SuperPoint on this rank's images into the device feature
+    """Two-phase multi-GPU matching of an image set (module docstring): the extractor on this rank's images into the device feature
     store, one all_gather of the float16 feature blocks, LightGlue or SuperGlue on this rank's share of the pair list, gather of the
     match tables.  ``dist`` is ``torch.distributed`` (initialised, nccl) or None for a single process.
+
+    Phase 2 is one loop over pair batches for every mode (``match`` / ``match_verified``, tiled or not): the matcher, the
+    verification when asked, then the batch's results reach the host in two synchronising steps, the counts (with F and n_inliers
+    when verifying) and then only the table rows in use.
 
     ``matcher="superglue"``: ``lg_weights`` is the SuperGlue state dict and ``lg_conf`` its configuration (``sinkhorn_iterations``,
     ``match_threshold``, ``gnn_layers``), and phase 2 runs the batched device SuperGlue on the store's slots.
@@ -351,6 +330,7 @@ class ImageSetMatcher:
         self.world = dist.get_world_size() if dist is not None and dist.is_initialized() else 1
         self.rank = dist.get_rank() if self.world > 1 else 0
         self.n, self.H, self.W = n_images, height, width
+        self.slots = [store_slot(i, n_images, self.world) for i in range(n_images)]
         self.extractor = extractor
         self.cap = int(sp_conf["max_keypoints"]) if extractor == "superpoint" else int(sp_conf.get("max_num_keypoints", 4000))
         if self.cap < 1:
@@ -422,15 +402,12 @@ class ImageSetMatcher:
             self.pre_sl = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
             self.pre_cnt = torch.zeros(batch_pairs, self.T * self.T, dtype=torch.int32, device=dev)
         self.gv = verification_conf(verification)
-        if self.gv is not None and self.gv["method"] != "NONE":  # verification outputs of one pair batch + pinned host copies
+        if self.gv is not None and self.gv["method"] != "NONE":  # verification outputs of one pair batch
             self.v = torch.zeros(batch_pairs, gv_cap, 2, dtype=torch.int64, device=dev)
             self.nv = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
             self.F = torch.zeros(batch_pairs, 9, device=dev)
             self.mask = torch.zeros(batch_pairs, gv_cap, dtype=torch.uint8, device=dev)
             self.ninl = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
-            if self.tiling is None:
-                self.host_out = {k: torch.zeros_like(t, device="cpu").pin_memory() for k, t in
-                                 (("m", self.m), ("nm", self.nm), ("v", self.v), ("nv", self.nv), ("F", self.F), ("ninl", self.ninl))}
 
         class _DevArr:  # zero-copy torch view of the store's device allocation (for the NCCL all_gather)
             def __init__(self, ptr, shape):
@@ -447,21 +424,23 @@ class ImageSetMatcher:
             if self.presel:
                 self._extract_preselection(d_images, image_ids, st)
             return self._extract_tiled(d_images, image_ids, st)
-        if self.extractor == "aliked":
-            for k, i in enumerate(image_ids):
-                self.al.extract_dev(d_images[k].data_ptr(), self.H, self.W, 3, self.kp.data_ptr(), self.sc.data_ptr(), self.de.data_ptr(),
-                                    self.cnt.data_ptr(), self.cap, st)
-                self.store.put_dev(store_slot(i, self.n, self.world), self.kp.data_ptr(), self.sc.data_ptr(), self.de.data_ptr(), self.cap,
-                                   self.cnt.data_ptr(), self.H, self.W, None, st)
-            return
         for b0 in range(0, len(image_ids), self.B):
             ids = image_ids[b0:b0 + self.B]
-            nb = len(ids)
-            self.sp.extract_dev(d_images[b0:b0 + nb].data_ptr(), nb, self.H, self.W, self.kp.data_ptr(), self.sc.data_ptr(),
-                                self.de.data_ptr(), self.cnt.data_ptr(), self.cap, st)
+            self._extract_rows(d_images[b0:b0 + len(ids)], self.H, self.W, st)
             for k, i in enumerate(ids):
-                self.store.put_dev(store_slot(i, self.n, self.world), self.kp[k].data_ptr(), self.sc[k].data_ptr(), self.de[k].data_ptr(),
-                                   self.cap, self.cnt[k:k + 1].data_ptr(), self.H, self.W, None, st)
+                self.store.put_dev(self.slots[i], self.kp[k].data_ptr(), self.sc[k].data_ptr(), self.de[k].data_ptr(), self.cap,
+                                   self.cnt[k:k + 1].data_ptr(), self.H, self.W, None, st)
+
+    def _extract_rows(self, src, h, w, st):
+        """The configured extractor on the len(src) h x w images or tiles of `src` into rows [0, len(src)) of kp / sc / de / cnt:
+        SuperPoint in calls of at most batch_images, ALIKED one per call."""
+        step = self.B if self.extractor == "superpoint" else 1
+        for r in range(0, len(src), step):
+            ptrs = (self.kp[r].data_ptr(), self.sc[r].data_ptr(), self.de[r].data_ptr(), self.cnt[r:].data_ptr(), self.cap, st)
+            if self.extractor == "superpoint":
+                self.sp.extract_dev(src[r].data_ptr(), min(step, len(src) - r), h, w, *ptrs)
+            else:
+                self.al.extract_dev(src[r].data_ptr(), h, w, 3, *ptrs)
 
     def _extract_preselection(self, d_images, image_ids, st):
         """PRESELECTION's low-resolution extraction, once per image: INTER_AREA down-sampling, SuperPoint into the image's slot rows of
@@ -471,7 +450,7 @@ class ImageSetMatcher:
             ids = image_ids[b0:b0 + self.B]
             self.ctx.resize_area_dev(d_images[b0:b0 + len(ids)].data_ptr(), len(ids), self.H, self.W, self.low.data_ptr(), self.pre_h,
                                      self.pre_w, st)
-            slots = [store_slot(i, self.n, self.world) for i in ids]
+            slots = [self.slots[i] for i in ids]
             k = 0
             while k < len(ids):  # the extractor writes consecutive rows: one call per run of consecutive slots
                 e = k + 1
@@ -485,23 +464,14 @@ class ImageSetMatcher:
 
     def _extract_tiled(self, d_images, image_ids, st):
         """Groups of G images: tile cut, the extractor over their G * T tiles, one tile merge into their slots."""
-        (th, tw), (oh, ow), T, K = self.tiling["tile_hw"], self.tiling["overlap_hw"], self.T, self.cap
+        (th, tw), (oh, ow) = self.tiling["tile_hw"], self.tiling["overlap_hw"]
         for g0 in range(0, len(image_ids), self.G):
             ids = image_ids[g0:g0 + self.G]
-            nt = len(ids) * T
             self.ctx.tile_cut_dev(d_images[g0:g0 + len(ids)].data_ptr(), len(ids), self.H, self.W, self.C, th, tw, oh, ow,
                                   self.tiles.data_ptr(), st)
-            if self.extractor == "superpoint":
-                for t0 in range(0, nt, self.B):
-                    k = min(self.B, nt - t0)
-                    self.sp.extract_dev(self.tiles[t0].data_ptr(), k, th, tw, self.kp[t0].data_ptr(), self.sc[t0].data_ptr(),
-                                        self.de[t0].data_ptr(), self.cnt[t0:].data_ptr(), K, st)
-            else:
-                for t in range(nt):
-                    self.al.extract_dev(self.tiles[t].data_ptr(), th, tw, 3, self.kp[t].data_ptr(), self.sc[t].data_ptr(), self.de[t].data_ptr(),
-                                        self.cnt[t:].data_ptr(), K, st)
-            self.store.tile_merge_dev([store_slot(i, self.n, self.world) for i in ids], self.H, self.W, th, tw, oh, ow, self.kp.data_ptr(),
-                                      self.sc.data_ptr(), self.de.data_ptr(), self.cnt.data_ptr(), K, st)
+            self._extract_rows(self.tiles[:len(ids) * self.T], th, tw, st)
+            self.store.tile_merge_dev([self.slots[i] for i in ids], self.H, self.W, th, tw, oh, ow, self.kp.data_ptr(), self.sc.data_ptr(),
+                                      self.de.data_ptr(), self.cnt.data_ptr(), self.cap, st)
 
     def exchange(self):
         """The collective of the path: every rank's float16 feature blocks to every rank (NCCL all_gather over NVLink).  With tiling,
@@ -515,7 +485,7 @@ class ImageSetMatcher:
             step = max(1, 65535 // self.T)
             for b0 in range(0, self.n, step):
                 ids = range(b0, min(self.n, b0 + step))
-                self.store.tile_views_dev([store_slot(i, self.n, self.world) for i in ids], self.T, self.views, [i * self.T for i in ids],
+                self.store.tile_views_dev([self.slots[i] for i in ids], self.T, self.views, [i * self.T for i in ids],
                                           self.vmap.data_ptr(), st)
 
     def _match_slots(self, store, s0, s1, st):
@@ -526,11 +496,6 @@ class ImageSetMatcher:
         else:
             self.lg.match_dev([store.feats_dev(s) for s in s0], [store.feats_dev(s) for s in s1], self.m.data_ptr(), self.ms.data_ptr(),
                               self.nm.data_ptr(), self.sl.data_ptr(), self.cap, st)
-
-    def _match_batch(self, chunk, st):
-        """Enqueue the matcher on one pair batch (outputs in self.m / self.ms / self.nm)."""
-        self._match_slots(self.store, [store_slot(i, self.n, self.world) for i, _ in chunk],
-                          [store_slot(j, self.n, self.world) for _, j in chunk], st)
 
     def _pre_feats(self, slot):
         """The float32 low-resolution features of a slot as LightGlue input, normalised by their own extent."""
@@ -551,8 +516,8 @@ class ImageSetMatcher:
         flags = self.torch.zeros(max(len(pairs), 1), T * T, dtype=self.torch.uint8, device=self.pre_cnt.device)
         for b0 in range(0, len(pairs), self.P):
             chunk = pairs[b0:b0 + self.P]
-            f0 = [self._pre_feats(store_slot(i, self.n, self.world)) for i, _ in chunk]
-            f1 = [self._pre_feats(store_slot(j, self.n, self.world)) for _, j in chunk]
+            f0 = [self._pre_feats(self.slots[i]) for i, _ in chunk]
+            f1 = [self._pre_feats(self.slots[j]) for _, j in chunk]
             self.lg_pre.match_dev(f0, f1, self.pre_m.data_ptr(), self.pre_ms.data_ptr(), self.pre_nm.data_ptr(), self.pre_sl.data_ptr(), K, st)
             self.ctx.tile_preselect_dev(f0, f1, self.pre_m.data_ptr(), self.pre_nm.data_ptr(), K, self.H, self.W, th, tw, oh, ow, self.pre_scale,
                                         self.pre_scale, self.tiling["min_matches_per_tile"], self.pre_cnt.data_ptr(), flags[b0].data_ptr(), st)
@@ -574,9 +539,13 @@ class ImageSetMatcher:
             lists.append(lst)
         return lists
 
-    def _match_tiled_batch(self, chunk, lists, st):
-        """Enqueue the matcher on the selected tile pairs of the image pairs `chunk` (views i * T + t) and the tile-pair match merge
-        (outputs in self.mm / self.nmm)."""
+    def _enqueue_match(self, chunk, lists, st):
+        """Enqueue the matcher on the image pairs `chunk` and return where it leaves their tables: (tables, counts, capacity).
+        Untiled: the store slots, (m, nm, cap).  Tiled: the tile pairs `lists` out of the views (i * T + t), then the tile-pair match
+        merge, (mm, nmm, cap2)."""
+        if lists is None:
+            self._match_slots(self.store, [self.slots[i] for i, _ in chunk], [self.slots[j] for _, j in chunk], st)
+            return self.m, self.nm, self.cap
         T = self.T
         v0 = [i * T + a for (i, _), lst in zip(chunk, lists) for a, _ in lst]
         v1 = [j * T + b for (_, j), lst in zip(chunk, lists) for _, b in lst]
@@ -585,116 +554,84 @@ class ImageSetMatcher:
         offsets = np.concatenate([[0], np.cumsum([len(lst) for lst in lists])])
         self.ctx.tile_match_merge_dev(offsets, v0, v1, self.vmap.data_ptr(), self.views.cap, self.m.data_ptr(), self.nm.data_ptr(), self.cap,
                                       self.mm.data_ptr(), self.nmm.data_ptr(), self.cap2, st)
+        return self.mm, self.nmm, self.cap2
 
-    def _read_tables(self, m, nm, Q):
-        """Host copies of the first Q tables of m [P][cap][2] with counts nm (the first copy synchronises)."""
-        n = np.minimum(nm[:Q].cpu().numpy(), m.shape[1])
-        rows = int(n.max(initial=0))
-        h = m[:Q, :rows].cpu().numpy()
-        return [h[k, :n[k]].copy() for k in range(Q)]
+    def _read_back(self, tables, extras, Q, stream):
+        """Host copies of the first Q entries of a batch in two synchronising steps: the counts of every (tables, counts, capacity) in
+        `tables` together with the `extras` tensors, then only the rows in use of each table, [:Q, :max(min(count, capacity))].
+        The copies of a step are non-blocking (into pinned memory from torch's host allocator), so each step ends in one synchronise.
+        Returns (per table, its Q arrays; the extras as numpy)."""
+        first = [t[:Q].to("cpu", non_blocking=True) for t in [nm for _, nm, _ in tables] + list(extras)]
+        stream.synchronize()
+        counts = [np.minimum(h.numpy(), cap) for h, (_, _, cap) in zip(first, tables)]
+        rows = [m[:Q, :int(n.max(initial=0))].to("cpu", non_blocking=True) for (m, _, _), n in zip(tables, counts)]
+        stream.synchronize()
+        return ([[h[k, :n[k]].copy() for k in range(Q)] for h, n in zip((r.numpy() for r in rows), counts)],
+                [h.numpy() for h in first[len(tables):]])
+
+    def _match_batches(self, pairs, pair_ids, tile_pairs, verify):
+        """Phase 2 of ``match`` and, with `verify`, of ``match_verified``: per batch of image pairs the matcher, then with `verify`
+        dimb_gv_verify_dev on its tables (same stream, keypoints from the store's slots), then ``_read_back``.  Untiled, every image
+        pair is one unit of a batch; tiled, its tile pairs are."""
+        from .geometric_verification import gv_seed
+        if self.tiling is None and tile_pairs is not None:
+            raise ValueError("tile_pairs needs an ImageSetMatcher built with tiling")
+        stream = self.torch.cuda.current_stream()
+        lists = None if self.tiling is None else self._tile_pair_lists(pairs, tile_pairs)
+        g, out = self.gv, {}
+        for s, e in pack_tile_batches([1] * len(pairs) if lists is None else [len(lst) for lst in lists], self.P):
+            chunk, ids = pairs[s:e], pair_ids[s:e]
+            m, nm, cap = self._enqueue_match(chunk, None if lists is None else lists[s:e], stream.cuda_stream)
+            if not verify:
+                (raw,), _ = self._read_back([(m, nm, cap)], (), e - s, stream)
+                out.update(zip(ids, raw))
+            else:
+                f0 = [self.store.feats_dev(self.slots[i]) for i, _ in chunk]
+                f1 = [self.store.feats_dev(self.slots[j]) for _, j in chunk]
+                self.ctx.gv_verify_dev(f0, f1, m.data_ptr(), nm.data_ptr(), cap, [gv_seed(g["seed"], k) for k in ids], g["threshold"],
+                                       g["max_iters"], g["min_inliers_per_pair"], g["min_inlier_ratio_per_pair"], self.v.data_ptr(),
+                                       self.nv.data_ptr(), self.F.data_ptr(), self.mask.data_ptr(), self.ninl.data_ptr(), stream.cuda_stream)
+                (raw, ver), (F, ninl) = self._read_back([(m, nm, cap), (self.v, self.nv, cap)], (self.F, self.ninl), e - s, stream)
+                for k, i in enumerate(ids):
+                    out[i] = (raw[k], ver[k], F[k].reshape(3, 3).copy() if np.any(F[k]) else None, int(ninl[k]))
+        return out
 
     def match(self, pairs, pair_ids, tile_pairs=None):
-        """Phase 2: LightGlue or SuperGlue on `pairs` = [(i, j), ...] (this rank's share); returns {pair id: int64 (S,2)} after ONE
-        device->host copy per batch.  Features are read in place from the store (float16, no rounding left to do).  Tiled: the tables
-        are the merged image-pair tables; `tile_pairs` optionally gives each pair's list of (t0, t1)."""
-        st = self.torch.cuda.current_stream().cuda_stream
-        out = {}
-        if self.tiling is not None:
-            lists = self._tile_pair_lists(pairs, tile_pairs)
-            for s, e in pack_tile_batches([len(lst) for lst in lists], self.P):
-                self._match_tiled_batch(pairs[s:e], lists[s:e], st)
-                for k, m in enumerate(self._read_tables(self.mm, self.nmm, e - s)):
-                    out[pair_ids[s + k]] = m
-            return out
-        if tile_pairs is not None:
-            raise ValueError("tile_pairs needs an ImageSetMatcher built with tiling")
-        for b0 in range(0, len(pairs), self.P):
-            chunk = pairs[b0:b0 + self.P]
-            self._match_batch(chunk, st)
-            nm = self.nm[:len(chunk)].cpu().numpy()
-            m = self.m[:len(chunk)].cpu().numpy()
-            for k in range(len(chunk)):
-                out[pair_ids[b0 + k]] = m[k, :nm[k]].copy()
-        return out
+        """Phase 2: LightGlue or SuperGlue on `pairs` = [(i, j), ...] (this rank's share); returns {pair id: int64 (S,2)}.  Each pair
+        batch comes back in two synchronising steps: the counts, then only the table rows in use.  Features are read in place from the
+        store (float16, no rounding left to do).  Tiled: the tables are the merged image-pair tables; `tile_pairs` optionally gives
+        each pair's list of (t0, t1)."""
+        return self._match_batches(pairs, pair_ids, tile_pairs, verify=False)
 
     def match_verified(self, pairs, pair_ids, tile_pairs=None):
         """Phase 2 with geometric verification: returns {pair id: (raw int64 (S,2), verified int64 (V,2), F (3,3) float32 or None,
-        n_inliers)}.  Per batch the matcher and dimb_gv_verify_dev are enqueued on the same stream and the results come back with
-        ONE synchronise.  Tiled: the merged tables are verified against the merged slots."""
-        from .geometric_verification import gv_seed
+        n_inliers)}.  Per batch the matcher and dimb_gv_verify_dev are enqueued on the same stream, and the results come back in two
+        synchronising steps: the raw and verified counts with F and n_inliers, then only the rows in use of both tables.  Tiled: the
+        merged tables are verified against the merged slots."""
         if self.gv is None:
             raise RuntimeError("ImageSetMatcher was built without verification")
         if self.gv["method"] == "NONE":  # the reference skips the estimator: verified = raw, no F
             return {k: (m, m.copy(), None, len(m)) for k, m in self.match(pairs, pair_ids, tile_pairs).items()}
-        if self.tiling is not None:
-            return self._match_verified_tiled(pairs, pair_ids, tile_pairs)
-        if tile_pairs is not None:
-            raise ValueError("tile_pairs needs an ImageSetMatcher built with tiling")
-        torch, st = self.torch, self.torch.cuda.current_stream()
-        g, h = self.gv, self.host_out
-        out = {}
-        for b0 in range(0, len(pairs), self.P):
-            chunk, ids = pairs[b0:b0 + self.P], pair_ids[b0:b0 + self.P]
-            self._match_batch(chunk, st.cuda_stream)
-            f0 = [self.store.feats_dev(store_slot(i, self.n, self.world)) for i, _ in chunk]
-            f1 = [self.store.feats_dev(store_slot(j, self.n, self.world)) for _, j in chunk]
-            self.ctx.gv_verify_dev(f0, f1, self.m.data_ptr(), self.nm.data_ptr(), self.cap, [gv_seed(g["seed"], k) for k in ids],
-                                   g["threshold"], g["max_iters"], g["min_inliers_per_pair"], g["min_inlier_ratio_per_pair"],
-                                   self.v.data_ptr(), self.nv.data_ptr(), self.F.data_ptr(), self.mask.data_ptr(), self.ninl.data_ptr(),
-                                   st.cuda_stream)
-            P = len(chunk)
-            for k in ("nm", "nv", "F", "ninl", "m", "v"):
-                h[k][:P].copy_(getattr(self, k)[:P], non_blocking=True)
-            st.synchronize()
-            nm, nv, F, ninl = h["nm"][:P].numpy(), h["nv"][:P].numpy(), h["F"][:P].numpy(), h["ninl"][:P].numpy()
-            m, v = h["m"].numpy(), h["v"].numpy()
-            for k in range(P):
-                n = min(int(nm[k]), self.cap)
-                out[ids[k]] = (m[k, :n].copy(), v[k, :int(nv[k])].copy(), F[k].reshape(3, 3).copy() if np.any(F[k]) else None,
-                               int(ninl[k]))
-        return out
+        return self._match_batches(pairs, pair_ids, tile_pairs, verify=True)
 
-    def _match_verified_tiled(self, pairs, pair_ids, tile_pairs):
-        from .geometric_verification import gv_seed
-        st, g = self.torch.cuda.current_stream(), self.gv
-        lists = self._tile_pair_lists(pairs, tile_pairs)
-        out = {}
-        for s, e in pack_tile_batches([len(lst) for lst in lists], self.P):
-            chunk, ids = pairs[s:e], pair_ids[s:e]
-            self._match_tiled_batch(chunk, lists[s:e], st.cuda_stream)
-            f0 = [self.store.feats_dev(store_slot(i, self.n, self.world)) for i, _ in chunk]
-            f1 = [self.store.feats_dev(store_slot(j, self.n, self.world)) for _, j in chunk]
-            self.ctx.gv_verify_dev(f0, f1, self.mm.data_ptr(), self.nmm.data_ptr(), self.cap2, [gv_seed(g["seed"], k) for k in ids],
-                                   g["threshold"], g["max_iters"], g["min_inliers_per_pair"], g["min_inlier_ratio_per_pair"],
-                                   self.v.data_ptr(), self.nv.data_ptr(), self.F.data_ptr(), self.mask.data_ptr(), self.ninl.data_ptr(),
-                                   st.cuda_stream)
-            Q = e - s
-            raw = self._read_tables(self.mm, self.nmm, Q)
-            ver = self._read_tables(self.v, self.nv, Q)
-            F, ninl = self.F[:Q].cpu().numpy(), self.ninl[:Q].cpu().numpy()
-            for k in range(Q):
-                out[ids[k]] = (raw[k], ver[k], F[k].reshape(3, 3).copy() if np.any(F[k]) else None, int(ninl[k]))
-        return out
+    def _run(self, match, gather, d_images, my_image_ids, pairs, costs, tile_pairs):
+        """extract -> exchange -> `match` on this rank's share of `pairs` -> `gather` to rank 0."""
+        self.extract(d_images, my_image_ids)
+        self.exchange()
+        mine = shard_pairs(len(pairs), self.world, self.rank, costs)
+        res = match([pairs[k] for k in mine], mine, None if tile_pairs is None else [tile_pairs[k] for k in mine])
+        return gather(mine, [res[k] for k in mine], len(pairs), self.dist if self.world > 1 else None,
+                      self.torch.device("cuda", self.ctx.device) if self.world > 1 else None)
 
     def run(self, d_images, my_image_ids, pairs, costs=None, tile_pairs=None):
         """extract -> exchange -> match my share -> gather to rank 0.  Returns the list of match tables on rank 0 (None elsewhere).
         tile_pairs (tiled only): per pair of `pairs`, its list of (t0, t1)."""
-        self.extract(d_images, my_image_ids)
-        self.exchange()
-        mine = shard_pairs(len(pairs), self.world, self.rank, costs)
-        res = self.match([pairs[k] for k in mine], mine, None if tile_pairs is None else [tile_pairs[k] for k in mine])
-        return gather_match_tables(mine, [res[k] for k in mine], len(pairs), self.dist if self.world > 1 else None,
-                                   self.torch.device("cuda", self.ctx.device) if self.world > 1 else None)
+        return self._run(self.match, gather_match_tables, d_images, my_image_ids, pairs, costs, tile_pairs)
 
     def run_verified(self, d_images, my_image_ids, pairs, costs=None, tile_pairs=None):
         """extract -> exchange -> match and verify my share -> gather to rank 0.  Returns, on rank 0, the list of
         (raw, verified, F, n_inliers) per pair (None elsewhere); ``export_colmap`` turns it into a COLMAP database."""
-        self.extract(d_images, my_image_ids)
-        self.exchange()
-        mine = shard_pairs(len(pairs), self.world, self.rank, costs)
-        res = self.match_verified([pairs[k] for k in mine], mine, None if tile_pairs is None else [tile_pairs[k] for k in mine])
-        return gather_verified(mine, [res[k] for k in mine], len(pairs), self.dist if self.world > 1 else None,
-                               self.torch.device("cuda", self.ctx.device) if self.world > 1 else None)
+        return self._run(self.match_verified, gather_verified, d_images, my_image_ids, pairs, costs, tile_pairs)
 
     def export_colmap(self, pairs, results, database_path, image_names=None, **kwargs) -> dict:
         """Rank 0: the COLMAP database of this image set (``export_verified_to_colmap`` on this matcher's feature store)."""

@@ -240,6 +240,38 @@ def test_aliked_tile_merge_equals_extract_by_tile(ctx, al_weights):
     assert np.array_equal(tables[0], exp) and len(exp) > 0
 
 
+@pytest.mark.gpu
+def test_image_set_matcher_aliked_untiled_equals_serial_flow(ctx, al_weights):
+    """ALIKED without tiling: 3 RGB images, all pairs, batch_images=2 (the extraction crosses a chunk boundary) and batch_pairs=2.
+    The store holds AlikedExtractor._extract + as_half_roundtrip of every image, and every table equals the LightGlue plugin's
+    _match_pairs (input_dim 128) on those features."""
+    import torch
+    from dim_b200 import synthetic, weights
+    from dim_b200.config import Config
+    from dim_b200.extractors.aliked import AlikedExtractor
+    from dim_b200.io_h5 import as_half_roundtrip
+    from dim_b200.matchers.lightglue import LightGlueMatcher
+    from dim_b200.pairs_generator import pairs_from_bruteforce
+    from dim_b200.sharded import ImageSetMatcher
+    a = synthetic.blocks_image(301, 512)[:384]
+    imgs = np.stack([a] + [synthetic.warp_pair(a, 50 + k, jitter=24.0) for k in (1, 2)]).astype(np.float32)
+    al_conf = {"max_num_keypoints": 1024, "detection_threshold": 0.2, "nms_radius": 3}
+    w_lg = weights.lightglue_seeded(input_dim=128, seed=0)
+    pairs = pairs_from_bruteforce([0, 1, 2])
+    eng = ImageSetMatcher(ctx, al_weights, w_lg, 3, 384, 512, al_conf, {}, batch_images=2, batch_pairs=2, extractor="aliked")
+    tables = eng.run(torch.from_numpy(imgs).cuda(), [0, 1, 2], pairs)
+    ext = AlikedExtractor(Config(pipeline="aliked+lightglue", extractor={"model_name": "aliked-n16rot", **al_conf, "weights_dict": al_weights}))
+    feats = [as_half_roundtrip({**ext._extract(img), "image_size": np.array(img.shape[:2])}) for img in imgs]
+    for i in range(3):
+        got = eng.store.get(i)
+        for k in ("keypoints", "descriptors", "scores"):
+            assert got[k].shape == feats[i][k].shape and np.array_equal(got[k], feats[i][k]), (i, k)
+    plugin = LightGlueMatcher(Config(pipeline="aliked+lightglue", matcher={"weights_dict": w_lg}), local_features="aliked")
+    for (i, j), t in zip(pairs, tables):
+        assert np.array_equal(t, plugin._match_pairs(feats[i], feats[j])), (i, j)
+    assert min(len(f["keypoints"]) for f in feats) > 100 and sum(len(t) for t in tables) > 0
+
+
 def _gray_set(n, H=768, W=1024):
     from dim_b200 import synthetic
     a = synthetic.blocks_image(40, max(H, W))[:H, :W]
