@@ -181,7 +181,8 @@ _selftest = None
 
 
 def load_selftest_library():
-    """libdimb200_selftest.so: the production GEMM template behind a C = A B^T entry and the host drive of the RANSAC arithmetic.
+    """libdimb200_selftest.so: the production GEMM template behind a C = A B^T entry, the flash-attention kernels behind an
+    attention entry and the host drive of the RANSAC arithmetic.
     Test / tool infrastructure - the product library exports none of it.  Its context is its own (dimb_ctx_create of
     THIS library); never mix handles of the two libraries."""
     global _selftest
@@ -198,6 +199,8 @@ def load_selftest_library():
         lib.dimb_last_error.restype = C.c_char_p
         lib.dimb_ctx_set_precision.argtypes = [vp, ip]
         lib.dimb_selftest_gemm.argtypes = [vp, vp, vp, vp, ip, ip, ip, ip]
+        fp = C.c_float
+        lib.dimb_selftest_attention.argtypes = [vp, ip, vp, vp, vp, vp, ip, ip, ip, ip, vp, vp, ip, fp, fp, fp]
         lib.dimb_gv_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_uint, vp, vp]
         _selftest = lib
     return _selftest
@@ -228,6 +231,33 @@ class SelfTest:
         Cm = np.zeros((M, N), np.float32)
         self.check(self.lib.dimb_selftest_gemm(self.h, _ptr(A), _ptr(B), _ptr(Cm), M, N, K, bn), "selftest_gemm")
         return Cm
+
+    def attention(self, variant: int, Q: np.ndarray, K, V: np.ndarray, n, heads: int = 4, stopped=None, cross: bool = False,
+                  lazy: float = -1.0, pad: float = 0.0, out_pad: float = 0.0) -> np.ndarray:
+        """The flash-attention kernels through their production launches (dimb_selftest_attention), precision of the context.
+        variant 0 (LightGlue / SuperGlue, 4 heads x 64): Q, K, V [S][4][NP][64], n [S] live rows per side, stopped [S/2]; with
+        cross the keys of side s are the q rows of side s ^ 1 (K unused).  Returns the context buffer [S][NP][256] (head h at
+        columns 64 h).  variant 1 (head dim <= 128): Q [n0][heads * hd], K / V [n1][heads * hd], n = (n0, n1); returns
+        [NPp][heads * hd], NPp = max(n0, n1, 1) rounded up to 128.  Rows past the live counts hold `pad` on the way in; the
+        output buffer starts as `out_pad`.  lazy: rescale threshold in log2 units, in [0, 15]; negative = the context's."""
+        Q = np.ascontiguousarray(Q, np.float32)
+        V = np.ascontiguousarray(V, np.float32)
+        K = None if K is None else np.ascontiguousarray(K, np.float32)
+        nn = np.ascontiguousarray(n, np.int32)
+        if variant == 0:
+            S, H, NP, hd = Q.shape
+            st = np.ascontiguousarray(stopped if stopped is not None else np.zeros(S // 2), np.int32)
+            out = np.zeros((S, NP, H * hd), np.float32)
+        else:
+            H, hd, NP = int(heads), Q.shape[1] // int(heads), max(int(nn[0]), int(nn[1]), 1)
+            S, st = 1, np.zeros(1, np.int32)
+            out = np.zeros(((NP + 127) // 128 * 128, H * hd), np.float32)
+            if K.shape[0] == 0:  # no keys: the entry still wants valid pointers
+                K = V = np.zeros((1, H * hd), np.float32)
+        self.check(self.lib.dimb_selftest_attention(self.h, int(variant), _ptr(Q), _ptr(K) if K is not None else None, _ptr(V), _ptr(out),
+                                                    S, H, hd, NP, _ptr(nn), _ptr(st), int(bool(cross)), float(lazy), float(pad),
+                                                    float(out_pad)), "selftest_attention")
+        return out
 
     def __del__(self):
         try:

@@ -242,7 +242,11 @@ int dimb_ctx_create(int device, dimb_ctx** out) {
   const char* e = getenv("DIMB_TC");
   if (e && e[0] == '0') ctx->use_tc = 0;
   const char* lz = getenv("DIMB_ATTN_LAZY");
-  if (lz) ctx->attn_lazy = static_cast<float>(atof(lz));
+  if (lz) {  // NaN, inf, out of range or no number at all: keep the default (common.cuh: kAttnLazyMax)
+    char* end = nullptr;
+    const float v = strtof(lz, &end);
+    if (end != lz && v >= 0.f && v <= kAttnLazyMax) ctx->attn_lazy = v;
+  }
   const char* k3 = getenv("DIMB_K32");
   if (k3) ctx->k32 = k3[0] == '1';
   const char* b2 = getenv("DIMB_BN256");

@@ -14,6 +14,10 @@
 #include "../../include/dimb200.h"
 
 // ---------------------------------------------------------------- errors
+// Largest lazy-rescale threshold of the attention kernel (attention.cuh), in log2 units: the softmax numerators P reach 2^lazy and
+// their hi plane is fp16 (largest finite value 65504 < 2^16), so 15 is the last whole threshold that cannot overflow it.
+constexpr float kAttnLazyMax = 15.f;
+
 struct dimb_ctx {
   int device = 0;
   int num_sms = 132;
@@ -22,7 +26,9 @@ struct dimb_ctx {
   int k32 = 0;            // 32-wide K stages (half-size stages) for the 128 x 256 LightGlue tiles (gemm.cuh CONV 3); DIMB_K32=1
   int bn256 = 0;          // LightGlue q/k projection and FFN0 on 128 x 256 output tiles (DIMB_BN256=1); default 128 x 128: spill-free
   int nms_ver = 2;        // simple_nms kernel: 2 = bit-mask kernel (sp_nms2_kernel), 1 = first cut (DIMB_NMS)
-  float attn_lazy = 8.f;  // lazy-rescale threshold of the attention kernel in log2 units (DIMB_ATTN_LAZY; 0 = rescale on every new maximum)
+  // lazy-rescale threshold of the attention kernel in log2 units (DIMB_ATTN_LAZY; 0 = rescale on every new maximum).  Only finite
+  // values in [0, kAttnLazyMax] are taken from the environment, anything else keeps 8: P <= 2^lazy must fit the fp16 hi plane.
+  float attn_lazy = 8.f;
   std::string last_error;
   std::vector<void*> allocs;            // device memory owned by the context itself
   std::vector<void*>* owner = nullptr;
