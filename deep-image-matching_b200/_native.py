@@ -23,7 +23,7 @@ EXPORTS = [
     "dimb_ctx_set_tensor_path", "dimb_ctx_launch_count", "dimb_read_dev",
     "dimb_sp_create", "dimb_sp_destroy", "dimb_sp_extract", "dimb_sp_extract_dev", "dimb_sp_debug_read",
     "dimb_lg_create", "dimb_lg_destroy", "dimb_lg_match", "dimb_lg_match_dev", "dimb_lg_debug_read",
-    "dimb_nn_match", "dimb_nn_match_dev", "dimb_ctx_profile", "dimb_ctx_profile_read", "dimb_pipe_create", "dimb_pipe_destroy",
+    "dimb_nn_match", "dimb_nn_match_dev", "dimb_nn_match_batch_dev", "dimb_ctx_profile", "dimb_ctx_profile_read", "dimb_pipe_create", "dimb_pipe_destroy",
     "dimb_pipe_match_image_pairs", "dimb_pipe_match_image_pairs_u8", "dimb_pipe_match_image_pairs_dev", "dimb_pipe_outputs_dev", "dimb_pipe_features_dev", "dimb_sp_ctx",
     "dimb_sg_weight_count", "dimb_sg_create", "dimb_sg_destroy", "dimb_sg_match", "dimb_sg_match_dev", "dimb_fstore_sg_feats_dev",
     "dimb_aliked_create", "dimb_aliked_destroy", "dimb_aliked_extract", "dimb_aliked_extract_dev", "dimb_aliked_debug_read",
@@ -124,6 +124,7 @@ def load_library():
     lib.dimb_lg_debug_read.argtypes = [vp, ip, ip, vp, C.c_size_t]
     lib.dimb_nn_match.argtypes = [vp, vp, ip, vp, ip, ip, ip, fp, vp, vp, C.POINTER(ip), ip]
     lib.dimb_nn_match_dev.argtypes = [vp, vp, ip, ip, vp, ip, ip, ip, ip, ip, fp, vp, vp, vp, ip, vp]
+    lib.dimb_nn_match_batch_dev.argtypes = [vp, ip, C.POINTER(FeatsDev), C.POINTER(FeatsDev), ip, ip, fp, vp, vp, vp, ip, vp]
     lib.dimb_ctx_profile.argtypes = [vp, ip]
     lib.dimb_ctx_profile_read.argtypes = [vp, C.c_char_p, C.c_size_t]
     lib.dimb_pipe_create.argtypes = [vp, vp, ip, ip, ip, ip, C.POINTER(vp)]
@@ -431,6 +432,17 @@ class Context:
         """Device-pointer variant (ints are device addresses); asynchronous on `stream`."""
         self.check(self.lib.dimb_nn_match_dev(self.h, d_desc0, n0, ld0, d_desc1, n1, ld1, D, int(f16), NN_MODES[mode], float(th), d_idx,
                                               d_dist, d_n, cap, stream), "dimb_nn_match_dev")
+
+    def nn_match_batch_dev(self, f0: list, f1: list, D: int, mode: str, th: float, d_idx: int, d_dist: int, d_n: int, cap: int,
+                           stream: int = 0):
+        """Brute-force NN matching of len(f0) pairs (dimb_nn_match_batch_dev): f0 / f1 are lists of FeatsDev (e.g.
+        FeatureStoreDev.feats_dev) whose counts stay on the device.  Outputs are device buffers (ints are device addresses): d_idx
+        [P][cap][2] int64, d_dist [P][cap] float32, d_n [P] int32 (the full count).  Asynchronous on `stream`."""
+        P = len(f0)
+        a0 = (FeatsDev * P)(*f0)
+        a1 = (FeatsDev * P)(*f1)
+        self.check(self.lib.dimb_nn_match_batch_dev(self.h, P, a0, a1, int(D), NN_MODES[mode], float(th), d_idx, d_dist, d_n, cap, stream),
+                   "dimb_nn_match_batch_dev")
 
 
 SP_ORDER = ["conv1a", "conv1b", "conv2a", "conv2b", "conv3a", "conv3b", "conv4a", "conv4b", "convPa", "convPb",

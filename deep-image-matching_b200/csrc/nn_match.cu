@@ -1,4 +1,4 @@
-// nn_match.cu - brute-force descriptor matcher (dimb_nn_match), replacing KorniaMatcher._match_pairs
+// nn_match.cu - brute-force descriptor matcher (dimb_nn_match*), replacing KorniaMatcher._match_pairs
 // (reference matchers/kornia_matcher.py:27-54 -> kornia.feature.DescriptorMatcher nn/mnn/snn/smnn).
 //
 // The reference materialises the full n0 x n1 distance matrix (torch.cdist, 268 MB at 8192^2) and runs
@@ -7,6 +7,17 @@
 // (|a|^2 + |b|^2 - 2ab, clamped, sqrt) and a per-row running (best, second best, argbest) over each
 // 32-column chunk; a small merge kernel reduces the chunk partials.  The column statistics needed by the
 // mutual / symmetric modes are the same kernel with the operands swapped.
+//
+// One batched engine serves P pairs = 2P sides per call with the keypoint counts on the device (dimb_nn_match_batch_dev);
+// dimb_nn_match_dev and dimb_nn_match are its P = 1 callers.  Side s owns rows [s * NPp, (s + 1) * NPp) of the operand buffers
+// (NPp = the largest n_cap rounded up to 128), pair p is sides 2p and 2p + 1:
+//   prep   : one launch over all sides: fp16 hi (/ lo) planes, squared norms (zero on padding rows) and the live count of every side
+//            (0 for both sides of a pair kornia leaves empty, so that no later kernel works on it)
+//   top2   : one persistent GEMM over all pairs per direction (rows of sides 2p, then of sides 2p + 1 for mnn / smnn); tiles past a
+//            side's count, and pairs with an empty partner, are skipped on the device.  The host-count callers (P = 1) launch exactly
+//            the tiles of their counts with the counts as kernel arguments and a B panel that may stay resident in shared memory
+//   merge  : chunk partials -> (best, second, argbest) per live row, one launch per direction (the directions share the partials)
+//   select : one CTA per pair, kornia's mode logic and the ordered compaction into [P][cap] tables
 #include <algorithm>
 #include <vector>
 
@@ -18,69 +29,139 @@ namespace {
 // (it spills), so the wider tile's halved A re-reads are not worth it
 constexpr int kNnBN = 128;
 
+// one side of the engine (dimb_feats_dev, resolved)
+struct NNSideIn {
+  const void* desc;  // (D, n) rows of pitch ld, float32 or float16
+  const int* n;      // device count (rows = min(*n, n_cap)), or NULL: n_cap rows (the host-count entries)
+  int n_cap, ld, f16, round_fp16;
+};
+
+__host__ __device__ inline bool nn_trivially_empty(int n0, int n1, int mode) {
+  // kornia: empty inputs / fewer than two candidates for the ratio tests -> no match
+  return n0 == 0 || n1 == 0 || (mode == DIMB_NN_SNN && n1 < 2) || (mode == DIMB_NN_SMNN && (n0 < 2 || n1 < 2));
+}
+
+__device__ __forceinline__ int nn_side_rows(const NNSideIn& s) { return s.n ? max(0, min(*s.n, s.n_cap)) : s.n_cap; }
+
+// Running (best, second best, argbest) of one row over the 32 columns n..n+31 of a GEMM tile, written as the partial of chunk n / 32
+// at pd1 / pd2 / pi1 [o].  Squared distances |a|^2 + |b|^2 - 2ab are compared as they are: sqrt is monotone, so the order inside a
+// chunk is that of the distances (two columns whose squared distances differ in the last bit but whose square roots round to the
+// same float would be a tie for torch.cdist + min and are an ordered pair here: measure-zero, and the merge kernel compares the chunk
+// partials in the sqrt domain again).  This removes the IEEE sqrt (8 instructions) from the per-element path.
+__device__ __forceinline__ void nn_top2_chunk(const float (&v)[32], float a2, const float* __restrict__ nb, int n, int n_cols, float* pd1,
+                                              float* pd2, int* pi1, size_t o) {
+  float d1 = INFINITY, d2 = INFINITY;
+  int i1 = 0x7fffffff;
+  const float4* nb4 = reinterpret_cast<const float4*>(nb + n);  // norms are padded to a multiple of 128 columns
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    const float4 b = __ldg(nb4 + q);
+    const float bb[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int j = 4 * q + e;
+      float d = fmaf(-2.f, v[j], a2 + bb[e]);
+      if (n + j >= n_cols) d = INFINITY;
+      if (d < d1) {
+        d2 = d1;
+        d1 = d;
+        i1 = n + j;
+      } else if (d < d2) {
+        d2 = d;
+      }
+    }
+  }
+  pd1[o] = d1;
+  pd2[o] = d2;
+  pi1[o] = i1;
+}
+
+// Top-2 epilogue of one pair with host counts (dimb_nn_match_dev / dimb_nn_match): the A and B maps start at the row side and its
+// partner, the launch covers exactly the tiles of the counts, and the counts are kernel arguments.  The B panel is the same for
+// every tile, so it may stay resident in shared memory.
 struct EpiNNTop2 : EpiBase {
   const float *na, *nb;  // squared norms of A rows / B rows
   float *pd1, *pd2;      // [rows][chunks] best / second best SQUARED distance of each 32-column chunk
   int* pi1;              // [rows][chunks] argbest
   int n_rows, n_cols, chunks;
-  // Squared distances |a|^2 + |b|^2 - 2ab are compared as they are: sqrt is monotone, so the order inside a chunk is that of
-  // the distances (two columns whose squared distances differ in the last bit but whose square roots round to the same float
-  // would be a tie for torch.cdist + min and are an ordered pair here: measure-zero, and the merge kernel compares the
-  // chunk partials in the sqrt domain again).  This removes the IEEE sqrt (8 instructions) from the per-element path.
   __device__ void operator()(const TileCoord& tc, int r, int n, float (&v)[32], float*) const {
     const int row = tc.m0 + r;
     if (row >= n_rows) return;
-    const float a2 = na[row];
-    float d1 = INFINITY, d2 = INFINITY;
-    int i1 = 0x7fffffff;
-    const float4* nb4 = reinterpret_cast<const float4*>(nb + n);  // nb is padded to a multiple of 256 columns
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      const float4 b = __ldg(nb4 + q);
-      const float bb[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int j = 4 * q + e;
-        float d = fmaf(-2.f, v[j], a2 + bb[e]);
-        if (n + j >= n_cols) d = INFINITY;
-        if (d < d1) {
-          d2 = d1;
-          d1 = d;
-          i1 = n + j;
-        } else if (d < d2) {
-          d2 = d;
-        }
-      }
-    }
-    const size_t o = static_cast<size_t>(row) * chunks + (n >> 5);
-    pd1[o] = d1;
-    pd2[o] = d2;
-    pi1[o] = i1;
+    nn_top2_chunk(v, na[row], nb, n, n_cols, pd1, pd2, pi1, static_cast<size_t>(row) * chunks + (n >> 5));
   }
 };
 
-// (D,n) descriptors (fp32 or fp16, row pitch ld) -> [n_pad][Dp] fp16 hi/lo + squared norms; block (32,8) transposing 32x32
-// tiles.  Dp = D rounded up to 64: the padding columns are zero, which changes no distance (any descriptor size works).
-// any_lo is set when some value is not exactly fp16: only then does the GEMM need the lo planes.
-template <class T>
-__global__ void nn_prep_kernel(const T* __restrict__ d, int D, int Dp, int n, int ld, __half* __restrict__ hi, __half* __restrict__ lo,
-                               float* __restrict__ norm, int* __restrict__ any_lo) {
+// Top-2 epilogue of P pairs with device counts: rows of sides 2p + swap against their partner sides 2p + 1 - swap, both maps over
+// all sides; row tiles at or past a side's live count, and pairs with an empty partner, are skipped on the device.
+struct EpiNNTop2Batch : EpiBase {
+  static constexpr bool kConstB = false;
+  const float* norm;     // [2P][NPp] squared norms
+  const int* n_live;     // [2P] live rows
+  float *pd1, *pd2;      // [P][NPp][stride]
+  int* pi1;
+  int NPp, tps, swap, stride;  // tps: row tiles per pair in the launch
+  __device__ int m0_of(int t) const { return ((t / tps) * 2 + swap) * NPp + (t % tps) * kTileM; }
+  __device__ bool tile_active(const TileCoord& tc) const {
+    const int side = tc.m0 / NPp;
+    return tc.m0 - side * NPp < n_live[side] && tc.n0 < n_live[side ^ 1];
+  }
+  __device__ int b_row_offset(const TileCoord& tc) const { return ((tc.m0 / NPp) ^ 1) * NPp; }
+  __device__ void operator()(const TileCoord& tc, int r, int n, float (&v)[32], float*) const {
+    const int side = tc.m0 / NPp, row = tc.m0 - side * NPp + r;
+    if (row >= n_live[side]) return;
+    nn_top2_chunk(v, norm[tc.m0 + r], norm + (side ^ 1) * NPp, n, n_live[side ^ 1], pd1, pd2, pi1,
+                  (static_cast<size_t>(side >> 1) * NPp + row) * stride + (n >> 5));
+  }
+};
+
+// grid (NPp / 32, 2P), block (32, 8): (D,n) descriptors of every side -> [2P][NPp][Dp] fp16 hi (/ lo) + squared norms, transposing
+// 32x32 tiles.  Dp = D rounded up to 64: the padding columns are zero, which changes no distance (any descriptor size works).  Rows
+// past the live count get a zero norm (keeping the masked padded columns finite) and no hi / lo.  round_fp16 rounds float32 inputs
+// to fp16 first (round to nearest even, the features.h5 cast).  any_lo is set when some value is not exactly fp16: only then does
+// the GEMM need the lo planes.
+__global__ void nn_prep_kernel(const NNSideIn* __restrict__ in, int mode, int D, int Dp, int NPp, __half* __restrict__ hi,
+                               __half* __restrict__ lo, float* __restrict__ norm, int* __restrict__ n_live, int* __restrict__ any_lo) {
   __shared__ float tile[32][33];
-  const int t0 = blockIdx.x * 32, tx = threadIdx.x, ty = threadIdx.y;
+  const int side = blockIdx.y, t0 = blockIdx.x * 32, tx = threadIdx.x, ty = threadIdx.y;
+  const NNSideIn si = in[side];
+  const int na = nn_side_rows(in[side & ~1]), nb = nn_side_rows(in[side | 1]);
+  const int n = nn_trivially_empty(na, nb, mode) ? 0 : ((side & 1) ? nb : na);
+  if (blockIdx.x == 0 && tx == 0 && ty == 0) n_live[side] = n;
+  const size_t r0 = static_cast<size_t>(side) * NPp;
+  if (t0 >= n) {
+    if (tx == 0)
+      for (int k = ty; k < 32; k += 8) norm[r0 + t0 + k] = 0.f;
+    return;
+  }
+  // row k = ty + 8 q of the tile (q = 0..3, unrolled so that acc stays in registers)
   float acc[4] = {0.f, 0.f, 0.f, 0.f};
   bool nz = false;
   for (int c0 = 0; c0 < Dp; c0 += 32) {
-    for (int k = ty; k < 32; k += 8)
-      tile[k][tx] = (t0 + tx < n && c0 + k < D) ? static_cast<float>(d[static_cast<size_t>(c0 + k) * ld + t0 + tx]) : 0.f;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int k = ty + 8 * q;
+      float v = 0.f;
+      if (t0 + tx < n && c0 + k < D) {
+        const size_t o = static_cast<size_t>(c0 + k) * si.ld + t0 + tx;
+        if (si.f16) {
+          v = __half2float(static_cast<const __half*>(si.desc)[o]);
+        } else {
+          v = static_cast<const float*>(si.desc)[o];
+          if (si.round_fp16) v = __half2float(__float2half_rn(v));
+        }
+      }
+      tile[k][tx] = v;
+    }
     __syncthreads();
-    int q = 0;
-    for (int k = ty; k < 32; k += 8, ++q) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int k = ty + 8 * q;
       const float v = tile[tx][k];  // token t0+k, channel c0+tx
       if (t0 + k < n) {
         __half h, l;
         split_f32(v, h, l);
-        hi[static_cast<size_t>(t0 + k) * Dp + c0 + tx] = h;
-        if (lo) lo[static_cast<size_t>(t0 + k) * Dp + c0 + tx] = l;
+        hi[(r0 + t0 + k) * Dp + c0 + tx] = h;
+        if (lo) lo[(r0 + t0 + k) * Dp + c0 + tx] = l;
         nz |= __half2float(l) != 0.f;
       }
       float sq = v * v;
@@ -90,22 +171,31 @@ __global__ void nn_prep_kernel(const T* __restrict__ d, int D, int Dp, int n, in
     }
     __syncthreads();
   }
-  int q = 0;
-  for (int k = ty; k < 32; k += 8, ++q)
-    if (tx == 0 && t0 + k < n) norm[t0 + k] = acc[q];
+#pragma unroll
+  for (int q = 0; q < 4; ++q)
+    if (tx == 0) norm[r0 + t0 + ty + 8 * q] = acc[q];  // 0 on rows past n: their tile values are zero
   if (any_lo && __any_sync(0xffffffffu, nz) && tx == 0) atomicOr(any_lo, 1);
 }
 
-// warp per row: merge chunk partials -> best, second, arg (first index wins ties); the partials are squared distances, the
-// comparison happens on the distances (clamp at 0, IEEE sqrt) like torch.cdist + min / topk
-__global__ void nn_merge_kernel(const float* __restrict__ pd1, const float* __restrict__ pd2, const int* __restrict__ pi1, int rows,
-                                int chunks, float* __restrict__ d1, float* __restrict__ d2, int* __restrict__ i1) {
-  const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (row >= rows) return;
+// warp per row of the sides 2p + swap (rows_pp rows per pair in the grid; rows past the live count exit): merge the chunk partials
+// that hold a live column of the partner, chunks [0, ceil(n / 32)) -> best, second, arg (first index wins ties) at row side * NPp + row
+// of d1 / d2 / i1.  Only those chunks are written on every path: the CUDA-core twin of the GEMM (DIMB_TC=0) has 32-column tiles and
+// skips the ones past the partner's count, and the chunks past them in a 128-column tensor-core tile are all +inf, which changes no
+// result.  The partials are squared distances, the comparison happens on the distances (clamp at 0, IEEE sqrt) like torch.cdist + min /
+// topk.
+__global__ void nn_merge_kernel(const float* __restrict__ pd1, const float* __restrict__ pd2, const int* __restrict__ pi1,
+                                const int* __restrict__ n_live, int P, int NPp, int rows_pp, int swap, int stride, float* __restrict__ d1,
+                                float* __restrict__ d2, int* __restrict__ i1) {
+  const int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (q >= P * rows_pp) return;
+  const int p = q / rows_pp, row = q - p * rows_pp, side = 2 * p + swap;
+  if (row >= n_live[side]) return;
+  const int chunks = ceil_div(n_live[side ^ 1], 32);
+  const size_t base = (static_cast<size_t>(p) * NPp + row) * stride;
   float b1 = INFINITY, b2 = INFINITY;
   int bi = 0x7fffffff;
   for (int c = lane; c < chunks; c += 32) {
-    const size_t o = static_cast<size_t>(row) * chunks + c;
+    const size_t o = base + c;
     const float x1 = sqrtf(fmaxf(pd1[o], 0.f)), x2 = sqrtf(fmaxf(pd2[o], 0.f));
     const int xi = pi1[o];
     if (x1 < b1 || (x1 == b1 && xi < bi)) {
@@ -129,20 +219,27 @@ __global__ void nn_merge_kernel(const float* __restrict__ pd1, const float* __re
     }
   }
   if (lane == 0) {
-    d1[row] = b1;
-    d2[row] = b2;
-    i1[row] = bi;
+    const size_t out = static_cast<size_t>(side) * NPp + row;
+    d1[out] = b1;
+    d2[out] = b2;
+    i1[out] = bi;
   }
 }
 
-// one CTA: apply the kornia mode logic and compact in ascending row order
+// one CTA per pair: apply the kornia mode logic to the row statistics of its sides (forward at side 2p, backward at side 2p + 1) and
+// compact in ascending row order into the pair's [cap] rows; count = the full number of matches
 __global__ void __launch_bounds__(1024)
-nn_select_kernel(int mode, float th, int n0, int n1, const float* __restrict__ fd1, const float* __restrict__ fd2,
-                 const int* __restrict__ fi1, const float* __restrict__ bd1, const float* __restrict__ bd2, const int* __restrict__ bi1,
-                 long long* __restrict__ idx, float* __restrict__ dist, int* __restrict__ count, int cap) {
+nn_select_kernel(int mode, float th, const int* __restrict__ n_live, int NPp, const float* __restrict__ sd1, const float* __restrict__ sd2,
+                 const int* __restrict__ si1, long long* __restrict__ idx_all, float* __restrict__ dist_all, int* __restrict__ count, int cap) {
   __shared__ int wsum[32];
   __shared__ int s_base;
-  const int t = threadIdx.x;
+  const int t = threadIdx.x, p = blockIdx.x;
+  const int n0 = n_live[2 * p], n1 = n_live[2 * p + 1];
+  const size_t f = static_cast<size_t>(2 * p) * NPp, b = f + NPp;
+  const float *fd1 = sd1 + f, *fd2 = sd2 + f, *bd1 = sd1 + b, *bd2 = sd2 + b;
+  const int *fi1 = si1 + f, *bi1 = si1 + b;
+  long long* idx = idx_all + static_cast<size_t>(p) * cap * 2;
+  float* dist = dist_all + static_cast<size_t>(p) * cap;
   if (t == 0) s_base = 0;
   __syncthreads();
   const int ms = min(n0, n1);
@@ -151,28 +248,28 @@ nn_select_kernel(int mode, float th, int n0, int n1, const float* __restrict__ f
   for (int base = 0; base < iters; base += blockDim.x) {
     const int i = base + t;
     bool valid = false;
-    long long a = 0, b = 0;
+    long long a = 0, bb = 0;
     float dv = 0.f;
     if (i < iters) {
       if (mode == DIMB_NN_NN) {
-        valid = true, a = i, b = fi1[i], dv = fd1[i];
+        valid = true, a = i, bb = fi1[i], dv = fd1[i];
       } else if (mode == DIMB_NN_MNN) {
         if (!swapped) {
           const int j = fi1[i];
-          valid = bi1[j] == i, a = i, b = j, dv = fd1[i];
+          valid = bi1[j] == i, a = i, bb = j, dv = fd1[i];
         } else {
           const int j = bi1[i];  // i indexes desc2
-          valid = fi1[j] == i, a = j, b = i, dv = bd1[i];
+          valid = fi1[j] == i, a = j, bb = i, dv = bd1[i];
         }
       } else if (mode == DIMB_NN_SNN) {
         const float ratio = fd1[i] / fd2[i];
-        valid = ratio <= th, a = i, b = fi1[i], dv = ratio;
+        valid = ratio <= th, a = i, bb = fi1[i], dv = ratio;
       } else {  // SMNN
         const float rf = fd1[i] / fd2[i];
         const int j = fi1[i];
         const float rb = bd1[j] / bd2[j];
         valid = (rf <= th) && (rb <= th) && (bi1[j] == i);
-        a = i, b = j, dv = fmaxf(rf, rb);
+        a = i, bb = j, dv = fmaxf(rf, rb);
       }
     }
     const unsigned bal = __ballot_sync(0xffffffffu, valid);
@@ -183,7 +280,7 @@ nn_select_kernel(int mode, float th, int n0, int n1, const float* __restrict__ f
     before += __popc(bal & ((1u << (t & 31)) - 1u));
     if (valid && before < cap) {
       idx[2 * before] = a;
-      idx[2 * before + 1] = b;
+      idx[2 * before + 1] = bb;
       dist[before] = dv;
     }
     __syncthreads();
@@ -194,129 +291,185 @@ nn_select_kernel(int mode, float th, int n0, int n1, const float* __restrict__ f
     }
     __syncthreads();
   }
-  if (t == 0) *count = s_base;
+  if (t == 0) count[p] = s_base;
 }
 
-struct NNSide {
-  __half *hi, *lo;
-  float* norm;
-  CUtensorMap mA[2], mB[2];
+// Launch geometry of one call: NPp rows per side; per direction (0: rows of sides 2p, 1: rows of sides 2p + 1) the row tiles per
+// pair and the padded partner columns.  Device counts: every tile of NPp (dead ones are skipped on the device).  Host counts
+// (P = 1): exactly the tiles of the counts.
+struct NNShape {
+  int P, NPp, tps[2], npad[2];
+  bool host;  // the counts are host_n (P = 1): EpiNNTop2 with the counts as kernel arguments
+  int hn[2];
 };
 
-int nn_rowtop2(dimb_ctx* ctx, cudaStream_t st, const NNSide& A, int na, const NNSide& B, int nb, int Dp, bool split, float* pd1, float* pd2,
-               int* pi1, float* d1, float* d2, int* i1) {
-  EpiNNTop2 e;
-  e.na = A.norm;
-  e.nb = B.norm;
-  e.pd1 = pd1;
-  e.pd2 = pd2;
-  e.pi1 = pi1;
-  e.n_rows = na;
-  e.n_cols = nb;
-  e.chunks = round_up(nb, kNnBN) / 32;
-  TcOperands ops;
-  ops.Ah = A.mA[0];
-  ops.Al = A.mA[1];
-  ops.Bh = B.mB[0];
-  ops.Bl = B.mB[1];
-  GemmArgs g{};
-  g.num_kb = Dp / 64;
-  g.M = na;
-  g.N = nb;
-  g.Ah = A.hi;
-  g.Al = A.lo;
-  g.Bh = B.hi;
-  g.Bl = B.lo;
-  g.lda = Dp;
-  g.ldb = Dp;
-  // descriptors that are exactly fp16 (everything read back from features.h5 is) have zero lo planes: ONE MMA per product is
-  // exact, and the 256-descriptor B panel (128 KB) stays resident in shared memory while the A tiles stream
-  DIMB_TRY((launch_gemm<kNnBN, false>(ctx, st, ops, g, e, ceil_div(na, kTileM), round_up(nb, kNnBN), "nn.top2_gemm", split ? 1 : 0)));
-  ProfScope prof(ctx, st, "nn.merge");
-  nn_merge_kernel<<<ceil_div(na * 32, 256), 256, 0, st>>>(pd1, pd2, pi1, na, e.chunks, d1, d2, i1);
-  DIMB_LAUNCH_CHECK(ctx);
-  return DIMB_OK;
+NNShape nn_shape(int P, int max_cap, const int* host_n) {
+  NNShape s;
+  s.P = P;
+  s.host = host_n != nullptr;
+  s.hn[0] = host_n ? host_n[0] : 0;
+  s.hn[1] = host_n ? host_n[1] : 0;
+  s.NPp = std::max(round_up(max_cap, kNnBN), kNnBN);
+  for (int d = 0; d < 2; ++d) {
+    s.tps[d] = host_n ? ceil_div(host_n[d], kTileM) : s.NPp / kTileM;
+    s.npad[d] = host_n ? round_up(host_n[d ^ 1], kNnBN) : s.NPp;
+  }
+  return s;
 }
 
 struct NNWork {  // grow-only scratch of one matching call (context slots: no cudaMalloc / cudaFree in steady state)
-  NNSide s[2];
-  float *pd1, *pd2, *fd1, *fd2, *bd1, *bd2;
-  int *pi1, *fi1, *bi1, *any_lo;
-  int Dp, p0, p1;
+  __half *hi, *lo;  // [2P][NPp][Dp]; lo is NULL without the split
+  float* norm;      // [2P][NPp]
+  NNSideIn* sides;  // [2P]
+  int* n_live;      // [2P]
+  float *pd1, *pd2; // [P][NPp][NPp / 32] chunk partials, shared by the two directions
+  int* pi1;
+  float *d1, *d2;   // [2P][NPp] merged row statistics
+  int *i1, *any_lo;
+  CUtensorMap mA[2][2], mB[2][2];  // [direction][hi, lo]: host counts: the row side / its partner only; else all rows
+  int Dp;
 };
 
-int nn_workspace(dimb_ctx* ctx, int n0, int n1, int D, NNWork* w) {
-  int slot = 8;  // slots 0..7 belong to the host-buffer entry (staging + outputs)
+// slots 0..7 belong to the host-buffer entry (staging + outputs)
+int nn_workspace(dimb_ctx* ctx, const NNShape& sh, int D, bool want_lo, NNWork* w) {
+  int slot = 8;
   auto alloc = [&](void* p, size_t bytes) -> int { return dimb_scratch(ctx, slot++, bytes, reinterpret_cast<void**>(p)); };
-  w->Dp = round_up(D, 64);
-  w->p0 = round_up(n0, kNnBN);
-  w->p1 = round_up(n1, kNnBN);
-  for (int i = 0; i < 2; ++i) {
-    const int pn = i ? w->p1 : w->p0;
-    NNSide& sd = w->s[i];
-    DIMB_TRY(alloc(&sd.hi, static_cast<size_t>(pn) * w->Dp * sizeof(__half)));
-    DIMB_TRY(alloc(&sd.lo, static_cast<size_t>(pn) * w->Dp * sizeof(__half)));
-    DIMB_TRY(alloc(&sd.norm, static_cast<size_t>(pn) * sizeof(float)));
-    DIMB_TRY(dimb_tmap_2d(ctx, &sd.mA[0], sd.hi, pn, w->Dp, w->Dp, kTileM));
-    DIMB_TRY(dimb_tmap_2d(ctx, &sd.mA[1], sd.lo, pn, w->Dp, w->Dp, kTileM));
-    DIMB_TRY(dimb_tmap_2d(ctx, &sd.mB[0], sd.hi, pn, w->Dp, w->Dp, kNnBN));  // as B operand: boxes of kNnBN rows
-    DIMB_TRY(dimb_tmap_2d(ctx, &sd.mB[1], sd.lo, pn, w->Dp, w->Dp, kNnBN));
-  }
-  const size_t pm = std::max(w->p0, w->p1), ch = pm / 32;
-  DIMB_TRY(alloc(&w->pd1, pm * ch * sizeof(float)));
-  DIMB_TRY(alloc(&w->pd2, pm * ch * sizeof(float)));
-  DIMB_TRY(alloc(&w->pi1, pm * ch * sizeof(int)));
-  DIMB_TRY(alloc(&w->fd1, w->p0 * sizeof(float)));
-  DIMB_TRY(alloc(&w->fd2, w->p0 * sizeof(float)));
-  DIMB_TRY(alloc(&w->fi1, w->p0 * sizeof(int)));
-  DIMB_TRY(alloc(&w->bd1, w->p1 * sizeof(float)));
-  DIMB_TRY(alloc(&w->bd2, w->p1 * sizeof(float)));
-  DIMB_TRY(alloc(&w->bi1, w->p1 * sizeof(int)));
+  const int P = sh.P, NPp = sh.NPp, Dp = w->Dp = round_up(D, 64);
+  const size_t rows = static_cast<size_t>(2 * P) * NPp, plane = rows * Dp * sizeof(__half);
+  DIMB_TRY(alloc(&w->hi, plane));
+  DIMB_TRY(alloc(&w->lo, want_lo ? plane : 256));
+  if (!want_lo) w->lo = nullptr;
+  DIMB_TRY(alloc(&w->norm, rows * sizeof(float)));
+  DIMB_TRY(alloc(&w->sides, 2 * P * sizeof(NNSideIn)));
+  DIMB_TRY(alloc(&w->n_live, 2 * P * sizeof(int)));
+  const size_t part = static_cast<size_t>(P) * NPp * (NPp / 32);
+  DIMB_TRY(alloc(&w->pd1, part * sizeof(float)));
+  DIMB_TRY(alloc(&w->pd2, part * sizeof(float)));
+  DIMB_TRY(alloc(&w->pi1, part * sizeof(int)));
+  DIMB_TRY(alloc(&w->d1, rows * sizeof(float)));
+  DIMB_TRY(alloc(&w->d2, rows * sizeof(float)));
+  DIMB_TRY(alloc(&w->i1, rows * sizeof(int)));
   DIMB_TRY(alloc(&w->any_lo, sizeof(int)));
+  __half* planes[2] = {w->hi, want_lo ? w->lo : w->hi};
+  for (int d = 0; d < 2; ++d)
+    for (int pl = 0; pl < 2; ++pl) {
+      __half* a = planes[pl] + (sh.host ? static_cast<size_t>(d) * NPp * Dp : 0);
+      __half* b = planes[pl] + (sh.host ? static_cast<size_t>(d ^ 1) * NPp * Dp : 0);
+      const size_t r = sh.host ? NPp : rows;
+      DIMB_TRY(dimb_tmap_2d(ctx, &w->mA[d][pl], a, r, Dp, Dp, kTileM));
+      DIMB_TRY(dimb_tmap_2d(ctx, &w->mB[d][pl], b, r, Dp, Dp, kNnBN));  // as B operand: boxes of kNnBN rows
+    }
   return DIMB_OK;
 }
 
-// prep of both sides on `st`; the rows of the padded operands beyond n are left as they are (their distances are never read:
-// the epilogue masks columns >= n_cols and rows >= n_rows)
-int nn_prep(dimb_ctx* ctx, cudaStream_t st, const NNWork& w, const void* d0, int n0, int ld0, const void* d1, int n1, int ld1, int D,
-            int f16, bool want_lo) {
-  ProfScope prof(ctx, st, "nn.prep");
-  DIMB_CUDA_OK(ctx, cudaMemsetAsync(w.any_lo, 0, sizeof(int), st));
-  for (int i = 0; i < 2; ++i) {
-    const void* d = i ? d1 : d0;
-    const int n = i ? n1 : n0, ld = i ? ld1 : ld0, pn = i ? w.p1 : w.p0;
-    const NNSide& sd = w.s[i];
-    // zero norms of the padding rows keep the (masked) padded columns finite
-    DIMB_CUDA_OK(ctx, cudaMemsetAsync(sd.norm, 0, static_cast<size_t>(pn) * sizeof(float), st));
-    if (f16)
-      nn_prep_kernel<__half><<<ceil_div(n, 32), dim3(32, 8), 0, st>>>(static_cast<const __half*>(d), D, w.Dp, n, ld, sd.hi, nullptr, sd.norm, nullptr);
-    else
-      nn_prep_kernel<float><<<ceil_div(n, 32), dim3(32, 8), 0, st>>>(static_cast<const float*>(d), D, w.Dp, n, ld, sd.hi,
-                                                                   want_lo ? sd.lo : nullptr, sd.norm, w.any_lo);
-    DIMB_LAUNCH_CHECK(ctx);
+// rows of sides 2p + d against sides 2p + 1 - d: top-2 GEMM of every pair, then the merge
+int nn_direction(dimb_ctx* ctx, cudaStream_t st, const NNWork& w, const NNShape& sh, int d, bool split) {
+  const TcOperands ops{w.mA[d][0], w.mA[d][1], w.mB[d][0], w.mB[d][1]};
+  const size_t a_off = sh.host ? static_cast<size_t>(d) * sh.NPp * w.Dp : 0, b_off = sh.host ? static_cast<size_t>(d ^ 1) * sh.NPp * w.Dp : 0;
+  const int m_tiles = sh.P * sh.tps[d], stride = sh.npad[d] / 32;
+  GemmArgs g{};
+  g.num_kb = w.Dp / 64;
+  g.M = sh.host ? sh.hn[d] : 2 * sh.P * sh.NPp;
+  g.N = sh.npad[d];
+  g.Ah = w.hi + a_off;
+  g.Al = w.lo ? w.lo + a_off : nullptr;
+  g.Bh = w.hi + b_off;
+  g.Bl = w.lo ? w.lo + b_off : nullptr;
+  g.lda = w.Dp;
+  g.ldb = w.Dp;
+  // descriptors that are exactly fp16 (everything read back from features.h5 is) have zero lo planes: ONE MMA per product is
+  // exact, and (host counts) the 256-descriptor B panel (128 KB) stays resident in shared memory while the A tiles stream
+  if (sh.host) {
+    EpiNNTop2 e;
+    e.na = w.norm + static_cast<size_t>(d) * sh.NPp;
+    e.nb = w.norm + static_cast<size_t>(d ^ 1) * sh.NPp;
+    e.pd1 = w.pd1;
+    e.pd2 = w.pd2;
+    e.pi1 = w.pi1;
+    e.n_rows = sh.hn[d];
+    e.n_cols = sh.hn[d ^ 1];
+    e.chunks = stride;
+    DIMB_TRY((launch_gemm<kNnBN, false>(ctx, st, ops, g, e, m_tiles, sh.npad[d], "nn.top2_gemm", split ? 1 : 0)));
+  } else {
+    EpiNNTop2Batch e;
+    e.norm = w.norm;
+    e.n_live = w.n_live;
+    e.pd1 = w.pd1;
+    e.pd2 = w.pd2;
+    e.pi1 = w.pi1;
+    e.NPp = sh.NPp;
+    e.tps = sh.tps[d];
+    e.swap = d;
+    e.stride = stride;
+    DIMB_TRY((launch_gemm<kNnBN, false>(ctx, st, ops, g, e, m_tiles, sh.npad[d], "nn.top2_gemm", split ? 1 : 0)));
   }
-  return DIMB_OK;
-}
-
-int nn_core(dimb_ctx* ctx, cudaStream_t st, const NNWork& w, int n0, int n1, bool split, int mode, float th, long long* d_idx, float* d_dist,
-            int* d_n, int cap) {
-  DIMB_TRY(nn_rowtop2(ctx, st, w.s[0], n0, w.s[1], n1, w.Dp, split, w.pd1, w.pd2, w.pi1, w.fd1, w.fd2, w.fi1));
-  if (mode == DIMB_NN_MNN || mode == DIMB_NN_SMNN)
-    DIMB_TRY(nn_rowtop2(ctx, st, w.s[1], n1, w.s[0], n0, w.Dp, split, w.pd1, w.pd2, w.pi1, w.bd1, w.bd2, w.bi1));
-  ProfScope prof(ctx, st, "nn.select");
-  nn_select_kernel<<<1, 1024, 0, st>>>(mode, th, n0, n1, w.fd1, w.fd2, w.fi1, w.bd1, w.bd2, w.bi1, d_idx, d_dist, d_n, cap);
+  ProfScope prof(ctx, st, "nn.merge");
+  const int rows_pp = sh.tps[d] * kTileM;
+  nn_merge_kernel<<<ceil_div(sh.P * rows_pp, 8), 256, 0, st>>>(w.pd1, w.pd2, w.pi1, w.n_live, sh.P, sh.NPp, rows_pp, d, stride, w.d1, w.d2,
+                                                               w.i1);
   DIMB_LAUNCH_CHECK(ctx);
   return DIMB_OK;
 }
 
-bool nn_trivially_empty(int n0, int n1, int mode) {
-  // kornia: empty inputs / fewer than two candidates for the ratio tests -> no match
-  return n0 == 0 || n1 == 0 || (mode == DIMB_NN_SNN && n1 < 2) || (mode == DIMB_NN_SMNN && (n0 < 2 || n1 < 2));
+// The engine on 2P sides.  split: 1 / 0 = three / one MMA per product; -1 = decide from the prepared operands (one host
+// synchronise: the host entry's check for descriptors that are exactly fp16).
+int nn_run(dimb_ctx* ctx, cudaStream_t st, const std::vector<NNSideIn>& sides, const NNShape& sh, int D, int mode, float th, int split,
+           long long* d_idx, float* d_dist, int* d_n, int cap) {
+  NNWork w;
+  DIMB_TRY(nn_workspace(ctx, sh, D, split != 0, &w));
+  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(w.sides, sides.data(), sides.size() * sizeof(NNSideIn), cudaMemcpyHostToDevice, st));
+  {
+    ProfScope prof(ctx, st, "nn.prep");
+    if (split < 0) DIMB_CUDA_OK(ctx, cudaMemsetAsync(w.any_lo, 0, sizeof(int), st));
+    nn_prep_kernel<<<dim3(sh.NPp / 32, 2 * sh.P), dim3(32, 8), 0, st>>>(w.sides, mode, D, w.Dp, sh.NPp, w.hi, w.lo, w.norm, w.n_live,
+                                                                         split < 0 ? w.any_lo : nullptr);
+    DIMB_LAUNCH_CHECK(ctx);
+  }
+  if (split < 0) {
+    int any_lo = 0;
+    DIMB_CUDA_OK(ctx, cudaMemcpyAsync(&any_lo, w.any_lo, sizeof(int), cudaMemcpyDeviceToHost, st));
+    DIMB_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    split = any_lo != 0;
+  }
+  DIMB_TRY(nn_direction(ctx, st, w, sh, 0, split));
+  if (mode == DIMB_NN_MNN || mode == DIMB_NN_SMNN) DIMB_TRY(nn_direction(ctx, st, w, sh, 1, split));
+  ProfScope prof(ctx, st, "nn.select");
+  nn_select_kernel<<<sh.P, 1024, 0, st>>>(mode, th, w.n_live, sh.NPp, w.d1, w.d2, w.i1, d_idx, d_dist, d_n, cap);
+  DIMB_LAUNCH_CHECK(ctx);
+  return DIMB_OK;
 }
 
 }  // namespace
 
 extern "C" {
+
+// P pairs on device features with device counts (contract in dimb200.h): validation before any CUDA call, then the engine.
+int dimb_nn_match_batch_dev(dimb_ctx* ctx, int P, const dimb_feats_dev* f0, const dimb_feats_dev* f1, int D, int mode, float th,
+                            int64_t* d_idx, float* d_dist, int* d_n, int cap, void* stream) {
+  if (!ctx || !f0 || !f1 || !d_idx || !d_dist || !d_n || P < 1 || cap < 1 || D < 1 || mode < 0 || mode > 3) {
+    if (ctx) dimb_set_error(ctx, "dimb_nn_match_batch_dev: invalid argument (NULL array or output, P >= 1, cap >= 1, D >= 1, mode 0..3)");
+    return DIMB_ERR_ARG;
+  }
+  std::vector<NNSideIn> sides(2 * P);
+  int max_cap = 0;
+  bool any_f32 = false;
+  for (int p = 0; p < P; ++p)
+    for (int sd = 0; sd < 2; ++sd) {
+      const dimb_feats_dev& f = sd ? f1[p] : f0[p];
+      if (!f.descriptors || !f.n || f.n_cap < 0 || f.desc_layout != 0 || f.desc_ld < 0) {
+        dimb_set_error(ctx, "dimb_nn_match_batch_dev: pair " + std::to_string(p) + " side " + std::to_string(sd) +
+                                ": NULL descriptors / n, n_cap < 0, or desc_layout other than 0 ((D,n) rows)");
+        return DIMB_ERR_ARG;
+      }
+      sides[2 * p + sd] = NNSideIn{f.descriptors, f.n, f.n_cap, f.desc_ld ? f.desc_ld : f.n_cap, f.f16 ? 1 : 0, f.round_fp16 ? 1 : 0};
+      max_cap = std::max(max_cap, f.n_cap);
+      any_f32 |= !f.f16 && !f.round_fp16;
+    }
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const bool split = any_f32 && ctx->precision == DIMB_PRECISION_EXACT;
+  return nn_run(ctx, static_cast<cudaStream_t>(stream), sides, nn_shape(P, max_cap, nullptr), D, mode, th, split ? 1 : 0,
+                reinterpret_cast<long long*>(d_idx), d_dist, d_n, cap);
+}
 
 // Device-resident entry: descriptors (D,n) with row pitch ld in HBM (fp32, or fp16 as the device feature store keeps them),
 // results in device buffers, asynchronous on `stream`.  fp16 input takes the single-MMA path (exact: the values ARE fp16).
@@ -333,11 +486,12 @@ int dimb_nn_match_dev(dimb_ctx* ctx, const void* d_desc0, int n0, int ld0, const
     return DIMB_OK;
   }
   if (!d_desc0 || !d_desc1) return DIMB_ERR_ARG;
-  NNWork w;
-  DIMB_TRY(nn_workspace(ctx, n0, n1, D, &w));
+  const int f16 = desc_f16 ? 1 : 0, hn[2] = {n0, n1};
+  const std::vector<NNSideIn> sides = {NNSideIn{d_desc0, nullptr, n0, ld0 ? ld0 : n0, f16, 0},
+                                       NNSideIn{d_desc1, nullptr, n1, ld1 ? ld1 : n1, f16, 0}};
   const bool split = !desc_f16 && ctx->precision == DIMB_PRECISION_EXACT;  // fp32 input: no host round trip to learn whether lo == 0
-  DIMB_TRY(nn_prep(ctx, st, w, d_desc0, n0, ld0 ? ld0 : n0, d_desc1, n1, ld1 ? ld1 : n1, D, desc_f16, split));
-  return nn_core(ctx, st, w, n0, n1, split, mode, th, reinterpret_cast<long long*>(d_idx), d_dist, d_n, cap);
+  return nn_run(ctx, st, sides, nn_shape(1, std::max(n0, n1), hn), D, mode, th, split ? 1 : 0, reinterpret_cast<long long*>(d_idx), d_dist,
+                d_n, cap);
 }
 
 int dimb_nn_match(dimb_ctx* ctx, const float* d0, int n0, const float* d1, int n1, int D, int mode, float th, int64_t* idx, float* dist,
@@ -359,18 +513,13 @@ int dimb_nn_match(dimb_ctx* ctx, const float* d0, int n0, const float* d1, int n
   DIMB_TRY(dimb_scratch(ctx, 2, static_cast<size_t>(cap) * 2 * sizeof(long long), reinterpret_cast<void**>(&o_idx)));
   DIMB_TRY(dimb_scratch(ctx, 3, static_cast<size_t>(cap) * sizeof(float), reinterpret_cast<void**>(&o_dist)));
   DIMB_TRY(dimb_scratch(ctx, 4, sizeof(int), reinterpret_cast<void**>(&o_n)));
-  NNWork w;
-  DIMB_TRY(nn_workspace(ctx, n0, n1, D, &w));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(raw0, d0, static_cast<size_t>(D) * n0 * sizeof(float), cudaMemcpyHostToDevice, st));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(raw1, d1, static_cast<size_t>(D) * n1 * sizeof(float), cudaMemcpyHostToDevice, st));
-  const bool exact = ctx->precision == DIMB_PRECISION_EXACT;
-  DIMB_TRY(nn_prep(ctx, st, w, raw0, n0, n0, raw1, n1, n1, D, 0, exact));
-  int any_lo = 0;  // descriptors read back from features.h5 are exactly fp16: then the lo planes are zero and one MMA is exact
-  if (exact) {
-    DIMB_CUDA_OK(ctx, cudaMemcpyAsync(&any_lo, w.any_lo, sizeof(int), cudaMemcpyDeviceToHost, st));
-    DIMB_CUDA_OK(ctx, cudaStreamSynchronize(st));
-  }
-  DIMB_TRY(nn_core(ctx, st, w, n0, n1, exact && any_lo != 0, mode, th, o_idx, o_dist, o_n, cap));
+  const int hn[2] = {n0, n1};
+  const std::vector<NNSideIn> sides = {NNSideIn{raw0, nullptr, n0, n0, 0, 0}, NNSideIn{raw1, nullptr, n1, n1, 0, 0}};
+  // descriptors read back from features.h5 are exactly fp16: then the lo planes are zero and one MMA is exact
+  const int split = ctx->precision == DIMB_PRECISION_EXACT ? -1 : 0;
+  DIMB_TRY(nn_run(ctx, st, sides, nn_shape(1, std::max(n0, n1), hn), D, mode, th, split, o_idx, o_dist, o_n, cap));
   int cnt = 0;
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(&cnt, o_n, sizeof(int), cudaMemcpyDeviceToHost, st));
   DIMB_CUDA_OK(ctx, cudaStreamSynchronize(st));

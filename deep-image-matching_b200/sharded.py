@@ -7,8 +7,8 @@ match_pairs, image_matching.py:413-494, is the serial loop this replaces) run in
      ``store_slot``);
   2. ONE ``all_gather`` of the float16 feature blocks (NCCL over NVLink; ~1.07 MB per SuperPoint image) gives every rank all
      features (``all_gather_blocks``), then the pair list is dealt by longest-processing-time (``shard_pairs``) and each rank
-     matches its pairs (LightGlue or SuperGlue) out of its own HBM; the variable-length match tables are gathered to rank 0
-     (``gather_match_tables``).
+     matches its pairs (LightGlue, SuperGlue or kornia's brute-force nearest neighbours) out of its own HBM; the variable-length
+     match tables are gathered to rank 0 (``gather_match_tables``).
 With ``verification`` the matcher's tables of each pair batch go straight into the device geometric verification (fundamental-matrix
 RANSAC, ordered inlier compaction and the per-pair gate, one launch group per batch); raw tables, verified tables and F are gathered
 to rank 0 (``gather_verified``), and ``export_verified_to_colmap`` writes the COLMAP database from the store and those results.
@@ -183,6 +183,21 @@ def verification_conf(verification) -> dict | None:
     return conf
 
 
+def kornia_conf(conf) -> dict:
+    """The ``lg_conf`` of ImageSetMatcher(matcher="kornia_matcher"), validated: KorniaMatcher's keys ``match_mode`` (nn, mnn, snn or
+    smnn; default smnn) and ``th`` (default 0.8).  A bad mode raises the plugin's NotImplementedError."""
+    from ._native import NN_MODES
+    out = {"match_mode": "smnn", "th": 0.8}
+    unknown = set(conf or {}) - set(out)
+    if unknown:
+        raise ValueError(f"unknown kornia_matcher option(s) {sorted(unknown)}; expected some of {sorted(out)}")
+    out.update(conf or {})
+    if out["match_mode"] not in NN_MODES:
+        raise NotImplementedError(f"{out['match_mode']} is not supported. Try one of {list(NN_MODES)}")
+    out["th"] = float(out["th"])
+    return out
+
+
 TILE_SELECTIONS = ("grid", "exhaustive", "preselection")
 TILING_KEYS = ("min_matches_per_tile", "tile_overlap", "tile_preselection_size", "tile_selection", "tile_size")
 
@@ -251,8 +266,9 @@ def pack_tile_batches(n_tile_pairs, batch_pairs: int) -> list:
 
 class ImageSetMatcher:
     """Two-phase multi-GPU matching of an image set (module docstring): the extractor on this rank's images into the device feature
-    store, one all_gather of the float16 feature blocks, LightGlue or SuperGlue on this rank's share of the pair list, gather of the
-    match tables.  ``dist`` is ``torch.distributed`` (initialised, nccl) or None for a single process.
+    store, one all_gather of the float16 feature blocks, the configured matcher on this rank's share of the pair list, gather of the
+    match tables.  ``dist`` is ``torch.distributed`` (initialised, nccl) or None for a single process.  ``matcher``: "lightglue"
+    (default), "superglue" or "kornia_matcher".
 
     Phase 2 is one loop over pair batches for every mode (``match`` / ``match_verified``, tiled or not): the matcher, the
     verification when asked, then the batch's results reach the host in two synchronising steps, the counts (with F and n_inliers
@@ -260,6 +276,12 @@ class ImageSetMatcher:
 
     ``matcher="superglue"``: ``lg_weights`` is the SuperGlue state dict and ``lg_conf`` its configuration (``sinkhorn_iterations``,
     ``match_threshold``, ``gnn_layers``), and phase 2 runs the batched device SuperGlue on the store's slots.
+
+    ``matcher="kornia_matcher"``: KorniaMatcher's brute-force descriptor matching (kornia DescriptorMatcher).  ``lg_conf`` holds its
+    keys ``match_mode`` (nn / mnn / snn / smnn, default smnn) and ``th`` (default 0.8), checked by ``kornia_conf``; ``lg_weights`` is
+    not used (None is accepted) and no network is built.  Phase 2 runs dimb_nn_match_batch_dev on each pair batch of store slots or tile
+    views, counts read on the device; the tables are KorniaMatcher._match_pairs' on the store's features, and the distance (nn / mnn)
+    or ratio (snn / smnn) of every match is left in the device buffer ``ms``.  SuperPoint (256-d) and ALIKED (128-d) features.
 
     ``verification``: None (default) matches only (``run`` / ``match``).  A dict (keys and defaults in ``verification_conf``) enables
     ``run_verified`` / ``match_verified``: every pair batch is verified on the device right after matching (dimb_gv_verify_dev on the
@@ -286,8 +308,8 @@ class ImageSetMatcher:
     and runs SuperPoint (``tiling.SP_PRESELECTION_CONF``) into float32 per-slot buffers (about 4.2 MB per image, all-gathered by
     ``exchange``); ``match`` runs LightGlue (``tiling.LG_PRESELECTION_CONF``, keypoints normalised by their own extent) on the
     low-resolution features of each pair batch and keeps the tile pairs with more than ``min_matches_per_tile`` matches inside both
-    boxes.  ``preselection_weights``: the weights of that LightGlue (default ``lg_weights``; required with SuperGlue).  SuperPoint
-    only: ALIKED with preselection is refused.  The per-pair flags of one ``match`` call take T^2 bytes per pair on the device and
+    boxes.  ``preselection_weights``: the weights of that LightGlue (default ``lg_weights``; required with SuperGlue and
+    kornia_matcher).  SuperPoint only: ALIKED with preselection is refused.  The per-pair flags of one ``match`` call take T^2 bytes per pair on the device and
     on the host (``_preselect``), which matters only at hundreds of tiles per image."""
 
     def __init__(self, ctx, sp_weights: dict, lg_weights: dict, n_images: int, height: int, width: int, sp_conf: dict, lg_conf: dict,
@@ -296,12 +318,13 @@ class ImageSetMatcher:
         import torch
 
         from . import _native
-        if matcher not in ("lightglue", "superglue"):
-            raise ValueError(f'matcher must be "lightglue" or "superglue", got {matcher!r}')
+        if matcher not in ("lightglue", "superglue", "kornia_matcher"):
+            raise ValueError(f'matcher must be "lightglue", "superglue" or "kornia_matcher", got {matcher!r}')
         if extractor not in ("superpoint", "aliked"):
             raise ValueError(f'extractor must be "superpoint" or "aliked", got {extractor!r}')
         if extractor == "aliked" and matcher == "superglue":
             raise ValueError("SuperGlue matches SuperPoint features only; use matcher=\"lightglue\" with ALIKED")
+        self.nn_conf = kornia_conf(lg_conf) if matcher == "kornia_matcher" else None
         self.tiling = tiling_conf(tiling)
         self.presel = self.tiling is not None and self.tiling["tile_selection"] == "preselection"
         if self.presel:
@@ -311,8 +334,8 @@ class ImageSetMatcher:
             if self.tiling["tile_preselection_size"] > max(height, width):
                 raise ValueError(f"tile_preselection_size {self.tiling['tile_preselection_size']} exceeds the image's longest side "
                                  f"{max(height, width)}: preselection only downscales")
-            if matcher == "superglue" and preselection_weights is None:
-                raise ValueError("tile preselection with matcher=\"superglue\" needs preselection_weights (SuperPoint-LightGlue weights)")
+            if matcher != "lightglue" and preselection_weights is None:
+                raise ValueError(f"tile preselection with matcher=\"{matcher}\" needs preselection_weights (SuperPoint-LightGlue weights)")
             # the down-sampled size exactly as tiling.preselection_matches computes it
             self.pre_scale = self.tiling["tile_preselection_size"] / max(height, width)
             self.pre_w, self.pre_h = (int(round(x * self.pre_scale)) for x in (width, height))
@@ -322,7 +345,7 @@ class ImageSetMatcher:
             if "fix_sampling" in sp_conf and not sp_conf["fix_sampling"]:
                 raise ValueError("tiled SuperPoint extraction runs with fix_sampling=True (the reference's rule); fix_sampling=False was given")
             sp_conf = {**sp_conf, "fix_sampling": True}
-        if extractor == "aliked":
+        if extractor == "aliked" and matcher == "lightglue":
             lg_conf = {"input_dim": 128, **lg_conf}
             if lg_conf["input_dim"] != 128:
                 raise ValueError(f"LightGlue on ALIKED features needs input_dim=128, got {lg_conf['input_dim']}")
@@ -349,7 +372,7 @@ class ImageSetMatcher:
         self.matcher = matcher
         if matcher == "superglue":
             self.sg = _native.SuperGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=self.cap, **lg_conf)
-        else:
+        elif matcher == "lightglue":
             self.lg = _native.LightGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=self.cap, **lg_conf)
         self.ipr = images_per_rank(n_images, self.world)
         store_cap = self.cap if self.tiling is None else self.T * self.cap
@@ -493,6 +516,9 @@ class ImageSetMatcher:
         if self.matcher == "superglue":
             self.sg.match_dev([store.sg_feats_dev(s) for s in s0], [store.sg_feats_dev(s) for s in s1], self.m.data_ptr(), self.ms.data_ptr(),
                               self.nm.data_ptr(), self.cap, st)
+        elif self.matcher == "kornia_matcher":  # distances / ratios go to ms
+            self.ctx.nn_match_batch_dev([store.feats_dev(s) for s in s0], [store.feats_dev(s) for s in s1], self.D, self.nn_conf["match_mode"],
+                                        self.nn_conf["th"], self.m.data_ptr(), self.ms.data_ptr(), self.nm.data_ptr(), self.cap, st)
         else:
             self.lg.match_dev([store.feats_dev(s) for s in s0], [store.feats_dev(s) for s in s1], self.m.data_ptr(), self.ms.data_ptr(),
                               self.nm.data_ptr(), self.sl.data_ptr(), self.cap, st)
@@ -597,7 +623,7 @@ class ImageSetMatcher:
         return out
 
     def match(self, pairs, pair_ids, tile_pairs=None):
-        """Phase 2: LightGlue or SuperGlue on `pairs` = [(i, j), ...] (this rank's share); returns {pair id: int64 (S,2)}.  Each pair
+        """Phase 2: the configured matcher on `pairs` = [(i, j), ...] (this rank's share); returns {pair id: int64 (S,2)}.  Each pair
         batch comes back in two synchronising steps: the counts, then only the table rows in use.  Features are read in place from the
         store (float16, no rounding left to do).  Tiled: the tables are the merged image-pair tables; `tile_pairs` optionally gives
         each pair's list of (t0, t1)."""

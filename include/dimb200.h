@@ -180,6 +180,20 @@ int dimb_nn_match(dimb_ctx* ctx, const float* d0, int n0, const float* d1, int n
  * pairs_generator.py:22-34 keeps every image's descriptors in HBM and calls this once per pair. */
 int dimb_nn_match_dev(dimb_ctx* ctx, const void* d_desc0, int n0, int ld0, const void* d_desc1, int n1, int ld1, int D, int desc_f16,
                       int mode, float th, int64_t* d_idx, float* d_dist, int* d_n, int cap, void* stream);
+/* P pairs, asynchronous on `stream`, never synchronises once its scratch has grown to the call's size.  f0[p] / f1[p] (host arrays
+ * of P): only descriptors, n (device), n_cap, desc_layout (0 only), desc_ld, f16 and round_fp16 are read; rows = min(*n, n_cap).
+ * d_idx [P][cap][2] int64, d_dist [P][cap] (distance for nn / mnn, ratio for snn / smnn), d_n [P] = the full count (only the first
+ * cap rows are written), in the order and with the empty-input rules of dimb_nn_match (kornia's).  round_fp16 = 1 rounds float32
+ * descriptors to fp16 first (round to nearest even, the features.h5 cast).  Three MMAs per product (EXACT) only when some side is
+ * float32 without round_fp16; fp16 inputs are exact with one.  Results per pair do not depend on the other pairs of the call.
+ * dimb_nn_match_dev and dimb_nn_match run this engine with P = 1.  DIMB_ERR_ARG, before any CUDA call, for a NULL ctx / array /
+ * output / descriptors / n, P < 1, cap < 1, D < 1, mode outside 0..3, n_cap < 0 or desc_layout != 0.
+ * Scratch (context slots, grow-only), NPp = the largest n_cap rounded up to 128, Dp = D rounded up to 64: the fp16 operands
+ * 2P x NPp x Dp x 2 B (twice with the three-MMA split), and the chunk partials of the top-2 GEMM, P x NPp x NPp / 32 x 12 B, shared
+ * by the two directions of mnn / smnn: about 25 MB per pair at 8192 keypoints, 1.6 MB at 2048.
+ * Runs on the CUDA-core GEMM twin (DIMB_TC=0) as well.  Profile groups: nn.prep, nn.top2_gemm, nn.merge, nn.select. */
+int dimb_nn_match_batch_dev(dimb_ctx* ctx, int P, const dimb_feats_dev* f0, const dimb_feats_dev* f1, int D, int mode, float th,
+                            int64_t* d_idx, float* d_dist, int* d_n, int cap, void* stream);
 
 /* ------------------------------------------------------------------ device feature store (the features.h5 boundary kept in HBM)
  * Replaces, for the hot path, save_features_h5 (extractors/extractor_base.py:56-99: every array cast to float16, gzip-9, one
