@@ -31,6 +31,7 @@ EXPORTS = [
     "dimb_fstore_feats_dev", "dimb_fstore_block_dev", "dimb_gv_fundamental", "dimb_gv_fundamental_batch_dev", "dimb_gv_verify_dev",
     "dimb_tile_grid", "dimb_tile_cut_dev", "dimb_tile_merge_dev", "dimb_tile_views_dev", "dimb_tile_match_merge_dev",
     "dimb_resize_area_tab", "dimb_resize_area_dev", "dimb_kpts_extent_dev", "dimb_tile_preselect_dev",
+    "dimb_resize_area_linear_tab", "dimb_resize_area_linear_dev",
 ]
 
 
@@ -171,6 +172,8 @@ def load_library():
     lib.dimb_tile_match_merge_dev.argtypes = [vp, ip, vp, vp, vp, vp, ip, vp, vp, ip, vp, vp, ip, vp]
     lib.dimb_resize_area_tab.argtypes = [ip, ip, vp, vp, vp, ip, C.POINTER(ip)]
     lib.dimb_resize_area_dev.argtypes = [vp, vp, ip, ip, ip, vp, ip, ip, vp]
+    lib.dimb_resize_area_linear_tab.argtypes = [ip, ip, vp, vp, C.POINTER(ip)]
+    lib.dimb_resize_area_linear_dev.argtypes = [vp, vp, ip, ip, ip, vp, ip, ip, vp]
     lib.dimb_kpts_extent_dev.argtypes = [vp, ip, vp, ip, vp, vp, vp]
     lib.dimb_tile_preselect_dev.argtypes = [vp, ip, C.POINTER(FeatsDev), C.POINTER(FeatsDev), vp, vp, ip] + [ip] * 6 + \
         [C.c_double, C.c_double, ip, vp, vp, vp]
@@ -299,6 +302,15 @@ def resize_area_tab(ssize: int, dsize: int):
     return di[:n.value].copy(), si[:n.value].copy(), al[:n.value].copy()
 
 
+def resize_area_linear_tab(ssize: int, dsize: int):
+    """The coefficients of one axis that dimb_resize_area_linear_dev uses when INTER_AREA enlarges (dimb_resize_area_linear_tab, no
+    GPU needed): (s_idx int32 (dsize,), alpha float32 (dsize, 2), xmax)."""
+    si, al, xmax = np.zeros(max(int(dsize), 1), np.int32), np.zeros((max(int(dsize), 1), 2), np.float32), C.c_int()
+    if load_library().dimb_resize_area_linear_tab(int(ssize), int(dsize), _ptr(si), _ptr(al), C.byref(xmax)) != OK:
+        raise ValueError(f"INTER_AREA coefficients need sizes >= 1, got ssize {ssize}, dsize {dsize}")
+    return si, al, int(xmax.value)
+
+
 class Context:
     """One per device (dimb_ctx). precision: "exact" (fp16 hi/lo split, fp32-class) or "fast" (plain fp16)."""
 
@@ -409,6 +421,11 @@ class Context:
         """cv2.resize(INTER_AREA) of B float32 gray device images [B][H][W] -> [B][H2][W2], downscaling only (dimb_resize_area_dev);
         asynchronous on `stream`."""
         self.check(self.lib.dimb_resize_area_dev(self.h, d_src, B, H, W, d_dst, H2, W2, stream), "dimb_resize_area_dev")
+
+    def resize_area_linear_dev(self, d_src, B, H, W, d_dst, H2, W2, stream=0):
+        """cv2.resize(INTER_AREA) of B float32 gray device images [B][H][W] -> [B][H2][W2] when H2 > H or W2 > W, OpenCV's bilinear
+        emulation (dimb_resize_area_linear_dev); asynchronous on `stream`."""
+        self.check(self.lib.dimb_resize_area_linear_dev(self.h, d_src, B, H, W, d_dst, H2, W2, stream), "dimb_resize_area_linear_dev")
 
     def kpts_extent_dev(self, B, d_kpts, kpt_ld, d_counts, d_size_out, stream=0):
         """Own-extent normalisation size (1 + max) - min per axis of B keypoint sets [B][kpt_ld][2] -> d_size_out [B][2] float32

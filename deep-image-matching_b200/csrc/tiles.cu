@@ -391,6 +391,50 @@ __global__ void resize_area_fast_kernel(const float* __restrict__ src, float* __
   dst[(static_cast<size_t>(b) * H2 + dy) * W2 + dx] = __fmul_rn(sum, __fdiv_rn(1.f, static_cast<float>(area)));
 }
 
+// cv::resize's coefficient loop for INTER_AREA when an axis is enlarged (area_mode, ksize 2), one axis: inv = dsize / ssize and
+// scale = 1 / inv in double, as hal::resize computes them.  Returns xmax, the first d whose sx + 1 reaches the border (dsize if none).
+int area_linear_tab(int ssize, int dsize, int* s_idx, float* alpha) {
+  const double inv = static_cast<double>(dsize) / ssize, scale = 1.0 / inv;
+  int xmax = dsize;
+  for (int d = 0; d < dsize; ++d) {
+    int sx = static_cast<int>(std::floor(d * scale));
+    float fx = static_cast<float>((d + 1) - (sx + 1) * inv);
+    fx = fx <= 0 ? 0.f : fx - std::floor(fx);
+    if (sx + 1 >= ssize) {
+      xmax = std::min(xmax, d);
+      if (sx >= ssize - 1) fx = 0.f, sx = ssize - 1;
+    }
+    s_idx[d] = sx;
+    alpha[2 * d] = 1.f - fx;
+    alpha[2 * d + 1] = fx;
+  }
+  return xmax;
+}
+
+struct LinearTab {  // per axis: the source index [dsize] and the weight pairs [dsize][2]; columns dx >= xmax copy S[sx]
+  const int *xs, *ys;
+  const float2 *xa, *ya;
+  int xmax;
+};
+
+// resizeGeneric_ with HResizeLinear / VResizeLinear in float: each of the two source rows sy and min(sy + 1, H - 1) is resampled
+// horizontally as S[sx] * a0 + S[sx + 1] * a1 (S[sx] from xmax on), then out = row0 * b0 + row1 * b1; every product and sum is
+// rounded on its own (no FMA).
+__global__ void resize_area_linear_kernel(const float* __restrict__ src, float* __restrict__ dst, int H, int W, int H2, int W2,
+                                          LinearTab t) {
+  const int dx = blockIdx.x * blockDim.x + threadIdx.x, dy = blockIdx.y, b = blockIdx.z;
+  if (dx >= W2) return;
+  const int sx = t.xs[dx], sy = t.ys[dy];
+  const float2 a = t.xa[dx], be = t.ya[dy];
+  const float* img = src + static_cast<size_t>(b) * H * W;
+  auto hrow = [&](int y) {
+    const float* S = img + static_cast<size_t>(y) * W;
+    return dx < t.xmax ? __fadd_rn(__fmul_rn(S[sx], a.x), __fmul_rn(S[sx + 1], a.y)) : S[sx];
+  };
+  const float r0 = hrow(sy), r1 = hrow(min(sy + 1, H - 1));
+  dst[(static_cast<size_t>(b) * H2 + dy) * W2 + dx] = __fadd_rn(__fmul_rn(r0, be.x), __fmul_rn(r1, be.y));
+}
+
 // One CTA per image: size = (1 + max) - min per axis over its keypoints, {1, 1} without keypoints (min / max are exact in any order).
 __global__ void __launch_bounds__(256) kpts_extent_kernel(const float* __restrict__ kpts, int ld, const int* __restrict__ counts,
                                                           float* __restrict__ out) {
@@ -663,6 +707,38 @@ int dimb_resize_area_dev(dimb_ctx* ctx, const float* d_src, int B, int height, i
                   reinterpret_cast<const float*>(d_tab + o_xa + xa.size())};
   ProfScope prof(ctx, st, "tile.resize");
   resize_area_kernel<<<grid, 128, 0, st>>>(d_src, d_dst, height, width, height2, width2, t);
+  DIMB_LAUNCH_CHECK(ctx);
+  return DIMB_OK;
+}
+
+int dimb_resize_area_linear_tab(int ssize, int dsize, int* s_idx, float* alpha, int* xmax) {
+  if (ssize < 1 || dsize < 1 || !s_idx || !alpha || !xmax) return DIMB_ERR_ARG;
+  *xmax = area_linear_tab(ssize, dsize, s_idx, alpha);
+  return DIMB_OK;
+}
+
+int dimb_resize_area_linear_dev(dimb_ctx* ctx, const float* d_src, int B, int height, int width, float* d_dst, int height2, int width2,
+                                void* stream) {
+  if (!ctx || !d_src || !d_dst || B < 1 || B > 65535 || height < 1 || width < 1 || height > (1 << 20) || width > (1 << 20) || height2 < 1 ||
+      width2 < 1 || height2 > 65535 || width2 > (1 << 20) || (height2 <= height && width2 <= width))
+    return DIMB_ERR_ARG;
+  // one upload: the x and y weight pairs (float bits, first so that the float2 reads stay aligned), then x and y sources
+  std::vector<int> hp(3 * static_cast<size_t>(width2 + height2));
+  float* xa = reinterpret_cast<float*>(hp.data());
+  float* ya = xa + 2 * width2;
+  int* xs = hp.data() + 2 * (width2 + height2);
+  int* ys = xs + width2;
+  const int xmax = area_linear_tab(width, width2, xs, xa);
+  area_linear_tab(height, height2, ys, ya);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int* d_tab;
+  DIMB_TRY(dimb_scratch(ctx, kSlotResizeTab, hp.size() * sizeof(int), reinterpret_cast<void**>(&d_tab)));
+  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_tab, hp.data(), hp.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  const float2* d_w = reinterpret_cast<const float2*>(d_tab);
+  const int* d_s = d_tab + 2 * (width2 + height2);
+  const LinearTab t{d_s, d_s + width2, d_w, d_w + width2, xmax};
+  ProfScope prof(ctx, st, "tile.resize");
+  resize_area_linear_kernel<<<dim3(ceil_div(width2, 128), height2, B), 128, 0, st>>>(d_src, d_dst, height, width, height2, width2, t);
   DIMB_LAUNCH_CHECK(ctx);
   return DIMB_OK;
 }

@@ -15,7 +15,10 @@ to rank 0 (``gather_verified``), and ``export_verified_to_colmap`` writes the CO
 With ``tiling`` (the reference's tile_size / tile_overlap / tile_selection) high-resolution images are cut into tiles on the device,
 the extractor runs over tiles and every image's tile features are merged into its slot (ExtractorBase._extract_by_tile); after the
 exchange each rank splits the merged slots into per-tile views, matches the selected tile pairs out of the views and merges their
-tables into one table per image pair (MatcherBase._match_by_tile)."""
+tables into one table per image pair (MatcherBase._match_by_tile).
+With ``pair_generation`` ("matching_lowres") the pair list itself comes from the device: low-resolution SuperPoint in phase 1, the
+exchange of those features, LightGlue over every brute-force pair dealt to the ranks, and an all_gather of the match counts that
+leaves the same kept pairs on every rank (``lowres_pairs``, ``run_lowres``)."""
 from __future__ import annotations
 
 import numpy as np
@@ -66,10 +69,10 @@ def all_gather_blocks(store_tensor, n_images: int, dist=None):
     return (world - 1) * mine.numel()
 
 
-def _gather_arrays(local_ids, arrays, n_pairs: int, width: int, dtype, dist, device):
+def _gather_arrays(local_ids, arrays, n_pairs: int, width: int, dtype, dist, device, everywhere: bool = False):
     """Gather {pair id -> `dtype` array of `width` columns and any number of rows} from all ranks to rank 0: one all_gather of every
     rank's (pair count, most rows), one of the padded arrays, each row of the padded buffer being (pair id, rows, values...).
-    Returns the list by pair id on rank 0, pairs nobody sent left None (None elsewhere)."""
+    Returns the list by pair id on rank 0, pairs nobody sent left None (None elsewhere, unless `everywhere`: then on every rank)."""
     import torch
 
     arrays = [np.asarray(a, dtype).reshape(-1, width) for a in arrays]
@@ -92,7 +95,7 @@ def _gather_arrays(local_ids, arrays, n_pairs: int, width: int, dtype, dist, dev
     buf = torch.as_tensor(buf, device=dev)
     bufs = [torch.zeros_like(buf) for _ in range(world)]
     dist.all_gather(bufs, buf)
-    if rank != 0:
+    if rank != 0 and not everywhere:
         return None
     out = [None] * n_pairs
     for r in range(world):
@@ -107,6 +110,13 @@ def gather_match_tables(local_ids, local_matches, n_pairs: int, dist=None, devic
     """Gather {pair id -> int64 (S,2)} from all ranks to rank 0 (counts all_gather + padded all_gather).
     Returns the full list on rank 0 (None elsewhere)."""
     return _gather_arrays(local_ids, local_matches, n_pairs, 2, np.int64, dist, device)
+
+
+def gather_pair_counts(local_ids, local_counts, n_pairs: int, dist=None, device=None) -> list:
+    """Gather {pair id -> int count} from all ranks to EVERY rank (the same all_gathers as ``gather_match_tables``).  Returns the
+    list of n_pairs ints by pair id on every rank."""
+    full = _gather_arrays(local_ids, [[int(c)] for c in local_counts], n_pairs, 1, np.int64, dist, device, everywhere=True)
+    return [int(a[0, 0]) for a in full]
 
 
 def gather_verified(local_ids, local_results, n_pairs: int, dist=None, device=None):
@@ -238,6 +248,31 @@ def tiling_conf(tiling) -> dict | None:
     return out
 
 
+PAIR_GENERATION_KEYS = ("min_matches", "resize_max", "strategy")
+
+
+def pair_generation_conf(pair_generation) -> dict | None:
+    """The ``pair_generation`` argument of ImageSetMatcher, validated (None stays None).  ``strategy`` is required and must be
+    "matching_lowres" (the reference's default, pairs_generator.py:40-235); ``resize_max`` (int >= 1, default 1000) is the longest
+    side of the low-resolution images and ``min_matches`` (int >= 0, default 20) the count a pair must exceed to be kept."""
+    if pair_generation is None:
+        return None
+    unknown = set(pair_generation) - set(PAIR_GENERATION_KEYS)
+    if unknown:
+        raise ValueError(f"unknown pair_generation option(s) {sorted(unknown)}; expected some of {list(PAIR_GENERATION_KEYS)}")
+    if "strategy" not in pair_generation:
+        raise ValueError("pair_generation needs strategy")
+    if pair_generation["strategy"] != "matching_lowres":
+        raise ValueError(f"pair_generation strategy {pair_generation['strategy']!r} does not run on the device (only \"matching_lowres\" "
+                         "does); pass `pairs` built with pairs_from_bruteforce or pairs_from_sequential instead")
+    out = {"strategy": "matching_lowres", "resize_max": pair_generation.get("resize_max", 1000),
+           "min_matches": pair_generation.get("min_matches", 20)}
+    for key, low in (("resize_max", 1), ("min_matches", 0)):
+        if isinstance(out[key], bool) or not isinstance(out[key], int) or out[key] < low:
+            raise ValueError(f"{key} must be an int >= {low}, got {out[key]!r}")
+    return out
+
+
 def tile_pairs_for(selection: str, n_tiles: int) -> list:
     """The tile pairs of one image pair under a configured selection (tiling.tile_selection for equally tiled images): "grid" pairs
     tile t with tile t, "exhaustive" every (t0, t1), sorted."""
@@ -262,6 +297,78 @@ def pack_tile_batches(n_tile_pairs, batch_pairs: int) -> list:
     if start < len(n_tile_pairs):
         out.append((start, len(n_tile_pairs)))
     return out
+
+
+def _lowres_size(height: int, width: int, size: int):
+    """(scale, h, w) of an image down- or up-sampled so that its longest side is `size`, as pairs_generator.read_lowres and
+    tiling.preselection_matches compute it."""
+    scale = size / max(height, width)
+    w, h = (int(round(x * scale)) for x in (width, height))
+    return scale, h, w
+
+
+class _LowResSet:
+    """The low-resolution SuperPoint + LightGlue pass shared by tile preselection and pair generation.  ``extract`` resizes each image
+    once with INTER_AREA to longest side `size` (dimb_resize_area_dev, or dimb_resize_area_linear_dev when that enlarges an axis) and
+    runs SuperPoint (`sp_conf`) into float32 buffers per store slot (no float16 cast: these features never pass through features.h5
+    in the reference), with their own extent for LightGlue without image_size; ``buffers`` are what the exchange all-gathers (about
+    (256 + 2) * 4 * K bytes per slot); ``match`` runs LightGlue (`lg_conf`) on a batch of slot pairs into m / ms / nm / sl."""
+
+    def __init__(self, ctx, sp_weights, lg_weights, n_slots, height, width, size, sp_conf, lg_conf, batch_images, batch_pairs, device):
+        import torch
+
+        from . import _native
+        self.ctx, self.H, self.W = ctx, height, width
+        self.scale, self.h, self.w = _lowres_size(height, width, size)
+        K = self.K = sp_conf["max_keypoints"]
+        self.sp = _native.SuperPointNet(ctx, sp_weights, max_batch=batch_images, max_height=self.h, max_width=self.w, **sp_conf)
+        self.lg = _native.LightGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=K, **lg_conf)
+        self.low = torch.zeros(batch_images, self.h, self.w, device=device)
+        self.sc = torch.zeros(batch_images, K, device=device)  # written by the extractor, not read
+        self.kp = torch.zeros(n_slots, K, 2, device=device)
+        self.de = torch.zeros(n_slots, 256, K, device=device)
+        self.n = torch.zeros(n_slots, dtype=torch.int32, device=device)
+        self.size = torch.zeros(n_slots, 2, device=device)
+        self.m = torch.zeros(batch_pairs, K, 2, dtype=torch.int64, device=device)
+        self.ms = torch.zeros(batch_pairs, K, device=device)
+        self.nm = torch.zeros(batch_pairs, dtype=torch.int32, device=device)
+        self.sl = torch.zeros(batch_pairs, dtype=torch.int32, device=device)
+
+    @property
+    def buffers(self):
+        return self.kp, self.de, self.n, self.size
+
+    def extract(self, d_images, slots, batch, st):
+        """The H x W images `d_images` of store slots `slots`, `batch` per resize."""
+        enlarge = self.h > self.H or self.w > self.W
+        resize = self.ctx.resize_area_linear_dev if enlarge else self.ctx.resize_area_dev
+        K = self.K
+        for b0 in range(0, len(slots), batch):
+            ss = slots[b0:b0 + batch]
+            resize(d_images[b0:b0 + len(ss)].data_ptr(), len(ss), self.H, self.W, self.low.data_ptr(), self.h, self.w, st)
+            k = 0
+            while k < len(ss):  # the extractor writes consecutive rows: one call per run of consecutive slots
+                e = k + 1
+                while e < len(ss) and ss[e] == ss[k] + (e - k):
+                    e += 1
+                s = ss[k]
+                self.sp.extract_dev(self.low[k].data_ptr(), e - k, self.h, self.w, self.kp[s].data_ptr(), self.sc[k].data_ptr(),
+                                    self.de[s].data_ptr(), self.n[s:].data_ptr(), K, st)
+                self.ctx.kpts_extent_dev(e - k, self.kp[s].data_ptr(), K, self.n[s:].data_ptr(), self.size[s].data_ptr(), st)
+                k = e
+
+    def feats(self, slot):
+        """The float32 features of a slot as LightGlue input, normalised by their own extent."""
+        from . import _native
+        K = self.K
+        return _native.FeatsDev(self.kp[slot].data_ptr(), self.de[slot].data_ptr(), self.n[slot:].data_ptr(), K, 0, K, 0.0, 0.0, 0, 0, None,
+                                self.size[slot].data_ptr())
+
+    def match(self, s0, s1, st):
+        """Enqueue LightGlue on the slot pairs (s0[k], s1[k]); returns both sides' FeatsDev lists."""
+        f0, f1 = [self.feats(s) for s in s0], [self.feats(s) for s in s1]
+        self.lg.match_dev(f0, f1, self.m.data_ptr(), self.ms.data_ptr(), self.nm.data_ptr(), self.sl.data_ptr(), self.K, st)
+        return f0, f1
 
 
 class ImageSetMatcher:
@@ -310,11 +417,21 @@ class ImageSetMatcher:
     low-resolution features of each pair batch and keeps the tile pairs with more than ``min_matches_per_tile`` matches inside both
     boxes.  ``preselection_weights``: the weights of that LightGlue (default ``lg_weights``; required with SuperGlue and
     kornia_matcher).  SuperPoint only: ALIKED with preselection is refused.  The per-pair flags of one ``match`` call take T^2 bytes per pair on the device and
-    on the host (``_preselect``), which matters only at hundreds of tiles per image."""
+    on the host (``_preselect``), which matters only at hundreds of tiles per image.
+
+    ``pair_generation``: None (default; the pair list is an input) or a dict checked by ``pair_generation_conf``, the reference's
+    default strategy "matching_lowres" (pairs_generator.pairs_from_lowres) on the device.  ``extract`` also resizes each image once
+    with INTER_AREA to longest side ``resize_max`` (enlarging too, as the reference does for small photos) and runs SuperPoint
+    (``pairs_generator.SP_LOWRES_CONF``) into float32 per-slot buffers (about 2.1 MB per image, all-gathered by ``exchange``);
+    ``lowres_pairs`` runs LightGlue (``pairs_generator.LG_LOWRES_CONF``, own-extent normalisation) over every brute-force pair, dealt to
+    the ranks, and keeps the pairs with more than ``min_matches`` matches; ``run_lowres`` then matches the kept pairs.
+    ``lowres_weights``: the weights of that LightGlue (default ``lg_weights``; required with SuperGlue and kornia_matcher).  SuperPoint
+    only: ALIKED with pair generation is refused, and so is do_geometric_verification (an unknown key)."""
 
     def __init__(self, ctx, sp_weights: dict, lg_weights: dict, n_images: int, height: int, width: int, sp_conf: dict, lg_conf: dict,
                  batch_images: int = 16, batch_pairs: int = 32, dist=None, matcher: str = "lightglue", verification: dict | None = None,
-                 tiling: dict | None = None, extractor: str = "superpoint", preselection_weights: dict | None = None):
+                 tiling: dict | None = None, extractor: str = "superpoint", preselection_weights: dict | None = None,
+                 pair_generation: dict | None = None, lowres_weights: dict | None = None):
         import torch
 
         from . import _native
@@ -336,11 +453,17 @@ class ImageSetMatcher:
                                  f"{max(height, width)}: preselection only downscales")
             if matcher != "lightglue" and preselection_weights is None:
                 raise ValueError(f"tile preselection with matcher=\"{matcher}\" needs preselection_weights (SuperPoint-LightGlue weights)")
-            # the down-sampled size exactly as tiling.preselection_matches computes it
-            self.pre_scale = self.tiling["tile_preselection_size"] / max(height, width)
-            self.pre_w, self.pre_h = (int(round(x * self.pre_scale)) for x in (width, height))
-            if min(self.pre_h, self.pre_w) < 1:
+            if min(_lowres_size(height, width, self.tiling["tile_preselection_size"])[1:]) < 1:
                 raise ValueError(f"tile_preselection_size {self.tiling['tile_preselection_size']} down-samples a {height}x{width} image to nothing")
+        self.pairgen = pair_generation_conf(pair_generation)
+        if self.pairgen is not None:
+            if extractor == "aliked":
+                raise ValueError("pair generation runs SuperPoint on gray low-resolution images (the reference reads them as gray) and is "
+                                 "available with extractor=\"superpoint\" only; pass pairs with ALIKED")
+            if matcher != "lightglue" and lowres_weights is None:
+                raise ValueError(f"pair generation with matcher=\"{matcher}\" needs lowres_weights (SuperPoint-LightGlue weights)")
+            if min(_lowres_size(height, width, self.pairgen["resize_max"])[1:]) < 1:
+                raise ValueError(f"resize_max {self.pairgen['resize_max']} down-samples a {height}x{width} image to nothing")
         if self.tiling is not None and extractor == "superpoint":
             if "fix_sampling" in sp_conf and not sp_conf["fix_sampling"]:
                 raise ValueError("tiled SuperPoint extraction runs with fix_sampling=True (the reference's rule); fix_sampling=False was given")
@@ -402,28 +525,21 @@ class ImageSetMatcher:
             self.cap2 = gv_cap = min(batch_pairs, self.T * self.T) * self.cap
             self.mm = torch.zeros(batch_pairs, self.cap2, 2, dtype=torch.int64, device=dev)
             self.nmm = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
+        self.pre = self.lowres = None
         if self.presel:
-            # PRESELECTION (matcher_base.py:1055-1089) on the device: the networks of matcher_base.py:143-159, float32 low-resolution
-            # features per store slot (they never pass through features.h5 in the reference: no float16 cast), their own-extent size
-            # for LightGlue without image_size, and the outputs of one pair batch
+            # PRESELECTION (matcher_base.py:1055-1089) on the device with the networks of matcher_base.py:143-159, and the box counts
+            # of one pair batch
             from .tiling import LG_PRESELECTION_CONF, SP_PRESELECTION_CONF
-            K = self.pre_k = SP_PRESELECTION_CONF["max_keypoints"]
-            S = self.world * self.ipr
-            self.sp_pre = _native.SuperPointNet(ctx, sp_weights, max_batch=batch_images, max_height=self.pre_h, max_width=self.pre_w,
-                                                **SP_PRESELECTION_CONF)
-            self.lg_pre = _native.LightGlueNet(ctx, lg_weights if preselection_weights is None else preselection_weights,
-                                               max_pairs=batch_pairs, max_kpts=K, **LG_PRESELECTION_CONF)
-            self.low = torch.zeros(batch_images, self.pre_h, self.pre_w, device=dev)
-            self.pre_sc = torch.zeros(batch_images, K, device=dev)  # written by the extractor, not read by preselection
-            self.pre_kp = torch.zeros(S, K, 2, device=dev)
-            self.pre_de = torch.zeros(S, 256, K, device=dev)
-            self.pre_n = torch.zeros(S, dtype=torch.int32, device=dev)
-            self.pre_size = torch.zeros(S, 2, device=dev)
-            self.pre_m = torch.zeros(batch_pairs, K, 2, dtype=torch.int64, device=dev)
-            self.pre_ms = torch.zeros(batch_pairs, K, device=dev)
-            self.pre_nm = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
-            self.pre_sl = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
+            self.pre = _LowResSet(ctx, sp_weights, lg_weights if preselection_weights is None else preselection_weights, self.world * self.ipr,
+                                  height, width, self.tiling["tile_preselection_size"], SP_PRESELECTION_CONF, LG_PRESELECTION_CONF,
+                                  batch_images, batch_pairs, dev)
+            self.pre_h, self.pre_w = self.pre.h, self.pre.w
             self.pre_cnt = torch.zeros(batch_pairs, self.T * self.T, dtype=torch.int32, device=dev)
+        if self.pairgen is not None:
+            # matching_lowres (pairs_generator.py:40-235) with the networks of pairs_generator.py:104-126
+            from .pairs_generator import LG_LOWRES_CONF, SP_LOWRES_CONF
+            self.lowres = _LowResSet(ctx, sp_weights, lg_weights if lowres_weights is None else lowres_weights, self.world * self.ipr, height,
+                                     width, self.pairgen["resize_max"], SP_LOWRES_CONF, LG_LOWRES_CONF, batch_images, batch_pairs, dev)
         self.gv = verification_conf(verification)
         if self.gv is not None and self.gv["method"] != "NONE":  # verification outputs of one pair batch
             self.v = torch.zeros(batch_pairs, gv_cap, 2, dtype=torch.int64, device=dev)
@@ -443,9 +559,10 @@ class ImageSetMatcher:
         """Phase 1: d_images = float32 CUDA tensor holding this rank's images `image_ids`, 0..255: (k, H, W) gray for SuperPoint,
         (k, H, W, 3) RGB for ALIKED.  With tiling the images are full size and are cut into tiles on the device."""
         st = self.torch.cuda.current_stream().cuda_stream
+        for low in (self.pre, self.lowres):
+            if low is not None:
+                low.extract(d_images, [self.slots[i] for i in image_ids], self.B, st)
         if self.tiling is not None:
-            if self.presel:
-                self._extract_preselection(d_images, image_ids, st)
             return self._extract_tiled(d_images, image_ids, st)
         for b0 in range(0, len(image_ids), self.B):
             ids = image_ids[b0:b0 + self.B]
@@ -465,26 +582,6 @@ class ImageSetMatcher:
             else:
                 self.al.extract_dev(src[r].data_ptr(), h, w, 3, *ptrs)
 
-    def _extract_preselection(self, d_images, image_ids, st):
-        """PRESELECTION's low-resolution extraction, once per image: INTER_AREA down-sampling, SuperPoint into the image's slot rows of
-        the float32 preselection buffers, and the own extent of its keypoints."""
-        K = self.pre_k
-        for b0 in range(0, len(image_ids), self.B):
-            ids = image_ids[b0:b0 + self.B]
-            self.ctx.resize_area_dev(d_images[b0:b0 + len(ids)].data_ptr(), len(ids), self.H, self.W, self.low.data_ptr(), self.pre_h,
-                                     self.pre_w, st)
-            slots = [self.slots[i] for i in ids]
-            k = 0
-            while k < len(ids):  # the extractor writes consecutive rows: one call per run of consecutive slots
-                e = k + 1
-                while e < len(ids) and slots[e] == slots[k] + (e - k):
-                    e += 1
-                s = slots[k]
-                self.sp_pre.extract_dev(self.low[k].data_ptr(), e - k, self.pre_h, self.pre_w, self.pre_kp[s].data_ptr(), self.pre_sc[k].data_ptr(),
-                                        self.pre_de[s].data_ptr(), self.pre_n[s:].data_ptr(), K, st)
-                self.ctx.kpts_extent_dev(e - k, self.pre_kp[s].data_ptr(), K, self.pre_n[s:].data_ptr(), self.pre_size[s].data_ptr(), st)
-                k = e
-
     def _extract_tiled(self, d_images, image_ids, st):
         """Groups of G images: tile cut, the extractor over their G * T tiles, one tile merge into their slots."""
         (th, tw), (oh, ow) = self.tiling["tile_hw"], self.tiling["overlap_hw"]
@@ -500,9 +597,10 @@ class ImageSetMatcher:
         """The collective of the path: every rank's float16 feature blocks to every rank (NCCL all_gather over NVLink).  With tiling,
         every rank then builds the per-tile views of all images from the merged slots."""
         self.exchanged_bytes = all_gather_blocks(self.store_t, self.n, self.dist)
-        if self.presel:  # the low-resolution features of every image, for the preselection of any pair
-            for t in (self.pre_kp, self.pre_de, self.pre_n, self.pre_size):
-                self.exchanged_bytes += all_gather_blocks(t.view(self.torch.uint8).view(t.shape[0], -1), self.n, self.dist)
+        for low in (self.pre, self.lowres):  # the low-resolution features of every image, for any pair
+            if low is not None:
+                for t in low.buffers:
+                    self.exchanged_bytes += all_gather_blocks(t.view(self.torch.uint8).view(t.shape[0], -1), self.n, self.dist)
         if self.tiling is not None:
             st = self.torch.cuda.current_stream().cuda_stream
             step = max(1, 65535 // self.T)
@@ -523,13 +621,6 @@ class ImageSetMatcher:
             self.lg.match_dev([store.feats_dev(s) for s in s0], [store.feats_dev(s) for s in s1], self.m.data_ptr(), self.ms.data_ptr(),
                               self.nm.data_ptr(), self.sl.data_ptr(), self.cap, st)
 
-    def _pre_feats(self, slot):
-        """The float32 low-resolution features of a slot as LightGlue input, normalised by their own extent."""
-        from . import _native
-        K = self.pre_k
-        return _native.FeatsDev(self.pre_kp[slot].data_ptr(), self.pre_de[slot].data_ptr(), self.pre_n[slot:].data_ptr(), K, 0, K, 0.0, 0.0,
-                                0, 0, None, self.pre_size[slot].data_ptr())
-
     def _preselect(self, pairs):
         """PRESELECTION tile-pair lists of `pairs` (tiling.preselection_matches + tiling.tile_selection): per batch of batch_pairs,
         LightGlue on the low-resolution slots and the tile box count, then ONE device->host copy of every pair's flags.  Row-major
@@ -537,16 +628,14 @@ class ImageSetMatcher:
         counts of one batch (allocated with the matcher) batch_pairs * T^2 int32; at T in the tens that is kilobytes per pair, but at
         hundreds of tiles per image it reaches megabytes per pair, so a very large pair list is better matched in several calls."""
         st = self.torch.cuda.current_stream().cuda_stream
-        T, K = self.T, self.pre_k
+        T, pre = self.T, self.pre
         (th, tw), (oh, ow) = self.tiling["tile_hw"], self.tiling["overlap_hw"]
         flags = self.torch.zeros(max(len(pairs), 1), T * T, dtype=self.torch.uint8, device=self.pre_cnt.device)
         for b0 in range(0, len(pairs), self.P):
             chunk = pairs[b0:b0 + self.P]
-            f0 = [self._pre_feats(self.slots[i]) for i, _ in chunk]
-            f1 = [self._pre_feats(self.slots[j]) for _, j in chunk]
-            self.lg_pre.match_dev(f0, f1, self.pre_m.data_ptr(), self.pre_ms.data_ptr(), self.pre_nm.data_ptr(), self.pre_sl.data_ptr(), K, st)
-            self.ctx.tile_preselect_dev(f0, f1, self.pre_m.data_ptr(), self.pre_nm.data_ptr(), K, self.H, self.W, th, tw, oh, ow, self.pre_scale,
-                                        self.pre_scale, self.tiling["min_matches_per_tile"], self.pre_cnt.data_ptr(), flags[b0].data_ptr(), st)
+            f0, f1 = pre.match([self.slots[i] for i, _ in chunk], [self.slots[j] for _, j in chunk], st)
+            self.ctx.tile_preselect_dev(f0, f1, pre.m.data_ptr(), pre.nm.data_ptr(), pre.K, self.H, self.W, th, tw, oh, ow, pre.scale, pre.scale,
+                                        self.tiling["min_matches_per_tile"], self.pre_cnt.data_ptr(), flags[b0].data_ptr(), st)
         fl = flags[:len(pairs)].cpu().numpy().reshape(-1, T, T)
         return [[(int(a), int(b)) for a, b in zip(*np.nonzero(f))] for f in fl]
 
@@ -640,10 +729,49 @@ class ImageSetMatcher:
             return {k: (m, m.copy(), None, len(m)) for k, m in self.match(pairs, pair_ids, tile_pairs).items()}
         return self._match_batches(pairs, pair_ids, tile_pairs, verify=True)
 
+    def lowres_pairs(self):
+        """Pair generation "matching_lowres" (pairs_generator.pairs_from_lowres) on the low-resolution features, after ``exchange``.
+        The brute-force pairs (i < j, pairs_from_bruteforce order) are dealt by their keypoint products (one small device->host copy of
+        the counts), LightGlue runs on this rank's share per batch of batch_pairs, each batch's match counts are copied into one device
+        array without a host synchronise, and one device->host copy and an all_gather give every rank all counts.  Returns
+        (pairs, counts), the same on every rank: the pairs with more than ``min_matches`` matches, and the count of every brute-force
+        pair.  Memory: the low-resolution set holds (256 + 2) * 4 * 2048 bytes, about 2.1 MB, per image on every rank (2 GB at 1000
+        images)."""
+        from .pairs_generator import pairs_from_bruteforce
+        if self.lowres is None:
+            raise RuntimeError("ImageSetMatcher was built without pair_generation")
+        torch, low = self.torch, self.lowres
+        st = torch.cuda.current_stream().cuda_stream
+        brute = pairs_from_bruteforce(range(self.n))
+        n = low.n.cpu().numpy()[self.slots].astype(np.int64)
+        mine = shard_pairs(len(brute), self.world, self.rank, [n[i] * n[j] for i, j in brute])
+        counts = torch.zeros(max(len(mine), 1), dtype=torch.int32, device=low.nm.device)
+        for b0 in range(0, len(mine), self.P):
+            chunk = [brute[k] for k in mine[b0:b0 + self.P]]
+            low.match([self.slots[i] for i, _ in chunk], [self.slots[j] for _, j in chunk], st)
+            counts[b0:b0 + len(chunk)].copy_(low.nm[:len(chunk)])
+        counts = gather_pair_counts(mine, counts[:len(mine)].cpu().numpy(), len(brute), self.dist if self.world > 1 else None,
+                                    torch.device("cuda", self.ctx.device) if self.world > 1 else None)
+        return [p for p, c in zip(brute, counts) if c > self.pairgen["min_matches"]], counts
+
+    def run_lowres(self, d_images, my_image_ids, verified: bool = False):
+        """extract -> exchange -> ``lowres_pairs`` -> ``match`` (``match_verified`` with `verified`) on this rank's share of the kept
+        pairs -> gather to rank 0.  Returns (pairs, counts, results): the kept pairs and every brute-force pair's count on every rank,
+        and on rank 0 the results per kept pair as ``run`` / ``run_verified`` return them (None elsewhere).  With tiling, the configured
+        tile selection applies to the kept pairs."""
+        self.extract(d_images, my_image_ids)
+        self.exchange()
+        pairs, counts = self.lowres_pairs()
+        match, gather = (self.match_verified, gather_verified) if verified else (self.match, gather_match_tables)
+        return pairs, counts, self._match_share(match, gather, pairs, None, None)
+
     def _run(self, match, gather, d_images, my_image_ids, pairs, costs, tile_pairs):
         """extract -> exchange -> `match` on this rank's share of `pairs` -> `gather` to rank 0."""
         self.extract(d_images, my_image_ids)
         self.exchange()
+        return self._match_share(match, gather, pairs, costs, tile_pairs)
+
+    def _match_share(self, match, gather, pairs, costs, tile_pairs):
         mine = shard_pairs(len(pairs), self.world, self.rank, costs)
         res = match([pairs[k] for k in mine], mine, None if tile_pairs is None else [tile_pairs[k] for k in mine])
         return gather(mine, [res[k] for k in mine], len(pairs), self.dist if self.world > 1 else None,

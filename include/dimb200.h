@@ -318,6 +318,20 @@ int dimb_resize_area_tab(int ssize, int dsize, int* d_idx, int* s_idx, float* al
  * switches to a bilinear variant there) is refused: DIMB_ERR_ARG for H2 > H or W2 > W.  B, H2 <= 65535. */
 int dimb_resize_area_dev(dimb_ctx* ctx, const float* d_src, int B, int height, int width, float* d_dst, int height2, int width2,
                          void* stream);
+/* INTER_AREA when an axis is enlarged (pairs_generator.py's read_lowres enlarges small photos to resize_max): OpenCV then runs
+ * cv::resize's area_mode, a bilinear emulation on BOTH axes, as soon as one factor dsize / ssize exceeds 1.  Host only (no CUDA
+ * call): the coefficients of one axis for any 1 <= ssize, dsize, per destination index d (OpenCV's coefficient loop in double with
+ * inv = dsize / ssize, scale = 1 / inv): sx = floor(d * scale), fx = float((d + 1) - (sx + 1) * inv), fx = fx <= 0 ? 0 : fx - floor(fx);
+ * where sx + 1 >= ssize the first such d is *xmax (dsize if none), and for sx >= ssize - 1, sx = ssize - 1 and fx = 0.
+ * Out: s_idx [dsize], alpha [dsize][2] = {1 - fx, fx}.  DIMB_ERR_ARG for a size below 1 or a NULL pointer. */
+int dimb_resize_area_linear_tab(int ssize, int dsize, int* s_idx, float* alpha, int* xmax);
+/* B float32 gray images d_src [B][H][W] -> d_dst [B][H2][W2], bitwise cv2.resize(INTER_AREA) when H2 > H or W2 > W (resizeGeneric_
+ * with HResizeLinear / VResizeLinear in float over the tables above): each of the source rows sy and min(sy + 1, H - 1) is resampled
+ * as S[sx] * a0 + S[sx + 1] * a1 (S[sx] alone for columns from xmax on), then out = row0 * b0 + row1 * b1, the weights unchanged when
+ * the second row is clamped; every product and sum rounded separately (no FMA).  DIMB_ERR_ARG when no axis is enlarged (use
+ * dimb_resize_area_dev), otherwise the argument limits of dimb_resize_area_dev; profile group tile.resize.  CUDA cores. */
+int dimb_resize_area_linear_dev(dimb_ctx* ctx, const float* d_src, int B, int height, int width, float* d_dst, int height2, int width2,
+                                void* stream);
 /* normalize_keypoints' own-extent size for LightGlue without image_size (lightglue.py:26-27): per image b, over its
  * min(d_counts[b], kpt_ld) keypoints of d_kpts [B][kpt_ld][2] float32, d_size_out[b] = {(1 + max x) - min x, (1 + max y) - min y}
  * in float32, as dimb_lg_match computes it on the host; {1, 1} for an image without keypoints.  Feed it to dimb_lg_match_dev
