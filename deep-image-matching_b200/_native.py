@@ -31,7 +31,7 @@ EXPORTS = [
     "dimb_fstore_feats_dev", "dimb_fstore_block_dev", "dimb_gv_fundamental", "dimb_gv_fundamental_batch_dev", "dimb_gv_verify_dev",
     "dimb_tile_grid", "dimb_tile_cut_dev", "dimb_tile_merge_dev", "dimb_tile_views_dev", "dimb_tile_match_merge_dev",
     "dimb_resize_area_tab", "dimb_resize_area_dev", "dimb_kpts_extent_dev", "dimb_tile_preselect_dev",
-    "dimb_resize_area_linear_tab", "dimb_resize_area_linear_dev",
+    "dimb_resize_area_linear_tab", "dimb_resize_area_linear_dev", "dimb_pyr_size", "dimb_pyr_dev", "dimb_fstore_rescale_dev",
 ]
 
 
@@ -174,6 +174,9 @@ def load_library():
     lib.dimb_resize_area_dev.argtypes = [vp, vp, ip, ip, ip, vp, ip, ip, vp]
     lib.dimb_resize_area_linear_tab.argtypes = [ip, ip, vp, vp, C.POINTER(ip)]
     lib.dimb_resize_area_linear_dev.argtypes = [vp, vp, ip, ip, ip, vp, ip, ip, vp]
+    lib.dimb_pyr_size.argtypes = [ip, ip, ip, C.POINTER(ip), C.POINTER(ip)]
+    lib.dimb_pyr_dev.argtypes = [vp, vp, ip, ip, ip, ip, ip, vp, vp]
+    lib.dimb_fstore_rescale_dev.argtypes = [vp, ip, vp, ip, ip, ip, vp]
     lib.dimb_kpts_extent_dev.argtypes = [vp, ip, vp, ip, vp, vp, vp]
     lib.dimb_tile_preselect_dev.argtypes = [vp, ip, C.POINTER(FeatsDev), C.POINTER(FeatsDev), vp, vp, ip] + [ip] * 6 + \
         [C.c_double, C.c_double, ip, vp, vp, vp]
@@ -311,6 +314,15 @@ def resize_area_linear_tab(ssize: int, dsize: int):
     return si, al, int(xmax.value)
 
 
+def pyr_size(height: int, width: int, level: int):
+    """(H2, W2) of an image after `level` pyramid steps (dimb_pyr_size, no GPU needed): -1 one cv2.pyrUp, 0 none, 1..3 that many
+    cv2.pyrDown."""
+    h2, w2 = C.c_int(), C.c_int()
+    if load_library().dimb_pyr_size(int(height), int(width), int(level), C.byref(h2), C.byref(w2)) != OK:
+        raise ValueError(f"pyramid steps need a level in [-1, 3] and sizes in [1, 2^20], got {height}x{width}, level {level}")
+    return h2.value, w2.value
+
+
 class Context:
     """One per device (dimb_ctx). precision: "exact" (fp16 hi/lo split, fp32-class) or "fast" (plain fp16)."""
 
@@ -426,6 +438,11 @@ class Context:
         """cv2.resize(INTER_AREA) of B float32 gray device images [B][H][W] -> [B][H2][W2] when H2 > H or W2 > W, OpenCV's bilinear
         emulation (dimb_resize_area_linear_dev); asynchronous on `stream`."""
         self.check(self.lib.dimb_resize_area_linear_dev(self.h, d_src, B, H, W, d_dst, H2, W2, stream), "dimb_resize_area_linear_dev")
+
+    def pyr_dev(self, d_src, B, H, W, channels, level, d_dst, stream=0):
+        """cv2.pyrDown `level` times (1..3) or cv2.pyrUp once (-1) of B float32 device images [B][H][W][channels], 1 or 3 channels,
+        into d_dst [B][H2][W2][channels] (pyr_size), bitwise (dimb_pyr_dev); asynchronous on `stream`."""
+        self.check(self.lib.dimb_pyr_dev(self.h, d_src, B, H, W, channels, level, d_dst, stream), "dimb_pyr_dev")
 
     def kpts_extent_dev(self, B, d_kpts, kpt_ld, d_counts, d_size_out, stream=0):
         """Own-extent normalisation size (1 + max) - min per axis of B keypoint sets [B][kpt_ld][2] -> d_size_out [B][2] float32
@@ -824,6 +841,12 @@ class FeatureStoreDev:
         s, p = _int_array(slots)
         self.ctx.check(self.ctx.lib.dimb_tile_merge_dev(self.h, len(s), p, H, W, tile_h, tile_w, overlap_h, overlap_w, d_kpts, d_scores, d_desc,
                                                         d_counts, K, stream), "dimb_tile_merge_dev")
+
+    def rescale_dev(self, slots, level, H, W, stream=0):
+        """Keypoints of `slots` times 2^level and header image size H x W (dimb_fstore_rescale_dev): features extracted from an image
+        resized by `level` pyramid steps, back in the original image's pixels.  Asynchronous on `stream`."""
+        s, p = _int_array(slots)
+        self.ctx.check(self.ctx.lib.dimb_fstore_rescale_dev(self.h, len(s), p, int(level), int(H), int(W), stream), "dimb_fstore_rescale_dev")
 
     def tile_views_dev(self, src_slots, n_tiles, views: "FeatureStoreDev", dst_slots, d_map, stream=0):
         """Tile views of the merged slots src_slots (dimb_tile_views_dev): view slot dst_slots[b] + t of `views`, map row of the same

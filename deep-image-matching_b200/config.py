@@ -36,7 +36,7 @@ class Config:
     def __init__(self, general: dict | None = None, extractor: dict | None = None, matcher: dict | None = None,
                  pipeline: str | None = None):
         base = confs.get(pipeline, {"extractor": {}, "matcher": {}}) if pipeline else {"extractor": {}, "matcher": {}}
-        self.general = {"output_dir": Path("."), "verbose": False, "device": 0, "tile_size": (2400, 2000), "tile_overlap": 10,
-                        **(general or {})}  # tile defaults: config.py:61-63
+        self.general = {"output_dir": Path("."), "verbose": False, "device": 0, "quality": "high", "tile_size": (2400, 2000),
+                        "tile_overlap": 10, **(general or {})}  # tile defaults: config.py:61-63; quality: "high", the reference's default
         self.extractor = {**base["extractor"], **(extractor or {})}
         self.matcher = {**base["matcher"], **(matcher or {})}

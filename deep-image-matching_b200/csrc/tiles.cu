@@ -25,7 +25,7 @@ constexpr int kMaxTiles = 2048;        // tile_idx is stored as float16: integer
 constexpr int kChunk = 1024;           // records per shared-memory sort
 constexpr int kScanThreads = 1024;     // threads of the one-CTA-per-segment scans
 constexpr int kSlotKeysA = 64, kSlotKeysB = 65, kSlotParams = 66, kSlotSrc = 67, kSlotCount = 68;  // context scratch slots
-constexpr int kSlotResizeTab = 69, kSlotPreSides = 70;
+constexpr int kSlotResizeTab = 69, kSlotPreSides = 70, kSlotPyrA = 71, kSlotPyrB = 72, kSlotRescale = 73;
 constexpr int kCvFloatLanes = 4;        // float32 lanes of OpenCV's 128-bit baseline SIMD (ResizeAreaFastVec_SIMD_32f)
 constexpr unsigned long long kNoKey = ~0ull;
 constexpr int kBorder = 2;             // border_thr of extractor_base.py:335
@@ -435,6 +435,94 @@ __global__ void resize_area_linear_kernel(const float* __restrict__ src, float* 
   dst[(static_cast<size_t>(b) * H2 + dy) * W2 + dx] = __fadd_rn(__fmul_rn(r0, be.x), __fmul_rn(r1, be.y));
 }
 
+// cv::borderInterpolate with BORDER_REFLECT_101 (BORDER_DEFAULT): gfedcb|abcdefgh|gfedcba.
+__host__ __device__ __forceinline__ int reflect101(int p, int n) {
+  if (n == 1) return 0;
+  while (p < 0 || p >= n) p = p < 0 ? -p : 2 * n - 2 - p;
+  return p;
+}
+
+// The 1 4 6 4 1 tap sum of pyrDown_ in its two orders: OpenCV's scalar loops, s2 * 6 + (s1 + s3) * 4 + s0 + s4 left to right, and its
+// baseline-SIMD horizontal loop (PyrDownVecH, v_muladd without FMA), s2 * 6 + ((s1 + s3) * 4 + (s0 + s4)).
+__device__ __forceinline__ float pyr5_scalar(float s0, float s1, float s2, float s3, float s4) {
+  return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(s2, 6.f), __fmul_rn(__fadd_rn(s1, s3), 4.f)), s0), s4);
+}
+__device__ __forceinline__ float pyr5_vec(float s0, float s1, float s2, float s3, float s4) {
+  return __fadd_rn(__fmul_rn(s2, 6.f), __fadd_rn(__fmul_rn(__fadd_rn(s1, s3), 4.f), __fadd_rn(s0, s4)));
+}
+
+// cv::pyrDown (pyrDown_ with FltCast<float, 8>) of B images [H][W][C] -> [H2][W2][C], H2 = (H + 1) / 2, W2 = (W + 1) / 2; one
+// thread per output value.  Horizontal pass per source row: output column 0 and the columns from width0 = min((W - 3) / 2 + 1, W2)
+// on (the tabR border columns) use the scalar order, and so does the scalar tail of the vector loop, which covers columns
+// [1, 1 + floor((width0 - 1) / 4) * 4) for C = 1 and [1, width0 - 1) for C = 3 (one pixel per 4-lane step).  Vertical pass over the
+// five rows 2y - 2 .. 2y + 2 (reflect-101): PyrDownVecV's ((r1 + r3) + r2) * 4 + ((r0 + r4) + (r2 + r2)) on the first
+// floor(W2 * C / 4) * 4 values of the row, the scalar order on the rest, then * (1 / 256).  Every operation rounded on its own.
+__global__ void __launch_bounds__(128) pyr_down_kernel(const float* __restrict__ src, float* __restrict__ dst, int H, int W, int C, int H2,
+                                                       int W2) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, b = blockIdx.z;
+  const int row_len = W2 * C;
+  if (j >= row_len) return;
+  const int x = j / C, c = j - x * C;
+  const int width0 = min((W - 3) / 2 + 1, W2);  // C division truncates: 0 for W = 1
+  const bool hvec = C == 1 ? (x >= 1 && x < 1 + (width0 - 1) / 4 * 4) : (x >= 1 && x < width0 - 1);
+  int sx[5];
+#pragma unroll
+  for (int k = 0; k < 5; ++k) sx[k] = reflect101(2 * x - 2 + k, W) * C + c;
+  const float* img = src + static_cast<size_t>(b) * H * W * C;
+  float r[5];
+#pragma unroll
+  for (int k = 0; k < 5; ++k) {
+    const float* S = img + static_cast<size_t>(reflect101(2 * y - 2 + k, H)) * W * C;
+    r[k] = hvec ? pyr5_vec(S[sx[0]], S[sx[1]], S[sx[2]], S[sx[3]], S[sx[4]]) : pyr5_scalar(S[sx[0]], S[sx[1]], S[sx[2]], S[sx[3]], S[sx[4]]);
+  }
+  const float v = j < (row_len & ~(kCvFloatLanes - 1))
+                      ? __fadd_rn(__fmul_rn(__fadd_rn(__fadd_rn(r[1], r[3]), r[2]), 4.f), __fadd_rn(__fadd_rn(r[0], r[4]), __fadd_rn(r[2], r[2])))
+                      : pyr5_scalar(r[0], r[1], r[2], r[3], r[4]);
+  dst[(static_cast<size_t>(b) * H2 + y) * row_len + j] = __fmul_rn(v, 1.f / 256.f);
+}
+
+// cv::pyrUp (pyrUp_ with FltCast<float, 6>) of B images [H][W][C] -> [2H][2W][C]; one thread per output value.  Horizontal pass per
+// source row, output column X of source column x = X / 2: even X gives (S[x - 1] + S[x] * 6) + S[x + 1], odd X (S[x] + S[x + 1]) * 4,
+// except at the borders: X = 0 gives S[0] * 6 + S[1] * 2, X = 2W - 2 gives S[W - 2] + S[W - 1] * 7, X = 2W - 1 gives S[W - 1] * 8, and
+// a one-column image gives S[0] * 8 on both.  Vertical pass over the source rows y - 1, y, y + 1 of y = Y / 2 (row s read at
+// reflect101(2s, 2H) / 2): even Y gives (r0 + r1 * 6) + r2, odd Y (r1 + r2) * 4, then * (1 / 64).  Every operation rounded on its own.
+__global__ void __launch_bounds__(128) pyr_up_kernel(const float* __restrict__ src, float* __restrict__ dst, int H, int W, int C) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x, Y = blockIdx.y, b = blockIdx.z;
+  const int row_len = 2 * W * C;
+  if (j >= row_len) return;
+  const int X = j / C, c = j - X * C, x = X >> 1;
+  const bool odd = X & 1;
+  const float* img = src + static_cast<size_t>(b) * H * W * C;
+  auto hrow = [&](int sy) {
+    const float* S = img + static_cast<size_t>(sy) * W * C + c;
+    if (W == 1) return __fmul_rn(S[0], 8.f);
+    if (odd) return x == W - 1 ? __fmul_rn(S[x * C], 8.f) : __fmul_rn(__fadd_rn(S[x * C], S[(x + 1) * C]), 4.f);
+    if (x == 0) return __fadd_rn(__fmul_rn(S[0], 6.f), __fmul_rn(S[C], 2.f));
+    if (x == W - 1) return __fadd_rn(S[(x - 1) * C], __fmul_rn(S[x * C], 7.f));
+    return __fadd_rn(__fadd_rn(S[(x - 1) * C], __fmul_rn(S[x * C], 6.f)), S[(x + 1) * C]);
+  };
+  const int y = Y >> 1;
+  const float r1 = hrow(y), r2 = hrow(reflect101(2 * y + 2, 2 * H) / 2);
+  const float v = (Y & 1) ? __fmul_rn(__fadd_rn(r1, r2), 4.f)
+                          : __fadd_rn(__fadd_rn(hrow(reflect101(2 * y - 2, 2 * H) / 2), __fmul_rn(r1, 6.f)), r2);
+  dst[(static_cast<size_t>(b) * 2 * H + Y) * row_len + j] = __fmul_rn(v, 1.f / 64.f);
+}
+
+// Multiplies the float16 keypoints of B store slots by `scale` (a power of two) and writes [H, W] into their headers as
+// fs_put_kernel does.  grid (cap / 256, B); empty slots are left alone.
+__global__ void fs_rescale_kernel(FsLayout L, const int* __restrict__ slots, float scale, int H, int W) {
+  const SlotPtrs s = L.at(slots[blockIdx.y]);
+  if (!s.hdr[3]) return;
+  const int n = min(s.hdr[0], L.cap), i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    s.hdr[1] = static_cast<int>(__half2float(__float2half_rn(fminf(static_cast<float>(H), 65504.f))));
+    s.hdr[2] = static_cast<int>(__half2float(__float2half_rn(fminf(static_cast<float>(W), 65504.f))));
+  }
+  if (i >= n) return;
+  s.kpts[2 * i] = __float2half_rn(__fmul_rn(__half2float(s.kpts[2 * i]), scale));
+  s.kpts[2 * i + 1] = __float2half_rn(__fmul_rn(__half2float(s.kpts[2 * i + 1]), scale));
+}
+
 // One CTA per image: size = (1 + max) - min per axis over its keypoints, {1, 1} without keypoints (min / max are exact in any order).
 __global__ void __launch_bounds__(256) kpts_extent_kernel(const float* __restrict__ kpts, int ld, const int* __restrict__ counts,
                                                           float* __restrict__ out) {
@@ -739,6 +827,68 @@ int dimb_resize_area_linear_dev(dimb_ctx* ctx, const float* d_src, int B, int he
   const LinearTab t{d_s, d_s + width2, d_w, d_w + width2, xmax};
   ProfScope prof(ctx, st, "tile.resize");
   resize_area_linear_kernel<<<dim3(ceil_div(width2, 128), height2, B), 128, 0, st>>>(d_src, d_dst, height, width, height2, width2, t);
+  DIMB_LAUNCH_CHECK(ctx);
+  return DIMB_OK;
+}
+
+int dimb_pyr_size(int height, int width, int level, int* height2, int* width2) {
+  if (!height2 || !width2 || level < -1 || level > 3 || height < 1 || width < 1 || height > (1 << 20) || width > (1 << 20)) return DIMB_ERR_ARG;
+  int h = height, w = width;
+  if (level < 0) h *= 2, w *= 2;
+  for (int l = 0; l < level; ++l) h = (h + 1) / 2, w = (w + 1) / 2;
+  *height2 = h, *width2 = w;
+  return DIMB_OK;
+}
+
+int dimb_pyr_dev(dimb_ctx* ctx, const float* d_src, int B, int height, int width, int channels, int level, float* d_dst, void* stream) {
+  int h2, w2;
+  if (!ctx || !d_src || !d_dst || B < 1 || B > 65535 || (channels != 1 && channels != 3) || dimb_pyr_size(height, width, level, &h2, &w2) != DIMB_OK)
+    return DIMB_ERR_ARG;
+  // every launch has one CTA row per output row; the widest row is the source's (down) or the output's (up)
+  const long long rows = level < 0 ? 2ll * height : (height + 1) / 2, row_len = (level < 0 ? 2ll * width : width) * channels;
+  if (rows > 65535 || row_len >= (1ll << 30)) return DIMB_ERR_ARG;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (level == 0) {
+    DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_dst, d_src, static_cast<size_t>(B) * height * width * channels * sizeof(float),
+                                      cudaMemcpyDeviceToDevice, st));
+    return DIMB_OK;
+  }
+  float* mid[2] = {nullptr, nullptr};
+  for (int l = 1; l < level; ++l) {  // intermediates of a chain: level l's output in mid[(l - 1) % 2]
+    int hl, wl;
+    dimb_pyr_size(height, width, l, &hl, &wl);
+    DIMB_TRY(dimb_scratch(ctx, (l - 1) % 2 ? kSlotPyrB : kSlotPyrA, static_cast<size_t>(B) * hl * wl * channels * sizeof(float),
+                          reinterpret_cast<void**>(&mid[(l - 1) % 2])));
+  }
+  ProfScope prof(ctx, st, "tile.pyr");
+  if (level < 0) {
+    pyr_up_kernel<<<dim3(ceil_div(2 * width * channels, 128), 2 * height, B), 128, 0, st>>>(d_src, d_dst, height, width, channels);
+    DIMB_LAUNCH_CHECK(ctx);
+    return DIMB_OK;
+  }
+  const float* in = d_src;
+  int h = height, w = width;
+  for (int l = 1; l <= level; ++l) {
+    const int hn = (h + 1) / 2, wn = (w + 1) / 2;
+    float* out = l == level ? d_dst : mid[(l - 1) % 2];
+    pyr_down_kernel<<<dim3(ceil_div(wn * channels, 128), hn, B), 128, 0, st>>>(in, out, h, w, channels, hn, wn);
+    DIMB_LAUNCH_CHECK(ctx);
+    in = out, h = hn, w = wn;
+  }
+  return DIMB_OK;
+}
+
+int dimb_fstore_rescale_dev(dimb_fstore* fs, int B, const int* slots, int level, int height, int width, void* stream) {
+  if (!fs || !slots || B < 1 || B > 65535 || level < -1 || level > 3 || height < 1 || width < 1) return DIMB_ERR_ARG;
+  for (int b = 0; b < B; ++b)
+    if (slots[b] < 0 || slots[b] >= fs->n_slots) return DIMB_ERR_ARG;
+  dimb_ctx* ctx = fs->ctx;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int* d_slots;
+  DIMB_TRY(dimb_scratch(ctx, kSlotRescale, static_cast<size_t>(B) * sizeof(int), reinterpret_cast<void**>(&d_slots)));
+  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_slots, slots, B * sizeof(int), cudaMemcpyHostToDevice, st));
+  ProfScope prof(ctx, st, "tile.pyr");
+  fs_rescale_kernel<<<dim3(ceil_div(fs->cap, 256), B), 256, 0, st>>>(fs_layout(fs), d_slots, std::ldexp(1.f, level), height, width);
   DIMB_LAUNCH_CHECK(ctx);
   return DIMB_OK;
 }

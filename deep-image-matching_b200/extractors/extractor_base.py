@@ -1,9 +1,10 @@
 """Mirror of the reference's extractor plugin surface (src/deep_image_matching/extractors/extractor_base.py).
 
 Only what the hot path touches is restated: the constructor contract (:119-160), ``extract`` (:162-251: load,
-gray conversion quirk, ``_extract``, tile_idx, image_size, features.h5) and the abstract ``_extract`` /
-``_frame2tensor`` (:253-277).  Resizing by Quality and tiling (Tiler) are out of scope (SURVEY 2.1) and drop in
-unchanged when the class below is replaced by the reference's own base class (INTEGRATION.md).
+gray conversion quirk, ``_resize_image`` by quality, ``_extract``, tile_idx, ``_resize_features``, image_size of the original
+image, features.h5) and the abstract ``_extract`` / ``_frame2tensor`` (:253-277).  ``_extract_by_tile`` is restated for the tests
+of the device tiling; ``extract`` itself does not tile.  The class drops in unchanged when it is replaced by the reference's own
+base class (INTEGRATION.md).
 """
 from __future__ import annotations
 
@@ -37,7 +38,7 @@ def extractor_loader(root, model):
 
 
 class ExtractorBase(metaclass=ABCMeta):
-    _default_general_conf = {"force_cpu": False, "do_viz": False}
+    _default_general_conf = {"force_cpu": False, "do_viz": False, "quality": "high"}
     _default_conf = {}
     required_inputs = []
     grayscale = True
@@ -73,11 +74,39 @@ class ExtractorBase(metaclass=ABCMeta):
             image = cv2.cvtColor(image, cv2.COLOR_BGR2GRAY)  # sic: applied to an RGB array (SURVEY A.1)
         if self.as_float:
             image = image.astype(np.float32)
-        features = self._extract(image)
+        quality = self.config["general"]["quality"]
+        features = self._extract(self._resize_image(quality, image))
         features["tile_idx"] = np.zeros(features["keypoints"].shape[0], dtype=np.float32)
-        features["image_size"] = np.array(image.shape[:2])
+        features = self._resize_features(quality, features)
+        features["image_size"] = np.array(image.shape[:2])  # the original image's size, whatever the quality
         save_features_h5(feature_path, features, im_path.name, as_half=self.features_as_half)
         return feature_path
+
+    @staticmethod
+    def _resize_image(quality, image: np.ndarray) -> np.ndarray:
+        """extractor_base.py _resize_image: "highest" cv2.pyrUp, "high" unchanged, "medium" / "low" / "lowest" one, two or three
+        cv2.pyrDown (``sharded.quality_conf`` gives the level)."""
+        import cv2
+
+        from ..sharded import quality_conf
+        level = quality_conf(quality)
+        if level < 0:
+            return cv2.pyrUp(image)
+        for _ in range(level):
+            image = cv2.pyrDown(image)
+        return image
+
+    @staticmethod
+    def _resize_features(quality, features: dict) -> dict:
+        """extractor_base.py _resize_features: the keypoints (float32, in place) back to the original image, / 2 for "highest" and
+        * 2, * 4, * 8 for "medium", "low", "lowest"."""
+        from ..sharded import quality_conf
+        level = quality_conf(quality)
+        if level < 0:
+            features["keypoints"] /= 2
+        elif level > 0:
+            features["keypoints"] *= 2 ** level
+        return features
 
     def _extract_by_tile(self, image: np.ndarray, select_unique: bool = True) -> dict:
         """extractor_base.py:279-390: one ``_extract`` per tile of ``general.tile_size`` / ``tile_overlap``, keypoints moved to

@@ -18,7 +18,9 @@ exchange each rank splits the merged slots into per-tile views, matches the sele
 tables into one table per image pair (MatcherBase._match_by_tile).
 With ``pair_generation`` ("matching_lowres") the pair list itself comes from the device: low-resolution SuperPoint in phase 1, the
 exchange of those features, LightGlue over every brute-force pair dealt to the ranks, and an all_gather of the match counts that
-leaves the same kept pairs on every rank (``lowres_pairs``, ``run_lowres``)."""
+leaves the same kept pairs on every rank (``lowres_pairs``, ``run_lowres``).
+With ``quality`` other than "high" each image is resized on the device by cv2.pyrUp / cv2.pyrDown steps before extraction (plain or
+tiled) and the stored keypoints are scaled back to the original image (ExtractorBase._resize_image / _resize_features)."""
 from __future__ import annotations
 
 import numpy as np
@@ -273,6 +275,19 @@ def pair_generation_conf(pair_generation) -> dict | None:
     return out
 
 
+QUALITIES = {"highest": -1, "high": 0, "medium": 1, "low": 2, "lowest": 3}
+
+
+def quality_conf(quality="high") -> int:
+    """The pyramid level of the reference's extraction ``quality`` (ExtractorBase._resize_image / _resize_features): "highest" -1 (one
+    cv2.pyrUp, keypoints / 2), "high" 0 (unchanged, the default), "medium" 1, "low" 2 and "lowest" 3 (that many cv2.pyrDown, keypoints
+    * 2^level).  Case-insensitive; anything else raises ValueError."""
+    level = QUALITIES.get(quality.lower()) if isinstance(quality, str) else None
+    if level is None:
+        raise ValueError(f"quality must be one of {list(QUALITIES)}, got {quality!r}")
+    return level
+
+
 def tile_pairs_for(selection: str, n_tiles: int) -> list:
     """The tile pairs of one image pair under a configured selection (tiling.tile_selection for equally tiled images): "grid" pairs
     tile t with tile t, "exhaustive" every (t0, t1), sorted."""
@@ -426,12 +441,21 @@ class ImageSetMatcher:
     ``lowres_pairs`` runs LightGlue (``pairs_generator.LG_LOWRES_CONF``, own-extent normalisation) over every brute-force pair, dealt to
     the ranks, and keeps the pairs with more than ``min_matches`` matches; ``run_lowres`` then matches the kept pairs.
     ``lowres_weights``: the weights of that LightGlue (default ``lg_weights``; required with SuperGlue and kornia_matcher).  SuperPoint
-    only: ALIKED with pair generation is refused, and so is do_geometric_verification (an unknown key)."""
+    only: ALIKED with pair generation is refused, and so is do_geometric_verification (an unknown key).
+
+    ``quality``: the reference's extraction quality, checked by ``quality_conf`` ("high", the default, changes nothing).  ``height`` /
+    ``width`` stay the original image size and ``extract`` still takes full-size images: per extraction batch dimb_pyr_dev resizes them
+    (bitwise cv2.pyrUp for "highest", one to three cv2.pyrDown for "medium" / "low" / "lowest") into a buffer of the resized size, the
+    extractor (sized for the resized image, or tiles cut from it with the tile grid, border test and de-duplication in resized
+    pixels) runs on it, and one dimb_fstore_rescale_dev multiplies the stored float16 keypoints by 2^level and records the original
+    [H, W], as _resize_features and the h5 writer leave them.  Matching, verification and export then see original-pixel features.
+    Pair generation reads the original images.  Tile preselection with a quality other than "high" is refused, and so is a quality
+    that leaves an untiled image smaller than the extractor accepts (16 px per side for SuperPoint, 32 for ALIKED)."""
 
     def __init__(self, ctx, sp_weights: dict, lg_weights: dict, n_images: int, height: int, width: int, sp_conf: dict, lg_conf: dict,
                  batch_images: int = 16, batch_pairs: int = 32, dist=None, matcher: str = "lightglue", verification: dict | None = None,
                  tiling: dict | None = None, extractor: str = "superpoint", preselection_weights: dict | None = None,
-                 pair_generation: dict | None = None, lowres_weights: dict | None = None):
+                 pair_generation: dict | None = None, lowres_weights: dict | None = None, quality: str = "high"):
         import torch
 
         from . import _native
@@ -455,6 +479,16 @@ class ImageSetMatcher:
                 raise ValueError(f"tile preselection with matcher=\"{matcher}\" needs preselection_weights (SuperPoint-LightGlue weights)")
             if min(_lowres_size(height, width, self.tiling["tile_preselection_size"])[1:]) < 1:
                 raise ValueError(f"tile_preselection_size {self.tiling['tile_preselection_size']} down-samples a {height}x{width} image to nothing")
+        self.level = quality_conf(quality)
+        if self.level and self.presel:
+            raise ValueError(f"tile preselection runs at the original resolution here; quality {quality!r} with tile_selection "
+                             "\"preselection\" is not supported (use quality=\"high\", or grid / exhaustive tile selection)")
+        # the size the extractor sees (self.H x self.W stay the original image's)
+        self.h2, self.w2 = (height, width) if self.level == 0 else _native.pyr_size(height, width, self.level)
+        least = 16 if extractor == "superpoint" else 32
+        if self.level and tiling is None and min(self.h2, self.w2) < least:
+            raise ValueError(f"quality {quality!r} resizes a {height}x{width} image to {self.h2}x{self.w2}, below the {least} px per side "
+                             f"the {extractor} extractor needs")
         self.pairgen = pair_generation_conf(pair_generation)
         if self.pairgen is not None:
             if extractor == "aliked":
@@ -483,10 +517,10 @@ class ImageSetMatcher:
             raise ValueError(f"the image-set matcher needs a positive keypoint limit per extraction, got {self.cap}")
         self.D = 256 if extractor == "superpoint" else 128
         self.B, self.P = batch_images, batch_pairs
-        eh, ew = (height, width)
+        eh, ew = (self.h2, self.w2)
         if self.tiling is not None:
             eh, ew = self.tiling["tile_hw"]
-            self.grid = _native.tile_grid(height, width, eh, ew, *self.tiling["overlap_hw"])
+            self.grid = _native.tile_grid(self.h2, self.w2, eh, ew, *self.tiling["overlap_hw"])
             self.T = len(self.grid["origins"])
         if extractor == "superpoint":
             self.sp = _native.SuperPointNet(ctx, sp_weights, max_batch=batch_images, max_height=eh, max_width=ew, **sp_conf)
@@ -502,12 +536,14 @@ class ImageSetMatcher:
         self.store = _native.FeatureStoreDev(ctx, self.world * self.ipr, store_cap, self.D)
         dev = torch.device("cuda", ctx.device)
         # extraction outputs of one batch (float32, library layouts) and match outputs of one pair batch; tiled: the tiles of G images
-        n_ext = batch_images
+        n_ext = n_img = batch_images
+        self.C = 1 if extractor == "superpoint" else 3
         if self.tiling is not None:
-            self.G = max(1, batch_images // self.T)
+            self.G = n_img = max(1, batch_images // self.T)
             n_ext = self.G * self.T
-            self.C = 1 if extractor == "superpoint" else 3
             self.tiles = torch.zeros(n_ext, eh, ew, self.C, device=dev)
+        if self.level:  # the resized images of one extraction batch (tiled: of one group)
+            self.resized = torch.zeros((n_img, self.h2, self.w2) + ((3,) if self.C == 3 else ()), device=dev)
         self.kp = torch.zeros(n_ext, self.cap, 2, device=dev)
         self.sc = torch.zeros(n_ext, self.cap, device=dev)
         self.de = torch.zeros(n_ext, self.D, self.cap, device=dev)
@@ -566,10 +602,24 @@ class ImageSetMatcher:
             return self._extract_tiled(d_images, image_ids, st)
         for b0 in range(0, len(image_ids), self.B):
             ids = image_ids[b0:b0 + self.B]
-            self._extract_rows(d_images[b0:b0 + len(ids)], self.H, self.W, st)
+            src = self._resize(d_images[b0:b0 + len(ids)], st)
+            self._extract_rows(src, self.h2, self.w2, st)
             for k, i in enumerate(ids):
                 self.store.put_dev(self.slots[i], self.kp[k].data_ptr(), self.sc[k].data_ptr(), self.de[k].data_ptr(), self.cap,
-                                   self.cnt[k:k + 1].data_ptr(), self.H, self.W, None, st)
+                                   self.cnt[k:k + 1].data_ptr(), self.h2, self.w2, None, st)
+            self._rescale([self.slots[i] for i in ids], st)
+
+    def _resize(self, images, st):
+        """The images to extract from: `images` itself at quality "high", otherwise their pyramid steps in self.resized."""
+        if not self.level:
+            return images
+        self.ctx.pyr_dev(images.data_ptr(), len(images), self.H, self.W, self.C, self.level, self.resized.data_ptr(), st)
+        return self.resized[:len(images)]
+
+    def _rescale(self, slots, st):
+        """_resize_features on the slots just filled from resized images (nothing at quality "high")."""
+        if self.level:
+            self.store.rescale_dev(slots, self.level, self.H, self.W, st)
 
     def _extract_rows(self, src, h, w, st):
         """The configured extractor on the len(src) h x w images or tiles of `src` into rows [0, len(src)) of kp / sc / de / cnt:
@@ -587,11 +637,13 @@ class ImageSetMatcher:
         (th, tw), (oh, ow) = self.tiling["tile_hw"], self.tiling["overlap_hw"]
         for g0 in range(0, len(image_ids), self.G):
             ids = image_ids[g0:g0 + self.G]
-            self.ctx.tile_cut_dev(d_images[g0:g0 + len(ids)].data_ptr(), len(ids), self.H, self.W, self.C, th, tw, oh, ow,
-                                  self.tiles.data_ptr(), st)
+            src = self._resize(d_images[g0:g0 + len(ids)], st)
+            self.ctx.tile_cut_dev(src.data_ptr(), len(ids), self.h2, self.w2, self.C, th, tw, oh, ow, self.tiles.data_ptr(), st)
             self._extract_rows(self.tiles[:len(ids) * self.T], th, tw, st)
-            self.store.tile_merge_dev([self.slots[i] for i in ids], self.H, self.W, th, tw, oh, ow, self.kp.data_ptr(), self.sc.data_ptr(),
-                                      self.de.data_ptr(), self.cnt.data_ptr(), self.cap, st)
+            slots = [self.slots[i] for i in ids]
+            self.store.tile_merge_dev(slots, self.h2, self.w2, th, tw, oh, ow, self.kp.data_ptr(), self.sc.data_ptr(), self.de.data_ptr(),
+                                      self.cnt.data_ptr(), self.cap, st)
+            self._rescale(slots, st)
 
     def exchange(self):
         """The collective of the path: every rank's float16 feature blocks to every rank (NCCL all_gather over NVLink).  With tiling,

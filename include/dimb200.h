@@ -332,6 +332,28 @@ int dimb_resize_area_linear_tab(int ssize, int dsize, int* s_idx, float* alpha, 
  * dimb_resize_area_dev), otherwise the argument limits of dimb_resize_area_dev; profile group tile.resize.  CUDA cores. */
 int dimb_resize_area_linear_dev(dimb_ctx* ctx, const float* d_src, int B, int height, int width, float* d_dst, int height2, int width2,
                                 void* stream);
+/* Extraction quality (ExtractorBase._resize_image / _resize_features, extractor_base.py:205,224): the reference resizes every image
+ * by its `quality` before extracting and scales the keypoints back to the original image.  level: -1 = one cv2.pyrUp ("highest"),
+ * 0 = none ("high"), 1..3 = that many cv2.pyrDown ("medium", "low", "lowest").  Host only (no CUDA call): the size after `level`
+ * steps, pyrDown giving ((H + 1) / 2, (W + 1) / 2) and pyrUp (2H, 2W).  DIMB_ERR_ARG for a level outside [-1, 3], a size outside
+ * [1, 2^20] or a NULL pointer. */
+int dimb_pyr_size(int height, int width, int level, int* height2, int* width2);
+/* B float32 images d_src [B][H][W][channels] (channels 1 gray or 3 interleaved RGB) -> d_dst [B][H2][W2][channels] (dimb_pyr_size),
+ * bitwise cv2.pyrDown applied `level` times or cv2.pyrUp once (BORDER_DEFAULT = reflect-101), level 0 a copy.  pyrDown: horizontal
+ * 1 4 6 4 1 sums per source row, then the vertical sum over rows 2y - 2 .. 2y + 2 and * (1 / 256); pyrUp: 1 6 1 / 4 4 sums on the
+ * doubled grid and * (1 / 64); the order of every sum is OpenCV's, including the columns its 4-lane baseline SIMD loops cover, and
+ * every product and sum is rounded on its own (no FMA).  The intermediates of a chain live in the context's grow-only scratch, so
+ * the caller allocates only d_dst (which must not overlap d_src).  DIMB_ERR_ARG, before any CUDA call, for a NULL pointer, B
+ * outside [1, 65535], other channel counts, a bad size or level, or more than 65535 output rows in one step.  Profile group tile.pyr.
+ * CUDA cores. */
+int dimb_pyr_dev(dimb_ctx* ctx, const float* d_src, int B, int height, int width, int channels, int level, float* d_dst, void* stream);
+/* _resize_features on B store slots slots[b] (host array) filled from features of the resized image (dimb_fstore_put_dev, or
+ * dimb_tile_merge_dev on the resized grid): their float16 keypoints are multiplied by 2^level and the header's [H, W] becomes the
+ * original height x width (float16-rounded as dimb_fstore_put_dev stores it).  Scaling by a power of two commutes with rounding to
+ * float16 while the values stay normal (>= 2^-14), so this equals the reference's float32 scale followed by the h5 cast.  Empty slots
+ * are left alone.  DIMB_ERR_ARG, before any CUDA call, for a NULL pointer, B outside [1, 65535], a slot out of range, a level outside
+ * [-1, 3] or a size below 1.  Asynchronous on `stream`; profile group tile.pyr. */
+int dimb_fstore_rescale_dev(dimb_fstore* fs, int B, const int* slots, int level, int height, int width, void* stream);
 /* normalize_keypoints' own-extent size for LightGlue without image_size (lightglue.py:26-27): per image b, over its
  * min(d_counts[b], kpt_ld) keypoints of d_kpts [B][kpt_ld][2] float32, d_size_out[b] = {(1 + max x) - min x, (1 + max y) - min y}
  * in float32, as dimb_lg_match computes it on the host; {1, 1} for an image without keypoints.  Feed it to dimb_lg_match_dev
