@@ -205,16 +205,29 @@ def load_selftest_library():
         lib.dimb_last_error.argtypes = [vp]
         lib.dimb_last_error.restype = C.c_char_p
         lib.dimb_ctx_set_precision.argtypes = [vp, ip]
-        lib.dimb_selftest_gemm.argtypes = [vp, vp, vp, vp, ip, ip, ip, ip]
         fp = C.c_float
+        lib.dimb_selftest_gemm.argtypes = [vp, vp, vp, vp, vp, ip, ip, ip, ip, ip, fp, vp]
+        lib.dimb_selftest_gemm_plan.argtypes = [ip] * 8 + [vp]
+        lib.dimb_selftest_conv3x3.argtypes = [vp, vp, vp, vp, vp] + [ip] * 6 + [fp, fp, vp]
         lib.dimb_selftest_attention.argtypes = [vp, ip, vp, vp, vp, vp, ip, ip, ip, ip, vp, vp, ip, fp, fp, fp]
         lib.dimb_gv_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_uint, vp, vp]
         _selftest = lib
     return _selftest
 
 
+def gemm_plan(conv: int, bn: int, split: bool, const_b: bool, num_kb: int, m_tiles: int, n_tiles: int, num_sms: int):
+    """Launch plan (resb, sa, sb, smem_bytes, grid) of the persistent tensor-core kernel for one call shape, as launch_gemm computes
+    it (dimb_selftest_gemm_plan).  Host only: needs neither a context nor a GPU."""
+    out = np.zeros(5, np.int32)
+    rc = load_selftest_library().dimb_selftest_gemm_plan(conv, bn, int(bool(split)), int(bool(const_b)), num_kb, m_tiles, n_tiles,
+                                                         num_sms, _ptr(out))
+    if rc != OK:
+        raise DimbError(f"gemm_plan({conv}, {bn}, ...) failed (code {rc})")
+    return tuple(int(p) for p in out)
+
+
 class SelfTest:
-    """Context of the self-test library (tests/test_gpu_parity.py::test_tensor_core_gemm)."""
+    """Context of the self-test library (tests/test_gemm_conv_kernel.py, tests/test_attention_kernel.py)."""
 
     def __init__(self, device: int = 0):
         self.lib = load_selftest_library()
@@ -230,14 +243,38 @@ class SelfTest:
     def set_precision(self, precision: str):
         self.check(self.lib.dimb_ctx_set_precision(self.h, {"exact": 0, "fast": 1}[precision]), "set_precision")
 
-    def gemm(self, A: np.ndarray, B: np.ndarray, bn: int = 128) -> np.ndarray:
+    def gemm(self, A: np.ndarray, B: np.ndarray, bn: int = 128, bias=None, k32: bool = False, guard: float = 0.0):
+        """C = A B^T (+ bias) through the production GEMM launch (dimb_selftest_gemm), precision of the context.  A [M][K], B [N][K],
+        K a multiple of 64; k32: 32-wide K blocks (bn 256).  Rows of the operand allocations past M / N, and the output buffer, hold
+        `guard`.  Returns (C [M][N], tail [128][N] of the output buffer past the last row, plan
+        {resb, sa, sb, smem_bytes, grid} of the launch; -1s on the SIMT twin)."""
         A = np.ascontiguousarray(A, np.float32)
         B = np.ascontiguousarray(B, np.float32)
+        bias = None if bias is None else np.ascontiguousarray(bias, np.float32)
         M, K = A.shape
         N = B.shape[0]
-        Cm = np.zeros((M, N), np.float32)
-        self.check(self.lib.dimb_selftest_gemm(self.h, _ptr(A), _ptr(B), _ptr(Cm), M, N, K, bn), "selftest_gemm")
-        return Cm
+        Cm = np.zeros((M + 128, N), np.float32)
+        plan = np.zeros(5, np.int32)
+        self.check(self.lib.dimb_selftest_gemm(self.h, _ptr(A), _ptr(B), None if bias is None else _ptr(bias), _ptr(Cm), M, N, K, bn,
+                                               int(bool(k32)), float(guard), _ptr(plan)), "selftest_gemm")
+        return Cm[:M], Cm[M:], tuple(int(p) for p in plan)
+
+    def conv3x3(self, x: np.ndarray, w: np.ndarray, bias: np.ndarray, pool: bool, guard: float = 0.0, sentinel: float = 0.0):
+        """One SuperPoint 3x3 conv layer (zero padding, bias, ReLU, optional 2x2 max pool) through its production launch
+        (dimb_selftest_conv3x3), precision of the context.  x NHWC [B][H][W][cin], w OIHW [cout][cin][3][3].  The input allocation
+        holds one more image of `guard`; the output buffer starts as `sentinel`.  Returns (out [B][Ho][Wo][cout], tail: one more
+        output image of the buffer, plan as gemm())."""
+        x = np.ascontiguousarray(x, np.float32)
+        w = np.ascontiguousarray(w, np.float32)
+        bias = np.ascontiguousarray(bias, np.float32)
+        B, H, W, cin = x.shape
+        cout = w.shape[0]
+        Ho, Wo = (H // 2, W // 2) if pool else (H, W)
+        out = np.zeros((B + 1, Ho, Wo, cout), np.float32)
+        plan = np.zeros(5, np.int32)
+        self.check(self.lib.dimb_selftest_conv3x3(self.h, _ptr(x), _ptr(w), _ptr(bias), _ptr(out), B, H, W, cin, cout, int(bool(pool)),
+                                                  float(guard), float(sentinel), _ptr(plan)), "selftest_conv3x3")
+        return out[:B], out[B], tuple(int(p) for p in plan)
 
     def attention(self, variant: int, Q: np.ndarray, K, V: np.ndarray, n, heads: int = 4, stopped=None, cross: bool = False,
                   lazy: float = -1.0, pad: float = 0.0, out_pad: float = 0.0) -> np.ndarray:

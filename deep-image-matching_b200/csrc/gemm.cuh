@@ -448,24 +448,35 @@ PersCfg pers_config(int nkb, bool resb) {
   return c;
 }
 
-template <int BN, bool SPLIT, int CONV, class Epi>
-int launch_pers_auto(dimb_ctx* ctx, cudaStream_t st, const TcOperands& ops, const GemmArgs& g, const Epi& epi, int m_tiles, int n_pad) {
+// Launch plan of one persistent-kernel call: resident weights or not, ring depths, shared memory and grid.  Host only, so that
+// the plan of every call site can be checked without a GPU (dimb_selftest_gemm_plan).
+struct PersPlan {
+  bool resb;
+  PersCfg cfg;
+  int grid;
+};
+
+template <int BN, bool SPLIT, int CONV>
+PersPlan pers_plan(bool const_b, int num_kb, int m_tiles, int n_tiles, int num_sms) {
   using G = PersGeom<BN, SPLIT, CONV>;
-  const int n_tiles = n_pad / BN;
   // resident weights only where a CTA keeps seeing the same B panel (its tiles share the n-tile: the persistent
   // stride = grid size must be a multiple of n_tiles) and >= 2 A stages still fit
-  const int total = m_tiles * n_tiles, grid = total < ctx->num_sms ? total : ctx->num_sms;
-  const bool fits = Epi::kConstB && (G::kBudget - g.num_kb * G::kBTile) >= 2 * G::kAStage;
+  const int total = m_tiles * n_tiles, grid = total < num_sms ? total : num_sms;
+  const bool fits = const_b && (G::kBudget - num_kb * G::kBTile) >= 2 * G::kAStage;
   // a grid that is a multiple of n_tiles pins every CTA to one B panel; when the SM count is not such a multiple (the brute-force
   // matcher: 32 panels of 256 descriptors), giving up a few SMs is far cheaper than re-streaming B from L2 for every tile
   int rgrid = grid;
   if (fits && grid % n_tiles != 0 && n_tiles <= grid) rgrid = grid / n_tiles * n_tiles;
   const bool resb = fits && (rgrid % n_tiles == 0) && rgrid * 8 >= grid * 7;
-  if (resb)
-    return launch_pers<BN, SPLIT, CONV, true, Epi>(ctx, st, ops, g, epi, m_tiles, n_tiles, pers_config<BN, SPLIT, CONV>(g.num_kb, true),
-                                                   rgrid);
-  return launch_pers<BN, SPLIT, CONV, false, Epi>(ctx, st, ops, g, epi, m_tiles, n_tiles, pers_config<BN, SPLIT, CONV>(g.num_kb, false),
-                                                  grid);
+  return PersPlan{resb, pers_config<BN, SPLIT, CONV>(num_kb, resb), resb ? rgrid : grid};
+}
+
+template <int BN, bool SPLIT, int CONV, class Epi>
+int launch_pers_auto(dimb_ctx* ctx, cudaStream_t st, const TcOperands& ops, const GemmArgs& g, const Epi& epi, int m_tiles, int n_pad) {
+  const int n_tiles = n_pad / BN;
+  const PersPlan p = pers_plan<BN, SPLIT, CONV>(Epi::kConstB, g.num_kb, m_tiles, n_tiles, ctx->num_sms);
+  if (p.resb) return launch_pers<BN, SPLIT, CONV, true, Epi>(ctx, st, ops, g, epi, m_tiles, n_tiles, p.cfg, p.grid);
+  return launch_pers<BN, SPLIT, CONV, false, Epi>(ctx, st, ops, g, epi, m_tiles, n_tiles, p.cfg, p.grid);
 }
 
 // n_pad: output columns rounded up to a multiple of BN (B operand rows beyond N read as zero via TMA OOB fill).

@@ -1,10 +1,17 @@
-// selftest.cu - dimb_selftest_gemm: C = A * B^T through the production tensor-core GEMM (or its SIMT twin), and
-// dimb_selftest_attention: the flash-attention kernels through their production launches; used by tests/ to validate the
-// wgmma/TMA plumbing in isolation from the model code.
+// selftest.cu - test infrastructure of libdimb200_selftest.so, used by tests/ to validate kernels in isolation from the model code:
+//   dimb_selftest_gemm / dimb_selftest_conv3x3: the persistent tensor-core GEMM (gemm.cuh) through its production launch, as a plain
+//     C = A B^T and as the SuperPoint 3x3 conv layer (conv3x3.cuh), or their SIMT twin (DIMB_TC=0);
+//   dimb_selftest_gemm_plan: the launch plan of the persistent kernel, host only;
+//   dimb_selftest_attention: the flash-attention kernels through their production launches;
+//   dimb_gv_host: the RANSAC arithmetic of gv.cu on the host.
 #include <algorithm>
 #include <vector>
 
+#include "conv3x3.cuh"
 #include "gemm.cuh"
+
+extern "C" int dimb_selftest_gemm_plan(int conv, int bn, int split, int const_b, int num_kb, int m_tiles, int n_tiles, int num_sms,
+                                       int* out);
 
 namespace {
 __global__ void split_rows_kernel(const float* __restrict__ src, __half* __restrict__ hi, __half* __restrict__ lo, size_t n) {
@@ -15,84 +22,7 @@ __global__ void split_rows_kernel(const float* __restrict__ src, __half* __restr
   hi[i] = h;
   lo[i] = l;
 }
-}  // namespace
 
-// A [M][K], B [N][K], C [M][N] host fp32; K multiple of 64. bn: 64, 128 or 256 (CTA tile width).
-extern "C" int dimb_selftest_gemm(dimb_ctx* ctx, const float* A, const float* B, float* C, int M, int N, int K, int bn) {
-  if (!ctx || !A || !B || !C || K % 64 || M < 1 || N < 1) return DIMB_ERR_ARG;
-  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-  const int Mp = round_up(M, 128), Np = round_up(N, 256);
-  float *dA, *dB, *dC;
-  __half *ah, *al, *bh, *bl;
-  std::vector<void*> tmp;
-  auto alloc = [&](void** p, size_t b) -> int {
-    DIMB_CUDA_OK(ctx, cudaMalloc(p, b));
-    tmp.push_back(*p);
-    DIMB_CUDA_OK(ctx, cudaMemset(*p, 0, b));
-    return static_cast<int>(DIMB_OK);
-  };
-  int rc = DIMB_OK;
-  do {
-    if ((rc = alloc((void**)&dA, sizeof(float) * Mp * K))) break;
-    if ((rc = alloc((void**)&dB, sizeof(float) * Np * K))) break;
-    if ((rc = alloc((void**)&dC, sizeof(float) * Mp * N))) break;
-    if ((rc = alloc((void**)&ah, sizeof(__half) * Mp * K))) break;
-    if ((rc = alloc((void**)&al, sizeof(__half) * Mp * K))) break;
-    if ((rc = alloc((void**)&bh, sizeof(__half) * Np * K))) break;
-    if ((rc = alloc((void**)&bl, sizeof(__half) * Np * K))) break;
-    cudaMemcpy(dA, A, sizeof(float) * M * K, cudaMemcpyHostToDevice);
-    cudaMemcpy(dB, B, sizeof(float) * N * K, cudaMemcpyHostToDevice);
-    split_rows_kernel<<<ceil_div(Mp * K, 256), 256>>>(dA, ah, al, static_cast<size_t>(Mp) * K);
-    split_rows_kernel<<<ceil_div(Np * K, 256), 256>>>(dB, bh, bl, static_cast<size_t>(Np) * K);
-    TcOperands ops;
-    if ((rc = dimb_tmap_2d(ctx, &ops.Ah, ah, Mp, K, K, kTileM))) break;
-    if ((rc = dimb_tmap_2d(ctx, &ops.Al, al, Mp, K, K, kTileM))) break;
-    if ((rc = dimb_tmap_2d(ctx, &ops.Bh, bh, Np, K, K, bn))) break;
-    if ((rc = dimb_tmap_2d(ctx, &ops.Bl, bl, Np, K, K, bn))) break;
-    GemmArgs g{};
-    g.num_kb = K / 64;
-    g.M = M;
-    g.N = N;
-    g.Ah = ah;
-    g.Al = al;
-    g.Bh = bh;
-    g.Bl = bl;
-    g.lda = K;
-    g.ldb = K;
-    EpiStoreF32 e;
-    e.out = dC;
-    e.bias = nullptr;
-    e.ldc = N;
-    e.n_valid = N;
-    e.m_valid = M;
-    e.scale = 1.f;
-    const int mt = Mp / 128;
-    if (bn == 64)
-      rc = launch_gemm<64, false>(ctx, 0, ops, g, e, mt, round_up(N, 64));
-    else if (bn == 128)
-      rc = launch_gemm<128, false>(ctx, 0, ops, g, e, mt, round_up(N, 128));
-    else if (bn == 256)
-      rc = launch_gemm<256, false>(ctx, 0, ops, g, e, mt, round_up(N, 256));
-    else
-      rc = DIMB_ERR_ARG;
-    if (rc) break;
-    cudaError_t ce = cudaDeviceSynchronize();
-    if (ce != cudaSuccess) {
-      dimb_set_error(ctx, std::string("dimb_selftest_gemm: ") + cudaGetErrorString(ce));
-      rc = DIMB_ERR_CUDA;
-      break;
-    }
-    cudaMemcpy(C, dC, sizeof(float) * M * N, cudaMemcpyDeviceToHost);
-  } while (0);
-  for (void* p : tmp) cudaFree(p);
-  return rc;
-}
-
-// ------------------------------------------------------------------ attention self-test
-#include "attn_hd128.cuh"
-#include "lg_kernels.cuh"
-
-namespace {
 // temporary device buffers of one self-test call, freed on every return path
 struct DevTmp {
   dimb_ctx* ctx;
@@ -130,16 +60,165 @@ __global__ void join_rows_kernel(const __half* __restrict__ hi, const __half* __
   if (i < n) out[i] = __half2float(hi[i]) + (lo ? __half2float(lo[i]) : 0.f);
 }
 
-int sync_call(dimb_ctx* ctx) {
+int sync_call(dimb_ctx* ctx, const char* what) {
   cudaError_t ce = cudaGetLastError();
   if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
   if (ce != cudaSuccess) {
-    dimb_set_error(ctx, std::string("dimb_selftest_attention: ") + cudaGetErrorString(ce));
+    dimb_set_error(ctx, std::string(what) + ": " + cudaGetErrorString(ce));
     return DIMB_ERR_CUDA;
   }
   return DIMB_OK;
 }
 
+// out[5] = {resb, sa, sb, smem_bytes, grid} of pers_plan for one instantiation of the kernel
+template <int BN, int CONV>
+void plan_of(bool split, bool const_b, int num_kb, int m_tiles, int n_tiles, int num_sms, int* out) {
+  const PersPlan p = split ? pers_plan<BN, true, CONV>(const_b, num_kb, m_tiles, n_tiles, num_sms)
+                           : pers_plan<BN, false, CONV>(const_b, num_kb, m_tiles, n_tiles, num_sms);
+  out[0] = p.resb;
+  out[1] = p.cfg.sa;
+  out[2] = p.cfg.sb;
+  out[3] = p.cfg.smem_bytes;
+  out[4] = p.grid;
+}
+
+// the plan the persistent kernel of ctx runs with; -1s on the SIMT twin, which has none
+void launch_plan(dimb_ctx* ctx, int conv, int bn, bool const_b, int num_kb, int m_tiles, int n_tiles, int* out) {
+  if (!out) return;
+  if (!ctx->use_tc) {
+    std::fill(out, out + 5, -1);
+    return;
+  }
+  dimb_selftest_gemm_plan(conv, bn, ctx->precision == DIMB_PRECISION_EXACT, const_b, num_kb, m_tiles, n_tiles, ctx->num_sms, out);
+}
+}  // namespace
+
+// Launch plan of the persistent kernel (gemm.cuh pers_plan, as launch_gemm computes it) for one call shape, host only: no context, no
+// device.  conv: 0 plain GEMM (bn 64 / 128 / 256), 1 3x3 conv (bn 64 / 128), 3 32-wide K blocks (bn 256); split: EXACT operands
+// (hi / lo planes); const_b: Epi::kConstB of the epilogue; num_kb: B tiles per output tile.  out[5] = {resb, sa, sb, smem_bytes, grid}.
+extern "C" int dimb_selftest_gemm_plan(int conv, int bn, int split, int const_b, int num_kb, int m_tiles, int n_tiles, int num_sms,
+                                       int* out) {
+  if (!out || num_kb < 1 || m_tiles < 1 || n_tiles < 1 || num_sms < 1) return DIMB_ERR_ARG;
+  const bool s = split != 0, cb = const_b != 0;
+  if (conv == 0 && bn == 64) plan_of<64, 0>(s, cb, num_kb, m_tiles, n_tiles, num_sms, out);
+  else if (conv == 0 && bn == 128) plan_of<128, 0>(s, cb, num_kb, m_tiles, n_tiles, num_sms, out);
+  else if (conv == 0 && bn == 256) plan_of<256, 0>(s, cb, num_kb, m_tiles, n_tiles, num_sms, out);
+  else if (conv == 1 && bn == 64) plan_of<64, 1>(s, cb, num_kb, m_tiles, n_tiles, num_sms, out);
+  else if (conv == 1 && bn == 128) plan_of<128, 1>(s, cb, num_kb, m_tiles, n_tiles, num_sms, out);
+  else if (conv == 3 && bn == 256) plan_of<256, 3>(s, cb, num_kb, m_tiles, n_tiles, num_sms, out);
+  else return DIMB_ERR_ARG;
+  return DIMB_OK;
+}
+
+// C = A B^T (+ bias) through launch_gemm with the fp32 store epilogue (EpiStoreF32), precision of the context.
+//   A [M][K], B [N][K] host fp32, K a multiple of 64; bias [N] or null; ldc = N.  bn: 64, 128 or 256 (CTA tile width); k32: 32-wide K
+//   blocks on SWIZZLE_64B maps (gemm.cuh CONV 3, bn 256), as the LightGlue linears run with DIMB_K32=1.
+//   The tensor maps have exactly M and N rows, over allocations padded to whole tiles whose extra rows hold `guard`: rows past M / N
+//   reach the MMAs only as TMA out-of-bounds fill.  C [M + 128][N] starts as `guard` everywhere: the M output rows, then a tail that
+//   must stay untouched.  plan[5] (may be null): {resb, sa, sb, smem_bytes, grid} of the launch, -1s on the SIMT twin.
+extern "C" int dimb_selftest_gemm(dimb_ctx* ctx, const float* A, const float* B, const float* bias, float* C, int M, int N, int K, int bn,
+                                  int k32, float guard, int* plan) {
+  if (!ctx || !A || !B || !C || K < 64 || K % 64 || M < 1 || N < 1) return DIMB_ERR_ARG;
+  if ((bn != 64 && bn != 128 && bn != 256) || (k32 && bn != 256)) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const int Mp = round_up(M, kTileM), Np = round_up(N, 256), n_pad = round_up(N, bn), mt = Mp / kTileM;
+  std::vector<float> a(static_cast<size_t>(Mp) * K, guard), b(static_cast<size_t>(Np) * K, guard);
+  std::copy(A, A + static_cast<size_t>(M) * K, a.begin());
+  std::copy(B, B + static_cast<size_t>(N) * K, b.begin());
+  DevTmp t{ctx, {}};
+  __half *ah, *al, *bh, *bl;
+  float *d_bias = nullptr, *dC;
+  DIMB_TRY(t.split(a, &ah, &al));
+  DIMB_TRY(t.split(b, &bh, &bl));
+  if (bias) DIMB_TRY(t.upload(&d_bias, std::vector<float>(bias, bias + N)));
+  const size_t nc = static_cast<size_t>(M + kTileM) * N;
+  DIMB_TRY(t.upload(&dC, std::vector<float>(nc, guard)));
+  auto tmap = k32 ? dimb_tmap_2d_sw64 : dimb_tmap_2d;
+  TcOperands ops;
+  DIMB_TRY(tmap(ctx, &ops.Ah, ah, M, K, K, kTileM));
+  DIMB_TRY(tmap(ctx, &ops.Al, al, M, K, K, kTileM));
+  DIMB_TRY(tmap(ctx, &ops.Bh, bh, N, K, K, bn));
+  DIMB_TRY(tmap(ctx, &ops.Bl, bl, N, K, K, bn));
+  GemmArgs g{};
+  g.num_kb = K / (k32 ? 32 : 64);
+  g.k_total = K;
+  g.M = M;
+  g.N = N;
+  g.Ah = ah;
+  g.Al = al;
+  g.Bh = bh;
+  g.Bl = bl;
+  g.lda = K;
+  g.ldb = K;
+  EpiStoreF32 e;
+  e.out = dC;
+  e.bias = d_bias;
+  e.ldc = N;
+  e.n_valid = N;
+  e.m_valid = M;
+  e.scale = 1.f;
+  if (k32)
+    DIMB_TRY((launch_gemm<256, 3>(ctx, 0, ops, g, e, mt, n_pad)));
+  else if (bn == 64)
+    DIMB_TRY((launch_gemm<64, false>(ctx, 0, ops, g, e, mt, n_pad)));
+  else if (bn == 128)
+    DIMB_TRY((launch_gemm<128, false>(ctx, 0, ops, g, e, mt, n_pad)));
+  else
+    DIMB_TRY((launch_gemm<256, false>(ctx, 0, ops, g, e, mt, n_pad)));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_gemm"));
+  DIMB_CUDA_OK(ctx, cudaMemcpy(C, dC, sizeof(float) * nc, cudaMemcpyDeviceToHost));
+  launch_plan(ctx, k32 ? 3 : 0, bn, EpiStoreF32::kConstB, g.num_kb, mt, n_pad / bn, plan);
+  return DIMB_OK;
+}
+
+// One SuperPoint 3x3 conv layer (zero padding 1, bias, ReLU, optional 2x2 max pool) through make_conv_layer and run_conv3
+// (conv3x3.cuh), precision of the context.
+//   x: NHWC fp32 [B][H][W][cin]; w: OIHW fp32 [cout][cin][3][3]; bias [cout]; cin a multiple of 64, cout 64 or a multiple of 128.
+//   The input allocation holds one more image of `guard` after the B images, outside the tensor map (B x H x W pixels): a halo read
+//   past the last image, or across the image boundary, would bring it in.  `guard` must be finite: the ReLU turns NaN into 0.
+//   out: [B + 1][Ho][Wo][cout] with Ho, Wo = H / 2, W / 2 under pool: the B output images joined from their hi + lo planes (hi only in
+//   FAST), then one image of tail; every element starts as `sentinel` (fp16-exact), so unwritten and stray writes show.
+//   plan[5] (may be null): as dimb_selftest_gemm.
+extern "C" int dimb_selftest_conv3x3(dimb_ctx* ctx, const float* x, const float* w, const float* bias, float* out, int B, int H, int W,
+                                     int cin, int cout, int pool, float guard, float sentinel, int* plan) {
+  if (!ctx || !x || !w || !bias || !out || B < 1 || H < 1 || W < 1 || cin < 64 || cin % 64) return DIMB_ERR_ARG;
+  if ((cout != 64 && (cout < 128 || cout % 128)) || (pool && (H < 2 || W < 2))) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const bool exact = ctx->precision == DIMB_PRECISION_EXACT;
+  const int Ho = pool ? H / 2 : H, Wo = pool ? W / 2 : W;
+  const size_t img = static_cast<size_t>(H) * W * cin, nout = static_cast<size_t>(B + 1) * Ho * Wo * cout;
+  std::vector<float> xin(img * (B + 1), guard);
+  std::copy(x, x + img * B, xin.begin());
+  DevTmp t{ctx, {}};
+  __half *xh, *xl, *oh, *ol;
+  float* d_out;
+  DIMB_TRY(t.split(xin, &xh, &xl));
+  DIMB_TRY(t.split(std::vector<float>(nout, sentinel), &oh, &ol));
+  DIMB_TRY(t.get(&d_out, nout));
+  ConvLayer L;
+  {
+    OwnerScope own(ctx, &t.p);  // the layer's weights and bias are this call's temporaries
+    DIMB_TRY(make_conv_layer(ctx, L, w, bias, cout, cin, 3, conv_bn(cout)));
+  }
+  const int bn = conv_bn(cout);
+  if (bn == 64)
+    DIMB_TRY(pool ? (run_conv3<64, true>(ctx, 0, L, xh, xl, oh, ol, B, H, W, "selftest.conv3x3"))
+                  : (run_conv3<64, false>(ctx, 0, L, xh, xl, oh, ol, B, H, W, "selftest.conv3x3")));
+  else
+    DIMB_TRY(pool ? (run_conv3<128, true>(ctx, 0, L, xh, xl, oh, ol, B, H, W, "selftest.conv3x3"))
+                  : (run_conv3<128, false>(ctx, 0, L, xh, xl, oh, ol, B, H, W, "selftest.conv3x3")));
+  join_rows_kernel<<<ceil_div(static_cast<int>(nout), 256), 256>>>(oh, exact ? ol : nullptr, d_out, nout);
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_conv3x3"));
+  DIMB_CUDA_OK(ctx, cudaMemcpy(out, d_out, sizeof(float) * nout, cudaMemcpyDeviceToHost));
+  launch_plan(ctx, 1, bn, EpiConvRelu<false>::kConstB, 9 * (cin / 64), conv_m_tiles(B, H, W), L.cout_pad / bn, plan);
+  return DIMB_OK;
+}
+
+// ------------------------------------------------------------------ attention self-test
+#include "attn_hd128.cuh"
+#include "lg_kernels.cuh"
+
+namespace {
 // LightGlue / SuperGlue attention (lg_kernels.cuh) on operands packed as lightglue.cu packs them
 int selftest_attention_lg(dimb_ctx* ctx, const float* Q, const float* K, const float* V, float* out, int S, int NP, const int* n,
                           const int* stopped, int cross, float lazy, float pad, float out_pad) {
@@ -189,7 +268,7 @@ int selftest_attention_lg(dimb_ctx* ctx, const float* Q, const float* K, const f
   float* d_out;
   DIMB_TRY(t.get(&d_out, R * kD));
   join_rows_kernel<<<ceil_div(static_cast<int>(R * kD), 256), 256>>>(ch, exact ? cl : nullptr, d_out, R * kD);
-  DIMB_TRY(sync_call(ctx));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_attention"));
   DIMB_CUDA_OK(ctx, cudaMemcpy(out, d_out, sizeof(float) * R * kD, cudaMemcpyDeviceToHost));
   return DIMB_OK;
 }
@@ -236,7 +315,7 @@ int selftest_attention_hd128(dimb_ctx* ctx, const float* Q, const float* K, cons
   a.lazy = lazy;
   a.out = d_out, a.ldo = ld;
   DIMB_TRY(launch_attn_hd128(ctx, 0, mq, mk, mv, H, a, exact));
-  DIMB_TRY(sync_call(ctx));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_attention"));
   DIMB_CUDA_OK(ctx, cudaMemcpy(out, d_out, sizeof(float) * nel, cudaMemcpyDeviceToHost));
   return DIMB_OK;
 }

@@ -18,43 +18,11 @@
 #include <cmath>
 #include <cstring>
 
+#include "conv3x3.cuh"
 #include "detect.cuh"
 #include "gemm.cuh"
 
 namespace {
-
-// ------------------------------------------------------------------ epilogue: conv bias + ReLU (+2x2 max pool) -> NHWC hi/lo
-template <bool POOL>
-struct EpiConvRelu : EpiBase {
-  static constexpr int TW = kConvTW;  // pixels per tile row
-  __half *hi, *lo;
-  const float* bias;
-  int H, W;      // conv resolution
-  int Ho, Wo;    // output resolution (H/2, W/2 if POOL)
-  int C;         // output channels
-  __device__ void operator()(const TileCoord& tc, int r, int n, float (&v)[32], float*) const {
-    const int y = tc.y0 + r / TW, x = tc.x0 + r % TW;
-    add_bias32(v, bias, n);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-    int oy = y, ox = x;
-    bool write = (y < H) && (x < W);
-    if (POOL) {
-      // lane = (row % (32 / TW)) * TW + col: the 2x2 window lives in lanes l, l^1, l^TW (gemm.cuh tile shapes)
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        float t = fmaxf(v[j], __shfl_xor_sync(0xffffffffu, v[j], 1));
-        v[j] = fmaxf(t, __shfl_xor_sync(0xffffffffu, t, TW));
-      }
-      oy = y >> 1;
-      ox = x >> 1;
-      write = ((y & 1) == 0) && ((x & 1) == 0) && (oy < Ho) && (ox < Wo);
-    }
-    if (!write) return;
-    const size_t off = ((static_cast<size_t>(tc.b) * Ho + oy) * Wo + ox) * C + n;
-    store_split32(hi + off, lo ? lo + off : nullptr, v);
-  }
-};
 
 // ------------------------------------------------------------------ conv1a: Cin = 1, direct, CUDA cores
 // block = 16x16 pixels, one thread per pixel; two passes of 32 output channels (low register count -> 3 CTAs/SM).
@@ -207,14 +175,6 @@ __global__ void sp_describe_kernel(const int* __restrict__ sel_idx, const float*
   for (int j = 0; j < 8; ++j) o[static_cast<size_t>(lane * 8 + j) * cap] = acc[j] * inv;  // (D,N) layout
 }
 
-struct ConvLayer {
-  int cin, cout;
-  __half *wh = nullptr, *wl = nullptr;  // [cout_pad][9*cin] (3x3) or [cout_pad][cin] (1x1)
-  float* bias = nullptr;                // [cout_pad]
-  int cout_pad, k;
-  CUtensorMap tmBh, tmBl;
-};
-
 }  // namespace
 
 struct dimb_sp {
@@ -240,81 +200,6 @@ struct dimb_sp {
 namespace {
 
 enum { L1B = 0, L2A, L2B, L3A, L3B, L4A, L4B, LPA, LPB, LDA, LDB };
-
-int upload_split(dimb_ctx* ctx, const std::vector<float>& m, __half** hi, __half** lo) {
-  std::vector<__half> h(m.size()), l(m.size());
-  for (size_t i = 0; i < m.size(); ++i) {
-    h[i] = __float2half_rn(m[i]);
-    l[i] = __float2half_rn(m[i] - __half2float(h[i]));
-  }
-  DIMB_TRY(dimb_alloc_t(ctx, hi, m.size(), false));
-  DIMB_TRY(dimb_alloc_t(ctx, lo, m.size(), false));
-  DIMB_CUDA_OK(ctx, cudaMemcpy(*hi, h.data(), m.size() * sizeof(__half), cudaMemcpyHostToDevice));
-  DIMB_CUDA_OK(ctx, cudaMemcpy(*lo, l.data(), m.size() * sizeof(__half), cudaMemcpyHostToDevice));
-  return DIMB_OK;
-}
-
-// OIHW fp32 -> [cout_pad][tap*cin + c]
-int make_conv_layer(dimb_ctx* ctx, ConvLayer& L, const float* w, const float* b, int cout, int cin, int ks, int bn) {
-  L.cin = cin;
-  L.cout = cout;
-  L.cout_pad = round_up(cout, bn);
-  L.k = ks * ks * cin;
-  std::vector<float> m(static_cast<size_t>(L.cout_pad) * L.k, 0.f), bias(L.cout_pad, 0.f);
-  for (int o = 0; o < cout; ++o) {
-    bias[o] = b[o];
-    for (int c = 0; c < cin; ++c)
-      for (int t = 0; t < ks * ks; ++t) m[static_cast<size_t>(o) * L.k + t * cin + c] = w[(static_cast<size_t>(o) * cin + c) * ks * ks + t];
-  }
-  DIMB_TRY(upload_split(ctx, m, &L.wh, &L.wl));
-  DIMB_TRY(dimb_alloc_t(ctx, &L.bias, L.cout_pad, false));
-  DIMB_CUDA_OK(ctx, cudaMemcpy(L.bias, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice));
-  DIMB_TRY(dimb_tmap_2d(ctx, &L.tmBh, L.wh, L.cout_pad, L.k, L.k, bn));
-  DIMB_TRY(dimb_tmap_2d(ctx, &L.tmBl, L.wl, L.cout_pad, L.k, L.k, bn));
-  return DIMB_OK;
-}
-
-template <int BN, bool POOL>
-int run_conv3(dimb_sp* sp, cudaStream_t st, const ConvLayer& L, const __half* inh, const __half* inl, __half* outh, __half* outl,
-              int B, int H, int W, const char* tag) {
-  dimb_ctx* ctx = sp->ctx;
-  const bool exact = ctx->precision == DIMB_PRECISION_EXACT;
-  TcOperands ops;
-  GemmArgs g{};
-  g.cin_blocks = L.cin / 64;
-  g.H = H;
-  g.W = W;
-  g.N = L.cout;
-  g.Ah = inh;
-  g.Al = inl;
-  g.Bh = L.wh;
-  g.Bl = L.wl;
-  g.lda = L.cin;
-  g.ldb = L.k;
-  g.k_total = L.k;
-  auto fill = [&](auto& epi) {
-    epi.hi = outh;
-    epi.lo = exact ? outl : nullptr;
-    epi.bias = L.bias;
-    epi.H = H;
-    epi.W = W;
-    epi.Ho = POOL ? H / 2 : H;
-    epi.Wo = POOL ? W / 2 : W;
-    epi.C = L.cout;
-  };
-  // gemm.cuh CONV 1: one (8+2)-row halo box per dx serves the three dy taps
-  const int box_h = kConvTH + 2;
-  DIMB_TRY(dimb_tmap_nhwc(ctx, &ops.Ah, inh, B, H, W, L.cin, box_h, kConvTW));
-  DIMB_TRY(dimb_tmap_nhwc(ctx, &ops.Al, inl, B, H, W, L.cin, box_h, kConvTW));
-  ops.Bh = L.tmBh;
-  ops.Bl = L.tmBl;
-  g.num_kb = 9 * g.cin_blocks;
-  g.tiles_x = ceil_div(W, kConvTW);
-  g.tiles_y = ceil_div(H, kConvTH);
-  EpiConvRelu<POOL> epi;
-  fill(epi);
-  return launch_gemm<BN, 1>(ctx, st, ops, g, epi, B * g.tiles_x * g.tiles_y, L.cout_pad, tag);
-}
 
 // 1x1 conv = GEMM over cells, fp32 output [cells][ldc]
 int run_conv1_f32(dimb_sp* sp, cudaStream_t st, const ConvLayer& L, const __half* inh, const __half* inl, float* out, int cells,
@@ -381,7 +266,7 @@ int dimb_sp_create(dimb_ctx* ctx, const float* weights, size_t n_floats, const d
   p += 640;
   for (int i = 1; i < 12; ++i) {
     const int co = shp[i][0], ci = shp[i][1], ks = shp[i][2];
-    const int bn = co == 64 ? 64 : 128;
+    const int bn = conv_bn(co);
     const size_t nw = static_cast<size_t>(co) * ci * ks * ks;
     DIMB_TRY(make_conv_layer(ctx, sp->L[i - 1], p, p + nw, co, ci, ks, bn));
     p += nw + co;
@@ -453,15 +338,15 @@ int dimb_sp_extract_dev(dimb_sp* sp, const float* d_images, int B, int H, int W,
                                                                                            exact ? sp->a1l : nullptr, H, W);
     DIMB_LAUNCH_CHECK(ctx);
   }
-  DIMB_TRY((run_conv3<64, true>(sp, st, sp->L[L1B], sp->a1h, sp->a1l, sp->a1ph, sp->a1pl, B, H, W, "sp.conv1b")));
-  DIMB_TRY((run_conv3<64, false>(sp, st, sp->L[L2A], sp->a1ph, sp->a1pl, sp->a2h, sp->a2l, B, H2, W2, "sp.conv2a")));
-  DIMB_TRY((run_conv3<64, true>(sp, st, sp->L[L2B], sp->a2h, sp->a2l, sp->a2ph, sp->a2pl, B, H2, W2, "sp.conv2b")));
-  DIMB_TRY((run_conv3<128, false>(sp, st, sp->L[L3A], sp->a2ph, sp->a2pl, sp->a3h, sp->a3l, B, H4, W4, "sp.conv3a")));
-  DIMB_TRY((run_conv3<128, true>(sp, st, sp->L[L3B], sp->a3h, sp->a3l, sp->a3ph, sp->a3pl, B, H4, W4, "sp.conv3b")));
-  DIMB_TRY((run_conv3<128, false>(sp, st, sp->L[L4A], sp->a3ph, sp->a3pl, sp->a4h, sp->a4l, B, h, w, "sp.conv4a")));
-  DIMB_TRY((run_conv3<128, false>(sp, st, sp->L[L4B], sp->a4h, sp->a4l, sp->fth, sp->ftl, B, h, w, "sp.conv4b")));
-  DIMB_TRY((run_conv3<128, false>(sp, st, sp->L[LPA], sp->fth, sp->ftl, sp->pah, sp->pal, B, h, w, "sp.convPa")));
-  DIMB_TRY((run_conv3<128, false>(sp, st, sp->L[LDA], sp->fth, sp->ftl, sp->dah, sp->dal, B, h, w, "sp.convDa")));
+  DIMB_TRY((run_conv3<64, true>(sp->ctx, st, sp->L[L1B], sp->a1h, sp->a1l, sp->a1ph, sp->a1pl, B, H, W, "sp.conv1b")));
+  DIMB_TRY((run_conv3<64, false>(sp->ctx, st, sp->L[L2A], sp->a1ph, sp->a1pl, sp->a2h, sp->a2l, B, H2, W2, "sp.conv2a")));
+  DIMB_TRY((run_conv3<64, true>(sp->ctx, st, sp->L[L2B], sp->a2h, sp->a2l, sp->a2ph, sp->a2pl, B, H2, W2, "sp.conv2b")));
+  DIMB_TRY((run_conv3<128, false>(sp->ctx, st, sp->L[L3A], sp->a2ph, sp->a2pl, sp->a3h, sp->a3l, B, H4, W4, "sp.conv3a")));
+  DIMB_TRY((run_conv3<128, true>(sp->ctx, st, sp->L[L3B], sp->a3h, sp->a3l, sp->a3ph, sp->a3pl, B, H4, W4, "sp.conv3b")));
+  DIMB_TRY((run_conv3<128, false>(sp->ctx, st, sp->L[L4A], sp->a3ph, sp->a3pl, sp->a4h, sp->a4l, B, h, w, "sp.conv4a")));
+  DIMB_TRY((run_conv3<128, false>(sp->ctx, st, sp->L[L4B], sp->a4h, sp->a4l, sp->fth, sp->ftl, B, h, w, "sp.conv4b")));
+  DIMB_TRY((run_conv3<128, false>(sp->ctx, st, sp->L[LPA], sp->fth, sp->ftl, sp->pah, sp->pal, B, h, w, "sp.convPa")));
+  DIMB_TRY((run_conv3<128, false>(sp->ctx, st, sp->L[LDA], sp->fth, sp->ftl, sp->dah, sp->dal, B, h, w, "sp.convDa")));
   const int cells = B * h * w;
   DIMB_TRY(run_conv1_f32(sp, st, sp->L[LPB], sp->pah, sp->pal, sp->logits, cells, 65, "sp.convPb"));
   DIMB_TRY(run_conv1_f32(sp, st, sp->L[LDB], sp->dah, sp->dal, sp->ddesc, cells, 256, "sp.convDb"));

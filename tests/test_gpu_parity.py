@@ -44,20 +44,6 @@ def _check_lg(out, ref, th=0.1):
     return rep
 
 
-@pytest.mark.parametrize("m,n,k,bn", [(128, 128, 64, 128), (300, 200, 128, 64), (128, 256, 576, 256), (1000, 768, 512, 128)])
-def test_tensor_core_gemm(m, n, k, bn):
-    """The production GEMM template (gemm.cuh) behind the self-test library's C = A B^T entry."""
-    from dim_b200 import _native
-    st = _native.SelfTest(0)
-    rng = np.random.default_rng(m + n)
-    A, B = rng.standard_normal((m, k)).astype(np.float32), rng.standard_normal((n, k)).astype(np.float32)
-    ref = A.astype(np.float64) @ B.astype(np.float64).T
-    st.set_precision("exact")
-    assert np.abs(st.gemm(A, B, bn) - ref).max() / np.abs(ref).max() < 1e-5  # fp32 accumulation over K
-    st.set_precision("fast")
-    assert np.abs(st.gemm(A, B, bn) - ref).max() / np.abs(ref).max() < 3e-3
-
-
 @pytest.mark.parametrize("name", SP_CASES)
 def test_superpoint_golden(ctx, sp_golden, sp_weights, name):
     img, conf, ref = sp_case(sp_golden, name)
