@@ -63,7 +63,10 @@ def run_set(ctx, name, H, W, n, batch_pairs, reps):
         return [(int(a.stem), int(b.stem)) for a, b in pairs], counts
 
     def device():
-        low.extract(d_imgs, [eng.slots[i] for i in ids], eng.B, torch.cuda.current_stream().cuda_stream)
+        st = torch.cuda.current_stream().cuda_stream
+        for b0 in range(0, n, eng.B):  # the low-resolution pass of extract: one resize and its SuperPoint calls per batch
+            batch = ids[b0:b0 + eng.B]
+            low.extract(d_imgs[b0:b0 + len(batch)], batch, [eng.slots[i] for i in batch], st)
         return eng.lowres_pairs()
 
     arms = {"host": host, "device": device}

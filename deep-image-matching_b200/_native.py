@@ -32,6 +32,7 @@ EXPORTS = [
     "dimb_tile_grid", "dimb_tile_cut_dev", "dimb_tile_merge_dev", "dimb_tile_views_dev", "dimb_tile_match_merge_dev",
     "dimb_resize_area_tab", "dimb_resize_area_dev", "dimb_kpts_extent_dev", "dimb_tile_preselect_dev",
     "dimb_resize_area_linear_tab", "dimb_resize_area_linear_dev", "dimb_pyr_size", "dimb_pyr_dev", "dimb_fstore_rescale_dev",
+    "dimb_tile_preselect_pairs_dev",
 ]
 
 
@@ -180,6 +181,8 @@ def load_library():
     lib.dimb_kpts_extent_dev.argtypes = [vp, ip, vp, ip, vp, vp, vp]
     lib.dimb_tile_preselect_dev.argtypes = [vp, ip, C.POINTER(FeatsDev), C.POINTER(FeatsDev), vp, vp, ip] + [ip] * 6 + \
         [C.c_double, C.c_double, ip, vp, vp, vp]
+    lib.dimb_tile_preselect_pairs_dev.argtypes = [vp, ip, C.POINTER(FeatsDev), C.POINTER(FeatsDev), vp, vp, ip, vp] + [ip] * 4 + \
+        [vp, ip, vp, vp, vp]
     _lib = lib
     return lib
 
@@ -497,6 +500,22 @@ class Context:
         self.check(self.lib.dimb_tile_preselect_dev(self.h, Q, a0, a1, d_matches, d_n_matches, cap, H, W, tile_h, tile_w, overlap_h, overlap_w,
                                                     float(scale0), float(scale1), int(min_matches_per_tile), d_counts, d_flags, stream),
                    "dimb_tile_preselect_dev")
+
+    def tile_preselect_pairs_dev(self, f0: list, f1: list, d_matches, d_n_matches, cap, sizes, tile_h, tile_w, overlap_h, overlap_w, scales,
+                                 min_matches_per_tile, d_counts, d_flags, stream=0):
+        """PRESELECTION's box count for len(f0) image pairs of any sizes (dimb_tile_preselect_pairs_dev): sizes [(H0, W0, H1, W1)] and
+        scales [(scale0, scale1)] per pair.  Pair q's counts (int32) and flags (uint8) are the row-major [T0][T1] block starting at
+        element sum_{p<q} T0[p] * T1[p] of d_counts / d_flags.  Asynchronous on `stream`."""
+        Q = len(f0)
+        a0 = (FeatsDev * Q)(*f0)
+        a1 = (FeatsDev * Q)(*f1)
+        sz = np.ascontiguousarray(np.asarray(sizes, np.int64).reshape(-1, 4).astype(np.int32))
+        sc = np.ascontiguousarray(np.asarray(scales, np.float64).reshape(-1, 2))
+        if len(sz) != Q or len(sc) != Q:
+            raise ValueError(f"tile_preselect_pairs_dev needs one size row and one scale row per pair: {len(sz)} / {len(sc)} for {Q} pairs")
+        self.check(self.lib.dimb_tile_preselect_pairs_dev(self.h, Q, a0, a1, d_matches, d_n_matches, cap, _ptr(sz), tile_h, tile_w, overlap_h,
+                                                          overlap_w, _ptr(sc), int(min_matches_per_tile), d_counts, d_flags, stream),
+                   "dimb_tile_preselect_pairs_dev")
 
     def nn_match_dev(self, d_desc0: int, n0: int, d_desc1: int, n1: int, D: int, mode: str, th: float, d_idx: int, d_dist: int,
                      d_n: int, cap: int, f16: bool = False, ld0: int = 0, ld1: int = 0, stream: int = 0):

@@ -568,33 +568,41 @@ __device__ __forceinline__ void axis_cover(float v, int pad, int step, int size,
 
 __device__ __forceinline__ bool in_open(float v, int o, int size) { return v > static_cast<float>(o) && v < static_cast<float>(o + size); }
 
+struct PrePair {  // one image pair of a preselection batch: both sides' keypoints, tile grids and scales, and its count block
+  PreSide s0, s1;
+  Grid g0, g1;
+  float sc0, sc1;
+  size_t off;  // first element of the pair's [T0][T1] block of counts / flags
+};
+
 // grid (cap / 128, Q): one thread per match row; +1 for every (t0, t1) whose boxes both hold the row's full-resolution points.
-__global__ void tile_preselect_count_kernel(const PreSide* __restrict__ sides, const int64_t* __restrict__ matches, const int* __restrict__ n_matches,
-                                            int cap, Grid g, float sc0, float sc1, int* __restrict__ counts) {
+__global__ void tile_preselect_count_kernel(const PrePair* __restrict__ pairs, const int64_t* __restrict__ matches,
+                                            const int* __restrict__ n_matches, int cap, int* __restrict__ counts) {
   const int q = blockIdx.y, r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= min(n_matches[q], cap)) return;
   const int64_t* m = matches + (static_cast<size_t>(q) * cap + r) * 2;
-  const PreSide s0 = sides[2 * q], s1 = sides[2 * q + 1];
-  const float x0 = __fdiv_rn(pre_kpt(s0, 2 * m[0]), sc0), y0 = __fdiv_rn(pre_kpt(s0, 2 * m[0] + 1), sc0);
-  const float x1 = __fdiv_rn(pre_kpt(s1, 2 * m[1]), sc1), y1 = __fdiv_rn(pre_kpt(s1, 2 * m[1] + 1), sc1);
+  const PrePair& p = pairs[q];
+  const Grid g0 = p.g0, g1 = p.g1;
+  const float x0 = __fdiv_rn(pre_kpt(p.s0, 2 * m[0]), p.sc0), y0 = __fdiv_rn(pre_kpt(p.s0, 2 * m[0] + 1), p.sc0);
+  const float x1 = __fdiv_rn(pre_kpt(p.s1, 2 * m[1]), p.sc1), y1 = __fdiv_rn(pre_kpt(p.s1, 2 * m[1] + 1), p.sc1);
   constexpr float kFar = 4194304.f;  // 2^22: beyond every box (image and tile sides are below 2^20 / 2^14), and keeps the estimates in int
   if (!(fabsf(x0) < kFar && fabsf(y0) < kFar && fabsf(x1) < kFar && fabsf(y1) < kFar)) return;
-  const int T = g.tiles();
-  int* c = counts + static_cast<size_t>(q) * T * T;
+  const int T1 = g1.tiles();
+  int* c = counts + p.off;
   int r0lo, r0hi, c0lo, c0hi, r1lo, r1hi, c1lo, c1hi;
-  axis_cover(y0, g.pad_top, g.sy, g.th, g.rows, r0lo, r0hi);
-  axis_cover(x0, g.pad_left, g.sx, g.tw, g.cols, c0lo, c0hi);
-  axis_cover(y1, g.pad_top, g.sy, g.th, g.rows, r1lo, r1hi);
-  axis_cover(x1, g.pad_left, g.sx, g.tw, g.cols, c1lo, c1hi);
+  axis_cover(y0, g0.pad_top, g0.sy, g0.th, g0.rows, r0lo, r0hi);
+  axis_cover(x0, g0.pad_left, g0.sx, g0.tw, g0.cols, c0lo, c0hi);
+  axis_cover(y1, g1.pad_top, g1.sy, g1.th, g1.rows, r1lo, r1hi);
+  axis_cover(x1, g1.pad_left, g1.sx, g1.tw, g1.cols, c1lo, c1hi);
   for (int ra = r0lo; ra <= r0hi; ++ra) {
-    if (!in_open(y0, -g.pad_top + ra * g.sy, g.th)) continue;
+    if (!in_open(y0, -g0.pad_top + ra * g0.sy, g0.th)) continue;
     for (int ca = c0lo; ca <= c0hi; ++ca) {
-      if (!in_open(x0, -g.pad_left + ca * g.sx, g.tw)) continue;
-      const int t0 = ra * g.cols + ca;
+      if (!in_open(x0, -g0.pad_left + ca * g0.sx, g0.tw)) continue;
+      const int t0 = ra * g0.cols + ca;
       for (int rb = r1lo; rb <= r1hi; ++rb) {
-        if (!in_open(y1, -g.pad_top + rb * g.sy, g.th)) continue;
+        if (!in_open(y1, -g1.pad_top + rb * g1.sy, g1.th)) continue;
         for (int cb = c1lo; cb <= c1hi; ++cb)
-          if (in_open(x1, -g.pad_left + cb * g.sx, g.tw)) atomicAdd(c + static_cast<size_t>(t0) * T + rb * g.cols + cb, 1);
+          if (in_open(x1, -g1.pad_left + cb * g1.sx, g1.tw)) atomicAdd(c + static_cast<size_t>(t0) * T1 + rb * g1.cols + cb, 1);
       }
     }
   }
@@ -902,34 +910,53 @@ int dimb_kpts_extent_dev(dimb_ctx* ctx, int B, const float* d_kpts, int kpt_ld, 
   return DIMB_OK;
 }
 
-int dimb_tile_preselect_dev(dimb_ctx* ctx, int Q, const dimb_feats_dev* f0, const dimb_feats_dev* f1, const int64_t* d_matches,
-                            const int* d_n_matches, int cap, int height, int width, int tile_h, int tile_w, int overlap_h, int overlap_w,
-                            double scale0, double scale1, int min_matches_per_tile, int* d_counts, unsigned char* d_flags, void* stream) {
-  Grid g;
-  if (!ctx || !f0 || !f1 || !d_matches || !d_n_matches || !d_counts || !d_flags || Q < 1 || Q > 65535 || cap < 1 ||
-      !make_grid(height, width, tile_h, tile_w, overlap_h, overlap_w, &g) || min_matches_per_tile < 0)
+int dimb_tile_preselect_pairs_dev(dimb_ctx* ctx, int Q, const dimb_feats_dev* f0, const dimb_feats_dev* f1, const int64_t* d_matches,
+                                  const int* d_n_matches, int cap, const int* sizes, int tile_h, int tile_w, int overlap_h, int overlap_w,
+                                  const double* scales, int min_matches_per_tile, int* d_counts, unsigned char* d_flags, void* stream) {
+  if (!ctx || !f0 || !f1 || !d_matches || !d_n_matches || !sizes || !scales || !d_counts || !d_flags || Q < 1 || Q > 65535 || cap < 1 ||
+      min_matches_per_tile < 0)
     return DIMB_ERR_ARG;
-  const float sc0 = static_cast<float>(scale0), sc1 = static_cast<float>(scale1);  // numpy: float32 array / Python float in float32
-  if (!(std::isfinite(sc0) && sc0 > 0.f && std::isfinite(sc1) && sc1 > 0.f)) return DIMB_ERR_ARG;
-  std::vector<PreSide> hp(2 * Q);
+  std::vector<PrePair> hp(Q);
+  size_t n = 0;
   for (int q = 0; q < Q; ++q) {
-    if (!f0[q].keypoints || !f1[q].keypoints) return DIMB_ERR_ARG;
-    hp[2 * q] = PreSide{f0[q].keypoints, f0[q].f16, f0[q].round_fp16};
-    hp[2 * q + 1] = PreSide{f1[q].keypoints, f1[q].f16, f1[q].round_fp16};
+    PrePair& p = hp[q];
+    const int* s = sizes + 4 * q;
+    if (!f0[q].keypoints || !f1[q].keypoints || !make_grid(s[0], s[1], tile_h, tile_w, overlap_h, overlap_w, &p.g0) ||
+        !make_grid(s[2], s[3], tile_h, tile_w, overlap_h, overlap_w, &p.g1))
+      return DIMB_ERR_ARG;
+    p.sc0 = static_cast<float>(scales[2 * q]), p.sc1 = static_cast<float>(scales[2 * q + 1]);  // numpy: float32 array / Python float in float32
+    if (!(std::isfinite(p.sc0) && p.sc0 > 0.f && std::isfinite(p.sc1) && p.sc1 > 0.f)) return DIMB_ERR_ARG;
+    p.s0 = PreSide{f0[q].keypoints, f0[q].f16, f0[q].round_fp16};
+    p.s1 = PreSide{f1[q].keypoints, f1[q].f16, f1[q].round_fp16};
+    p.off = n;
+    n += static_cast<size_t>(p.g0.tiles()) * p.g1.tiles();
   }
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t n = static_cast<size_t>(Q) * g.tiles() * g.tiles();
-  PreSide* d_sides;
-  DIMB_TRY(dimb_scratch(ctx, kSlotPreSides, hp.size() * sizeof(PreSide), reinterpret_cast<void**>(&d_sides)));
-  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_sides, hp.data(), hp.size() * sizeof(PreSide), cudaMemcpyHostToDevice, st));
+  PrePair* d_pairs;
+  DIMB_TRY(dimb_scratch(ctx, kSlotPreSides, hp.size() * sizeof(PrePair), reinterpret_cast<void**>(&d_pairs)));
+  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_pairs, hp.data(), hp.size() * sizeof(PrePair), cudaMemcpyHostToDevice, st));
   ProfScope prof(ctx, st, "tile.preselect");
   DIMB_CUDA_OK(ctx, cudaMemsetAsync(d_counts, 0, n * sizeof(int), st));
-  tile_preselect_count_kernel<<<dim3(ceil_div(cap, 128), Q), 128, 0, st>>>(d_sides, d_matches, d_n_matches, cap, g, sc0, sc1, d_counts);
+  tile_preselect_count_kernel<<<dim3(ceil_div(cap, 128), Q), 128, 0, st>>>(d_pairs, d_matches, d_n_matches, cap, d_counts);
   DIMB_LAUNCH_CHECK(ctx);
   tile_preselect_flag_kernel<<<static_cast<int>(std::min<size_t>((n + 255) / 256, 4096)), 256, 0, st>>>(d_counts, n, min_matches_per_tile,
                                                                                                     d_flags);
   DIMB_LAUNCH_CHECK(ctx);
   return DIMB_OK;
+}
+
+int dimb_tile_preselect_dev(dimb_ctx* ctx, int Q, const dimb_feats_dev* f0, const dimb_feats_dev* f1, const int64_t* d_matches,
+                            const int* d_n_matches, int cap, int height, int width, int tile_h, int tile_w, int overlap_h, int overlap_w,
+                            double scale0, double scale1, int min_matches_per_tile, int* d_counts, unsigned char* d_flags, void* stream) {
+  if (Q < 1 || Q > 65535) return DIMB_ERR_ARG;
+  std::vector<int> sizes(4 * static_cast<size_t>(Q));
+  std::vector<double> scales(2 * static_cast<size_t>(Q));
+  for (int q = 0; q < Q; ++q) {
+    sizes[4 * q] = sizes[4 * q + 2] = height, sizes[4 * q + 1] = sizes[4 * q + 3] = width;
+    scales[2 * q] = scale0, scales[2 * q + 1] = scale1;
+  }
+  return dimb_tile_preselect_pairs_dev(ctx, Q, f0, f1, d_matches, d_n_matches, cap, sizes.data(), tile_h, tile_w, overlap_h, overlap_w,
+                                       scales.data(), min_matches_per_tile, d_counts, d_flags, stream);
 }
 
 }  // extern "C"

@@ -12,9 +12,9 @@ superpoint.py:25-31) with ``nms_radius 3, max_keypoints 2048, keypoint_threshold
 are normalised by their own extent (lightglue.py:26-27); ``use_superpoint`` is forced to True (:100); the KeyNet/AdaLAM
 branch is therefore dead code in the reference and absent here; the pair is kept if ``len(matches) > min_matches``.
 
-This host function serves image lists of mixed sizes and images on disk; for an equally sized image set already on the device,
-``ImageSetMatcher(pair_generation={"strategy": "matching_lowres", ...})`` gives the same pairs and counts without leaving the device
-and across GPUs (``sharded.ImageSetMatcher.lowres_pairs``).
+This host function serves images on disk; for an image set already on the device, of one size or of mixed sizes (per-image
+``height`` / ``width``), ``ImageSetMatcher(pair_generation={"strategy": "matching_lowres", ...})`` gives the same pairs and counts
+without leaving the device and across GPUs (``sharded.ImageSetMatcher.lowres_pairs``).
 """
 from __future__ import annotations
 

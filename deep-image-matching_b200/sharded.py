@@ -20,7 +20,9 @@ With ``pair_generation`` ("matching_lowres") the pair list itself comes from the
 exchange of those features, LightGlue over every brute-force pair dealt to the ranks, and an all_gather of the match counts that
 leaves the same kept pairs on every rank (``lowres_pairs``, ``run_lowres``).
 With ``quality`` other than "high" each image is resized on the device by cv2.pyrUp / cv2.pyrDown steps before extraction (plain or
-tiled) and the stored keypoints are scaled back to the original image (ExtractorBase._resize_image / _resize_features)."""
+tiled) and the stored keypoints are scaled back to the original image (ExtractorBase._resize_image / _resize_features).
+Images of a set may differ in size (per-image ``height`` / ``width``): each rank runs its images in groups of one size, and every slot,
+tile grid and low-resolution image keeps its own image's size."""
 from __future__ import annotations
 
 import numpy as np
@@ -288,14 +290,41 @@ def quality_conf(quality="high") -> int:
     return level
 
 
-def tile_pairs_for(selection: str, n_tiles: int) -> list:
-    """The tile pairs of one image pair under a configured selection (tiling.tile_selection for equally tiled images): "grid" pairs
-    tile t with tile t, "exhaustive" every (t0, t1), sorted."""
+def tile_pairs_for(selection: str, n_tiles: int, n_tiles1: int | None = None) -> list:
+    """The tile pairs of one image pair under a configured selection (tiling.tile_selection), image 0 cut into `n_tiles` tiles and
+    image 1 into `n_tiles1` (default: as many): "grid" pairs tile t with tile t for t < min(n_tiles, n_tiles1) (the reference zips
+    the two tile lists), "exhaustive" every (t0, t1), sorted."""
+    n_tiles1 = n_tiles if n_tiles1 is None else n_tiles1
     if selection == "grid":
-        return [(t, t) for t in range(n_tiles)]
+        return [(t, t) for t in range(min(n_tiles, n_tiles1))]
     if selection == "exhaustive":
-        return [(t0, t1) for t0 in range(n_tiles) for t1 in range(n_tiles)]
+        return [(t0, t1) for t0 in range(n_tiles) for t1 in range(n_tiles1)]
     raise ValueError(f"tile_selection must be one of {TILE_SELECTIONS}, got {selection!r}")
+
+
+def image_sizes(n_images: int, height, width) -> list:
+    """The (H, W) of every image of a set: `height` and `width` both ints (every image has that size) or both sequences of `n_images`
+    ints (image i is height[i] x width[i]).  Raises ValueError for any other form and for sizes below 1."""
+    seq = [isinstance(v, (list, tuple, range, np.ndarray)) for v in (height, width)]
+    if seq[0] != seq[1]:
+        raise ValueError(f"height and width must both be ints or both be sequences of n_images ints, got {height!r} and {width!r}")
+    if isinstance(n_images, bool) or not isinstance(n_images, (int, np.integer)) or n_images < 1:
+        raise ValueError(f"an image set needs n_images >= 1, got {n_images!r}")
+    hs, ws = (list(height), list(width)) if seq[0] else ([height] * n_images, [width] * n_images)
+    if len(hs) != n_images or len(ws) != n_images:
+        raise ValueError(f"height and width must hold one size per image: {len(hs)} and {len(ws)} for {n_images} images")
+    for v in hs + ws:
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 1:
+            raise ValueError(f"image sizes must be ints >= 1, got {v!r}")
+    return [(int(h), int(w)) for h, w in zip(hs, ws)]
+
+
+def _by_size(sizes, items) -> list:
+    """`items` grouped by sizes[item]: [((H, W), [items...])] in order of first appearance, item order kept inside a group."""
+    groups = {}
+    for k in items:
+        groups.setdefault(sizes[k], []).append(k)
+    return list(groups.items())
 
 
 def pack_tile_batches(n_tile_pairs, batch_pairs: int) -> list:
@@ -327,18 +356,26 @@ class _LowResSet:
     once with INTER_AREA to longest side `size` (dimb_resize_area_dev, or dimb_resize_area_linear_dev when that enlarges an axis) and
     runs SuperPoint (`sp_conf`) into float32 buffers per store slot (no float16 cast: these features never pass through features.h5
     in the reference), with their own extent for LightGlue without image_size; ``buffers`` are what the exchange all-gathers (about
-    (256 + 2) * 4 * K bytes per slot); ``match`` runs LightGlue (`lg_conf`) on a batch of slot pairs into m / ms / nm / sl."""
+    (256 + 2) * 4 * K bytes per slot); ``match`` runs LightGlue (`lg_conf`) on a batch of slot pairs into m / ms / nm / sl.
 
-    def __init__(self, ctx, sp_weights, lg_weights, n_slots, height, width, size, sp_conf, lg_conf, batch_images, batch_pairs, device):
+    `sizes` holds every image's (H, W): ``scales`` / ``low_sizes`` are each image's scale and (h, w), and for a set of one size
+    ``scale`` / ``h`` / ``w`` are those values (None otherwise).  SuperPoint is built for the largest low-resolution height and width,
+    and ``low`` is one flat buffer that each batch views as (k, h, w)."""
+
+    def __init__(self, ctx, sp_weights, lg_weights, n_slots, sizes, size, sp_conf, lg_conf, batch_images, batch_pairs, device):
         import torch
 
         from . import _native
-        self.ctx, self.H, self.W = ctx, height, width
-        self.scale, self.h, self.w = _lowres_size(height, width, size)
+        self.ctx = ctx
+        geom = {s: _lowres_size(*s, size) for s in dict.fromkeys(sizes)}
+        self.scales = [geom[s][0] for s in sizes]
+        self.low_sizes = [geom[s][1:] for s in sizes]
+        self.scale, self.h, self.w = geom[sizes[0]] if len(geom) == 1 else (None, None, None)
         K = self.K = sp_conf["max_keypoints"]
-        self.sp = _native.SuperPointNet(ctx, sp_weights, max_batch=batch_images, max_height=self.h, max_width=self.w, **sp_conf)
+        self.sp = _native.SuperPointNet(ctx, sp_weights, max_batch=batch_images, max_height=max(h for _, h, _ in geom.values()),
+                                        max_width=max(w for _, _, w in geom.values()), **sp_conf)
         self.lg = _native.LightGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=K, **lg_conf)
-        self.low = torch.zeros(batch_images, self.h, self.w, device=device)
+        self.low = torch.zeros(batch_images * max(h * w for _, h, w in geom.values()), device=device)
         self.sc = torch.zeros(batch_images, K, device=device)  # written by the extractor, not read
         self.kp = torch.zeros(n_slots, K, 2, device=device)
         self.de = torch.zeros(n_slots, 256, K, device=device)
@@ -353,24 +390,25 @@ class _LowResSet:
     def buffers(self):
         return self.kp, self.de, self.n, self.size
 
-    def extract(self, d_images, slots, batch, st):
-        """The H x W images `d_images` of store slots `slots`, `batch` per resize."""
-        enlarge = self.h > self.H or self.w > self.W
-        resize = self.ctx.resize_area_linear_dev if enlarge else self.ctx.resize_area_dev
-        K = self.K
-        for b0 in range(0, len(slots), batch):
-            ss = slots[b0:b0 + batch]
-            resize(d_images[b0:b0 + len(ss)].data_ptr(), len(ss), self.H, self.W, self.low.data_ptr(), self.h, self.w, st)
-            k = 0
-            while k < len(ss):  # the extractor writes consecutive rows: one call per run of consecutive slots
-                e = k + 1
-                while e < len(ss) and ss[e] == ss[k] + (e - k):
-                    e += 1
-                s = ss[k]
-                self.sp.extract_dev(self.low[k].data_ptr(), e - k, self.h, self.w, self.kp[s].data_ptr(), self.sc[k].data_ptr(),
-                                    self.de[s].data_ptr(), self.n[s:].data_ptr(), K, st)
-                self.ctx.kpts_extent_dev(e - k, self.kp[s].data_ptr(), K, self.n[s:].data_ptr(), self.size[s].data_ptr(), st)
-                k = e
+    def extract(self, images, image_ids, slots, st):
+        """One resize batch: the equally sized images `images` ((k, H, W), at most batch_images) of images `image_ids`, stored in
+        `slots`."""
+        H, W = images.shape[1:3]
+        h, w = self.low_sizes[image_ids[0]]
+        resize = self.ctx.resize_area_linear_dev if h > H or w > W else self.ctx.resize_area_dev
+        K, ss = self.K, slots
+        low = self.low[:len(ss) * h * w].view(len(ss), h, w)
+        resize(images.data_ptr(), len(ss), H, W, low.data_ptr(), h, w, st)
+        k = 0
+        while k < len(ss):  # the extractor writes consecutive rows: one call per run of consecutive slots
+            e = k + 1
+            while e < len(ss) and ss[e] == ss[k] + (e - k):
+                e += 1
+            s = ss[k]
+            self.sp.extract_dev(low[k].data_ptr(), e - k, h, w, self.kp[s].data_ptr(), self.sc[k].data_ptr(), self.de[s].data_ptr(),
+                                self.n[s:].data_ptr(), K, st)
+            self.ctx.kpts_extent_dev(e - k, self.kp[s].data_ptr(), K, self.n[s:].data_ptr(), self.size[s].data_ptr(), st)
+            k = e
 
     def feats(self, slot):
         """The float32 features of a slot as LightGlue input, normalised by their own extent."""
@@ -450,9 +488,21 @@ class ImageSetMatcher:
     pixels) runs on it, and one dimb_fstore_rescale_dev multiplies the stored float16 keypoints by 2^level and records the original
     [H, W], as _resize_features and the h5 writer leave them.  Matching, verification and export then see original-pixel features.
     Pair generation reads the original images.  Tile preselection with a quality other than "high" is refused, and so is a quality
-    that leaves an untiled image smaller than the extractor accepts (16 px per side for SuperPoint, 32 for ALIKED)."""
+    that leaves an untiled image smaller than the extractor accepts (16 px per side for SuperPoint, 32 for ALIKED).
 
-    def __init__(self, ctx, sp_weights: dict, lg_weights: dict, n_images: int, height: int, width: int, sp_conf: dict, lg_conf: dict,
+    Image sizes: ``height`` / ``width`` are ints (every image has that size) or sequences of ``n_images`` ints, image i being
+    height[i] x width[i] (checked by ``image_sizes``; every per-size rule above is checked for each image).  All ranks pass the same
+    sizes.  ``extract`` then takes a list of per-image tensors (or one stacked tensor when its images share a size), groups this rank's
+    images by size and runs each group as a set of that size: its own pyramid steps, batches, tile grid (T_i tiles, store capacity
+    max(T_i) * K, tile views at ``view_offsets[i]``), low-resolution size and scale, and its own [H, W] in every slot, so LightGlue,
+    SuperGlue, verification and the COLMAP cameras see each image's own size.  Grid selection pairs tile t with tile t for
+    t < min(T_i, T_j), as the reference's zip does.  The extractor is built for the largest extraction height and the largest width
+    of the set.  Per-image values: ``sizes``, ``ext_sizes`` (after quality), ``tile_counts`` and ``view_offsets``, and ``scales`` /
+    ``low_sizes`` of the low-resolution sets; for a set of one size ``H`` / ``W`` / ``h2`` / ``w2`` / ``T`` / ``G`` / ``pre_h`` /
+    ``pre_w`` hold that size's values, for a mixed set they are None.  A set given as lists of equal sizes is a set of one size: the
+    same launches and outputs as the int form."""
+
+    def __init__(self, ctx, sp_weights: dict, lg_weights: dict, n_images: int, height, width, sp_conf: dict, lg_conf: dict,
                  batch_images: int = 16, batch_pairs: int = 32, dist=None, matcher: str = "lightglue", verification: dict | None = None,
                  tiling: dict | None = None, extractor: str = "superpoint", preselection_weights: dict | None = None,
                  pair_generation: dict | None = None, lowres_weights: dict | None = None, quality: str = "high"):
@@ -467,28 +517,33 @@ class ImageSetMatcher:
             raise ValueError("SuperGlue matches SuperPoint features only; use matcher=\"lightglue\" with ALIKED")
         self.nn_conf = kornia_conf(lg_conf) if matcher == "kornia_matcher" else None
         self.tiling = tiling_conf(tiling)
+        self.sizes = image_sizes(n_images, height, width)
+        shapes = list(dict.fromkeys(self.sizes))  # the distinct sizes: every per-size rule is checked once per size
         self.presel = self.tiling is not None and self.tiling["tile_selection"] == "preselection"
         if self.presel:
             if extractor == "aliked":
                 raise ValueError("tile preselection runs on gray images and is available with extractor=\"superpoint\" only; "
                                  "pass tile_pairs with ALIKED")
-            if self.tiling["tile_preselection_size"] > max(height, width):
-                raise ValueError(f"tile_preselection_size {self.tiling['tile_preselection_size']} exceeds the image's longest side "
-                                 f"{max(height, width)}: preselection only downscales")
+            for H, W in shapes:
+                if self.tiling["tile_preselection_size"] > max(H, W):
+                    raise ValueError(f"tile_preselection_size {self.tiling['tile_preselection_size']} exceeds the image's longest side "
+                                     f"{max(H, W)}: preselection only downscales")
             if matcher != "lightglue" and preselection_weights is None:
                 raise ValueError(f"tile preselection with matcher=\"{matcher}\" needs preselection_weights (SuperPoint-LightGlue weights)")
-            if min(_lowres_size(height, width, self.tiling["tile_preselection_size"])[1:]) < 1:
-                raise ValueError(f"tile_preselection_size {self.tiling['tile_preselection_size']} down-samples a {height}x{width} image to nothing")
+            for H, W in shapes:
+                if min(_lowres_size(H, W, self.tiling["tile_preselection_size"])[1:]) < 1:
+                    raise ValueError(f"tile_preselection_size {self.tiling['tile_preselection_size']} down-samples a {H}x{W} image to nothing")
         self.level = quality_conf(quality)
         if self.level and self.presel:
             raise ValueError(f"tile preselection runs at the original resolution here; quality {quality!r} with tile_selection "
                              "\"preselection\" is not supported (use quality=\"high\", or grid / exhaustive tile selection)")
-        # the size the extractor sees (self.H x self.W stay the original image's)
-        self.h2, self.w2 = (height, width) if self.level == 0 else _native.pyr_size(height, width, self.level)
+        # the size the extractor sees (the sizes stay the original images')
+        ext = {s: s if self.level == 0 else _native.pyr_size(*s, self.level) for s in shapes}
         least = 16 if extractor == "superpoint" else 32
-        if self.level and tiling is None and min(self.h2, self.w2) < least:
-            raise ValueError(f"quality {quality!r} resizes a {height}x{width} image to {self.h2}x{self.w2}, below the {least} px per side "
-                             f"the {extractor} extractor needs")
+        for (H, W), (h2, w2) in ext.items():
+            if self.level and tiling is None and min(h2, w2) < least:
+                raise ValueError(f"quality {quality!r} resizes a {H}x{W} image to {h2}x{w2}, below the {least} px per side "
+                                 f"the {extractor} extractor needs")
         self.pairgen = pair_generation_conf(pair_generation)
         if self.pairgen is not None:
             if extractor == "aliked":
@@ -496,8 +551,22 @@ class ImageSetMatcher:
                                  "available with extractor=\"superpoint\" only; pass pairs with ALIKED")
             if matcher != "lightglue" and lowres_weights is None:
                 raise ValueError(f"pair generation with matcher=\"{matcher}\" needs lowres_weights (SuperPoint-LightGlue weights)")
-            if min(_lowres_size(height, width, self.pairgen["resize_max"])[1:]) < 1:
-                raise ValueError(f"resize_max {self.pairgen['resize_max']} down-samples a {height}x{width} image to nothing")
+            for H, W in shapes:
+                if min(_lowres_size(H, W, self.pairgen["resize_max"])[1:]) < 1:
+                    raise ValueError(f"resize_max {self.pairgen['resize_max']} down-samples a {H}x{W} image to nothing")
+        uniform = len(shapes) == 1
+        self.ext_sizes = [ext[s] for s in self.sizes]
+        # one size: the int attributes of that size; a mixed set has None there, and the per-image lists above and below
+        self.H, self.W = shapes[0] if uniform else (None, None)
+        self.h2, self.w2 = ext[shapes[0]] if uniform else (None, None)
+        self.grid = self.T = self.G = None
+        if self.tiling is not None:
+            grids = {s: _native.tile_grid(*ext[s], *self.tiling["tile_hw"], *self.tiling["overlap_hw"]) for s in shapes}
+            self.tile_counts = [len(grids[s]["origins"]) for s in self.sizes]
+            self.view_offsets = [int(v) for v in np.cumsum([0] + self.tile_counts[:-1])]
+            if uniform:
+                self.grid, self.T = grids[shapes[0]], self.tile_counts[0]
+                self.G = max(1, batch_images // self.T)
         if self.tiling is not None and extractor == "superpoint":
             if "fix_sampling" in sp_conf and not sp_conf["fix_sampling"]:
                 raise ValueError("tiled SuperPoint extraction runs with fix_sampling=True (the reference's rule); fix_sampling=False was given")
@@ -509,7 +578,7 @@ class ImageSetMatcher:
         self.torch, self.dist, self.ctx = torch, dist, ctx
         self.world = dist.get_world_size() if dist is not None and dist.is_initialized() else 1
         self.rank = dist.get_rank() if self.world > 1 else 0
-        self.n, self.H, self.W = n_images, height, width
+        self.n = n_images
         self.slots = [store_slot(i, n_images, self.world) for i in range(n_images)]
         self.extractor = extractor
         self.cap = int(sp_conf["max_keypoints"]) if extractor == "superpoint" else int(sp_conf.get("max_num_keypoints", 4000))
@@ -517,11 +586,11 @@ class ImageSetMatcher:
             raise ValueError(f"the image-set matcher needs a positive keypoint limit per extraction, got {self.cap}")
         self.D = 256 if extractor == "superpoint" else 128
         self.B, self.P = batch_images, batch_pairs
-        eh, ew = (self.h2, self.w2)
+        # the network takes the largest extraction height and width of the set (a set of portrait and landscape images over-sizes its
+        # workspace: 2048 x 2048 for 1536 x 2048 plus 2048 x 1536), or one tile
+        eh, ew = max(h for h, _ in ext.values()), max(w for _, w in ext.values())
         if self.tiling is not None:
             eh, ew = self.tiling["tile_hw"]
-            self.grid = _native.tile_grid(self.h2, self.w2, eh, ew, *self.tiling["overlap_hw"])
-            self.T = len(self.grid["origins"])
         if extractor == "superpoint":
             self.sp = _native.SuperPointNet(ctx, sp_weights, max_batch=batch_images, max_height=eh, max_width=ew, **sp_conf)
         else:
@@ -532,18 +601,19 @@ class ImageSetMatcher:
         elif matcher == "lightglue":
             self.lg = _native.LightGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=self.cap, **lg_conf)
         self.ipr = images_per_rank(n_images, self.world)
-        store_cap = self.cap if self.tiling is None else self.T * self.cap
-        self.store = _native.FeatureStoreDev(ctx, self.world * self.ipr, store_cap, self.D)
+        t_max = 1 if self.tiling is None else max(self.tile_counts)
+        self.store = _native.FeatureStoreDev(ctx, self.world * self.ipr, t_max * self.cap, self.D)
         dev = torch.device("cuda", ctx.device)
-        # extraction outputs of one batch (float32, library layouts) and match outputs of one pair batch; tiled: the tiles of G images
-        n_ext = n_img = batch_images
+        # extraction outputs of one batch (float32, library layouts) and match outputs of one pair batch; tiled: the tiles of the
+        # max(1, batch_images // T) images of one cut, T the tile count of their size
         self.C = 1 if extractor == "superpoint" else 3
+        n_img = {s: batch_images if self.tiling is None else max(1, batch_images // len(grids[s]["origins"])) for s in shapes}
+        n_ext = batch_images
         if self.tiling is not None:
-            self.G = n_img = max(1, batch_images // self.T)
-            n_ext = self.G * self.T
+            n_ext = max(n_img[s] * len(grids[s]["origins"]) for s in shapes)
             self.tiles = torch.zeros(n_ext, eh, ew, self.C, device=dev)
-        if self.level:  # the resized images of one extraction batch (tiled: of one group)
-            self.resized = torch.zeros((n_img, self.h2, self.w2) + ((3,) if self.C == 3 else ()), device=dev)
+        if self.level:  # the resized images of one extraction batch (tiled: of one cut), one flat buffer viewed per size
+            self.resized = torch.zeros(max(n_img[s] * ext[s][0] * ext[s][1] for s in shapes) * self.C, device=dev)
         self.kp = torch.zeros(n_ext, self.cap, 2, device=dev)
         self.sc = torch.zeros(n_ext, self.cap, device=dev)
         self.de = torch.zeros(n_ext, self.D, self.cap, device=dev)
@@ -554,11 +624,11 @@ class ImageSetMatcher:
         self.sl = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
         gv_cap = self.cap
         if self.tiling is not None:
-            # per-tile views of every image (slot i * T + t) with their row maps, and the merged tables of one batch: an image pair
-            # has at most min(batch_pairs, T * T) distinct tile pairs of at most K rows each, so cap2 holds every merged table whole
-            self.views = _native.FeatureStoreDev(ctx, n_images * self.T, self.cap, self.D)
-            self.vmap = torch.zeros(n_images * self.T, self.views.cap, dtype=torch.int32, device=dev)
-            self.cap2 = gv_cap = min(batch_pairs, self.T * self.T) * self.cap
+            # per-tile views of every image (slot view_offsets[i] + t) with their row maps, and the merged tables of one batch: an image
+            # pair has at most min(batch_pairs, T0 * T1) distinct tile pairs of at most K rows each, so cap2 holds every merged table whole
+            self.views = _native.FeatureStoreDev(ctx, sum(self.tile_counts), self.cap, self.D)
+            self.vmap = torch.zeros(sum(self.tile_counts), self.views.cap, dtype=torch.int32, device=dev)
+            self.cap2 = gv_cap = min(batch_pairs, t_max * t_max) * self.cap
             self.mm = torch.zeros(batch_pairs, self.cap2, 2, dtype=torch.int64, device=dev)
             self.nmm = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
         self.pre = self.lowres = None
@@ -567,15 +637,15 @@ class ImageSetMatcher:
             # of one pair batch
             from .tiling import LG_PRESELECTION_CONF, SP_PRESELECTION_CONF
             self.pre = _LowResSet(ctx, sp_weights, lg_weights if preselection_weights is None else preselection_weights, self.world * self.ipr,
-                                  height, width, self.tiling["tile_preselection_size"], SP_PRESELECTION_CONF, LG_PRESELECTION_CONF,
+                                  self.sizes, self.tiling["tile_preselection_size"], SP_PRESELECTION_CONF, LG_PRESELECTION_CONF,
                                   batch_images, batch_pairs, dev)
             self.pre_h, self.pre_w = self.pre.h, self.pre.w
-            self.pre_cnt = torch.zeros(batch_pairs, self.T * self.T, dtype=torch.int32, device=dev)
+            self.pre_cnt = torch.zeros(batch_pairs, t_max * t_max, dtype=torch.int32, device=dev)
         if self.pairgen is not None:
             # matching_lowres (pairs_generator.py:40-235) with the networks of pairs_generator.py:104-126
             from .pairs_generator import LG_LOWRES_CONF, SP_LOWRES_CONF
-            self.lowres = _LowResSet(ctx, sp_weights, lg_weights if lowres_weights is None else lowres_weights, self.world * self.ipr, height,
-                                     width, self.pairgen["resize_max"], SP_LOWRES_CONF, LG_LOWRES_CONF, batch_images, batch_pairs, dev)
+            self.lowres = _LowResSet(ctx, sp_weights, lg_weights if lowres_weights is None else lowres_weights, self.world * self.ipr,
+                                     self.sizes, self.pairgen["resize_max"], SP_LOWRES_CONF, LG_LOWRES_CONF, batch_images, batch_pairs, dev)
         self.gv = verification_conf(verification)
         if self.gv is not None and self.gv["method"] != "NONE":  # verification outputs of one pair batch
             self.v = torch.zeros(batch_pairs, gv_cap, 2, dtype=torch.int64, device=dev)
@@ -592,34 +662,74 @@ class ImageSetMatcher:
         self.exchanged_bytes = 0
 
     def extract(self, d_images, image_ids):
-        """Phase 1: d_images = float32 CUDA tensor holding this rank's images `image_ids`, 0..255: (k, H, W) gray for SuperPoint,
-        (k, H, W, 3) RGB for ALIKED.  With tiling the images are full size and are cut into tiles on the device."""
+        """Phase 1: this rank's images `image_ids` as float32 CUDA data, 0..255, gray for SuperPoint and RGB for ALIKED: one tensor
+        (k, H, W) / (k, H, W, 3) when they all have the same size, or a list of k tensors (H_i, W_i) / (H_i, W_i, 3) in `image_ids`
+        order.  Images are processed in groups of one size (image order kept inside a group), each group batched as a set of that
+        size; a shape that is not its image's declared size raises ValueError before any launch.  With tiling the images are full
+        size and are cut into tiles on the device.  A list is copied into one staging tensor per batch of batch_images, which feeds
+        the low-resolution sets and (untiled) the extractor; tiled extraction stages again per cut, whose size differs."""
         st = self.torch.cuda.current_stream().cuda_stream
-        for low in (self.pre, self.lowres):
-            if low is not None:
-                low.extract(d_images, [self.slots[i] for i in image_ids], self.B, st)
+        groups = self._groups(d_images, image_ids)
+        lows = [low for low in (self.pre, self.lowres) if low is not None]
         if self.tiling is not None:
-            return self._extract_tiled(d_images, image_ids, st)
-        for b0 in range(0, len(image_ids), self.B):
-            ids = image_ids[b0:b0 + self.B]
-            src = self._resize(d_images[b0:b0 + len(ids)], st)
-            self._extract_rows(src, self.h2, self.w2, st)
-            for k, i in enumerate(ids):
-                self.store.put_dev(self.slots[i], self.kp[k].data_ptr(), self.sc[k].data_ptr(), self.de[k].data_ptr(), self.cap,
-                                   self.cnt[k:k + 1].data_ptr(), self.h2, self.w2, None, st)
-            self._rescale([self.slots[i] for i in ids], st)
+            if lows:
+                for _, ids, src in self._batches(d_images, image_ids, groups, self.B):
+                    for low in lows:
+                        low.extract(src, ids, [self.slots[i] for i in ids], st)
+            return self._extract_tiled(d_images, image_ids, groups, st)
+        for (H, W), ids, src in self._batches(d_images, image_ids, groups, self.B):
+            slots = [self.slots[i] for i in ids]
+            for low in lows:
+                low.extract(src, ids, slots, st)
+            h2, w2 = self.ext_sizes[ids[0]]
+            src = self._resize(src, h2, w2, st)
+            self._extract_rows(src, h2, w2, st)
+            for k, s in enumerate(slots):
+                self.store.put_dev(s, self.kp[k].data_ptr(), self.sc[k].data_ptr(), self.de[k].data_ptr(), self.cap, self.cnt[k:k + 1].data_ptr(),
+                                   h2, w2, None, st)
+            self._rescale(slots, H, W, st)
 
-    def _resize(self, images, st):
-        """The images to extract from: `images` itself at quality "high", otherwise their pyramid steps in self.resized."""
+    def _batches(self, d_images, image_ids, groups, per):
+        """Per size group, its batches of at most `per` images in order: ((H, W), their image ids, the images staged as one tensor)."""
+        for size, ks in groups:
+            for b0 in range(0, len(ks), per):
+                yield size, [image_ids[k] for k in ks[b0:b0 + per]], self._stage(d_images, ks[b0:b0 + per])
+
+    def _groups(self, d_images, image_ids):
+        """This rank's images grouped by size: [((H, W), positions in image_ids)] (``_by_size``), after checking every image's shape
+        against its declared size."""
+        listed = isinstance(d_images, (list, tuple))
+        if (len(d_images) != len(image_ids)) if listed else (d_images.dim() < 3 or len(d_images) < len(image_ids)):
+            raise ValueError(f"extract needs one image per image id: {len(d_images)} images for {len(image_ids)} ids")
+        for k, i in enumerate(image_ids):
+            want = self.sizes[i] + ((3,) if self.C == 3 else ())
+            got = tuple(d_images[k].shape) if listed else tuple(d_images.shape[1:1 + len(want)])
+            if got != want or (listed and (d_images[k].dtype != self.torch.float32 or not d_images[k].is_cuda)):
+                raise ValueError(f"image {i} must be a float32 CUDA tensor of shape {want} (its declared size), got {tuple(d_images[k].shape)}")
+        return _by_size([self.sizes[i] for i in image_ids], range(len(image_ids)))
+
+    def _stage(self, d_images, ks):
+        """The images at positions `ks` of `d_images` as one contiguous (len(ks), H, W[, 3]) tensor: a view when they are consecutive
+        rows of one tensor, a copy otherwise."""
+        if isinstance(d_images, (list, tuple)):
+            return self.torch.stack([d_images[k] for k in ks])
+        if ks[-1] - ks[0] == len(ks) - 1:
+            return d_images[ks[0]:ks[0] + len(ks)]
+        return d_images[ks]
+
+    def _resize(self, images, h2, w2, st):
+        """The images to extract from: `images` itself at quality "high", otherwise their pyramid steps (h2 x w2) in self.resized."""
         if not self.level:
             return images
-        self.ctx.pyr_dev(images.data_ptr(), len(images), self.H, self.W, self.C, self.level, self.resized.data_ptr(), st)
-        return self.resized[:len(images)]
+        k, H, W = images.shape[:3]
+        out = self.resized[:k * h2 * w2 * self.C].view((k, h2, w2) + ((3,) if self.C == 3 else ()))
+        self.ctx.pyr_dev(images.data_ptr(), k, H, W, self.C, self.level, out.data_ptr(), st)
+        return out
 
-    def _rescale(self, slots, st):
-        """_resize_features on the slots just filled from resized images (nothing at quality "high")."""
+    def _rescale(self, slots, H, W, st):
+        """_resize_features on the slots just filled from resized H x W images (nothing at quality "high")."""
         if self.level:
-            self.store.rescale_dev(slots, self.level, self.H, self.W, st)
+            self.store.rescale_dev(slots, self.level, H, W, st)
 
     def _extract_rows(self, src, h, w, st):
         """The configured extractor on the len(src) h x w images or tiles of `src` into rows [0, len(src)) of kp / sc / de / cnt:
@@ -632,18 +742,23 @@ class ImageSetMatcher:
             else:
                 self.al.extract_dev(src[r].data_ptr(), h, w, 3, *ptrs)
 
-    def _extract_tiled(self, d_images, image_ids, st):
-        """Groups of G images: tile cut, the extractor over their G * T tiles, one tile merge into their slots."""
+    def _extract_tiled(self, d_images, image_ids, groups, st):
+        """Per size group (its own grid of T tiles), cuts of G = max(1, batch_images // T) images: tile cut, the extractor over their
+        G * T tiles, one tile merge into their slots."""
         (th, tw), (oh, ow) = self.tiling["tile_hw"], self.tiling["overlap_hw"]
-        for g0 in range(0, len(image_ids), self.G):
-            ids = image_ids[g0:g0 + self.G]
-            src = self._resize(d_images[g0:g0 + len(ids)], st)
-            self.ctx.tile_cut_dev(src.data_ptr(), len(ids), self.h2, self.w2, self.C, th, tw, oh, ow, self.tiles.data_ptr(), st)
-            self._extract_rows(self.tiles[:len(ids) * self.T], th, tw, st)
-            slots = [self.slots[i] for i in ids]
-            self.store.tile_merge_dev(slots, self.h2, self.w2, th, tw, oh, ow, self.kp.data_ptr(), self.sc.data_ptr(), self.de.data_ptr(),
-                                      self.cnt.data_ptr(), self.cap, st)
-            self._rescale(slots, st)
+        for (H, W), ks in groups:
+            first = image_ids[ks[0]]
+            (h2, w2), T = self.ext_sizes[first], self.tile_counts[first]
+            G = max(1, self.B // T)
+            for g0 in range(0, len(ks), G):
+                ids = [image_ids[k] for k in ks[g0:g0 + G]]
+                src = self._resize(self._stage(d_images, ks[g0:g0 + G]), h2, w2, st)
+                self.ctx.tile_cut_dev(src.data_ptr(), len(ids), h2, w2, self.C, th, tw, oh, ow, self.tiles.data_ptr(), st)
+                self._extract_rows(self.tiles[:len(ids) * T], th, tw, st)
+                slots = [self.slots[i] for i in ids]
+                self.store.tile_merge_dev(slots, h2, w2, th, tw, oh, ow, self.kp.data_ptr(), self.sc.data_ptr(), self.de.data_ptr(),
+                                          self.cnt.data_ptr(), self.cap, st)
+                self._rescale(slots, H, W, st)
 
     def exchange(self):
         """The collective of the path: every rank's float16 feature blocks to every rank (NCCL all_gather over NVLink).  With tiling,
@@ -655,11 +770,13 @@ class ImageSetMatcher:
                     self.exchanged_bytes += all_gather_blocks(t.view(self.torch.uint8).view(t.shape[0], -1), self.n, self.dist)
         if self.tiling is not None:
             st = self.torch.cuda.current_stream().cuda_stream
-            step = max(1, 65535 // self.T)
-            for b0 in range(0, self.n, step):
-                ids = range(b0, min(self.n, b0 + step))
-                self.store.tile_views_dev([self.slots[i] for i in ids], self.T, self.views, [i * self.T for i in ids],
-                                          self.vmap.data_ptr(), st)
+            for _, images in _by_size(self.sizes, range(self.n)):
+                T = self.tile_counts[images[0]]
+                step = max(1, 65535 // T)
+                for b0 in range(0, len(images), step):
+                    ids = images[b0:b0 + step]
+                    self.store.tile_views_dev([self.slots[i] for i in ids], T, self.views, [self.view_offsets[i] for i in ids],
+                                              self.vmap.data_ptr(), st)
 
     def _match_slots(self, store, s0, s1, st):
         """Enqueue the matcher on slot pairs (s0[k], s1[k]) of `store` (outputs in self.m / self.ms / self.nm)."""
@@ -675,47 +792,53 @@ class ImageSetMatcher:
 
     def _preselect(self, pairs):
         """PRESELECTION tile-pair lists of `pairs` (tiling.preselection_matches + tiling.tile_selection): per batch of batch_pairs,
-        LightGlue on the low-resolution slots and the tile box count, then ONE device->host copy of every pair's flags.  Row-major
-        flags give the lists sorted.  Memory: the flags take len(pairs) * T^2 bytes on the device and again on the host, and the
-        counts of one batch (allocated with the matcher) batch_pairs * T^2 int32; at T in the tens that is kilobytes per pair, but at
-        hundreds of tiles per image it reaches megabytes per pair, so a very large pair list is better matched in several calls."""
+        LightGlue on the low-resolution slots and the tile box count (dimb_tile_preselect_pairs_dev, each pair with both images' sizes
+        and scales), then ONE device->host copy of every pair's flags.  Pair (i, j) has a row-major T_i x T_j block of flags, which
+        gives its list sorted.  Memory: the flags take sum(T_i * T_j) bytes over the pairs on the device and again on the host, and the
+        counts of one batch (allocated with the matcher) batch_pairs * max(T)^2 int32; at T in the tens that is kilobytes per pair, but
+        at hundreds of tiles per image it reaches megabytes per pair, so a very large pair list is better matched in several calls."""
         st = self.torch.cuda.current_stream().cuda_stream
-        T, pre = self.T, self.pre
+        T, pre = self.tile_counts, self.pre
         (th, tw), (oh, ow) = self.tiling["tile_hw"], self.tiling["overlap_hw"]
-        flags = self.torch.zeros(max(len(pairs), 1), T * T, dtype=self.torch.uint8, device=self.pre_cnt.device)
+        offsets = np.cumsum([0] + [T[i] * T[j] for i, j in pairs])
+        flags = self.torch.zeros(max(int(offsets[-1]), 1), dtype=self.torch.uint8, device=self.pre_cnt.device)
         for b0 in range(0, len(pairs), self.P):
             chunk = pairs[b0:b0 + self.P]
             f0, f1 = pre.match([self.slots[i] for i, _ in chunk], [self.slots[j] for _, j in chunk], st)
-            self.ctx.tile_preselect_dev(f0, f1, pre.m.data_ptr(), pre.nm.data_ptr(), pre.K, self.H, self.W, th, tw, oh, ow, pre.scale, pre.scale,
-                                        self.tiling["min_matches_per_tile"], self.pre_cnt.data_ptr(), flags[b0].data_ptr(), st)
-        fl = flags[:len(pairs)].cpu().numpy().reshape(-1, T, T)
-        return [[(int(a), int(b)) for a, b in zip(*np.nonzero(f))] for f in fl]
+            self.ctx.tile_preselect_pairs_dev(f0, f1, pre.m.data_ptr(), pre.nm.data_ptr(), pre.K, [self.sizes[i] + self.sizes[j] for i, j in chunk],
+                                              th, tw, oh, ow, [(pre.scales[i], pre.scales[j]) for i, j in chunk],
+                                              self.tiling["min_matches_per_tile"], self.pre_cnt.data_ptr(), flags[int(offsets[b0]):].data_ptr(), st)
+        fl = flags.cpu().numpy()
+        return [[(int(a), int(b)) for a, b in zip(*np.nonzero(fl[offsets[q]:offsets[q + 1]].reshape(T[i], T[j])))]
+                for q, (i, j) in enumerate(pairs)]
 
     def _tile_pair_lists(self, pairs, tile_pairs):
+        T = self.tile_counts
         if tile_pairs is None:
             if self.presel:
                 return self._preselect(pairs)
-            return [tile_pairs_for(self.tiling["tile_selection"], self.T)] * len(pairs)
+            lists = {}  # one list per pair of tile counts
+            return [lists.setdefault((T[i], T[j]), tile_pairs_for(self.tiling["tile_selection"], T[i], T[j])) for i, j in pairs]
         if len(tile_pairs) != len(pairs):
             raise ValueError(f"tile_pairs must hold one list per image pair: {len(tile_pairs)} lists for {len(pairs)} pairs")
         lists = []
-        for lst in tile_pairs:
+        for (i, j), lst in zip(pairs, tile_pairs):
             lst = [(int(a), int(b)) for a, b in lst]
-            if any(not (0 <= a < self.T and 0 <= b < self.T) for a, b in lst):
-                raise ValueError(f"tile indices must lie in [0, {self.T})")
+            if any(not (0 <= a < T[i] and 0 <= b < T[j]) for a, b in lst):
+                raise ValueError(f"tile indices of image pair ({i}, {j}) must lie in [0, {T[i]}) x [0, {T[j]})")
             lists.append(lst)
         return lists
 
     def _enqueue_match(self, chunk, lists, st):
         """Enqueue the matcher on the image pairs `chunk` and return where it leaves their tables: (tables, counts, capacity).
-        Untiled: the store slots, (m, nm, cap).  Tiled: the tile pairs `lists` out of the views (i * T + t), then the tile-pair match
-        merge, (mm, nmm, cap2)."""
+        Untiled: the store slots, (m, nm, cap).  Tiled: the tile pairs `lists` out of the views (view_offsets[i] + t), then the
+        tile-pair match merge, (mm, nmm, cap2)."""
         if lists is None:
             self._match_slots(self.store, [self.slots[i] for i, _ in chunk], [self.slots[j] for _, j in chunk], st)
             return self.m, self.nm, self.cap
-        T = self.T
-        v0 = [i * T + a for (i, _), lst in zip(chunk, lists) for a, _ in lst]
-        v1 = [j * T + b for (_, j), lst in zip(chunk, lists) for _, b in lst]
+        off = self.view_offsets
+        v0 = [off[i] + a for (i, _), lst in zip(chunk, lists) for a, _ in lst]
+        v1 = [off[j] + b for (_, j), lst in zip(chunk, lists) for _, b in lst]
         if v0:
             self._match_slots(self.views, v0, v1, st)
         offsets = np.concatenate([[0], np.cumsum([len(lst) for lst in lists])])

@@ -359,13 +359,21 @@ int dimb_fstore_rescale_dev(dimb_fstore* fs, int B, const int* slots, int level,
  * in float32, as dimb_lg_match computes it on the host; {1, 1} for an image without keypoints.  Feed it to dimb_lg_match_dev
  * through dimb_feats_dev.size_f32_dev. */
 int dimb_kpts_extent_dev(dimb_ctx* ctx, int B, const float* d_kpts, int kpt_ld, const int* d_counts, float* d_size_out, void* stream);
-/* The box-count loop of tile_selection's PRESELECTION for Q image pairs of equally sized images (height x width, tiled as
- * dimb_tile_grid).  Pair q: the low-resolution match table d_matches[q] ([Q][cap][2] int64, rows = min(d_n_matches[q], cap), as
- * dimb_lg_match_dev writes it) indexes the keypoints of f0[q] / f1[q] (host arrays of Q; keypoints, f16 and round_fp16 are read).
- * Each matched keypoint maps back to full resolution as kpt / float(scale) (float32 division) and counts for tile pair (t0, t1) iff it
- * lies strictly inside both boxes: ox < x < ox + tile_w and oy < y < oy + tile_h.  Out (device): d_counts [Q][T*T] int32, the
- * count per tile pair t0 * T + t1; d_flags [Q][T*T] uint8 = count > min_matches_per_tile.  Integer counts: exact in any order.
- * DIMB_ERR_ARG for a bad geometry, scales that are not finite and positive, or min_matches_per_tile < 0. */
+/* The box-count loop of tile_selection's PRESELECTION for Q image pairs, each side on its own tile grid.  Pair q: the low-resolution
+ * match table d_matches[q] ([Q][cap][2] int64, rows = min(d_n_matches[q], cap), as dimb_lg_match_dev writes it) indexes the keypoints
+ * of f0[q] / f1[q] (host arrays of Q; keypoints, f16 and round_fp16 are read).  sizes: host [Q][4] int {H0, W0, H1, W1}, the
+ * full-resolution sizes of both images, each tiled as dimb_tile_grid with the shared tile and overlap (T0[q] and T1[q] tiles);
+ * scales: host [Q][2] double {scale0, scale1}, cast to float32.  Each matched keypoint maps back to full resolution as
+ * kpt / float(scale) (float32 division) and counts for tile pair (t0, t1) iff it lies strictly inside both boxes:
+ * ox < x < ox + tile_w and oy < y < oy + tile_h.  Out (device), pair q's block starting at element sum_{p<q} T0[p] * T1[p]:
+ * d_counts int32, the count of tile pair (t0, t1) at t0 * T1[q] + t1 (row-major), and d_flags uint8 in the same layout,
+ * count > min_matches_per_tile.  Integer counts: exact in any order.  DIMB_ERR_ARG, before any CUDA call, for a NULL pointer, Q outside
+ * [1, 65535], cap < 1, a bad size or grid on either side, scales that are not finite and positive, or min_matches_per_tile < 0. */
+int dimb_tile_preselect_pairs_dev(dimb_ctx* ctx, int Q, const dimb_feats_dev* f0, const dimb_feats_dev* f1, const int64_t* d_matches,
+                                  const int* d_n_matches, int cap, const int* sizes, int tile_h, int tile_w, int overlap_h, int overlap_w,
+                                  const double* scales, int min_matches_per_tile, int* d_counts, unsigned char* d_flags, void* stream);
+/* dimb_tile_preselect_pairs_dev for Q pairs of equally sized images (height x width) and one pair of scales: d_counts / d_flags
+ * [Q][T*T], the count of tile pair (t0, t1) at t0 * T + t1. */
 int dimb_tile_preselect_dev(dimb_ctx* ctx, int Q, const dimb_feats_dev* f0, const dimb_feats_dev* f1, const int64_t* d_matches,
                             const int* d_n_matches, int cap, int height, int width, int tile_h, int tile_w, int overlap_h, int overlap_w,
                             double scale0, double scale1, int min_matches_per_tile, int* d_counts, unsigned char* d_flags, void* stream);
