@@ -211,7 +211,9 @@ def load_selftest_library():
         fp = C.c_float
         lib.dimb_selftest_gemm.argtypes = [vp, vp, vp, vp, vp, ip, ip, ip, ip, ip, fp, vp]
         lib.dimb_selftest_gemm_plan.argtypes = [ip] * 8 + [vp]
-        lib.dimb_selftest_conv3x3.argtypes = [vp, vp, vp, vp, vp] + [ip] * 6 + [fp, fp, vp]
+        lib.dimb_selftest_conv3x3.argtypes = [vp, vp, vp, vp, vp] + [ip] * 7 + [fp, fp, vp]
+        lib.dimb_selftest_conv_mode.argtypes = [ip] * 5 + [vp]
+        lib.dimb_selftest_conv3x3_time.argtypes = [vp] + [ip] * 9 + [vp, vp]
         lib.dimb_selftest_attention.argtypes = [vp, ip, vp, vp, vp, vp, ip, ip, ip, ip, vp, vp, ip, fp, fp, fp]
         lib.dimb_gv_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_uint, vp, vp]
         _selftest = lib
@@ -227,6 +229,16 @@ def gemm_plan(conv: int, bn: int, split: bool, const_b: bool, num_kb: int, m_til
     if rc != OK:
         raise DimbError(f"gemm_plan({conv}, {bn}, ...) failed (code {rc})")
     return tuple(int(p) for p in out)
+
+
+def conv_mode(cout: int, B: int, H: int, W: int, num_sms: int) -> int:
+    """Tile shape the SuperPoint 3x3 conv launch picks on the tensor-core kernel, as the csrc/gemm.cuh CONV mode: 1 = 8 x 16 pixels,
+    2 = 16 x 16 pixels (dimb_selftest_conv_mode).  Host only."""
+    out = np.zeros(1, np.int32)
+    rc = load_selftest_library().dimb_selftest_conv_mode(cout, B, H, W, num_sms, _ptr(out))
+    if rc != OK:
+        raise DimbError(f"conv_mode({cout}, {B}, {H}, {W}, {num_sms}) failed (code {rc})")
+    return int(out[0])
 
 
 class SelfTest:
@@ -267,6 +279,12 @@ class SelfTest:
         (dimb_selftest_conv3x3), precision of the context.  x NHWC [B][H][W][cin], w OIHW [cout][cin][3][3].  The input allocation
         holds one more image of `guard`; the output buffer starts as `sentinel`.  Returns (out [B][Ho][Wo][cout], tail: one more
         output image of the buffer, plan as gemm())."""
+        return self.conv3x3_tiles(x, w, bias, pool, 0, guard, sentinel)[:3]
+
+    def conv3x3_tiles(self, x: np.ndarray, w: np.ndarray, bias: np.ndarray, pool: bool, tile: int, guard: float = 0.0,
+                      sentinel: float = 0.0):
+        """conv3x3() on one tile shape: tile 8 = 8 x 16 pixels, 16 = 16 x 16 pixels (cout 64), 0 = the shape production picks.
+        Returns (out, tail, plan, the csrc/gemm.cuh CONV mode that ran)."""
         x = np.ascontiguousarray(x, np.float32)
         w = np.ascontiguousarray(w, np.float32)
         bias = np.ascontiguousarray(bias, np.float32)
@@ -274,10 +292,19 @@ class SelfTest:
         cout = w.shape[0]
         Ho, Wo = (H // 2, W // 2) if pool else (H, W)
         out = np.zeros((B + 1, Ho, Wo, cout), np.float32)
-        plan = np.zeros(5, np.int32)
+        plan = np.zeros(6, np.int32)
         self.check(self.lib.dimb_selftest_conv3x3(self.h, _ptr(x), _ptr(w), _ptr(bias), _ptr(out), B, H, W, cin, cout, int(bool(pool)),
-                                                  float(guard), float(sentinel), _ptr(plan)), "selftest_conv3x3")
-        return out[:B], out[B], tuple(int(p) for p in plan)
+                                                  int(tile), float(guard), float(sentinel), _ptr(plan)), "selftest_conv3x3")
+        return out[:B], out[B], tuple(int(p) for p in plan[:5]), int(plan[5])
+
+    def conv3x3_time(self, B: int, H: int, W: int, cin: int, cout: int, pool: bool, tile: int, warm: int = 2, iters: int = 10):
+        """Device milliseconds per call of one 3x3 conv layer on device-generated activations (dimb_selftest_conv3x3_time),
+        precision of the context; tile as conv3x3_tiles().  Returns (ms, plan, CONV mode)."""
+        ms = np.zeros(1, np.float32)
+        plan = np.zeros(6, np.int32)
+        self.check(self.lib.dimb_selftest_conv3x3_time(self.h, B, H, W, cin, cout, int(bool(pool)), int(tile), warm, iters, _ptr(ms),
+                                                       _ptr(plan)), "selftest_conv3x3_time")
+        return float(ms[0]), tuple(int(p) for p in plan[:5]), int(plan[5])
 
     def attention(self, variant: int, Q: np.ndarray, K, V: np.ndarray, n, heads: int = 4, stopped=None, cross: bool = False,
                   lazy: float = -1.0, pad: float = 0.0, out_pad: float = 0.0) -> np.ndarray:

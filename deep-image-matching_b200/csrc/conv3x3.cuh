@@ -15,7 +15,8 @@ constexpr int conv_bn(int cout) { return cout == 64 ? 64 : 128; }
 // ------------------------------------------------------------------ epilogue: conv bias + ReLU (+2x2 max pool) -> NHWC hi/lo
 template <bool POOL>
 struct EpiConvRelu : EpiBase {
-  static constexpr int TW = kConvTW;  // pixels per tile row
+  static constexpr bool kScratch = false;
+  static constexpr int TW = kConvTW;  // pixels per tile row (both tile shapes)
   __half *hi, *lo;
   const float* bias;
   int H, W;      // conv resolution
@@ -86,13 +87,25 @@ int make_conv_layer(dimb_ctx* ctx, ConvLayer& L, const float* w, const float* b,
   return DIMB_OK;
 }
 
-// tiles of a 3x3 conv over B images of H x W (gemm.cuh CONV 1: 8 x 16 pixels per tile)
-inline int conv_m_tiles(int B, int H, int W) { return B * ceil_div(W, kConvTW) * ceil_div(H, kConvTH); }
+// tiles of a 3x3 conv over B images of H x W (gemm.cuh CONV 1: 8 x 16 pixels per tile, CONV 2: 16 x 16)
+inline int conv_m_tiles(int B, int H, int W, int conv = 1) {
+  return B * ceil_div(W, kConvTW) * ceil_div(H, conv == 2 ? kConvTH2 : kConvTH);
+}
 
-// 3x3 conv (zero padding 1) + bias + ReLU (+ 2x2 max pool) of NHWC hi/lo activations [B][H][W][cin] -> [B][Ho][Wo][cout]
-template <int BN, bool POOL>
-int run_conv3(dimb_ctx* ctx, cudaStream_t st, const ConvLayer& L, const __half* inh, const __half* inl, __half* outh, __half* outl,
-              int B, int H, int W, const char* tag) {
+// Tile shape (gemm.cuh CONV mode) of a 3x3 conv launch.  In EXACT the weights of the 64-channel layers do not fit next to the
+// A stages, so every tile streams all nine weight tiles from L2: 16 x 16 tiles cut the bytes fetched per output pixel from 2112 to
+// 1440.  FAST keeps those weights resident, and the taller tile still pays off there: fewer halo rows and half the per-tile
+// overheads per pixel (conv1b / conv2a / conv2b 1.20 / 1.02 / 1.36 x faster at the bench shapes, DESIGN.md section 4).  They are
+// used wherever they still give every SM at least two tiles (fewer, larger tiles would idle SMs on small inputs).
+inline int conv_mode(int cout, bool use_tc, int B, int H, int W, int num_sms) {
+  return conv_bn(cout) == 64 && use_tc && conv_m_tiles(B, H, W, 2) >= 2 * num_sms ? 2 : 1;
+}
+
+// run_conv3 on tiles of one shape (CONV 1 or 2)
+template <int BN, bool POOL, int CONV>
+int run_conv3_tiles(dimb_ctx* ctx, cudaStream_t st, const ConvLayer& L, const __half* inh, const __half* inl, __half* outh,
+                    __half* outl, int B, int H, int W, const char* tag) {
+  static_assert(CONV == 1 || (CONV == 2 && BN == 64), "16 x 16 tiles are instantiated for the 64-channel layers only");
   const bool exact = ctx->precision == DIMB_PRECISION_EXACT;
   TcOperands ops;
   GemmArgs g{};
@@ -117,18 +130,30 @@ int run_conv3(dimb_ctx* ctx, cudaStream_t st, const ConvLayer& L, const __half* 
     epi.Wo = POOL ? W / 2 : W;
     epi.C = L.cout;
   };
-  // gemm.cuh CONV 1: one (8+2)-row halo box per dx serves the three dy taps
-  const int box_h = kConvTH + 2;
-  DIMB_TRY(dimb_tmap_nhwc(ctx, &ops.Ah, inh, B, H, W, L.cin, box_h, kConvTW));
-  DIMB_TRY(dimb_tmap_nhwc(ctx, &ops.Al, inl, B, H, W, L.cin, box_h, kConvTW));
+  // gemm.cuh CONV 1 / 2: one (TH+2)-row halo box per dx serves the three dy taps
+  constexpr int TH = ConvTile<CONV>::TH;
+  DIMB_TRY(dimb_tmap_nhwc(ctx, &ops.Ah, inh, B, H, W, L.cin, TH + 2, kConvTW));
+  DIMB_TRY(dimb_tmap_nhwc(ctx, &ops.Al, inl, B, H, W, L.cin, TH + 2, kConvTW));
   ops.Bh = L.tmBh;
   ops.Bl = L.tmBl;
   g.num_kb = 9 * g.cin_blocks;
   g.tiles_x = ceil_div(W, kConvTW);
-  g.tiles_y = ceil_div(H, kConvTH);
+  g.tiles_y = ceil_div(H, TH);
   EpiConvRelu<POOL> epi;
   fill(epi);
-  return launch_gemm<BN, 1>(ctx, st, ops, g, epi, conv_m_tiles(B, H, W), L.cout_pad, tag);
+  return launch_gemm<BN, CONV>(ctx, st, ops, g, epi, conv_m_tiles(B, H, W, CONV), L.cout_pad, tag);
+}
+
+// 3x3 conv (zero padding 1) + bias + ReLU (+ 2x2 max pool) of NHWC hi/lo activations [B][H][W][cin] -> [B][Ho][Wo][cout], on the
+// tile shape conv_mode picks.  Both shapes give bitwise the same output: every element sees the same MMA sequence.
+template <int BN, bool POOL>
+int run_conv3(dimb_ctx* ctx, cudaStream_t st, const ConvLayer& L, const __half* inh, const __half* inl, __half* outh, __half* outl,
+              int B, int H, int W, const char* tag) {
+  if constexpr (BN == 64) {
+    if (conv_mode(L.cout, ctx->use_tc, B, H, W, ctx->num_sms) == 2)
+      return run_conv3_tiles<BN, POOL, 2>(ctx, st, L, inh, inl, outh, outl, B, H, W, tag);
+  }
+  return run_conv3_tiles<BN, POOL, 1>(ctx, st, L, inh, inl, outh, outl, B, H, W, tag);
 }
 
 }  // namespace

@@ -11,9 +11,10 @@
 //   128 fp32 accumulators per consumer thread plus the epilogue's working set without spilling.
 //   producer : cp.async.bulk.tensor -> swizzled smem stages, mbarrier full/empty ring
 //   consumers: warpgroup g issues wgmma (M = 64 rows 64g..64g+63 of the 128-row tile, N = BN, K = 16) into fp32
-//              registers; EXACT mode issues hi*hi + hi*lo + lo*hi per k-step (fp16 split operands).  After the
-//              last k-step the warpgroup stages its accumulator through shared memory, 64 columns at a time, so that
-//              thread r owns output row r and 32 consecutive columns -> fused epilogue functor
+//              registers (conv mode 2: rows 128g..128g+127 of a 256-row tile, two M = 64 halves); EXACT mode issues
+//              hi*hi + hi*lo + lo*hi per k-step (fp16 split operands).  After the last k-step the warpgroup stages its
+//              accumulator through shared memory, 64 columns at a time (mode 2: 16), so that thread r owns output row r
+//              and 32 consecutive columns -> fused epilogue functor
 //
 // A SIMT twin (simt_gemm_kernel) evaluates the same contraction on CUDA cores with the same
 // epilogue functors; it is a debug/bisect aid (DIMB_TC=0), never the default.  The kernel is persistent:
@@ -25,7 +26,7 @@
 struct TileCoord {
   int m0;         // GEMM: first global row of this 128-row tile
   int n0;         // first output column of this tile
-  int b, y0, x0;  // CONV: image index and top-left pixel of the 8x16 pixel tile
+  int b, y0, x0;  // CONV: image index and top-left pixel of the ConvTile<CONV>::TH x 16 pixel tile
 };
 
 struct GemmArgs {
@@ -59,18 +60,27 @@ static_assert(4 * kScratchFloats <= kStgFloats, "functor scratch must fit in the
 //   0  plain GEMM
 //   1  3x3 conv, tile = 8 rows x 16 pixels, one (8+2) x 16-pixel box of 64 channels per dx (three boxes per channel block);
 //      the three dy taps are the same stage at descriptor offsets of one box row (2048 B)
+//   2  3x3 conv, tile = 16 rows x 16 pixels, BN 64 only: as mode 1 with a (16+2) x 16-pixel box, so that every weight tile streamed
+//      from L2 serves 256 output pixels instead of 128.  A consumer warpgroup owns 128 pixel rows and issues two m64 wgmma per
+//      product; its accumulator is staged kStgCols2 columns at a time, which leaves no functor scratch (Epi::kScratch false)
 //   3  plain GEMM with 32-wide K blocks (64-byte rows, SWIZZLE_64B): half-size pipeline stages, so that more of them fit next to
 //      the 128 x 256 tiles
 constexpr int kConvTH = 8, kConvTW = 16;    // mode 1 tile
+constexpr int kConvTH2 = 16;                // mode 2 tile height
+// mode 2 staging: [64 rows][16 columns] per warpgroup, rows padded by 4 floats (80 B: the float4 row reads of 8 consecutive lanes hit 8
+// distinct 16-byte bank groups).  10 KB for both warpgroups instead of 35 KB: two A stages and four B slots fit next to it
+constexpr int kStgCols2 = 16, kStgPitch2 = kStgCols2 + 4;
+static_assert(32 % kStgCols2 == 0, "a thread's 32 epilogue columns are whole staging chunks");
+__host__ __device__ constexpr bool conv_is_3x3(int conv) { return conv == 1 || conv == 2; }
 template <int CONV>
 struct ConvTile {
-  static constexpr int TH = kConvTH, TW = kConvTW;
+  static constexpr int TH = CONV == 2 ? kConvTH2 : kConvTH, TW = kConvTW;
 };
 
 template <int CONV>
 __device__ __forceinline__ TileCoord make_tile_coord(const GemmArgs& g, int t) {
   TileCoord tc;
-  if (CONV == 1) {
+  if (conv_is_3x3(CONV)) {
     int per_img = g.tiles_x * g.tiles_y;
     tc.b = t / per_img;
     int rem = t - tc.b * per_img;
@@ -88,11 +98,11 @@ __device__ __forceinline__ TileCoord make_tile_coord(const GemmArgs& g, int t) {
 
 // ------------------------------------------------------------------ persistent tensor-core kernel
 // One CTA per SM loops over output tiles:
-//   * A and B have separate smem rings.  CONV mode fetches the activation tile ONCE per (dx, channel block) as
-//     a (8+2) x 16 pixel box and runs the three dy taps out of it by advancing the smem descriptor by one box row
-//     (16 px * 128 B = 2048 B, swizzle-atom aligned): 3 A loads per channel block instead of 9;
+//   * A and B have separate smem rings.  CONV modes 1 / 2 fetch the activation tile ONCE per (dx, channel block) as
+//     a (TH+2) x 16 pixel box (TH = 8 / 16) and run the three dy taps out of it by advancing the smem descriptor by one box
+//     row (16 px * 128 B = 2048 B, swizzle-atom aligned): 3 A loads per channel block instead of 9;
 //   * RESB: when all weight tiles of the layer fit (64->64 convs: 9 x 16 KB), they are loaded once per CTA and
-//     stay resident; only activations stream.
+//     stay resident; only activations stream.  Otherwise mode 2 releases each dy's B tile as its MMAs retire.
 struct PersCfg {
   int sa, sb;        // A / B ring depth (sb unused with RESB)
   int nkb_total;     // B tiles per output tile (RESB: resident tiles)
@@ -103,12 +113,15 @@ template <int BN, bool SPLIT, int CONV>
 struct PersGeom {
   static constexpr int kPl = SPLIT ? 2 : 1;
   static constexpr int kRowB = CONV == 3 ? 64 : 128;  // bytes per shared-memory operand row (K block of 32 / 64 halfs)
-  static constexpr int kABoxTx = CONV == 1 ? (kConvTH + 2) * kConvTW * 128 : kTileM * kRowB;  // bytes a TMA box delivers
+  static constexpr int kABoxTx =  // bytes a TMA box delivers
+      conv_is_3x3(CONV) ? (ConvTile<CONV>::TH + 2) * kConvTW * 128 : kTileM * kRowB;
   static constexpr int kABox = (kABoxTx + 1023) / 1024 * 1024;  // plane pitch inside a stage (swizzle-atom aligned)
   static constexpr int kATx = kPl * kABoxTx;
   static constexpr int kAStage = kPl * kABox;
   static constexpr int kBPlane = BN * kRowB;
   static constexpr int kBTile = kPl * kBPlane;
+  static constexpr int kStgFloats = CONV == 2 ? 64 * kStgPitch2 : ::kStgFloats;  // accumulator staging per consumer warpgroup
+  static constexpr int kStgBytes = 2 * kStgFloats * 4;
   static constexpr int kBudget = 232448 - 1024 - 1024 - kStgBytes;
 };
 
@@ -120,11 +133,15 @@ tc_gemm_pers_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_const
   using G = PersGeom<BN, SPLIT, CONV>;
   using namespace sm90;
   static_assert(BN % kStgCols == 0, "BN must be a multiple of the staging width");
+  static_assert(CONV != 2 || (BN == 64 && !Epi::kScratch), "mode 2: BN 64, and an epilogue without functor scratch");
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment by OFFSET from the __shared__ array (not by integer-casting the pointer): the compiler keeps the shared
   // address space and emits LDS / STS instead of generic LD / ST for every access derived from it
   uint8_t* smem = smem_raw + ((1024u - (sm90::smem_u32(smem_raw) & 1023u)) & 1023u);
-  constexpr bool ISCONV = CONV == 1;
+  constexpr bool ISCONV = conv_is_3x3(CONV);
+  constexpr int MH = CONV == 2 ? 2 : 1;  // 64-row MMA halves per consumer warpgroup
+  // mode 2 holds only three B slots: each dy's weight tile is released as soon as its MMAs retire (one commit group per dy)
+  constexpr bool EARLY_B = CONV == 2 && !RESB;
   constexpr bool K32 = CONV == 3;
   constexpr int KB_COLS = K32 ? 32 : 64;  // K elements per B tile / A stage
   constexpr int KSTEPS = K32 ? 2 : 4;     // 16-deep MMA steps per K block
@@ -138,7 +155,7 @@ tc_gemm_pers_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_const
   uint64_t* emptyA = fullA + SA;
   uint64_t* fullB = emptyA + SA;
   uint64_t* emptyB = fullB + nb_slots;
-  float* staging = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(fullA) + 1024);  // [2 warpgroups][kStgFloats]
+  float* staging = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(fullA) + 1024);  // [2 warpgroups][G::kStgFloats]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
@@ -259,12 +276,12 @@ tc_gemm_pers_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_const
   } else {  // ---------------- consumer warpgroup wg: rows 64 wg .. 64 wg + 63 of every tile
     setmaxnreg_inc<kConsumerRegs>();
     const int wg = warp >> 2, w4 = warp & 3;
-    // A rows of this warpgroup start 64 rows into the stage: 8 swizzle atoms of 8 rows, atom-aligned
-    const uint32_t a_wg = static_cast<uint32_t>(wg * 64 * G::kRowB);
-    float* stg = staging + wg * kStgFloats;
+    // A rows of this warpgroup start 64 MH rows into the stage: 8 MH swizzle atoms of 8 rows, atom-aligned
+    const uint32_t a_wg = static_cast<uint32_t>(wg * 64 * MH * G::kRowB);
+    float* stg = staging + wg * G::kStgFloats;
     uint32_t itA = 0, itB = 0;
     bool resb_ready = false;
-    float acc[BN / 2];
+    float acc[MH][BN / 2];
     for (int w = blockIdx.x; w < total; w += gridDim.x) {
       int n0;
       const TileCoord tc = tile_coord(w, n0);
@@ -289,51 +306,96 @@ tc_gemm_pers_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_const
             b_base = smem_u32(sB + sb * G::kBTile);
           }
           const uint32_t a_tap = a_base + (ISCONV ? dy * (kConvTW * 128) : 0);
-          const uint64_t a_h = make_sdesc(a_tap, kSbo, kLayout), a_l = make_sdesc(a_tap + G::kABox, kSbo, kLayout);
           const uint64_t b_h = make_sdesc(b_base, kSbo, kLayout), b_l = make_sdesc(b_base + G::kBPlane, kSbo, kLayout);
           wgmma_fence();
 #pragma unroll
           for (int k16 = 0; k16 < KSTEPS; ++k16) {
-            Wgmma<BN>::ss(acc, sdesc_advance_k(a_h, k16), sdesc_advance_k(b_h, k16), (o | dy | k16) != 0);
-            if (SPLIT) {
-              Wgmma<BN>::ss(acc, sdesc_advance_k(a_h, k16), sdesc_advance_k(b_l, k16), 1);
-              Wgmma<BN>::ss(acc, sdesc_advance_k(a_l, k16), sdesc_advance_k(b_h, k16), 1);
+#pragma unroll
+            for (int h = 0; h < MH; ++h) {  // every accumulator sees hi*hi, hi*lo, lo*hi per k16 step, whatever MH is
+              const uint32_t a_hh = a_tap + h * 64 * G::kRowB;
+              const uint64_t a_h = make_sdesc(a_hh, kSbo, kLayout), a_l = make_sdesc(a_hh + G::kABox, kSbo, kLayout);
+              Wgmma<BN>::ss(acc[h], sdesc_advance_k(a_h, k16), sdesc_advance_k(b_h, k16), (o | dy | k16) != 0);
+              if (SPLIT) {
+                Wgmma<BN>::ss(acc[h], sdesc_advance_k(a_h, k16), sdesc_advance_k(b_l, k16), 1);
+                Wgmma<BN>::ss(acc[h], sdesc_advance_k(a_l, k16), sdesc_advance_k(b_h, k16), 1);
+              }
             }
           }
+          if (EARLY_B) wgmma_commit();
         }
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_regs(acc);
-        if (lane == 0) {  // this warp is done with the stage and its B tiles
+        if (EARLY_B) {  // retire the dy groups in order, handing each weight tile back to the producer as soon as it is read
+          wgmma_wait<2>();
+          if (lane == 0) mbar_arrive(&emptyB[sb0]);
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(&emptyB[(sb0 + 1) % SB]);
+          wgmma_wait<0>();
+        } else {
+          wgmma_commit();
+          wgmma_wait<0>();
+        }
+#pragma unroll
+        for (int h = 0; h < MH; ++h) wgmma_fence_regs(acc[h]);
+        if (lane == 0) {  // this warp is done with the stage and its (remaining) B tiles
           mbar_arrive(&emptyA[s]);
           if (!RESB)
-            for (int dy = 0; dy < inner_n; ++dy) mbar_arrive(&emptyB[(sb0 + dy) % SB]);
+            for (int dy = EARLY_B ? 2 : 0; dy < inner_n; ++dy) mbar_arrive(&emptyB[(sb0 + dy) % SB]);
         }
         ++itA;
         if (!RESB) itB += inner_n;
       }
       resb_ready = true;  // every resident tile has been waited for once
-      // epilogue: accumulator -> staging (64 columns at a time) -> thread r = row of the tile, 32 consecutive columns
+      // epilogue: accumulator -> staging (mode 2: kStgCols2 columns at a time, otherwise 64) -> thread r = row of the tile, 32
+      // consecutive columns
       const int rr = 32 * (w4 & 1) + lane, cq = 32 * (w4 >> 1);
+      const int lr = 16 * w4 + (lane >> 2);
+      if constexpr (CONV == 2) {
+        // per 64-row half: stage the 64 columns chunk by chunk; warps 0, 1 collect columns 0-31, warps 2, 3 columns 32-63, then all
+        // four warps run the epilogue
+        constexpr int NCH = BN / kStgCols2, PER = 32 / kStgCols2;  // chunks per half, chunks per thread's 32 columns
 #pragma unroll
-      for (int c0 = 0; c0 < BN; c0 += kStgCols) {
-        const int lr = 16 * w4 + (lane >> 2);
+        for (int h = 0; h < MH; ++h) {
+          float v[32];
 #pragma unroll
-        for (int i = c0 / 8; i < (c0 + kStgCols) / 8; ++i) {
-          const int col = 8 * i - c0 + 2 * (lane & 3);
-          *reinterpret_cast<float2*>(stg + lr * kStgPitch + col) = make_float2(acc[4 * i], acc[4 * i + 1]);
-          *reinterpret_cast<float2*>(stg + (lr + 8) * kStgPitch + col) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+          for (int c = 0; c < NCH; ++c) {
+#pragma unroll
+            for (int i = c * kStgCols2 / 8; i < (c + 1) * kStgCols2 / 8; ++i) {
+              const int col = 8 * i - c * kStgCols2 + 2 * (lane & 3);
+              *reinterpret_cast<float2*>(stg + lr * kStgPitch2 + col) = make_float2(acc[h][4 * i], acc[h][4 * i + 1]);
+              *reinterpret_cast<float2*>(stg + (lr + 8) * kStgPitch2 + col) = make_float2(acc[h][4 * i + 2], acc[h][4 * i + 3]);
+            }
+            named_bar_sync(1 + wg, 128);
+            if ((w4 >> 1) == c / PER) {
+#pragma unroll
+              for (int q = 0; q < kStgCols2 / 4; ++q) {
+                const float4 x = *reinterpret_cast<const float4*>(stg + rr * kStgPitch2 + 4 * q);
+                const int j = (c % PER) * kStgCols2 + 4 * q;
+                v[j] = x.x, v[j + 1] = x.y, v[j + 2] = x.z, v[j + 3] = x.w;
+              }
+            }
+            named_bar_sync(1 + wg, 128);
+          }
+          epi(tc, 128 * wg + 64 * h + rr, n0 + cq, v, nullptr);
         }
-        named_bar_sync(1 + wg, 128);
-        float v[32];
+      } else {
 #pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float4 x = *reinterpret_cast<const float4*>(stg + rr * kStgPitch + cq + 4 * q);
-          v[4 * q] = x.x, v[4 * q + 1] = x.y, v[4 * q + 2] = x.z, v[4 * q + 3] = x.w;
+        for (int c0 = 0; c0 < BN; c0 += kStgCols) {
+#pragma unroll
+          for (int i = c0 / 8; i < (c0 + kStgCols) / 8; ++i) {
+            const int col = 8 * i - c0 + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(stg + lr * kStgPitch + col) = make_float2(acc[0][4 * i], acc[0][4 * i + 1]);
+            *reinterpret_cast<float2*>(stg + (lr + 8) * kStgPitch + col) = make_float2(acc[0][4 * i + 2], acc[0][4 * i + 3]);
+          }
+          named_bar_sync(1 + wg, 128);
+          float v[32];
+#pragma unroll
+          for (int q = 0; q < 8; ++q) {
+            const float4 x = *reinterpret_cast<const float4*>(stg + rr * kStgPitch + cq + 4 * q);
+            v[4 * q] = x.x, v[4 * q + 1] = x.y, v[4 * q + 2] = x.z, v[4 * q + 3] = x.w;
+          }
+          named_bar_sync(1 + wg, 128);
+          epi(tc, 64 * wg + rr, n0 + c0 + cq, v, stg + w4 * kScratchFloats);
+          named_bar_sync(1 + wg, 128);
         }
-        named_bar_sync(1 + wg, 128);
-        epi(tc, 64 * wg + rr, n0 + c0 + cq, v, stg + w4 * kScratchFloats);
-        named_bar_sync(1 + wg, 128);
       }
     }
     if (RESB && !resb_ready)  // no active tile: still drain the resident-weight loads before the CTA exits
@@ -344,6 +406,7 @@ tc_gemm_pers_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_const
 // ------------------------------------------------------------------ SIMT twin (debug path)
 template <int CONV>
 __device__ __forceinline__ float simt_load_a(const GemmArgs& g, const TileCoord& tc, int row, int k) {
+  static_assert(CONV != 2, "the SIMT twin runs 128-row tiles: 3x3 convs use mode 1");
   size_t off;
   if (CONV == 1) {
     const int cin = g.cin_blocks * 64;
@@ -431,6 +494,11 @@ PersCfg pers_config(int nkb, bool resb) {
     budget -= nkb * G::kBTile;
     c.sb = 0;
     c.sa = budget / G::kAStage;
+  } else if (CONV == 2) {
+    // the consumer hands each weight tile back as soon as its dy's MMAs retire, so three B slots already let the producer refill
+    // while the stage computes: double-buffer A first, then every B slot that fits (EXACT: 2 A stages, 4 B slots)
+    c.sa = budget >= 2 * G::kAStage + 3 * G::kBTile ? 2 : 1;
+    c.sb = (budget - c.sa * G::kAStage) / G::kBTile;
   } else {
     // conv consumes 3 B tiles per A stage: give B the deeper ring
     const int per = CONV == 1 ? 3 : 1;
@@ -444,7 +512,7 @@ PersCfg pers_config(int nkb, bool resb) {
   }
   if (c.sa > 8) c.sa = 8;
   if (c.sb > 12) c.sb = 12;
-  c.smem_bytes = c.sa * G::kAStage + (resb ? nkb : c.sb) * G::kBTile + 1024 + 1024 + kStgBytes;
+  c.smem_bytes = c.sa * G::kAStage + (resb ? nkb : c.sb) * G::kBTile + 1024 + 1024 + G::kStgBytes;
   return c;
 }
 
@@ -480,7 +548,7 @@ int launch_pers_auto(dimb_ctx* ctx, cudaStream_t st, const TcOperands& ops, cons
 }
 
 // n_pad: output columns rounded up to a multiple of BN (B operand rows beyond N read as zero via TMA OOB fill).
-// CONV + persistent: ops.Ah/Al must be NHWC maps with a (kConvTH+2) x kConvTW box (see dimb_tmap_nhwc callers).
+// CONV 1 / 2: ops.Ah/Al must be NHWC maps with a (ConvTile<CONV>::TH + 2) x kConvTW box (see dimb_tmap_nhwc callers).
 template <int BN, int CONV, class Epi>
 int launch_gemm(dimb_ctx* ctx, cudaStream_t st, const TcOperands& ops, GemmArgs g, const Epi& epi, int m_tiles, int n_pad,
                 const char* tag = "gemm", int force_split = -1) {
@@ -493,11 +561,16 @@ int launch_gemm(dimb_ctx* ctx, cudaStream_t st, const TcOperands& ops, GemmArgs 
     if (exact) return launch_pers_auto<BN, true, CONV, Epi>(ctx, st, ops, g, epi, m_tiles, n_pad);
     return launch_pers_auto<BN, false, CONV, Epi>(ctx, st, ops, g, epi, m_tiles, n_pad);
   }
-  if (force_split < 0 ? ctx->precision != DIMB_PRECISION_EXACT : force_split == 0) g.Al = g.Bl = nullptr;
-  dim3 grid(m_tiles, n_pad / 32);
-  simt_gemm_kernel<CONV, Epi><<<grid, 128, 0, st>>>(g, epi);
-  DIMB_LAUNCH_CHECK(ctx);
-  return DIMB_OK;
+  if constexpr (CONV == 2) {
+    dimb_set_error(ctx, std::string(tag) + ": 16 x 16 conv tiles need the tensor-core kernel (DIMB_TC=0 runs 8 x 16 tiles)");
+    return DIMB_ERR_UNSUPPORTED;
+  } else {
+    if (force_split < 0 ? ctx->precision != DIMB_PRECISION_EXACT : force_split == 0) g.Al = g.Bl = nullptr;
+    dim3 grid(m_tiles, n_pad / 32);
+    simt_gemm_kernel<CONV, Epi><<<grid, 128, 0, st>>>(g, epi);
+    DIMB_LAUNCH_CHECK(ctx);
+    return DIMB_OK;
+  }
 }
 
 // ------------------------------------------------------------------ generic epilogues
@@ -506,6 +579,7 @@ int launch_gemm(dimb_ctx* ctx, cudaStream_t st, const TcOperands& ops, GemmArgs 
 // the B rows a tile multiplies with (stacked per-layer weights, or "the other image" for similarity matrices).
 struct EpiBase {
   static constexpr bool kConstB = true;       // b_row_offset() == 0 for every tile (B panel may stay resident)
+  static constexpr bool kScratch = true;      // operator() uses its per-warp scratch (conv mode 2 has none to give)
   __device__ int m0_of(int t) const { return t * kTileM; }
   __device__ int b_row_offset(const TileCoord&) const { return 0; }
   __device__ bool tile_active(const TileCoord&) const { return true; }

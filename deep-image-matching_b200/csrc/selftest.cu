@@ -14,6 +14,39 @@ extern "C" int dimb_selftest_gemm_plan(int conv, int bn, int split, int const_b,
                                        int* out);
 
 namespace {
+// run_conv3 on the tile shape of gemm.cuh CONV mode `conv` (1: 8 x 16, 2: 16 x 16, BN 64 only)
+template <int BN, bool POOL>
+int run_conv3_mode(dimb_ctx* ctx, const ConvLayer& L, const __half* xh, const __half* xl, __half* oh, __half* ol, int B, int H, int W,
+                   int conv, const char* tag) {
+  if constexpr (BN == 64) {
+    if (conv == 2) return run_conv3_tiles<64, POOL, 2>(ctx, 0, L, xh, xl, oh, ol, B, H, W, tag);
+  }
+  return run_conv3_tiles<BN, POOL, 1>(ctx, 0, L, xh, xl, oh, ol, B, H, W, tag);
+}
+
+// gemm.cuh CONV mode of a conv3x3 self-test call: tile 0 = the production choice (conv_mode), 8 = 8 x 16 tiles, 16 = 16 x 16 tiles
+// (cout 64 on the tensor-core kernel); -1 when the tile cannot run
+int selftest_conv_mode(dimb_ctx* ctx, int tile, int cout, int B, int H, int W) {
+  if (tile == 0) return conv_mode(cout, ctx->use_tc, B, H, W, ctx->num_sms);
+  if (tile == 8) return 1;
+  if (tile == 16 && conv_bn(cout) == 64 && ctx->use_tc) return 2;
+  return -1;
+}
+
+// hash of (seed, i) -> a value in [-1, 1) with 15 significant bits, split into fp16 hi / lo planes (lo null: hi only)
+__global__ void fill_split_kernel(__half* __restrict__ hi, __half* __restrict__ lo, size_t n, unsigned seed) {
+  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    uint32_t h = static_cast<uint32_t>(i) * 0x9E3779B1u ^ static_cast<uint32_t>(i >> 32) * 0x85EBCA77u ^ seed;
+    h ^= h >> 15;
+    h *= 0x2C1B3C6Du;
+    h ^= h >> 12;
+    const float v = static_cast<float>(h & 0xFFFFu) * (1.f / 32768.f) - 1.f;
+    __half a, b;
+    split_f32(v, a, b);
+    hi[i] = a;
+    if (lo) lo[i] = b;
+  }
+}
 __global__ void split_rows_kernel(const float* __restrict__ src, __half* __restrict__ hi, __half* __restrict__ lo, size_t n) {
   const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -94,7 +127,8 @@ void launch_plan(dimb_ctx* ctx, int conv, int bn, bool const_b, int num_kb, int 
 }  // namespace
 
 // Launch plan of the persistent kernel (gemm.cuh pers_plan, as launch_gemm computes it) for one call shape, host only: no context, no
-// device.  conv: 0 plain GEMM (bn 64 / 128 / 256), 1 3x3 conv (bn 64 / 128), 3 32-wide K blocks (bn 256); split: EXACT operands
+// device.  conv: 0 plain GEMM (bn 64 / 128 / 256), 1 3x3 conv on 8 x 16 tiles (bn 64 / 128), 2 3x3 conv on 16 x 16 tiles (bn 64),
+// 3 32-wide K blocks (bn 256); split: EXACT operands
 // (hi / lo planes); const_b: Epi::kConstB of the epilogue; num_kb: B tiles per output tile.  out[5] = {resb, sa, sb, smem_bytes, grid}.
 extern "C" int dimb_selftest_gemm_plan(int conv, int bn, int split, int const_b, int num_kb, int m_tiles, int n_tiles, int num_sms,
                                        int* out) {
@@ -105,6 +139,7 @@ extern "C" int dimb_selftest_gemm_plan(int conv, int bn, int split, int const_b,
   else if (conv == 0 && bn == 256) plan_of<256, 0>(s, cb, num_kb, m_tiles, n_tiles, num_sms, out);
   else if (conv == 1 && bn == 64) plan_of<64, 1>(s, cb, num_kb, m_tiles, n_tiles, num_sms, out);
   else if (conv == 1 && bn == 128) plan_of<128, 1>(s, cb, num_kb, m_tiles, n_tiles, num_sms, out);
+  else if (conv == 2 && bn == 64) plan_of<64, 2>(s, cb, num_kb, m_tiles, n_tiles, num_sms, out);
   else if (conv == 3 && bn == 256) plan_of<256, 3>(s, cb, num_kb, m_tiles, n_tiles, num_sms, out);
   else return DIMB_ERR_ARG;
   return DIMB_OK;
@@ -178,11 +213,15 @@ extern "C" int dimb_selftest_gemm(dimb_ctx* ctx, const float* A, const float* B,
 //   past the last image, or across the image boundary, would bring it in.  `guard` must be finite: the ReLU turns NaN into 0.
 //   out: [B + 1][Ho][Wo][cout] with Ho, Wo = H / 2, W / 2 under pool: the B output images joined from their hi + lo planes (hi only in
 //   FAST), then one image of tail; every element starts as `sentinel` (fp16-exact), so unwritten and stray writes show.
-//   plan[5] (may be null): as dimb_selftest_gemm.
+//   tile: 0 = the tile shape production picks for this call (conv3x3.cuh conv_mode), 8 = 8 x 16 pixels, 16 = 16 x 16 pixels (cout 64,
+//   tensor-core kernel only).
+//   plan[6] (may be null): as dimb_selftest_gemm, then the gemm.cuh CONV mode that ran (1 or 2).
 extern "C" int dimb_selftest_conv3x3(dimb_ctx* ctx, const float* x, const float* w, const float* bias, float* out, int B, int H, int W,
-                                     int cin, int cout, int pool, float guard, float sentinel, int* plan) {
+                                     int cin, int cout, int pool, int tile, float guard, float sentinel, int* plan) {
   if (!ctx || !x || !w || !bias || !out || B < 1 || H < 1 || W < 1 || cin < 64 || cin % 64) return DIMB_ERR_ARG;
   if ((cout != 64 && (cout < 128 || cout % 128)) || (pool && (H < 2 || W < 2))) return DIMB_ERR_ARG;
+  const int mode = selftest_conv_mode(ctx, tile, cout, B, H, W);
+  if (mode < 0) return DIMB_ERR_ARG;
   DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
   const bool exact = ctx->precision == DIMB_PRECISION_EXACT;
   const int Ho = pool ? H / 2 : H, Wo = pool ? W / 2 : W;
@@ -201,16 +240,96 @@ extern "C" int dimb_selftest_conv3x3(dimb_ctx* ctx, const float* x, const float*
     DIMB_TRY(make_conv_layer(ctx, L, w, bias, cout, cin, 3, conv_bn(cout)));
   }
   const int bn = conv_bn(cout);
-  if (bn == 64)
-    DIMB_TRY(pool ? (run_conv3<64, true>(ctx, 0, L, xh, xl, oh, ol, B, H, W, "selftest.conv3x3"))
-                  : (run_conv3<64, false>(ctx, 0, L, xh, xl, oh, ol, B, H, W, "selftest.conv3x3")));
-  else
-    DIMB_TRY(pool ? (run_conv3<128, true>(ctx, 0, L, xh, xl, oh, ol, B, H, W, "selftest.conv3x3"))
-                  : (run_conv3<128, false>(ctx, 0, L, xh, xl, oh, ol, B, H, W, "selftest.conv3x3")));
+  const char* tag = "selftest.conv3x3";
+  if (tile == 0) {  // the production entry itself
+    if (bn == 64)
+      DIMB_TRY(pool ? (run_conv3<64, true>(ctx, 0, L, xh, xl, oh, ol, B, H, W, tag)) : (run_conv3<64, false>(ctx, 0, L, xh, xl, oh, ol, B, H, W, tag)));
+    else
+      DIMB_TRY(pool ? (run_conv3<128, true>(ctx, 0, L, xh, xl, oh, ol, B, H, W, tag))
+                    : (run_conv3<128, false>(ctx, 0, L, xh, xl, oh, ol, B, H, W, tag)));
+  } else if (bn == 64) {
+    DIMB_TRY(pool ? (run_conv3_mode<64, true>(ctx, L, xh, xl, oh, ol, B, H, W, mode, tag))
+                  : (run_conv3_mode<64, false>(ctx, L, xh, xl, oh, ol, B, H, W, mode, tag)));
+  } else {
+    DIMB_TRY(pool ? (run_conv3_mode<128, true>(ctx, L, xh, xl, oh, ol, B, H, W, mode, tag))
+                  : (run_conv3_mode<128, false>(ctx, L, xh, xl, oh, ol, B, H, W, mode, tag)));
+  }
   join_rows_kernel<<<ceil_div(static_cast<int>(nout), 256), 256>>>(oh, exact ? ol : nullptr, d_out, nout);
   DIMB_TRY(sync_call(ctx, "dimb_selftest_conv3x3"));
   DIMB_CUDA_OK(ctx, cudaMemcpy(out, d_out, sizeof(float) * nout, cudaMemcpyDeviceToHost));
-  launch_plan(ctx, 1, bn, EpiConvRelu<false>::kConstB, 9 * (cin / 64), conv_m_tiles(B, H, W), L.cout_pad / bn, plan);
+  launch_plan(ctx, mode, bn, EpiConvRelu<false>::kConstB, 9 * (cin / 64), conv_m_tiles(B, H, W, mode), L.cout_pad / bn, plan);
+  if (plan) plan[5] = mode;
+  return DIMB_OK;
+}
+
+// Host only: the gemm.cuh CONV mode (tile shape) run_conv3 picks for a conv of B images of H x W with `cout` output channels on a
+// device with num_sms SMs (conv3x3.cuh conv_mode), tensor-core kernel, either precision.
+extern "C" int dimb_selftest_conv_mode(int cout, int B, int H, int W, int num_sms, int* out) {
+  if (!out || B < 1 || H < 1 || W < 1 || num_sms < 1 || cout < 1) return DIMB_ERR_ARG;
+  *out = conv_mode(cout, true, B, H, W, num_sms);
+  return DIMB_OK;
+}
+
+// Device time of one 3x3 conv layer at a production size, precision of the context: device-generated activations
+// [B][H][W][cin] (hi / lo planes), seeded weights, `warm` untimed calls, then `iters` calls between CUDA events.  tile as
+// dimb_selftest_conv3x3.  ms: milliseconds per call.  plan[6] (may be null): as dimb_selftest_conv3x3.
+extern "C" int dimb_selftest_conv3x3_time(dimb_ctx* ctx, int B, int H, int W, int cin, int cout, int pool, int tile, int warm, int iters,
+                                          float* ms, int* plan) {
+  if (!ctx || !ms || B < 1 || H < 2 || W < 2 || cin < 64 || cin % 64 || warm < 0 || iters < 1) return DIMB_ERR_ARG;
+  if (cout != 64 && (cout < 128 || cout % 128)) return DIMB_ERR_ARG;
+  const int mode = selftest_conv_mode(ctx, tile, cout, B, H, W);
+  if (mode < 0) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const bool exact = ctx->precision == DIMB_PRECISION_EXACT;
+  const int Ho = pool ? H / 2 : H, Wo = pool ? W / 2 : W;
+  const size_t nin = static_cast<size_t>(B) * H * W * cin, nout = static_cast<size_t>(B) * Ho * Wo * cout;
+  DevTmp t{ctx, {}};
+  __half *xh, *xl, *oh, *ol;
+  DIMB_TRY(t.get(&xh, nin));
+  DIMB_TRY(t.get(&xl, nin));
+  DIMB_TRY(t.get(&oh, nout));
+  DIMB_TRY(t.get(&ol, nout));
+  fill_split_kernel<<<4 * ctx->num_sms, 256>>>(xh, exact ? xl : nullptr, nin, 12345u);
+  DIMB_CUDA_OK(ctx, cudaGetLastError());
+  std::vector<float> w(static_cast<size_t>(cout) * cin * 9), bias(cout);
+  uint32_t s = 1;
+  for (float& v : w) v = static_cast<float>((s = s * 1664525u + 1013904223u) >> 8) * (0.1f / 16777216.f) - 0.05f;
+  for (float& v : bias) v = static_cast<float>((s = s * 1664525u + 1013904223u) >> 8) * (0.2f / 16777216.f) - 0.1f;
+  ConvLayer L;
+  {
+    OwnerScope own(ctx, &t.p);
+    DIMB_TRY(make_conv_layer(ctx, L, w.data(), bias.data(), cout, cin, 3, conv_bn(cout)));
+  }
+  const int bn = conv_bn(cout);
+  auto run = [&]() {
+    const char* tag = "selftest.conv3x3_time";
+    if (bn == 64)
+      return pool ? run_conv3_mode<64, true>(ctx, L, xh, xl, oh, ol, B, H, W, mode, tag)
+                  : run_conv3_mode<64, false>(ctx, L, xh, xl, oh, ol, B, H, W, mode, tag);
+    return pool ? run_conv3_mode<128, true>(ctx, L, xh, xl, oh, ol, B, H, W, mode, tag)
+                : run_conv3_mode<128, false>(ctx, L, xh, xl, oh, ol, B, H, W, mode, tag);
+  };
+  for (int i = 0; i < warm; ++i) DIMB_TRY(run());
+  cudaEvent_t e0, e1;
+  DIMB_CUDA_OK(ctx, cudaEventCreate(&e0));
+  DIMB_CUDA_OK(ctx, cudaEventCreate(&e1));
+  auto cuda_ok = [&](cudaError_t ce, const char* what) -> int {
+    if (ce == cudaSuccess) return DIMB_OK;
+    dimb_set_error(ctx, std::string("dimb_selftest_conv3x3_time: ") + what + ": " + cudaGetErrorString(ce));
+    return DIMB_ERR_CUDA;
+  };
+  int rc = cuda_ok(cudaEventRecord(e0, 0), "cudaEventRecord");
+  for (int i = 0; i < iters && rc == DIMB_OK; ++i) rc = run();
+  if (rc == DIMB_OK) rc = cuda_ok(cudaEventRecord(e1, 0), "cudaEventRecord");
+  if (rc == DIMB_OK) rc = sync_call(ctx, "dimb_selftest_conv3x3_time");
+  float total = 0.f;
+  if (rc == DIMB_OK) rc = cuda_ok(cudaEventElapsedTime(&total, e0, e1), "cudaEventElapsedTime");
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  DIMB_TRY(rc);
+  *ms = total / iters;
+  launch_plan(ctx, mode, bn, EpiConvRelu<false>::kConstB, 9 * (cin / 64), conv_m_tiles(B, H, W, mode), L.cout_pad / bn, plan);
+  if (plan) plan[5] = mode;
   return DIMB_OK;
 }
 
