@@ -32,7 +32,7 @@ EXPORTS = [
     "dimb_tile_grid", "dimb_tile_cut_dev", "dimb_tile_merge_dev", "dimb_tile_views_dev", "dimb_tile_match_merge_dev",
     "dimb_resize_area_tab", "dimb_resize_area_dev", "dimb_kpts_extent_dev", "dimb_tile_preselect_dev",
     "dimb_resize_area_linear_tab", "dimb_resize_area_linear_dev", "dimb_pyr_size", "dimb_pyr_dev", "dimb_fstore_rescale_dev",
-    "dimb_tile_preselect_pairs_dev",
+    "dimb_tile_preselect_pairs_dev", "dimb_rot90_dev", "dimb_fstore_unrotate_dev",
 ]
 
 
@@ -178,6 +178,8 @@ def load_library():
     lib.dimb_pyr_size.argtypes = [ip, ip, ip, C.POINTER(ip), C.POINTER(ip)]
     lib.dimb_pyr_dev.argtypes = [vp, vp, ip, ip, ip, ip, ip, vp, vp]
     lib.dimb_fstore_rescale_dev.argtypes = [vp, ip, vp, ip, ip, ip, vp]
+    lib.dimb_rot90_dev.argtypes = [vp, vp, ip, ip, ip, ip, vp, vp, vp]
+    lib.dimb_fstore_unrotate_dev.argtypes = [vp, ip, vp, vp, vp, vp, vp]
     lib.dimb_kpts_extent_dev.argtypes = [vp, ip, vp, ip, vp, vp, vp]
     lib.dimb_tile_preselect_dev.argtypes = [vp, ip, C.POINTER(FeatsDev), C.POINTER(FeatsDev), vp, vp, ip] + [ip] * 6 + \
         [C.c_double, C.c_double, ip, vp, vp, vp]
@@ -510,6 +512,14 @@ class Context:
         """cv2.pyrDown `level` times (1..3) or cv2.pyrUp once (-1) of B float32 device images [B][H][W][channels], 1 or 3 channels,
         into d_dst [B][H2][W2][channels] (pyr_size), bitwise (dimb_pyr_dev); asynchronous on `stream`."""
         self.check(self.lib.dimb_pyr_dev(self.h, d_src, B, H, W, channels, level, d_dst, stream), "dimb_pyr_dev")
+
+    def rot90_dev(self, d_src, B, H, W, channels, rotations, d_dst, stream=0):
+        """cv2.rotate of B float32 device images [B][H][W][channels], 1 or 3 channels, by rotations[b] in (0, 90, 180, 270) degrees
+        clockwise, into d_dst (image b at b * H * W * channels, (W, H) for 90 / 270), bitwise (dimb_rot90_dev); asynchronous on `stream`."""
+        r, p = _int_array(rotations)
+        if len(r) != B:
+            raise ValueError(f"rot90_dev needs one rotation per image: {len(r)} for {B} images")
+        self.check(self.lib.dimb_rot90_dev(self.h, d_src, B, H, W, channels, p, d_dst, stream), "dimb_rot90_dev")
 
     def kpts_extent_dev(self, B, d_kpts, kpt_ld, d_counts, d_size_out, stream=0):
         """Own-extent normalisation size (1 + max) - min per axis of B keypoint sets [B][kpt_ld][2] -> d_size_out [B][2] float32
@@ -930,6 +940,15 @@ class FeatureStoreDev:
         resized by `level` pyramid steps, back in the original image's pixels.  Asynchronous on `stream`."""
         s, p = _int_array(slots)
         self.ctx.check(self.ctx.lib.dimb_fstore_rescale_dev(self.h, len(s), p, int(level), int(H), int(W), stream), "dimb_fstore_rescale_dev")
+
+    def unrotate_dev(self, slots, rotations, heights, widths, stream=0):
+        """Keypoints of `slots`, extracted from images turned by `rotations` (degrees clockwise), back on the original heights[b] x
+        widths[b] images, and those sizes in the headers (dimb_fstore_unrotate_dev).  Asynchronous on `stream`."""
+        arrays = [_int_array(v) for v in (slots, rotations, heights, widths)]
+        if len({len(a) for a, _ in arrays}) != 1:
+            raise ValueError("unrotate_dev needs one rotation, height and width per slot")
+        self.ctx.check(self.ctx.lib.dimb_fstore_unrotate_dev(self.h, len(arrays[0][0]), *[p for _, p in arrays], stream),
+                       "dimb_fstore_unrotate_dev")
 
     def tile_views_dev(self, src_slots, n_tiles, views: "FeatureStoreDev", dst_slots, d_map, stream=0):
         """Tile views of the merged slots src_slots (dimb_tile_views_dev): view slot dst_slots[b] + t of `views`, map row of the same

@@ -25,7 +25,9 @@ constexpr int kMaxTiles = 2048;        // tile_idx is stored as float16: integer
 constexpr int kChunk = 1024;           // records per shared-memory sort
 constexpr int kScanThreads = 1024;     // threads of the one-CTA-per-segment scans
 constexpr int kSlotKeysA = 64, kSlotKeysB = 65, kSlotParams = 66, kSlotSrc = 67, kSlotCount = 68;  // context scratch slots
-constexpr int kSlotResizeTab = 69, kSlotPreSides = 70, kSlotPyrA = 71, kSlotPyrB = 72, kSlotRescale = 73;
+constexpr int kSlotResizeTab = 69, kSlotPreSides = 70, kSlotPyrA = 71, kSlotPyrB = 72, kSlotRescale = 73, kSlotRotCodes = 74;
+constexpr int kSlotUnrotate = 75;
+constexpr int kRotTile = 32;            // dimb_rot90_dev: source tile side (pixels), staged in shared memory
 constexpr int kCvFloatLanes = 4;        // float32 lanes of OpenCV's 128-bit baseline SIMD (ResizeAreaFastVec_SIMD_32f)
 constexpr unsigned long long kNoKey = ~0ull;
 constexpr int kBorder = 2;             // border_thr of extractor_base.py:335
@@ -508,10 +510,12 @@ __global__ void __launch_bounds__(128) pyr_up_kernel(const float* __restrict__ s
   dst[(static_cast<size_t>(b) * 2 * H + Y) * row_len + j] = __fmul_rn(v, 1.f / 64.f);
 }
 
-// Multiplies the float16 keypoints of B store slots by `scale` (a power of two) and writes [H, W] into their headers as
-// fs_put_kernel does.  grid (cap / 256, B); empty slots are left alone.
-__global__ void fs_rescale_kernel(FsLayout L, const int* __restrict__ slots, float scale, int H, int W) {
-  const SlotPtrs s = L.at(slots[blockIdx.y]);
+// The keypoint pass shared by the store remaps below: for a non-empty slot, thread (0, 0) writes [H, W] into the header as
+// fs_put_kernel does, and keypoint i (one per thread of a (cap / 256)-wide grid row) becomes map(x, y) in float32, rounded to float16.
+// Empty slots are left alone.
+template <class Map>
+__device__ __forceinline__ void fs_remap_slot(const FsLayout& L, int slot, int H, int W, Map map) {
+  const SlotPtrs s = L.at(slot);
   if (!s.hdr[3]) return;
   const int n = min(s.hdr[0], L.cap), i = blockIdx.x * blockDim.x + threadIdx.x;
   if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -519,8 +523,63 @@ __global__ void fs_rescale_kernel(FsLayout L, const int* __restrict__ slots, flo
     s.hdr[2] = static_cast<int>(__half2float(__float2half_rn(fminf(static_cast<float>(W), 65504.f))));
   }
   if (i >= n) return;
-  s.kpts[2 * i] = __float2half_rn(__fmul_rn(__half2float(s.kpts[2 * i]), scale));
-  s.kpts[2 * i + 1] = __float2half_rn(__fmul_rn(__half2float(s.kpts[2 * i + 1]), scale));
+  const float2 p = map(__half2float(s.kpts[2 * i]), __half2float(s.kpts[2 * i + 1]));
+  s.kpts[2 * i] = __float2half_rn(p.x);
+  s.kpts[2 * i + 1] = __float2half_rn(p.y);
+}
+
+// Multiplies the float16 keypoints of B store slots by `scale` (a power of two) and writes [H, W] into their headers.  grid (cap / 256, B).
+__global__ void fs_rescale_kernel(FsLayout L, const int* __restrict__ slots, float scale, int H, int W) {
+  fs_remap_slot(L, slots[blockIdx.y], H, W, [scale](float x, float y) { return make_float2(__fmul_rn(x, scale), __fmul_rn(y, scale)); });
+}
+
+struct Unrotate {  // one slot of dimb_fstore_unrotate_dev: its rotation code (0..3 quarter turns clockwise) and original size
+  int slot, quarter, H, W;
+};
+
+// The inverse of cv2.rotate on pixel indices of the original H x W image, per slot: (x', y') in the rotated image ->
+// 90: (y', H - 1 - x'), 180: (W - 1 - x', H - 1 - y'), 270: (W - 1 - y', x'), each difference one float32 rounding.  grid (cap / 256, B).
+__global__ void fs_unrotate_kernel(FsLayout L, const Unrotate* __restrict__ items) {
+  const Unrotate u = items[blockIdx.y];
+  const float h1 = static_cast<float>(u.H - 1), w1 = static_cast<float>(u.W - 1);
+  const int q = u.quarter;
+  fs_remap_slot(L, u.slot, u.H, u.W, [=](float x, float y) {
+    if (q == 1) return make_float2(y, __fsub_rn(h1, x));
+    if (q == 2) return make_float2(__fsub_rn(w1, x), __fsub_rn(h1, y));
+    if (q == 3) return make_float2(__fsub_rn(w1, y), x);
+    return make_float2(x, y);
+  });
+}
+
+// cv2.rotate of B float32 images [H][W][C] by per-image quarter turns quarter[b] (0 = copy, 1 = 90 clockwise, 2 = 180, 3 = 270); image
+// b of dst starts at b * H * W * C and is [H][W][C] (0, 180) or [W][H][C] (90, 270).  One CTA per 32 x 32-pixel source tile, staged in
+// shared memory (row stride 32 C + 1 floats, so that the transposed reads of 90 / 270 hit 32 distinct banks); the CTA then writes the
+// tile's image under the rotation row by row, so global reads and writes both run along rows.  A permutation: bitwise cv2.rotate.
+// grid (ceil(W / 32), ceil(H / 32), B), block (32, 8).
+__global__ void __launch_bounds__(256) rot90_kernel(const float* __restrict__ src, float* __restrict__ dst, int H, int W, int C,
+                                                    const int* __restrict__ quarter) {
+  __shared__ float tile[kRotTile][kRotTile * 3 + 1];
+  const int q = quarter[blockIdx.z], x0 = blockIdx.x * kRotTile, y0 = blockIdx.y * kRotTile, lane = threadIdx.x;
+  const size_t img = static_cast<size_t>(blockIdx.z) * H * W * C;
+  const int row_len = min(kRotTile, W - x0) * C;
+  for (int r = threadIdx.y; r < kRotTile && y0 + r < H; r += blockDim.y)
+    for (int e = lane; e < row_len; e += kRotTile) tile[r][e] = src[img + (static_cast<size_t>(y0 + r) * W + x0) * C + e];
+  __syncthreads();
+  // destination row a of the tile's image (a = 0..31) and pixel p along it -> source pixel (sy, sx) of the tile
+  const bool turn = q & 1;
+  const int Wd = turn ? H : W;
+  for (int a = threadIdx.y; a < kRotTile; a += blockDim.y) {
+    for (int e = lane; e < kRotTile * C; e += kRotTile) {
+      const int p = e / C, c = e - p * C;
+      int sy, sx, dy, dx;
+      if (q == 0) sy = a, sx = p, dy = y0 + a, dx = x0 + p;
+      else if (q == 1) sy = kRotTile - 1 - p, sx = a, dy = x0 + a, dx = H - y0 - kRotTile + p;
+      else if (q == 2) sy = kRotTile - 1 - a, sx = kRotTile - 1 - p, dy = H - y0 - kRotTile + a, dx = W - x0 - kRotTile + p;
+      else sy = p, sx = kRotTile - 1 - a, dy = W - x0 - kRotTile + a, dx = y0 + p;
+      if (y0 + sy >= H || x0 + sx >= W) continue;
+      dst[img + (static_cast<size_t>(dy) * Wd + dx) * C + c] = tile[sy][sx * C + c];
+    }
+  }
 }
 
 // One CTA per image: size = (1 + max) - min per axis over its keypoints, {1, 1} without keypoints (min / max are exact in any order).
@@ -897,6 +956,49 @@ int dimb_fstore_rescale_dev(dimb_fstore* fs, int B, const int* slots, int level,
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_slots, slots, B * sizeof(int), cudaMemcpyHostToDevice, st));
   ProfScope prof(ctx, st, "tile.pyr");
   fs_rescale_kernel<<<dim3(ceil_div(fs->cap, 256), B), 256, 0, st>>>(fs_layout(fs), d_slots, std::ldexp(1.f, level), height, width);
+  DIMB_LAUNCH_CHECK(ctx);
+  return DIMB_OK;
+}
+
+// upright (image_matching.py:496 rotates the images, :703 rotates the keypoints back)
+int dimb_rot90_dev(dimb_ctx* ctx, const float* d_src, int B, int height, int width, int channels, const int* rotations, float* d_dst,
+                   void* stream) {
+  if (!ctx || !d_src || !d_dst || !rotations || B < 1 || B > 65535 || (channels != 1 && channels != 3) || height < 1 || width < 1 ||
+      height > (1 << 20) || width > (1 << 20) || ceil_div(height, kRotTile) > 65535)
+    return DIMB_ERR_ARG;
+  std::vector<int> quarter(B);
+  for (int b = 0; b < B; ++b) {
+    if (rotations[b] != 0 && rotations[b] != 90 && rotations[b] != 180 && rotations[b] != 270) return DIMB_ERR_ARG;
+    quarter[b] = rotations[b] / 90;
+  }
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int* d_quarter;
+  DIMB_TRY(dimb_scratch(ctx, kSlotRotCodes, static_cast<size_t>(B) * sizeof(int), reinterpret_cast<void**>(&d_quarter)));
+  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_quarter, quarter.data(), B * sizeof(int), cudaMemcpyHostToDevice, st));
+  ProfScope prof(ctx, st, "tile.rot");
+  rot90_kernel<<<dim3(ceil_div(width, kRotTile), ceil_div(height, kRotTile), B), dim3(kRotTile, 8), 0, st>>>(d_src, d_dst, height, width,
+                                                                                                              channels, d_quarter);
+  DIMB_LAUNCH_CHECK(ctx);
+  return DIMB_OK;
+}
+
+int dimb_fstore_unrotate_dev(dimb_fstore* fs, int B, const int* slots, const int* rotations, const int* heights, const int* widths,
+                             void* stream) {
+  if (!fs || !slots || !rotations || !heights || !widths || B < 1 || B > 65535) return DIMB_ERR_ARG;
+  std::vector<Unrotate> items(B);
+  for (int b = 0; b < B; ++b) {
+    const int r = rotations[b];
+    if (slots[b] < 0 || slots[b] >= fs->n_slots || (r != 0 && r != 90 && r != 180 && r != 270) || heights[b] < 1 || widths[b] < 1)
+      return DIMB_ERR_ARG;
+    items[b] = {slots[b], r / 90, heights[b], widths[b]};
+  }
+  dimb_ctx* ctx = fs->ctx;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  Unrotate* d_items;
+  DIMB_TRY(dimb_scratch(ctx, kSlotUnrotate, static_cast<size_t>(B) * sizeof(Unrotate), reinterpret_cast<void**>(&d_items)));
+  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_items, items.data(), B * sizeof(Unrotate), cudaMemcpyHostToDevice, st));
+  ProfScope prof(ctx, st, "tile.rot");
+  fs_unrotate_kernel<<<dim3(ceil_div(fs->cap, 256), B), 256, 0, st>>>(fs_layout(fs), d_items);
   DIMB_LAUNCH_CHECK(ctx);
   return DIMB_OK;
 }

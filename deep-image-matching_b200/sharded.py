@@ -123,6 +123,25 @@ def gather_pair_counts(local_ids, local_counts, n_pairs: int, dist=None, device=
     return [int(a[0, 0]) for a in full]
 
 
+def upright_waves(pairs, n_images: int, count, dist=None, device=None):
+    """The upright search over the ranks, wave by wave (``upright.upright_schedule``): each wave's decisions are dealt round-robin
+    (``shard_pairs``), ``count(my decisions, rotations so far)`` gives the four counts (rotations 0, 90, 180, 270) of each of this rank's
+    decisions in order, and one ``gather_pair_counts`` (four ids per decision) gives every rank the wave's counts and so its
+    rotations.  Returns (rotations, {(target, reference): [c_0, c_90, c_180, c_270]}), the same on every rank."""
+    from .upright import choose, upright_schedule
+    world = dist.get_world_size() if dist is not None and dist.is_initialized() else 1
+    rank = dist.get_rank() if world > 1 else 0
+    rotations, counts = [0] * n_images, {}
+    for wave in upright_schedule(pairs, n_images):
+        mine = shard_pairs(len(wave), world, rank)
+        local = np.asarray(count([wave[q] for q in mine], list(rotations)), np.int64).reshape(-1)
+        full = gather_pair_counts([4 * q + r for q in mine for r in range(4)], local, 4 * len(wave), dist if world > 1 else None, device)
+        for q, (t, a) in enumerate(wave):
+            counts[(t, a)] = full[4 * q:4 * q + 4]
+            rotations[t] = choose(counts[(t, a)])
+    return rotations, counts
+
+
 def gather_verified(local_ids, local_results, n_pairs: int, dist=None, device=None):
     """Gather {pair id -> (raw (S,2), verified (V,2), F (3,3) float32 or None, n_inliers)} from all ranks to rank 0: the two int64
     tables, and F and the count as one fixed-width float64 row per pair (exact for float32 and int32).
@@ -277,6 +296,27 @@ def pair_generation_conf(pair_generation) -> dict | None:
     return out
 
 
+UPRIGHT_KEYS = ("max_keypoints", "resize_max")
+
+
+def upright_conf(upright) -> dict | None:
+    """The ``upright`` argument of ImageSetMatcher, validated (None stays None): ``resize_max`` (required int >= 1, the longest side of
+    the search images; no default, as none is pinned) and ``max_keypoints`` (int >= 1, default 2048, the search SuperPoint's cap:
+    the plugin default -1, no cap, has no device buffer)."""
+    if upright is None:
+        return None
+    unknown = set(upright) - set(UPRIGHT_KEYS)
+    if unknown:
+        raise ValueError(f"unknown upright option(s) {sorted(unknown)}; expected some of {list(UPRIGHT_KEYS)}")
+    if "resize_max" not in upright:
+        raise ValueError("upright needs resize_max")
+    out = {"resize_max": upright["resize_max"], "max_keypoints": upright.get("max_keypoints", 2048)}
+    for key in UPRIGHT_KEYS:
+        if isinstance(out[key], bool) or not isinstance(out[key], int) or out[key] < 1:
+            raise ValueError(f"upright {key} must be an int >= 1, got {out[key]!r}")
+    return out
+
+
 QUALITIES = {"highest": -1, "high": 0, "medium": 1, "low": 2, "lowest": 3}
 
 
@@ -360,9 +400,14 @@ class _LowResSet:
 
     `sizes` holds every image's (H, W): ``scales`` / ``low_sizes`` are each image's scale and (h, w), and for a set of one size
     ``scale`` / ``h`` / ``w`` are those values (None otherwise).  SuperPoint is built for the largest low-resolution height and width,
-    and ``low`` is one flat buffer that each batch views as (k, h, w)."""
+    and ``low`` is one flat buffer that each batch views as (k, h, w).
 
-    def __init__(self, ctx, sp_weights, lg_weights, n_slots, sizes, size, sp_conf, lg_conf, batch_images, batch_pairs, device):
+    With `rotations` (the upright search) every slot holds four entries, 4 * slot + ROTATIONS.index(r): the features of its
+    low-resolution image turned by r (dimb_rot90_dev).  Per batch SuperPoint runs twice, on the 0 / 180 images (h x w) and on the
+    90 / 270 images (w x h), into staging rows that are then copied to their entries; ``low`` holds the four turns of one batch."""
+
+    def __init__(self, ctx, sp_weights, lg_weights, n_slots, sizes, size, sp_conf, lg_conf, batch_images, batch_pairs, device,
+                 rotations=False):
         import torch
 
         from . import _native
@@ -372,15 +417,25 @@ class _LowResSet:
         self.low_sizes = [geom[s][1:] for s in sizes]
         self.scale, self.h, self.w = geom[sizes[0]] if len(geom) == 1 else (None, None, None)
         K = self.K = sp_conf["max_keypoints"]
-        self.sp = _native.SuperPointNet(ctx, sp_weights, max_batch=batch_images, max_height=max(h for _, h, _ in geom.values()),
-                                        max_width=max(w for _, _, w in geom.values()), **sp_conf)
+        self.E = 4 if rotations else 1
+        mh, mw = max(h for _, h, _ in geom.values()), max(w for _, _, w in geom.values())
+        if rotations:
+            mh = mw = max(mh, mw)
+        self.sp = _native.SuperPointNet(ctx, sp_weights, max_batch=batch_images * (2 if rotations else 1), max_height=mh, max_width=mw,
+                                        **sp_conf)
         self.lg = _native.LightGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=K, **lg_conf)
-        self.low = torch.zeros(batch_images * max(h * w for _, h, w in geom.values()), device=device)
-        self.sc = torch.zeros(batch_images, K, device=device)  # written by the extractor, not read
+        self.low = torch.zeros(self.E * batch_images * max(h * w for _, h, w in geom.values()), device=device)
+        self.sc = torch.zeros(self.E * batch_images, K, device=device)  # written by the extractor, not read
+        n_slots *= self.E
         self.kp = torch.zeros(n_slots, K, 2, device=device)
         self.de = torch.zeros(n_slots, 256, K, device=device)
         self.n = torch.zeros(n_slots, dtype=torch.int32, device=device)
         self.size = torch.zeros(n_slots, 2, device=device)
+        if rotations:  # staging rows of one batch's four turns
+            self.st_kp = torch.zeros(4 * batch_images, K, 2, device=device)
+            self.st_de = torch.zeros(4 * batch_images, 256, K, device=device)
+            self.st_n = torch.zeros(4 * batch_images, dtype=torch.int32, device=device)
+            self.st_size = torch.zeros(4 * batch_images, 2, device=device)
         self.m = torch.zeros(batch_pairs, K, 2, dtype=torch.int64, device=device)
         self.ms = torch.zeros(batch_pairs, K, device=device)
         self.nm = torch.zeros(batch_pairs, dtype=torch.int32, device=device)
@@ -399,6 +454,8 @@ class _LowResSet:
         K, ss = self.K, slots
         low = self.low[:len(ss) * h * w].view(len(ss), h, w)
         resize(images.data_ptr(), len(ss), H, W, low.data_ptr(), h, w, st)
+        if self.E == 4:
+            return self._extract_turns(low, ss, st)
         k = 0
         while k < len(ss):  # the extractor writes consecutive rows: one call per run of consecutive slots
             e = k + 1
@@ -409,6 +466,25 @@ class _LowResSet:
                                 self.n[s:].data_ptr(), K, st)
             self.ctx.kpts_extent_dev(e - k, self.kp[s].data_ptr(), K, self.n[s:].data_ptr(), self.size[s].data_ptr(), st)
             k = e
+
+    def _extract_turns(self, low, slots, st):
+        """The four turns of the k resized images `low` (k, h, w): low[0:k] as it is, then 180, 90 and 270 turns in ``self.low`` (the
+        0 / 180 block and the 90 / 270 block each contiguous), SuperPoint once per block into the staging rows, one copy per buffer to
+        the entries 4 * slot + ROTATIONS.index(r)."""
+        from .upright import ROTATIONS
+        K = self.K
+        k, h, w = low.shape
+        turns = (0, 180, 90, 270)  # staging order: rows [j * k, (j + 1) * k) hold turn turns[j]
+        for j, r in enumerate(turns[1:], 1):
+            self.ctx.rot90_dev(low.data_ptr(), k, h, w, 1, [r] * k, self.low[j * k * h * w:].data_ptr(), st)
+        for j0, (bh, bw) in ((0, (h, w)), (2, (w, h))):
+            rows = slice(j0 * k, (j0 + 2) * k)
+            self.sp.extract_dev(self.low[j0 * k * h * w:].data_ptr(), 2 * k, bh, bw, self.st_kp[rows].data_ptr(), self.sc.data_ptr(),
+                                self.st_de[rows].data_ptr(), self.st_n[rows].data_ptr(), K, st)
+            self.ctx.kpts_extent_dev(2 * k, self.st_kp[rows].data_ptr(), K, self.st_n[rows].data_ptr(), self.st_size[rows].data_ptr(), st)
+        idx = self.n.new_tensor([4 * s + ROTATIONS.index(r) for r in turns for s in slots]).long()
+        for dst, src in ((self.kp, self.st_kp), (self.de, self.st_de), (self.n, self.st_n), (self.size, self.st_size)):
+            dst.index_copy_(0, idx, src[:4 * k])
 
     def feats(self, slot):
         """The float32 features of a slot as LightGlue input, normalised by their own extent."""
@@ -500,12 +576,26 @@ class ImageSetMatcher:
     of the set.  Per-image values: ``sizes``, ``ext_sizes`` (after quality), ``tile_counts`` and ``view_offsets``, and ``scales`` /
     ``low_sizes`` of the low-resolution sets; for a set of one size ``H`` / ``W`` / ``h2`` / ``w2`` / ``T`` / ``G`` / ``pre_h`` /
     ``pre_w`` hold that size's values, for a mixed set they are None.  A set given as lists of equal sizes is a set of one size: the
-    same launches and outputs as the int form."""
+    same launches and outputs as the int form.
+
+    ``upright``: None (default) or a dict checked by ``upright_conf`` (``resize_max`` required, ``max_keypoints`` default 2048), the
+    reference's upright option with the rules of ``upright.py``.  ``upright`` searches each image's rotation over the pair list
+    (``rotations``, the same on every rank), ``extract`` then extracts the rotated images, ``match`` / ``match_verified`` match in the
+    rotated frames (F mapped back to original pixels by ``upright.rotate_back_F``), and ``rotate_back`` puts the stored keypoints and
+    ``image_size`` back on the original images, after which matching is refused until the next ``extract``; ``run`` /
+    ``run_verified`` / ``run_lowres`` chain the steps (``run_lowres`` searches over the kept pairs), and ``export_colmap`` writes
+    original-frame keypoints and camera sizes.  ``tile_idx`` keeps the rotated image's tile indices.  ``upright_weights``: the
+    search's SuperPoint-LightGlue weights (default ``lg_weights``; required with SuperGlue and kornia_matcher).  Refused: ALIKED, tile
+    preselection, and explicit ``tile_pairs``.  Every per-size rule is checked for both orientations of every image, and the extractor
+    workspace, the store and the tile views are sized for both, since the rotations are unknown at construction (a set of 1536 x 2048
+    images gets a 2048 x 2048 workspace); the search holds four float32 feature entries per image (about 8.5 MB at 2048 keypoints)
+    on every rank, and ``extract`` one rotated batch of batch_images full-size images at a time."""
 
     def __init__(self, ctx, sp_weights: dict, lg_weights: dict, n_images: int, height, width, sp_conf: dict, lg_conf: dict,
                  batch_images: int = 16, batch_pairs: int = 32, dist=None, matcher: str = "lightglue", verification: dict | None = None,
                  tiling: dict | None = None, extractor: str = "superpoint", preselection_weights: dict | None = None,
-                 pair_generation: dict | None = None, lowres_weights: dict | None = None, quality: str = "high"):
+                 pair_generation: dict | None = None, lowres_weights: dict | None = None, quality: str = "high", upright: dict | None = None,
+                 upright_weights: dict | None = None):
         import torch
 
         from . import _native
@@ -518,8 +608,20 @@ class ImageSetMatcher:
         self.nn_conf = kornia_conf(lg_conf) if matcher == "kornia_matcher" else None
         self.tiling = tiling_conf(tiling)
         self.sizes = image_sizes(n_images, height, width)
-        shapes = list(dict.fromkeys(self.sizes))  # the distinct sizes: every per-size rule is checked once per size
+        self.up = upright_conf(upright)
+        # the distinct sizes: every per-size rule is checked once per size; with upright for both orientations of every image
+        shapes = list(dict.fromkeys(self.sizes + ([(w, h) for h, w in self.sizes] if self.up else [])))
         self.presel = self.tiling is not None and self.tiling["tile_selection"] == "preselection"
+        if self.up is not None:
+            if extractor == "aliked":
+                raise ValueError("upright searches with SuperPoint on gray images and is available with extractor=\"superpoint\" only")
+            if self.presel:
+                raise ValueError("upright with tile_selection \"preselection\" is not supported; use grid or exhaustive tile selection")
+            if matcher != "lightglue" and upright_weights is None:
+                raise ValueError(f"upright with matcher=\"{matcher}\" needs upright_weights (SuperPoint-LightGlue weights)")
+            for H, W in shapes:
+                if min(_lowres_size(H, W, self.up["resize_max"])[1:]) < 1:
+                    raise ValueError(f"upright resize_max {self.up['resize_max']} down-samples a {H}x{W} image to nothing")
         if self.presel:
             if extractor == "aliked":
                 raise ValueError("tile preselection runs on gray images and is available with extractor=\"superpoint\" only; "
@@ -555,15 +657,16 @@ class ImageSetMatcher:
                 if min(_lowres_size(H, W, self.pairgen["resize_max"])[1:]) < 1:
                     raise ValueError(f"resize_max {self.pairgen['resize_max']} down-samples a {H}x{W} image to nothing")
         uniform = len(shapes) == 1
-        self.ext_sizes = [ext[s] for s in self.sizes]
+        self._ext = ext
         # one size: the int attributes of that size; a mixed set has None there, and the per-image lists above and below
         self.H, self.W = shapes[0] if uniform else (None, None)
         self.h2, self.w2 = ext[shapes[0]] if uniform else (None, None)
         self.grid = self.T = self.G = None
+        self._grids = grids = None
         if self.tiling is not None:
-            grids = {s: _native.tile_grid(*ext[s], *self.tiling["tile_hw"], *self.tiling["overlap_hw"]) for s in shapes}
-            self.tile_counts = [len(grids[s]["origins"]) for s in self.sizes]
-            self.view_offsets = [int(v) for v in np.cumsum([0] + self.tile_counts[:-1])]
+            self._grids = grids = {s: _native.tile_grid(*ext[s], *self.tiling["tile_hw"], *self.tiling["overlap_hw"]) for s in shapes}
+        self._set_frames(self.sizes)
+        if self.tiling is not None:
             if uniform:
                 self.grid, self.T = grids[shapes[0]], self.tile_counts[0]
                 self.G = max(1, batch_images // self.T)
@@ -601,7 +704,7 @@ class ImageSetMatcher:
         elif matcher == "lightglue":
             self.lg = _native.LightGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=self.cap, **lg_conf)
         self.ipr = images_per_rank(n_images, self.world)
-        t_max = 1 if self.tiling is None else max(self.tile_counts)
+        t_max = 1 if self.tiling is None else max(len(g["origins"]) for g in grids.values())
         self.store = _native.FeatureStoreDev(ctx, self.world * self.ipr, t_max * self.cap, self.D)
         dev = torch.device("cuda", ctx.device)
         # extraction outputs of one batch (float32, library layouts) and match outputs of one pair batch; tiled: the tiles of the
@@ -626,8 +729,10 @@ class ImageSetMatcher:
         if self.tiling is not None:
             # per-tile views of every image (slot view_offsets[i] + t) with their row maps, and the merged tables of one batch: an image
             # pair has at most min(batch_pairs, T0 * T1) distinct tile pairs of at most K rows each, so cap2 holds every merged table whole
-            self.views = _native.FeatureStoreDev(ctx, sum(self.tile_counts), self.cap, self.D)
-            self.vmap = torch.zeros(sum(self.tile_counts), self.views.cap, dtype=torch.int32, device=dev)
+            # (upright: room for each image's larger grid of its two orientations)
+            n_views = sum(max(len(grids[s]["origins"]), len(grids[s[::-1]]["origins"]) if self.up else 0) for s in self.sizes)
+            self.views = _native.FeatureStoreDev(ctx, n_views, self.cap, self.D)
+            self.vmap = torch.zeros(n_views, self.views.cap, dtype=torch.int32, device=dev)
             self.cap2 = gv_cap = min(batch_pairs, t_max * t_max) * self.cap
             self.mm = torch.zeros(batch_pairs, self.cap2, 2, dtype=torch.int64, device=dev)
             self.nmm = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
@@ -646,6 +751,17 @@ class ImageSetMatcher:
             from .pairs_generator import LG_LOWRES_CONF, SP_LOWRES_CONF
             self.lowres = _LowResSet(ctx, sp_weights, lg_weights if lowres_weights is None else lowres_weights, self.world * self.ipr,
                                      self.sizes, self.pairgen["resize_max"], SP_LOWRES_CONF, LG_LOWRES_CONF, batch_images, batch_pairs, dev)
+        self.search = self.rotations = None
+        self._turned_back = False
+        if self.up is not None:
+            # find_matches_per_rotation (image_matching.py:69-118) with the plugins' default networks; fixed descriptor sampling when
+            # tiling or pair generation is configured (quirk A.6), otherwise sp_conf's
+            from .upright import LG_UPRIGHT_CONF, SP_UPRIGHT_CONF
+            fix = self.tiling is not None or self.pairgen is not None or bool(sp_conf.get("fix_sampling", False))
+            self.search = _LowResSet(ctx, sp_weights, lg_weights if upright_weights is None else upright_weights, self.world * self.ipr,
+                                     self.sizes, self.up["resize_max"], {**SP_UPRIGHT_CONF, "max_keypoints": self.up["max_keypoints"],
+                                                                         "fix_sampling": fix},
+                                     LG_UPRIGHT_CONF, batch_images, batch_pairs, dev, rotations=True)
         self.gv = verification_conf(verification)
         if self.gv is not None and self.gv["method"] != "NONE":  # verification outputs of one pair batch
             self.v = torch.zeros(batch_pairs, gv_cap, 2, dtype=torch.int64, device=dev)
@@ -667,8 +783,18 @@ class ImageSetMatcher:
         order.  Images are processed in groups of one size (image order kept inside a group), each group batched as a set of that
         size; a shape that is not its image's declared size raises ValueError before any launch.  With tiling the images are full
         size and are cut into tiles on the device.  A list is copied into one staging tensor per batch of batch_images, which feeds
-        the low-resolution sets and (untiled) the extractor; tiled extraction stages again per cut, whose size differs."""
+        the low-resolution sets and (untiled) the extractor; tiled extraction stages again per cut, whose size differs.
+
+        With upright the images are the unrotated ones, ``upright`` must have run (RuntimeError otherwise), and each staged batch is
+        first turned by its images' rotations at full size (dimb_rot90_dev, one launch per batch into one buffer of the batch,
+        ``_extract_turned``); everything else (quality, tile cut, extractor, by rotated size) runs on the rotated images.  The
+        low-resolution sets were filled by ``upright`` from the unrotated images."""
         st = self.torch.cuda.current_stream().cuda_stream
+        if self.up is not None:
+            if self.rotations is None:
+                raise RuntimeError("ImageSetMatcher was built with upright: run upright() before extract()")
+            self._turned_back = False
+            return self._extract_turned(d_images, image_ids, st)
         groups = self._groups(d_images, image_ids)
         lows = [low for low in (self.pre, self.lowres) if low is not None]
         if self.tiling is not None:
@@ -678,16 +804,49 @@ class ImageSetMatcher:
                         low.extract(src, ids, [self.slots[i] for i in ids], st)
             return self._extract_tiled(d_images, image_ids, groups, st)
         for (H, W), ids, src in self._batches(d_images, image_ids, groups, self.B):
-            slots = [self.slots[i] for i in ids]
             for low in lows:
-                low.extract(src, ids, slots, st)
-            h2, w2 = self.ext_sizes[ids[0]]
-            src = self._resize(src, h2, w2, st)
-            self._extract_rows(src, h2, w2, st)
-            for k, s in enumerate(slots):
-                self.store.put_dev(s, self.kp[k].data_ptr(), self.sc[k].data_ptr(), self.de[k].data_ptr(), self.cap, self.cnt[k:k + 1].data_ptr(),
-                                   h2, w2, None, st)
-            self._rescale(slots, H, W, st)
+                low.extract(src, ids, [self.slots[i] for i in ids], st)
+            self._extract_batch(src, ids, H, W, st)
+
+    def _extract_batch(self, src, ids, H, W, st):
+        """Untiled extraction of the H x W images `src` (at most batch_images) of images `ids` into their slots: quality's resize, the
+        extractor, put_dev, quality's rescale."""
+        slots = [self.slots[i] for i in ids]
+        h2, w2 = self.ext_sizes[ids[0]]
+        src = self._resize(src, h2, w2, st)
+        self._extract_rows(src, h2, w2, st)
+        for k, s in enumerate(slots):
+            self.store.put_dev(s, self.kp[k].data_ptr(), self.sc[k].data_ptr(), self.de[k].data_ptr(), self.cap, self.cnt[k:k + 1].data_ptr(),
+                               h2, w2, None, st)
+        self._rescale(slots, H, W, st)
+
+    def _extract_turned(self, d_images, image_ids, st):
+        """Upright extraction: per original size, the images whose frame keeps that size (0, 180) come before those it swaps (90, 270),
+        then batches of batch_images are staged (a view for consecutive rows of one tensor) and turned by one dimb_rot90_dev launch
+        into one buffer of the batch, which therefore holds at most two runs of one frame size; each run goes to the extraction of a
+        batch (untiled) or of cuts of its tile grid (tiled) as it is, without another copy.  Rotation 0 is copied too: one memory-bound
+        pass is cheaper than the extra extractor call a third run would cost."""
+        torch, C = self.torch, self.C
+        px = (3,) if C == 3 else ()
+        for (H, W), ks in self._groups(d_images, image_ids, self.sizes):
+            ks = sorted(ks, key=lambda k: self.rotations[image_ids[k]] in (90, 270))  # stable: image order kept in each run
+            for b0 in range(0, len(ks), self.B):
+                part = ks[b0:b0 + self.B]
+                ids = [image_ids[k] for k in part]
+                buf = torch.empty(len(part) * H * W * C, device=self.kp.device)
+                self.ctx.rot90_dev(self._stage(d_images, part).data_ptr(), len(part), H, W, C, [self.rotations[i] for i in ids],
+                                   buf.data_ptr(), st)
+                n0 = sum(self.rotations[i] in (0, 180) for i in ids)
+                for a, b, (h, w) in ((0, n0, (H, W)), (n0, len(ids), (W, H))):
+                    if a == b:
+                        continue
+                    run = buf[a * H * W * C:b * H * W * C].view((b - a, h, w) + px)
+                    if self.tiling is None:
+                        self._extract_batch(run, ids[a:b], h, w, st)
+                        continue
+                    G = max(1, self.B // self.tile_counts[ids[a]])
+                    for g0 in range(0, b - a, G):
+                        self._extract_cut(run[g0:g0 + G], ids[a + g0:a + g0 + G], h, w, st)
 
     def _batches(self, d_images, image_ids, groups, per):
         """Per size group, its batches of at most `per` images in order: ((H, W), their image ids, the images staged as one tensor)."""
@@ -695,18 +854,28 @@ class ImageSetMatcher:
             for b0 in range(0, len(ks), per):
                 yield size, [image_ids[k] for k in ks[b0:b0 + per]], self._stage(d_images, ks[b0:b0 + per])
 
-    def _groups(self, d_images, image_ids):
+    def _set_frames(self, frames):
+        """The per-image sizes extraction sees, `frames` (the declared sizes, or with upright the rotated ones), and what follows from
+        them: ``ext_sizes`` after quality, and with tiling ``tile_counts`` and ``view_offsets``."""
+        self.frames = list(frames)
+        self.ext_sizes = [self._ext[s] for s in self.frames]
+        if self.tiling is not None:
+            self.tile_counts = [len(self._grids[s]["origins"]) for s in self.frames]
+            self.view_offsets = [int(v) for v in np.cumsum([0] + self.tile_counts[:-1])]
+
+    def _groups(self, d_images, image_ids, sizes=None):
         """This rank's images grouped by size: [((H, W), positions in image_ids)] (``_by_size``), after checking every image's shape
-        against its declared size."""
+        against its size in `sizes` (default: ``frames``, the declared sizes unless upright has rotated them)."""
+        sizes = self.frames if sizes is None else sizes
         listed = isinstance(d_images, (list, tuple))
         if (len(d_images) != len(image_ids)) if listed else (d_images.dim() < 3 or len(d_images) < len(image_ids)):
             raise ValueError(f"extract needs one image per image id: {len(d_images)} images for {len(image_ids)} ids")
         for k, i in enumerate(image_ids):
-            want = self.sizes[i] + ((3,) if self.C == 3 else ())
+            want = sizes[i] + ((3,) if self.C == 3 else ())
             got = tuple(d_images[k].shape) if listed else tuple(d_images.shape[1:1 + len(want)])
             if got != want or (listed and (d_images[k].dtype != self.torch.float32 or not d_images[k].is_cuda)):
                 raise ValueError(f"image {i} must be a float32 CUDA tensor of shape {want} (its declared size), got {tuple(d_images[k].shape)}")
-        return _by_size([self.sizes[i] for i in image_ids], range(len(image_ids)))
+        return _by_size([sizes[i] for i in image_ids], range(len(image_ids)))
 
     def _stage(self, d_images, ks):
         """The images at positions `ks` of `d_images` as one contiguous (len(ks), H, W[, 3]) tensor: a view when they are consecutive
@@ -745,38 +914,50 @@ class ImageSetMatcher:
     def _extract_tiled(self, d_images, image_ids, groups, st):
         """Per size group (its own grid of T tiles), cuts of G = max(1, batch_images // T) images: tile cut, the extractor over their
         G * T tiles, one tile merge into their slots."""
-        (th, tw), (oh, ow) = self.tiling["tile_hw"], self.tiling["overlap_hw"]
         for (H, W), ks in groups:
-            first = image_ids[ks[0]]
-            (h2, w2), T = self.ext_sizes[first], self.tile_counts[first]
-            G = max(1, self.B // T)
+            G = max(1, self.B // self.tile_counts[image_ids[ks[0]]])
             for g0 in range(0, len(ks), G):
-                ids = [image_ids[k] for k in ks[g0:g0 + G]]
-                src = self._resize(self._stage(d_images, ks[g0:g0 + G]), h2, w2, st)
-                self.ctx.tile_cut_dev(src.data_ptr(), len(ids), h2, w2, self.C, th, tw, oh, ow, self.tiles.data_ptr(), st)
-                self._extract_rows(self.tiles[:len(ids) * T], th, tw, st)
-                slots = [self.slots[i] for i in ids]
-                self.store.tile_merge_dev(slots, h2, w2, th, tw, oh, ow, self.kp.data_ptr(), self.sc.data_ptr(), self.de.data_ptr(),
-                                          self.cnt.data_ptr(), self.cap, st)
-                self._rescale(slots, H, W, st)
+                self._extract_cut(self._stage(d_images, ks[g0:g0 + G]), [image_ids[k] for k in ks[g0:g0 + G]], H, W, st)
+
+    def _extract_cut(self, src, ids, H, W, st):
+        """One cut of the H x W images `src` (at most G of them) of images `ids`: quality's resize, tile cut, the extractor over their
+        tiles, one tile merge into their slots, quality's rescale."""
+        (th, tw), (oh, ow) = self.tiling["tile_hw"], self.tiling["overlap_hw"]
+        (h2, w2), T = self.ext_sizes[ids[0]], self.tile_counts[ids[0]]
+        src = self._resize(src, h2, w2, st)
+        self.ctx.tile_cut_dev(src.data_ptr(), len(ids), h2, w2, self.C, th, tw, oh, ow, self.tiles.data_ptr(), st)
+        self._extract_rows(self.tiles[:len(ids) * T], th, tw, st)
+        slots = [self.slots[i] for i in ids]
+        self.store.tile_merge_dev(slots, h2, w2, th, tw, oh, ow, self.kp.data_ptr(), self.sc.data_ptr(), self.de.data_ptr(),
+                                  self.cnt.data_ptr(), self.cap, st)
+        self._rescale(slots, H, W, st)
 
     def exchange(self):
         """The collective of the path: every rank's float16 feature blocks to every rank (NCCL all_gather over NVLink).  With tiling,
-        every rank then builds the per-tile views of all images from the merged slots."""
+        every rank then builds the per-tile views of all images from the merged slots.  With upright the low-resolution sets were
+        exchanged by ``upright``."""
         self.exchanged_bytes = all_gather_blocks(self.store_t, self.n, self.dist)
-        for low in (self.pre, self.lowres):  # the low-resolution features of every image, for any pair
-            if low is not None:
-                for t in low.buffers:
-                    self.exchanged_bytes += all_gather_blocks(t.view(self.torch.uint8).view(t.shape[0], -1), self.n, self.dist)
+        if self.up is None:
+            self.exchanged_bytes += self._exchange_lows((self.pre, self.lowres))
         if self.tiling is not None:
             st = self.torch.cuda.current_stream().cuda_stream
-            for _, images in _by_size(self.sizes, range(self.n)):
+            for _, images in _by_size(self.frames, range(self.n)):
                 T = self.tile_counts[images[0]]
                 step = max(1, 65535 // T)
                 for b0 in range(0, len(images), step):
                     ids = images[b0:b0 + step]
                     self.store.tile_views_dev([self.slots[i] for i in ids], T, self.views, [self.view_offsets[i] for i in ids],
                                               self.vmap.data_ptr(), st)
+
+    def _exchange_lows(self, lows) -> int:
+        """The low-resolution features of every image, for any pair: one all_gather per buffer of each set in `lows` (None skipped; a
+        slot's four search entries travel together).  Returns the bytes received."""
+        received = 0
+        for low in lows:
+            if low is not None:
+                for t in low.buffers:
+                    received += all_gather_blocks(t.view(self.torch.uint8).view(t.shape[0] // low.E, -1), self.n, self.dist)
+        return received
 
     def _match_slots(self, store, s0, s1, st):
         """Enqueue the matcher on slot pairs (s0[k], s1[k]) of `store` (outputs in self.m / self.ms / self.nm)."""
@@ -866,6 +1047,11 @@ class ImageSetMatcher:
         from .geometric_verification import gv_seed
         if self.tiling is None and tile_pairs is not None:
             raise ValueError("tile_pairs needs an ImageSetMatcher built with tiling")
+        if self.up is not None:
+            if tile_pairs is not None:
+                raise ValueError("explicit tile_pairs cannot be used with upright: the tile grids depend on the rotations the search picks")
+            if self._turned_back:
+                raise RuntimeError("the keypoints were rotated back (rotate_back); matching runs in the rotated frames, before it")
         stream = self.torch.cuda.current_stream()
         lists = None if self.tiling is None else self._tile_pair_lists(pairs, tile_pairs)
         g, out = self.gv, {}
@@ -882,8 +1068,12 @@ class ImageSetMatcher:
                                        g["max_iters"], g["min_inliers_per_pair"], g["min_inlier_ratio_per_pair"], self.v.data_ptr(),
                                        self.nv.data_ptr(), self.F.data_ptr(), self.mask.data_ptr(), self.ninl.data_ptr(), stream.cuda_stream)
                 (raw, ver), (F, ninl) = self._read_back([(m, nm, cap), (self.v, self.nv, cap)], (self.F, self.ninl), e - s, stream)
-                for k, i in enumerate(ids):
-                    out[i] = (raw[k], ver[k], F[k].reshape(3, 3).copy() if np.any(F[k]) else None, int(ninl[k]))
+                for k, (i, (a, b)) in enumerate(zip(ids, chunk)):
+                    Fk = F[k].reshape(3, 3).copy() if np.any(F[k]) else None
+                    if self.up is not None:  # F of the rotated frames -> original pixels
+                        from .upright import rotate_back_F
+                        Fk = rotate_back_F(Fk, self.rotations[a], self.sizes[a], self.rotations[b], self.sizes[b])
+                    out[i] = (raw[k], ver[k], Fk, int(ninl[k]))
         return out
 
     def match(self, pairs, pair_ids, tile_pairs=None):
@@ -934,14 +1124,91 @@ class ImageSetMatcher:
         pairs -> gather to rank 0.  Returns (pairs, counts, results): the kept pairs and every brute-force pair's count on every rank,
         and on rank 0 the results per kept pair as ``run`` / ``run_verified`` return them (None elsewhere).  With tiling, the configured
         tile selection applies to the kept pairs."""
+        match, gather = (self.match_verified, gather_verified) if verified else (self.match, gather_match_tables)
+        if self.up is not None:  # pair generation reads the unrotated images, and the search runs over the kept pairs
+            self._search_extract(d_images, my_image_ids)
+            pairs, counts = self.lowres_pairs()
+            self._search(pairs)
+            self.extract(d_images, my_image_ids)
+            self.exchange()
+            return pairs, counts, self._match_share(match, gather, pairs, None, None)
         self.extract(d_images, my_image_ids)
         self.exchange()
         pairs, counts = self.lowres_pairs()
-        match, gather = (self.match_verified, gather_verified) if verified else (self.match, gather_match_tables)
         return pairs, counts, self._match_share(match, gather, pairs, None, None)
 
+    def upright(self, d_images, my_image_ids, pairs):
+        """The upright search (find_matches_per_rotation, image_matching.py:69-118) over `pairs`, the schedule and rules of
+        ``upright.upright_schedule`` / ``upright.upright_rotations``.  `d_images`: this rank's unrotated images, as ``extract`` takes them.
+
+        Each rank resizes its images once (INTER_AREA, longest side ``resize_max``), turns each low-resolution image three ways
+        (dimb_rot90_dev) and runs SuperPoint on all four turns (two calls per batch, one per shape) into four float32 entries per slot;
+        the entries of every image then go to every rank (all_gather of about (256 + 2) * 4 * K * 4 bytes, 8.5 MB at K = 2048, per
+        image).  Then wave by wave: the wave's decisions are dealt to the ranks (``shard_pairs``), LightGlue runs on the four entry
+        pairs (reference at its rotation, target at each turn) of every decision in batches of batch_pairs, and one device->host copy
+        of the counts and one ``gather_pair_counts`` give every rank the wave's counts, hence its rotations, which the next wave needs
+        on the host.  So the search costs one host synchronise per wave: one for a brute-force list (everything hangs off image 0), up
+        to n - 1 for a sequential chain.  This path runs SuperPoint 4 times per image, the reference 1 + 4 times per visited pair.
+
+        Returns (rotations, counts), the same on every rank: the rotation of every image in degrees clockwise, and
+        {(target, reference): [c_0, c_90, c_180, c_270]}; sets ``rotations``.  Afterwards ``extract`` takes the same unrotated images."""
+        self._search_extract(d_images, my_image_ids)
+        return self._search(pairs)
+
+    def _search_extract(self, d_images, my_image_ids):
+        """One staging pass over the unrotated images for the low-resolution work (the search entries, and the pair-generation set when
+        configured), then their exchange."""
+        if self.up is None:
+            raise RuntimeError("ImageSetMatcher was built without upright")
+        st = self.torch.cuda.current_stream().cuda_stream
+        lows = [low for low in (self.lowres, self.search) if low is not None]
+        for _, ids, src in self._batches(d_images, my_image_ids, self._groups(d_images, my_image_ids, self.sizes), self.B):
+            for low in lows:
+                low.extract(src, ids, [self.slots[i] for i in ids], st)
+        self.exchanged_bytes = self._exchange_lows(lows)
+
+    def _search(self, pairs):
+        """The waves of ``upright_schedule(pairs)`` on the exchanged search entries (``upright``)."""
+        from .upright import ROTATIONS, rotated_size
+        torch, low = self.torch, self.search
+        st = torch.cuda.current_stream().cuda_stream
+
+        def count(decisions, rotations):  # LightGlue on the four entry pairs of each decision, counts copied on the device
+            e0 = [4 * self.slots[a] + ROTATIONS.index(rotations[a]) for _, a in decisions for _ in ROTATIONS]
+            e1 = [4 * self.slots[t] + r for t, _ in decisions for r in range(4)]
+            got = torch.zeros(max(len(e0), 1), dtype=torch.int32, device=low.nm.device)
+            for b0 in range(0, len(e0), self.P):
+                q = len(e0[b0:b0 + self.P])
+                low.match(e0[b0:b0 + q], e1[b0:b0 + q], st)
+                got[b0:b0 + q].copy_(low.nm[:q])
+            return got[:len(e0)].cpu().numpy()
+        rotations, counts = upright_waves(pairs, self.n, count, self.dist if self.world > 1 else None,
+                                          torch.device("cuda", self.ctx.device) if self.world > 1 else None)
+        self.rotations = rotations
+        self._set_frames([rotated_size(h, w, r) for (h, w), r in zip(self.sizes, rotations)])
+        return rotations, counts
+
+    def rotate_back(self):
+        """Upright, after matching: the keypoints of every slot with a non-zero rotation back on its original image, and the original
+        size in its header (one dimb_fstore_unrotate_dev launch; quality's rescale has already put them in the rotated full-size
+        frame).  ``tile_idx`` keeps the indices of the rotated image's tile grid.  ``match`` / ``match_verified`` refuse to run after it."""
+        if self.up is None or self.rotations is None:
+            raise RuntimeError("rotate_back needs an ImageSetMatcher built with upright, after upright()")
+        if self._turned_back:
+            return
+        turned = [i for i in range(self.n) if self.rotations[i]]
+        if turned:
+            self.store.unrotate_dev([self.slots[i] for i in turned], [self.rotations[i] for i in turned], [self.sizes[i][0] for i in turned],
+                                    [self.sizes[i][1] for i in turned], self.torch.cuda.current_stream().cuda_stream)
+        self._turned_back = True
+
     def _run(self, match, gather, d_images, my_image_ids, pairs, costs, tile_pairs):
-        """extract -> exchange -> `match` on this rank's share of `pairs` -> `gather` to rank 0."""
+        """extract -> exchange -> `match` on this rank's share of `pairs` -> `gather` to rank 0 (upright: the search first, and the
+        keypoints rotated back before the gather)."""
+        if self.up is not None:
+            if tile_pairs is not None:
+                raise ValueError("explicit tile_pairs cannot be used with upright: the tile grids depend on the rotations the search picks")
+            self.upright(d_images, my_image_ids, pairs)
         self.extract(d_images, my_image_ids)
         self.exchange()
         return self._match_share(match, gather, pairs, costs, tile_pairs)
@@ -949,6 +1216,8 @@ class ImageSetMatcher:
     def _match_share(self, match, gather, pairs, costs, tile_pairs):
         mine = shard_pairs(len(pairs), self.world, self.rank, costs)
         res = match([pairs[k] for k in mine], mine, None if tile_pairs is None else [tile_pairs[k] for k in mine])
+        if self.up is not None:
+            self.rotate_back()
         return gather(mine, [res[k] for k in mine], len(pairs), self.dist if self.world > 1 else None,
                       self.torch.device("cuda", self.ctx.device) if self.world > 1 else None)
 

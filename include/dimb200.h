@@ -354,6 +354,23 @@ int dimb_pyr_dev(dimb_ctx* ctx, const float* d_src, int B, int height, int width
  * are left alone.  DIMB_ERR_ARG, before any CUDA call, for a NULL pointer, B outside [1, 65535], a slot out of range, a level outside
  * [-1, 3] or a size below 1.  Asynchronous on `stream`; profile group tile.pyr. */
 int dimb_fstore_rescale_dev(dimb_fstore* fs, int B, const int* slots, int level, int height, int width, void* stream);
+/* upright (image_matching.py:496): cv2.rotate of B float32 images d_src [B][H][W][channels] (channels 1 gray or 3 interleaved RGB) by
+ * rotations[b] (host array, each 0, 90 = ROTATE_90_CLOCKWISE, 180 = ROTATE_180 or 270 = ROTATE_90_COUNTERCLOCKWISE; mixed values in
+ * one call) into d_dst, image b starting at element b * H * W * channels and being [H][W][channels] (0, 180) or [W][H][channels]
+ * (90, 270).  A permutation, so bitwise cv2.rotate.  One host->device copy of the codes (context scratch) and one launch; d_dst must
+ * not overlap d_src.  DIMB_ERR_ARG, before any CUDA call, for a NULL pointer, B outside [1, 65535], other channel counts, a size
+ * outside [1, 2^20] or another rotation value.  Asynchronous on `stream`; profile group tile.rot.  CUDA cores, memory-bound
+ * (2 * B * H * W * channels * 4 bytes). */
+int dimb_rot90_dev(dimb_ctx* ctx, const float* d_src, int B, int height, int width, int channels, const int* rotations, float* d_dst,
+                   void* stream);
+/* upright (image_matching.py:703): the keypoints of B store slots slots[b] (host arrays throughout), extracted from their image turned
+ * by rotations[b] with cv2.rotate, back on pixel indices of the original heights[b] x widths[b] image: in float32, (x', y') ->
+ * 90: (y', H - 1 - x'), 180: (W - 1 - x', H - 1 - y'), 270: (W - 1 - y', x'), 0: unchanged, then rounded to float16; the header's [H, W]
+ * becomes the original size (float16-rounded as dimb_fstore_put_dev stores it).  Scores, descriptors and tile_idx are untouched, and
+ * empty slots are left alone.  DIMB_ERR_ARG, before any CUDA call, for a NULL pointer, B outside [1, 65535], a slot out of range,
+ * another rotation value or a size below 1.  Asynchronous on `stream`; profile group tile.rot. */
+int dimb_fstore_unrotate_dev(dimb_fstore* fs, int B, const int* slots, const int* rotations, const int* heights, const int* widths,
+                             void* stream);
 /* normalize_keypoints' own-extent size for LightGlue without image_size (lightglue.py:26-27): per image b, over its
  * min(d_counts[b], kpt_ld) keypoints of d_kpts [B][kpt_ld][2] float32, d_size_out[b] = {(1 + max x) - min x, (1 + max y) - min y}
  * in float32, as dimb_lg_match computes it on the host; {1, 1} for an image without keypoints.  Feed it to dimb_lg_match_dev
