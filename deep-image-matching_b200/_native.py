@@ -194,7 +194,8 @@ _selftest = None
 
 def load_selftest_library():
     """libdimb200_selftest.so: the production GEMM template behind a C = A B^T entry, the flash-attention kernels behind an
-    attention entry and the host drive of the RANSAC arithmetic.
+    attention entry, keypoint detection (simple_nms, compaction, top-k) and the SuperPoint head kernels behind their own entries, and
+    the host drive of the RANSAC arithmetic.
     Test / tool infrastructure - the product library exports none of it.  Its context is its own (dimb_ctx_create of
     THIS library); never mix handles of the two libraries."""
     global _selftest
@@ -217,6 +218,10 @@ def load_selftest_library():
         lib.dimb_selftest_conv_mode.argtypes = [ip] * 5 + [vp]
         lib.dimb_selftest_conv3x3_time.argtypes = [vp] + [ip] * 9 + [vp, vp]
         lib.dimb_selftest_attention.argtypes = [vp, ip, vp, vp, vp, vp, ip, ip, ip, ip, vp, vp, ip, fp, fp, fp]
+        lib.dimb_selftest_nms_plan.argtypes = [ip, ip, vp]
+        lib.dimb_selftest_detect.argtypes = [vp, vp] + [ip] * 5 + [fp, vp, ip, ip, ip, fp] + [vp] * 8
+        lib.dimb_selftest_sp_softmax.argtypes = [vp, vp, ip, ip, ip, fp, vp]
+        lib.dimb_selftest_sp_describe.argtypes = [vp] * 5 + [ip] * 5 + [fp, vp, vp, vp]
         lib.dimb_gv_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_uint, vp, vp]
         _selftest = lib
     return _selftest
@@ -243,8 +248,22 @@ def conv_mode(cout: int, B: int, H: int, W: int, num_sms: int) -> int:
     return int(out[0])
 
 
+def nms_plan(r: int, cut: int = 0):
+    """Launch plan (kernel, tile, threads, smem_bytes) of simple_nms at radius r (dimb_selftest_nms_plan): kernel 1 = first cut, 2 =
+    bit-mask kernel.  cut 0 = the production choice of a default context, 1 = first cut (radii 0..8), 2 = bit-mask kernel (radii
+    1..5).  Host only."""
+    out = np.zeros(4, np.int32)
+    rc = load_selftest_library().dimb_selftest_nms_plan(int(r), int(cut), _ptr(out))
+    if rc != OK:
+        raise DimbError(f"nms_plan({r}, {cut}) failed (code {rc})")
+    return tuple(int(p) for p in out)
+
+
+DET_TAIL = 1024  # elements past the valid ones in every output buffer of the detection / head self-tests
+
+
 class SelfTest:
-    """Context of the self-test library (tests/test_gemm_conv_kernel.py, tests/test_attention_kernel.py)."""
+    """Context of the self-test library (tests/test_gemm_conv_kernel.py, tests/test_attention_kernel.py, tests/test_detect_kernel.py)."""
 
     def __init__(self, device: int = 0):
         self.lib = load_selftest_library()
@@ -333,6 +352,57 @@ class SelfTest:
         self.check(self.lib.dimb_selftest_attention(self.h, int(variant), _ptr(Q), _ptr(K) if K is not None else None, _ptr(V), _ptr(out),
                                                     S, H, hd, NP, _ptr(nn), _ptr(st), int(bool(cross)), float(lazy), float(pad),
                                                     float(out_pad)), "selftest_attention")
+        return out
+
+    def detect(self, scores: np.ndarray, r: int, cut: int = 0, thr: float = 0.0, thr_per_image=None, border: int = 0, K: int = -1,
+               cap: int | None = None, sentinel: float = -777.0) -> dict:
+        """simple_nms, candidate compaction and top-k through their production launches (dimb_selftest_detect).  scores [B][H][W]
+        positive; cut as nms_plan() except that 0 follows the context (DIMB_NMS); candidates are nms > thr (thr_per_image [B]: through
+        the device-threshold argument) at least `border` pixels inside; K = -1 keeps every candidate; cap defaults to K (H * W when
+        K = -1).  Every buffer starts as `sentinel` (int buffers: its bit pattern).  Returns a dict of nms [B][H][W], cand_count [B],
+        cand_idx / cand_score [B][H * W], sel_idx / sel_score [B][cap], sel_count [B], '<name>_tail' [DET_TAIL] for each, and plan."""
+        s = np.ascontiguousarray(scores, np.float32)
+        B, H, W = s.shape
+        cap = int(cap if cap is not None else (K if K > 0 else H * W))
+        tp = None if thr_per_image is None else np.ascontiguousarray(thr_per_image, np.float32)
+        n, ns = B * H * W, B * cap
+        bufs = {"nms": (np.float32, n), "cand_count": (np.int32, B), "cand_idx": (np.int32, n), "cand_score": (np.float32, n),
+                "sel_idx": (np.int32, ns), "sel_score": (np.float32, ns), "sel_count": (np.int32, B)}
+        raw = {k: np.zeros(m + DET_TAIL, t) for k, (t, m) in bufs.items()}
+        plan = np.zeros(4, np.int32)
+        self.check(self.lib.dimb_selftest_detect(self.h, _ptr(s), B, H, W, int(r), int(cut), float(thr), None if tp is None else _ptr(tp),
+                                                 int(border), int(K), cap, float(sentinel), *(_ptr(raw[k]) for k in bufs), _ptr(plan)),
+                   "selftest_detect")
+        shapes = {"nms": (B, H, W), "cand_idx": (B, H * W), "cand_score": (B, H * W), "sel_idx": (B, cap), "sel_score": (B, cap)}
+        out = {k: raw[k][:m].reshape(shapes.get(k, (B,))) for k, (_, m) in bufs.items()}
+        out.update({k + "_tail": raw[k][m:] for k, (_, m) in bufs.items()})
+        out["plan"] = tuple(int(p) for p in plan)
+        return out
+
+    def sp_softmax(self, logits: np.ndarray, B: int, h: int, w: int, sentinel: float = -777.0):
+        """sp_softmax_d2s_kernel through its production launch (dimb_selftest_sp_softmax): logits [B * h * w][65] -> (scores
+        [B][8h][8w], tail [DET_TAIL] of the output buffer, which starts as `sentinel`)."""
+        lg = np.ascontiguousarray(logits, np.float32)
+        out = np.zeros(B * h * w * 64 + DET_TAIL, np.float32)
+        self.check(self.lib.dimb_selftest_sp_softmax(self.h, _ptr(lg), B, h, w, float(sentinel), _ptr(out)), "selftest_sp_softmax")
+        return out[:-DET_TAIL].reshape(B, 8 * h, 8 * w), out[-DET_TAIL:]
+
+    def sp_describe(self, sel_idx: np.ndarray, sel_score: np.ndarray, sel_count, dense: np.ndarray, h: int, w: int, fix_sampling: bool,
+                    sentinel: float = -777.0) -> dict:
+        """sp_describe_kernel through its production launch (dimb_selftest_sp_describe).  sel_idx / sel_score [B][cap], sel_count [B],
+        dense [B][h * w][256].  Returns kpts [B][cap][2], scores [B][cap], desc [B][256][cap] and '<name>_tail' [DET_TAIL] of each
+        buffer; every buffer starts as `sentinel`."""
+        si = np.ascontiguousarray(sel_idx, np.int32)
+        ss = np.ascontiguousarray(sel_score, np.float32)
+        sc = np.ascontiguousarray(sel_count, np.int32)
+        d = np.ascontiguousarray(dense, np.float32)
+        B, cap = si.shape
+        shapes = {"kpts": (B, cap, 2), "scores": (B, cap), "desc": (B, 256, cap)}
+        raw = {k: np.zeros(int(np.prod(s)) + DET_TAIL, np.float32) for k, s in shapes.items()}
+        self.check(self.lib.dimb_selftest_sp_describe(self.h, _ptr(si), _ptr(ss), _ptr(sc), _ptr(d), B, h, w, cap, int(bool(fix_sampling)),
+                                                      float(sentinel), *(_ptr(raw[k]) for k in shapes)), "selftest_sp_describe")
+        out = {k: raw[k][:-DET_TAIL].reshape(s) for k, s in shapes.items()}
+        out.update({k + "_tail": raw[k][-DET_TAIL:] for k in shapes})
         return out
 
     def __del__(self):

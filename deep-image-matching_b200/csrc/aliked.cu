@@ -898,24 +898,16 @@ int dimb_aliked_extract_dev(dimb_aliked* al, const float* image, int H, int W, i
     DIMB_LAUNCH_CHECK(ctx);
   }
   const int r = cf.nms_radius;
-  const int nch = ceil_div(H * W, kChunk);
   {
   ProfScope prof(ctx, st, "al.detect");
-  DIMB_TRY(launch_nms(ctx, st, al->score, al->nms, 1, H, W, r));
+  DIMB_TRY(launch_nms(ctx, st, al->score, al->nms, 1, H, W, r, ctx->nms_ver));
   // threshold mode (aliked.py:152-160): nms > detection_threshold; if nothing passes, nms > mean(score_map).
   // Decided on the device: count, then al_threshold_kernel fixes the threshold, then count / scan / compact with it.
-  sp_count_kernel<<<dim3(nch, 1), 256, 0, st>>>(al->nms, al->chunk_count, H, W, cf.detection_threshold, r, nch, nullptr);
-  DIMB_LAUNCH_CHECK(ctx);
-  sp_scan_kernel<<<1, 32, 0, st>>>(al->chunk_count, al->chunk_off, al->cand_count, nch);
-  DIMB_LAUNCH_CHECK(ctx);
+  const CandBufs cand{al->chunk_count, al->chunk_off, al->cand_count, al->cand_idx, al->cand_score};
+  DIMB_TRY(launch_candidates(ctx, st, al->nms, cand, 1, H, W, cf.detection_threshold, r, nullptr, false));
   al_threshold_kernel<<<1, 1024, 0, st>>>(al->score, H * W, al->cand_count, cf.detection_threshold, al->thr_dev);
   DIMB_LAUNCH_CHECK(ctx);
-  sp_count_kernel<<<dim3(nch, 1), 256, 0, st>>>(al->nms, al->chunk_count, H, W, 0.f, r, nch, al->thr_dev);
-  DIMB_LAUNCH_CHECK(ctx);
-  sp_scan_kernel<<<1, 32, 0, st>>>(al->chunk_count, al->chunk_off, al->cand_count, nch);
-  DIMB_LAUNCH_CHECK(ctx);
-  sp_compact_kernel<<<dim3(nch, 1), 256, 0, st>>>(al->nms, al->chunk_off, al->cand_idx, al->cand_score, H, W, 0.f, r, nch, al->thr_dev);
-  DIMB_LAUNCH_CHECK(ctx);
+  DIMB_TRY(launch_candidates(ctx, st, al->nms, cand, 1, H, W, 0.f, r, al->thr_dev, true));
   if (al->sel_cap < cap) {
     if (al->sel_cap > 0)  // release the smaller per-keypoint buffers of an earlier call
       for (void* old : {static_cast<void*>(al->sel_idx), static_cast<void*>(al->sel_score), static_cast<void*>(al->kxy), static_cast<void*>(al->kscore),
@@ -939,15 +931,7 @@ int dimb_aliked_extract_dev(dimb_aliked* al, const float* image, int H, int W, i
     DIMB_TRY(dimb_tmap_2d(ctx, &al->m_f2[1], al->f2l, rows / 16, 2048, 2048, kTileM));
     al->sel_cap = cap;
   }
-  {
-    int Pw = 1;
-    while (Pw < std::max(K, 1)) Pw <<= 1;
-    const size_t smem = static_cast<size_t>(Pw) * sizeof(unsigned long long);
-    DIMB_TRY(dimb_func_smem(ctx, sp_select_kernel, static_cast<int>(smem)));
-    sp_select_kernel<<<1, kSelThreads, smem, st>>>(al->cand_idx, al->cand_score, al->cand_count, al->sel_idx, al->sel_score, count,
-                                                   H * W, K, cap, Pw);
-    DIMB_LAUNCH_CHECK(ctx);
-  }
+  DIMB_TRY(launch_select(ctx, st, cand, al->sel_idx, al->sel_score, count, 1, H * W, K, cap));
   al_dkd_refine_kernel<<<ceil_div(cap, 128), 128, 0, st>>>(al->score, H, W, r, al->sel_idx, count, cap, al->kxy, scores, al->kscore);
   DIMB_LAUNCH_CHECK(ctx);
   }

@@ -17,6 +17,8 @@
 // Largest lazy-rescale threshold of the attention kernel (attention.cuh), in log2 units: the softmax numerators P reach 2^lazy and
 // their hi plane is fp16 (largest finite value 65504 < 2^16), so 15 is the last whole threshold that cannot overflow it.
 constexpr float kAttnLazyMax = 15.f;
+// Opt-in dynamic shared memory per block on sm_90 (cudaDevAttrMaxSharedMemoryPerBlockOptin of the H100).
+constexpr int kSmemOptin = 232448;
 
 struct dimb_ctx {
   int device = 0;

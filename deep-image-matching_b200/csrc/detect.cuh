@@ -2,6 +2,8 @@
 // simple_nms (identical in both reference models: superpoint.py:47-63, aliked.py:66-89), threshold + border
 // compaction in row-major order, and top-k selection (radix select + bitonic sort).
 #pragma once
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace {
@@ -558,33 +560,48 @@ __global__ void __launch_bounds__(kSelThreads) sp_select_kernel(const int* __res
 }
 
 
-// launches simple_nms on a [B][H][W] score map
-inline int launch_nms(dimb_ctx* ctx, cudaStream_t st, const float* scores, float* out, int B, int H, int W, int r) {
-  if (ctx->nms_ver == 2 && r >= 1 && r <= 5) {  // bit-mask kernel (DIMB_NMS=1 selects the first cut below)
+// How simple_nms runs at radius r: kernel 2 = sp_nms2_kernel (bit masks), 1 = sp_nms_kernel (first cut); tile x tile outputs per CTA.
+struct NmsPlan {
+  int kernel, tile, threads, smem;
+};
+
+// ver: ctx->nms_ver (2: the bit-mask kernel for radii 1..5 and the first cut for the others; 1: the first cut at every radius, DIMB_NMS=1)
+inline NmsPlan nms_plan(int r, int ver) {
+  if (ver == 2 && r >= 1 && r <= 5) {
+    static constexpr int smem2[5] = {Nms2<1>::kSmem, Nms2<2>::kSmem, Nms2<3>::kSmem, Nms2<4>::kSmem, Nms2<5>::kSmem};
+    return {2, kNmsTile, Nms2<1>::kThreads, smem2[r - 1]};
+  }
+  // five S x S planes (S = tile + 10 r): four float, two byte masks.  64 x 64 outputs per CTA unless the 5r halo no longer fits
+  auto smem = [r](int t) { return (t + 10 * r) * ((t + 10 * r) | 1) * static_cast<int>(4 * sizeof(float) + 2); };
+  const int T = smem(kNmsTile) > kSmemOptin ? 32 : kNmsTile;
+  return {1, T, 1024, smem(T)};
+}
+
+// launches simple_nms on a [B][H][W] score map with the kernel nms_plan(r, ver) picks (production: ver = ctx->nms_ver)
+inline int launch_nms(dimb_ctx* ctx, cudaStream_t st, const float* scores, float* out, int B, int H, int W, int r, int ver) {
+  const NmsPlan p = nms_plan(r, ver);
+  if (p.kernel == 2) {
     dim3 grid2(ceil_div(W, kNmsTile), ceil_div(H, kNmsTile), B);
-    auto launch2 = [&](auto kern, size_t smem2) -> int {
-      DIMB_TRY(dimb_func_smem(ctx, kern, static_cast<int>(smem2)));
-      kern<<<grid2, 512, smem2, st>>>(scores, out, H, W);
+    auto launch2 = [&](auto kern) -> int {
+      DIMB_TRY(dimb_func_smem(ctx, kern, p.smem));
+      kern<<<grid2, p.threads, p.smem, st>>>(scores, out, H, W);
       return DIMB_OK;
     };
     switch (r) {
-      case 1: DIMB_TRY(launch2(sp_nms2_kernel<1>, Nms2<1>::kSmem)); break;
-      case 2: DIMB_TRY(launch2(sp_nms2_kernel<2>, Nms2<2>::kSmem)); break;
-      case 3: DIMB_TRY(launch2(sp_nms2_kernel<3>, Nms2<3>::kSmem)); break;
-      case 4: DIMB_TRY(launch2(sp_nms2_kernel<4>, Nms2<4>::kSmem)); break;
-      default: DIMB_TRY(launch2(sp_nms2_kernel<5>, Nms2<5>::kSmem)); break;
+      case 1: DIMB_TRY(launch2(sp_nms2_kernel<1>)); break;
+      case 2: DIMB_TRY(launch2(sp_nms2_kernel<2>)); break;
+      case 3: DIMB_TRY(launch2(sp_nms2_kernel<3>)); break;
+      case 4: DIMB_TRY(launch2(sp_nms2_kernel<4>)); break;
+      default: DIMB_TRY(launch2(sp_nms2_kernel<5>)); break;
     }
     DIMB_LAUNCH_CHECK(ctx);
     return DIMB_OK;
   }
-  int T = kNmsTile;  // 64x64 outputs per CTA unless the 5r halo no longer fits in shared memory
-  if (static_cast<size_t>(T + 10 * r) * ((T + 10 * r) | 1) * (4 * sizeof(float) + 2) > 220 * 1024) T = 32;
-  const int S = T + 10 * r;
-  const size_t smem = static_cast<size_t>(S) * (S | 1) * (4 * sizeof(float) + 2);
+  const int T = p.tile;
   dim3 grid(ceil_div(W, T), ceil_div(H, T), B);
   auto launch = [&](auto kern) -> int {
-    DIMB_TRY(dimb_func_smem(ctx, kern, static_cast<int>(smem)));
-    kern<<<grid, 1024, smem, st>>>(scores, out, H, W, r, T);
+    DIMB_TRY(dimb_func_smem(ctx, kern, p.smem));
+    kern<<<grid, p.threads, p.smem, st>>>(scores, out, H, W, r, T);
     return DIMB_OK;
   };
   switch (r) {  // the reference's configurations use 2/3 (pipelines), 4 (defaults) and 5 (tile preselection)
@@ -594,6 +611,40 @@ inline int launch_nms(dimb_ctx* ctx, cudaStream_t st, const float* scores, float
     case 5: DIMB_TRY(launch(sp_nms_kernel<5>)); break;
     default: DIMB_TRY(launch(sp_nms_kernel<-1>)); break;
   }
+  DIMB_LAUNCH_CHECK(ctx);
+  return DIMB_OK;
+}
+
+// Candidate buffers of B images of H x W: chunk_count / chunk_off [B][ceil(H W / kChunk)], cand_count [B], cand_idx / cand_score [B][H W]
+struct CandBufs {
+  int *chunk_count, *chunk_off, *cand_count, *cand_idx;
+  float* cand_score;
+};
+
+// Pixels of nms with score > thr, at least `border` pixels inside the image: counted (cand_count) and, with `compact`, written in
+// row-major order to cand_idx / cand_score.  thr_dev [B] (may be null): per-image thresholds read on the device, replacing thr.
+inline int launch_candidates(dimb_ctx* ctx, cudaStream_t st, const float* nms, const CandBufs& c, int B, int H, int W, float thr,
+                             int border, const float* thr_dev, bool compact) {
+  const int nch = ceil_div(H * W, kChunk);
+  sp_count_kernel<<<dim3(nch, B), 256, 0, st>>>(nms, c.chunk_count, H, W, thr, border, nch, thr_dev);
+  DIMB_LAUNCH_CHECK(ctx);
+  sp_scan_kernel<<<B, 32, 0, st>>>(c.chunk_count, c.chunk_off, c.cand_count, nch);
+  DIMB_LAUNCH_CHECK(ctx);
+  if (compact) {
+    sp_compact_kernel<<<dim3(nch, B), 256, 0, st>>>(nms, c.chunk_off, c.cand_idx, c.cand_score, H, W, thr, border, nch, thr_dev);
+    DIMB_LAUNCH_CHECK(ctx);
+  }
+  return DIMB_OK;
+}
+
+// Top-K of each image's candidates (sp_select_kernel) into sel_idx / sel_score [B][cap], counts to sel_count [B]; K < 0 keeps all
+inline int launch_select(dimb_ctx* ctx, cudaStream_t st, const CandBufs& c, int* sel_idx, float* sel_score, int* sel_count, int B, int HW,
+                         int K, int cap) {
+  int P = 1;  // the bitonic sort runs on K keys padded to a power of two
+  while (P < std::max(K, 1)) P <<= 1;
+  const size_t smem = static_cast<size_t>(P) * sizeof(unsigned long long);
+  DIMB_TRY(dimb_func_smem(ctx, sp_select_kernel, static_cast<int>(smem)));
+  sp_select_kernel<<<B, kSelThreads, smem, st>>>(c.cand_idx, c.cand_score, c.cand_count, sel_idx, sel_score, sel_count, HW, K, cap, P);
   DIMB_LAUNCH_CHECK(ctx);
   return DIMB_OK;
 }

@@ -122,7 +122,7 @@ struct PersGeom {
   static constexpr int kBTile = kPl * kBPlane;
   static constexpr int kStgFloats = CONV == 2 ? 64 * kStgPitch2 : ::kStgFloats;  // accumulator staging per consumer warpgroup
   static constexpr int kStgBytes = 2 * kStgFloats * 4;
-  static constexpr int kBudget = 232448 - 1024 - 1024 - kStgBytes;
+  static constexpr int kBudget = kSmemOptin - 1024 - 1024 - kStgBytes;
 };
 
 template <int BN, bool SPLIT, int CONV, bool RESB, class Epi>

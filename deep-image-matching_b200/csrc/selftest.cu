@@ -3,8 +3,12 @@
 //     C = A B^T and as the SuperPoint 3x3 conv layer (conv3x3.cuh), or their SIMT twin (DIMB_TC=0);
 //   dimb_selftest_gemm_plan: the launch plan of the persistent kernel, host only;
 //   dimb_selftest_attention: the flash-attention kernels through their production launches;
+//   dimb_selftest_detect: simple_nms, candidate compaction and top-k (detect.cuh) through their production launches;
+//   dimb_selftest_nms_plan: the launch plan of simple_nms, host only;
+//   dimb_selftest_sp_softmax / dimb_selftest_sp_describe: the SuperPoint head kernels (sp_head.cuh) through their production launches;
 //   dimb_gv_host: the RANSAC arithmetic of gv.cu on the host.
 #include <algorithm>
+#include <cstring>
 #include <vector>
 
 #include "conv3x3.cuh"
@@ -471,6 +475,163 @@ extern "C" int dimb_selftest_attention(dimb_ctx* ctx, int variant, const float* 
     return selftest_attention_hd128(ctx, Q, K, V, out, H, hd, NP, n, lazy, pad, out_pad);
   }
   return DIMB_ERR_ARG;
+}
+
+// ------------------------------------------------------------------ keypoint detection and the SuperPoint head kernels
+#include <climits>
+
+#include "detect.cuh"
+#include "sp_head.cuh"
+
+namespace {
+constexpr int kDetTail = 1024;  // elements past the last valid one in every output buffer of these entries
+
+// nms_plan version of a self-test cut: 0 = the production choice (prod_ver: ctx->nms_ver), 1 = first cut, 2 = bit-mask kernel
+// (radii 1..5 only); -1 when the cut cannot run at radius r
+int selftest_nms_ver(int r, int cut, int prod_ver) {
+  if (r < 0 || r > 8) return -1;
+  if (cut == 0) return prod_ver;
+  if (cut == 1) return 1;
+  if (cut == 2 && r >= 1 && r <= 5) return 2;
+  return -1;
+}
+
+void plan_out(const NmsPlan& p, int* out) {
+  out[0] = p.kernel;
+  out[1] = p.tile;
+  out[2] = p.threads;
+  out[3] = p.smem;
+}
+
+// int buffers start as the bit pattern of the float sentinel
+int sentinel_bits(float sentinel) {
+  int v;
+  memcpy(&v, &sentinel, sizeof v);
+  return v;
+}
+
+template <class T>
+int download(dimb_ctx* ctx, T* host, const T* dev, size_t n) {
+  DIMB_CUDA_OK(ctx, cudaMemcpy(host, dev, sizeof(T) * n, cudaMemcpyDeviceToHost));
+  return DIMB_OK;
+}
+}  // namespace
+
+// Launch plan of simple_nms at radius r (detect.cuh nms_plan), host only.  cut 0: the production choice of a default context (bit-mask
+// kernel for radii 1..5, first cut otherwise), 1: the first cut (sp_nms_kernel, radii 0..8), 2: the bit-mask kernel (sp_nms2_kernel,
+// radii 1..5).  out[4] = {kernel (1 first cut, 2 bit-mask), tile, threads, dynamic shared memory bytes}.
+extern "C" int dimb_selftest_nms_plan(int r, int cut, int* out) {
+  const int ver = selftest_nms_ver(r, cut, 2);
+  if (!out || ver < 0) return DIMB_ERR_ARG;
+  plan_out(nms_plan(r, ver), out);
+  return DIMB_OK;
+}
+
+// simple_nms, candidate compaction and top-k (detect.cuh) through the launch helpers SuperPoint and ALIKED run, on host fp32 scores
+// [B][H][W] (positive: the select kernel orders scores by their bits).
+//   r, cut: radius and kernel as dimb_selftest_nms_plan, except that cut 0 follows the context (DIMB_NMS=1 selects the first cut).
+//   thr >= 0: candidates are nms > thr; thr_per_image [B] (may be null) replaces it through the device-threshold argument, as ALIKED
+//   passes its threshold.  border: candidates lie at least `border` pixels inside the image.  K: top-k (-1 keeps every candidate, in
+//   row-major order), 1..kMaxTopK; cap >= K: selection slots per image.
+// Every output buffer holds kDetTail more elements after the valid ones, and starts as `sentinel` (int buffers: its bit pattern):
+//   nms [B H W], cand_count [B], cand_idx / cand_score [B][H W] (image b's first cand_count[b] entries are valid), sel_idx / sel_score
+//   [B][cap] (image b's first min(sel_count[b], cap)), sel_count [B].  plan[4] (may be null): the simple_nms plan that ran.
+extern "C" int dimb_selftest_detect(dimb_ctx* ctx, const float* scores, int B, int H, int W, int r, int cut, float thr,
+                                    const float* thr_per_image, int border, int K, int cap, float sentinel, float* nms, int* cand_count,
+                                    int* cand_idx, float* cand_score, int* sel_idx, float* sel_score, int* sel_count, int* plan) {
+  if (!ctx || !scores || !nms || !cand_count || !cand_idx || !cand_score || !sel_idx || !sel_score || !sel_count) return DIMB_ERR_ARG;
+  if (B < 1 || H < 1 || W < 1 || static_cast<long long>(B) * H * W > INT_MAX || border < 0 || !(thr >= 0.f)) return DIMB_ERR_ARG;
+  if (K == 0 || K < -1 || K > kMaxTopK || cap < 1 || K > cap) return DIMB_ERR_ARG;
+  if (thr_per_image)
+    for (int b = 0; b < B; ++b)
+      if (!(thr_per_image[b] >= 0.f)) return DIMB_ERR_ARG;
+  const int ver = selftest_nms_ver(r, cut, ctx->nms_ver);
+  if (ver < 0) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const int HW = H * W, nch = ceil_div(HW, kChunk);
+  const size_t npix = static_cast<size_t>(B) * HW, nsel = static_cast<size_t>(B) * cap;
+  const int isent = sentinel_bits(sentinel);
+  DevTmp t{ctx, {}};
+  float *d_scores, *d_nms, *d_cs, *d_ss, *d_thr = nullptr;
+  int *d_cc, *d_ci, *d_si, *d_sc;
+  CandBufs c;
+  DIMB_TRY(t.upload(&d_scores, std::vector<float>(scores, scores + npix)));
+  DIMB_TRY(t.upload(&d_nms, std::vector<float>(npix + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_cc, std::vector<int>(B + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_ci, std::vector<int>(npix + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_cs, std::vector<float>(npix + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_si, std::vector<int>(nsel + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_ss, std::vector<float>(nsel + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_sc, std::vector<int>(B + kDetTail, isent)));
+  DIMB_TRY(t.get(&c.chunk_count, static_cast<size_t>(B) * nch));
+  DIMB_TRY(t.get(&c.chunk_off, static_cast<size_t>(B) * nch));
+  if (thr_per_image) DIMB_TRY(t.upload(&d_thr, std::vector<float>(thr_per_image, thr_per_image + B)));
+  c.cand_count = d_cc;
+  c.cand_idx = d_ci;
+  c.cand_score = d_cs;
+  DIMB_TRY(launch_nms(ctx, 0, d_scores, d_nms, B, H, W, r, ver));
+  DIMB_TRY(launch_candidates(ctx, 0, d_nms, c, B, H, W, thr, border, d_thr, true));
+  DIMB_TRY(launch_select(ctx, 0, c, d_si, d_ss, d_sc, B, HW, K, cap));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_detect"));
+  DIMB_TRY(download(ctx, nms, d_nms, npix + kDetTail));
+  DIMB_TRY(download(ctx, cand_count, d_cc, B + kDetTail));
+  DIMB_TRY(download(ctx, cand_idx, d_ci, npix + kDetTail));
+  DIMB_TRY(download(ctx, cand_score, d_cs, npix + kDetTail));
+  DIMB_TRY(download(ctx, sel_idx, d_si, nsel + kDetTail));
+  DIMB_TRY(download(ctx, sel_score, d_ss, nsel + kDetTail));
+  DIMB_TRY(download(ctx, sel_count, d_sc, B + kDetTail));
+  if (plan) plan_out(nms_plan(r, ver), plan);
+  return DIMB_OK;
+}
+
+// sp_softmax_d2s_kernel through its production launch: logits [B h w][65] fp32 -> scores [B][8h][8w] (+ kDetTail, starting as
+// `sentinel`).
+extern "C" int dimb_selftest_sp_softmax(dimb_ctx* ctx, const float* logits, int B, int h, int w, float sentinel, float* scores) {
+  if (!ctx || !logits || !scores || B < 1 || h < 1 || w < 1 || static_cast<long long>(B) * h * w * 64 > INT_MAX) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const size_t cells = static_cast<size_t>(B) * h * w, n = cells * 64 + kDetTail;
+  DevTmp t{ctx, {}};
+  float *d_logits, *d_scores;
+  DIMB_TRY(t.upload(&d_logits, std::vector<float>(logits, logits + cells * 65)));
+  DIMB_TRY(t.upload(&d_scores, std::vector<float>(n, sentinel)));
+  DIMB_TRY(launch_sp_softmax(ctx, 0, d_logits, d_scores, B, h, w));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_sp_softmax"));
+  return download(ctx, scores, d_scores, n);
+}
+
+// sp_describe_kernel through its production launch.  sel_idx / sel_score [B][cap]: selected pixels of the 8h x 8w score map (the first
+// min(sel_count[b], cap) of image b are read, and must lie in the map); dense [B][h w][256] fp32 (convDb output, not normalised).
+// Outputs start as `sentinel` and hold kDetTail more elements: kpts [B][cap][2] (x, y), scores [B][cap], desc [B][256][cap].
+extern "C" int dimb_selftest_sp_describe(dimb_ctx* ctx, const int* sel_idx, const float* sel_score, const int* sel_count, const float* dense,
+                                         int B, int h, int w, int cap, int fix_sampling, float sentinel, float* kpts, float* scores,
+                                         float* desc) {
+  if (!ctx || !sel_idx || !sel_score || !sel_count || !dense || !kpts || !scores || !desc) return DIMB_ERR_ARG;
+  if (B < 1 || h < 1 || w < 1 || cap < 1 || static_cast<long long>(B) * h * w * 256 > INT_MAX || static_cast<long long>(B) * cap * 256 > INT_MAX)
+    return DIMB_ERR_ARG;
+  for (int b = 0; b < B; ++b) {
+    if (sel_count[b] < 0) return DIMB_ERR_ARG;
+    for (int k = 0; k < std::min(sel_count[b], cap); ++k) {
+      const int p = sel_idx[static_cast<size_t>(b) * cap + k];
+      if (p < 0 || p >= h * w * 64) return DIMB_ERR_ARG;
+    }
+  }
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const size_t nsel = static_cast<size_t>(B) * cap;
+  DevTmp t{ctx, {}};
+  int *d_si, *d_sc;
+  float *d_ss, *d_dense, *d_kpts, *d_scores, *d_desc;
+  DIMB_TRY(t.upload(&d_si, std::vector<int>(sel_idx, sel_idx + nsel)));
+  DIMB_TRY(t.upload(&d_ss, std::vector<float>(sel_score, sel_score + nsel)));
+  DIMB_TRY(t.upload(&d_sc, std::vector<int>(sel_count, sel_count + B)));
+  DIMB_TRY(t.upload(&d_dense, std::vector<float>(dense, dense + static_cast<size_t>(B) * h * w * 256)));
+  DIMB_TRY(t.upload(&d_kpts, std::vector<float>(nsel * 2 + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_scores, std::vector<float>(nsel + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_desc, std::vector<float>(nsel * 256 + kDetTail, sentinel)));
+  DIMB_TRY(launch_sp_describe(ctx, 0, d_si, d_ss, d_sc, d_dense, d_kpts, d_scores, d_desc, B, h, w, cap, fix_sampling));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_sp_describe"));
+  DIMB_TRY(download(ctx, kpts, d_kpts, nsel * 2 + kDetTail));
+  DIMB_TRY(download(ctx, scores, d_scores, nsel + kDetTail));
+  return download(ctx, desc, d_desc, nsel * 256 + kDetTail);
 }
 
 // ------------------------------------------------------------------ CPU drive of the RANSAC arithmetic of gv.cu (gv_math.cuh)

@@ -21,6 +21,7 @@
 #include "conv3x3.cuh"
 #include "detect.cuh"
 #include "gemm.cuh"
+#include "sp_head.cuh"
 
 namespace {
 
@@ -88,91 +89,6 @@ __global__ void __launch_bounds__(256, 3) sp_conv1a_kernel(const __grid_constant
     *reinterpret_cast<uint4*>(hi + g) = *reinterpret_cast<const uint4*>(sthi + off);
     if (lo) *reinterpret_cast<uint4*>(lo + g) = *reinterpret_cast<const uint4*>(stlo + off);
   }
-}
-
-// ------------------------------------------------------------------ softmax over 65 logits + depth-to-space
-// one warp per cell; logits [B*h*w][65] fp32 -> scores [B][8h][8w]       (superpoint.py:175-179)
-__global__ void sp_softmax_d2s_kernel(const float* __restrict__ logits, float* __restrict__ scores, int B, int h, int w) {
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (warp >= B * h * w) return;
-  const float* L = logits + static_cast<size_t>(warp) * 65;
-  const float a = L[lane], b2 = L[lane + 32], c = (lane == 0) ? L[64] : -INFINITY;
-  float m = fmaxf(fmaxf(a, b2), c);
-#pragma unroll
-  for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  const float ea = expf(a - m), eb = expf(b2 - m), ec = (lane == 0) ? expf(c - m) : 0.f;
-  float s = ea + eb + ec;
-#pragma unroll
-  for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  const int b = warp / (h * w), cell = warp - b * h * w, cy = cell / w, cx = cell - cy * w;
-  float* out = scores + (static_cast<size_t>(b) * h * 8 + cy * 8) * (w * 8) + cx * 8;
-  out[(lane >> 3) * (w * 8) + (lane & 7)] = ea / s;            // channel j = lane     -> (j/8, j%8)
-  out[((lane >> 3) + 4) * (w * 8) + (lane & 7)] = eb / s;      // channel j = lane+32
-}
-
-// ------------------------------------------------------------------ keypoints + descriptor sampling
-// warp per keypoint.  dense: [B][h*w][256] fp32 (convDb output, not yet normalised)
-__global__ void sp_describe_kernel(const int* __restrict__ sel_idx, const float* __restrict__ sel_score,
-                                   const int* __restrict__ sel_count, const float* __restrict__ dense, float* __restrict__ kpts,
-                                   float* __restrict__ scores, float* __restrict__ desc, int W8, int h, int w, int cap,
-                                   int fix_sampling) {
-  const int b = blockIdx.y;
-  const int k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  const int n = min(sel_count[b], cap);
-  if (k >= n) return;
-  const int p = sel_idx[static_cast<size_t>(b) * cap + k];
-  const int py = p / W8, px = p - py * W8;
-  const float x = static_cast<float>(px), y = static_cast<float>(py);
-  if (lane == 0) {
-    kpts[(static_cast<size_t>(b) * cap + k) * 2 + 0] = x;  // torch.flip(k,[1]).float(): (x, y)
-    kpts[(static_cast<size_t>(b) * cap + k) * 2 + 1] = y;
-    scores[static_cast<size_t>(b) * cap + k] = sel_score[static_cast<size_t>(b) * cap + k];
-  }
-  float ix, iy;
-  if (fix_sampling) {  // extractors/superpoint.py:16-27, align_corners=False
-    const float gx = (x + 0.5f) / (static_cast<float>(w) * 8.f) * 2.f - 1.f;
-    const float gy = (y + 0.5f) / (static_cast<float>(h) * 8.f) * 2.f - 1.f;
-    ix = ((gx + 1.f) * w - 1.f) / 2.f;
-    iy = ((gy + 1.f) * h - 1.f) / 2.f;
-  } else {  // thirdparty superpoint.py:81-98, align_corners=True
-    const float gx = (x - 4.f + 0.5f) / (w * 8.f - 4.f - 0.5f) * 2.f - 1.f;
-    const float gy = (y - 4.f + 0.5f) / (h * 8.f - 4.f - 0.5f) * 2.f - 1.f;
-    ix = ((gx + 1.f) / 2.f) * (w - 1);
-    iy = ((gy + 1.f) / 2.f) * (h - 1);
-  }
-  const float fx = floorf(ix), fy = floorf(iy);
-  const int x0 = static_cast<int>(fx), y0 = static_cast<int>(fy);
-  const float wx1 = ix - fx, wx0 = (fx + 1.f) - ix, wy1 = iy - fy, wy0 = (fy + 1.f) - iy;
-  float acc[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-  const float* D = dense + static_cast<size_t>(b) * h * w * 256;
-#pragma unroll
-  for (int cidx = 0; cidx < 4; ++cidx) {
-    const int cx = x0 + (cidx & 1), cy = y0 + (cidx >> 1);
-    const float wgt = ((cidx & 1) ? wx1 : wx0) * ((cidx >> 1) ? wy1 : wy0);
-    if (cx < 0 || cx >= w || cy < 0 || cy >= h) continue;  // padding_mode="zeros"
-    const float* d = D + (static_cast<size_t>(cy) * w + cx) * 256 + lane * 8;
-    const float4 q0 = *reinterpret_cast<const float4*>(d), q1 = *reinterpret_cast<const float4*>(d + 4);
-    const float e[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
-    float ss = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) ss = fmaf(e[j], e[j], ss);
-#pragma unroll
-    for (int o = 16; o; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-    const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);  // F.normalize(descriptors, p=2, dim=1)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[j] = fmaf(wgt, e[j] * inv, acc[j]);
-  }
-  float ss = 0.f;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) ss = fmaf(acc[j], acc[j], ss);
-#pragma unroll
-  for (int o = 16; o; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-  const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
-  float* o = desc + static_cast<size_t>(b) * 256 * cap + k;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) o[static_cast<size_t>(lane * 8 + j) * cap] = acc[j] * inv;  // (D,N) layout
 }
 
 }  // namespace
@@ -352,22 +268,15 @@ int dimb_sp_extract_dev(dimb_sp* sp, const float* d_images, int B, int H, int W,
   DIMB_TRY(run_conv1_f32(sp, st, sp->L[LDB], sp->dah, sp->dal, sp->ddesc, cells, 256, "sp.convDb"));
   {
     ProfScope prof(ctx, st, "sp.softmax");
-    sp_softmax_d2s_kernel<<<ceil_div(cells * 32, 256), 256, 0, st>>>(sp->logits, sp->scores, B, h, w);
-    DIMB_LAUNCH_CHECK(ctx);
+    DIMB_TRY(launch_sp_softmax(ctx, st, sp->logits, sp->scores, B, h, w));
   }
   {
     ProfScope prof(ctx, st, "sp.nms");
-    DIMB_TRY(launch_nms(ctx, st, sp->scores, sp->nms, B, H8, W8, cf.nms_radius));
+    DIMB_TRY(launch_nms(ctx, st, sp->scores, sp->nms, B, H8, W8, cf.nms_radius, ctx->nms_ver));
   }
-  const int nch = ceil_div(H8 * W8, kChunk);
   ProfScope prof_sel(ctx, st, "sp.select+describe");
-  sp_count_kernel<<<dim3(nch, B), 256, 0, st>>>(sp->nms, sp->chunk_count, H8, W8, cf.keypoint_threshold, cf.remove_borders, nch, nullptr);
-  DIMB_LAUNCH_CHECK(ctx);
-  sp_scan_kernel<<<B, 32, 0, st>>>(sp->chunk_count, sp->chunk_off, sp->cand_count, nch);
-  DIMB_LAUNCH_CHECK(ctx);
-  sp_compact_kernel<<<dim3(nch, B), 256, 0, st>>>(sp->nms, sp->chunk_off, sp->cand_idx, sp->cand_score, H8, W8,
-                                                   cf.keypoint_threshold, cf.remove_borders, nch, nullptr);
-  DIMB_LAUNCH_CHECK(ctx);
+  const CandBufs cand{sp->chunk_count, sp->chunk_off, sp->cand_count, sp->cand_idx, sp->cand_score};
+  DIMB_TRY(launch_candidates(ctx, st, sp->nms, cand, B, H8, W8, cf.keypoint_threshold, cf.remove_borders, nullptr, true));
   if (sp->sel_cap < cap) {  // selection scratch [max_batch][cap]; the smaller buffers of an earlier call are released
     dimb_free(ctx, sp->sel_idx);
     dimb_free(ctx, sp->sel_score);
@@ -375,20 +284,9 @@ int dimb_sp_extract_dev(dimb_sp* sp, const float* d_images, int B, int H, int W,
     DIMB_TRY(dimb_alloc_t(ctx, &sp->sel_score, static_cast<size_t>(cf.max_batch) * cap));
     sp->sel_cap = cap;
   }
-  {
-    int P = 1;
-    const int K = cf.max_keypoints;
-    while (P < std::max(K, 1)) P <<= 1;
-    const size_t smem = static_cast<size_t>(P) * sizeof(unsigned long long);
-    DIMB_TRY(dimb_func_smem(ctx, sp_select_kernel, static_cast<int>(smem)));
-    sp_select_kernel<<<B, kSelThreads, smem, st>>>(sp->cand_idx, sp->cand_score, sp->cand_count, sp->sel_idx, sp->sel_score,
-                                                   d_counts, H8 * W8, K, cap, P);
-    DIMB_LAUNCH_CHECK(ctx);
-  }
-  sp_describe_kernel<<<dim3(ceil_div(cap * 32, 256), B), 256, 0, st>>>(sp->sel_idx, sp->sel_score, d_counts, sp->ddesc, d_kpts,
-                                                                        d_scores, d_desc, W8, h, w, cap, cf.fix_sampling);
-  DIMB_LAUNCH_CHECK(ctx);
-  return DIMB_OK;
+  DIMB_TRY(launch_select(ctx, st, cand, sp->sel_idx, sp->sel_score, d_counts, B, H8 * W8, cf.max_keypoints, cap));
+  return launch_sp_describe(ctx, st, sp->sel_idx, sp->sel_score, d_counts, sp->ddesc, d_kpts, d_scores, d_desc, B, h, w, cap,
+                            cf.fix_sampling);
 }
 
 int dimb_sp_extract(dimb_sp* sp, const float* images, int B, int H, int W, float* kpts, float* scores, float* desc, int* counts,
