@@ -31,7 +31,7 @@ EXPORTS = [
     "dimb_fstore_feats_dev", "dimb_fstore_block_dev", "dimb_gv_fundamental", "dimb_gv_fundamental_batch_dev", "dimb_gv_verify_dev",
     "dimb_tile_grid", "dimb_tile_cut_dev", "dimb_tile_merge_dev", "dimb_tile_views_dev", "dimb_tile_match_merge_dev",
     "dimb_resize_area_tab", "dimb_resize_area_dev", "dimb_kpts_extent_dev", "dimb_tile_preselect_dev",
-    "dimb_resize_area_linear_tab", "dimb_resize_area_linear_dev", "dimb_pyr_size", "dimb_pyr_dev", "dimb_fstore_rescale_dev",
+    "dimb_resize_area_linear_tab", "dimb_resize_area_linear_dev", "dimb_resize_area_rgb_dev", "dimb_pyr_size", "dimb_pyr_dev", "dimb_fstore_rescale_dev",
     "dimb_tile_preselect_pairs_dev", "dimb_rot90_dev", "dimb_fstore_unrotate_dev",
 ]
 
@@ -175,6 +175,7 @@ def load_library():
     lib.dimb_resize_area_dev.argtypes = [vp, vp, ip, ip, ip, vp, ip, ip, vp]
     lib.dimb_resize_area_linear_tab.argtypes = [ip, ip, vp, vp, C.POINTER(ip)]
     lib.dimb_resize_area_linear_dev.argtypes = [vp, vp, ip, ip, ip, vp, ip, ip, vp]
+    lib.dimb_resize_area_rgb_dev.argtypes = [vp, vp, ip, ip, ip, vp, ip, ip, vp]
     lib.dimb_pyr_size.argtypes = [ip, ip, ip, C.POINTER(ip), C.POINTER(ip)]
     lib.dimb_pyr_dev.argtypes = [vp, vp, ip, ip, ip, ip, ip, vp, vp]
     lib.dimb_fstore_rescale_dev.argtypes = [vp, ip, vp, ip, ip, ip, vp]
@@ -577,6 +578,12 @@ class Context:
         """cv2.resize(INTER_AREA) of B float32 gray device images [B][H][W] -> [B][H2][W2] when H2 > H or W2 > W, OpenCV's bilinear
         emulation (dimb_resize_area_linear_dev); asynchronous on `stream`."""
         self.check(self.lib.dimb_resize_area_linear_dev(self.h, d_src, B, H, W, d_dst, H2, W2, stream), "dimb_resize_area_linear_dev")
+
+    def resize_area_rgb_dev(self, d_src, B, H, W, d_dst, H2, W2, stream=0):
+        """cv2.resize(pairs_generator.gray_from_rgb(img), (W2, H2), interpolation=INTER_AREA) of B float32 RGB device images [B][H][W][3]
+        -> gray [B][H2][W2], any size relation, the gray rule applied per source pixel as it is read (dimb_resize_area_rgb_dev);
+        asynchronous on `stream`."""
+        self.check(self.lib.dimb_resize_area_rgb_dev(self.h, d_src, B, H, W, d_dst, H2, W2, stream), "dimb_resize_area_rgb_dev")
 
     def pyr_dev(self, d_src, B, H, W, channels, level, d_dst, stream=0):
         """cv2.pyrDown `level` times (1..3) or cv2.pyrUp once (-1) of B float32 device images [B][H][W][channels], 1 or 3 channels,

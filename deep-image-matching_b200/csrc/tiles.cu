@@ -354,18 +354,36 @@ struct AreaTab {  // per axis: the entries of output index d are [ofs[d], ofs[d 
   const float *xa, *ya;
 };
 
+// The source pixels of the INTER_AREA kernels, read through a pointer to a pixel's first value: a gray image [H][W] as it is, or an
+// RGB image [H][W][3] made gray per pixel by the project's gray rule (pairs_generator.gray_from_rgb): each channel rounded half to
+// even and clamped to 0..255 (cvRound, then saturate_cast<uchar>), then cv::cvtColor's RGB2GRAY in 15-bit fixed point,
+// (9798 R + 19235 G + 3735 B + 2^14) >> 15.  The gray value is an integer in 0..255, so the arithmetic after it is the gray path's.
+struct GrayPixel {
+  static constexpr int kChannels = 1;
+  static __device__ __forceinline__ float load(const float* px) { return *px; }
+};
+struct RgbGrayPixel {
+  static constexpr int kChannels = 3;
+  static __device__ __forceinline__ float load(const float* px) {
+    const auto u8 = [](float v) { return min(max(__float2int_rn(v), 0), 255); };
+    return static_cast<float>((9798 * u8(px[0]) + 19235 * u8(px[1]) + 3735 * u8(px[2]) + 16384) >> 15);
+  }
+};
+
 // resizeArea_: per output pixel, the rows of the y-table in order; buf = sum of S * alpha in x-table order from 0; the first row sets
 // sum = beta * buf, the others add beta * buf.  Every product and sum is rounded on its own, as OpenCV's scalar code does.
+template <class Px>
 __global__ void resize_area_kernel(const float* __restrict__ src, float* __restrict__ dst, int H, int W, int H2, int W2, AreaTab t) {
+  constexpr int C = Px::kChannels;
   const int dx = blockIdx.x * blockDim.x + threadIdx.x, dy = blockIdx.y, b = blockIdx.z;
   if (dx >= W2) return;
-  const float* img = src + static_cast<size_t>(b) * H * W;
+  const float* img = src + static_cast<size_t>(b) * H * W * C;
   const int x0 = t.xofs[dx], x1 = t.xofs[dx + 1], j0 = t.yofs[dy], j1 = t.yofs[dy + 1];
   float sum = 0.f;
   for (int j = j0; j < j1; ++j) {
-    const float* row = img + static_cast<size_t>(t.ysrc[j]) * W;
+    const float* row = img + static_cast<size_t>(t.ysrc[j]) * W * C;
     float buf = 0.f;
-    for (int k = x0; k < x1; ++k) buf = __fadd_rn(buf, __fmul_rn(row[t.xsrc[k]], t.xa[k]));
+    for (int k = x0; k < x1; ++k) buf = __fadd_rn(buf, __fmul_rn(Px::load(row + t.xsrc[k] * C), t.xa[k]));
     const float v = __fmul_rn(t.ya[j], buf);
     sum = j == j0 ? v : __fadd_rn(sum, v);
   }
@@ -374,14 +392,16 @@ __global__ void resize_area_kernel(const float* __restrict__ src, float* __restr
 
 // resizeAreaFast_ for integer factors (fy, fx): the block row-major, sum += ((a + b) + c) + d per four pixels, then sum * (1.f / area).
 // For 2 x 2 OpenCV's vector loop (ResizeAreaFastVec_SIMD_32f) covers the columns dx < vec_end and computes ((a + b) + (c + d)) * 0.25f;
-// the scalar loop above takes the rest of the row.
+// the scalar loop above takes the rest of the row.  fy = fx = 1 with vec_end = 0 returns the source pixels exactly.
+template <class Px>
 __global__ void resize_area_fast_kernel(const float* __restrict__ src, float* __restrict__ dst, int H, int W, int H2, int W2, int fy, int fx,
                                         int vec_end) {
+  constexpr int C = Px::kChannels;
   const int dx = blockIdx.x * blockDim.x + threadIdx.x, dy = blockIdx.y, b = blockIdx.z;
   if (dx >= W2) return;
-  const float* S = src + (static_cast<size_t>(b) * H + static_cast<size_t>(dy) * fy) * W + static_cast<size_t>(dx) * fx;
+  const float* S = src + ((static_cast<size_t>(b) * H + static_cast<size_t>(dy) * fy) * W + static_cast<size_t>(dx) * fx) * C;
   const int area = fy * fx;
-  auto at = [&](int k) { return S[static_cast<size_t>(k / fx) * W + k % fx]; };
+  auto at = [&](int k) { return Px::load(S + (static_cast<size_t>(k / fx) * W + k % fx) * C); };
   if (dx < vec_end) {
     dst[(static_cast<size_t>(b) * H2 + dy) * W2 + dx] = __fmul_rn(__fadd_rn(__fadd_rn(at(0), at(1)), __fadd_rn(at(2), at(3))), 0.25f);
     return;
@@ -422,19 +442,94 @@ struct LinearTab {  // per axis: the source index [dsize] and the weight pairs [
 // resizeGeneric_ with HResizeLinear / VResizeLinear in float: each of the two source rows sy and min(sy + 1, H - 1) is resampled
 // horizontally as S[sx] * a0 + S[sx + 1] * a1 (S[sx] from xmax on), then out = row0 * b0 + row1 * b1; every product and sum is
 // rounded on its own (no FMA).
+template <class Px>
 __global__ void resize_area_linear_kernel(const float* __restrict__ src, float* __restrict__ dst, int H, int W, int H2, int W2,
                                           LinearTab t) {
+  constexpr int C = Px::kChannels;
   const int dx = blockIdx.x * blockDim.x + threadIdx.x, dy = blockIdx.y, b = blockIdx.z;
   if (dx >= W2) return;
   const int sx = t.xs[dx], sy = t.ys[dy];
   const float2 a = t.xa[dx], be = t.ya[dy];
-  const float* img = src + static_cast<size_t>(b) * H * W;
+  const float* img = src + static_cast<size_t>(b) * H * W * C;
   auto hrow = [&](int y) {
-    const float* S = img + static_cast<size_t>(y) * W;
-    return dx < t.xmax ? __fadd_rn(__fmul_rn(S[sx], a.x), __fmul_rn(S[sx + 1], a.y)) : S[sx];
+    const float* S = img + static_cast<size_t>(y) * W * C;
+    return dx < t.xmax ? __fadd_rn(__fmul_rn(Px::load(S + sx * C), a.x), __fmul_rn(Px::load(S + (sx + 1) * C), a.y)) : Px::load(S + sx * C);
   };
   const float r0 = hrow(sy), r1 = hrow(min(sy + 1, H - 1));
   dst[(static_cast<size_t>(b) * H2 + dy) * W2 + dx] = __fadd_rn(__fmul_rn(r0, be.x), __fmul_rn(r1, be.y));
+}
+
+// The launches of the INTER_AREA entries for source pixels Px, arguments checked by the entry: the integer-factor kernel when both
+// factors are integers (1 x 1 included), otherwise the table kernel with one upload of both axes' tables.
+template <class Px>
+int resize_area_launch(dimb_ctx* ctx, const float* d_src, int B, int height, int width, float* d_dst, int height2, int width2,
+                       cudaStream_t st) {
+  const dim3 grid(ceil_div(width2, 128), height2, B);
+  const int fy = area_fast_factor(height, height2), fx = area_fast_factor(width, width2);
+  if (fy && fx) {
+    // OpenCV's baseline build vectorises float rows 128 bits (4 lanes) wide; only 2 x 2 has a vector loop
+    const int vec_end = fy == 2 && fx == 2 ? width2 / kCvFloatLanes * kCvFloatLanes : 0;
+    ProfScope prof(ctx, st, "tile.resize");
+    resize_area_fast_kernel<Px><<<grid, 128, 0, st>>>(d_src, d_dst, height, width, height2, width2, fy, fx, vec_end);
+    DIMB_LAUNCH_CHECK(ctx);
+    return DIMB_OK;
+  }
+  // one upload: x offsets [W2 + 1], x sources, y offsets [H2 + 1], y sources, then the x and y weights (float bits)
+  std::vector<int> xd, xs, yd, ys;
+  std::vector<float> xa, ya;
+  area_tab(width, width2, &xd, &xs, &xa);
+  area_tab(height, height2, &yd, &ys, &ya);
+  auto offsets = [](const std::vector<int>& d, int n) {
+    std::vector<int> o(n + 1, 0);
+    for (int v : d) ++o[v + 1];
+    for (int i = 0; i < n; ++i) o[i + 1] += o[i];
+    return o;
+  };
+  std::vector<int> hp = offsets(xd, width2);
+  const size_t o_xs = hp.size();
+  hp.insert(hp.end(), xs.begin(), xs.end());
+  const size_t o_yofs = hp.size();
+  const std::vector<int> yo = offsets(yd, height2);
+  hp.insert(hp.end(), yo.begin(), yo.end());
+  const size_t o_ys = hp.size();
+  hp.insert(hp.end(), ys.begin(), ys.end());
+  const size_t o_xa = hp.size();
+  hp.resize(o_xa + xa.size() + ya.size());
+  std::memcpy(hp.data() + o_xa, xa.data(), xa.size() * sizeof(float));
+  std::memcpy(hp.data() + o_xa + xa.size(), ya.data(), ya.size() * sizeof(float));
+  int* d_tab;
+  DIMB_TRY(dimb_scratch(ctx, kSlotResizeTab, hp.size() * sizeof(int), reinterpret_cast<void**>(&d_tab)));
+  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_tab, hp.data(), hp.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  const AreaTab t{d_tab, d_tab + o_xs, d_tab + o_yofs, d_tab + o_ys, reinterpret_cast<const float*>(d_tab + o_xa),
+                  reinterpret_cast<const float*>(d_tab + o_xa + xa.size())};
+  ProfScope prof(ctx, st, "tile.resize");
+  resize_area_kernel<Px><<<grid, 128, 0, st>>>(d_src, d_dst, height, width, height2, width2, t);
+  DIMB_LAUNCH_CHECK(ctx);
+  return DIMB_OK;
+}
+
+// The bilinear emulation of INTER_AREA when an axis is enlarged, for source pixels Px, arguments checked by the entry.
+template <class Px>
+int resize_area_linear_launch(dimb_ctx* ctx, const float* d_src, int B, int height, int width, float* d_dst, int height2, int width2,
+                              cudaStream_t st) {
+  // one upload: the x and y weight pairs (float bits, first so that the float2 reads stay aligned), then x and y sources
+  std::vector<int> hp(3 * static_cast<size_t>(width2 + height2));
+  float* xa = reinterpret_cast<float*>(hp.data());
+  float* ya = xa + 2 * width2;
+  int* xs = hp.data() + 2 * (width2 + height2);
+  int* ys = xs + width2;
+  const int xmax = area_linear_tab(width, width2, xs, xa);
+  area_linear_tab(height, height2, ys, ya);
+  int* d_tab;
+  DIMB_TRY(dimb_scratch(ctx, kSlotResizeTab, hp.size() * sizeof(int), reinterpret_cast<void**>(&d_tab)));
+  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_tab, hp.data(), hp.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  const float2* d_w = reinterpret_cast<const float2*>(d_tab);
+  const int* d_s = d_tab + 2 * (width2 + height2);
+  const LinearTab t{d_s, d_s + width2, d_w, d_w + width2, xmax};
+  ProfScope prof(ctx, st, "tile.resize");
+  resize_area_linear_kernel<Px><<<dim3(ceil_div(width2, 128), height2, B), 128, 0, st>>>(d_src, d_dst, height, width, height2, width2, t);
+  DIMB_LAUNCH_CHECK(ctx);
+  return DIMB_OK;
 }
 
 // cv::borderInterpolate with BORDER_REFLECT_101 (BORDER_DEFAULT): gfedcb|abcdefgh|gfedcba.
@@ -822,48 +917,7 @@ int dimb_resize_area_dev(dimb_ctx* ctx, const float* d_src, int B, int height, i
     DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_dst, d_src, static_cast<size_t>(B) * height * width * sizeof(float), cudaMemcpyDeviceToDevice, st));
     return DIMB_OK;
   }
-  const dim3 grid(ceil_div(width2, 128), height2, B);
-  const int fy = area_fast_factor(height, height2), fx = area_fast_factor(width, width2);
-  if (fy && fx) {
-    // OpenCV's baseline build vectorises float rows 128 bits (4 lanes) wide; only 2 x 2 has a vector loop
-    const int vec_end = fy == 2 && fx == 2 ? width2 / kCvFloatLanes * kCvFloatLanes : 0;
-    ProfScope prof(ctx, st, "tile.resize");
-    resize_area_fast_kernel<<<grid, 128, 0, st>>>(d_src, d_dst, height, width, height2, width2, fy, fx, vec_end);
-    DIMB_LAUNCH_CHECK(ctx);
-    return DIMB_OK;
-  }
-  // one upload: x offsets [W2 + 1], x sources, y offsets [H2 + 1], y sources, then the x and y weights (float bits)
-  std::vector<int> xd, xs, yd, ys;
-  std::vector<float> xa, ya;
-  area_tab(width, width2, &xd, &xs, &xa);
-  area_tab(height, height2, &yd, &ys, &ya);
-  auto offsets = [](const std::vector<int>& d, int n) {
-    std::vector<int> o(n + 1, 0);
-    for (int v : d) ++o[v + 1];
-    for (int i = 0; i < n; ++i) o[i + 1] += o[i];
-    return o;
-  };
-  std::vector<int> hp = offsets(xd, width2);
-  const size_t o_xs = hp.size();
-  hp.insert(hp.end(), xs.begin(), xs.end());
-  const size_t o_yofs = hp.size();
-  const std::vector<int> yo = offsets(yd, height2);
-  hp.insert(hp.end(), yo.begin(), yo.end());
-  const size_t o_ys = hp.size();
-  hp.insert(hp.end(), ys.begin(), ys.end());
-  const size_t o_xa = hp.size();
-  hp.resize(o_xa + xa.size() + ya.size());
-  std::memcpy(hp.data() + o_xa, xa.data(), xa.size() * sizeof(float));
-  std::memcpy(hp.data() + o_xa + xa.size(), ya.data(), ya.size() * sizeof(float));
-  int* d_tab;
-  DIMB_TRY(dimb_scratch(ctx, kSlotResizeTab, hp.size() * sizeof(int), reinterpret_cast<void**>(&d_tab)));
-  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_tab, hp.data(), hp.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-  const AreaTab t{d_tab, d_tab + o_xs, d_tab + o_yofs, d_tab + o_ys, reinterpret_cast<const float*>(d_tab + o_xa),
-                  reinterpret_cast<const float*>(d_tab + o_xa + xa.size())};
-  ProfScope prof(ctx, st, "tile.resize");
-  resize_area_kernel<<<grid, 128, 0, st>>>(d_src, d_dst, height, width, height2, width2, t);
-  DIMB_LAUNCH_CHECK(ctx);
-  return DIMB_OK;
+  return resize_area_launch<GrayPixel>(ctx, d_src, B, height, width, d_dst, height2, width2, st);
 }
 
 int dimb_resize_area_linear_tab(int ssize, int dsize, int* s_idx, float* alpha, int* xmax) {
@@ -877,25 +931,18 @@ int dimb_resize_area_linear_dev(dimb_ctx* ctx, const float* d_src, int B, int he
   if (!ctx || !d_src || !d_dst || B < 1 || B > 65535 || height < 1 || width < 1 || height > (1 << 20) || width > (1 << 20) || height2 < 1 ||
       width2 < 1 || height2 > 65535 || width2 > (1 << 20) || (height2 <= height && width2 <= width))
     return DIMB_ERR_ARG;
-  // one upload: the x and y weight pairs (float bits, first so that the float2 reads stay aligned), then x and y sources
-  std::vector<int> hp(3 * static_cast<size_t>(width2 + height2));
-  float* xa = reinterpret_cast<float*>(hp.data());
-  float* ya = xa + 2 * width2;
-  int* xs = hp.data() + 2 * (width2 + height2);
-  int* ys = xs + width2;
-  const int xmax = area_linear_tab(width, width2, xs, xa);
-  area_linear_tab(height, height2, ys, ya);
+  return resize_area_linear_launch<GrayPixel>(ctx, d_src, B, height, width, d_dst, height2, width2, static_cast<cudaStream_t>(stream));
+}
+
+int dimb_resize_area_rgb_dev(dimb_ctx* ctx, const float* d_src, int B, int height, int width, float* d_dst, int height2, int width2,
+                             void* stream) {
+  if (!ctx || !d_src || !d_dst || B < 1 || B > 65535 || height < 1 || width < 1 || height > (1 << 20) || width > (1 << 20) || height2 < 1 ||
+      width2 < 1 || height2 > 65535 || width2 > (1 << 20))
+    return DIMB_ERR_ARG;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int* d_tab;
-  DIMB_TRY(dimb_scratch(ctx, kSlotResizeTab, hp.size() * sizeof(int), reinterpret_cast<void**>(&d_tab)));
-  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_tab, hp.data(), hp.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-  const float2* d_w = reinterpret_cast<const float2*>(d_tab);
-  const int* d_s = d_tab + 2 * (width2 + height2);
-  const LinearTab t{d_s, d_s + width2, d_w, d_w + width2, xmax};
-  ProfScope prof(ctx, st, "tile.resize");
-  resize_area_linear_kernel<<<dim3(ceil_div(width2, 128), height2, B), 128, 0, st>>>(d_src, d_dst, height, width, height2, width2, t);
-  DIMB_LAUNCH_CHECK(ctx);
-  return DIMB_OK;
+  if (height2 > height || width2 > width)
+    return resize_area_linear_launch<RgbGrayPixel>(ctx, d_src, B, height, width, d_dst, height2, width2, st);
+  return resize_area_launch<RgbGrayPixel>(ctx, d_src, B, height, width, d_dst, height2, width2, st);  // equal size: factors 1 x 1
 }
 
 int dimb_pyr_size(int height, int width, int level, int* height2, int* width2) {

@@ -52,6 +52,19 @@ def read_lowres(path, resize_max: int) -> np.ndarray:
     return cv2.resize(i0, size_new, interpolation=cv2.INTER_AREA)
 
 
+def gray_from_rgb(rgb) -> np.ndarray:
+    """The gray image of an RGB image (H, W, 3), float32 0..255 as ALIKED sets hold them: the gray image the low-resolution passes of
+    an ALIKED set (pair generation, tile preselection, the upright search) resize and run SuperPoint on.
+
+    The reference reads those passes' images with ``cv2.IMREAD_GRAYSCALE``, which for JPEG returns the codec's own luma plane; that
+    cannot be derived from the decoded RGB, so this project fixes the rule instead: each channel rounded half to even and clamped to
+    0..255, then cv2.cvtColor RGB2GRAY, in integers ``(9798 R + 19235 G + 3735 B + 16384) >> 15``.  It is the luma with R first,
+    unlike the gray images SuperPoint sets take, which carry the reference's BGR2GRAY-on-RGB order (SURVEY A.1).
+    ``ImageSetMatcher`` applies the same rule on the device (dimb_resize_area_rgb_dev)."""
+    import cv2
+    return cv2.cvtColor(np.clip(np.rint(rgb), 0, 255).astype(np.uint8), cv2.COLOR_RGB2GRAY).astype(np.float32)
+
+
 def pairs_from_lowres(img_list, resize_max: int = 1000, min_matches: int = 20, max_keypoints: int = 1024,
                       use_superpoint: bool = True, do_geometric_verification: bool = False, *, lightglue_weights: dict | None = None,
                       superpoint_weights: dict | None = None, device: int = 0, pair_batch: int = 16,

@@ -392,8 +392,9 @@ def _lowres_size(height: int, width: int, size: int):
 
 
 class _LowResSet:
-    """The low-resolution SuperPoint + LightGlue pass shared by tile preselection and pair generation.  ``extract`` resizes each image
-    once with INTER_AREA to longest side `size` (dimb_resize_area_dev, or dimb_resize_area_linear_dev when that enlarges an axis) and
+    """The low-resolution SuperPoint + LightGlue pass shared by tile preselection, pair generation and the upright search.  ``extract``
+    resizes each image once with INTER_AREA to longest side `size` (gray images: dimb_resize_area_dev, or dimb_resize_area_linear_dev
+    when that enlarges an axis; RGB images of an ALIKED set: dimb_resize_area_rgb_dev, gray_from_rgb's rule fused into the resize) and
     runs SuperPoint (`sp_conf`) into float32 buffers per store slot (no float16 cast: these features never pass through features.h5
     in the reference), with their own extent for LightGlue without image_size; ``buffers`` are what the exchange all-gathers (about
     (256 + 2) * 4 * K bytes per slot); ``match`` runs LightGlue (`lg_conf`) on a batch of slot pairs into m / ms / nm / sl.
@@ -446,11 +447,14 @@ class _LowResSet:
         return self.kp, self.de, self.n, self.size
 
     def extract(self, images, image_ids, slots, st):
-        """One resize batch: the equally sized images `images` ((k, H, W), at most batch_images) of images `image_ids`, stored in
-        `slots`."""
+        """One resize batch: the equally sized images `images` (gray (k, H, W) or RGB (k, H, W, 3), at most batch_images) of images
+        `image_ids`, stored in `slots`.  RGB images are made gray by ``pairs_generator.gray_from_rgb``'s rule inside the resize."""
         H, W = images.shape[1:3]
         h, w = self.low_sizes[image_ids[0]]
-        resize = self.ctx.resize_area_linear_dev if h > H or w > W else self.ctx.resize_area_dev
+        if images.dim() == 4:
+            resize = self.ctx.resize_area_rgb_dev
+        else:
+            resize = self.ctx.resize_area_linear_dev if h > H or w > W else self.ctx.resize_area_dev
         K, ss = self.K, slots
         low = self.low[:len(ss) * h * w].view(len(ss), h, w)
         resize(images.data_ptr(), len(ss), H, W, low.data_ptr(), h, w, st)
@@ -529,7 +533,13 @@ class ImageSetMatcher:
 
     ``extractor``: "superpoint" (default; gray images (k, H, W)) or "aliked" (RGB images (k, H, W, 3); ``sp_weights`` / ``sp_conf``
     are the ALIKED weights and the ``AlikedNet`` configuration, one image or tile per extraction call, 128-d descriptors, LightGlue
-    built with input_dim 128).  ALIKED with SuperGlue is refused.
+    built with input_dim 128).  ALIKED with SuperGlue is refused.  The low-resolution passes below (tile preselection, pair generation,
+    upright) run SuperPoint + SuperPoint-LightGlue for either extractor, as the reference does.  An ALIKED set feeds them the gray image
+    of each RGB image by ``pairs_generator.gray_from_rgb``'s rule (R first, not the BGR2GRAY order of a SuperPoint set's input), applied
+    per source pixel inside the resize (dimb_resize_area_rgb_dev); ``superpoint_weights`` is their SuperPoint (default
+    ``weights.superpoint_v1()``, the checkpoint the reference's hloc SuperPoint loads; refused with SuperPoint sets, where ``sp_weights``
+    is that network), and since ``lg_weights`` is then an input_dim-128 LightGlue, ``preselection_weights`` / ``lowres_weights`` /
+    ``upright_weights`` are required for the passes configured, whatever the matcher.
 
     ``tiling``: None (default) or a dict checked by ``tiling_conf``.  With tiling, ``extract`` takes full-size images, cuts their tiles
     on the device, runs the extractor over tiles (SuperPoint ``batch_images`` tiles per call, network sized for one tile, with
@@ -545,7 +555,7 @@ class ImageSetMatcher:
     ``exchange``); ``match`` runs LightGlue (``tiling.LG_PRESELECTION_CONF``, keypoints normalised by their own extent) on the
     low-resolution features of each pair batch and keeps the tile pairs with more than ``min_matches_per_tile`` matches inside both
     boxes.  ``preselection_weights``: the weights of that LightGlue (default ``lg_weights``; required with SuperGlue and
-    kornia_matcher).  SuperPoint only: ALIKED with preselection is refused.  The per-pair flags of one ``match`` call take T^2 bytes per pair on the device and
+    kornia_matcher, and with ALIKED).  The per-pair flags of one ``match`` call take T^2 bytes per pair on the device and
     on the host (``_preselect``), which matters only at hundreds of tiles per image.
 
     ``pair_generation``: None (default; the pair list is an input) or a dict checked by ``pair_generation_conf``, the reference's
@@ -554,8 +564,8 @@ class ImageSetMatcher:
     (``pairs_generator.SP_LOWRES_CONF``) into float32 per-slot buffers (about 2.1 MB per image, all-gathered by ``exchange``);
     ``lowres_pairs`` runs LightGlue (``pairs_generator.LG_LOWRES_CONF``, own-extent normalisation) over every brute-force pair, dealt to
     the ranks, and keeps the pairs with more than ``min_matches`` matches; ``run_lowres`` then matches the kept pairs.
-    ``lowres_weights``: the weights of that LightGlue (default ``lg_weights``; required with SuperGlue and kornia_matcher).  SuperPoint
-    only: ALIKED with pair generation is refused, and so is do_geometric_verification (an unknown key).
+    ``lowres_weights``: the weights of that LightGlue (default ``lg_weights``; required with SuperGlue, kornia_matcher and ALIKED).
+    do_geometric_verification is refused (an unknown key).
 
     ``quality``: the reference's extraction quality, checked by ``quality_conf`` ("high", the default, changes nothing).  ``height`` /
     ``width`` stay the original image size and ``extract`` still takes full-size images: per extraction batch dimb_pyr_dev resizes them
@@ -585,7 +595,9 @@ class ImageSetMatcher:
     ``image_size`` back on the original images, after which matching is refused until the next ``extract``; ``run`` /
     ``run_verified`` / ``run_lowres`` chain the steps (``run_lowres`` searches over the kept pairs), and ``export_colmap`` writes
     original-frame keypoints and camera sizes.  ``tile_idx`` keeps the rotated image's tile indices.  ``upright_weights``: the
-    search's SuperPoint-LightGlue weights (default ``lg_weights``; required with SuperGlue and kornia_matcher).  Refused: ALIKED, tile
+    search's SuperPoint-LightGlue weights (default ``lg_weights``; required with SuperGlue, kornia_matcher and ALIKED).  With ALIKED
+    the search runs on the gray images of the RGB originals and ALIKED extracts from the turned RGB images; ``rotate_back`` turns the
+    stored float16 keypoints back and rounds them to float16 again, which ALIKED's sub-pixel keypoints can feel.  Refused: tile
     preselection, and explicit ``tile_pairs``.  Every per-size rule is checked for both orientations of every image, and the extractor
     workspace, the store and the tile views are sized for both, since the rotations are unknown at construction (a set of 1536 x 2048
     images gets a 2048 x 2048 workspace); the search holds four float32 feature entries per image (about 8.5 MB at 2048 keypoints)
@@ -595,7 +607,7 @@ class ImageSetMatcher:
                  batch_images: int = 16, batch_pairs: int = 32, dist=None, matcher: str = "lightglue", verification: dict | None = None,
                  tiling: dict | None = None, extractor: str = "superpoint", preselection_weights: dict | None = None,
                  pair_generation: dict | None = None, lowres_weights: dict | None = None, quality: str = "high", upright: dict | None = None,
-                 upright_weights: dict | None = None):
+                 upright_weights: dict | None = None, superpoint_weights: dict | None = None):
         import torch
 
         from . import _native
@@ -605,6 +617,9 @@ class ImageSetMatcher:
             raise ValueError(f'extractor must be "superpoint" or "aliked", got {extractor!r}')
         if extractor == "aliked" and matcher == "superglue":
             raise ValueError("SuperGlue matches SuperPoint features only; use matcher=\"lightglue\" with ALIKED")
+        if extractor == "superpoint" and superpoint_weights is not None:
+            raise ValueError("superpoint_weights is the low-resolution SuperPoint of an ALIKED set; with extractor=\"superpoint\" sp_weights "
+                             "is that network")
         self.nn_conf = kornia_conf(lg_conf) if matcher == "kornia_matcher" else None
         self.tiling = tiling_conf(tiling)
         self.sizes = image_sizes(n_images, height, width)
@@ -612,9 +627,11 @@ class ImageSetMatcher:
         # the distinct sizes: every per-size rule is checked once per size; with upright for both orientations of every image
         shapes = list(dict.fromkeys(self.sizes + ([(w, h) for h, w in self.sizes] if self.up else [])))
         self.presel = self.tiling is not None and self.tiling["tile_selection"] == "preselection"
+        # an ALIKED set's lg_weights is an input_dim-128 LightGlue: its low-resolution passes need their SuperPoint-LightGlue weights
+        aliked_lg = "the superpoint_lightglue state dict (lg_weights of an ALIKED set is an input_dim-128 LightGlue)"
         if self.up is not None:
-            if extractor == "aliked":
-                raise ValueError("upright searches with SuperPoint on gray images and is available with extractor=\"superpoint\" only")
+            if extractor == "aliked" and upright_weights is None:
+                raise ValueError(f"upright with extractor=\"aliked\" needs upright_weights, {aliked_lg}")
             if self.presel:
                 raise ValueError("upright with tile_selection \"preselection\" is not supported; use grid or exhaustive tile selection")
             if matcher != "lightglue" and upright_weights is None:
@@ -623,9 +640,8 @@ class ImageSetMatcher:
                 if min(_lowres_size(H, W, self.up["resize_max"])[1:]) < 1:
                     raise ValueError(f"upright resize_max {self.up['resize_max']} down-samples a {H}x{W} image to nothing")
         if self.presel:
-            if extractor == "aliked":
-                raise ValueError("tile preselection runs on gray images and is available with extractor=\"superpoint\" only; "
-                                 "pass tile_pairs with ALIKED")
+            if extractor == "aliked" and preselection_weights is None:
+                raise ValueError(f"tile preselection with extractor=\"aliked\" needs preselection_weights, {aliked_lg}")
             for H, W in shapes:
                 if self.tiling["tile_preselection_size"] > max(H, W):
                     raise ValueError(f"tile_preselection_size {self.tiling['tile_preselection_size']} exceeds the image's longest side "
@@ -648,9 +664,8 @@ class ImageSetMatcher:
                                  f"the {extractor} extractor needs")
         self.pairgen = pair_generation_conf(pair_generation)
         if self.pairgen is not None:
-            if extractor == "aliked":
-                raise ValueError("pair generation runs SuperPoint on gray low-resolution images (the reference reads them as gray) and is "
-                                 "available with extractor=\"superpoint\" only; pass pairs with ALIKED")
+            if extractor == "aliked" and lowres_weights is None:
+                raise ValueError(f"pair generation with extractor=\"aliked\" needs lowres_weights, {aliked_lg}")
             if matcher != "lightglue" and lowres_weights is None:
                 raise ValueError(f"pair generation with matcher=\"{matcher}\" needs lowres_weights (SuperPoint-LightGlue weights)")
             for H, W in shapes:
@@ -737,11 +752,15 @@ class ImageSetMatcher:
             self.mm = torch.zeros(batch_pairs, self.cap2, 2, dtype=torch.int64, device=dev)
             self.nmm = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
         self.pre = self.lowres = None
+        low_sp = sp_weights  # the low-resolution SuperPoint: the set's own, or for an ALIKED set superpoint_weights
+        if extractor == "aliked" and (self.presel or self.pairgen is not None or self.up is not None):
+            from .weights import superpoint_v1
+            low_sp = superpoint_v1() if superpoint_weights is None else superpoint_weights
         if self.presel:
             # PRESELECTION (matcher_base.py:1055-1089) on the device with the networks of matcher_base.py:143-159, and the box counts
             # of one pair batch
             from .tiling import LG_PRESELECTION_CONF, SP_PRESELECTION_CONF
-            self.pre = _LowResSet(ctx, sp_weights, lg_weights if preselection_weights is None else preselection_weights, self.world * self.ipr,
+            self.pre = _LowResSet(ctx, low_sp, lg_weights if preselection_weights is None else preselection_weights, self.world * self.ipr,
                                   self.sizes, self.tiling["tile_preselection_size"], SP_PRESELECTION_CONF, LG_PRESELECTION_CONF,
                                   batch_images, batch_pairs, dev)
             self.pre_h, self.pre_w = self.pre.h, self.pre.w
@@ -749,7 +768,7 @@ class ImageSetMatcher:
         if self.pairgen is not None:
             # matching_lowres (pairs_generator.py:40-235) with the networks of pairs_generator.py:104-126
             from .pairs_generator import LG_LOWRES_CONF, SP_LOWRES_CONF
-            self.lowres = _LowResSet(ctx, sp_weights, lg_weights if lowres_weights is None else lowres_weights, self.world * self.ipr,
+            self.lowres = _LowResSet(ctx, low_sp, lg_weights if lowres_weights is None else lowres_weights, self.world * self.ipr,
                                      self.sizes, self.pairgen["resize_max"], SP_LOWRES_CONF, LG_LOWRES_CONF, batch_images, batch_pairs, dev)
         self.search = self.rotations = None
         self._turned_back = False
@@ -758,7 +777,7 @@ class ImageSetMatcher:
             # tiling or pair generation is configured (quirk A.6), otherwise sp_conf's
             from .upright import LG_UPRIGHT_CONF, SP_UPRIGHT_CONF
             fix = self.tiling is not None or self.pairgen is not None or bool(sp_conf.get("fix_sampling", False))
-            self.search = _LowResSet(ctx, sp_weights, lg_weights if upright_weights is None else upright_weights, self.world * self.ipr,
+            self.search = _LowResSet(ctx, low_sp, lg_weights if upright_weights is None else upright_weights, self.world * self.ipr,
                                      self.sizes, self.up["resize_max"], {**SP_UPRIGHT_CONF, "max_keypoints": self.up["max_keypoints"],
                                                                          "fix_sampling": fix},
                                      LG_UPRIGHT_CONF, batch_images, batch_pairs, dev, rotations=True)

@@ -332,6 +332,17 @@ int dimb_resize_area_linear_tab(int ssize, int dsize, int* s_idx, float* alpha, 
  * dimb_resize_area_dev), otherwise the argument limits of dimb_resize_area_dev; profile group tile.resize.  CUDA cores. */
 int dimb_resize_area_linear_dev(dimb_ctx* ctx, const float* d_src, int B, int height, int width, float* d_dst, int height2, int width2,
                                 void* stream);
+/* The low-resolution gray image of an RGB image in one pass (the low-resolution passes of ALIKED sets): B float32 RGB images
+ * d_src [B][H][W][3] -> gray d_dst [B][H2][W2], bitwise cv2.resize(gray_from_rgb(img), (W2, H2), interpolation=INTER_AREA) for any
+ * size relation.  The gray rule (pairs_generator.gray_from_rgb) is applied to every source pixel as it is read, so no full-size gray
+ * image is staged: each channel rounded half to even and clamped to 0..255, then (9798 R + 19235 G + 3735 B + 2^14) >> 15, the
+ * RGB2GRAY of cv::cvtColor on uint8 (R first: not the BGR2GRAY order of the SuperPoint input).  The resize is then that of
+ * dimb_resize_area_dev (integer factors, 1 x 1 for H2 == H and W2 == W, or the area tables) or, when H2 > H or W2 > W, that of
+ * dimb_resize_area_linear_dev, with the same arithmetic.  DIMB_ERR_ARG (before any CUDA call) for B outside [1, 65535], H or W
+ * outside [1, 2^20], H2 outside [1, 65535], W2 outside [1, 2^20] or a NULL pointer; profile group tile.resize; asynchronous on
+ * `stream`.  CUDA cores. */
+int dimb_resize_area_rgb_dev(dimb_ctx* ctx, const float* d_src, int B, int height, int width, float* d_dst, int height2, int width2,
+                             void* stream);
 /* Extraction quality (ExtractorBase._resize_image / _resize_features, extractor_base.py:205,224): the reference resizes every image
  * by its `quality` before extracting and scales the keypoints back to the original image.  level: -1 = one cv2.pyrUp ("highest"),
  * 0 = none ("high"), 1..3 = that many cv2.pyrDown ("medium", "low", "lowest").  Host only (no CUDA call): the size after `level`
