@@ -20,7 +20,7 @@ NN_MODES = {"nn": 0, "mnn": 1, "snn": 2, "smnn": 3}
 
 EXPORTS = [
     "dimb_version", "dimb_ctx_create", "dimb_ctx_destroy", "dimb_last_error", "dimb_ctx_set_precision",
-    "dimb_ctx_set_tensor_path", "dimb_ctx_launch_count", "dimb_read_dev",
+    "dimb_ctx_launch_count", "dimb_read_dev",
     "dimb_sp_create", "dimb_sp_destroy", "dimb_sp_extract", "dimb_sp_extract_dev", "dimb_sp_debug_read",
     "dimb_lg_create", "dimb_lg_destroy", "dimb_lg_match", "dimb_lg_match_dev", "dimb_lg_debug_read",
     "dimb_nn_match", "dimb_nn_match_dev", "dimb_nn_match_batch_dev", "dimb_ctx_profile", "dimb_ctx_profile_read", "dimb_pipe_create", "dimb_pipe_destroy",
@@ -108,7 +108,6 @@ def load_library():
     lib.dimb_last_error.argtypes = [vp]
     lib.dimb_last_error.restype = C.c_char_p
     lib.dimb_ctx_set_precision.argtypes = [vp, ip]
-    lib.dimb_ctx_set_tensor_path.argtypes = [vp, ip]
     lib.dimb_ctx_launch_count.argtypes = [vp]
     lib.dimb_ctx_launch_count.restype = C.c_ulonglong
     lib.dimb_read_dev.argtypes = [vp, vp, vp, C.c_size_t]
@@ -251,8 +250,7 @@ def conv_mode(cout: int, B: int, H: int, W: int, num_sms: int) -> int:
 
 def nms_plan(r: int, cut: int = 0):
     """Launch plan (kernel, tile, threads, smem_bytes) of simple_nms at radius r (dimb_selftest_nms_plan): kernel 1 = first cut, 2 =
-    bit-mask kernel.  cut 0 = the production choice of a default context, 1 = first cut (radii 0..8), 2 = bit-mask kernel (radii
-    1..5).  Host only."""
+    bit-mask kernel.  cut 0 = the production choice, 1 = first cut (radii 0..8), 2 = bit-mask kernel (radii 1..5).  Host only."""
     out = np.zeros(4, np.int32)
     rc = load_selftest_library().dimb_selftest_nms_plan(int(r), int(cut), _ptr(out))
     if rc != OK:
@@ -284,7 +282,7 @@ class SelfTest:
         """C = A B^T (+ bias) through the production GEMM launch (dimb_selftest_gemm), precision of the context.  A [M][K], B [N][K],
         K a multiple of 64; k32: 32-wide K blocks (bn 256).  Rows of the operand allocations past M / N, and the output buffer, hold
         `guard`.  Returns (C [M][N], tail [128][N] of the output buffer past the last row, plan
-        {resb, sa, sb, smem_bytes, grid} of the launch; -1s on the SIMT twin)."""
+        {resb, sa, sb, smem_bytes, grid} of the launch)."""
         A = np.ascontiguousarray(A, np.float32)
         B = np.ascontiguousarray(B, np.float32)
         bias = None if bias is None else np.ascontiguousarray(bias, np.float32)
@@ -358,7 +356,7 @@ class SelfTest:
     def detect(self, scores: np.ndarray, r: int, cut: int = 0, thr: float = 0.0, thr_per_image=None, border: int = 0, K: int = -1,
                cap: int | None = None, sentinel: float = -777.0) -> dict:
         """simple_nms, candidate compaction and top-k through their production launches (dimb_selftest_detect).  scores [B][H][W]
-        positive; cut as nms_plan() except that 0 follows the context (DIMB_NMS); candidates are nms > thr (thr_per_image [B]: through
+        positive; cut as nms_plan(); candidates are nms > thr (thr_per_image [B]: through
         the device-threshold argument) at least `border` pixels inside; K = -1 keeps every candidate; cap defaults to K (H * W when
         K = -1).  Every buffer starts as `sentinel` (int buffers: its bit pattern).  Returns a dict of nms [B][H][W], cand_count [B],
         cand_idx / cand_score [B][H * W], sel_idx / sel_score [B][cap], sel_count [B], '<name>_tail' [DET_TAIL] for each, and plan."""
@@ -468,7 +466,7 @@ class Context:
 
     _per_device: dict = {}
 
-    def __init__(self, device: int = 0, precision: str | None = None, tensor_path: bool | None = None):
+    def __init__(self, device: int = 0, precision: str | None = None):
         self.lib = load_library()
         h = C.c_void_p()
         rc = self.lib.dimb_ctx_create(device, C.byref(h))
@@ -479,8 +477,6 @@ class Context:
         self.device = device
         if precision is not None:
             self.set_precision(precision)
-        if tensor_path is not None:
-            self.set_tensor_path(tensor_path)
 
     @classmethod
     def get(cls, device: int = 0) -> "Context":
@@ -495,9 +491,6 @@ class Context:
 
     def set_precision(self, precision: str):
         self.check(self.lib.dimb_ctx_set_precision(self.h, {"exact": 0, "fast": 1}[precision]), "set_precision")
-
-    def set_tensor_path(self, use_tc: bool):
-        self.check(self.lib.dimb_ctx_set_tensor_path(self.h, int(bool(use_tc))), "set_tensor_path")
 
     @property
     def launches(self) -> int:

@@ -900,7 +900,7 @@ int dimb_aliked_extract_dev(dimb_aliked* al, const float* image, int H, int W, i
   const int r = cf.nms_radius;
   {
   ProfScope prof(ctx, st, "al.detect");
-  DIMB_TRY(launch_nms(ctx, st, al->score, al->nms, 1, H, W, r, ctx->nms_ver));
+  DIMB_TRY(launch_nms(ctx, st, al->score, al->nms, 1, H, W, r, kNmsProductionVer));
   // threshold mode (aliked.py:152-160): nms > detection_threshold; if nothing passes, nms > mean(score_map).
   // Decided on the device: count, then al_threshold_kernel fixes the threshold, then count / scan / compact with it.
   const CandBufs cand{al->chunk_count, al->chunk_off, al->cand_count, al->cand_idx, al->cand_score};
@@ -950,7 +950,7 @@ int dimb_aliked_extract_dev(dimb_aliked* al, const float* image, int H, int W, i
     TcOperands ops;
     ops.Ah = al->m_fs[0], ops.Al = al->m_fs[1], ops.Bh = al->m_sf[0], ops.Bl = al->m_sf[1];
     GemmArgs g{};
-    g.num_kb = 2, g.M = cap * 16, g.N = 128, g.Ah = al->fsh, g.Al = al->fsl, g.Bh = al->sfh, g.Bl = al->sfl, g.lda = 128, g.ldb = 128;
+    g.num_kb = 2, g.M = cap * 16, g.N = 128;
     DIMB_TRY((launch_gemm<128, false>(ctx, st, ops, g, e, ceil_div(cap * 16, kTileM), 128, "al.sddh_sf_gemm")));
   }
   {  // aggregation einsum 'ncp,pcd->nd': [cap][2048] x [128][2048]^T
@@ -959,7 +959,7 @@ int dimb_aliked_extract_dev(dimb_aliked* al, const float* image, int H, int W, i
     TcOperands ops;
     ops.Ah = al->m_f2[0], ops.Al = al->m_f2[1], ops.Bh = al->m_ag[0], ops.Bl = al->m_ag[1];
     GemmArgs g{};
-    g.num_kb = 32, g.M = cap, g.N = 128, g.Ah = al->f2h, g.Al = al->f2l, g.Bh = al->agh, g.Bl = al->agl, g.lda = 2048, g.ldb = 2048;
+    g.num_kb = 32, g.M = cap, g.N = 128;
     DIMB_TRY((launch_gemm<128, false>(ctx, st, ops, g, e, ceil_div(cap, kTileM), 128, "al.sddh_agg_gemm")));
   }
   ProfScope prof(ctx, st, "al.sddh_norm");

@@ -239,8 +239,6 @@ int dimb_ctx_create(int device, dimb_ctx** out) {
     return DIMB_ERR_UNSUPPORTED;
   }
   ctx->num_sms = prop.multiProcessorCount;
-  const char* e = getenv("DIMB_TC");
-  if (e && e[0] == '0') ctx->use_tc = 0;
   const char* lz = getenv("DIMB_ATTN_LAZY");
   if (lz) {  // NaN, inf, out of range or no number at all: keep the default (common.cuh: kAttnLazyMax)
     char* end = nullptr;
@@ -251,8 +249,6 @@ int dimb_ctx_create(int device, dimb_ctx** out) {
   if (k3) ctx->k32 = k3[0] == '1';
   const char* b2 = getenv("DIMB_BN256");
   if (b2) ctx->bn256 = b2[0] == '1';
-  const char* nv = getenv("DIMB_NMS");
-  if (nv && atoi(nv) == 1) ctx->nms_ver = 1;
   const char* p = getenv("DIMB_PRECISION");
   if (p && !strcmp(p, "fast")) ctx->precision = DIMB_PRECISION_FAST;
   *out = ctx;
@@ -271,12 +267,6 @@ const char* dimb_last_error(dimb_ctx* ctx) { return ctx ? ctx->last_error.c_str(
 int dimb_ctx_set_precision(dimb_ctx* ctx, int precision) {
   if (!ctx || (precision != DIMB_PRECISION_EXACT && precision != DIMB_PRECISION_FAST)) return DIMB_ERR_ARG;
   ctx->precision = precision;
-  return DIMB_OK;
-}
-
-int dimb_ctx_set_tensor_path(dimb_ctx* ctx, int use_tc) {
-  if (!ctx) return DIMB_ERR_ARG;
-  ctx->use_tc = use_tc ? 1 : 0;
   return DIMB_OK;
 }
 

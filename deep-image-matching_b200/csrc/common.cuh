@@ -23,11 +23,9 @@ constexpr int kSmemOptin = 232448;
 struct dimb_ctx {
   int device = 0;
   int num_sms = 132;
-  int use_tc = 1;        // 1 = wgmma tensor path, 0 = SIMT CUDA-core debug path (DIMB_TC=0)
   int precision = DIMB_PRECISION_EXACT;
   int k32 = 0;            // 32-wide K stages (half-size stages) for the 128 x 256 LightGlue tiles (gemm.cuh CONV 3); DIMB_K32=1
   int bn256 = 0;          // LightGlue q/k projection and FFN0 on 128 x 256 output tiles (DIMB_BN256=1); default 128 x 128: spill-free
-  int nms_ver = 2;        // simple_nms kernel: 2 = bit-mask kernel (sp_nms2_kernel), 1 = first cut (DIMB_NMS)
   // lazy-rescale threshold of the attention kernel in log2 units (DIMB_ATTN_LAZY; 0 = rescale on every new maximum).  Only finite
   // values in [0, kAttnLazyMax] are taken from the environment, anything else keeps 8: P <= 2^lazy must fit the fp16 hi plane.
   float attn_lazy = 8.f;

@@ -97,8 +97,8 @@ inline int conv_m_tiles(int B, int H, int W, int conv = 1) {
 // 1440.  FAST keeps those weights resident, and the taller tile still pays off there: fewer halo rows and half the per-tile
 // overheads per pixel (conv1b / conv2a / conv2b 1.20 / 1.02 / 1.36 x faster at the bench shapes, DESIGN.md section 4).  They are
 // used wherever they still give every SM at least two tiles (fewer, larger tiles would idle SMs on small inputs).
-inline int conv_mode(int cout, bool use_tc, int B, int H, int W, int num_sms) {
-  return conv_bn(cout) == 64 && use_tc && conv_m_tiles(B, H, W, 2) >= 2 * num_sms ? 2 : 1;
+inline int conv_mode(int cout, int B, int H, int W, int num_sms) {
+  return conv_bn(cout) == 64 && conv_m_tiles(B, H, W, 2) >= 2 * num_sms ? 2 : 1;
 }
 
 // run_conv3 on tiles of one shape (CONV 1 or 2)
@@ -113,13 +113,6 @@ int run_conv3_tiles(dimb_ctx* ctx, cudaStream_t st, const ConvLayer& L, const __
   g.H = H;
   g.W = W;
   g.N = L.cout;
-  g.Ah = inh;
-  g.Al = inl;
-  g.Bh = L.wh;
-  g.Bl = L.wl;
-  g.lda = L.cin;
-  g.ldb = L.k;
-  g.k_total = L.k;
   auto fill = [&](auto& epi) {
     epi.hi = outh;
     epi.lo = exact ? outl : nullptr;
@@ -150,7 +143,7 @@ template <int BN, bool POOL>
 int run_conv3(dimb_ctx* ctx, cudaStream_t st, const ConvLayer& L, const __half* inh, const __half* inl, __half* outh, __half* outl,
               int B, int H, int W, const char* tag) {
   if constexpr (BN == 64) {
-    if (conv_mode(L.cout, ctx->use_tc, B, H, W, ctx->num_sms) == 2)
+    if (conv_mode(L.cout, B, H, W, ctx->num_sms) == 2)
       return run_conv3_tiles<BN, POOL, 2>(ctx, st, L, inh, inl, outh, outl, B, H, W, tag);
   }
   return run_conv3_tiles<BN, POOL, 1>(ctx, st, L, inh, inl, outh, outl, B, H, W, tag);

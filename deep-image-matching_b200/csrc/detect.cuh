@@ -565,7 +565,8 @@ struct NmsPlan {
   int kernel, tile, threads, smem;
 };
 
-// ver: ctx->nms_ver (2: the bit-mask kernel for radii 1..5 and the first cut for the others; 1: the first cut at every radius, DIMB_NMS=1)
+// ver 2: the bit-mask kernel for radii 1..5 and the first cut for the others (what production runs); 1: the first cut at every radius
+constexpr int kNmsProductionVer = 2;
 inline NmsPlan nms_plan(int r, int ver) {
   if (ver == 2 && r >= 1 && r <= 5) {
     static constexpr int smem2[5] = {Nms2<1>::kSmem, Nms2<2>::kSmem, Nms2<3>::kSmem, Nms2<4>::kSmem, Nms2<5>::kSmem};
@@ -577,7 +578,7 @@ inline NmsPlan nms_plan(int r, int ver) {
   return {1, T, 1024, smem(T)};
 }
 
-// launches simple_nms on a [B][H][W] score map with the kernel nms_plan(r, ver) picks (production: ver = ctx->nms_ver)
+// launches simple_nms on a [B][H][W] score map with the kernel nms_plan(r, ver) picks (production: ver = kNmsProductionVer)
 inline int launch_nms(dimb_ctx* ctx, cudaStream_t st, const float* scores, float* out, int B, int H, int W, int r, int ver) {
   const NmsPlan p = nms_plan(r, ver);
   if (p.kernel == 2) {

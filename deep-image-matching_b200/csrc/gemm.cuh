@@ -16,9 +16,7 @@
 //              accumulator through shared memory, 64 columns at a time (mode 2: 16), so that thread r owns output row r
 //              and 32 consecutive columns -> fused epilogue functor
 //
-// A SIMT twin (simt_gemm_kernel) evaluates the same contraction on CUDA cores with the same
-// epilogue functors; it is a debug/bisect aid (DIMB_TC=0), never the default.  The kernel is persistent:
-// one CTA per SM; the producer fills the stages of the next tile while the consumers run the epilogue.
+// The kernel is persistent: one CTA per SM; the producer fills the stages of the next tile while the consumers run the epilogue.
 #pragma once
 #include "common.cuh"
 #include "sm90.cuh"
@@ -29,16 +27,18 @@ struct TileCoord {
   int b, y0, x0;  // CONV: image index and top-left pixel of the ConvTile<CONV>::TH x 16 pixel tile
 };
 
+// Field order: the kernel reads num_kb, cin_blocks, tiles_x and tiles_y, and each of them shares its 8-byte word with a field it does
+// not read.  With tiles_x and tiles_y in one word nvcc loads them as a pair and schedules the 3x3 conv kernels differently: the
+// 128 -> 256 channel SuperPoint convolutions (convPa, convDa) then ran about 4 % slower on an H100 SXM at 700 W.
 struct GemmArgs {
   int num_kb;      // B tiles per output tile: K / 64 (CONV 3: K / 32)
-  int k_total;     // total K for the SIMT twin; 0 = num_kb * 64
   int M;           // GEMM: valid rows of A
-  int N;           // valid rows of B (output columns)
   int cin_blocks;  // CONV: Cin / 64
-  int H, W;        // CONV: spatial size
-  int tiles_x, tiles_y;
-  const __half *Ah, *Al, *Bh, *Bl;  // raw operands (SIMT twin); Al/Bl null in FAST mode
-  int lda, ldb;
+  int N;           // valid rows of B (output columns)
+  int H;           // CONV: image height
+  int tiles_x;     // CONV: tiles per image row / column
+  int tiles_y;
+  int W;           // CONV: image width
 };
 
 constexpr int kTileM = 128;
@@ -403,71 +403,6 @@ tc_gemm_pers_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_const
   }
 }
 
-// ------------------------------------------------------------------ SIMT twin (debug path)
-template <int CONV>
-__device__ __forceinline__ float simt_load_a(const GemmArgs& g, const TileCoord& tc, int row, int k) {
-  static_assert(CONV != 2, "the SIMT twin runs 128-row tiles: 3x3 convs use mode 1");
-  size_t off;
-  if (CONV == 1) {
-    const int cin = g.cin_blocks * 64;
-    const int tap = k / cin, c = k - tap * cin;
-    const int dy = tap / 3, dx = tap - dy * 3;
-    const int y = tc.y0 + row / ConvTile<CONV>::TW + dy - 1, x = tc.x0 + row % ConvTile<CONV>::TW + dx - 1;
-    if (y < 0 || y >= g.H || x < 0 || x >= g.W) return 0.f;
-    off = ((static_cast<size_t>(tc.b) * g.H + y) * g.W + x) * cin + c;
-  } else {
-    const int gm = tc.m0 + row;
-    if (gm >= g.M) return 0.f;
-    off = static_cast<size_t>(gm) * g.lda + k;
-  }
-  float v = __half2float(g.Ah[off]);
-  if (g.Al) v += __half2float(g.Al[off]);
-  return v;
-}
-
-template <int CONV, class Epi>
-__global__ void __launch_bounds__(128) simt_gemm_kernel(GemmArgs g, Epi epi) {
-  TileCoord tc = make_tile_coord<CONV>(g, blockIdx.x);
-  if (CONV != 1) tc.m0 = epi.m0_of(blockIdx.x);
-  tc.n0 = blockIdx.y * 32;
-  if (!epi.tile_active(tc)) return;
-  const int b_off = epi.b_row_offset(tc);
-  __shared__ float As[128][33];
-  __shared__ float Bs[32][33];
-  __shared__ __align__(16) float scratchS[4 * kScratchFloats];  // the SIMT twin has 4 warps
-  const int t = threadIdx.x, n0 = blockIdx.y * 32;
-  float acc[32];
-#pragma unroll
-  for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-  const int K = g.k_total ? g.k_total : g.num_kb * 64;
-  for (int k0 = 0; k0 < K; k0 += 32) {
-    const int kk = t & 31;
-    for (int i = 0; i < 32; ++i) {
-      const int row = i * 4 + (t >> 5);
-      As[row][kk] = simt_load_a<CONV>(g, tc, row, k0 + kk);
-    }
-    for (int i = 0; i < 8; ++i) {
-      const int nn = i * 4 + (t >> 5);
-      float b = 0.f;
-      if (n0 + nn < g.N) {
-        const size_t off = static_cast<size_t>(n0 + nn + b_off) * g.ldb + k0 + kk;
-        b = __half2float(g.Bh[off]);
-        if (g.Bl) b += __half2float(g.Bl[off]);
-      }
-      Bs[nn][kk] = b;
-    }
-    __syncthreads();
-#pragma unroll 4
-    for (int k = 0; k < 32; ++k) {
-      const float a = As[t][k];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) acc[j] = fmaf(a, Bs[j][k], acc[j]);
-    }
-    __syncthreads();
-  }
-  epi(tc, t, n0, acc, scratchS + (t >> 5) * kScratchFloats);
-}
-
 // ------------------------------------------------------------------ launch
 struct TcOperands {
   CUtensorMap Ah, Al, Bh, Bl;
@@ -550,27 +485,15 @@ int launch_pers_auto(dimb_ctx* ctx, cudaStream_t st, const TcOperands& ops, cons
 // n_pad: output columns rounded up to a multiple of BN (B operand rows beyond N read as zero via TMA OOB fill).
 // CONV 1 / 2: ops.Ah/Al must be NHWC maps with a (ConvTile<CONV>::TH + 2) x kConvTW box (see dimb_tmap_nhwc callers).
 template <int BN, int CONV, class Epi>
-int launch_gemm(dimb_ctx* ctx, cudaStream_t st, const TcOperands& ops, GemmArgs g, const Epi& epi, int m_tiles, int n_pad,
+int launch_gemm(dimb_ctx* ctx, cudaStream_t st, const TcOperands& ops, const GemmArgs& g, const Epi& epi, int m_tiles, int n_pad,
                 const char* tag = "gemm", int force_split = -1) {
   // force_split: -1 = by the context's precision; 0 / 1 = operands known to be exactly fp16 (lo planes are zero: one MMA per
   // product IS exact) / to need the split regardless of the precision mode
   if (m_tiles <= 0) return DIMB_OK;
   ProfScope prof(ctx, st, tag);
-  if (ctx->use_tc) {
-    const bool exact = force_split < 0 ? ctx->precision == DIMB_PRECISION_EXACT : force_split != 0;
-    if (exact) return launch_pers_auto<BN, true, CONV, Epi>(ctx, st, ops, g, epi, m_tiles, n_pad);
-    return launch_pers_auto<BN, false, CONV, Epi>(ctx, st, ops, g, epi, m_tiles, n_pad);
-  }
-  if constexpr (CONV == 2) {
-    dimb_set_error(ctx, std::string(tag) + ": 16 x 16 conv tiles need the tensor-core kernel (DIMB_TC=0 runs 8 x 16 tiles)");
-    return DIMB_ERR_UNSUPPORTED;
-  } else {
-    if (force_split < 0 ? ctx->precision != DIMB_PRECISION_EXACT : force_split == 0) g.Al = g.Bl = nullptr;
-    dim3 grid(m_tiles, n_pad / 32);
-    simt_gemm_kernel<CONV, Epi><<<grid, 128, 0, st>>>(g, epi);
-    DIMB_LAUNCH_CHECK(ctx);
-    return DIMB_OK;
-  }
+  const bool exact = force_split < 0 ? ctx->precision == DIMB_PRECISION_EXACT : force_split != 0;
+  if (exact) return launch_pers_auto<BN, true, CONV, Epi>(ctx, st, ops, g, epi, m_tiles, n_pad);
+  return launch_pers_auto<BN, false, CONV, Epi>(ctx, st, ops, g, epi, m_tiles, n_pad);
 }
 
 // ------------------------------------------------------------------ generic epilogues

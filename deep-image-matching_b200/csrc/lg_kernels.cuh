@@ -276,47 +276,4 @@ inline int launch_lg_attention(dimb_ctx* ctx, cudaStream_t st, dim3 grid, const 
   return DIMB_OK;
 }
 
-// SIMT twin of the attention (debug path): warp per query row, online softmax over keys.
-__global__ void lg_attn_simt_kernel(AttnArgs a, const __half* __restrict__ qh, const __half* __restrict__ ql,
-                                    const __half* __restrict__ kh, const __half* __restrict__ kl, const __half* __restrict__ vth,
-                                    const __half* __restrict__ vtl) {
-  const int side = blockIdx.z, head = blockIdx.y, NP = a.rows.NP;
-  const int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  const int ks = a.cross ? (side ^ 1) : side;
-  if (a.rows.stopped[side >> 1] != 0) return;
-  const int nq = a.rows.n_act[side], nk = a.rows.n_act[ks];
-  if (q >= nq) return;
-  const size_t qo = ((static_cast<size_t>(side) * kHeads + head) * NP + q) * kHd;
-  float q0 = __half2float(qh[qo + lane]) + (ql ? __half2float(ql[qo + lane]) : 0.f);
-  float q1 = __half2float(qh[qo + lane + 32]) + (ql ? __half2float(ql[qo + lane + 32]) : 0.f);
-  float m = -INFINITY, l = 0.f, o0 = 0.f, o1 = 0.f;
-  for (int k = 0; k < nk; ++k) {
-    const size_t ko = ((static_cast<size_t>(ks) * kHeads + head) * NP + k) * kHd;
-    float d = q0 * (__half2float(kh[ko + lane]) + (kl ? __half2float(kl[ko + lane]) : 0.f)) +
-              q1 * (__half2float(kh[ko + lane + 32]) + (kl ? __half2float(kl[ko + lane + 32]) : 0.f));
-#pragma unroll
-    for (int o = 16; o; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
-    d *= a.scale;
-    const float mn = fmaxf(m, d), al = expf(m - mn), p = expf(d - mn);
-    const size_t vo = (static_cast<size_t>(ks) * kHeads + head) * kHd * NP + k;
-    const float v0 = __half2float(vth[vo + static_cast<size_t>(lane) * NP]) + (vtl ? __half2float(vtl[vo + static_cast<size_t>(lane) * NP]) : 0.f);
-    const float v1 = __half2float(vth[vo + static_cast<size_t>(lane + 32) * NP]) +
-                     (vtl ? __half2float(vtl[vo + static_cast<size_t>(lane + 32) * NP]) : 0.f);
-    l = l * al + p;
-    o0 = o0 * al + p * v0;
-    o1 = o1 * al + p * v1;
-    m = mn;
-  }
-  const size_t oo = (static_cast<size_t>(side) * NP + q) * kD + head * kHd;
-  const float r0 = nk ? o0 / l : 0.f, r1 = nk ? o1 / l : 0.f;
-  __half h, lo;
-  split_f32(r0, h, lo);
-  a.ctx_h[oo + lane] = h;
-  if (a.ctx_l) a.ctx_l[oo + lane] = lo;
-  split_f32(r1, h, lo);
-  a.ctx_h[oo + lane + 32] = h;
-  if (a.ctx_l) a.ctx_l[oo + lane + 32] = lo;
-}
-
-
 }  // namespace

@@ -576,8 +576,8 @@ int upload_f32(dimb_ctx* ctx, float** d, const float* src, size_t n) {
 }
 
 template <class Epi>
-int lg_gemm(dimb_lg* lg, cudaStream_t st, const CUtensorMap* A /*[2] hi,lo*/, const __half* Ah, const __half* Al, int lda, const Lin& w,
-            const Epi& epi, int m_tiles, const char* tag, bool wide = false, const CUtensorMap* A32 = nullptr) {
+int lg_gemm(dimb_lg* lg, cudaStream_t st, const CUtensorMap* A /*[2] hi,lo*/, const Lin& w, const Epi& epi, int m_tiles, const char* tag,
+            bool wide = false, const CUtensorMap* A32 = nullptr) {
   TcOperands ops;
   ops.Ah = A[0];
   ops.Al = A[1];
@@ -587,17 +587,11 @@ int lg_gemm(dimb_lg* lg, cudaStream_t st, const CUtensorMap* A /*[2] hi,lo*/, co
   g.num_kb = w.k / 64;
   g.M = lg->R;
   g.N = w.n;
-  g.Ah = Ah;
-  g.Al = Al;
-  g.Bh = w.wh;
-  g.Bl = w.wl;
-  g.lda = lda;
-  g.ldb = w.k;
   // 128 x 256 tiles (DIMB_BN256=1): per MMA k-step 30 KB of shared-memory traffic per 128 x 128 of output instead of 36 KB (the
   // 128 x 128 EXACT tile is bound by the shared-memory pipe - operand reads + TMA fill - at ~66 % of the tensor pipe)
   // (same-box A/B, 37 pairs: q/k projection 3.62 -> 3.07 ms, FFN0 4.66 -> 3.93 ms per step; no gain for the HBM-bound FFN3 and a loss
   // for the 256-wide out_proj, which stay on 128 x 128 tiles)
-  if (wide && lg->ctx->bn256 && w.has256 && lg->ctx->use_tc) {
+  if (wide && lg->ctx->bn256 && w.has256) {
     if (lg->ctx->k32 && A32) {  // four 48 KB stages instead of two 96 KB ones (gemm.cuh CONV 3)
       ops.Ah = A32[0], ops.Al = A32[1];
       ops.Bh = w.tmh256k32, ops.Bl = w.tml256k32;
@@ -622,15 +616,9 @@ int run_attention(dimb_lg* lg, cudaStream_t st, const LgRows& rows, int cross, i
   a.scale = 0.125f;  // hd^-0.5
   a.lazy = ctx->attn_lazy;
   ProfScope prof(ctx, st, cross ? "lg.attn_cross" : "lg.attn_self");
-  if (ctx->use_tc) {
-    dim3 grid(ceil_div(lg->NP, 2 * kTileM), kHeads, S);
-    const CUtensorMap* K = cross ? lg->m_q64 : lg->m_k64;
-    DIMB_TRY(launch_lg_attention(ctx, st, grid, lg->m_q128, K, lg->m_vt, a, exact));
-  } else {
-    dim3 grid(ceil_div(lg->NP * 32, 256), kHeads, S);
-    lg_attn_simt_kernel<<<grid, 256, 0, st>>>(a, lg->qh, exact ? lg->ql : nullptr, cross ? lg->qh : lg->kh,
-                                              exact ? (cross ? lg->ql : lg->kl) : nullptr, lg->vth, exact ? lg->vtl : nullptr);
-  }
+  dim3 grid(ceil_div(lg->NP, 2 * kTileM), kHeads, S);
+  const CUtensorMap* K = cross ? lg->m_q64 : lg->m_k64;
+  DIMB_TRY(launch_lg_attention(ctx, st, grid, lg->m_q128, K, lg->m_vt, a, exact));
   DIMB_LAUNCH_CHECK(ctx);
   return DIMB_OK;
 }
@@ -898,7 +886,7 @@ int dimb_lg_match_dev(dimb_lg* lg, int P, const dimb_feats_dev* f0, const dimb_f
     e.xl = exact ? lg->xl[0] : nullptr;
     e.bias = lg->inproj.bias;
     e.residual = 0;
-    DIMB_TRY(lg_gemm(lg, st, lg->m_xin, lg->xinh, lg->xinl, din, lg->inproj, e, m_tiles, "lg.input_proj"));
+    DIMB_TRY(lg_gemm(lg, st, lg->m_xin, lg->inproj, e, m_tiles, "lg.input_proj"));
   }
 
   for (int i = 0; i < L; ++i) {
@@ -933,18 +921,12 @@ int dimb_lg_match_dev(dimb_lg* lg, int P, const dimb_feats_dev* f0, const dimb_f
         g.num_kb = d / 64;
         g.M = lg->R;
         g.N = blk ? d : 2 * d;
-        g.Ah = lg->xh[cur];
-        g.Al = lg->xl[cur];
-        g.Bh = qkv.wh;
-        g.Bl = qkv.wl;
-        g.lda = 2 * d;
-        g.ldb = d;
-        if (ctx->bn256 && qkv.has256 && ctx->use_tc && ctx->k32) {
+        if (ctx->bn256 && qkv.has256 && ctx->k32) {
           ops.Ah = lg->m_x32[cur][0], ops.Al = lg->m_x32[cur][1];
           ops.Bh = qkv.tmh256k32, ops.Bl = qkv.tml256k32;
           g.num_kb = d / 32;
           DIMB_TRY((launch_gemm<256, 3>(ctx, st, ops, g, e, m_tiles, blk ? d : 2 * d, "lg.qk")));
-        } else if (ctx->bn256 && qkv.has256 && ctx->use_tc) {
+        } else if (ctx->bn256 && qkv.has256) {
           ops.Bh = qkv.tmh256;
           ops.Bl = qkv.tml256;
           DIMB_TRY((launch_gemm<256, false>(ctx, st, ops, g, e, m_tiles, blk ? d : 2 * d, "lg.qk")));
@@ -969,12 +951,6 @@ int dimb_lg_match_dev(dimb_lg* lg, int P, const dimb_feats_dev* f0, const dimb_f
         g.num_kb = d / 64;
         g.M = qkv.n;
         g.N = R;
-        g.Ah = qkv.wh;
-        g.Al = qkv.wl;
-        g.Bh = lg->xh[cur];
-        g.Bl = lg->xl[cur];
-        g.lda = d;
-        g.ldb = 2 * d;
         DIMB_TRY((launch_gemm<128, false>(ctx, st, ops, g, e, 2, R, "lg.vT")));
       }
       DIMB_TRY(run_attention(lg, st, rows, blk, S));
@@ -986,7 +962,7 @@ int dimb_lg_match_dev(dimb_lg* lg, int P, const dimb_feats_dev* f0, const dimb_f
         e.bias = outp.bias;
         e.ldc = 2 * d;
         e.col_off = d;
-        DIMB_TRY(lg_gemm(lg, st, lg->m_ctx, lg->ctxh, lg->ctxl, d, outp, e, m_tiles, "lg.out_proj"));
+        DIMB_TRY(lg_gemm(lg, st, lg->m_ctx, outp, e, m_tiles, "lg.out_proj"));
       }
       {
         EpiLgF32 e;
@@ -994,7 +970,7 @@ int dimb_lg_match_dev(dimb_lg* lg, int P, const dimb_feats_dev* f0, const dimb_f
         e.out = lg->h1;
         e.bias = f0.bias;
         e.ldc = 2 * d;
-        DIMB_TRY(lg_gemm(lg, st, lg->m_x[cur], lg->xh[cur], lg->xl[cur], 2 * d, f0, e, m_tiles, "lg.ffn0", true, lg->m_x32[cur]));
+        DIMB_TRY(lg_gemm(lg, st, lg->m_x[cur], f0, e, m_tiles, "lg.ffn0", true, lg->m_x32[cur]));
       }
       {
         ProfScope prof_ln(ctx, st, "lg.ln_gelu");
@@ -1010,7 +986,7 @@ int dimb_lg_match_dev(dimb_lg* lg, int P, const dimb_feats_dev* f0, const dimb_f
         e.xl = exact ? lg->xl[cur] : nullptr;
         e.bias = f3.bias;
         e.residual = 1;
-        DIMB_TRY(lg_gemm(lg, st, lg->m_h2, lg->h2h, lg->h2l, 2 * d, f3, e, m_tiles, "lg.ffn3"));
+        DIMB_TRY(lg_gemm(lg, st, lg->m_h2, f3, e, m_tiles, "lg.ffn3"));
       }
     }
     if (i == L - 1 || !adaptive) continue;  // no early stopping or adaptive width at the last layer (lightglue.py:494)
@@ -1053,13 +1029,7 @@ int dimb_lg_match_dev(dimb_lg* lg, int P, const dimb_feats_dev* f0, const dimb_f
     GemmArgs g{};
     g.num_kb = d / 64;
     g.M = R;
-    g.N = L * d;  // SIMT bound on B rows (offset included)
-    g.Ah = lg->fh;
-    g.Al = lg->fl;
-    g.Bh = lg->fproj.wh;
-    g.Bl = lg->fproj.wl;
-    g.lda = d;
-    g.ldb = d;
+    g.N = L * d;  // B rows: the stacked projections of all L layers, b_row_offset picks a pair's layer
     DIMB_TRY((launch_gemm<128, false>(ctx, st, ops, g, e, m_tiles, d, "lg.final_proj")));
   }
   {
@@ -1077,12 +1047,6 @@ int dimb_lg_match_dev(dimb_lg* lg, int P, const dimb_feats_dev* f0, const dimb_f
     g.num_kb = d / 64;
     g.M = R;
     g.N = R;
-    g.Ah = lg->mdh;
-    g.Al = lg->mdl;
-    g.Bh = lg->mdh;
-    g.Bl = lg->mdl;
-    g.lda = d;
-    g.ldb = d;
     DIMB_TRY((launch_gemm<128, false>(ctx, st, ops, g, e, P * (NP / kTileM), NP, "lg.sim")));
   }
   ProfScope prof_asg(ctx, st, "lg.assign_reduce");

@@ -214,7 +214,7 @@ int lgx_create(dimb_ctx* ctx, const float* weights, size_t n_floats, const dimb_
   DIMB_TRY(dimb_alloc_t(ctx, &g->arg0, NP));
   DIMB_TRY(dimb_alloc_t(ctx, &g->arg1, NP));
   DIMB_TRY(dimb_alloc_t(ctx, &g->idx, NP));
-  // head dims 65..128 (LighterGlue: 96): attention on the tensor cores (attn_hd128.cuh); DIMB_TC=0 keeps the fp32 kernel
+  // head dims 65..128 (LighterGlue: 96): attention on the tensor cores (attn_hd128.cuh); other head dims run the fp32 kernel
   g->tc_attn = hd > 64 && hd <= kXHd;
   if (g->tc_attn) {
     g->NPp = (g->NP + kAttnTile - 1) / kAttnTile * kAttnTile;
@@ -305,7 +305,7 @@ static int lgx_match_pair(dimb_lgx* g, const dimb_feats& f0, const dimb_feats& f
     DIMB_CUDA_OK(ctx, cudaStreamSynchronize(st));  // desc_in / kpts are reused by the other side
   }
   const bool do_stop = cf.depth_confidence > 0, do_prune = cf.width_confidence > 0;
-  const bool tc = g->tc_attn && ctx->use_tc;
+  const bool tc = g->tc_attn;
   const int m_total = n[0] + n[1];
   std::vector<float> tok[2], sc;
   bool have_tok = false;

@@ -179,10 +179,8 @@ __global__ void nn_prep_kernel(const NNSideIn* __restrict__ in, int mode, int D,
 
 // warp per row of the sides 2p + swap (rows_pp rows per pair in the grid; rows past the live count exit): merge the chunk partials
 // that hold a live column of the partner, chunks [0, ceil(n / 32)) -> best, second, arg (first index wins ties) at row side * NPp + row
-// of d1 / d2 / i1.  Only those chunks are written on every path: the CUDA-core twin of the GEMM (DIMB_TC=0) has 32-column tiles and
-// skips the ones past the partner's count, and the chunks past them in a 128-column tensor-core tile are all +inf, which changes no
-// result.  The partials are squared distances, the comparison happens on the distances (clamp at 0, IEEE sqrt) like torch.cdist + min /
-// topk.
+// of d1 / d2 / i1.  The chunks past them in a 128-column tile are all +inf and would change no result.  The partials are squared
+// distances, the comparison happens on the distances (clamp at 0, IEEE sqrt) like torch.cdist + min / topk.
 __global__ void nn_merge_kernel(const float* __restrict__ pd1, const float* __restrict__ pd2, const int* __restrict__ pi1,
                                 const int* __restrict__ n_live, int P, int NPp, int rows_pp, int swap, int stride, float* __restrict__ d1,
                                 float* __restrict__ d2, int* __restrict__ i1) {
@@ -365,18 +363,11 @@ int nn_workspace(dimb_ctx* ctx, const NNShape& sh, int D, bool want_lo, NNWork* 
 // rows of sides 2p + d against sides 2p + 1 - d: top-2 GEMM of every pair, then the merge
 int nn_direction(dimb_ctx* ctx, cudaStream_t st, const NNWork& w, const NNShape& sh, int d, bool split) {
   const TcOperands ops{w.mA[d][0], w.mA[d][1], w.mB[d][0], w.mB[d][1]};
-  const size_t a_off = sh.host ? static_cast<size_t>(d) * sh.NPp * w.Dp : 0, b_off = sh.host ? static_cast<size_t>(d ^ 1) * sh.NPp * w.Dp : 0;
   const int m_tiles = sh.P * sh.tps[d], stride = sh.npad[d] / 32;
   GemmArgs g{};
   g.num_kb = w.Dp / 64;
   g.M = sh.host ? sh.hn[d] : 2 * sh.P * sh.NPp;
   g.N = sh.npad[d];
-  g.Ah = w.hi + a_off;
-  g.Al = w.lo ? w.lo + a_off : nullptr;
-  g.Bh = w.hi + b_off;
-  g.Bl = w.lo ? w.lo + b_off : nullptr;
-  g.lda = w.Dp;
-  g.ldb = w.Dp;
   // descriptors that are exactly fp16 (everything read back from features.h5 is) have zero lo planes: ONE MMA per product is
   // exact, and (host counts) the 256-descriptor B panel (128 KB) stays resident in shared memory while the A tiles stream
   if (sh.host) {

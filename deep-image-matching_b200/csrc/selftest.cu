@@ -1,6 +1,6 @@
 // selftest.cu - test infrastructure of libdimb200_selftest.so, used by tests/ to validate kernels in isolation from the model code:
 //   dimb_selftest_gemm / dimb_selftest_conv3x3: the persistent tensor-core GEMM (gemm.cuh) through its production launch, as a plain
-//     C = A B^T and as the SuperPoint 3x3 conv layer (conv3x3.cuh), or their SIMT twin (DIMB_TC=0);
+//     C = A B^T and as the SuperPoint 3x3 conv layer (conv3x3.cuh);
 //   dimb_selftest_gemm_plan: the launch plan of the persistent kernel, host only;
 //   dimb_selftest_attention: the flash-attention kernels through their production launches;
 //   dimb_selftest_detect: simple_nms, candidate compaction and top-k (detect.cuh) through their production launches;
@@ -29,11 +29,11 @@ int run_conv3_mode(dimb_ctx* ctx, const ConvLayer& L, const __half* xh, const __
 }
 
 // gemm.cuh CONV mode of a conv3x3 self-test call: tile 0 = the production choice (conv_mode), 8 = 8 x 16 tiles, 16 = 16 x 16 tiles
-// (cout 64 on the tensor-core kernel); -1 when the tile cannot run
+// (cout 64 only); -1 when the tile cannot run
 int selftest_conv_mode(dimb_ctx* ctx, int tile, int cout, int B, int H, int W) {
-  if (tile == 0) return conv_mode(cout, ctx->use_tc, B, H, W, ctx->num_sms);
+  if (tile == 0) return conv_mode(cout, B, H, W, ctx->num_sms);
   if (tile == 8) return 1;
-  if (tile == 16 && conv_bn(cout) == 64 && ctx->use_tc) return 2;
+  if (tile == 16 && conv_bn(cout) == 64) return 2;
   return -1;
 }
 
@@ -119,13 +119,9 @@ void plan_of(bool split, bool const_b, int num_kb, int m_tiles, int n_tiles, int
   out[4] = p.grid;
 }
 
-// the plan the persistent kernel of ctx runs with; -1s on the SIMT twin, which has none
+// the plan the persistent kernel of ctx runs with
 void launch_plan(dimb_ctx* ctx, int conv, int bn, bool const_b, int num_kb, int m_tiles, int n_tiles, int* out) {
   if (!out) return;
-  if (!ctx->use_tc) {
-    std::fill(out, out + 5, -1);
-    return;
-  }
   dimb_selftest_gemm_plan(conv, bn, ctx->precision == DIMB_PRECISION_EXACT, const_b, num_kb, m_tiles, n_tiles, ctx->num_sms, out);
 }
 }  // namespace
@@ -154,7 +150,7 @@ extern "C" int dimb_selftest_gemm_plan(int conv, int bn, int split, int const_b,
 //   blocks on SWIZZLE_64B maps (gemm.cuh CONV 3, bn 256), as the LightGlue linears run with DIMB_K32=1.
 //   The tensor maps have exactly M and N rows, over allocations padded to whole tiles whose extra rows hold `guard`: rows past M / N
 //   reach the MMAs only as TMA out-of-bounds fill.  C [M + 128][N] starts as `guard` everywhere: the M output rows, then a tail that
-//   must stay untouched.  plan[5] (may be null): {resb, sa, sb, smem_bytes, grid} of the launch, -1s on the SIMT twin.
+//   must stay untouched.  plan[5] (may be null): {resb, sa, sb, smem_bytes, grid} of the launch.
 extern "C" int dimb_selftest_gemm(dimb_ctx* ctx, const float* A, const float* B, const float* bias, float* C, int M, int N, int K, int bn,
                                   int k32, float guard, int* plan) {
   if (!ctx || !A || !B || !C || K < 64 || K % 64 || M < 1 || N < 1) return DIMB_ERR_ARG;
@@ -180,15 +176,8 @@ extern "C" int dimb_selftest_gemm(dimb_ctx* ctx, const float* A, const float* B,
   DIMB_TRY(tmap(ctx, &ops.Bl, bl, N, K, K, bn));
   GemmArgs g{};
   g.num_kb = K / (k32 ? 32 : 64);
-  g.k_total = K;
   g.M = M;
   g.N = N;
-  g.Ah = ah;
-  g.Al = al;
-  g.Bh = bh;
-  g.Bl = bl;
-  g.lda = K;
-  g.ldb = K;
   EpiStoreF32 e;
   e.out = dC;
   e.bias = d_bias;
@@ -217,8 +206,8 @@ extern "C" int dimb_selftest_gemm(dimb_ctx* ctx, const float* A, const float* B,
 //   past the last image, or across the image boundary, would bring it in.  `guard` must be finite: the ReLU turns NaN into 0.
 //   out: [B + 1][Ho][Wo][cout] with Ho, Wo = H / 2, W / 2 under pool: the B output images joined from their hi + lo planes (hi only in
 //   FAST), then one image of tail; every element starts as `sentinel` (fp16-exact), so unwritten and stray writes show.
-//   tile: 0 = the tile shape production picks for this call (conv3x3.cuh conv_mode), 8 = 8 x 16 pixels, 16 = 16 x 16 pixels (cout 64,
-//   tensor-core kernel only).
+//   tile: 0 = the tile shape production picks for this call (conv3x3.cuh conv_mode), 8 = 8 x 16 pixels, 16 = 16 x 16 pixels
+//   (cout 64 only).
 //   plan[6] (may be null): as dimb_selftest_gemm, then the gemm.cuh CONV mode that ran (1 or 2).
 extern "C" int dimb_selftest_conv3x3(dimb_ctx* ctx, const float* x, const float* w, const float* bias, float* out, int B, int H, int W,
                                      int cin, int cout, int pool, int tile, float guard, float sentinel, int* plan) {
@@ -267,10 +256,10 @@ extern "C" int dimb_selftest_conv3x3(dimb_ctx* ctx, const float* x, const float*
 }
 
 // Host only: the gemm.cuh CONV mode (tile shape) run_conv3 picks for a conv of B images of H x W with `cout` output channels on a
-// device with num_sms SMs (conv3x3.cuh conv_mode), tensor-core kernel, either precision.
+// device with num_sms SMs (conv3x3.cuh conv_mode), either precision.
 extern "C" int dimb_selftest_conv_mode(int cout, int B, int H, int W, int num_sms, int* out) {
   if (!out || B < 1 || H < 1 || W < 1 || num_sms < 1 || cout < 1) return DIMB_ERR_ARG;
-  *out = conv_mode(cout, true, B, H, W, num_sms);
+  *out = conv_mode(cout, B, H, W, num_sms);
   return DIMB_OK;
 }
 
@@ -375,19 +364,14 @@ int selftest_attention_lg(dimb_ctx* ctx, const float* Q, const float* K, const f
   a.scale = 0.125f;  // hd^-0.5
   a.lazy = lazy;
   const __half *kh_ = cross ? qh : kh, *kl_ = cross ? ql : kl;  // cross: keys = the q rows of the other side (shared to_qk)
-  if (ctx->use_tc) {  // tensor maps as lightglue.cu builds them: Q box 128 rows, K box 64 rows, V^T box 64 rows
-    CUtensorMap mq[2], mk[2], mv[2];
-    const uint64_t rows = static_cast<uint64_t>(S) * kHeads * NP;
-    for (int pl = 0; pl < 2; ++pl) {
-      DIMB_TRY(dimb_tmap_2d(ctx, &mq[pl], pl ? ql : qh, rows, kHd, kHd, kTileM));
-      DIMB_TRY(dimb_tmap_2d(ctx, &mk[pl], pl ? kl_ : kh_, rows, kHd, kHd, kBlkK));
-      DIMB_TRY(dimb_tmap_2d(ctx, &mv[pl], pl ? vl : vh, static_cast<uint64_t>(S) * kHeads * kHd, NP, NP, kHd));
-    }
-    DIMB_TRY(launch_lg_attention(ctx, 0, dim3(1, kHeads, S), mq, mk, mv, a, exact));
-  } else {
-    lg_attn_simt_kernel<<<dim3(ceil_div(NP * 32, 256), kHeads, S), 256>>>(a, qh, exact ? ql : nullptr, kh_, exact ? kl_ : nullptr, vh,
-                                                                          exact ? vl : nullptr);
+  CUtensorMap mq[2], mk[2], mv[2];  // as lightglue.cu builds them: Q box 128 rows, K box 64 rows, V^T box 64 rows
+  const uint64_t rows = static_cast<uint64_t>(S) * kHeads * NP;
+  for (int pl = 0; pl < 2; ++pl) {
+    DIMB_TRY(dimb_tmap_2d(ctx, &mq[pl], pl ? ql : qh, rows, kHd, kHd, kTileM));
+    DIMB_TRY(dimb_tmap_2d(ctx, &mk[pl], pl ? kl_ : kh_, rows, kHd, kHd, kBlkK));
+    DIMB_TRY(dimb_tmap_2d(ctx, &mv[pl], pl ? vl : vh, static_cast<uint64_t>(S) * kHeads * kHd, NP, NP, kHd));
   }
+  DIMB_TRY(launch_lg_attention(ctx, 0, dim3(1, kHeads, S), mq, mk, mv, a, exact));
   float* d_out;
   DIMB_TRY(t.get(&d_out, R * kD));
   join_rows_kernel<<<ceil_div(static_cast<int>(R * kD), 256), 256>>>(ch, exact ? cl : nullptr, d_out, R * kD);
@@ -399,10 +383,6 @@ int selftest_attention_lg(dimb_ctx* ctx, const float* Q, const float* K, const f
 // shape-generic attention (attn_hd128.cuh) on operands packed by the production packers at NP rounded up to the query tile
 int selftest_attention_hd128(dimb_ctx* ctx, const float* Q, const float* K, const float* V, float* out, int H, int hd, int NP, const int* n,
                              float lazy, float pad, float out_pad) {
-  if (!ctx->use_tc) {
-    dimb_set_error(ctx, "dimb_selftest_attention: variant 1 is the tensor-core kernel (DIMB_TC=0 runs the fp32 kernel of the generic path)");
-    return DIMB_ERR_UNSUPPORTED;
-  }
   const bool exact = ctx->precision == DIMB_PRECISION_EXACT;
   const int NPp = round_up(NP, kAttnTile), ld = H * hd;
   const size_t nel = static_cast<size_t>(NPp) * ld, pl_el = static_cast<size_t>(H) * NPp * kXHd;
@@ -445,8 +425,8 @@ int selftest_attention_hd128(dimb_ctx* ctx, const float* Q, const float* K, cons
 }  // namespace
 
 // Flash attention (attention.cuh) through its production launches, on host fp32 operands; precision from ctx.
-//   variant 0: lg_attn_kernel (LightGlue / SuperGlue, H = 4 heads of hd = 64) via launch_lg_attention, or its SIMT twin
-//     lg_attn_simt_kernel when ctx->use_tc == 0.  Q, K, V [S][4][NP][64] (S even, NP a multiple of 128), live rows n[S], stopped[S / 2]
+//   variant 0: lg_attn_kernel (LightGlue / SuperGlue, H = 4 heads of hd = 64) via launch_lg_attention.  Q, K, V [S][4][NP][64] (S even,
+//     NP a multiple of 128), live rows n[S], stopped[S / 2]
 //     (nonzero: the pair is stopped); cross: the keys of side s are the q rows of side s ^ 1 (K unused, may be null).  out: the
 //     context buffer [S * NP][256], hi + lo planes (hi only in FAST), every row.
 //   variant 1: gx_attn_tc_kernel (head dim hd <= 128, even, padded to 128) via launch_attn_hd128, operands packed by
@@ -486,11 +466,11 @@ extern "C" int dimb_selftest_attention(dimb_ctx* ctx, int variant, const float* 
 namespace {
 constexpr int kDetTail = 1024;  // elements past the last valid one in every output buffer of these entries
 
-// nms_plan version of a self-test cut: 0 = the production choice (prod_ver: ctx->nms_ver), 1 = first cut, 2 = bit-mask kernel
+// nms_plan version of a self-test cut: 0 = the production choice (kNmsProductionVer), 1 = first cut, 2 = bit-mask kernel
 // (radii 1..5 only); -1 when the cut cannot run at radius r
-int selftest_nms_ver(int r, int cut, int prod_ver) {
+int version_of_cut(int r, int cut) {
   if (r < 0 || r > 8) return -1;
-  if (cut == 0) return prod_ver;
+  if (cut == 0) return kNmsProductionVer;
   if (cut == 1) return 1;
   if (cut == 2 && r >= 1 && r <= 5) return 2;
   return -1;
@@ -517,11 +497,11 @@ int download(dimb_ctx* ctx, T* host, const T* dev, size_t n) {
 }
 }  // namespace
 
-// Launch plan of simple_nms at radius r (detect.cuh nms_plan), host only.  cut 0: the production choice of a default context (bit-mask
-// kernel for radii 1..5, first cut otherwise), 1: the first cut (sp_nms_kernel, radii 0..8), 2: the bit-mask kernel (sp_nms2_kernel,
+// Launch plan of simple_nms at radius r (detect.cuh nms_plan), host only.  cut 0: the production choice (bit-mask kernel for radii
+// 1..5, first cut otherwise), 1: the first cut (sp_nms_kernel, radii 0..8), 2: the bit-mask kernel (sp_nms2_kernel,
 // radii 1..5).  out[4] = {kernel (1 first cut, 2 bit-mask), tile, threads, dynamic shared memory bytes}.
 extern "C" int dimb_selftest_nms_plan(int r, int cut, int* out) {
-  const int ver = selftest_nms_ver(r, cut, 2);
+  const int ver = version_of_cut(r, cut);
   if (!out || ver < 0) return DIMB_ERR_ARG;
   plan_out(nms_plan(r, ver), out);
   return DIMB_OK;
@@ -529,7 +509,7 @@ extern "C" int dimb_selftest_nms_plan(int r, int cut, int* out) {
 
 // simple_nms, candidate compaction and top-k (detect.cuh) through the launch helpers SuperPoint and ALIKED run, on host fp32 scores
 // [B][H][W] (positive: the select kernel orders scores by their bits).
-//   r, cut: radius and kernel as dimb_selftest_nms_plan, except that cut 0 follows the context (DIMB_NMS=1 selects the first cut).
+//   r, cut: radius and kernel as dimb_selftest_nms_plan.
 //   thr >= 0: candidates are nms > thr; thr_per_image [B] (may be null) replaces it through the device-threshold argument, as ALIKED
 //   passes its threshold.  border: candidates lie at least `border` pixels inside the image.  K: top-k (-1 keeps every candidate, in
 //   row-major order), 1..kMaxTopK; cap >= K: selection slots per image.
@@ -545,7 +525,7 @@ extern "C" int dimb_selftest_detect(dimb_ctx* ctx, const float* scores, int B, i
   if (thr_per_image)
     for (int b = 0; b < B; ++b)
       if (!(thr_per_image[b] >= 0.f)) return DIMB_ERR_ARG;
-  const int ver = selftest_nms_ver(r, cut, ctx->nms_ver);
+  const int ver = version_of_cut(r, cut);
   if (ver < 0) return DIMB_ERR_ARG;
   DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
   const int HW = H * W, nch = ceil_div(HW, kChunk);

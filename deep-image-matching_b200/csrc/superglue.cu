@@ -20,8 +20,7 @@
 //   matches  : row / column max and first argmax of the log assignment, then one CTA per pair for the mutual check, the threshold
 //              and the ordered compaction into the [P][cap] tables of dimb_lg_match_dev
 // Done once at create time: BatchNorm folding, and the reference's (dim, heads)-interleaved channel order of `view(b, dim, heads, n)`
-// (:111-113) permuted to head-major.  dimb_sg_match stages one host pair and runs the same engine with P = 1; its plain fp32 twin of
-// the GNN and Sinkhorn (DIMB_TC=0) remains as the debug path of that host entry.
+// (:111-113) permuted to head-major.  dimb_sg_match stages one host pair and runs the same engine with P = 1.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -181,32 +180,6 @@ __global__ void sg_sink_rows_kernel(const float* __restrict__ S, int ld, size_t 
   if (lane == 0) out[static_cast<size_t>(p) * vld + i] = ((i == m) ? norm + log_bin : norm) - (mx + logf(s));
 }
 
-// couplings (:175-177): fill the dustbin row / column of the (m+1) x (n+1) matrix with alpha (plain fp32 twin)
-__global__ void sg_fill_bins_kernel(float* __restrict__ Z, int ld, int m, int n, const float* __restrict__ alpha) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const float a = alpha[0];
-  if (i <= n) Z[static_cast<size_t>(m) * ld + i] = a;
-  if (i < m) Z[static_cast<size_t>(i) * ld + n] = a;
-}
-
-// One Sinkhorn half step of the plain fp32 twin (:158-165) on the materialised (m+1) x (n+1) couplings: out[i] = log_marg(i) -
-// logsumexp_j(Z[i][j] + add[j]) over rows (dir 0) or columns (dir 1); log_marg = norm, norm + log(other count) for the dustbin.
-__global__ void sg_sinkhorn_kernel(const float* __restrict__ Z, int ld, int m1, int n1, int dir, const float* __restrict__ add,
-                                   float* __restrict__ out, const float* __restrict__ pc) {
-  const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  const int cnt = dir == 0 ? m1 : n1, len = dir == 0 ? n1 : m1;
-  if (i >= cnt) return;
-  float mx = -INFINITY;
-  for (int j = lane; j < len; j += 32) mx = fmaxf(mx, (dir == 0 ? Z[static_cast<size_t>(i) * ld + j] : Z[static_cast<size_t>(j) * ld + i]) + add[j]);
-#pragma unroll
-  for (int of = 16; of; of >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, of));
-  float s = 0.f;
-  for (int j = lane; j < len; j += 32) s += expf((dir == 0 ? Z[static_cast<size_t>(i) * ld + j] : Z[static_cast<size_t>(j) * ld + i]) + add[j] - mx);
-#pragma unroll
-  for (int of = 16; of; of >>= 1) s += __shfl_xor_sync(0xffffffffu, s, of);
-  if (lane == 0) out[i] = ((i == cnt - 1) ? pc[0] + pc[1 + dir] : pc[0]) - (mx + logf(s));
-}
-
 // Row maximum and first argmax of Z[i][j] + u[i] + v[j] - norm over the inner m x n block of every pair (:279-280): warp per row,
 // grid (ceil(NPs * 32 / 256), P); results at [p * NPs + i].
 __global__ void sg_row_max_kernel(const float* __restrict__ Z, int ld, size_t pstride, const int* __restrict__ n_act, const float* __restrict__ u,
@@ -323,9 +296,6 @@ struct SgTcLin {  // fp16 hi/lo planes [n][k] + fp32 bias + TMA maps (boxes of 1
 struct SgTcLayer {
   SgTcLin qkv, merge, mlp0, mlp3;  // qkv = [Wq ; Wk ; Wv] stacked (768 x 256), head-major rows
 };
-struct SgLayer {
-  SgLin q, k, v, merge, mlp0, mlp3;
-};
 
 }  // namespace
 
@@ -336,8 +306,6 @@ struct dimb_sg {
   int NP, L, max_pairs;
   std::vector<int> cross;  // per GNN layer: 1 = cross, 0 = self
   SgLin kenc[5];
-  std::vector<SgLayer> layers;
-  SgLin final_proj;
   float* bin_score;
   // ---- batched engine (side s = rows [s * NPt, (s + 1) * NPt) of every token buffer, NPt = NP rounded up to 128)
   int NPt = 0, vld = 0, wave = 1;  // vld: pitch of the per-pair u / v vectors; wave: pairs per Sinkhorn launch (L2-resident blocks)
@@ -351,26 +319,16 @@ struct dimb_sg {
   float *pc = nullptr, *uu = nullptr, *vv = nullptr, *best0 = nullptr;  // pc [P][4] Sinkhorn constants, uu / vv [P][vld]
   int *arg0 = nullptr, *arg1 = nullptr;                                 // best0 / arg0 / arg1 [P][NPt]
   CUtensorMap m_x[2], m_ctx[2], m_h2[2], m_md[2], m_q128[2], m_k64[2], m_vt[2];
-  // ---- host entry: staging of one host pair, output tables, plain fp32 twin of the GNN and Sinkhorn (DIMB_TC=0)
+  // ---- host entry: staging of one host pair, output tables
   float *st_kp = nullptr, *st_sc = nullptr, *st_desc = nullptr;
   int* st_n = nullptr;
   int64_t* o_m = nullptr;
   float* o_ms = nullptr;
   int* o_nm = nullptr;
   int o_cap = 0;
-  float *cat = nullptr, *q[2], *k[2], *v[2], *att, *hid, *md[2], *Z;
 };
 
 namespace {
-
-int sg_linear(dimb_sg* g, cudaStream_t st, const float* A, int lda, const SgLin& l, float* C, int ldc, int M, int relu, float scale = 1.f,
-              const float* resid = nullptr, int ldr = 0) {
-  if (M <= 0) return DIMB_OK;
-  dim3 grid(ceil_div(l.n, 64), ceil_div(M, 64));
-  gx_linear_kernel<<<grid, 256, 0, st>>>(A, lda, l.w, l.k, l.b, C, ldc, M, l.n, l.k, scale, resid, ldr, relu);
-  DIMB_LAUNCH_CHECK(g->ctx);
-  return DIMB_OK;
-}
 
 // host-side weight preparation: 1x1 conv [n][k] (+ optional eval BatchNorm folded in), optional row / column permutations
 struct HostLin {
@@ -438,8 +396,7 @@ int upload(dimb_ctx* ctx, SgLin& d, const HostLin& h) {
 
 // one GEMM over the token rows of all S sides: C = A [S * NPt][K] * W^T on the wgmma kernel of gemm.cuh with epilogue `epi`
 template <class Epi>
-int sg_tc_gemm(dimb_sg* g, cudaStream_t st, int S, const CUtensorMap* A, const __half* Ah, const __half* Al, int lda, const SgTcLin& w,
-               int n_out, const Epi& epi, const char* tag) {
+int sg_tc_gemm(dimb_sg* g, cudaStream_t st, int S, const CUtensorMap* A, const SgTcLin& w, int n_out, const Epi& epi, const char* tag) {
   TcOperands ops;
   ops.Ah = A[0];
   ops.Al = A[1];
@@ -449,12 +406,6 @@ int sg_tc_gemm(dimb_sg* g, cudaStream_t st, int S, const CUtensorMap* A, const _
   ga.num_kb = w.k / 64;
   ga.M = S * g->NPt;
   ga.N = n_out;
-  ga.Ah = Ah;
-  ga.Al = Al;
-  ga.Bh = w.wh;
-  ga.Bl = w.wl;
-  ga.lda = lda;
-  ga.ldb = w.k;
   return launch_gemm<128, false>(g->ctx, st, ops, ga, epi, S * g->NPt / kTileM, n_out, tag);
 }
 
@@ -496,7 +447,7 @@ int sg_gnn_tc(dimb_sg* g, cudaStream_t st, int P) {
       e.cs = e.sn = nullptr;
       e.qh = g->qh, e.ql = exact ? g->ql : nullptr, e.kh = g->kh, e.kl = exact ? g->kl : nullptr;
       e.cross = 1;
-      DIMB_TRY(sg_tc_gemm(g, st, S, g->m_x, g->xh, g->xl, 2 * d, ly.qkv, 2 * d, e, "sg.qk"));
+      DIMB_TRY(sg_tc_gemm(g, st, S, g->m_x, ly.qkv, 2 * d, e, "sg.qk"));
     }
     {  // V^T: weights as the A operand (rows 512..767 of the stacked projection), tokens as B
       EpiVT e;
@@ -509,8 +460,6 @@ int sg_gnn_tc(dimb_sg* g, cudaStream_t st, int P) {
       GemmArgs ga{};
       ga.num_kb = d / 64;
       ga.M = ly.qkv.n, ga.N = R;
-      ga.Ah = ly.qkv.wh, ga.Al = ly.qkv.wl, ga.Bh = g->xh, ga.Bl = g->xl;
-      ga.lda = d, ga.ldb = 2 * d;
       DIMB_TRY((launch_gemm<128, false>(ctx, st, ops, ga, e, 2, R, "sg.vT")));
     }
     {  // attention: self layers attend to their own side, cross layers to the keys AND values of the other side
@@ -531,7 +480,7 @@ int sg_gnn_tc(dimb_sg* g, cudaStream_t st, int P) {
       e.hi = g->xh, e.lo = exact ? g->xl : nullptr;
       e.bias = ly.merge.bias;
       e.ldc = 2 * d, e.col_off = d;
-      DIMB_TRY(sg_tc_gemm(g, st, S, g->m_ctx, g->ctxh, g->ctxl, d, ly.merge, d, e, "sg.merge"));
+      DIMB_TRY(sg_tc_gemm(g, st, S, g->m_ctx, ly.merge, d, e, "sg.merge"));
     }
     {  // MLP0 (BatchNorm folded) + ReLU
       EpiSgReluSplit e;
@@ -539,7 +488,7 @@ int sg_gnn_tc(dimb_sg* g, cudaStream_t st, int P) {
       e.hi = g->h2h, e.lo = exact ? g->h2l : nullptr;
       e.bias = ly.mlp0.bias;
       e.ldc = 2 * d;
-      DIMB_TRY(sg_tc_gemm(g, st, S, g->m_x, g->xh, g->xl, 2 * d, ly.mlp0, 2 * d, e, "sg.mlp0"));
+      DIMB_TRY(sg_tc_gemm(g, st, S, g->m_x, ly.mlp0, 2 * d, e, "sg.mlp0"));
     }
     {  // x += MLP3(...)
       EpiLgResidual e;
@@ -548,7 +497,7 @@ int sg_gnn_tc(dimb_sg* g, cudaStream_t st, int P) {
       e.xh = g->xh, e.xl = exact ? g->xl : nullptr;
       e.bias = ly.mlp3.bias;
       e.residual = 1;
-      DIMB_TRY(sg_tc_gemm(g, st, S, g->m_h2, g->h2h, g->h2l, 2 * d, ly.mlp3, d, e, "sg.mlp3"));
+      DIMB_TRY(sg_tc_gemm(g, st, S, g->m_h2, ly.mlp3, d, e, "sg.mlp3"));
     }
   }
   {  // mdesc = final_proj(x) / 256^0.25 on each side, so that the score block is mdesc0 . mdesc1^T / sqrt(256) (:262-265)
@@ -557,7 +506,7 @@ int sg_gnn_tc(dimb_sg* g, cudaStream_t st, int P) {
     e.bias = g->tc_final.bias;
     e.ldc = d, e.col_off = 0, e.n_valid = d, e.m_valid = R;
     e.scale = 0.25f;
-    DIMB_TRY(sg_tc_gemm(g, st, S, g->m_x, g->xh, g->xl, 2 * d, g->tc_final, d, e, "sg.final_proj"));
+    DIMB_TRY(sg_tc_gemm(g, st, S, g->m_x, g->tc_final, d, e, "sg.final_proj"));
   }
   {
     EpiSim e;
@@ -570,8 +519,6 @@ int sg_gnn_tc(dimb_sg* g, cudaStream_t st, int P) {
     GemmArgs ga{};
     ga.num_kb = d / 64;
     ga.M = R, ga.N = R;
-    ga.Ah = g->mdh, ga.Al = g->mdl, ga.Bh = g->mdh, ga.Bl = g->mdl;
-    ga.lda = d, ga.ldb = d;
     DIMB_TRY((launch_gemm<128, false>(ctx, st, ops, ga, e, P * (NPt / kTileM), NPt, "sg.scores")));
     e.sim = g->simT;  // the same products with the operand roles swapped: scores^T, so that the column sweeps of Sinkhorn read rows
     e.swap = 1;
@@ -594,56 +541,6 @@ int sg_matches(dimb_sg* g, cudaStream_t st, int P, const float* Z, int ld, size_
                                         reinterpret_cast<long long*>(d_matches), d_mscores, d_n_matches, cap);
   DIMB_LAUNCH_CHECK(ctx);
   return DIMB_OK;
-}
-
-// DIMB_TC=0 debug path of the host entry: one pair (features staged in d[2], n[2] live counts known on the host) through the same
-// input kernel and encoder, then the plain fp32 GNN and Sinkhorn on the materialised couplings.
-int sg_match_plain(dimb_sg* g, cudaStream_t st, const SgSideIn* hin, const int n[2], int cap) {
-  dimb_ctx* ctx = g->ctx;
-  const int NP = g->NP, d = kSgD, m = n[0], nn = n[1];
-  DIMB_CUDA_OK(ctx, cudaMemcpyAsync(g->side_in, hin, 2 * sizeof(SgSideIn), cudaMemcpyHostToDevice, st));
-  sg_input_kernel<<<dim3(ceil_div(NP, 32), 2), dim3(32, 8), 0, st>>>(g->side_in, NP, g->cat, 2 * d, g->enc_in, g->n_act, g->stopped, g->pc);
-  DIMB_LAUNCH_CHECK(ctx);
-  DIMB_TRY(sg_encoder(g, st, 2, NP, g->cat, 2 * d));
-  float* cat[2] = {g->cat, g->cat + static_cast<size_t>(NP) * 2 * d};
-  for (int i = 0; i < g->L; ++i) {  // AttentionalGNN (:132-152): deltas of both sides from the OLD descriptors
-    const SgLayer& ly = g->layers[i];
-    for (int s = 0; s < 2; ++s) {
-      const int src = g->cross[i] ? 1 - s : s;
-      DIMB_TRY(sg_linear(g, st, cat[s], 2 * d, ly.q, g->q[s], d, n[s], 0));
-      DIMB_TRY(sg_linear(g, st, cat[src], 2 * d, ly.k, g->k[s], d, n[src], 0));
-      DIMB_TRY(sg_linear(g, st, cat[src], 2 * d, ly.v, g->v[s], d, n[src], 0));
-    }
-    for (int s = 0; s < 2; ++s) {
-      const int src = g->cross[i] ? 1 - s : s;
-      dim3 grid(ceil_div(n[s], 8), kSgHeads);
-      gx_attention_kernel<64><<<grid, 256, 0, st>>>(g->q[s], g->k[s], g->v[s], n[s], n[src], d, kSgHd, g->att, d);
-      DIMB_LAUNCH_CHECK(ctx);
-      DIMB_TRY(sg_linear(g, st, g->att, d, ly.merge, cat[s] + d, 2 * d, n[s], 0));  // message -> right half of [x | message]
-    }
-    for (int s = 0; s < 2; ++s) {  // x += mlp([x | message])
-      DIMB_TRY(sg_linear(g, st, cat[s], 2 * d, ly.mlp0, g->hid, 2 * d, n[s], 1));
-      DIMB_TRY(sg_linear(g, st, g->hid, 2 * d, ly.mlp3, cat[s], 2 * d, n[s], 0, 1.f, cat[s], 2 * d));
-    }
-  }
-  for (int s = 0; s < 2; ++s) DIMB_TRY(sg_linear(g, st, cat[s], 2 * d, g->final_proj, g->md[s], d, n[s], 0));
-  const int ld = nn + 1;
-  {  // scores = mdesc0 . mdesc1^T / sqrt(256) into the top-left block of the couplings
-    dim3 grid(ceil_div(nn, 64), ceil_div(m, 64));
-    gx_linear_kernel<<<grid, 256, 0, st>>>(g->md[0], d, g->md[1], d, nullptr, g->Z, ld, m, nn, d, 1.f / 16.f, nullptr, 0, 0);
-    DIMB_LAUNCH_CHECK(ctx);
-  }
-  sg_fill_bins_kernel<<<ceil_div(std::max(m, nn) + 1, 256), 256, 0, st>>>(g->Z, ld, m, nn, g->bin_score);
-  DIMB_LAUNCH_CHECK(ctx);
-  DIMB_CUDA_OK(ctx, cudaMemsetAsync(g->uu, 0, g->vld * sizeof(float), st));
-  DIMB_CUDA_OK(ctx, cudaMemsetAsync(g->vv, 0, g->vld * sizeof(float), st));
-  for (int it = 0; it < g->conf.sinkhorn_iterations; ++it) {
-    sg_sinkhorn_kernel<<<ceil_div((m + 1) * 32, 256), 256, 0, st>>>(g->Z, ld, m + 1, nn + 1, 0, g->vv, g->uu, g->pc);
-    DIMB_LAUNCH_CHECK(ctx);
-    sg_sinkhorn_kernel<<<ceil_div((nn + 1) * 32, 256), 256, 0, st>>>(g->Z, ld, m + 1, nn + 1, 1, g->uu, g->vv, g->pc);
-    DIMB_LAUNCH_CHECK(ctx);
-  }
-  return sg_matches(g, st, 1, g->Z, ld, 0, NP, g->o_m, g->o_ms, g->o_nm, cap);
 }
 
 }  // namespace
@@ -686,7 +583,6 @@ int dimb_sg_create(dimb_ctx* ctx, const float* weights, size_t n_floats, const d
     if (i < 4) fold_bn(l, p);
     DIMB_TRY(upload(ctx, g->kenc[i], l));
   }
-  g->layers.resize(g->L);
   g->tc.resize(g->L);
   for (int i = 0; i < g->L; ++i) {  // state_dict order: attn.merge, attn.proj.0/1/2, mlp.0, mlp.1 (BN), mlp.3
     HostLin merge = take_conv(p, kSgD, kSgD), q = take_conv(p, kSgD, kSgD), k = take_conv(p, kSgD, kSgD), v = take_conv(p, kSgD, kSgD);
@@ -694,51 +590,28 @@ int dimb_sg_create(dimb_ctx* ctx, const float* weights, size_t n_floats, const d
     fold_bn(m0, p);
     HostLin m3 = take_conv(p, kSgD, 2 * kSgD);
     permute_rows(q), permute_rows(k), permute_rows(v), permute_cols(merge);
-    {
-      HostLin qkv = q;
-      qkv.n = 3 * kSgD;
-      qkv.w.insert(qkv.w.end(), k.w.begin(), k.w.end());
-      qkv.w.insert(qkv.w.end(), v.w.begin(), v.w.end());
-      qkv.b.insert(qkv.b.end(), k.b.begin(), k.b.end());
-      qkv.b.insert(qkv.b.end(), v.b.begin(), v.b.end());
-      SgTcLayer& t = g->tc[i];
-      DIMB_TRY(upload_tc(ctx, t.qkv, qkv));
-      DIMB_TRY(upload_tc(ctx, t.merge, merge));
-      DIMB_TRY(upload_tc(ctx, t.mlp0, m0));
-      DIMB_TRY(upload_tc(ctx, t.mlp3, m3));
-    }
-    SgLayer& ly = g->layers[i];
-    DIMB_TRY(upload(ctx, ly.q, q));
-    DIMB_TRY(upload(ctx, ly.k, k));
-    DIMB_TRY(upload(ctx, ly.v, v));
-    DIMB_TRY(upload(ctx, ly.merge, merge));
-    DIMB_TRY(upload(ctx, ly.mlp0, m0));
-    DIMB_TRY(upload(ctx, ly.mlp3, m3));
+    HostLin qkv = q;
+    qkv.n = 3 * kSgD;
+    qkv.w.insert(qkv.w.end(), k.w.begin(), k.w.end());
+    qkv.w.insert(qkv.w.end(), v.w.begin(), v.w.end());
+    qkv.b.insert(qkv.b.end(), k.b.begin(), k.b.end());
+    qkv.b.insert(qkv.b.end(), v.b.begin(), v.b.end());
+    SgTcLayer& t = g->tc[i];
+    DIMB_TRY(upload_tc(ctx, t.qkv, qkv));
+    DIMB_TRY(upload_tc(ctx, t.merge, merge));
+    DIMB_TRY(upload_tc(ctx, t.mlp0, m0));
+    DIMB_TRY(upload_tc(ctx, t.mlp3, m3));
   }
-  {
-    HostLin fp = take_conv(p, kSgD, kSgD);
-    DIMB_TRY(upload(ctx, g->final_proj, fp));
-    DIMB_TRY(upload_tc(ctx, g->tc_final, fp));
-  }
+  DIMB_TRY(upload_tc(ctx, g->tc_final, take_conv(p, kSgD, kSgD)));
   DIMB_TRY(dimb_alloc_t(ctx, &g->bin_score, 1, false));
   DIMB_CUDA_OK(ctx, cudaMemcpy(g->bin_score, p, sizeof(float), cudaMemcpyHostToDevice));
   const size_t NP = g->NP, PP = g->max_pairs, d = kSgD;
-  {  // host entry: staging of one pair, outputs, plain fp32 twin
+  {  // host entry: staging of one pair, outputs
     DIMB_TRY(dimb_alloc_t(ctx, &g->st_kp, 2 * NP * 2));
     DIMB_TRY(dimb_alloc_t(ctx, &g->st_sc, 2 * NP));
     DIMB_TRY(dimb_alloc_t(ctx, &g->st_desc, 2 * d * NP));
     DIMB_TRY(dimb_alloc_t(ctx, &g->st_n, 2));
     DIMB_TRY(dimb_alloc_t(ctx, &g->o_nm, 1));
-    DIMB_TRY(dimb_alloc_t(ctx, &g->cat, 2 * NP * 2 * d));
-    for (int s = 0; s < 2; ++s) {
-      DIMB_TRY(dimb_alloc_t(ctx, &g->q[s], NP * d));
-      DIMB_TRY(dimb_alloc_t(ctx, &g->k[s], NP * d));
-      DIMB_TRY(dimb_alloc_t(ctx, &g->v[s], NP * d));
-      DIMB_TRY(dimb_alloc_t(ctx, &g->md[s], NP * d));
-    }
-    DIMB_TRY(dimb_alloc_t(ctx, &g->att, NP * d));
-    DIMB_TRY(dimb_alloc_t(ctx, &g->hid, NP * 2 * d));
-    DIMB_TRY(dimb_alloc_t(ctx, &g->Z, (NP + 1) * (NP + 1)));
   }
   {  // batched engine
     const size_t NPt = round_up(g->NP, 128), S = 2 * PP, R = S * NPt;
@@ -808,11 +681,6 @@ int dimb_sg_match_dev(dimb_sg* g, int P, const dimb_sg_feats_dev* f0, const dimb
       hin[2 * p + sd] = SgSideIn{f.keypoints, f.descriptors, f.scores, f.n, f.n_cap, f.desc_ld ? f.desc_ld : f.n_cap, f.f16, f.round_fp16,
                                  f.height, f.width, f.size_dev};
     }
-  if (!ctx->use_tc) {
-    dimb_set_error(ctx, "dimb_sg_match_dev: the device entry runs on the tensor-core path only (tensor path is off: DIMB_TC=0 or "
-                        "dimb_ctx_set_tensor_path); dimb_sg_match serves the fp32 debug path");
-    return DIMB_ERR_UNSUPPORTED;
-  }
   OwnerScope own(ctx, &g->mem);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(g->side_in, hin.data(), S * sizeof(SgSideIn), cudaMemcpyHostToDevice, st));
@@ -849,8 +717,7 @@ int dimb_sg_match_dev(dimb_sg* g, int P, const dimb_sg_feats_dev* f0, const dimb
 }
 
 // One pair.  Outputs (host): matches [cap][2] int64 ascending in column 0 (correspondence_matrix_from_matches0, superglue.py:44-52),
-// mscores [cap] (matching_scores0 of the matched rows), n_matches.  Stages the pair and runs dimb_sg_match_dev with P = 1
-// (or, with the tensor path off, the plain fp32 twin).
+// mscores [cap] (matching_scores0 of the matched rows), n_matches.  Stages the pair and runs dimb_sg_match_dev with P = 1.
 int dimb_sg_match(dimb_sg* g, const dimb_sg_feats* f0, const dimb_sg_feats* f1, int64_t* matches, float* mscores, int* n_matches, int cap) {
   if (!g || !f0 || !f1 || !matches || !mscores || !n_matches || cap < 1) return DIMB_ERR_ARG;
   dimb_ctx* ctx = g->ctx;
@@ -873,7 +740,6 @@ int dimb_sg_match(dimb_sg* g, const dimb_sg_feats* f0, const dimb_sg_feats* f1, 
     g->o_cap = cap;
   }
   dimb_sg_feats_dev df[2];
-  SgSideIn hin[2];
   for (int s = 0; s < 2; ++s) {
     const dimb_sg_feats& f = *F[s];
     float* kp = g->st_kp + static_cast<size_t>(s) * NP * 2;
@@ -885,13 +751,9 @@ int dimb_sg_match(dimb_sg* g, const dimb_sg_feats* f0, const dimb_sg_feats* f1, 
     DIMB_CUDA_OK(ctx, cudaMemcpyAsync(kp, f.keypoints, static_cast<size_t>(n[s]) * 2 * sizeof(float), cudaMemcpyHostToDevice, st));
     DIMB_CUDA_OK(ctx, cudaMemcpyAsync(sc, f.scores, static_cast<size_t>(n[s]) * sizeof(float), cudaMemcpyHostToDevice, st));
     df[s] = dimb_sg_feats_dev{kp, de, sc, g->st_n + s, n[s], NP, 0, 0, f.height, f.width, nullptr};
-    hin[s] = SgSideIn{kp, de, sc, g->st_n + s, n[s], NP, 0, 0, f.height, f.width, nullptr};
   }
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(g->st_n, n, 2 * sizeof(int), cudaMemcpyHostToDevice, st));
-  if (ctx->use_tc)
-    DIMB_TRY(dimb_sg_match_dev(g, 1, &df[0], &df[1], g->o_m, g->o_ms, g->o_nm, cap, st));
-  else
-    DIMB_TRY(sg_match_plain(g, st, hin, n, cap));
+  DIMB_TRY(dimb_sg_match_dev(g, 1, &df[0], &df[1], g->o_m, g->o_ms, g->o_nm, cap, st));
   int cnt = 0;
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(&cnt, g->o_nm, sizeof(int), cudaMemcpyDeviceToHost, st));
   DIMB_CUDA_OK(ctx, cudaStreamSynchronize(st));

@@ -130,12 +130,6 @@ int run_conv1_f32(dimb_sp* sp, cudaStream_t st, const ConvLayer& L, const __half
   g.num_kb = L.cin / 64;
   g.M = cells;
   g.N = L.cout;
-  g.Ah = inh;
-  g.Al = inl;
-  g.Bh = L.wh;
-  g.Bl = L.wl;
-  g.lda = L.cin;
-  g.ldb = L.k;
   EpiStoreF32 epi;
   epi.out = out;
   epi.bias = L.bias;
@@ -272,7 +266,7 @@ int dimb_sp_extract_dev(dimb_sp* sp, const float* d_images, int B, int H, int W,
   }
   {
     ProfScope prof(ctx, st, "sp.nms");
-    DIMB_TRY(launch_nms(ctx, st, sp->scores, sp->nms, B, H8, W8, cf.nms_radius, ctx->nms_ver));
+    DIMB_TRY(launch_nms(ctx, st, sp->scores, sp->nms, B, H8, W8, cf.nms_radius, kNmsProductionVer));
   }
   ProfScope prof_sel(ctx, st, "sp.select+describe");
   const CandBufs cand{sp->chunk_count, sp->chunk_off, sp->cand_count, sp->cand_idx, sp->cand_score};

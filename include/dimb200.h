@@ -54,9 +54,6 @@ int dimb_ctx_create(int device, dimb_ctx** out);
 void dimb_ctx_destroy(dimb_ctx* ctx);
 const char* dimb_last_error(dimb_ctx* ctx);
 int dimb_ctx_set_precision(dimb_ctx* ctx, int precision);
-/* 1 (default): wgmma tensor-core kernels.  0: CUDA-core SIMT kernels with the same epilogues
- * (debug aid to bisect a tensor-path problem; also selectable with env DIMB_TC=0). */
-int dimb_ctx_set_tensor_path(dimb_ctx* ctx, int use_tc);
 /* Number of kernels this library has launched on ctx (bench.py "gpu_launches"). */
 unsigned long long dimb_ctx_launch_count(dimb_ctx* ctx);
 const char* dimb_version(void);
@@ -191,7 +188,7 @@ int dimb_nn_match_dev(dimb_ctx* ctx, const void* d_desc0, int n0, int ld0, const
  * Scratch (context slots, grow-only), NPp = the largest n_cap rounded up to 128, Dp = D rounded up to 64: the fp16 operands
  * 2P x NPp x Dp x 2 B (twice with the three-MMA split), and the chunk partials of the top-2 GEMM, P x NPp x NPp / 32 x 12 B, shared
  * by the two directions of mnn / smnn: about 25 MB per pair at 8192 keypoints, 1.6 MB at 2048.
- * Runs on the CUDA-core GEMM twin (DIMB_TC=0) as well.  Profile groups: nn.prep, nn.top2_gemm, nn.merge, nn.select. */
+ * Profile groups: nn.prep, nn.top2_gemm, nn.merge, nn.select. */
 int dimb_nn_match_batch_dev(dimb_ctx* ctx, int P, const dimb_feats_dev* f0, const dimb_feats_dev* f1, int D, int mode, float th,
                             int64_t* d_idx, float* d_dist, int* d_n, int cap, void* stream);
 
@@ -250,7 +247,7 @@ typedef struct {
  * when the gate rejects the pair; d_F [P][9] (x1^T F x0 = 0, zeros when no model); d_mask [P][cap]; d_n_inliers [P].  Pairs with
  * fewer than 8 raw matches (or no model): mask all ones, F zeros, n_inliers = n_raw, then the gate.  DIMB_ERR_ARG, before any CUDA
  * call, for a NULL ctx / f0 / f1 / seeds / conf / buffer / keypoint pointer, P < 1, cap < 1, threshold <= 0, min_inliers < 0 or
- * min_inlier_ratio outside [0, 1].  CUDA-core kernels: runs with DIMB_TC=0 as well. */
+ * min_inlier_ratio outside [0, 1]. */
 int dimb_gv_verify_dev(dimb_ctx* ctx, int P, const dimb_feats_dev* f0, const dimb_feats_dev* f1, const int64_t* d_matches,
                        const int* d_n_matches, int cap, const unsigned* seeds, const dimb_gv_conf* conf, int64_t* d_verified,
                        int* d_n_verified, float* d_F, unsigned char* d_mask, int* d_n_inliers, void* stream);
@@ -259,7 +256,7 @@ int dimb_gv_verify_dev(dimb_ctx* ctx, int P, const dimb_feats_dev* f0, const dim
  * Device counterparts of ExtractorBase._extract_by_tile (extractors/extractor_base.py:279-390) and MatcherBase._match_by_tile
  * (matchers/matcher_base.py:362-485).  Every entry is asynchronous on `stream` and never synchronises (once its context scratch has
  * grown to the call's size), is bitwise reproducible and independent of how images or pairs are batched, and returns DIMB_ERR_ARG
- * before any CUDA call for a NULL pointer or an out-of-range size.  CUDA-core kernels: they run with DIMB_TC=0 as well.
+ * before any CUDA call for a NULL pointer or an out-of-range size.
  * Profile groups: tile.cut, tile.merge, tile.views, tile.match_merge.
  *
  * Tile geometry (utils/tiling.py Tiler.compute_tiles_by_size): tile_h x tile_w windows stepped by (tile - overlap), on the image
@@ -508,7 +505,7 @@ typedef struct {
 } dimb_sg_feats_dev;
 /* P <= max_pairs pairs on device pointers, asynchronous on `stream` (never synchronises).  Outputs as dimb_lg_match_dev:
  * d_matches [P][cap][2] int64 ascending in column 0, d_mscores [P][cap], d_n_matches [P] (the full count, also when it exceeds
- * cap; only the first cap rows are written).  Needs the tensor-core path: DIMB_ERR_UNSUPPORTED with DIMB_TC=0. */
+ * cap; only the first cap rows are written). */
 int dimb_sg_match_dev(dimb_sg* sg, int P, const dimb_sg_feats_dev* f0, const dimb_sg_feats_dev* f1, int64_t* d_matches, float* d_mscores,
                       int* d_n_matches, int cap, void* stream);
 /* The slot as SuperGlue device input: f16 = 1, scores from the slot's score block, size_dev = the slot header's [H,W]. */

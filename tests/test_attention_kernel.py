@@ -1,7 +1,7 @@
 """Flash attention (csrc/attention.cuh) on its own, against a float64 softmax(scale Q K^T) V of the same fp32 operands.
 
 The kernels run through their production launches in the self-test library (dimb_selftest_attention): lg_attn_kernel (LightGlue /
-SuperGlue: 4 heads x 64, self and cross, several sides with their own live counts and stopped pairs), its SIMT twin (DIMB_TC=0), and
+SuperGlue: 4 heads x 64, self and cross, several sides with their own live counts and stopped pairs) and
 gx_attn_tc_kernel (the shape-generic path: head dim padded to 128).  Padding rows hold a large finite value, as the stale rows of
 earlier layers do in production, and the output buffer starts as a sentinel, so the mask and the rows that must not be written are
 checked as well as the values.
@@ -345,21 +345,6 @@ def test_attention_is_bitwise_repeatable(st):
     q, k, v, _ = design("random", 300, 1000, 96, np.random.default_rng(8))
     a, b = (st.attention(1, q, k, v, (300, 1000), heads=1, lazy=8.0, pad=PAD, out_pad=OUT_PAD) for _ in range(2))
     assert np.array_equal(a, b)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("cross", [False, True], ids=["self", "cross"])
-def test_lg_attention_simt_twin(cross):
-    """The SIMT twin (DIMB_TC=0, the debug path) on the same packed buffers meets the EXACT bound."""
-    st = _selftest({"DIMB_TC": "0"})
-    st.set_precision("exact")
-    for pattern in PATTERNS:
-        for i in (1, 5, 8, 9):
-            nq, nk = SHAPES[i]
-            n, stopped = _lg_live_counts(i, nq, nk)
-            Q, K, V, hot = lg_case(pattern, n, cross, np.random.default_rng(i))
-            out = st.attention(0, Q, None if cross else K, V, n, stopped=stopped, cross=cross, pad=PAD, out_pad=OUT_PAD)
-            check_lg(out, Q, K, V, n, stopped, cross, pattern, hot, EXACT_TOL)
 
 
 @pytest.mark.gpu

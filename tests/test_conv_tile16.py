@@ -2,8 +2,8 @@
 and, bitwise, against the 8 x 16-pixel tiles (mode 1) on the same inputs.
 
 Mode 2 runs every output element through the same wgmma sequence as mode 1 ((dx, channel block), dy, k16, then hi * hi, hi * lo, lo * hi),
-so the two tile shapes must agree bit for bit.  run_conv3 picks mode 2 by shape (conv3x3.cuh conv_mode): 64 output channels, the
-tensor-core kernel, and at least two 16 x 16 tiles per SM, in either precision; the GPU cases pass the tile shape explicitly through the self-test
+so the two tile shapes must agree bit for bit.  run_conv3 picks mode 2 by shape (conv3x3.cuh conv_mode): 64 output channels and at
+least two 16 x 16 tiles per SM, in either precision; the GPU cases pass the tile shape explicitly through the self-test
 entry (dimb_selftest_conv3x3), and one case checks the production choice.  The reference, the bound model and the case kinds (designed,
 shift, random) are those of test_gemm_conv_kernel.py.
 """
@@ -181,17 +181,6 @@ def test_tile16_bitwise_repeatable(st):
     x, w, bias = K.conv_case("random", 2, 115, 155, 64, 64, np.random.default_rng(13))
     r1, r2 = (st.conv3x3_tiles(x, w, bias, True, 16, guard=K.GUARD, sentinel=K.SENTINEL)[0] for _ in range(2))
     assert np.array_equal(r1.view(np.uint32), r2.view(np.uint32))
-
-
-@pytest.mark.gpu
-def test_tile16_refused_on_the_simt_twin():
-    """The SIMT twin (DIMB_TC=0) runs 128-row tiles only: 16 x 16 tiles are refused, and production keeps 8 x 16 there."""
-    from dim_b200 import _native
-    st = K._selftest({"DIMB_TC": "0"})
-    x, w, bias = K.conv_case("designed", 1, 16, 16, 64, 64, np.random.default_rng(0))
-    with pytest.raises(_native.DimbError):
-        st.conv3x3_tiles(x, w, bias, False, 16)
-    assert st.conv3x3_tiles(x, w, bias, False, 0)[3] == 1
 
 
 @pytest.mark.gpu

@@ -1,7 +1,7 @@
 """Keypoint detection (csrc/detect.cuh) and the SuperPoint head kernels (csrc/sp_head.cuh) on their own, against exact references.
 
 Every extractor ends in the same machinery: simple_nms (the bit-mask kernel sp_nms2_kernel for radii 1..5, the first cut sp_nms_kernel
-for radius 0, radii 6..8 and every radius under DIMB_NMS=1), threshold + border compaction in row-major order, and top-k selection
+for radius 0 and radii 6..8), threshold + border compaction in row-major order, and top-k selection
 (radix select, a tie rank over blocks of 1024 candidates, a bitonic sort).  The self-test library runs them through the launch helpers
 SuperPoint and ALIKED call (dimb_selftest_detect), with every output buffer starting as a sentinel and followed by a tail, so unwritten
 slots and stray writes both show.  These are exact operations, so the GPU tests compare bitwise:

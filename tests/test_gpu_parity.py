@@ -243,28 +243,6 @@ def test_lightglue_kernel_variants(lg_golden, env):
         _check_lg(lg.match([({**f0, "_layout": 0}, {**f1, "_layout": 0})])[0], ref)
 
 
-@pytest.mark.parametrize("env", [{"DIMB_NMS": "1"}])
-def test_superpoint_kernel_variants(sp_weights, env):
-    """The selectable SuperPoint kernels (first-cut NMS) against the oracle, like the defaults."""
-    from dim_b200 import _native, synthetic
-    from oracle import superpoint as o_sp
-    old = {k: os.environ.get(k) for k in env}
-    os.environ.update(env)
-    try:
-        vctx = _native.Context(0)
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
-    conf = {"nms_radius": 3, "keypoint_threshold": 0.0005, "max_keypoints": 512}
-    g, _ = synthetic.synthetic_pair(6, 384)
-    g = g[:320]
-    out = _sp_net(vctx, sp_weights, conf, 1, 320, 384).extract(g[None])[0]
-    _check_sp(out, o_sp.extract(g, sp_weights, conf), g, conf, sp_weights)
-
-
 def test_lightglue_batched_pairs_and_layouts(ctx, lg_golden):
     """Several pairs of different sizes in one call, (N,D) and (D,N) layouts, non-square image_size (quirk A.3)."""
     from dim_b200 import _native

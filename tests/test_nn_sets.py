@@ -123,8 +123,9 @@ def _oracle(f0, f1, mode, th):
 @pytest.mark.gpu
 @pytest.mark.parametrize("mode,th", MODES)
 def test_batch_equals_single_pair_entry_and_oracle(ctx, nn_store, mode, th):
-    """One mixed batch of store pairs (counts 0, 1, 2, 129, 700 and capacity; n0 > n1 and n0 < n1): per pair bitwise the single-pair
-    device entry with host-read counts, and the kornia oracle's indices (distances within 1e-4)."""
+    """One mixed batch of store pairs (counts 0, 1, 2, 129, 300, 650, 700 and capacity; n0 > n1 and n0 < n1; 129, 300, 650 and 700 end
+    inside a 128-column tile): per pair bitwise the single-pair device entry with host-read counts, and the kornia oracle's indices
+    (distances within 1e-4)."""
     store, _ = nn_store
     out, _ = _batch(ctx, [store.feats_dev(a) for a, _ in PAIRS], [store.feats_dev(b) for _, b in PAIRS], mode, th)
     for p, (s0, s1) in enumerate(PAIRS):
@@ -169,25 +170,6 @@ def test_batch_entry_rejects_bad_arguments(ctx, nn_store):
     assert call(ok) == 0  # the same arguments without the fault run
     torch.cuda.synchronize()
     assert int(n.cpu()[0]) > 0
-
-
-@pytest.mark.gpu
-def test_cuda_core_path_equals_single_pair_entry(nn_store):
-    """The CUDA-core twin of the GEMM (tensor path off, DIMB_TC=0's debug path; 32-column tiles, the ones past a partner's count
-    skipped): the mixed batch in every mode, after calls that leave other data in the scratch, equals the single-pair entry bitwise and
-    the oracle's indices.  Counts 700, 300, 129 and 650 end inside a 128-column tile."""
-    from dim_b200 import _native
-    store, _ = nn_store
-    simt = _native.Context(0, tensor_path=False)
-    f0, f1 = [store.feats_dev(a) for a, _ in PAIRS], [store.feats_dev(b) for _, b in PAIRS]
-    for mode, th in MODES:
-        out, _ = _batch(simt, f0, f1, mode, th)
-        for p, (s0, s1) in enumerate(PAIRS):
-            _bitwise(out[p], _single_dev(simt, store, s0, s1, mode, th))
-            ridx, rdist = _oracle(store.get(s0), store.get(s1), mode, th)
-            assert np.array_equal(out[p][0], ridx), (mode, p, len(out[p][0]), len(ridx))
-            if len(rdist):
-                assert np.abs(out[p][1] - rdist).max() < 1e-4, (mode, p)
 
 
 class _F32Side:

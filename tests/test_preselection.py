@@ -285,7 +285,7 @@ def _planted(H, W, th, tw, ov_hw, scale, seed):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("geom", [((768, 1024), (512, 512), 64, 0.5), ((1000, 1300), (256, 384), 32, 0.375), ((2048, 2048), (256, 256), 0, 0.25)])
-def test_tile_preselect_dev_equals_tile_selection(ctx, geom):
+def test_device_tile_preselection_equals_tile_selection(ctx, geom):
     """The box count against tiling.tile_selection on planted matches: strict edges, negative origins, an empty table, T up to 64,
     tile_w != tile_h; min_matches_per_tile 5, then a count that occurs (not selected) and one below it (selected)."""
     import torch
@@ -316,21 +316,20 @@ def test_tile_preselect_dev_equals_tile_selection(ctx, geom):
     v = int(np.median(nz))
     assert T >= 4 and v >= 1 and len(host[1][0]) == 7 * T
     for mm in (5, v, v - 1):
-        for c in (ctx, _native.Context(0, tensor_path=False)):  # CUDA-core kernels: the same with the tensor path off
-            counts = torch.full((len(cases), T * T), -1, dtype=torch.int32, device="cuda")
-            flags = torch.full((len(cases), T * T), 7, dtype=torch.uint8, device="cuda")
-            c.tile_preselect_dev(f0, f1, d_m.data_ptr(), d_nm.data_ptr(), cap, H, W, th, tw, *ov_hw, scale, scale, mm, counts.data_ptr(),
-                                 flags.data_ptr(), 0)
-            counts, flags = counts.cpu().numpy().reshape(-1, T, T), flags.cpu().numpy().reshape(-1, T, T)
-            for q, (kp0, kp1, exp) in enumerate(host):
-                assert np.array_equal(counts[q], exp), (mm, q)
-                lst = tiling.tile_selection(img, img, "preselection", tile_size, overlap, kp0=kp0, kp1=kp1, min_matches_per_tile=mm)
-                assert [(int(a), int(b)) for a, b in zip(*np.nonzero(flags[q]))] == lst, (mm, q)
-            assert not flags[2].any() and not counts[2].any()  # the empty table
-            if mm == v:
-                assert not flags[0][counts[0] == v].any()
-            if mm == v - 1:
-                assert flags[0][counts[0] == v].all()
+        counts = torch.full((len(cases), T * T), -1, dtype=torch.int32, device="cuda")
+        flags = torch.full((len(cases), T * T), 7, dtype=torch.uint8, device="cuda")
+        ctx.tile_preselect_dev(f0, f1, d_m.data_ptr(), d_nm.data_ptr(), cap, H, W, th, tw, *ov_hw, scale, scale, mm, counts.data_ptr(),
+                               flags.data_ptr(), 0)
+        counts, flags = counts.cpu().numpy().reshape(-1, T, T), flags.cpu().numpy().reshape(-1, T, T)
+        for q, (kp0, kp1, exp) in enumerate(host):
+            assert np.array_equal(counts[q], exp), (mm, q)
+            lst = tiling.tile_selection(img, img, "preselection", tile_size, overlap, kp0=kp0, kp1=kp1, min_matches_per_tile=mm)
+            assert [(int(a), int(b)) for a, b in zip(*np.nonzero(flags[q]))] == lst, (mm, q)
+        assert not flags[2].any() and not counts[2].any()  # the empty table
+        if mm == v:
+            assert not flags[0][counts[0] == v].any()
+        if mm == v - 1:
+            assert flags[0][counts[0] == v].all()
 
 
 def _gray_set(n, H=768, W=1024):

@@ -223,7 +223,7 @@ def test_match_dev_is_asynchronous(sg_net, batch):
 
 
 @pytest.mark.gpu
-def test_argument_errors_tensor_path_and_fast_mode(sg_net, sg_case, batch):
+def test_argument_errors_and_fast_mode(sg_net, sg_case, batch):
     from dim_b200 import _native
     from dim_b200.io_h5 import as_half_roundtrip
     sides, _, _ = batch
@@ -237,10 +237,6 @@ def test_argument_errors_tensor_path_and_fast_mode(sg_net, sg_case, batch):
     no_scores.s.scores = None
     with pytest.raises(_native.DimbError, match=r"code -3"):  # NULL scores
         _run(sg_net, [(no_scores, sides[0][1])])
-    simt = _native.Context(0, tensor_path=False)
-    net = _native.SuperGlueNet(simt, sg_case[0], max_kpts=MAXK, max_pairs=6)
-    with pytest.raises(_native.DimbError, match=r"code -4"):
-        _run(net, sides)
     fast = _native.Context(0, precision="fast")
     net = _native.SuperGlueNet(fast, sg_case[0], max_kpts=MAXK, max_pairs=6)
     res, _, _ = _run(net, sides)
