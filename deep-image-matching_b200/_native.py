@@ -194,8 +194,8 @@ _selftest = None
 
 def load_selftest_library():
     """libdimb200_selftest.so: the production GEMM template behind a C = A B^T entry, the flash-attention kernels behind an
-    attention entry, keypoint detection (simple_nms, compaction, top-k) and the SuperPoint head kernels behind their own entries, and
-    the host drive of the RANSAC arithmetic.
+    attention entry, keypoint detection (simple_nms, compaction, top-k), the SuperPoint head kernels and the matching heads (LightGlue
+    assignment and tail, SuperGlue Sinkhorn) behind their own entries, and the host drive of the RANSAC arithmetic.
     Test / tool infrastructure - the product library exports none of it.  Its context is its own (dimb_ctx_create of
     THIS library); never mix handles of the two libraries."""
     global _selftest
@@ -222,6 +222,10 @@ def load_selftest_library():
         lib.dimb_selftest_detect.argtypes = [vp, vp] + [ip] * 5 + [fp, vp, ip, ip, ip, fp] + [vp] * 8
         lib.dimb_selftest_sp_softmax.argtypes = [vp, vp, ip, ip, ip, fp, vp]
         lib.dimb_selftest_sp_describe.argtypes = [vp] * 5 + [ip] * 5 + [fp, vp, vp, vp]
+        lib.dimb_selftest_lg_assign.argtypes = [vp, ip, ip] + [vp] * 6 + [fp, ip, fp] + [vp] * 8
+        lib.dimb_selftest_lg_tail.argtypes = [vp, ip, ip, vp, vp, fp, vp, fp] + [vp] * 6 + [ip, fp, fp, fp, ip, ip, ip, fp] + [vp] * 6
+        lib.dimb_selftest_lgx_assign.argtypes = [vp, ip, ip, ip] + [vp] * 5 + [fp, ip, fp] + [vp] * 11
+        lib.dimb_selftest_sg_sinkhorn.argtypes = [vp, ip, vp, vp, vp, fp, fp, vp, vp, ip, ip, fp, ip, fp] + [vp] * 9
         lib.dimb_gv_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_uint, vp, vp]
         _selftest = lib
     return _selftest
@@ -262,7 +266,8 @@ DET_TAIL = 1024  # elements past the valid ones in every output buffer of the de
 
 
 class SelfTest:
-    """Context of the self-test library (tests/test_gemm_conv_kernel.py, tests/test_attention_kernel.py, tests/test_detect_kernel.py)."""
+    """Context of the self-test library (tests/test_gemm_conv_kernel.py, tests/test_attention_kernel.py, tests/test_detect_kernel.py,
+    tests/test_match_heads.py)."""
 
     def __init__(self, device: int = 0):
         self.lib = load_selftest_library()
@@ -402,6 +407,102 @@ class SelfTest:
                                                       float(sentinel), *(_ptr(raw[k]) for k in shapes)), "selftest_sp_describe")
         out = {k: raw[k][:-DET_TAIL].reshape(s) for k, s in shapes.items()}
         out.update({k + "_tail": raw[k][-DET_TAIL:] for k in shapes})
+        return out
+
+    def _run(self, fn, what, bufs, *args):
+        """Calls fn(handle, *args, *pointers of bufs); bufs: name -> (dtype, valid length).  Every buffer holds DET_TAIL more
+        elements.  Returns (name -> the valid part, name -> the tail)."""
+        raw = {k: np.zeros(m + DET_TAIL, t) for k, (t, m) in bufs.items()}
+        self.check(fn(self.h, *args, *(_ptr(raw[k]) for k in bufs)), what)
+        return {k: raw[k][:m] for k, (_, m) in bufs.items()}, {k: raw[k][m:] for k, (_, m) in bufs.items()}
+
+    def lg_assign(self, sim: np.ndarray, nf, n_orig, layer, indf: np.ndarray, z: np.ndarray, th: float, cap: int,
+                  sentinel: float = -777.0) -> dict:
+        """The LightGlue assignment through its launch helper (dimb_selftest_lg_assign).  sim [P][NP][NP] (NP a multiple of 128),
+        nf / n_orig [2P], layer [P], indf / z [2P][NP] (z = logsigmoid(matchability)).  Returns rmax / rlog / best / arg0 (rows, side
+        2p), cmax / clog / arg1 (columns, side 2p + 1), best_other (the best buffer at side 2p + 1, which nothing writes), each [P][NP],
+        matches [P][cap][2], mscores [P][cap], n_matches / stop_layer [P], and '<name>_tail' of every buffer."""
+        sim = np.ascontiguousarray(sim, np.float32)
+        P, NP, _ = sim.shape
+        R = 2 * P * NP
+        bufs = {"smax": (np.float32, R), "slog": (np.float32, R), "best": (np.float32, R), "arg": (np.int32, R),
+                "matches": (np.int64, 2 * P * cap), "mscores": (np.float32, P * cap), "n_matches": (np.int32, P),
+                "stop_layer": (np.int32, P)}
+        ins = [np.ascontiguousarray(a, t) for a, t in ((nf, np.int32), (n_orig, np.int32), (layer, np.int32), (indf, np.int32),
+                                                        (z, np.float32))]
+        o, tail = self._run(self.lib.dimb_selftest_lg_assign, "selftest_lg_assign", bufs, P, NP, _ptr(sim), *(_ptr(a) for a in ins),
+                            float(th), int(cap), float(sentinel))
+        side = {k: o[k].reshape(P, 2, NP) for k in ("smax", "slog", "best", "arg")}
+        out = {"rmax": side["smax"][:, 0], "rlog": side["slog"][:, 0], "best": side["best"][:, 0], "arg0": side["arg"][:, 0],
+               "cmax": side["smax"][:, 1], "clog": side["slog"][:, 1], "best_other": side["best"][:, 1], "arg1": side["arg"][:, 1],
+               "matches": o["matches"].reshape(P, cap, 2), "mscores": o["mscores"].reshape(P, cap), "n_matches": o["n_matches"],
+               "stop_layer": o["stop_layer"]}
+        out.update({k + "_tail": v for k, v in tail.items()})
+        return out
+
+    def lg_tail(self, P: int, NP: int, n_act, n_orig, stopped, counter, layer: int, thr: float, depth_conf: float, keep_thr: float,
+                do_stop: bool, do_prune: bool, prune_min: int, x32=None, wt=None, bt: float = 0.0, wm=None, bm: float = 0.0, tok=None,
+                mat=None, sentinel: float = -777.0) -> dict:
+        """The LightGlue per-layer tail (dimb_selftest_lg_tail): from tokens x32 [2P * NP][256] with the confidence / matchability
+        weights (lg_conf_kernel, then lg_decide_kernel), or, with x32 None, lg_decide_kernel alone on the given tok / mat [2P * NP].
+        n_act / n_orig [2P], stopped / counter [P]: the state before.  Returns tok, mat, map [2P][NP], n_next [2P], counter and
+        stopped [P] after the call, and '<name>_tail' of every buffer."""
+        R = 2 * P * NP
+        f32 = lambda a: None if a is None else np.ascontiguousarray(a, np.float32)
+        x32, wt, wm, tok, mat = f32(x32), f32(wt), f32(wm), f32(tok), f32(mat)
+        ptr = lambda a: None if a is None else _ptr(a)
+        ins = [np.ascontiguousarray(a, np.int32) for a in (n_act, n_orig, stopped, counter)]
+        bufs = {"tok": (np.float32, R), "mat": (np.float32, R), "counter": (np.int32, P), "stopped": (np.int32, P), "map": (np.int32, R),
+                "n_next": (np.int32, 2 * P)}
+        o, tail = self._run(self.lib.dimb_selftest_lg_tail, "selftest_lg_tail", bufs, int(P), int(NP), ptr(x32), ptr(wt), float(bt),
+                            ptr(wm), float(bm), ptr(tok), ptr(mat), *(_ptr(a) for a in ins), int(layer), float(thr), float(depth_conf),
+                            float(keep_thr), int(bool(do_stop)), int(bool(do_prune)), int(prune_min), float(sentinel))
+        out = {k: o[k].reshape(2 * P, NP) if k in ("tok", "mat", "map") else o[k] for k in o}
+        out.update({k + "_tail": v for k, v in tail.items()})
+        return out
+
+    def lgx_assign(self, sim: np.ndarray, z0, z1, ind0, ind1, th: float, cap: int, sentinel: float = -777.0) -> dict:
+        """The shape-generic LightGlue assignment of one pair (dimb_selftest_lgx_assign): sim [m][ld] (live columns n = len(z1)), raw
+        matchability logits z0 [m] / z1 [n], original indices ind0 / ind1.  Returns rlse, ls0, best0, arg0 [m], clse, ls1, best1,
+        arg1 [n], matches [cap][2], mscores [cap], n_matches, and '<name>_tail' of every buffer."""
+        sim = np.ascontiguousarray(sim, np.float32)
+        z0, z1 = np.ascontiguousarray(z0, np.float32), np.ascontiguousarray(z1, np.float32)
+        i0, i1 = np.ascontiguousarray(ind0, np.int32), np.ascontiguousarray(ind1, np.int32)
+        m, n, ld = len(z0), len(z1), sim.shape[1]
+        bufs = {"rlse": (np.float32, m), "clse": (np.float32, n), "ls0": (np.float32, m), "ls1": (np.float32, n),
+                "best0": (np.float32, m), "arg0": (np.int32, m), "best1": (np.float32, n), "arg1": (np.int32, n),
+                "matches": (np.int64, 2 * cap), "mscores": (np.float32, cap), "n_matches": (np.int32, 1)}
+        o, tail = self._run(self.lib.dimb_selftest_lgx_assign, "selftest_lgx_assign", bufs, m, n, ld, _ptr(sim), _ptr(z0), _ptr(z1),
+                            _ptr(i0), _ptr(i1), float(th), int(cap), float(sentinel))
+        o["matches"] = o["matches"].reshape(cap, 2)
+        o["n_matches"] = int(o["n_matches"][0])
+        o.update({k + "_tail": v for k, v in tail.items() if k != "n_matches"})
+        return o
+
+    def sg_sinkhorn(self, scores: list, alpha: float, wave: int = 1, half_steps: int = 200, th: float = 0.2, cap: int | None = None,
+                    u=None, v=None, pad: float = 1e6, sentinel: float = -777.0) -> dict:
+        """SuperGlue's Sinkhorn and matching through their launch helpers (dimb_selftest_sg_sinkhorn).  scores: P float32 blocks
+        [m_p][n_p]; the device layout is [P][NPt][NPt], NPt = max(m, n, 1) rounded up to 128, padding `pad`.  u / v [P][NPt + 1] or
+        None (zeros): the duals before the first half step.  Returns NPt, pc [P][4], u / v [P][NPt + 1], best0 / arg0 / arg1 [P][NPt],
+        matches [P][cap][2], mscores [P][cap], n_matches [P], and '<name>_tail' of every buffer."""
+        P = len(scores)
+        m = np.array([s.shape[0] for s in scores], np.int32)
+        n = np.array([s.shape[1] for s in scores], np.int32)
+        NPt = -(-max(int(m.max()), int(n.max()), 1) // 128) * 128
+        cap = int(cap if cap is not None else max(int(m.max()), 1))
+        flat = np.ascontiguousarray(np.concatenate([np.asarray(s, np.float32).reshape(-1) for s in scores] + [np.zeros(1, np.float32)]))
+        uv = [None if a is None else np.ascontiguousarray(a, np.float32).reshape(P * (NPt + 1)) for a in (u, v)]
+        bufs = {"pc": (np.float32, 4 * P), "u": (np.float32, P * (NPt + 1)), "v": (np.float32, P * (NPt + 1)),
+                "best0": (np.float32, P * NPt), "arg0": (np.int32, P * NPt), "arg1": (np.int32, P * NPt),
+                "matches": (np.int64, 2 * P * cap), "mscores": (np.float32, P * cap), "n_matches": (np.int32, P)}
+        o, tail = self._run(self.lib.dimb_selftest_sg_sinkhorn, "selftest_sg_sinkhorn", bufs, P, _ptr(m), _ptr(n), _ptr(flat), float(alpha),
+                            float(pad), None if uv[0] is None else _ptr(uv[0]), None if uv[1] is None else _ptr(uv[1]), int(wave),
+                            int(half_steps), float(th), cap, float(sentinel))
+        shapes = {"pc": (P, 4), "u": (P, NPt + 1), "v": (P, NPt + 1), "best0": (P, NPt), "arg0": (P, NPt), "arg1": (P, NPt),
+                  "matches": (P, cap, 2), "mscores": (P, cap)}
+        out = {k: o[k].reshape(shapes[k]) if k in shapes else o[k] for k in o}
+        out["NPt"] = NPt
+        out.update({k + "_tail": v for k, v in tail.items()})
         return out
 
     def __del__(self):

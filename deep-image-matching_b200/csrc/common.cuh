@@ -129,6 +129,16 @@ __device__ __forceinline__ void split2_f32(float a, float b, __half2& hi, __half
   lo = __floats2half2_rn(a - f.x, b - f.y);
 }
 
+// ---------------------------------------------------------------- first argmax with torch.max semantics
+// (v, i) takes the place of the running best (bv, bi): NaN ranks above every number (the first NaN wins), then the larger value, then
+// the smaller index.  Starting from (-INFINITY, INT_MAX), a row of -inf therefore yields its first index and a row holding a NaN the
+// first NaN, so every index an argmax writes lies inside the row; finite rows give the first maximum, as a plain v > bv scan does.
+__device__ __forceinline__ bool argmax_takes(float v, int i, float bv, int bi) {
+  const bool vn = isnan(v), bn = isnan(bv);
+  if (vn || bn) return vn && (!bn || i < bi);
+  return v > bv || (v == bv && i < bi);
+}
+
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ inline int round_up(int a, int b) { return ceil_div(a, b) * b; }
 

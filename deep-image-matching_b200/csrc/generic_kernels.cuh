@@ -209,7 +209,7 @@ __global__ void gx_lse_kernel(const float* __restrict__ sim, int ld, int m, int 
 __device__ __forceinline__ float log_sigmoid(float z) { return fminf(z, 0.f) - log1pf(expf(-fabsf(z))); }
 
 // row (dir 0) / column (dir 1) maximum and first argmax of scores = (sim - rlse) + (sim - clse) + logsig(z0) + logsig(z1)
-// in the association of the reference (lightglue.py:246-256: scores0 + scores1 + certainties)
+// in the association of the reference (lightglue.py:246-256: scores0 + scores1 + certainties), torch.max order (argmax_takes)
 __global__ void gx_argmax_kernel(const float* __restrict__ sim, int ld, int m, int n, const float* __restrict__ rlse,
                                  const float* __restrict__ clse, const float* __restrict__ z0, const float* __restrict__ z1, int dir,
                                  float* __restrict__ best, int* __restrict__ arg) {
@@ -222,13 +222,13 @@ __global__ void gx_argmax_kernel(const float* __restrict__ sim, int ld, int m, i
     const int r = dir == 0 ? i : j, c = dir == 0 ? j : i;
     const float sv = sim[static_cast<size_t>(r) * ld + c];
     const float val = ((sv - rlse[r]) + (sv - clse[c])) + (log_sigmoid(z0[r]) + log_sigmoid(z1[c]));
-    if (val > bv) bv = val, bi = j;
+    if (argmax_takes(val, j, bv, bi)) bv = val, bi = j;
   }
 #pragma unroll
   for (int of = 16; of; of >>= 1) {
     const float ov = __shfl_xor_sync(0xffffffffu, bv, of);
     const int oi = __shfl_xor_sync(0xffffffffu, bi, of);
-    if (ov > bv || (ov == bv && oi < bi)) bv = ov, bi = oi;
+    if (argmax_takes(ov, oi, bv, bi)) bv = ov, bi = oi;
   }
   if (lane == 0) best[i] = bv, arg[i] = bi;
 }

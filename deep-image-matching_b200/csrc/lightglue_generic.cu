@@ -442,19 +442,8 @@ static int lgx_match_pair(dimb_lgx* g, const dimb_feats& f0, const dimb_feats& f
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(a0.data(), g->arg0, n[0] * sizeof(int), cudaMemcpyDeviceToHost, st));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(a1.data(), g->arg1, n[1] * sizeof(int), cudaMemcpyDeviceToHost, st));
   DIMB_CUDA_OK(ctx, cudaStreamSynchronize(st));
-  int cnt = 0;
-  for (int r = 0; r < n[0]; ++r) {
-    const int c = a0[r];
-    if (a1[c] != r) continue;  // mutual
-    const float e = std::exp(b0[r]);
-    if (!(e > static_cast<float>(cf.filter_threshold))) continue;
-    if (cnt < cap) {
-      matches[2 * cnt] = ind[0][r];
-      matches[2 * cnt + 1] = ind[1][c];
-      mscores[cnt] = e;
-    }
-    ++cnt;
-  }
+  const int cnt = lgx_filter(n[0], n[1], b0.data(), a0.data(), a1.data(), ind[0].data(), ind[1].data(),
+                             static_cast<float>(cf.filter_threshold), matches, mscores, cap);
   *n_matches = cnt;
   if (cnt > cap) {
     dimb_set_error(ctx, "dimb_lg_match: more matches than cap");

@@ -6,6 +6,9 @@
 //   dimb_selftest_detect: simple_nms, candidate compaction and top-k (detect.cuh) through their production launches;
 //   dimb_selftest_nms_plan: the launch plan of simple_nms, host only;
 //   dimb_selftest_sp_softmax / dimb_selftest_sp_describe: the SuperPoint head kernels (sp_head.cuh) through their production launches;
+//   dimb_selftest_lg_assign / dimb_selftest_lg_tail: the LightGlue assignment and per-layer tail (lg_assign.cuh) through their launch
+//     helpers; dimb_selftest_lgx_assign: the shape-generic LightGlue assignment and host filter; dimb_selftest_sg_sinkhorn: SuperGlue's
+//     Sinkhorn and mutual-max matching (sg_assign.cuh);
 //   dimb_gv_host: the RANSAC arithmetic of gv.cu on the host.
 #include <algorithm>
 #include <cstring>
@@ -667,4 +670,260 @@ extern "C" int dimb_gv_host(const float* k0, const float* k1, int n, float thres
   for (int j = 0; j < 9; ++j) F[j] = bf[j];
   for (int i = 0; i < n; ++i) mask[i] = gv::sampson2(bf, k0[2 * i], k0[2 * i + 1], k1[2 * i], k1[2 * i + 1]) < thr2;
   return DIMB_OK;
+}
+
+// ------------------------------------------------------------------ matching heads: LightGlue assignment and tail, SuperGlue Sinkhorn
+#include "generic_kernels.cuh"
+#include "lg_assign.cuh"
+#include "lightglue_generic.cuh"
+#include "sg_assign.cuh"
+
+namespace {
+// logsigmoid of the shape-generic path, as gx_argmax_kernel evaluates it
+__global__ void log_sigmoid_kernel(const float* __restrict__ z, float* __restrict__ out, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = log_sigmoid(z[i]);
+}
+
+// dst[p] = src[p]^T for P square NP x NP blocks: grid (NP / 32, NP / 32, P), block (32, 8)
+__global__ void transpose_blocks_kernel(const float* __restrict__ src, float* __restrict__ dst, int NP) {
+  __shared__ float tile[32][33];
+  const size_t off = static_cast<size_t>(blockIdx.z) * NP * NP;
+  const int x0 = blockIdx.x * 32, y0 = blockIdx.y * 32;
+  for (int k = threadIdx.y; k < 32; k += 8) tile[k][threadIdx.x] = src[off + static_cast<size_t>(y0 + k) * NP + x0 + threadIdx.x];
+  __syncthreads();
+  for (int k = threadIdx.y; k < 32; k += 8) dst[off + static_cast<size_t>(x0 + k) * NP + y0 + threadIdx.x] = tile[threadIdx.x][k];
+}
+
+bool counts_ok(const int* c, int len, int hi) {
+  for (int k = 0; k < len; ++k)
+    if (c[k] < 0 || c[k] > hi) return false;
+  return true;
+}
+}  // namespace
+
+// The LightGlue assignment (lg_assign.cuh launch_lg_assign) on P pairs in the production layout, host fp32 inputs.
+//   sim [P][NP][NP] (NP a multiple of 128; pair p live nf[2p] x nf[2p + 1], the rest as given: padding is read only by a wrong kernel),
+//   nf / n_orig [2P], layer [P], indf [2P][NP], z [2P][NP] = logsigmoid(matchability); th: filter threshold; cap >= 1.
+// Every output starts as `sentinel` (int buffers: its bit pattern, matches: that int sign-extended) and holds kDetTail more elements:
+//   smax / slog / best / arg [2P][NP] (row statistics, row maxima and row argmaxes at side 2p; column statistics and argmaxes at side
+//   2p + 1), matches [P][cap][2], mscores [P][cap], n_matches / stop_layer [P].
+extern "C" int dimb_selftest_lg_assign(dimb_ctx* ctx, int P, int NP, const float* sim, const int* nf, const int* n_orig, const int* layer,
+                                       const int* indf, const float* z, float th, int cap, float sentinel, float* smax, float* slog,
+                                       float* best, int* arg, int64_t* matches, float* mscores, int* n_matches, int* stop_layer) {
+  if (!ctx || !sim || !nf || !n_orig || !layer || !indf || !z || !smax || !slog || !best || !arg || !matches || !mscores || !n_matches ||
+      !stop_layer)
+    return DIMB_ERR_ARG;
+  if (P < 1 || NP < 128 || NP % 128 || cap < 1 || !counts_ok(nf, 2 * P, NP) || !counts_ok(n_orig, 2 * P, INT_MAX)) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const size_t R = static_cast<size_t>(2) * P * NP, nt = static_cast<size_t>(P) * cap;
+  const int isent = sentinel_bits(sentinel);
+  DevTmp t{ctx, {}};
+  float *d_sim, *d_z, *d_smax, *d_slog, *d_best, *d_ms;
+  int *d_nf, *d_no, *d_layer, *d_indf, *d_arg, *d_nm, *d_sl;
+  long long* d_m;
+  DIMB_TRY(t.upload(&d_sim, std::vector<float>(sim, sim + static_cast<size_t>(P) * NP * NP)));
+  DIMB_TRY(t.upload(&d_z, std::vector<float>(z, z + R)));
+  DIMB_TRY(t.upload(&d_nf, std::vector<int>(nf, nf + 2 * P)));
+  DIMB_TRY(t.upload(&d_no, std::vector<int>(n_orig, n_orig + 2 * P)));
+  DIMB_TRY(t.upload(&d_layer, std::vector<int>(layer, layer + P)));
+  DIMB_TRY(t.upload(&d_indf, std::vector<int>(indf, indf + R)));
+  DIMB_TRY(t.upload(&d_smax, std::vector<float>(R + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_slog, std::vector<float>(R + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_best, std::vector<float>(R + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_arg, std::vector<int>(R + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_m, std::vector<long long>(2 * nt + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_ms, std::vector<float>(nt + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_nm, std::vector<int>(P + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_sl, std::vector<int>(P + kDetTail, isent)));
+  DIMB_TRY(launch_lg_assign(ctx, 0, P, NP, d_sim, d_nf, d_no, d_layer, d_z, d_indf, th, d_smax, d_slog, d_best, d_arg, d_m, d_ms, d_nm, d_sl,
+                            cap));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_lg_assign"));
+  DIMB_TRY(download(ctx, smax, d_smax, R + kDetTail));
+  DIMB_TRY(download(ctx, slog, d_slog, R + kDetTail));
+  DIMB_TRY(download(ctx, best, d_best, R + kDetTail));
+  DIMB_TRY(download(ctx, arg, d_arg, R + kDetTail));
+  DIMB_TRY(download(ctx, reinterpret_cast<long long*>(matches), d_m, 2 * nt + kDetTail));
+  DIMB_TRY(download(ctx, mscores, d_ms, nt + kDetTail));
+  DIMB_TRY(download(ctx, n_matches, d_nm, P + kDetTail));
+  return download(ctx, stop_layer, d_sl, P + kDetTail);
+}
+
+// The LightGlue per-layer tail (lg_assign.cuh) on P pairs, side s = rows [s NP, (s + 1) NP), live rows n_act [2P], n_orig [2P],
+// stopped_in / counter_in [P] (the state before the call).
+//   x32 [2P NP][256] given: launch_lg_tail - lg_conf_kernel (confidence weights wt / bt, matchability weights wm / bm) then
+//   lg_decide_kernel; tok and mat start as `sentinel`.  x32 null: launch_lg_decide alone on the given tok_in / mat_in [2P NP].
+//   thr: this layer's confidence threshold; depth_conf, keep_thr = 1 - width_confidence, do_stop, do_prune, prune_min as production.
+// Outputs hold kDetTail more elements: tok / mat / map [2P NP], n_next [2P] (int buffers start as the sentinel's bits), counter /
+// stopped [P] (start as counter_in / stopped_in).
+extern "C" int dimb_selftest_lg_tail(dimb_ctx* ctx, int P, int NP, const float* x32, const float* wt, float bt, const float* wm, float bm,
+                                     const float* tok_in, const float* mat_in, const int* n_act, const int* n_orig, const int* stopped_in,
+                                     const int* counter_in, int layer, float thr, float depth_conf, float keep_thr, int do_stop,
+                                     int do_prune, int prune_min, float sentinel, float* tok, float* mat, int* counter, int* stopped, int* map,
+                                     int* n_next) {
+  if (!ctx || !n_act || !n_orig || !stopped_in || !counter_in || !tok || !mat || !counter || !stopped || !map || !n_next) return DIMB_ERR_ARG;
+  if (x32 ? (!wt || !wm) : (!tok_in || !mat_in)) return DIMB_ERR_ARG;
+  if (P < 1 || NP < 1 || layer < 0 || !counts_ok(n_act, 2 * P, NP) || !counts_ok(n_orig, 2 * P, INT_MAX)) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const size_t R = static_cast<size_t>(2) * P * NP;
+  const int isent = sentinel_bits(sentinel);
+  DevTmp t{ctx, {}};
+  float *d_tok, *d_mat;
+  int *d_na, *d_no, *d_st, *d_cnt, *d_map, *d_nn;
+  std::vector<float> ht(R + kDetTail, sentinel), hm(R + kDetTail, sentinel);
+  if (!x32) {
+    std::copy(tok_in, tok_in + R, ht.begin());
+    std::copy(mat_in, mat_in + R, hm.begin());
+  }
+  std::vector<int> hs(P + kDetTail, isent), hc(P + kDetTail, isent);
+  std::copy(stopped_in, stopped_in + P, hs.begin());
+  std::copy(counter_in, counter_in + P, hc.begin());
+  DIMB_TRY(t.upload(&d_tok, ht));
+  DIMB_TRY(t.upload(&d_mat, hm));
+  DIMB_TRY(t.upload(&d_st, hs));
+  DIMB_TRY(t.upload(&d_cnt, hc));
+  DIMB_TRY(t.upload(&d_na, std::vector<int>(n_act, n_act + 2 * P)));
+  DIMB_TRY(t.upload(&d_no, std::vector<int>(n_orig, n_orig + 2 * P)));
+  DIMB_TRY(t.upload(&d_map, std::vector<int>(R + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_nn, std::vector<int>(2 * P + kDetTail, isent)));
+  if (x32) {
+    float *d_x, *d_wt, *d_wm;
+    DIMB_TRY(t.upload(&d_x, std::vector<float>(x32, x32 + R * kD)));
+    DIMB_TRY(t.upload(&d_wt, std::vector<float>(wt, wt + kD)));
+    DIMB_TRY(t.upload(&d_wm, std::vector<float>(wm, wm + kD)));
+    DIMB_TRY(launch_lg_tail(ctx, 0, P, LgRows{d_na, d_st, NP}, d_x, d_wt, bt, d_wm, bm, d_tok, d_mat, d_nn, d_no, d_st, d_cnt, d_map, layer,
+                            thr, depth_conf, keep_thr, do_stop, do_prune, prune_min));
+  } else {
+    DIMB_TRY(launch_lg_decide(ctx, 0, P, NP, d_na, d_nn, d_no, d_st, d_cnt, d_tok, d_mat, d_map, layer, thr, depth_conf, keep_thr, do_stop,
+                              do_prune, prune_min));
+  }
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_lg_tail"));
+  DIMB_TRY(download(ctx, tok, d_tok, R + kDetTail));
+  DIMB_TRY(download(ctx, mat, d_mat, R + kDetTail));
+  DIMB_TRY(download(ctx, counter, d_cnt, P + kDetTail));
+  DIMB_TRY(download(ctx, stopped, d_st, P + kDetTail));
+  DIMB_TRY(download(ctx, map, d_map, R + kDetTail));
+  return download(ctx, n_next, d_nn, 2 * P + kDetTail);
+}
+
+// The assignment of the shape-generic LightGlue for one pair, as lightglue_generic.cu runs it: gx_lse_kernel and gx_argmax_kernel in
+// both directions, then the host filter lgx_filter.  sim [m][ld] (ld >= n; m, n >= 1), raw matchability logits z0 [m] / z1 [n],
+// original indices ind0 [m] / ind1 [n].  Outputs hold kDetTail more elements and start as `sentinel` (int buffers: its bit pattern,
+// matches: that int sign-extended): rlse / ls0 / best0 / arg0 [m], clse / ls1 / best1 / arg1 [n] (ls = logsigmoid(z) as the device
+// evaluates it), matches [cap][2], mscores [cap]; n_matches [1] the full count.
+extern "C" int dimb_selftest_lgx_assign(dimb_ctx* ctx, int m, int n, int ld, const float* sim, const float* z0, const float* z1, const int* ind0,
+                                        const int* ind1, float th, int cap, float sentinel, float* rlse, float* clse, float* ls0, float* ls1,
+                                        float* best0, int* arg0, float* best1, int* arg1, int64_t* matches, float* mscores, int* n_matches) {
+  if (!ctx || !sim || !z0 || !z1 || !ind0 || !ind1 || !rlse || !clse || !ls0 || !ls1 || !best0 || !arg0 || !best1 || !arg1 || !matches ||
+      !mscores || !n_matches)
+    return DIMB_ERR_ARG;
+  if (m < 1 || n < 1 || ld < n || cap < 1) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const int isent = sentinel_bits(sentinel);
+  const size_t nm = static_cast<size_t>(m) + kDetTail, nn = static_cast<size_t>(n) + kDetTail;
+  DevTmp t{ctx, {}};
+  float *d_sim, *d_z0, *d_z1, *d_rl, *d_cl, *d_l0, *d_l1, *d_b0, *d_b1;
+  int *d_a0, *d_a1;
+  DIMB_TRY(t.upload(&d_sim, std::vector<float>(sim, sim + static_cast<size_t>(m) * ld)));
+  DIMB_TRY(t.upload(&d_z0, std::vector<float>(z0, z0 + m)));
+  DIMB_TRY(t.upload(&d_z1, std::vector<float>(z1, z1 + n)));
+  for (float** b : {&d_rl, &d_l0, &d_b0}) DIMB_TRY(t.upload(b, std::vector<float>(nm, sentinel)));
+  for (float** b : {&d_cl, &d_l1, &d_b1}) DIMB_TRY(t.upload(b, std::vector<float>(nn, sentinel)));
+  DIMB_TRY(t.upload(&d_a0, std::vector<int>(nm, isent)));
+  DIMB_TRY(t.upload(&d_a1, std::vector<int>(nn, isent)));
+  gx_lse_kernel<<<ceil_div(m * 32, 256), 256>>>(d_sim, ld, m, n, 0, d_rl);
+  DIMB_LAUNCH_CHECK(ctx);
+  gx_lse_kernel<<<ceil_div(n * 32, 256), 256>>>(d_sim, ld, m, n, 1, d_cl);
+  DIMB_LAUNCH_CHECK(ctx);
+  gx_argmax_kernel<<<ceil_div(m * 32, 256), 256>>>(d_sim, ld, m, n, d_rl, d_cl, d_z0, d_z1, 0, d_b0, d_a0);
+  DIMB_LAUNCH_CHECK(ctx);
+  gx_argmax_kernel<<<ceil_div(n * 32, 256), 256>>>(d_sim, ld, m, n, d_rl, d_cl, d_z0, d_z1, 1, d_b1, d_a1);
+  DIMB_LAUNCH_CHECK(ctx);
+  log_sigmoid_kernel<<<ceil_div(m, 256), 256>>>(d_z0, d_l0, m);
+  log_sigmoid_kernel<<<ceil_div(n, 256), 256>>>(d_z1, d_l1, n);
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_lgx_assign"));
+  DIMB_TRY(download(ctx, rlse, d_rl, nm));
+  DIMB_TRY(download(ctx, clse, d_cl, nn));
+  DIMB_TRY(download(ctx, ls0, d_l0, nm));
+  DIMB_TRY(download(ctx, ls1, d_l1, nn));
+  DIMB_TRY(download(ctx, best0, d_b0, nm));
+  DIMB_TRY(download(ctx, arg0, d_a0, nm));
+  DIMB_TRY(download(ctx, best1, d_b1, nn));
+  DIMB_TRY(download(ctx, arg1, d_a1, nn));
+  std::fill(matches, matches + 2 * static_cast<size_t>(cap) + kDetTail, static_cast<int64_t>(isent));
+  std::fill(mscores, mscores + static_cast<size_t>(cap) + kDetTail, sentinel);
+  *n_matches = lgx_filter(m, n, best0, arg0, arg1, ind0, ind1, th, matches, mscores, cap);
+  return DIMB_OK;
+}
+
+// SuperGlue's optimal-transport head (sg_assign.cuh) on P pairs: launch_sg_sinkhorn, then launch_sg_matches.
+//   scores: the P score blocks one after the other, block p [m[p]][n[p]] row-major; a pair with an empty side counts as 0 x 0, as
+//   superglue.cu's input kernel makes it.  They are laid out as production lays them: [P][NPt][NPt] with NPt = max(m, n, 1) rounded up
+//   to 128, padding `pad`, and the transposes built on the device.  alpha: bin score.  u_in / v_in [P][NPt + 1] (null: zeros, as
+//   production starts): the duals before the first half step.  wave >= 1: pairs per launch; half_steps >= 0: row pass, column pass,
+//   row pass, ... (production: 2 x sinkhorn_iterations).  th, cap: match threshold and table rows per pair.
+// Outputs hold kDetTail more elements and start as `sentinel` (int buffers: its bit pattern, matches: that int sign-extended): pc [P][4]
+// (sg_pair_consts; the fourth entry stays), u / v [P][NPt + 1], best0 / arg0 / arg1 [P][NPt], matches [P][cap][2], mscores [P][cap],
+// n_matches [P].
+extern "C" int dimb_selftest_sg_sinkhorn(dimb_ctx* ctx, int P, const int* m, const int* n, const float* scores, float alpha, float pad,
+                                         const float* u_in, const float* v_in, int wave, int half_steps, float th, int cap, float sentinel,
+                                         float* pc, float* u, float* v, float* best0, int* arg0, int* arg1, int64_t* matches, float* mscores,
+                                         int* n_matches) {
+  if (!ctx || !m || !n || !scores || !pc || !u || !v || !best0 || !arg0 || !arg1 || !matches || !mscores || !n_matches) return DIMB_ERR_ARG;
+  if (P < 1 || wave < 1 || half_steps < 0 || cap < 1 || !counts_ok(m, P, 1 << 14) || !counts_ok(n, P, 1 << 14)) return DIMB_ERR_ARG;
+  int mx = 1;
+  for (int p = 0; p < P; ++p) mx = std::max(mx, std::max(m[p], n[p]));
+  const int NPt = round_up(mx, 128), vld = NPt + 1;
+  const size_t ps = static_cast<size_t>(NPt) * NPt, nv = static_cast<size_t>(P) * vld, nb = static_cast<size_t>(P) * NPt,
+               nt = static_cast<size_t>(P) * cap;
+  std::vector<float> hs(P * ps, pad), hpc(4 * P + kDetTail, sentinel);
+  std::vector<int> na(2 * P);
+  size_t off = 0;
+  for (int p = 0; p < P; ++p) {
+    for (int i = 0; i < m[p]; ++i) std::copy(scores + off + static_cast<size_t>(i) * n[p], scores + off + static_cast<size_t>(i + 1) * n[p],
+                                             hs.begin() + p * ps + static_cast<size_t>(i) * NPt);
+    off += static_cast<size_t>(m[p]) * n[p];
+    const bool empty = m[p] == 0 || n[p] == 0;
+    na[2 * p] = empty ? 0 : m[p];
+    na[2 * p + 1] = empty ? 0 : n[p];
+    sg_pair_consts(na[2 * p], na[2 * p + 1], &hpc[4 * p]);
+  }
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const int isent = sentinel_bits(sentinel);
+  std::vector<float> hu(nv + kDetTail, sentinel), hv(nv + kDetTail, sentinel);
+  std::fill(hu.begin(), hu.begin() + nv, 0.f);
+  std::fill(hv.begin(), hv.begin() + nv, 0.f);
+  if (u_in) std::copy(u_in, u_in + nv, hu.begin());
+  if (v_in) std::copy(v_in, v_in + nv, hv.begin());
+  DevTmp t{ctx, {}};
+  float *d_sim, *d_simT, *d_alpha, *d_pc, *d_u, *d_v, *d_b0, *d_ms;
+  int *d_na, *d_a0, *d_a1, *d_nm;
+  long long* d_m;
+  DIMB_TRY(t.upload(&d_sim, hs));
+  DIMB_TRY(t.get(&d_simT, hs.size()));
+  DIMB_TRY(t.upload(&d_alpha, std::vector<float>{alpha}));
+  DIMB_TRY(t.upload(&d_pc, hpc));
+  DIMB_TRY(t.upload(&d_na, na));
+  DIMB_TRY(t.upload(&d_u, hu));
+  DIMB_TRY(t.upload(&d_v, hv));
+  DIMB_TRY(t.upload(&d_b0, std::vector<float>(nb + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_a0, std::vector<int>(nb + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_a1, std::vector<int>(nb + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_m, std::vector<long long>(2 * nt + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_ms, std::vector<float>(nt + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_nm, std::vector<int>(P + kDetTail, isent)));
+  transpose_blocks_kernel<<<dim3(NPt / 32, NPt / 32, P), dim3(32, 8)>>>(d_sim, d_simT, NPt);
+  DIMB_CUDA_OK(ctx, cudaGetLastError());
+  DIMB_TRY(launch_sg_sinkhorn(ctx, 0, P, wave, half_steps, d_sim, d_simT, NPt, d_na, d_alpha, d_u, d_v, vld, d_pc));
+  DIMB_TRY(launch_sg_matches(ctx, 0, P, d_sim, NPt, ps, NPt, d_na, d_u, d_v, vld, d_pc, th, d_b0, d_a0, d_a1, d_m, d_ms, d_nm, cap));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_sg_sinkhorn"));
+  std::copy(hpc.begin(), hpc.end(), pc);
+  DIMB_TRY(download(ctx, u, d_u, nv + kDetTail));
+  DIMB_TRY(download(ctx, v, d_v, nv + kDetTail));
+  DIMB_TRY(download(ctx, best0, d_b0, nb + kDetTail));
+  DIMB_TRY(download(ctx, arg0, d_a0, nb + kDetTail));
+  DIMB_TRY(download(ctx, arg1, d_a1, nb + kDetTail));
+  DIMB_TRY(download(ctx, reinterpret_cast<long long*>(matches), d_m, 2 * nt + kDetTail));
+  DIMB_TRY(download(ctx, mscores, d_ms, nt + kDetTail));
+  return download(ctx, n_matches, d_nm, P + kDetTail);
 }
