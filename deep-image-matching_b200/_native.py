@@ -1088,9 +1088,14 @@ class FeatureStoreDev:
                        "dimb_fstore_get")
         return {"keypoints": k, "descriptors": d, "scores": s, "tile_idx": t, "image_size": size.astype(np.int32)}
 
-    def feats_dev(self, slot: int) -> FeatsDev:
+    def feats_dev(self, slot: int, size=None) -> FeatsDev:
+        """The slot as LightGlue / NN input.  size: None (the slot header's [H,W] through size_dev), or an explicit normalisation size
+        (size0, size1) carried in the struct with size_dev NULL (LighterGlue's [W,H])."""
         f = FeatsDev()
         self.ctx.check(self.ctx.lib.dimb_fstore_feats_dev(self.h, slot, C.byref(f)), "dimb_fstore_feats_dev")
+        if size is not None:
+            f.size_dev = None
+            f.size0, f.size1 = float(size[0]), float(size[1])
         return f
 
     def sg_feats_dev(self, slot: int) -> SgFeatsDev:

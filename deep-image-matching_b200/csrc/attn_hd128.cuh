@@ -24,9 +24,8 @@ struct AttnXArgs {
 };
 
 // fp32 rows [n][ld] (head h at columns h*hd) -> fp16 hi / lo planes [H][NP][128]; rows >= n and columns >= hd are zero
-__global__ void gx_pack_rows_kernel(const float* __restrict__ src, int ld, int n, int hd, int NP, __half* __restrict__ hi,
-                                    __half* __restrict__ lo) {
-  const int row = blockIdx.x, head = blockIdx.y, c = threadIdx.x;  // 128 threads
+__device__ __forceinline__ void gx_pack_rows_one(const float* __restrict__ src, int ld, int n, int hd, int NP, __half* __restrict__ hi,
+                                                 __half* __restrict__ lo, int row, int head, int c) {
   float v = 0.f;
   if (row < n && c < hd) v = src[static_cast<size_t>(row) * ld + head * hd + c];
   __half h, l;
@@ -35,12 +34,16 @@ __global__ void gx_pack_rows_kernel(const float* __restrict__ src, int ld, int n
   hi[o] = h;
   if (lo) lo[o] = l;
 }
+__global__ void gx_pack_rows_kernel(const float* __restrict__ src, int ld, int n, int hd, int NP, __half* __restrict__ hi,
+                                    __half* __restrict__ lo) {
+  gx_pack_rows_one(src, ld, n, hd, NP, hi, lo, blockIdx.x, blockIdx.y, threadIdx.x);  // 128 threads
+}
 
 // fp32 rows [n][ld] -> transposed fp16 hi / lo planes [H][128][NP] (the K-major B operand of P V); columns >= n and rows >= hd are zero
-__global__ void gx_pack_vt_kernel(const float* __restrict__ src, int ld, int n, int hd, int NP, __half* __restrict__ hi,
-                                  __half* __restrict__ lo) {
+__device__ __forceinline__ void gx_pack_vt_block(const float* __restrict__ src, int ld, int n, int hd, int NP, __half* __restrict__ hi,
+                                                 __half* __restrict__ lo, int t0, int c0, int head) {
   __shared__ float tile[32][33];
-  const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32, head = blockIdx.z, tx = threadIdx.x, ty = threadIdx.y;  // (32, 8)
+  const int tx = threadIdx.x, ty = threadIdx.y;  // (32, 8)
   for (int k = ty; k < 32; k += 8) {
     const int tok = t0 + k, c = c0 + tx;
     tile[k][tx] = (tok < n && c < hd) ? src[static_cast<size_t>(tok) * ld + head * hd + c] : 0.f;
@@ -54,6 +57,10 @@ __global__ void gx_pack_vt_kernel(const float* __restrict__ src, int ld, int n, 
     hi[o] = h;
     if (lo) lo[o] = l;
   }
+}
+__global__ void gx_pack_vt_kernel(const float* __restrict__ src, int ld, int n, int hd, int NP, __half* __restrict__ hi,
+                                  __half* __restrict__ lo) {
+  gx_pack_vt_block(src, ld, n, hd, NP, hi, lo, blockIdx.x * 32, blockIdx.y * 32, blockIdx.z);
 }
 
 struct AttnOutX {  // O rows of one head -> fp32 [nq][ldo], head h at columns h * hd; padding columns >= hd dropped

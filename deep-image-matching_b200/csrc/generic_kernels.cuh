@@ -57,10 +57,9 @@ __global__ void __launch_bounds__(256) gx_linear_kernel(const float* __restrict_
 }
 
 // keypoint normalisation (lightglue.py:24-34) + Fourier encoding (:57-70): enc [2][N][hd] = cos / sin, each frequency twice
-__global__ void gx_posenc_kernel(const float* __restrict__ kpts, int n, float size0, float size1, const float* __restrict__ Wr /*[hd/2][2]*/,
-                                 int hd, float* __restrict__ enc, int np) {
-  const int i = blockIdx.x, f = threadIdx.x;
-  if (i >= n || f >= hd / 2) return;
+// (one keypoint i, one frequency f; shared with the batched prep of lightglue_generic.cu)
+__device__ __forceinline__ void gx_posenc_one(const float* __restrict__ kpts, int i, int f, float size0, float size1,
+                                              const float* __restrict__ Wr, int hd, float* __restrict__ enc, int np) {
   const float sc = fmaxf(size0, size1) / 2.f;
   const float x = (kpts[2 * i] - size0 / 2.f) / sc, y = (kpts[2 * i + 1] - size1 / 2.f) / sc;
   const float pr = x * Wr[2 * f] + y * Wr[2 * f + 1];
@@ -69,12 +68,16 @@ __global__ void gx_posenc_kernel(const float* __restrict__ kpts, int n, float si
   e0[0] = c, e0[1] = c;
   e0[static_cast<size_t>(np) * hd] = s, e0[static_cast<size_t>(np) * hd + 1] = s;
 }
+__global__ void gx_posenc_kernel(const float* __restrict__ kpts, int n, float size0, float size1, const float* __restrict__ Wr /*[hd/2][2]*/,
+                                 int hd, float* __restrict__ enc, int np) {
+  const int i = blockIdx.x, f = threadIdx.x;
+  if (i >= n || f >= hd / 2) return;
+  gx_posenc_one(kpts, i, f, size0, size1, Wr, hd, enc, np);
+}
 
 // Wqkv output [N][3d] interleaved as (h, hd, 3) (lightglue.py:153-154) -> q, k (rotary applied, :47-54), v, each [N][d]
-__global__ void gx_qkv_rotary_kernel(const float* __restrict__ qkv, int n, int d, int hd, const float* __restrict__ enc, int np,
-                                     float* __restrict__ q, float* __restrict__ k, float* __restrict__ v) {
-  const int i = blockIdx.x, c = threadIdx.x * 2;  // channel pair (c, c+1) of the model dimension
-  if (i >= n || c >= d) return;
+__device__ __forceinline__ void gx_qkv_rotary_one(const float* __restrict__ qkv, int i, int c, int d, int hd, const float* __restrict__ enc,
+                                                  int np, float* __restrict__ q, float* __restrict__ k, float* __restrict__ v) {
   const float* r = qkv + static_cast<size_t>(i) * 3 * d;
   const int dd = c % hd;  // position inside the head: the encoding is shared by the heads
   const float c0 = enc[static_cast<size_t>(i) * hd + dd], c1 = enc[static_cast<size_t>(i) * hd + dd + 1];
@@ -88,14 +91,21 @@ __global__ void gx_qkv_rotary_kernel(const float* __restrict__ qkv, int n, int d
   v[o] = r[c * 3 + 2];
   v[o + 1] = r[(c + 1) * 3 + 2];
 }
+__global__ void gx_qkv_rotary_kernel(const float* __restrict__ qkv, int n, int d, int hd, const float* __restrict__ enc, int np,
+                                     float* __restrict__ q, float* __restrict__ k, float* __restrict__ v) {
+  const int i = blockIdx.x, c = threadIdx.x * 2;  // channel pair (c, c+1) of the model dimension
+  if (i >= n || c >= d) return;
+  gx_qkv_rotary_one(qkv, i, c, d, hd, enc, np, q, k, v);
+}
 
 // softmax(q k^T * hd^-0.5) v, fp32.  CTA = 8 warps = 8 queries of one head sharing 32-key tiles of K and V in shared memory;
 // lane = key of the tile for the logits, lane = channel (mod 32) for the output.  Online softmax.  HDP = hd rounded up to 32.
+// The CTA body takes its query block and head explicitly (the batched path adds a grid dimension over the sides).
 template <int HDP>
-__global__ void __launch_bounds__(256) gx_attention_kernel(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
-                                                           int nq, int nk, int d, int hd, float* __restrict__ out, int ldo) {
+__device__ __forceinline__ void gx_attention_block(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
+                                                   int nq, int nk, int d, int hd, float* __restrict__ out, int ldo, int qblk, int head) {
   __shared__ float sk[32][HDP + 1], sv[32][HDP], sq[8][HDP];
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, head = blockIdx.y, qi = blockIdx.x * 8 + w;
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, qi = qblk * 8 + w;
   const int co = head * hd;
   for (int c = lane; c < HDP; c += 32) sq[w][c] = (qi < nq && c < hd) ? q[static_cast<size_t>(qi) * d + co + c] : 0.f;
   const float scale = 1.f / sqrtf(static_cast<float>(hd));
@@ -139,12 +149,15 @@ __global__ void __launch_bounds__(256) gx_attention_kernel(const float* __restri
     if (c < hd) out[static_cast<size_t>(qi) * ldo + co + c] = nk > 0 ? o[j] / l : 0.f;  // empty key set -> zeros (lightglue.py:103-104)
   }
 }
+template <int HDP>
+__global__ void __launch_bounds__(256) gx_attention_kernel(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
+                                                           int nq, int nk, int d, int hd, float* __restrict__ out, int ldo) {
+  gx_attention_block<HDP>(q, k, v, nq, nk, d, hd, out, ldo, blockIdx.x, blockIdx.y);
+}
 
 // y = gelu(layer_norm(x)) over the n features of a row, eps 1e-5, exact (erf) GELU; warp per row
-__global__ void gx_ln_gelu_kernel(const float* __restrict__ x, int rows, int n, const float* __restrict__ g, const float* __restrict__ b,
-                                  float* __restrict__ y) {
-  const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (row >= rows) return;
+__device__ __forceinline__ void gx_ln_gelu_row(const float* __restrict__ x, int row, int lane, int n, const float* __restrict__ g,
+                                               const float* __restrict__ b, float* __restrict__ y) {
   const float* r = x + static_cast<size_t>(row) * n;
   float s = 0.f;
   for (int c = lane; c < n; c += 32) s += r[c];
@@ -164,17 +177,27 @@ __global__ void gx_ln_gelu_kernel(const float* __restrict__ x, int rows, int n, 
     y[static_cast<size_t>(row) * n + c] = 0.5f * t * (1.f + erff(t * 0.70710678118654752440f));
   }
 }
-
-// z[row] = x[row] . w + b (token confidence / matchability logits); warp per row
-__global__ void gx_rowdot_kernel(const float* __restrict__ x, int ldx, int rows, int n, const float* __restrict__ w, const float* __restrict__ b,
-                                 float* __restrict__ z) {
+__global__ void gx_ln_gelu_kernel(const float* __restrict__ x, int rows, int n, const float* __restrict__ g, const float* __restrict__ b,
+                                  float* __restrict__ y) {
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (row >= rows) return;
+  gx_ln_gelu_row(x, row, lane, n, g, b, y);
+}
+
+// z[row] = x[row] . w + b (token confidence / matchability logits); warp per row
+__device__ __forceinline__ void gx_rowdot_row(const float* __restrict__ x, int ldx, int row, int lane, int n, const float* __restrict__ w,
+                                              const float* __restrict__ b, float* __restrict__ z) {
   float s = 0.f;
   for (int c = lane; c < n; c += 32) s = fmaf(x[static_cast<size_t>(row) * ldx + c], w[c], s);
 #pragma unroll
   for (int of = 16; of; of >>= 1) s += __shfl_xor_sync(0xffffffffu, s, of);
   if (lane == 0) z[row] = s + b[0];
+}
+__global__ void gx_rowdot_kernel(const float* __restrict__ x, int ldx, int rows, int n, const float* __restrict__ w, const float* __restrict__ b,
+                                 float* __restrict__ z) {
+  const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (row >= rows) return;
+  gx_rowdot_row(x, ldx, row, lane, n, w, b, z);
 }
 
 // pruning gather: dst row i = src row idx[i] for the state (stride ld, d used) and both halves of the encoding
@@ -191,10 +214,9 @@ __global__ void gx_gather_kernel(const float* __restrict__ xs, float* __restrict
 }
 
 // log-sum-exp of the rows (dir 0) or columns (dir 1) of sim [m][n] (row stride ld); warp per row / column
-__global__ void gx_lse_kernel(const float* __restrict__ sim, int ld, int m, int n, int dir, float* __restrict__ lse) {
-  const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  const int cnt = dir == 0 ? m : n, len = dir == 0 ? n : m;
-  if (i >= cnt) return;
+__device__ __forceinline__ void gx_lse_one(const float* __restrict__ sim, int ld, int m, int n, int dir, float* __restrict__ lse, int i,
+                                           int lane) {
+  const int len = dir == 0 ? n : m;
   float mx = -INFINITY;
   for (int j = lane; j < len; j += 32) mx = fmaxf(mx, dir == 0 ? sim[static_cast<size_t>(i) * ld + j] : sim[static_cast<size_t>(j) * ld + i]);
 #pragma unroll
@@ -205,17 +227,20 @@ __global__ void gx_lse_kernel(const float* __restrict__ sim, int ld, int m, int 
   for (int of = 16; of; of >>= 1) s += __shfl_xor_sync(0xffffffffu, s, of);
   if (lane == 0) lse[i] = mx + logf(s);
 }
+__global__ void gx_lse_kernel(const float* __restrict__ sim, int ld, int m, int n, int dir, float* __restrict__ lse) {
+  const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (i >= (dir == 0 ? m : n)) return;
+  gx_lse_one(sim, ld, m, n, dir, lse, i, lane);
+}
 
 __device__ __forceinline__ float log_sigmoid(float z) { return fminf(z, 0.f) - log1pf(expf(-fabsf(z))); }
 
 // row (dir 0) / column (dir 1) maximum and first argmax of scores = (sim - rlse) + (sim - clse) + logsig(z0) + logsig(z1)
 // in the association of the reference (lightglue.py:246-256: scores0 + scores1 + certainties), torch.max order (argmax_takes)
-__global__ void gx_argmax_kernel(const float* __restrict__ sim, int ld, int m, int n, const float* __restrict__ rlse,
-                                 const float* __restrict__ clse, const float* __restrict__ z0, const float* __restrict__ z1, int dir,
-                                 float* __restrict__ best, int* __restrict__ arg) {
-  const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  const int cnt = dir == 0 ? m : n, len = dir == 0 ? n : m;
-  if (i >= cnt) return;
+__device__ __forceinline__ void gx_argmax_one(const float* __restrict__ sim, int ld, int m, int n, const float* __restrict__ rlse,
+                                              const float* __restrict__ clse, const float* __restrict__ z0, const float* __restrict__ z1,
+                                              int dir, float* __restrict__ best, int* __restrict__ arg, int i, int lane) {
+  const int len = dir == 0 ? n : m;
   float bv = -INFINITY;
   int bi = 0x7fffffff;
   for (int j = lane; j < len; j += 32) {
@@ -231,6 +256,13 @@ __global__ void gx_argmax_kernel(const float* __restrict__ sim, int ld, int m, i
     if (argmax_takes(ov, oi, bv, bi)) bv = ov, bi = oi;
   }
   if (lane == 0) best[i] = bv, arg[i] = bi;
+}
+__global__ void gx_argmax_kernel(const float* __restrict__ sim, int ld, int m, int n, const float* __restrict__ rlse,
+                                 const float* __restrict__ clse, const float* __restrict__ z0, const float* __restrict__ z1, int dir,
+                                 float* __restrict__ best, int* __restrict__ arg) {
+  const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (i >= (dir == 0 ? m : n)) return;
+  gx_argmax_one(sim, ld, m, n, rlse, clse, z0, z1, dir, best, arg, i, lane);
 }
 
 }  // namespace

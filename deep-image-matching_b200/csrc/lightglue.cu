@@ -565,10 +565,7 @@ int dimb_lg_match_dev(dimb_lg* lg, int P, const dimb_feats_dev* f0, const dimb_f
                       int* d_n_matches, int* d_stop_layer, int cap, void* stream) {
   if (!lg || !f0 || !f1 || P < 1 || P > lg->conf.max_pairs || cap < 1) return DIMB_ERR_ARG;
   dimb_ctx* ctx = lg->ctx;
-  if (lg->gen) {
-    dimb_set_error(ctx, "dimb_lg_match_dev: the device-pointer entry exists for descriptor_dim 256 / 4 heads only; use dimb_lg_match");
-    return DIMB_ERR_UNSUPPORTED;
-  }
+  if (lg->gen) return lgx_match_dev(lg->gen, P, f0, f1, d_matches, d_mscores, d_n_matches, d_stop_layer, cap, static_cast<cudaStream_t>(stream));
   OwnerScope own(ctx, &lg->mem);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const dimb_lg_conf& cf = lg->conf;

@@ -10,6 +10,9 @@ int lgx_create(dimb_ctx* ctx, const float* weights, size_t n_floats, const dimb_
 void lgx_destroy(dimb_lgx* g);
 int lgx_match(dimb_lgx* g, int P, const dimb_feats* f0, const dimb_feats* f1, int64_t* matches, float* mscores, int* n_matches,
               int* stop_layer, int cap);
+// dimb_lg_match_dev for these shapes: P <= max_pairs pairs on device pointers, asynchronous on `st`, bitwise equal to lgx_match
+int lgx_match_dev(dimb_lgx* g, int P, const dimb_feats_dev* f0, const dimb_feats_dev* f1, int64_t* d_matches, float* d_mscores, int* d_n_matches,
+                  int* d_stop_layer, int cap, cudaStream_t st);
 
 // filter_matches (lightglue.py:281-297) of the shape-generic path on the host, from the row / column argmaxes a0 [n0] / a1 [n1] and the
 // row maxima b0 [n0] the device wrote: row r matches column c = a0[r] when a1[c] == r and exp(b0[r]) > th.  Matches go out in row

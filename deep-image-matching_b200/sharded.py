@@ -231,6 +231,30 @@ def kornia_conf(conf) -> dict:
     return out
 
 
+def lighterglue_conf(conf) -> dict:
+    """The ``lg_conf`` of ImageSetMatcher(matcher="lighterglue"), validated like ``kornia_conf``: only ``filter_threshold`` (default 0.1)
+    of LighterGlueMatcher's configuration reaches the network (the plugin's ``min_conf``); the network itself is ``LIGHTERGLUE_CONF``
+    (depth confidence -1, width confidence 0.95)."""
+    out = {"filter_threshold": 0.1}
+    unknown = set(conf or {}) - set(out)
+    if unknown:
+        raise ValueError(f"unknown lighterglue option(s) {sorted(unknown)}; expected some of {sorted(out)}")
+    out.update(conf or {})
+    out["filter_threshold"] = float(out["filter_threshold"])
+    return out
+
+
+def given_features_conf(sp_conf) -> tuple:
+    """(K, D) of an ImageSetMatcher(extractor=None): ``sp_conf`` = {"max_keypoints": K, "descriptor_dim": D}, both ints >= 1."""
+    unknown = set(sp_conf or {}) - {"max_keypoints", "descriptor_dim"}
+    if unknown:
+        raise ValueError(f"with extractor=None sp_conf holds max_keypoints and descriptor_dim only, got {sorted(unknown)}")
+    K, D = (sp_conf or {}).get("max_keypoints"), (sp_conf or {}).get("descriptor_dim")
+    if not all(isinstance(v, (int, np.integer)) and not isinstance(v, bool) and v >= 1 for v in (K, D)):
+        raise ValueError(f"with extractor=None sp_conf needs max_keypoints and descriptor_dim, ints >= 1, got {K!r} and {D!r}")
+    return int(K), int(D)
+
+
 TILE_SELECTIONS = ("grid", "exhaustive", "preselection")
 TILING_KEYS = ("min_matches_per_tile", "tile_overlap", "tile_preselection_size", "tile_selection", "tile_size")
 
@@ -523,6 +547,15 @@ class ImageSetMatcher:
     views, counts read on the device; the tables are KorniaMatcher._match_pairs' on the store's features, and the distance (nn / mnn)
     or ratio (snn / smnn) of every match is left in the device buffer ``ms``.  SuperPoint (256-d) and ALIKED (128-d) features.
 
+    ``extractor=None``: given features.  No extraction network is built; ``sp_conf`` is ``{"max_keypoints": K, "descriptor_dim": D}``
+    (``given_features_conf``), which sizes the store, and ``put_features`` replaces ``extract`` (``run_features`` /
+    ``run_features_verified`` chain the steps).  Tiling, pair generation, upright and a quality other than "high" need the images and
+    are refused.  ``matcher="lighterglue"`` (given 64-d XFeat features only): the LighterGlue network (``LIGHTERGLUE_CONF``;
+    ``lg_weights`` None loads the vendored checkpoint), ``lg_conf`` checked by ``lighterglue_conf`` (``filter_threshold`` only), each
+    side normalised by [W, H] as LighterGlueMatcher does; pair batches run dimb_lg_match_dev on the shape-generic batched engine, and
+    the tables are LighterGlueMatcher._match_pairs' on the store's features.  With given features "lightglue" takes input_dim = D (256
+    or 128), "superglue" D = 256 and "kornia_matcher" any D.
+
     ``verification``: None (default) matches only (``run`` / ``match``).  A dict (keys and defaults in ``verification_conf``) enables
     ``run_verified`` / ``match_verified``: every pair batch is verified on the device right after matching (dimb_gv_verify_dev on the
     store's float16 keypoints, seed ``gv_seed(seed, pair id)``).  The gate: a pair keeps its verified table iff
@@ -611,10 +644,30 @@ class ImageSetMatcher:
         import torch
 
         from . import _native
-        if matcher not in ("lightglue", "superglue", "kornia_matcher"):
-            raise ValueError(f'matcher must be "lightglue", "superglue" or "kornia_matcher", got {matcher!r}')
-        if extractor not in ("superpoint", "aliked"):
-            raise ValueError(f'extractor must be "superpoint" or "aliked", got {extractor!r}')
+        if matcher not in ("lightglue", "superglue", "kornia_matcher", "lighterglue"):
+            raise ValueError(f'matcher must be "lightglue", "superglue", "kornia_matcher" or "lighterglue", got {matcher!r}')
+        if extractor not in ("superpoint", "aliked", None):
+            raise ValueError(f'extractor must be "superpoint", "aliked" or None (given features), got {extractor!r}')
+        if matcher == "lighterglue" and extractor is not None:
+            raise ValueError(f"LighterGlue matches XFeat features only, which are given (extractor=None), not extracted by {extractor}")
+        given = None
+        if extractor is None:
+            given = given_features_conf(sp_conf)
+            for name, val, off in (("tiling", tiling, None), ("pair_generation", pair_generation, None), ("upright", upright, None),
+                                   ("quality", quality, "high")):
+                if val != off:
+                    raise ValueError(f"{name} needs the images; with extractor=None (given features) it is not supported")
+            D = given[1]
+            if matcher == "lighterglue" and D != 64:
+                raise ValueError(f"LighterGlue matches 64-d XFeat descriptors, got descriptor_dim {D}")
+            if matcher == "lightglue":
+                lg_conf = {"input_dim": D, **(lg_conf or {})}
+                if D not in (256, 128) or lg_conf["input_dim"] != D:
+                    raise ValueError(f"LightGlue on given features needs input_dim = descriptor_dim, 256 or 128, got {lg_conf['input_dim']} "
+                                     f"and {D}")
+            if matcher == "superglue" and D != 256:
+                raise ValueError(f"SuperGlue matches 256-d descriptors (with scores), got descriptor_dim {D}")
+        self.ltg_conf = lighterglue_conf(lg_conf) if matcher == "lighterglue" else None
         if extractor == "aliked" and matcher == "superglue":
             raise ValueError("SuperGlue matches SuperPoint features only; use matcher=\"lightglue\" with ALIKED")
         if extractor == "superpoint" and superpoint_weights is not None:
@@ -699,10 +752,13 @@ class ImageSetMatcher:
         self.n = n_images
         self.slots = [store_slot(i, n_images, self.world) for i in range(n_images)]
         self.extractor = extractor
-        self.cap = int(sp_conf["max_keypoints"]) if extractor == "superpoint" else int(sp_conf.get("max_num_keypoints", 4000))
+        if given is not None:
+            self.cap, self.D = given
+        else:
+            self.cap = int(sp_conf["max_keypoints"]) if extractor == "superpoint" else int(sp_conf.get("max_num_keypoints", 4000))
+            self.D = 256 if extractor == "superpoint" else 128
         if self.cap < 1:
             raise ValueError(f"the image-set matcher needs a positive keypoint limit per extraction, got {self.cap}")
-        self.D = 256 if extractor == "superpoint" else 128
         self.B, self.P = batch_images, batch_pairs
         # the network takes the largest extraction height and width of the set (a set of portrait and landscape images over-sizes its
         # workspace: 2048 x 2048 for 1536 x 2048 plus 2048 x 1536), or one tile
@@ -711,13 +767,17 @@ class ImageSetMatcher:
             eh, ew = self.tiling["tile_hw"]
         if extractor == "superpoint":
             self.sp = _native.SuperPointNet(ctx, sp_weights, max_batch=batch_images, max_height=eh, max_width=ew, **sp_conf)
-        else:
+        elif extractor == "aliked":
             self.al = _native.AlikedNet(ctx, sp_weights, max_height=eh, max_width=ew, **sp_conf)
         self.matcher = matcher
         if matcher == "superglue":
             self.sg = _native.SuperGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=self.cap, **lg_conf)
         elif matcher == "lightglue":
             self.lg = _native.LightGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=self.cap, **lg_conf)
+        elif matcher == "lighterglue":
+            from .matchers.lighterglue import LIGHTERGLUE_CONF, lighterglue_weights
+            self.lg = _native.LightGlueNet(ctx, lighterglue_weights() if lg_weights is None else lg_weights, max_pairs=batch_pairs,
+                                           max_kpts=self.cap, filter_threshold=self.ltg_conf["filter_threshold"], **LIGHTERGLUE_CONF)
         self.ipr = images_per_rank(n_images, self.world)
         t_max = 1 if self.tiling is None else max(len(g["origins"]) for g in grids.values())
         self.store = _native.FeatureStoreDev(ctx, self.world * self.ipr, t_max * self.cap, self.D)
@@ -732,10 +792,11 @@ class ImageSetMatcher:
             self.tiles = torch.zeros(n_ext, eh, ew, self.C, device=dev)
         if self.level:  # the resized images of one extraction batch (tiled: of one cut), one flat buffer viewed per size
             self.resized = torch.zeros(max(n_img[s] * ext[s][0] * ext[s][1] for s in shapes) * self.C, device=dev)
-        self.kp = torch.zeros(n_ext, self.cap, 2, device=dev)
-        self.sc = torch.zeros(n_ext, self.cap, device=dev)
-        self.de = torch.zeros(n_ext, self.D, self.cap, device=dev)
-        self.cnt = torch.zeros(n_ext, dtype=torch.int32, device=dev)
+        if extractor is not None:
+            self.kp = torch.zeros(n_ext, self.cap, 2, device=dev)
+            self.sc = torch.zeros(n_ext, self.cap, device=dev)
+            self.de = torch.zeros(n_ext, self.D, self.cap, device=dev)
+            self.cnt = torch.zeros(n_ext, dtype=torch.int32, device=dev)
         self.m = torch.zeros(batch_pairs, self.cap, 2, dtype=torch.int64, device=dev)
         self.ms = torch.zeros(batch_pairs, self.cap, device=dev)
         self.nm = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
@@ -808,6 +869,8 @@ class ImageSetMatcher:
         first turned by its images' rotations at full size (dimb_rot90_dev, one launch per batch into one buffer of the batch,
         ``_extract_turned``); everything else (quality, tile cut, extractor, by rotated size) runs on the rotated images.  The
         low-resolution sets were filled by ``upright`` from the unrotated images."""
+        if self.extractor is None:
+            raise RuntimeError("ImageSetMatcher was built with extractor=None: its features are given with put_features()")
         st = self.torch.cuda.current_stream().cuda_stream
         if self.up is not None:
             if self.rotations is None:
@@ -826,6 +889,32 @@ class ImageSetMatcher:
             for low in lows:
                 low.extract(src, ids, [self.slots[i] for i in ids], st)
             self._extract_batch(src, ids, H, W, st)
+
+    def put_features(self, feats, image_ids):
+        """Phase 1 with given features (extractor=None), in place of ``extract``: this rank's images `image_ids` as FeaturesDicts in
+        get_features' contract (keypoints (N,2), descriptors (D,N), scores (N,), image_size [H,W]), put into their store slots with the
+        float16 cast of the h5 writer (FeatureStoreDev.put).  Every entry is checked before the first put: image_size must be the
+        image's declared size, D the set's descriptor_dim and N at most max_keypoints (ValueError otherwise)."""
+        if self.extractor is not None:
+            raise RuntimeError(f"put_features needs an ImageSetMatcher built with extractor=None, not {self.extractor!r}")
+        if len(feats) != len(image_ids):
+            raise ValueError(f"put_features needs one FeaturesDict per image id: {len(feats)} for {len(image_ids)} ids")
+        for f, i in zip(feats, image_ids):
+            k, d = np.asarray(f["keypoints"]), np.asarray(f["descriptors"])
+            n = k.shape[0] if k.ndim == 2 and k.shape[1] == 2 else -1
+            if n < 0:
+                raise ValueError(f"image {i}: keypoints must be (N,2), got {k.shape}")
+            if d.shape != (self.D, n):
+                raise ValueError(f"image {i}: descriptors must be ({self.D},{n}) for descriptor_dim {self.D}, got {d.shape}")
+            if n > self.cap:
+                raise ValueError(f"image {i}: {n} keypoints, above max_keypoints={self.cap}")
+            if f.get("scores") is not None and np.asarray(f["scores"]).shape != (n,):
+                raise ValueError(f"image {i}: scores must be ({n},), got {np.asarray(f['scores']).shape}")
+            size = np.asarray(f.get("image_size", ())).ravel()
+            if size.shape != (2,) or tuple(int(v) for v in size) != tuple(self.sizes[i]) or np.any(size != np.round(size)):
+                raise ValueError(f"image {i}: image_size must be its declared size {list(self.sizes[i])} ([H,W]), got {size.tolist()}")
+        for f, i in zip(feats, image_ids):
+            self.store.put(self.slots[i], f)
 
     def _extract_batch(self, src, ids, H, W, st):
         """Untiled extraction of the H x W images `src` (at most batch_images) of images `ids` into their slots: quality's resize, the
@@ -986,6 +1075,11 @@ class ImageSetMatcher:
         elif self.matcher == "kornia_matcher":  # distances / ratios go to ms
             self.ctx.nn_match_batch_dev([store.feats_dev(s) for s in s0], [store.feats_dev(s) for s in s1], self.D, self.nn_conf["match_mode"],
                                         self.nn_conf["th"], self.m.data_ptr(), self.ms.data_ptr(), self.nm.data_ptr(), self.cap, st)
+        elif self.matcher == "lighterglue":  # LighterGlueMatcher's [H,W] -> [W,H] swap of image_size, as explicit sizes
+            by_slot = {self.slots[i]: i for i in range(self.n)}
+            f0 = [store.feats_dev(s, size=self.sizes[by_slot[s]][::-1]) for s in s0]
+            f1 = [store.feats_dev(s, size=self.sizes[by_slot[s]][::-1]) for s in s1]
+            self.lg.match_dev(f0, f1, self.m.data_ptr(), self.ms.data_ptr(), self.nm.data_ptr(), self.sl.data_ptr(), self.cap, st)
         else:
             self.lg.match_dev([store.feats_dev(s) for s in s0], [store.feats_dev(s) for s in s1], self.m.data_ptr(), self.ms.data_ptr(),
                               self.nm.data_ptr(), self.sl.data_ptr(), self.cap, st)
@@ -1249,6 +1343,18 @@ class ImageSetMatcher:
         """extract -> exchange -> match and verify my share -> gather to rank 0.  Returns, on rank 0, the list of
         (raw, verified, F, n_inliers) per pair (None elsewhere); ``export_colmap`` turns it into a COLMAP database."""
         return self._run(self.match_verified, gather_verified, d_images, my_image_ids, pairs, costs, tile_pairs)
+
+    def run_features(self, feats, my_image_ids, pairs, costs=None):
+        """``run`` with given features: put_features -> exchange -> match my share -> gather to rank 0."""
+        self.put_features(feats, my_image_ids)
+        self.exchange()
+        return self._match_share(self.match, gather_match_tables, pairs, costs, None)
+
+    def run_features_verified(self, feats, my_image_ids, pairs, costs=None):
+        """``run_verified`` with given features: put_features -> exchange -> match and verify my share -> gather to rank 0."""
+        self.put_features(feats, my_image_ids)
+        self.exchange()
+        return self._match_share(self.match_verified, gather_verified, pairs, costs, None)
 
     def export_colmap(self, pairs, results, database_path, image_names=None, **kwargs) -> dict:
         """Rank 0: the COLMAP database of this image set (``export_verified_to_colmap`` on this matcher's feature store)."""
