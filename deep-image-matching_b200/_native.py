@@ -220,6 +220,7 @@ def load_selftest_library():
         lib.dimb_selftest_attention.argtypes = [vp, ip, vp, vp, vp, vp, ip, ip, ip, ip, vp, vp, ip, fp, fp, fp]
         lib.dimb_selftest_nms_plan.argtypes = [ip, ip, vp]
         lib.dimb_selftest_detect.argtypes = [vp, vp] + [ip] * 5 + [fp, vp, ip, ip, ip, fp] + [vp] * 8
+        lib.dimb_selftest_select.argtypes = [vp, vp] + [ip] * 5 + [fp, vp] + [ip] * 5 + [fp] + [vp] * 7 + [ip, vp]
         lib.dimb_selftest_sp_softmax.argtypes = [vp, vp, ip, ip, ip, fp, vp]
         lib.dimb_selftest_sp_describe.argtypes = [vp] * 5 + [ip] * 5 + [fp, vp, vp, vp]
         lib.dimb_selftest_lg_assign.argtypes = [vp, ip, ip] + [vp] * 6 + [fp, ip, fp] + [vp] * 8
@@ -381,6 +382,30 @@ class SelfTest:
         out = {k: raw[k][:m].reshape(shapes.get(k, (B,))) for k, (_, m) in bufs.items()}
         out.update({k + "_tail": raw[k][m:] for k, (_, m) in bufs.items()})
         out["plan"] = tuple(int(p) for p in plan)
+        return out
+
+    def select(self, scores: np.ndarray, r: int, K: int, cut: int = 0, thr: float = 0.0, thr_per_image=None, border: int = 0,
+               cap: int | None = None, sort_all: bool = False, grid: bool = False, sentinel: float = -777.0, iters: int = 0) -> dict:
+        """detect() with the top-k selection of any K >= 1 (dimb_selftest_select).  sort_all: ALIKED's top-k mode (sorted even when
+        count <= K, then the first non-candidate pixels up to K; K <= H * W).  grid: the grid-wide path whatever K (default: the path
+        production runs for K).  iters > 0: the selection alone is timed over that many more runs, out["ms"] per run.  Returns
+        detect()'s dict without plan."""
+        s = np.ascontiguousarray(scores, np.float32)
+        B, H, W = s.shape
+        cap = int(cap if cap is not None else K)
+        tp = None if thr_per_image is None else np.ascontiguousarray(thr_per_image, np.float32)
+        n, ns = B * H * W, B * cap
+        bufs = {"nms": (np.float32, n), "cand_count": (np.int32, B), "cand_idx": (np.int32, n), "cand_score": (np.float32, n),
+                "sel_idx": (np.int32, ns), "sel_score": (np.float32, ns), "sel_count": (np.int32, B)}
+        raw = {k: np.zeros(m + DET_TAIL, t) for k, (t, m) in bufs.items()}
+        ms = np.zeros(1, np.float32)
+        self.check(self.lib.dimb_selftest_select(self.h, _ptr(s), B, H, W, int(r), int(cut), float(thr), None if tp is None else _ptr(tp),
+                                                 int(border), int(K), cap, int(bool(sort_all)), int(bool(grid)), float(sentinel),
+                                                 *(_ptr(raw[k]) for k in bufs), int(iters), _ptr(ms)), "selftest_select")
+        shapes = {"nms": (B, H, W), "cand_idx": (B, H * W), "cand_score": (B, H * W), "sel_idx": (B, cap), "sel_score": (B, cap)}
+        out = {k: raw[k][:m].reshape(shapes.get(k, (B,))) for k, (_, m) in bufs.items()}
+        out.update({k + "_tail": raw[k][m:] for k, (_, m) in bufs.items()})
+        out["ms"] = float(ms[0])
         return out
 
     def sp_softmax(self, logits: np.ndarray, B: int, h: int, w: int, sentinel: float = -777.0):
@@ -859,8 +884,13 @@ def pack_aliked_weights(w: dict) -> np.ndarray:
     return np.ascontiguousarray(np.concatenate([np.asarray(w[n], np.float32).ravel() for n in aliked_weight_names()]))
 
 
+ALIKED_N_LIMIT = 20000  # the keypoint cut of ALIKED's threshold / mean modes when max_num_keypoints <= 0 (aliked.py:585)
+
+
 class AlikedNet:
-    """Handle on dimb_aliked: ALIKED-n16(rot) extraction of one image per call (the reference path is batch-1)."""
+    """Handle on dimb_aliked: ALIKED-n16(rot) extraction of one image per call (the reference path is batch-1).  Detection modes as
+    the LightGlue port's DKD: threshold (detection_threshold > 0), top-k (detection_threshold <= 0 < max_num_keypoints: exactly
+    max_num_keypoints keypoints) and mean (both <= 0)."""
 
     def __init__(self, ctx: Context, weights: dict, max_num_keypoints=4000, detection_threshold=0.2, nms_radius=2,
                  max_height=1024, max_width=1024):
@@ -877,7 +907,7 @@ class AlikedNet:
         H, W = image.shape[:2]
         ch = 1 if image.ndim == 2 else image.shape[2]
         k = self.conf.max_num_keypoints
-        cap = cap or (k if k > 0 else 16384)
+        cap = cap or (k if k > 0 else ALIKED_N_LIMIT)  # top-k mode returns exactly k, the other modes at most k (or n_limit)
         while True:
             kp = np.zeros((cap, 2), np.float32)
             sc = np.zeros(cap, np.float32)

@@ -10,7 +10,7 @@
 //   al_conv1x1_kernel        laterals, downsample shortcuts, score_head.0
 //   al_deform_conv_kernel    torchvision.ops.deform_conv2d semantics (blocks 3-4): offsets from a 3x3 conv, clamped
 //   al_avgpool_kernel, al_aggregate_kernel (bilinear x2/x8/x32, align_corners=True, concat), al_normalize_kernel
-//   detect.cuh               simple_nms, threshold + border compaction, n_limit selection (shared with SuperPoint)
+//   detect.cuh               simple_nms, threshold + border compaction, n_limit / top-k selection (shared with SuperPoint)
 //   al_dkd_refine_kernel     soft-argmax (T = 0.1) sub-pixel keypoints, score dispersity, bilinear score
 //   al_sddh_*                deformable descriptor head: offsets + sampling kernels, two tensor-core GEMMs (gemm.cuh)
 #include <algorithm>
@@ -538,10 +538,10 @@ __global__ void al_sddh_norm_kernel(const float* __restrict__ d /*[cap][128]*/, 
   desc[static_cast<size_t>(lane * 4 + 3) * cap + k] = v.w * inv;
 }
 
-// thr_out = thr if some pixel passed it, else mean(score_map) (aliked.py:158-160)
+// thr_out = thr if some pixel passed it, else mean(score_map) (aliked.py:158-160); cand_count null: always the mean (mean mode)
 __global__ void __launch_bounds__(1024) al_threshold_kernel(const float* __restrict__ score, int HW, const int* __restrict__ cand_count,
                                                             float thr, float* __restrict__ thr_out) {
-  if (*cand_count > 0) {
+  if (cand_count && *cand_count > 0) {
     if (threadIdx.x == 0) *thr_out = thr;
     return;
   }
@@ -590,9 +590,15 @@ struct dimb_aliked {
   float *cand_score, *sel_score, *kxy, *disp, *kscore, *o_kpts, *o_desc;
   float* thr_dev = nullptr;
   int sel_cap = 0, out_cap = 0;
+  TopkScratch topk;  // grid-wide top-k (keypoint limit > kMaxTopK)
 };
 
 namespace {
+
+constexpr int kAlikedNLimit = 20000;  // ALIKED.n_limit_max (aliked.py:585): the cut when max_num_keypoints <= 0
+
+// Keypoints the selection keeps at most: top-k mode's K, or threshold / mean mode's n_limit (aliked.py:585-592)
+int aliked_limit(const dimb_aliked_conf& c) { return c.max_num_keypoints > 0 ? c.max_num_keypoints : kAlikedNLimit; }
 
 int up_f32(dimb_ctx* ctx, float** d, const float* src, size_t n) {
   DIMB_TRY(dimb_alloc_t(ctx, d, n, false));
@@ -702,9 +708,8 @@ int dimb_aliked_create(dimb_ctx* ctx, const float* weights, size_t n_floats, con
                             " (aliked-n16 / aliked-n16rot)");
     return DIMB_ERR_ARG;
   }
-  if (conf->nms_radius < 1 || conf->nms_radius > 5 || conf->max_height < 32 || conf->max_width < 32 || conf->detection_threshold <= 0.f ||
-      conf->max_num_keypoints > kMaxTopK) {
-    dimb_set_error(ctx, "dimb_aliked_create: unsupported configuration (threshold mode with detection_threshold > 0 only)");
+  if (conf->nms_radius < 1 || conf->nms_radius > 5 || conf->max_height < 32 || conf->max_width < 32) {
+    dimb_set_error(ctx, "dimb_aliked_create: unsupported configuration (nms_radius 1..5, max_height and max_width >= 32)");
     return DIMB_ERR_UNSUPPORTED;
   }
   dimb_aliked* al = new dimb_aliked();
@@ -816,6 +821,7 @@ int dimb_aliked_create(dimb_ctx* ctx, const float* weights, size_t n_floats, con
   DIMB_TRY(dimb_alloc_t(ctx, &al->cand_count, 1));
   DIMB_TRY(dimb_alloc_t(ctx, &al->sel_count, 1));
   DIMB_TRY(dimb_alloc_t(ctx, &al->thr_dev, 1));
+  if (aliked_limit(*conf) > kMaxTopK) DIMB_TRY(topk_reserve(ctx, al->topk, 1, static_cast<int>(P), aliked_limit(*conf)));
   *out = guard.release();
   return DIMB_OK;
 }
@@ -843,8 +849,15 @@ int dimb_aliked_extract_dev(dimb_aliked* al, const float* image, int H, int W, i
     dimb_set_error(ctx, "dimb_aliked_extract: image larger than the workspace given at create time");
     return DIMB_ERR_ARG;
   }
-  const int n_limit = cf.max_num_keypoints > 0 ? cf.max_num_keypoints : 20000;
-  const int K = n_limit <= kMaxTopK ? n_limit : -1;  // beyond the sort capacity: keep all, fail if the limit would have fired
+  // top-k mode (detection_threshold <= 0 < max_num_keypoints): the K largest of the border-zeroed NMS map, as torch.topk; otherwise
+  // K is the n_limit cut of threshold / mean mode
+  const bool topk = cf.detection_threshold <= 0.f && cf.max_num_keypoints > 0;
+  const int K = aliked_limit(cf);
+  if (topk && static_cast<long long>(K) > static_cast<long long>(H) * W) {
+    dimb_set_error(ctx, "dimb_aliked_extract: max_num_keypoints " + std::to_string(K) + " exceeds the " + std::to_string(H * W) +
+                            " pixels of the image (top-k mode)");
+    return DIMB_ERR_ARG;
+  }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t P = static_cast<size_t>(Hp) * Wp;
   const int H2 = Hp / 2, W2 = Wp / 2, H8 = Hp / 8, W8 = Wp / 8, H32 = Hp / 32, W32 = Wp / 32;
@@ -901,21 +914,29 @@ int dimb_aliked_extract_dev(dimb_aliked* al, const float* image, int H, int W, i
   {
   ProfScope prof(ctx, st, "al.detect");
   DIMB_TRY(launch_nms(ctx, st, al->score, al->nms, 1, H, W, r, kNmsProductionVer));
-  // threshold mode (aliked.py:152-160): nms > detection_threshold; if nothing passes, nms > mean(score_map).
-  // Decided on the device: count, then al_threshold_kernel fixes the threshold, then count / scan / compact with it.
   const CandBufs cand{al->chunk_count, al->chunk_off, al->cand_count, al->cand_idx, al->cand_score};
-  DIMB_TRY(launch_candidates(ctx, st, al->nms, cand, 1, H, W, cf.detection_threshold, r, nullptr, false));
-  al_threshold_kernel<<<1, 1024, 0, st>>>(al->score, H * W, al->cand_count, cf.detection_threshold, al->thr_dev);
-  DIMB_LAUNCH_CHECK(ctx);
-  DIMB_TRY(launch_candidates(ctx, st, al->nms, cand, 1, H, W, 0.f, r, al->thr_dev, true));
+  if (topk) {
+    // the nonzero pixels of the border-zeroed NMS map; topk_fill_kernel appends zero pixels when there are fewer than K
+    DIMB_TRY(launch_candidates(ctx, st, al->nms, cand, 1, H, W, 0.f, r, nullptr, true));
+  } else {
+    // threshold mode (aliked.py:152-160): nms > detection_threshold; if nothing passes, nms > mean(score_map).  Mean mode
+    // (detection_threshold <= 0): nms > mean(score_map).  Decided on the device: count, then al_threshold_kernel fixes the
+    // threshold, then count / scan / compact with it.
+    const bool mean_mode = cf.detection_threshold <= 0.f;
+    if (!mean_mode) DIMB_TRY(launch_candidates(ctx, st, al->nms, cand, 1, H, W, cf.detection_threshold, r, nullptr, false));
+    al_threshold_kernel<<<1, 1024, 0, st>>>(al->score, H * W, mean_mode ? nullptr : al->cand_count, cf.detection_threshold, al->thr_dev);
+    DIMB_LAUNCH_CHECK(ctx);
+    DIMB_TRY(launch_candidates(ctx, st, al->nms, cand, 1, H, W, 0.f, r, al->thr_dev, true));
+  }
+  const int scap = std::max(cap, K);  // the selection writes up to K entries whatever cap is
   if (al->sel_cap < cap) {
     if (al->sel_cap > 0)  // release the smaller per-keypoint buffers of an earlier call
       for (void* old : {static_cast<void*>(al->sel_idx), static_cast<void*>(al->sel_score), static_cast<void*>(al->kxy), static_cast<void*>(al->kscore),
                         static_cast<void*>(al->off), static_cast<void*>(al->dsc), static_cast<void*>(al->fsh), static_cast<void*>(al->fsl),
                         static_cast<void*>(al->f2h), static_cast<void*>(al->f2l)})
         dimb_free(ctx, old);
-    DIMB_TRY(dimb_alloc_t(ctx, &al->sel_idx, cap));
-    DIMB_TRY(dimb_alloc_t(ctx, &al->sel_score, cap));
+    DIMB_TRY(dimb_alloc_t(ctx, &al->sel_idx, scap));
+    DIMB_TRY(dimb_alloc_t(ctx, &al->sel_score, scap));
     DIMB_TRY(dimb_alloc_t(ctx, &al->kxy, static_cast<size_t>(cap) * 2));
     DIMB_TRY(dimb_alloc_t(ctx, &al->kscore, cap));
     const size_t rows = static_cast<size_t>(round_up(cap, kTileM)) * 16;  // SDDH operands, padded to whole GEMM tiles
@@ -931,7 +952,7 @@ int dimb_aliked_extract_dev(dimb_aliked* al, const float* image, int H, int W, i
     DIMB_TRY(dimb_tmap_2d(ctx, &al->m_f2[1], al->f2l, rows / 16, 2048, 2048, kTileM));
     al->sel_cap = cap;
   }
-  DIMB_TRY(launch_select(ctx, st, cand, al->sel_idx, al->sel_score, count, 1, H * W, K, cap));
+  DIMB_TRY(launch_select(ctx, st, cand, al->sel_idx, al->sel_score, count, 1, H * W, K, scap, &al->topk, topk));
   al_dkd_refine_kernel<<<ceil_div(cap, 128), 128, 0, st>>>(al->score, H, W, r, al->sel_idx, count, cap, al->kxy, scores, al->kscore);
   DIMB_LAUNCH_CHECK(ctx);
   }
@@ -997,11 +1018,6 @@ int dimb_aliked_extract(dimb_aliked* al, const float* image, int H, int W, int c
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(scores, al->disp, static_cast<size_t>(cap) * sizeof(float), cudaMemcpyDeviceToHost, st));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(desc, al->o_desc, static_cast<size_t>(cap) * 128 * sizeof(float), cudaMemcpyDeviceToHost, st));
   DIMB_CUDA_OK(ctx, cudaStreamSynchronize(st));
-  const int n_limit = al->conf.max_num_keypoints > 0 ? al->conf.max_num_keypoints : 20000;
-  if (*count > n_limit) {
-    dimb_set_error(ctx, "dimb_aliked_extract: more than 16384 candidates with max_num_keypoints <= 0 is not supported");
-    return DIMB_ERR_UNSUPPORTED;
-  }
   if (*count > cap) {
     dimb_set_error(ctx, "dimb_aliked_extract: more keypoints than cap");
     return DIMB_ERR_CAPACITY;

@@ -441,8 +441,11 @@ __global__ void __launch_bounds__(256) sp_compact_kernel(const float* __restrict
 }
 
 // ------------------------------------------------------------------ top-k (superpoint.py:74-78): radix select + bitonic sort
-// One CTA per image.  If count <= K (or K < 0): keep everything in row-major order.  Otherwise pick the K
+// One CTA per image, K <= kMaxTopK.  If count <= K (or K < 0): keep everything in row-major order.  Otherwise pick the K
 // largest scores (ties at the cut resolved by smaller pixel index) and order them score-desc, index-asc.
+// kSortAll (ALIKED's top-k mode, torch.topk returns sorted values): count <= K keeps every candidate too, but sorted; sel_count is K
+// and topk_fill_kernel writes slots count .. K-1.
+template <bool kSortAll>
 __global__ void __launch_bounds__(kSelThreads) sp_select_kernel(const int* __restrict__ cand_idx, const float* __restrict__ cand_score,
                                                                 const int* __restrict__ cand_count, int* __restrict__ sel_idx,
                                                                 float* __restrict__ sel_score, int* __restrict__ sel_count,
@@ -456,7 +459,7 @@ __global__ void __launch_bounds__(kSelThreads) sp_select_kernel(const int* __res
   const float* cs = cand_score + static_cast<size_t>(b) * HW;
   int* oi = sel_idx + static_cast<size_t>(b) * cap;
   float* os = sel_score + static_cast<size_t>(b) * cap;
-  if (K < 0 || C <= K) {
+  if (!kSortAll && (K < 0 || C <= K)) {
     if (t == 0) sel_count[b] = C;  // host checks C <= cap
     for (int i = t; i < C && i < cap; i += blockDim.x) {
       oi[i] = ci[i];
@@ -464,78 +467,85 @@ __global__ void __launch_bounds__(kSelThreads) sp_select_kernel(const int* __res
     }
     return;
   }
-  // ---- radix select of the K-th largest score (scores > 0 -> float bits are order preserving)
-  if (t == 0) {
-    s_prefix = 0;
-    s_remaining = K;
-  }
-  __syncthreads();
-  for (int shift = 24; shift >= 0; shift -= 8) {
-    if (t < 256) hist[t] = 0;
+  int n = K;  // keys to sort
+  if (kSortAll && C <= K) {
+    for (int i = t; i < C; i += blockDim.x)
+      keys[i] = (static_cast<unsigned long long>(~__float_as_uint(cs[i])) << 32) | static_cast<unsigned>(ci[i]);
+    n = C;
+  } else {
+    // ---- radix select of the K-th largest score (scores > 0 -> float bits are order preserving)
+    if (t == 0) {
+      s_prefix = 0;
+      s_remaining = K;
+    }
     __syncthreads();
-    const unsigned prefix = s_prefix;
-    const unsigned himask = shift == 24 ? 0u : (0xffffffffu << (shift + 8));
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      if (t < 256) hist[t] = 0;
+      __syncthreads();
+      const unsigned prefix = s_prefix;
+      const unsigned himask = shift == 24 ? 0u : (0xffffffffu << (shift + 8));
+      for (int i = t; i < C; i += blockDim.x) {
+        const unsigned u = __float_as_uint(cs[i]);
+        if ((u & himask) == prefix) atomicAdd(&hist[(u >> shift) & 255u], 1u);
+      }
+      __syncthreads();
+      if (t == 0) {
+        unsigned rem = s_remaining, d = 255;
+        for (;; --d) {  // walk digits from large to small
+          if (hist[d] >= rem) break;
+          rem -= hist[d];
+          if (d == 0) break;
+        }
+        s_prefix = prefix | (d << shift);
+        s_remaining = rem;  // how many elements equal to the final threshold are still needed
+      }
+      __syncthreads();
+    }
+    const unsigned T = s_prefix;       // bit pattern of the K-th largest score
+    const unsigned need_ties = s_remaining;
+    if (t == 0) {
+      s_ngreater = 0;
+      s_tiepos = 0;
+    }
+    __syncthreads();
+    // ---- gather: strictly greater first (any order, sorted below), then the first `need_ties` ties by index.
+    // key = (~scorebits << 32) | pixel index : ascending key order == score desc, index asc
     for (int i = t; i < C; i += blockDim.x) {
       const unsigned u = __float_as_uint(cs[i]);
-      if ((u & himask) == prefix) atomicAdd(&hist[(u >> shift) & 255u], 1u);
-    }
-    __syncthreads();
-    if (t == 0) {
-      unsigned rem = s_remaining, d = 255;
-      for (;; --d) {  // walk digits from large to small
-        if (hist[d] >= rem) break;
-        rem -= hist[d];
-        if (d == 0) break;
+      if (u > T) {
+        const unsigned pos = atomicAdd(&s_ngreater, 1u);
+        keys[pos] = (static_cast<unsigned long long>(~u) << 32) | static_cast<unsigned>(ci[i]);
       }
-      s_prefix = prefix | (d << shift);
-      s_remaining = rem;  // how many elements equal to the final threshold are still needed
     }
     __syncthreads();
-  }
-  const unsigned T = s_prefix;       // bit pattern of the K-th largest score
-  const unsigned need_ties = s_remaining;
-  if (t == 0) {
-    s_ngreater = 0;
-    s_tiepos = 0;
-  }
-  __syncthreads();
-  // ---- gather: strictly greater first (any order, sorted below), then the first `need_ties` ties by index.
-  // key = (~scorebits << 32) | pixel index : ascending key order == score desc, index asc
-  for (int i = t; i < C; i += blockDim.x) {
-    const unsigned u = __float_as_uint(cs[i]);
-    if (u > T) {
-      const unsigned pos = atomicAdd(&s_ngreater, 1u);
-      keys[pos] = (static_cast<unsigned long long>(~u) << 32) | static_cast<unsigned>(ci[i]);
+    const unsigned G = s_ngreater;  // == K - need_ties
+    // ties: candidates are stored in increasing pixel index, so rank among ties = number of earlier ties
+    for (int base = 0; base < C; base += blockDim.x) {
+      const int i = base + t;
+      const bool tie = i < C && __float_as_uint(cs[i]) == T;
+      // block-wide ordered rank via ballot + warp counts
+      __shared__ unsigned wcnt[32];
+      const unsigned bal = __ballot_sync(0xffffffffu, tie);
+      if ((t & 31) == 0) wcnt[t >> 5] = __popc(bal);
+      __syncthreads();
+      unsigned before = s_tiepos;
+      for (int wv = 0; wv < (t >> 5); ++wv) before += wcnt[wv];
+      before += __popc(bal & ((1u << (t & 31)) - 1u));
+      if (tie && before < need_ties)
+        keys[G + before] = (static_cast<unsigned long long>(~T) << 32) | static_cast<unsigned>(ci[i]);
+      __syncthreads();
+      if (t == 0) {
+        unsigned tot = 0;
+        for (int wv = 0; wv < 32; ++wv) tot += wcnt[wv];
+        s_tiepos += tot;
+      }
+      __syncthreads();
     }
   }
-  __syncthreads();
-  const unsigned G = s_ngreater;  // == K - need_ties
-  // ties: candidates are stored in increasing pixel index, so rank among ties = number of earlier ties
-  for (int base = 0; base < C; base += blockDim.x) {
-    const int i = base + t;
-    const bool tie = i < C && __float_as_uint(cs[i]) == T;
-    // block-wide ordered rank via ballot + warp counts
-    __shared__ unsigned wcnt[32];
-    const unsigned bal = __ballot_sync(0xffffffffu, tie);
-    if ((t & 31) == 0) wcnt[t >> 5] = __popc(bal);
-    __syncthreads();
-    unsigned before = s_tiepos;
-    for (int wv = 0; wv < (t >> 5); ++wv) before += wcnt[wv];
-    before += __popc(bal & ((1u << (t & 31)) - 1u));
-    if (tie && before < need_ties)
-      keys[G + before] = (static_cast<unsigned long long>(~T) << 32) | static_cast<unsigned>(ci[i]);
-    __syncthreads();
-    if (t == 0) {
-      unsigned tot = 0;
-      for (int wv = 0; wv < 32; ++wv) tot += wcnt[wv];
-      s_tiepos += tot;
-    }
-    __syncthreads();
-  }
-  // ---- bitonic sort of K keys padded to a power of two
+  // ---- bitonic sort of n keys padded to a power of two
   int P = 1;
-  while (P < K) P <<= 1;
-  for (int i = K + t; i < P; i += blockDim.x) keys[i] = ~0ull;
+  while (P < n) P <<= 1;
+  for (int i = n + t; i < P; i += blockDim.x) keys[i] = ~0ull;
   __syncthreads();
   for (int k = 2; k <= P; k <<= 1)
     for (int j = k >> 1; j > 0; j >>= 1) {
@@ -552,11 +562,342 @@ __global__ void __launch_bounds__(kSelThreads) sp_select_kernel(const int* __res
       }
       __syncthreads();
     }
-  for (int i = t; i < K; i += blockDim.x) {
+  for (int i = t; i < n; i += blockDim.x) {
     oi[i] = static_cast<int>(keys[i] & 0xffffffffull);
     os[i] = __uint_as_float(~static_cast<unsigned>(keys[i] >> 32));
   }
   if (t == 0) sel_count[b] = K;
+}
+
+
+// Sort-always selection with count C < K: slot C + j takes the j-th pixel (row-major) that is not a candidate, with score 0 (the NMS
+// value torch.topk reports for it when the candidates are exactly the nonzero pixels, as in ALIKED's top-k mode).  Needs K <= HW.
+__global__ void __launch_bounds__(256) topk_fill_kernel(const int* __restrict__ cand_idx, const int* __restrict__ cand_count,
+                                                        int* __restrict__ sel_idx, float* __restrict__ sel_score, int HW, int K, int cap) {
+  const int b = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
+  const int C = cand_count[b];
+  if (j >= K - C) return;
+  // candidates ascend, so ci[i] - i never decreases; the m candidates with ci[i] - i <= j are the ones before the j-th other pixel
+  const int* ci = cand_idx + static_cast<size_t>(b) * HW;
+  int lo = 0, hi = C;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (ci[mid] - mid <= j) lo = mid + 1;
+    else hi = mid;
+  }
+  sel_idx[static_cast<size_t>(b) * cap + C + j] = j + lo;
+  sel_score[static_cast<size_t>(b) * cap + C + j] = 0.f;
+}
+
+// ------------------------------------------------------------------ grid-wide top-k (K > kMaxTopK)
+// Same selection rule and output as sp_select_kernel, with every stage spread over a grid of CTAs per image:
+//   1. radix select of the K-th largest score: four 8-bit digit passes, each a per-CTA shared histogram added into a [B][256] global
+//      one, then topk_digit_kernel walks the digits (thread 0 of sp_select_kernel's walk) and keeps (prefix, ties still needed);
+//   2. ordered gather: chunked count / scan / write keeps every candidate above the threshold and the first `needed` ties, in
+//      ascending pixel index;
+//   3. stable LSD radix sort of the kept ones on the inverted score bits (four 8-bit passes: per-CTA digit counts, per-image scan,
+//      stable scatter), so that equal scores stay in ascending index order.  The last pass writes sel_idx / sel_score.
+// The decisions (select or keep all, sort or not) are taken per image on the device; nothing waits for the host.
+constexpr int kTopkThreads = 256;
+constexpr int kTopkSelGrid = 64;   // histogram CTAs per image (grid-stride over the candidates)
+constexpr int kSortTile = 2048;    // keys per CTA of a sort pass: 8 warps x 256, each warp a contiguous run
+enum { kTkPrefix = 0, kTkNeed, kTkSelect, kTkSort, kTkState = 8 };  // per-image state words
+
+// Device scratch of the grid-wide path for up to B images of HW pixels at top-K
+struct TopkScratch {
+  unsigned* hist = nullptr;         // [B][256] digit histogram of the running select pass
+  unsigned* state = nullptr;        // [B][kTkState]
+  int *chunk_cnt = nullptr, *gt_off = nullptr, *tie_off = nullptr;  // [B][ceil(HW / kChunk)] gather counts and offsets
+  int* digit_off = nullptr;         // [B][ceil(K / kSortTile)][256] sort-pass digit counts, then offsets
+  unsigned long long *keys0 = nullptr, *keys1 = nullptr;  // [B][K] ping-pong sort keys (~score bits << 32 | pixel index)
+  int B = 0, HW = 0, K = 0;         // capacity
+};
+
+// element counts of TopkScratch's buffers: hist, state, one chunk array, digit_off, one key array
+struct TopkSizes {
+  size_t hist, state, chunks, digits, keys;
+};
+inline TopkSizes topk_sizes(int B, int HW, int K) {
+  const size_t b = B;
+  return {b * 256, b * kTkState, b * ceil_div(HW, kChunk), b * ceil_div(K, kSortTile) * 256, b * K};
+}
+
+__device__ __forceinline__ unsigned long long topk_key(unsigned u, int idx) {
+  return (static_cast<unsigned long long>(~u) << 32) | static_cast<unsigned>(idx);
+}
+
+__global__ void __launch_bounds__(kTopkThreads) topk_init_kernel(const int* __restrict__ cand_count, int K, int sort_all,
+                                                                 unsigned* __restrict__ hist, unsigned* __restrict__ state,
+                                                                 int* __restrict__ sel_count) {
+  const int b = blockIdx.x;
+  hist[b * 256 + threadIdx.x] = 0u;
+  if (threadIdx.x == 0) {
+    const int C = cand_count[b], keep = min(C, K);
+    unsigned* s = state + b * kTkState;
+    s[kTkPrefix] = 0u;  // with no select pass every candidate (score > 0) is above the threshold 0
+    s[kTkNeed] = K;
+    s[kTkSelect] = C > K;
+    s[kTkSort] = (C > K || sort_all) ? keep : 0;  // keys to sort; 0: the gather writes the output in row-major order
+    sel_count[b] = sort_all ? K : keep;
+  }
+}
+
+// one digit pass of the radix select: histogram of digit (u >> shift) & 255 over the candidates matching the prefix so far
+__global__ void __launch_bounds__(kTopkThreads) topk_hist_kernel(const float* __restrict__ cand_score, const int* __restrict__ cand_count,
+                                                                 const unsigned* __restrict__ state, unsigned* __restrict__ hist, int HW,
+                                                                 int shift) {
+  const int b = blockIdx.y, t = threadIdx.x, lane = t & 31;
+  if (!state[b * kTkState + kTkSelect]) return;
+  __shared__ unsigned h[256];
+  h[t] = 0u;
+  __syncthreads();
+  const int C = cand_count[b];
+  const float* cs = cand_score + static_cast<size_t>(b) * HW;
+  const unsigned prefix = state[b * kTkState + kTkPrefix];
+  const unsigned himask = shift == 24 ? 0u : (0xffffffffu << (shift + 8));
+  for (int base = blockIdx.x * kTopkThreads; base < C; base += gridDim.x * kTopkThreads) {  // block-uniform trip count
+    const int i = base + t;
+    unsigned d = 0xffffffffu;
+    if (i < C) {
+      const unsigned u = __float_as_uint(cs[i]);
+      if ((u & himask) == prefix) d = (u >> shift) & 255u;
+    }
+    const unsigned peers = __match_any_sync(0xffffffffu, d);  // scores cluster in few digits: one shared atomic per digit and warp
+    if (d != 0xffffffffu && lane == __ffs(peers) - 1) atomicAdd(&h[d], __popc(peers));
+  }
+  __syncthreads();
+  if (h[t]) atomicAdd(&hist[b * 256 + t], h[t]);
+}
+
+__global__ void __launch_bounds__(kTopkThreads) topk_digit_kernel(unsigned* __restrict__ hist, unsigned* __restrict__ state, int shift) {
+  const int b = blockIdx.x, t = threadIdx.x;
+  unsigned* s = state + b * kTkState;
+  if (!s[kTkSelect]) return;
+  __shared__ unsigned h[256];
+  h[t] = hist[b * 256 + t];
+  hist[b * 256 + t] = 0u;  // ready for the next pass
+  __syncthreads();
+  if (t == 0) {
+    unsigned rem = s[kTkNeed], d = 255;
+    for (;; --d) {  // walk digits from large to small
+      if (h[d] >= rem) break;
+      rem -= h[d];
+      if (d == 0) break;
+    }
+    s[kTkPrefix] |= d << shift;
+    s[kTkNeed] = rem;  // after the last pass: how many candidates equal to the threshold are still needed
+  }
+}
+
+// per chunk of kChunk candidates: (above threshold << 16) | (equal to threshold)
+__global__ void __launch_bounds__(kTopkThreads) topk_gather_count_kernel(const float* __restrict__ cand_score,
+                                                                         const int* __restrict__ cand_count,
+                                                                         const unsigned* __restrict__ state, int* __restrict__ chunk_cnt,
+                                                                         int HW, int nchunks) {
+  const int b = blockIdx.y, chunk = blockIdx.x;
+  const int C = cand_count[b];
+  if (chunk * kChunk >= C) return;
+  const float* cs = cand_score + static_cast<size_t>(b) * HW;
+  const unsigned T = state[b * kTkState + kTkPrefix];
+  int cnt = 0;
+  const int base = chunk * kChunk + threadIdx.x * 16;
+  for (int i = 0; i < 16; ++i) {
+    const int p = base + i;
+    if (p < C) {
+      const unsigned u = __float_as_uint(cs[p]);
+      cnt += u > T ? 0x10000 : (u == T ? 1 : 0);
+    }
+  }
+  __shared__ int red[kTopkThreads / 32];
+#pragma unroll
+  for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = cnt;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int tot = 0;
+    for (int i = 0; i < kTopkThreads / 32; ++i) tot += red[i];
+    chunk_cnt[b * nchunks + chunk] = tot;
+  }
+}
+
+__global__ void topk_gather_scan_kernel(const int* __restrict__ chunk_cnt, const int* __restrict__ cand_count, int* __restrict__ gt_off,
+                                        int* __restrict__ tie_off, int nchunks) {
+  const int b = blockIdx.x;
+  if (threadIdx.x == 0) {  // a few hundred chunks at most: a serial scan, as sp_scan_kernel
+    const int live = ceil_div(cand_count[b], kChunk);
+    int gt = 0, tie = 0;
+    for (int i = 0; i < live; ++i) {
+      const int c = chunk_cnt[b * nchunks + i];
+      gt_off[b * nchunks + i] = gt;
+      tie_off[b * nchunks + i] = tie;
+      gt += c >> 16;
+      tie += c & 0xffff;
+    }
+  }
+}
+
+// writes the kept candidates of one chunk at their rank in index order: to the sort keys, or straight to the output when the image
+// needs no sort (count <= K, not sort-always)
+__global__ void __launch_bounds__(kTopkThreads) topk_gather_write_kernel(const int* __restrict__ cand_idx,
+                                                                         const float* __restrict__ cand_score,
+                                                                         const int* __restrict__ cand_count,
+                                                                         const unsigned* __restrict__ state, const int* __restrict__ gt_off,
+                                                                         const int* __restrict__ tie_off, unsigned long long* __restrict__ keys,
+                                                                         int* __restrict__ sel_idx, float* __restrict__ sel_score, int HW,
+                                                                         int K, int cap, int nchunks) {
+  const int b = blockIdx.y, chunk = blockIdx.x;
+  const int C = cand_count[b];
+  if (chunk * kChunk >= C) return;
+  const unsigned* s = state + b * kTkState;
+  const unsigned T = s[kTkPrefix], need = s[kTkNeed];
+  const bool sort = s[kTkSort] != 0u;
+  const int* ci = cand_idx + static_cast<size_t>(b) * HW;
+  const float* cs = cand_score + static_cast<size_t>(b) * HW;
+  const int base = chunk * kChunk + threadIdx.x * 16;
+  unsigned u[16];
+  int cnt = 0;
+  for (int i = 0; i < 16; ++i) {
+    const int p = base + i;
+    u[i] = p < C ? __float_as_uint(cs[p]) : 0u;  // 0: neither above nor equal to a threshold of a positive score
+    cnt += u[i] > T ? 0x10000 : (u[i] == T && p < C ? 1 : 0);
+  }
+  // block exclusive scan of the packed counts (each field at most kChunk)
+  __shared__ int wsum[kTopkThreads / 32];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int inc = cnt;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += v;
+  }
+  if (lane == 31) wsum[wid] = inc;
+  __syncthreads();
+  int ex = inc - cnt;
+  for (int i = 0; i < wid; ++i) ex += wsum[i];
+  unsigned gt = gt_off[b * nchunks + chunk] + (ex >> 16), tie = tie_off[b * nchunks + chunk] + (ex & 0xffff);
+  unsigned long long* ko = keys + static_cast<size_t>(b) * K;
+  int* oi = sel_idx + static_cast<size_t>(b) * cap;
+  float* os = sel_score + static_cast<size_t>(b) * cap;
+  for (int i = 0; i < 16; ++i) {
+    const int p = base + i;
+    if (p >= C) break;
+    unsigned pos;
+    bool keep = false;
+    if (u[i] > T) {
+      keep = true;
+      pos = gt + min(tie, need);  // kept before it: every earlier candidate above T and the first `need` earlier ties
+      ++gt;
+    } else if (u[i] == T) {
+      keep = tie < need;
+      pos = gt + tie;
+      ++tie;
+    }
+    if (!keep) continue;
+    if (sort) {
+      ko[pos] = topk_key(u[i], ci[p]);
+    } else {
+      oi[pos] = ci[p];
+      os[pos] = __uint_as_float(u[i]);
+    }
+  }
+}
+
+// One pass of the LSD sort on digit (key >> shift) & 255.  Each warp walks its contiguous 256 keys 32 at a time, in order; lanes with
+// the same digit rank among themselves with __match_any_sync, so equal digits keep their input order (stable).  SCATTER false: the
+// CTA's digit counts to digit_off.  SCATTER true: digit_off holds the CTA's first output slot per digit (topk_sort_scan_kernel).
+template <bool SCATTER>
+__global__ void __launch_bounds__(kTopkThreads) topk_sort_pass_kernel(const unsigned long long* __restrict__ src,
+                                                                      unsigned long long* __restrict__ dst, int* __restrict__ sel_idx,
+                                                                      float* __restrict__ sel_score, int* __restrict__ digit_off,
+                                                                      const unsigned* __restrict__ state, int K, int cap, int nblk,
+                                                                      int shift) {
+  const int b = blockIdx.y, t = threadIdx.x, lane = t & 31, w = t >> 5;
+  const int n = static_cast<int>(state[b * kTkState + kTkSort]);
+  const int blk0 = blockIdx.x * kSortTile;
+  if (blk0 >= n) return;
+  __shared__ int wh[kTopkThreads / 32][256];  // per-warp digit counts, then per-warp running output slots
+  for (int i = t; i < kTopkThreads / 32 * 256; i += kTopkThreads) (&wh[0][0])[i] = 0;
+  __syncthreads();
+  const unsigned long long* in = src + static_cast<size_t>(b) * K;
+  const int seg = blk0 + w * (kSortTile / (kTopkThreads / 32));
+  constexpr int kRounds = kSortTile / kTopkThreads;
+  for (int r = 0; r < kRounds; ++r) {
+    const int i = seg + r * 32 + lane;
+    const unsigned d = i < n ? static_cast<unsigned>(in[i] >> shift) & 255u : 0xffffffffu;
+    const unsigned peers = __match_any_sync(0xffffffffu, d);
+    if (d != 0xffffffffu && lane == __ffs(peers) - 1) wh[w][d] += __popc(peers);
+    __syncwarp();
+  }
+  __syncthreads();
+  int* off = digit_off + (static_cast<size_t>(b) * nblk + blockIdx.x) * 256;
+  if (!SCATTER) {
+    int tot = 0;
+#pragma unroll
+    for (int q = 0; q < kTopkThreads / 32; ++q) tot += wh[q][t];
+    off[t] = tot;
+    return;
+  }
+  {
+    int run = off[t];
+#pragma unroll
+    for (int q = 0; q < kTopkThreads / 32; ++q) {
+      const int c = wh[q][t];
+      wh[q][t] = run;
+      run += c;
+    }
+  }
+  __syncthreads();
+  const bool last = dst == nullptr;
+  unsigned long long* out = last ? nullptr : dst + static_cast<size_t>(b) * K;
+  int* oi = sel_idx + static_cast<size_t>(b) * cap;
+  float* os = sel_score + static_cast<size_t>(b) * cap;
+  const unsigned lt = (1u << lane) - 1u;
+  for (int r = 0; r < kRounds; ++r) {
+    const int i = seg + r * 32 + lane;
+    const unsigned long long key = i < n ? in[i] : 0ull;
+    const unsigned d = i < n ? static_cast<unsigned>(key >> shift) & 255u : 0xffffffffu;
+    const unsigned peers = __match_any_sync(0xffffffffu, d);
+    if (d != 0xffffffffu) {
+      const int pos = wh[w][d] + __popc(peers & lt);
+      if (last) {
+        oi[pos] = static_cast<int>(key & 0xffffffffull);
+        os[pos] = __uint_as_float(~static_cast<unsigned>(key >> 32));
+      } else {
+        out[pos] = key;
+      }
+    }
+    __syncwarp();
+    if (d != 0xffffffffu && lane == __ffs(peers) - 1) wh[w][d] += __popc(peers);
+    __syncwarp();
+  }
+}
+
+// digit_off [B][nblk][256]: per-CTA digit counts -> first output slot of each (CTA, digit), digits ascending, CTAs in order
+__global__ void __launch_bounds__(256) topk_sort_scan_kernel(int* __restrict__ digit_off, const unsigned* __restrict__ state, int nblk) {
+  const int b = blockIdx.x, d = threadIdx.x, lane = d & 31, w = d >> 5;
+  const int n = static_cast<int>(state[b * kTkState + kTkSort]);
+  if (n == 0) return;
+  const int live = ceil_div(n, kSortTile);
+  int* off = digit_off + static_cast<size_t>(b) * nblk * 256;
+  int run = 0;
+  for (int k = 0; k < live; ++k) {
+    const int c = off[k * 256 + d];
+    off[k * 256 + d] = run;
+    run += c;
+  }
+  // exclusive scan of the digit totals
+  __shared__ int ws[8];
+  int inc = run;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += v;
+  }
+  if (lane == 31) ws[w] = inc;
+  __syncthreads();
+  int base = inc - run;
+  for (int q = 0; q < w; ++q) base += ws[q];
+  for (int k = 0; k < live; ++k) off[k * 256 + d] += base;
 }
 
 
@@ -638,15 +979,79 @@ inline int launch_candidates(dimb_ctx* ctx, cudaStream_t st, const float* nms, c
   return DIMB_OK;
 }
 
-// Top-K of each image's candidates (sp_select_kernel) into sel_idx / sel_score [B][cap], counts to sel_count [B]; K < 0 keeps all
+// Grows s to B images of HW pixels at top-K.  The buffers belong to the current owner (OwnerScope) of the context.
+inline int topk_reserve(dimb_ctx* ctx, TopkScratch& s, int B, int HW, int K) {
+  if (s.hist && B <= s.B && HW <= s.HW && K <= s.K) return DIMB_OK;
+  for (void* p : {static_cast<void*>(s.hist), static_cast<void*>(s.state), static_cast<void*>(s.chunk_cnt), static_cast<void*>(s.gt_off),
+                  static_cast<void*>(s.tie_off), static_cast<void*>(s.digit_off), static_cast<void*>(s.keys0), static_cast<void*>(s.keys1)})
+    dimb_free(ctx, p);
+  s = TopkScratch{};
+  const TopkSizes z = topk_sizes(B, HW, K);
+  DIMB_TRY(dimb_alloc_t(ctx, &s.hist, z.hist));
+  DIMB_TRY(dimb_alloc_t(ctx, &s.state, z.state));
+  DIMB_TRY(dimb_alloc_t(ctx, &s.chunk_cnt, z.chunks));
+  DIMB_TRY(dimb_alloc_t(ctx, &s.gt_off, z.chunks));
+  DIMB_TRY(dimb_alloc_t(ctx, &s.tie_off, z.chunks));
+  DIMB_TRY(dimb_alloc_t(ctx, &s.digit_off, z.digits));
+  DIMB_TRY(dimb_alloc_t(ctx, &s.keys0, z.keys, false));
+  DIMB_TRY(dimb_alloc_t(ctx, &s.keys1, z.keys, false));
+  s.B = B, s.HW = HW, s.K = K;
+  return DIMB_OK;
+}
+
+// Top-K of each image's candidates into sel_idx / sel_score [B][cap], counts to sel_count [B]; K < 0 keeps all (in row-major order).
+// K <= kMaxTopK runs sp_select_kernel, larger K (or any K >= 1 with `grid`, for tests) the grid-wide path with scratch `tk`
+// (topk_reserve'd for B, HW, K).  sort_all (1 <= K <= HW): ALIKED's top-k mode, see sp_select_kernel.
 inline int launch_select(dimb_ctx* ctx, cudaStream_t st, const CandBufs& c, int* sel_idx, float* sel_score, int* sel_count, int B, int HW,
-                         int K, int cap) {
-  int P = 1;  // the bitonic sort runs on K keys padded to a power of two
-  while (P < std::max(K, 1)) P <<= 1;
-  const size_t smem = static_cast<size_t>(P) * sizeof(unsigned long long);
-  DIMB_TRY(dimb_func_smem(ctx, sp_select_kernel, static_cast<int>(smem)));
-  sp_select_kernel<<<B, kSelThreads, smem, st>>>(c.cand_idx, c.cand_score, c.cand_count, sel_idx, sel_score, sel_count, HW, K, cap, P);
-  DIMB_LAUNCH_CHECK(ctx);
+                         int K, int cap, TopkScratch* tk, bool sort_all, bool grid = false) {
+  if (K <= kMaxTopK && !grid) {
+    int P = 1;  // the bitonic sort runs on K keys padded to a power of two
+    while (P < std::max(K, 1)) P <<= 1;
+    const size_t smem = static_cast<size_t>(P) * sizeof(unsigned long long);
+    auto kern = sort_all ? sp_select_kernel<true> : sp_select_kernel<false>;
+    DIMB_TRY(dimb_func_smem(ctx, kern, static_cast<int>(smem)));
+    kern<<<B, kSelThreads, smem, st>>>(c.cand_idx, c.cand_score, c.cand_count, sel_idx, sel_score, sel_count, HW, K, cap, P);
+    DIMB_LAUNCH_CHECK(ctx);
+  } else {
+    if (!tk || B > tk->B || HW > tk->HW || K > tk->K) {
+      dimb_set_error(ctx, "launch_select: top-k scratch smaller than the call");
+      return DIMB_ERR_ARG;
+    }
+    const int nch = ceil_div(HW, kChunk), nblk = ceil_div(K, kSortTile);
+    topk_init_kernel<<<B, kTopkThreads, 0, st>>>(c.cand_count, K, sort_all ? 1 : 0, tk->hist, tk->state, sel_count);
+    DIMB_LAUNCH_CHECK(ctx);
+    const dim3 hgrid(std::min(kTopkSelGrid, ceil_div(HW, kTopkThreads * 16)), B);
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      topk_hist_kernel<<<hgrid, kTopkThreads, 0, st>>>(c.cand_score, c.cand_count, tk->state, tk->hist, HW, shift);
+      DIMB_LAUNCH_CHECK(ctx);
+      topk_digit_kernel<<<B, kTopkThreads, 0, st>>>(tk->hist, tk->state, shift);
+      DIMB_LAUNCH_CHECK(ctx);
+    }
+    topk_gather_count_kernel<<<dim3(nch, B), kTopkThreads, 0, st>>>(c.cand_score, c.cand_count, tk->state, tk->chunk_cnt, HW, nch);
+    DIMB_LAUNCH_CHECK(ctx);
+    topk_gather_scan_kernel<<<B, 32, 0, st>>>(tk->chunk_cnt, c.cand_count, tk->gt_off, tk->tie_off, nch);
+    DIMB_LAUNCH_CHECK(ctx);
+    topk_gather_write_kernel<<<dim3(nch, B), kTopkThreads, 0, st>>>(c.cand_idx, c.cand_score, c.cand_count, tk->state, tk->gt_off,
+                                                                    tk->tie_off, tk->keys0, sel_idx, sel_score, HW, K, cap, nch);
+    DIMB_LAUNCH_CHECK(ctx);
+    // keys0 -> keys1 -> keys0 -> keys1 -> sel_idx / sel_score
+    const dim3 sgrid(nblk, B);
+    for (int pass = 0; pass < 4; ++pass) {
+      const unsigned long long* src = pass & 1 ? tk->keys1 : tk->keys0;
+      unsigned long long* dst = pass == 3 ? nullptr : (pass & 1 ? tk->keys0 : tk->keys1);
+      const int shift = 32 + 8 * pass;
+      topk_sort_pass_kernel<false><<<sgrid, kTopkThreads, 0, st>>>(src, dst, sel_idx, sel_score, tk->digit_off, tk->state, K, cap, nblk, shift);
+      DIMB_LAUNCH_CHECK(ctx);
+      topk_sort_scan_kernel<<<B, 256, 0, st>>>(tk->digit_off, tk->state, nblk);
+      DIMB_LAUNCH_CHECK(ctx);
+      topk_sort_pass_kernel<true><<<sgrid, kTopkThreads, 0, st>>>(src, dst, sel_idx, sel_score, tk->digit_off, tk->state, K, cap, nblk, shift);
+      DIMB_LAUNCH_CHECK(ctx);
+    }
+  }
+  if (sort_all) {
+    topk_fill_kernel<<<dim3(ceil_div(K, 256), B), 256, 0, st>>>(c.cand_idx, c.cand_count, sel_idx, sel_score, HW, K, cap);
+    DIMB_LAUNCH_CHECK(ctx);
+  }
   return DIMB_OK;
 }
 

@@ -554,7 +554,7 @@ extern "C" int dimb_selftest_detect(dimb_ctx* ctx, const float* scores, int B, i
   c.cand_score = d_cs;
   DIMB_TRY(launch_nms(ctx, 0, d_scores, d_nms, B, H, W, r, ver));
   DIMB_TRY(launch_candidates(ctx, 0, d_nms, c, B, H, W, thr, border, d_thr, true));
-  DIMB_TRY(launch_select(ctx, 0, c, d_si, d_ss, d_sc, B, HW, K, cap));
+  DIMB_TRY(launch_select(ctx, 0, c, d_si, d_ss, d_sc, B, HW, K, cap, nullptr, false));
   DIMB_TRY(sync_call(ctx, "dimb_selftest_detect"));
   DIMB_TRY(download(ctx, nms, d_nms, npix + kDetTail));
   DIMB_TRY(download(ctx, cand_count, d_cc, B + kDetTail));
@@ -564,6 +564,92 @@ extern "C" int dimb_selftest_detect(dimb_ctx* ctx, const float* scores, int B, i
   DIMB_TRY(download(ctx, sel_score, d_ss, nsel + kDetTail));
   DIMB_TRY(download(ctx, sel_count, d_sc, B + kDetTail));
   if (plan) plan_out(nms_plan(r, ver), plan);
+  return DIMB_OK;
+}
+
+// dimb_selftest_detect with the selection of any K: the same arguments and buffers, and
+//   K >= 1, cap >= K; sort_all: ALIKED's top-k mode (sorted even when count <= K, slots count .. K-1 filled with the first pixels
+//   that are not candidates; needs K <= H W); path 0: the selection production runs for K (sp_select_kernel up to kMaxTopK, the
+//   grid-wide path above), 1: the grid-wide path at any K.
+//   iters > 0: afterwards the selection alone runs `iters` more times on the same candidates; ms = device milliseconds per run.
+extern "C" int dimb_selftest_select(dimb_ctx* ctx, const float* scores, int B, int H, int W, int r, int cut, float thr,
+                                    const float* thr_per_image, int border, int K, int cap, int sort_all, int path, float sentinel,
+                                    float* nms, int* cand_count, int* cand_idx, float* cand_score, int* sel_idx, float* sel_score,
+                                    int* sel_count, int iters, float* ms) {
+  if (!ctx || !scores || !nms || !cand_count || !cand_idx || !cand_score || !sel_idx || !sel_score || !sel_count) return DIMB_ERR_ARG;
+  if (B < 1 || H < 1 || W < 1 || static_cast<long long>(B) * H * W > INT_MAX || border < 0 || !(thr >= 0.f)) return DIMB_ERR_ARG;
+  if (K < 1 || cap < K || (sort_all && K > H * W) || (path != 0 && path != 1) || iters < 0 || (iters > 0 && !ms)) return DIMB_ERR_ARG;
+  if (thr_per_image)
+    for (int b = 0; b < B; ++b)
+      if (!(thr_per_image[b] >= 0.f)) return DIMB_ERR_ARG;
+  const int ver = version_of_cut(r, cut);
+  if (ver < 0) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const int HW = H * W, nch = ceil_div(HW, kChunk);
+  const size_t npix = static_cast<size_t>(B) * HW, nsel = static_cast<size_t>(B) * cap;
+  const int isent = sentinel_bits(sentinel);
+  DevTmp t{ctx, {}};
+  float *d_scores, *d_nms, *d_cs, *d_ss, *d_thr = nullptr;
+  int *d_cc, *d_ci, *d_si, *d_sc;
+  CandBufs c;
+  DIMB_TRY(t.upload(&d_scores, std::vector<float>(scores, scores + npix)));
+  DIMB_TRY(t.upload(&d_nms, std::vector<float>(npix + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_cc, std::vector<int>(B + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_ci, std::vector<int>(npix + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_cs, std::vector<float>(npix + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_si, std::vector<int>(nsel + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_ss, std::vector<float>(nsel + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_sc, std::vector<int>(B + kDetTail, isent)));
+  DIMB_TRY(t.get(&c.chunk_count, static_cast<size_t>(B) * nch));
+  DIMB_TRY(t.get(&c.chunk_off, static_cast<size_t>(B) * nch));
+  if (thr_per_image) DIMB_TRY(t.upload(&d_thr, std::vector<float>(thr_per_image, thr_per_image + B)));
+  c.cand_count = d_cc;
+  c.cand_idx = d_ci;
+  c.cand_score = d_cs;
+  // scratch of the grid-wide path, the sizes topk_reserve gives it (the dirty contents production meets after earlier calls: 0xff)
+  TopkScratch tk;
+  const TopkSizes z = topk_sizes(B, HW, K);
+  DIMB_TRY(t.get(&tk.hist, z.hist));
+  DIMB_TRY(t.get(&tk.state, z.state));
+  DIMB_TRY(t.get(&tk.chunk_cnt, z.chunks));
+  DIMB_TRY(t.get(&tk.gt_off, z.chunks));
+  DIMB_TRY(t.get(&tk.tie_off, z.chunks));
+  DIMB_TRY(t.get(&tk.digit_off, z.digits));
+  DIMB_TRY(t.get(&tk.keys0, z.keys));
+  DIMB_TRY(t.get(&tk.keys1, z.keys));
+  DIMB_CUDA_OK(ctx, cudaMemset(tk.hist, 0xff, z.hist * sizeof(unsigned)));
+  DIMB_CUDA_OK(ctx, cudaMemset(tk.digit_off, 0xff, z.digits * sizeof(int)));
+  DIMB_CUDA_OK(ctx, cudaMemset(tk.keys0, 0xff, z.keys * sizeof(unsigned long long)));
+  DIMB_CUDA_OK(ctx, cudaMemset(tk.keys1, 0xff, z.keys * sizeof(unsigned long long)));
+  tk.B = B, tk.HW = HW, tk.K = K;
+  auto select = [&]() { return launch_select(ctx, 0, c, d_si, d_ss, d_sc, B, HW, K, cap, &tk, sort_all != 0, path == 1); };
+  DIMB_TRY(launch_nms(ctx, 0, d_scores, d_nms, B, H, W, r, ver));
+  DIMB_TRY(launch_candidates(ctx, 0, d_nms, c, B, H, W, thr, border, d_thr, true));
+  DIMB_TRY(select());
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_select"));
+  DIMB_TRY(download(ctx, nms, d_nms, npix + kDetTail));
+  DIMB_TRY(download(ctx, cand_count, d_cc, B + kDetTail));
+  DIMB_TRY(download(ctx, cand_idx, d_ci, npix + kDetTail));
+  DIMB_TRY(download(ctx, cand_score, d_cs, npix + kDetTail));
+  DIMB_TRY(download(ctx, sel_idx, d_si, nsel + kDetTail));
+  DIMB_TRY(download(ctx, sel_score, d_ss, nsel + kDetTail));
+  DIMB_TRY(download(ctx, sel_count, d_sc, B + kDetTail));
+  if (iters > 0) {
+    DIMB_TRY(select());  // warm-up
+    cudaEvent_t e0, e1;
+    DIMB_CUDA_OK(ctx, cudaEventCreate(&e0));
+    DIMB_CUDA_OK(ctx, cudaEventCreate(&e1));
+    int rc = cudaEventRecord(e0, 0) == cudaSuccess ? DIMB_OK : DIMB_ERR_CUDA;
+    for (int i = 0; i < iters && rc == DIMB_OK; ++i) rc = select();
+    if (rc == DIMB_OK && cudaEventRecord(e1, 0) != cudaSuccess) rc = DIMB_ERR_CUDA;
+    if (rc == DIMB_OK) rc = sync_call(ctx, "dimb_selftest_select (timing)");
+    float total = 0.f;
+    if (rc == DIMB_OK && cudaEventElapsedTime(&total, e0, e1) != cudaSuccess) rc = DIMB_ERR_CUDA;
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    DIMB_TRY(rc);
+    *ms = total / iters;
+  }
   return DIMB_OK;
 }
 

@@ -109,6 +109,7 @@ struct dimb_sp {
   float *o_kpts = nullptr, *o_scores = nullptr, *o_desc = nullptr;
   int* o_counts = nullptr;
   int o_cap = 0, sel_cap = 0;
+  TopkScratch topk;  // grid-wide top-k (max_keypoints > kMaxTopK)
   // last-call geometry (debug taps)
   int lastB = 0, lastH = 0, lastW = 0;
 };
@@ -156,8 +157,7 @@ int dimb_sp_create(dimb_ctx* ctx, const float* weights, size_t n_floats, const d
     dimb_set_error(ctx, "dimb_sp_create: weight blob has " + std::to_string(n_floats) + " floats, expected " + std::to_string(need));
     return DIMB_ERR_ARG;
   }
-  if (conf->nms_radius < 0 || conf->nms_radius > 8 || conf->max_keypoints == 0 || conf->max_keypoints < -1 ||
-      conf->max_keypoints > kMaxTopK || conf->max_batch < 1 || conf->max_height < 16 || conf->max_width < 16) {
+  if (conf->nms_radius < 0 || conf->nms_radius > 8 || conf->max_keypoints == 0 || conf->max_keypoints < -1 || conf->max_batch < 1 || conf->max_height < 16 || conf->max_width < 16) {
     dimb_set_error(ctx, "dimb_sp_create: unsupported configuration (\"max_keypoints\" must be positive or -1)");
     return DIMB_ERR_ARG;
   }
@@ -209,6 +209,7 @@ int dimb_sp_create(dimb_ctx* ctx, const float* weights, size_t n_floats, const d
   DIMB_TRY(dimb_alloc_t(ctx, &sp->chunk_count, B * nch));
   DIMB_TRY(dimb_alloc_t(ctx, &sp->chunk_off, B * nch));
   DIMB_TRY(dimb_alloc_t(ctx, &sp->cand_count, B));
+  if (conf->max_keypoints > kMaxTopK) DIMB_TRY(topk_reserve(ctx, sp->topk, static_cast<int>(B), static_cast<int>(H * W), conf->max_keypoints));
   *out = guard.release();
   return DIMB_OK;
 }
@@ -278,7 +279,8 @@ int dimb_sp_extract_dev(dimb_sp* sp, const float* d_images, int B, int H, int W,
     DIMB_TRY(dimb_alloc_t(ctx, &sp->sel_score, static_cast<size_t>(cf.max_batch) * cap));
     sp->sel_cap = cap;
   }
-  DIMB_TRY(launch_select(ctx, st, cand, sp->sel_idx, sp->sel_score, d_counts, B, H8 * W8, cf.max_keypoints, cap));
+  DIMB_TRY(launch_select(ctx, st, cand, sp->sel_idx, sp->sel_score, d_counts, B, H8 * W8, cf.max_keypoints, cap, &sp->topk,
+                         false));
   return launch_sp_describe(ctx, st, sp->sel_idx, sp->sel_score, d_counts, sp->ddesc, d_kpts, d_scores, d_desc, B, h, w, cap,
                             cf.fix_sampling);
 }

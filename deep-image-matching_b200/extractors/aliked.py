@@ -38,8 +38,6 @@ class AlikedExtractor(ExtractorBase):
         model_name = cfg.get("model_name", "aliked-n16")
         if model_name not in _SUPPORTED:
             raise NotImplementedError(f"libdimb200 implements {_SUPPORTED}; got model_name={model_name!r}")
-        if cfg["detection_threshold"] <= 0:
-            raise NotImplementedError("top-k detection mode (detection_threshold <= 0) is not implemented in libdimb200")
         self._ctx = _native.Context.get(int(self.config["general"].get("device", 0)))
         self._weights = cfg.get("weights_dict") or aliked_weights(model_name)  # checkpoint follows model_name (aliked.py:581-587)
         self._net = None

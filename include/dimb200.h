@@ -69,7 +69,7 @@ int dimb_ctx_profile_read(dimb_ctx* ctx, char* buf, size_t n);
 typedef struct {
   int nms_radius;            /* config.py:96  (3)      */
   float keypoint_threshold;  /* config.py:97  (0.0005) */
-  int max_keypoints;         /* config.py:98  (2048); -1 = unlimited */
+  int max_keypoints;         /* config.py:98  (2048); -1 = unlimited; any positive limit (above 16384 a grid-wide top-k runs) */
   int remove_borders;        /* superpoint.py default (4) */
   int fix_sampling;          /* 0: thirdparty superpoint.py:81-98, 1: extractors/superpoint.py:16-27 */
   int max_batch;             /* workspace sizing: images per call */
@@ -436,16 +436,22 @@ dimb_ctx* dimb_sp_ctx(dimb_sp* sp);
 /* ---------------------------------------------------------------------------------------------------------
  * ALIKED extraction.  Replaces AlikedExtractor._extract (reference src/deep_image_matching/extractors/aliked.py:45-64)
  * and the model it drives (thirdparty/LightGlue/lightglue/aliked.py:560-693: encoder with deformable blocks :367-449,
- * DKD detector :92-244, SDDH descriptor head :452-558).  Supported: aliked-n16 / aliked-n16rot (dim 128, K 3, M 16),
- * threshold detection mode (detection_threshold > 0, the reference's only configured mode).
+ * DKD detector :92-244, SDDH descriptor head :452-558).  Supported: aliked-n16 / aliked-n16rot (dim 128, K 3, M 16), and
+ * the three detection modes of DKD (top_k = -1 if detection_threshold > 0 else max_num_keypoints):
+ *   threshold mode  detection_threshold > 0: NMS pixels above it (above mean(score_map) if none is), the n_limit best of them;
+ *   top-k mode      detection_threshold <= 0 < max_num_keypoints: exactly max_num_keypoints keypoints, the largest of the
+ *                   border-zeroed NMS map, score-descending (torch.topk).  Fewer nonzero NMS pixels than that: the rest are the
+ *                   first zero pixels in row-major order.  max_num_keypoints > H * W is refused (DIMB_ERR_ARG);
+ *   mean mode       detection_threshold <= 0 and max_num_keypoints <= 0: NMS pixels above mean(score_map), the 20000 best.
+ * Kept keypoints are row-major when no cut fires, else score-descending (ties: smaller pixel index first).
  *
  * weights: fp32 blob, the model's state_dict tensors in state_dict order without num_batches_tracked
  * (block1.conv1.weight ... desc_head.sf_conv.weight; 678316 floats).
  * Reproduced quirk: `scores` are the DKD score *dispersities* (aliked.py:682 swaps the names; SURVEY A.5). */
 typedef struct dimb_aliked dimb_aliked;
 typedef struct dimb_aliked_conf {
-  int max_num_keypoints;      /* n_limit; <= 0 -> 20000 (aliked.py:585) */
-  float detection_threshold;  /* 0.2 */
+  int max_num_keypoints;      /* threshold / mean mode: n_limit, <= 0 -> 20000 (aliked.py:585); top-k mode: K.  Any value */
+  float detection_threshold;  /* 0.2; <= 0: top-k or mean mode */
   int nms_radius;             /* 2 */
   int max_height, max_width;  /* workspace size */
 } dimb_aliked_conf;
