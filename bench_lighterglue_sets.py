@@ -1,8 +1,9 @@
-"""LighterGlue over an image set of given XFeat features on one GPU: the per-pair plugin against the batched device engine.
+"""LighterGlue over an image set of given XFeat features on one GPU: the plugin one pair at a time against image-set batches.
 
 n "images" (default 24 -> 276 pairs) are built from the golden XFeat features of the reference's two photos (tests/golden/
 lighterglue_golden.npz): the photos, then seeded subsets and permutations of their keypoints, up to 2048 each.  Every pair is matched
-  (a) by LighterGlueMatcher._match_pairs per pair on store.get features (the shape-generic per-pair entry, host-staged, synchronising),
+  (a) by LighterGlueMatcher._match_pairs per pair on store.get features (dimb_lg_match: each pair staged from the host into the
+      batched engine at P = 1, synchronising),
   (b) by sharded.ImageSetMatcher(extractor=None, matcher="lighterglue").match at batch_pairs 8 and 32 (dimb_lg_match_dev on the store).
 The tables of (a) and (b) are compared.  Each arm is timed after a warm-up run with a device synchronise at the end; the lgx.* device
 times (dimb_ctx_profile) and launch counts come from a separate profiled run.  The card's name and power limit are read in the same

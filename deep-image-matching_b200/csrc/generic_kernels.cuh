@@ -1,12 +1,12 @@
-// generic_kernels.cuh - plain fp32 CUDA-core kernels shared by the shape-generic LightGlue (lightglue_generic.cu) and SuperGlue
-// (superglue.cu) paths: tiled linear layer, warp-per-query online-softmax attention, LayerNorm+GELU, row dot products, gathers,
-// log-sum-exp / argmax over a score matrix.  They trade speed for generality; the tensor-core kernels live in gemm.cuh / lightglue.cu.
+// generic_kernels.cuh - plain fp32 CUDA-core kernel bodies of the shape-generic LightGlue (lightglue_generic.cu, lgx_assign.cuh) and
+// SuperGlue (superglue.cu) paths: tiled linear layer, warp-per-query online-softmax attention, LayerNorm+GELU, row dot products,
+// log-sum-exp / argmax over a score matrix.  The kernels that launch them add a grid dimension over the sides or pairs.  They trade speed
+// for generality; the tensor-core kernels live in gemm.cuh / lightglue.cu.
 #pragma once
 #include "common.cuh"
 
 namespace {
 
-// ------------------------------------------------------------------ kernels
 // C[m][n] = act((sum_k A[m*lda + k] * W[n*ldw + k] + bias[n]) * scale) (+ resid[m*ldr + n]), act = ReLU or identity; 64 x 64 tile, 256 threads, 4 x 4 outputs
 // per thread, K streamed through shared memory 16 at a time (k ascending per output: deterministic summation order).
 // The tile body is shared with SuperGlue's batched keypoint encoder (one more grid dimension over the sides).
@@ -50,11 +50,6 @@ __device__ __forceinline__ void gx_linear_tile(const float* __restrict__ A, int 
     }
   }
 }
-__global__ void __launch_bounds__(256) gx_linear_kernel(const float* __restrict__ A, int lda, const float* __restrict__ W, int ldw,
-                                                        const float* __restrict__ bias, float* __restrict__ C, int ldc, int M, int N, int K,
-                                                        float scale, const float* __restrict__ resid, int ldr, int relu) {
-  gx_linear_tile(A, lda, W, ldw, bias, C, ldc, M, N, K, scale, resid, ldr, relu, blockIdx.y * 64);
-}
 
 // keypoint normalisation (lightglue.py:24-34) + Fourier encoding (:57-70): enc [2][N][hd] = cos / sin, each frequency twice
 // (one keypoint i, one frequency f; shared with the batched prep of lightglue_generic.cu)
@@ -67,12 +62,6 @@ __device__ __forceinline__ void gx_posenc_one(const float* __restrict__ kpts, in
   float* e0 = enc + static_cast<size_t>(i) * hd + 2 * f;
   e0[0] = c, e0[1] = c;
   e0[static_cast<size_t>(np) * hd] = s, e0[static_cast<size_t>(np) * hd + 1] = s;
-}
-__global__ void gx_posenc_kernel(const float* __restrict__ kpts, int n, float size0, float size1, const float* __restrict__ Wr /*[hd/2][2]*/,
-                                 int hd, float* __restrict__ enc, int np) {
-  const int i = blockIdx.x, f = threadIdx.x;
-  if (i >= n || f >= hd / 2) return;
-  gx_posenc_one(kpts, i, f, size0, size1, Wr, hd, enc, np);
 }
 
 // Wqkv output [N][3d] interleaved as (h, hd, 3) (lightglue.py:153-154) -> q, k (rotary applied, :47-54), v, each [N][d]
@@ -90,12 +79,6 @@ __device__ __forceinline__ void gx_qkv_rotary_one(const float* __restrict__ qkv,
   k[o + 1] = k1 * c1 + k0 * s1;
   v[o] = r[c * 3 + 2];
   v[o + 1] = r[(c + 1) * 3 + 2];
-}
-__global__ void gx_qkv_rotary_kernel(const float* __restrict__ qkv, int n, int d, int hd, const float* __restrict__ enc, int np,
-                                     float* __restrict__ q, float* __restrict__ k, float* __restrict__ v) {
-  const int i = blockIdx.x, c = threadIdx.x * 2;  // channel pair (c, c+1) of the model dimension
-  if (i >= n || c >= d) return;
-  gx_qkv_rotary_one(qkv, i, c, d, hd, enc, np, q, k, v);
 }
 
 // softmax(q k^T * hd^-0.5) v, fp32.  CTA = 8 warps = 8 queries of one head sharing 32-key tiles of K and V in shared memory;
@@ -149,11 +132,6 @@ __device__ __forceinline__ void gx_attention_block(const float* __restrict__ q, 
     if (c < hd) out[static_cast<size_t>(qi) * ldo + co + c] = nk > 0 ? o[j] / l : 0.f;  // empty key set -> zeros (lightglue.py:103-104)
   }
 }
-template <int HDP>
-__global__ void __launch_bounds__(256) gx_attention_kernel(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
-                                                           int nq, int nk, int d, int hd, float* __restrict__ out, int ldo) {
-  gx_attention_block<HDP>(q, k, v, nq, nk, d, hd, out, ldo, blockIdx.x, blockIdx.y);
-}
 
 // y = gelu(layer_norm(x)) over the n features of a row, eps 1e-5, exact (erf) GELU; warp per row
 __device__ __forceinline__ void gx_ln_gelu_row(const float* __restrict__ x, int row, int lane, int n, const float* __restrict__ g,
@@ -177,12 +155,6 @@ __device__ __forceinline__ void gx_ln_gelu_row(const float* __restrict__ x, int 
     y[static_cast<size_t>(row) * n + c] = 0.5f * t * (1.f + erff(t * 0.70710678118654752440f));
   }
 }
-__global__ void gx_ln_gelu_kernel(const float* __restrict__ x, int rows, int n, const float* __restrict__ g, const float* __restrict__ b,
-                                  float* __restrict__ y) {
-  const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (row >= rows) return;
-  gx_ln_gelu_row(x, row, lane, n, g, b, y);
-}
 
 // z[row] = x[row] . w + b (token confidence / matchability logits); warp per row
 __device__ __forceinline__ void gx_rowdot_row(const float* __restrict__ x, int ldx, int row, int lane, int n, const float* __restrict__ w,
@@ -193,25 +165,7 @@ __device__ __forceinline__ void gx_rowdot_row(const float* __restrict__ x, int l
   for (int of = 16; of; of >>= 1) s += __shfl_xor_sync(0xffffffffu, s, of);
   if (lane == 0) z[row] = s + b[0];
 }
-__global__ void gx_rowdot_kernel(const float* __restrict__ x, int ldx, int rows, int n, const float* __restrict__ w, const float* __restrict__ b,
-                                 float* __restrict__ z) {
-  const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (row >= rows) return;
-  gx_rowdot_row(x, ldx, row, lane, n, w, b, z);
-}
 
-// pruning gather: dst row i = src row idx[i] for the state (stride ld, d used) and both halves of the encoding
-__global__ void gx_gather_kernel(const float* __restrict__ xs, float* __restrict__ xd, int ld, int d, const float* __restrict__ es,
-                                 float* __restrict__ ed, int hd, int np, const int* __restrict__ idx, int n) {
-  const int i = blockIdx.x;
-  if (i >= n) return;
-  const int s = idx[i];
-  for (int c = threadIdx.x; c < d; c += blockDim.x) xd[static_cast<size_t>(i) * ld + c] = xs[static_cast<size_t>(s) * ld + c];
-  for (int c = threadIdx.x; c < hd; c += blockDim.x) {
-    ed[static_cast<size_t>(i) * hd + c] = es[static_cast<size_t>(s) * hd + c];
-    ed[(static_cast<size_t>(np) + i) * hd + c] = es[(static_cast<size_t>(np) + s) * hd + c];
-  }
-}
 
 // log-sum-exp of the rows (dir 0) or columns (dir 1) of sim [m][n] (row stride ld); warp per row / column
 __device__ __forceinline__ void gx_lse_one(const float* __restrict__ sim, int ld, int m, int n, int dir, float* __restrict__ lse, int i,
@@ -226,11 +180,6 @@ __device__ __forceinline__ void gx_lse_one(const float* __restrict__ sim, int ld
 #pragma unroll
   for (int of = 16; of; of >>= 1) s += __shfl_xor_sync(0xffffffffu, s, of);
   if (lane == 0) lse[i] = mx + logf(s);
-}
-__global__ void gx_lse_kernel(const float* __restrict__ sim, int ld, int m, int n, int dir, float* __restrict__ lse) {
-  const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (i >= (dir == 0 ? m : n)) return;
-  gx_lse_one(sim, ld, m, n, dir, lse, i, lane);
 }
 
 __device__ __forceinline__ float log_sigmoid(float z) { return fminf(z, 0.f) - log1pf(expf(-fabsf(z))); }
@@ -256,13 +205,6 @@ __device__ __forceinline__ void gx_argmax_one(const float* __restrict__ sim, int
     if (argmax_takes(ov, oi, bv, bi)) bv = ov, bi = oi;
   }
   if (lane == 0) best[i] = bv, arg[i] = bi;
-}
-__global__ void gx_argmax_kernel(const float* __restrict__ sim, int ld, int m, int n, const float* __restrict__ rlse,
-                                 const float* __restrict__ clse, const float* __restrict__ z0, const float* __restrict__ z1, int dir,
-                                 float* __restrict__ best, int* __restrict__ arg) {
-  const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (i >= (dir == 0 ? m : n)) return;
-  gx_argmax_one(sim, ld, m, n, rlse, clse, z0, z1, dir, best, arg, i, lane);
 }
 
 }  // namespace

@@ -374,6 +374,7 @@ int dimb_lg_create(dimb_ctx* ctx, const float* weights, size_t n_floats, const d
     dimb_lg* lg = new dimb_lg();
     lg->ctx = ctx;
     lg->conf = *cf;
+    lg->S = 2 * cf->max_pairs, lg->NP = cf->max_kpts, lg->din = cf->input_dim;  // what dimb_lg_match's host staging reads
     const int rc = lgx_create(ctx, weights, n_floats, cf, &lg->gen);
     if (rc != DIMB_OK) {
       delete lg;
@@ -787,7 +788,6 @@ int dimb_lg_match_dev(dimb_lg* lg, int P, const dimb_feats_dev* f0, const dimb_f
 int dimb_lg_match(dimb_lg* lg, int P, const dimb_feats* f0, const dimb_feats* f1, int64_t* matches, float* mscores, int* n_matches,
                   int* stop_layer, int cap) {
   if (!lg || !f0 || !f1 || !matches || !mscores || !n_matches || !stop_layer || P < 1 || P > lg->conf.max_pairs) return DIMB_ERR_ARG;
-  if (lg->gen) return lgx_match(lg->gen, P, f0, f1, matches, mscores, n_matches, stop_layer, cap);
   dimb_ctx* ctx = lg->ctx;
   OwnerScope own(ctx, &lg->mem);
   DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));

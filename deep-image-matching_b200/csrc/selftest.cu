@@ -7,8 +7,8 @@
 //   dimb_selftest_nms_plan: the launch plan of simple_nms, host only;
 //   dimb_selftest_sp_softmax / dimb_selftest_sp_describe: the SuperPoint head kernels (sp_head.cuh) through their production launches;
 //   dimb_selftest_lg_assign / dimb_selftest_lg_tail: the LightGlue assignment and per-layer tail (lg_assign.cuh) through their launch
-//     helpers; dimb_selftest_lgx_assign: the shape-generic LightGlue assignment and host filter; dimb_selftest_sg_sinkhorn: SuperGlue's
-//     Sinkhorn and mutual-max matching (sg_assign.cuh);
+//     helpers; dimb_selftest_lgx_assign: the shape-generic LightGlue assignment and filter (lgx_assign.cuh) through its launch helper;
+//     dimb_selftest_sg_sinkhorn: SuperGlue's Sinkhorn and mutual-max matching (sg_assign.cuh);
 //   dimb_gv_host: the RANSAC arithmetic of gv.cu on the host.
 #include <algorithm>
 #include <cstring>
@@ -383,46 +383,34 @@ int selftest_attention_lg(dimb_ctx* ctx, const float* Q, const float* K, const f
   return DIMB_OK;
 }
 
-// shape-generic attention (attn_hd128.cuh) on operands packed by the production packers at NP rounded up to the query tile
+// shape-generic attention (attn_hd128.cuh) through hd128_attend, on one pair of two sides of NPp rows (NP rounded up to the query tile):
+// side 0 holds Q as its q rows, side 1 K as its q rows and V as its v rows, and side 0 attends to side 1 in the cross form.  With
+// n[0] == n[1] side 0 holds K and V itself and attends to its own keys (the self form), side 1 is empty.
 int selftest_attention_hd128(dimb_ctx* ctx, const float* Q, const float* K, const float* V, float* out, int H, int hd, int NP, const int* n,
                              float lazy, float pad, float out_pad) {
-  const bool exact = ctx->precision == DIMB_PRECISION_EXACT;
-  const int NPp = round_up(NP, kAttnTile), ld = H * hd;
-  const size_t nel = static_cast<size_t>(NPp) * ld, pl_el = static_cast<size_t>(H) * NPp * kXHd;
-  std::vector<float> q(nel, pad), k(nel, pad), v(nel, pad);  // rows past the live counts hold `pad`: the packers copy all NPp rows
+  const int NPp = round_up(NP, kAttnTile), ld = H * hd, self = n[0] == n[1];
+  const size_t side = static_cast<size_t>(NPp) * ld, pl_el = 2 * static_cast<size_t>(H) * NPp * kXHd;
+  std::vector<float> q(2 * side, pad), k(2 * side, pad), v(2 * side, pad);  // rows past the live counts: `pad`, not read by the packers
   std::copy(Q, Q + static_cast<size_t>(n[0]) * ld, q.begin());
-  std::copy(K, K + static_cast<size_t>(n[1]) * ld, k.begin());
-  std::copy(V, V + static_cast<size_t>(n[1]) * ld, v.begin());
+  std::copy(K, K + static_cast<size_t>(n[1]) * ld, self ? k.begin() : q.begin() + side);
+  std::copy(V, V + static_cast<size_t>(n[1]) * ld, self ? v.begin() : v.begin() + side);
   DevTmp t{ctx, {}};
   float *fq, *fk, *fv, *d_out;
-  __half *qp[2], *kp[2], *vp[2];
+  int *d_n, *d_stop;
+  Hd128Ops o;
+  o.S = 2, o.h = H, o.d = ld, o.hd = hd, o.NP = NPp, o.NPp = NPp;
   DIMB_TRY(t.upload(&fq, q));
   DIMB_TRY(t.upload(&fk, k));
   DIMB_TRY(t.upload(&fv, v));
-  DIMB_TRY(t.upload(&d_out, std::vector<float>(nel, out_pad)));
-  for (int pl = 0; pl < 2; ++pl) {
-    DIMB_TRY(t.get(&qp[pl], pl_el));
-    DIMB_TRY(t.get(&kp[pl], pl_el));
-    DIMB_TRY(t.get(&vp[pl], pl_el));
-  }
-  gx_pack_rows_kernel<<<dim3(NPp, H), kXHd>>>(fq, ld, NPp, hd, NPp, qp[0], exact ? qp[1] : nullptr);
-  gx_pack_rows_kernel<<<dim3(NPp, H), kXHd>>>(fk, ld, NPp, hd, NPp, kp[0], exact ? kp[1] : nullptr);
-  gx_pack_vt_kernel<<<dim3(NPp / 32, kXHd / 32, H), dim3(32, 8)>>>(fv, ld, NPp, hd, NPp, vp[0], exact ? vp[1] : nullptr);
-  DIMB_CUDA_OK(ctx, cudaGetLastError());
-  CUtensorMap mq[2], mk[2], mv[2];  // as lightglue_generic.cu: Q box 128 rows, K box 64 rows, V^T box 128 rows
-  for (int pl = 0; pl < 2; ++pl) {
-    DIMB_TRY(dimb_tmap_2d(ctx, &mq[pl], qp[pl], static_cast<uint64_t>(H) * NPp, kXHd, kXHd, kAttnTile));
-    DIMB_TRY(dimb_tmap_2d(ctx, &mk[pl], kp[pl], static_cast<uint64_t>(H) * NPp, kXHd, kXHd, kAttnBlk));
-    DIMB_TRY(dimb_tmap_2d(ctx, &mv[pl], vp[pl], static_cast<uint64_t>(H) * kXHd, NPp, NPp, kXHd));
-  }
-  AttnXArgs a;
-  a.nq = n[0], a.nk = n[1], a.NP = NPp, a.hd = hd;
-  a.scale = 1.f / sqrtf(static_cast<float>(hd));
-  a.lazy = lazy;
-  a.out = d_out, a.ldo = ld;
-  DIMB_TRY(launch_attn_hd128(ctx, 0, mq, mk, mv, H, a, exact));
+  DIMB_TRY(t.upload(&d_out, std::vector<float>(2 * side, out_pad)));
+  DIMB_TRY(t.upload(&d_n, std::vector<int>{n[0], self ? 0 : n[1]}));
+  DIMB_TRY(t.upload(&d_stop, std::vector<int>{0}));
+  for (int pl = 0; pl < 2; ++pl)
+    for (__half** p : {&o.q[pl], &o.k[pl], &o.vt[pl]}) DIMB_TRY(t.get(p, pl_el));
+  DIMB_TRY(hd128_maps(ctx, o));
+  DIMB_TRY(hd128_attend(ctx, 0, o, 2, fq, fk, fv, !self, d_n, d_stop, lazy, d_out));
   DIMB_TRY(sync_call(ctx, "dimb_selftest_attention"));
-  DIMB_CUDA_OK(ctx, cudaMemcpy(out, d_out, sizeof(float) * nel, cudaMemcpyDeviceToHost));
+  DIMB_CUDA_OK(ctx, cudaMemcpy(out, d_out, sizeof(float) * side, cudaMemcpyDeviceToHost));
   return DIMB_OK;
 }
 }  // namespace
@@ -432,10 +420,11 @@ int selftest_attention_hd128(dimb_ctx* ctx, const float* Q, const float* K, cons
 //     NP a multiple of 128), live rows n[S], stopped[S / 2]
 //     (nonzero: the pair is stopped); cross: the keys of side s are the q rows of side s ^ 1 (K unused, may be null).  out: the
 //     context buffer [S * NP][256], hi + lo planes (hi only in FAST), every row.
-//   variant 1: gx_attn_tc_kernel (head dim hd <= 128, even, padded to 128) via launch_attn_hd128, operands packed by
-//     gx_pack_rows_kernel / gx_pack_vt_kernel.  Q [n[0]][H * hd], K / V [n[1]][H * hd], NP >= n[0], n[1]; S, stopped and cross unused.
-//     out: [NPp][H * hd] fp32 with NPp = NP rounded up to 128.
-// Every Q / K row and V^T column past the live counts holds `pad` (stale values of earlier layers in production), and the output
+//   variant 1: lgx_attn_tc_kernel (head dim hd <= 128, even, padded to 128) via hd128_attend, which packs the operands
+//     (lgx_pack_rows_kernel / lgx_pack_vt_kernel) as the shape-generic LightGlue runs them: the cross form, or the self form when
+//     n[0] == n[1].  Q [n[0]][H * hd], K / V [n[1]][H * hd], NP >= n[0], n[1]; S, stopped and cross unused.  out: [NPp][H * hd] fp32
+//     with NPp = NP rounded up to 128.
+// Every Q / K / V row past the live counts holds `pad` (stale values of earlier layers in production), and the output
 // buffer starts as `out_pad`, so rows the kernel must not write can be checked.  lazy: rescale threshold in log2 units, in
 // [0, kAttnLazyMax]; negative = the context's (DIMB_ATTN_LAZY).
 extern "C" int dimb_selftest_attention(dimb_ctx* ctx, int variant, const float* Q, const float* K, const float* V, float* out, int S,
@@ -759,13 +748,14 @@ extern "C" int dimb_gv_host(const float* k0, const float* k1, int n, float thres
 }
 
 // ------------------------------------------------------------------ matching heads: LightGlue assignment and tail, SuperGlue Sinkhorn
-#include "generic_kernels.cuh"
+#include <limits>
+
 #include "lg_assign.cuh"
-#include "lightglue_generic.cuh"
+#include "lgx_assign.cuh"
 #include "sg_assign.cuh"
 
 namespace {
-// logsigmoid of the shape-generic path, as gx_argmax_kernel evaluates it
+// logsigmoid of the shape-generic path, as lgx_assign_kernel evaluates it
 __global__ void log_sigmoid_kernel(const float* __restrict__ z, float* __restrict__ out, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) out[i] = log_sigmoid(z[i]);
@@ -892,11 +882,12 @@ extern "C" int dimb_selftest_lg_tail(dimb_ctx* ctx, int P, int NP, const float* 
   return download(ctx, n_next, d_nn, 2 * P + kDetTail);
 }
 
-// The assignment of the shape-generic LightGlue for one pair, as lightglue_generic.cu runs it: gx_lse_kernel and gx_argmax_kernel in
-// both directions, then the host filter lgx_filter.  sim [m][ld] (ld >= n; m, n >= 1), raw matchability logits z0 [m] / z1 [n],
-// original indices ind0 [m] / ind1 [n].  Outputs hold kDetTail more elements and start as `sentinel` (int buffers: its bit pattern,
-// matches: that int sign-extended): rlse / ls0 / best0 / arg0 [m], clse / ls1 / best1 / arg1 [n] (ls = logsigmoid(z) as the device
-// evaluates it), matches [cap][2], mscores [cap]; n_matches [1] the full count.
+// The assignment of the shape-generic LightGlue for one pair through launch_lgx_assign (lgx_assign.cuh), with P = 1 in the production
+// layout at row stride NP = max(m, ld) + kDetTail: log-sum-exp, maxima and argmaxes in both directions, then the device filter.
+// sim [m][ld] (ld >= n; m, n >= 1), raw matchability logits z0 [m] / z1 [n], original indices ind0 [m] / ind1 [n]; the cells of the
+// layout outside sim hold NaN.  Outputs hold kDetTail more elements and start as `sentinel` (int buffers: its bit pattern, matches: that
+// int sign-extended): rlse / ls0 / best0 / arg0 [m], clse / ls1 / best1 / arg1 [n] (ls = logsigmoid(z) as the device evaluates it),
+// matches [cap][2], mscores [cap]; n_matches [1] the full count.
 extern "C" int dimb_selftest_lgx_assign(dimb_ctx* ctx, int m, int n, int ld, const float* sim, const float* z0, const float* z1, const int* ind0,
                                         const int* ind1, float th, int cap, float sentinel, float* rlse, float* clse, float* ls0, float* ls1,
                                         float* best0, int* arg0, float* best1, int* arg1, int64_t* matches, float* mscores, int* n_matches) {
@@ -905,41 +896,48 @@ extern "C" int dimb_selftest_lgx_assign(dimb_ctx* ctx, int m, int n, int ld, con
     return DIMB_ERR_ARG;
   if (m < 1 || n < 1 || ld < n || cap < 1) return DIMB_ERR_ARG;
   DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-  const int isent = sentinel_bits(sentinel);
-  const size_t nm = static_cast<size_t>(m) + kDetTail, nn = static_cast<size_t>(n) + kDetTail;
+  const int isent = sentinel_bits(sentinel), NP = std::max(m, ld) + kDetTail;  // side 0's tails end before side 1's rows
+  const size_t nm = static_cast<size_t>(m) + kDetTail, nn = static_cast<size_t>(n) + kDetTail, R = 2 * static_cast<size_t>(NP);
+  const float nan = std::numeric_limits<float>::quiet_NaN();
+  std::vector<float> hsim(static_cast<size_t>(NP) * NP, nan), hz(R, nan);
+  std::vector<int> hind(R, -1);
+  for (size_t r = 0; r < static_cast<size_t>(m); ++r) std::copy(sim + r * ld, sim + (r + 1) * ld, hsim.begin() + r * NP);
+  std::copy(z0, z0 + m, hz.begin());
+  std::copy(z1, z1 + n, hz.begin() + NP);
+  std::copy(ind0, ind0 + m, hind.begin());
+  std::copy(ind1, ind1 + n, hind.begin() + NP);
   DevTmp t{ctx, {}};
-  float *d_sim, *d_z0, *d_z1, *d_rl, *d_cl, *d_l0, *d_l1, *d_b0, *d_b1;
-  int *d_a0, *d_a1;
-  DIMB_TRY(t.upload(&d_sim, std::vector<float>(sim, sim + static_cast<size_t>(m) * ld)));
-  DIMB_TRY(t.upload(&d_z0, std::vector<float>(z0, z0 + m)));
-  DIMB_TRY(t.upload(&d_z1, std::vector<float>(z1, z1 + n)));
-  for (float** b : {&d_rl, &d_l0, &d_b0}) DIMB_TRY(t.upload(b, std::vector<float>(nm, sentinel)));
-  for (float** b : {&d_cl, &d_l1, &d_b1}) DIMB_TRY(t.upload(b, std::vector<float>(nn, sentinel)));
-  DIMB_TRY(t.upload(&d_a0, std::vector<int>(nm, isent)));
-  DIMB_TRY(t.upload(&d_a1, std::vector<int>(nn, isent)));
-  gx_lse_kernel<<<ceil_div(m * 32, 256), 256>>>(d_sim, ld, m, n, 0, d_rl);
-  DIMB_LAUNCH_CHECK(ctx);
-  gx_lse_kernel<<<ceil_div(n * 32, 256), 256>>>(d_sim, ld, m, n, 1, d_cl);
-  DIMB_LAUNCH_CHECK(ctx);
-  gx_argmax_kernel<<<ceil_div(m * 32, 256), 256>>>(d_sim, ld, m, n, d_rl, d_cl, d_z0, d_z1, 0, d_b0, d_a0);
-  DIMB_LAUNCH_CHECK(ctx);
-  gx_argmax_kernel<<<ceil_div(n * 32, 256), 256>>>(d_sim, ld, m, n, d_rl, d_cl, d_z0, d_z1, 1, d_b1, d_a1);
-  DIMB_LAUNCH_CHECK(ctx);
-  log_sigmoid_kernel<<<ceil_div(m, 256), 256>>>(d_z0, d_l0, m);
-  log_sigmoid_kernel<<<ceil_div(n, 256), 256>>>(d_z1, d_l1, n);
+  float *d_sim, *d_z, *d_rl, *d_cl, *d_l0, *d_l1, *d_best, *d_ms;
+  int *d_nf, *d_stop, *d_ind, *d_arg, *d_nm, *d_sl;
+  long long* d_m;
+  DIMB_TRY(t.upload(&d_sim, hsim));
+  DIMB_TRY(t.upload(&d_z, hz));
+  DIMB_TRY(t.upload(&d_ind, hind));
+  DIMB_TRY(t.upload(&d_nf, std::vector<int>{m, n}));
+  DIMB_TRY(t.upload(&d_stop, std::vector<int>{0}));
+  for (float** b : {&d_rl, &d_cl}) DIMB_TRY(t.upload(b, std::vector<float>(NP + kDetTail, sentinel)));
+  for (float** b : {&d_l0, &d_l1}) DIMB_TRY(t.upload(b, std::vector<float>(NP, sentinel)));
+  DIMB_TRY(t.upload(&d_best, std::vector<float>(R + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_arg, std::vector<int>(R + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_m, std::vector<long long>(2 * static_cast<size_t>(cap) + kDetTail, isent)));
+  DIMB_TRY(t.upload(&d_ms, std::vector<float>(static_cast<size_t>(cap) + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_nm, std::vector<int>(1, isent)));
+  DIMB_TRY(t.upload(&d_sl, std::vector<int>(1, isent)));
+  DIMB_TRY(launch_lgx_assign(ctx, 0, 1, NP, d_sim, d_nf, d_z, d_stop, 1, d_ind, th, d_rl, d_cl, d_best, d_arg, d_m, d_ms, d_nm, d_sl, cap));
+  log_sigmoid_kernel<<<ceil_div(m, 256), 256>>>(d_z, d_l0, m);
+  log_sigmoid_kernel<<<ceil_div(n, 256), 256>>>(d_z + NP, d_l1, n);
   DIMB_TRY(sync_call(ctx, "dimb_selftest_lgx_assign"));
   DIMB_TRY(download(ctx, rlse, d_rl, nm));
   DIMB_TRY(download(ctx, clse, d_cl, nn));
   DIMB_TRY(download(ctx, ls0, d_l0, nm));
   DIMB_TRY(download(ctx, ls1, d_l1, nn));
-  DIMB_TRY(download(ctx, best0, d_b0, nm));
-  DIMB_TRY(download(ctx, arg0, d_a0, nm));
-  DIMB_TRY(download(ctx, best1, d_b1, nn));
-  DIMB_TRY(download(ctx, arg1, d_a1, nn));
-  std::fill(matches, matches + 2 * static_cast<size_t>(cap) + kDetTail, static_cast<int64_t>(isent));
-  std::fill(mscores, mscores + static_cast<size_t>(cap) + kDetTail, sentinel);
-  *n_matches = lgx_filter(m, n, best0, arg0, arg1, ind0, ind1, th, matches, mscores, cap);
-  return DIMB_OK;
+  DIMB_TRY(download(ctx, best0, d_best, nm));
+  DIMB_TRY(download(ctx, arg0, d_arg, nm));
+  DIMB_TRY(download(ctx, best1, d_best + NP, nn));
+  DIMB_TRY(download(ctx, arg1, d_arg + NP, nn));
+  DIMB_TRY(download(ctx, reinterpret_cast<long long*>(matches), d_m, 2 * static_cast<size_t>(cap) + kDetTail));
+  DIMB_TRY(download(ctx, mscores, d_ms, static_cast<size_t>(cap) + kDetTail));
+  return download(ctx, n_matches, d_nm, 1);
 }
 
 // SuperGlue's optimal-transport head (sg_assign.cuh) on P pairs: launch_sg_sinkhorn, then launch_sg_matches.

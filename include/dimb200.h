@@ -133,7 +133,9 @@ typedef struct {
 } dimb_feats;
 
 /* P pairs.  Outputs (host): matches [P][cap][2] int64 (ascending in column 0), mscores [P][cap],
- * n_matches [P], stop_layer [P] (1-based layer count executed, the reference's "stop").
+ * n_matches [P], stop_layer [P] (1-based layer count executed, the reference's "stop").  The pairs are staged into
+ * dimb_lg_match_dev; all P are checked before any launch, and a count above cap returns DIMB_ERR_CAPACITY after every pair's
+ * outputs (its first cap matches, its full count) are written.
  * Replaces LightGlueMatcher._match_pairs (matchers/lightglue.py:102-125) and LighterGlueMatcher._match_pairs
  * (matchers/lighterglue.py:105-262). */
 int dimb_lg_match(dimb_lg* lg, int P, const dimb_feats* f0, const dimb_feats* f1, int64_t* matches, float* mscores,
@@ -158,9 +160,9 @@ typedef struct {
  * call, exists); d_matches [P][cap][2] int64 ascending in column 0, d_mscores [P][cap], d_n_matches [P] (the full count, also above
  * cap; only cap rows are written), d_stop_layer [P] are device buffers.  A pair with an empty side gets stop 1 and 0 matches.
  * DIMB_ERR_ARG, before any CUDA call, for P outside [1, max_pairs], cap < 1, n_cap above max_kpts or a NULL pointer.  Every shape:
- * descriptor_dim 256 / 4 heads runs the tensor-core kernels; other shapes (LighterGlue: 96 / 1 head) run the batched form of
- * dimb_lg_match's shape-generic path, bit for bit equal to it.  For those shapes, size0 = size1 = 0 with no size_dev /
- * size_f32_dev normalises by the keypoints' own extent (1 + max) - min, as dimb_lg_match does without has_size. */
+ * descriptor_dim 256 / 4 heads runs the tensor-core kernels; other shapes (LighterGlue: 96 / 1 head) run the shape-generic
+ * engine.  dimb_lg_match stages host pairs into this entry for both.  For the shape-generic engine, size0 = size1 = 0 with no
+ * size_dev / size_f32_dev normalises by the keypoints' own extent (1 + max) - min, as dimb_lg_match does without has_size. */
 int dimb_lg_match_dev(dimb_lg* lg, int P, const dimb_feats_dev* f0, const dimb_feats_dev* f1, int64_t* d_matches,
                       float* d_mscores, int* d_n_matches, int* d_stop_layer, int cap, void* stream);
 /* Debug tap: fp32 descriptors x[side][row][d] after the last executed layer of the LAST call (host copy). */

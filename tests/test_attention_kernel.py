@@ -2,9 +2,10 @@
 
 The kernels run through their production launches in the self-test library (dimb_selftest_attention): lg_attn_kernel (LightGlue /
 SuperGlue: 4 heads x 64, self and cross, several sides with their own live counts and stopped pairs) and
-gx_attn_tc_kernel (the shape-generic path: head dim padded to 128).  Padding rows hold a large finite value, as the stale rows of
-earlier layers do in production, and the output buffer starts as a sentinel, so the mask and the rows that must not be written are
-checked as well as the values.
+lgx_attn_tc_kernel (the shape-generic path: head dim padded to 128, operands packed by hd128_attend as production packs them, the
+cross form and, where the live counts are equal, the self form).  Padding rows hold a large finite value, as the stale rows of earlier
+layers do in production, and the output buffer starts as a sentinel, so the mask (the packers' for the shape-generic path) and the rows
+that must not be written are checked as well as the values.
 
 Logits are designed: query rows are (A, A, b_i, noise) and key rows (u_hi, u_lo, w_j, noise), so the logit of (i, j) is
 A (u_hi + u_lo) + b_i w_j + noise.  Every operand is fp16-exact and every partial sum a multiple of 2^-12 below 2^11, so Q K^T is exact
@@ -309,7 +310,8 @@ def test_lg_attention(st, pattern, cross):
 @pytest.mark.gpu
 @pytest.mark.parametrize("pattern", PATTERNS)
 def test_hd128_attention(st, pattern):
-    """gx_attn_tc_kernel (the shape-generic path, head dim padded to 128) over every shape, lazy threshold and precision."""
+    """lgx_attn_tc_kernel with its packers (the shape-generic path, head dim padded to 128) over every shape, lazy threshold and
+    precision."""
     for i, (nq, nk) in enumerate(SHAPES):
         hd, H = HD128[i % len(HD128)]
         rng = np.random.default_rng(100 + i)

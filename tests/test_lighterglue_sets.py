@@ -1,6 +1,6 @@
-"""Batched, device-resident LighterGlue (dimb_lg_match_dev for shape-generic LightGlue) against the per-pair entry, bit for bit, and
-ImageSetMatcher on given features (extractor=None): LighterGlue, kornia_matcher and LightGlue sets against the matcher plugins on
-the store's features."""
+"""Batched, device-resident LighterGlue (dimb_lg_match_dev for shape-generic LightGlue): the host entry's staging, batch position and
+P invariance, the trained goldens and the oracle on seeded shapes, and ImageSetMatcher on given features (extractor=None): LighterGlue,
+kornia_matcher and LightGlue sets against the matcher plugins on the store's features."""
 import sqlite3
 
 import numpy as np
@@ -129,6 +129,11 @@ def _run_dev(net, sides, cap=K, stream=0):
     return [{"matches": m[p, :min(nm[p], cap)], "scores": ms[p, :min(nm[p], cap)], "stop": int(sl[p]), "n": int(nm[p])} for p in range(P)]
 
 
+def _as_dev_result(r):
+    """A LightGlueNet.match result in the form of _run_dev's."""
+    return {**r, "n": len(r["matches"])}
+
+
 def _bitwise(got, exp, what=""):
     assert got["stop"] == exp["stop"], (what, got["stop"], exp["stop"])
     assert got["n"] == len(exp["matches"]), (what, got["n"], len(exp["matches"]))
@@ -156,17 +161,21 @@ def _mixed_pairs(f0, f1):
 @pytest.mark.gpu
 @pytest.mark.parametrize("precision", ["exact", "fast"])
 @pytest.mark.parametrize("name", LTG_CASES)
-def test_dev_equals_per_pair_entry_trained(ctx, ltg_golden, ltg_weights, name, precision):
-    """Trained LighterGlue, each golden configuration: match_dev at P = 1, 4 and 8 over mixed pairs equals LightGlueNet.match (the per-pair
-    entry) bit for bit - matches, scores, counts and stop layers - and still reproduces the reference on the golden pair.  The device
-    evaluates the host's expf with glibc's own algorithm, so no confidence or exp(max) near a threshold can decide differently."""
+def test_host_staging_and_batch_invariance_trained(ctx, ltg_golden, ltg_weights, name, precision):
+    """Trained LighterGlue, each golden configuration, mixed pairs: LightGlueNet.match (host (D,N) arrays staged by dimb_lg_match, the
+    own extent of a side without a size computed on the host) at P = 8 equals match_dev on device sides (own extent on the device) at
+    P = 1, 4 and 8 and LightGlueNet.match one pair at a time, bit for bit - matches, scores, counts and stop layers - and reproduces the
+    reference on the golden pair."""
     from oracle.compare import compare_matches
     f0, f1, conf, ref = ltg_case(ltg_golden, name)
     ctx.set_precision(precision)
     try:
         net = _ltg_net(ctx, ltg_weights, conf, 8)
         pairs = _mixed_pairs(f0, f1)
-        exp = net.match([(_host(a, s), _host(b, s)) for a, b, s in pairs])
+        host = [(_host(a, s), _host(b, s)) for a, b, s in pairs]
+        exp = net.match(host)
+        for k, pair in enumerate(host):
+            _bitwise(_as_dev_result(net.match([pair])[0]), exp[k], (name, precision, "host P = 1", k))
         sides = [(_Dev(a, size=s), _Dev(b, size=s)) for a, b, s in pairs]
         for P in (1, 4, 8):
             for p0 in range(0, len(pairs), P):
@@ -203,7 +212,7 @@ def test_input_forms_batch_position_async_and_cap(ctx, ltg_golden, ltg_weights):
     forms.append((_S(slot[0]), _S(slot[1])))
     for k, got in enumerate(_run_dev(net, forms)):
         _bitwise(got, exp, ("form", k))
-    # own extent computed on the device == the per-pair entry's host extent == that extent given explicitly
+    # own extent computed on the device == the host entry's extent == that extent given explicitly
     own = net.match([(_host(r0, False), _host(r1, False))])[0]
     ext = lambda f: {**f, "image_size": (1 + f["keypoints"].max(0)) - f["keypoints"].min(0)}
     for got in _run_dev(net, [(_Dev(r0, size=False), _Dev(r1, size=False)), (_Dev(ext(r0)), _Dev(ext(r1)))]):
@@ -241,9 +250,12 @@ def test_input_forms_batch_position_async_and_cap(ctx, ltg_golden, ltg_weights):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape", [(96, 1), (128, 2)])
-def test_seeded_shapes_equal_per_pair_entry(ctx, ltg_golden, shape):
-    """Seeded weights: head dim 96 (tensor-core attention, attn_hd128) and 64 (gx_attention_kernel), adaptive, bitwise per pair."""
+def test_seeded_shapes_against_oracle(ctx, ltg_golden, shape):
+    """Seeded weights: head dim 96 (tensor-core attention, attn_hd128) and 64 (lgx_attention_kernel), adaptive, EXACT: each pair as the
+    oracle matches it (stop layer equal, matches equal but at the filter threshold), and P = 4 staged from the host equal to P = 1 on
+    device sides bit for bit."""
     from oracle import lightglue as o_lg
+    from oracle.compare import compare_matches
     d, h = shape
     f0, f1, _, _ = ltg_case(ltg_golden, "fixed")
     conf = {**o_lg.DEFAULT_CONF, "input_dim": 64, "descriptor_dim": d, "num_heads": h, "n_layers": 4, "depth_confidence": 0.95,
@@ -252,8 +264,10 @@ def test_seeded_shapes_equal_per_pair_entry(ctx, ltg_golden, shape):
     net = _ltg_net(ctx, w, conf, 4)
     pairs = _mixed_pairs(f0, f1)[:4]
     exp = net.match([(_host(a, s), _host(b, s)) for a, b, s in pairs])
-    for k, got in enumerate(_run_dev(net, [(_Dev(a, size=s), _Dev(b, size=s)) for a, b, s in pairs])):
-        _bitwise(got, exp[k], (shape, k))
+    for k, (a, b, s) in enumerate(pairs):
+        _bitwise(_run_dev(net, [(_Dev(a, size=s), _Dev(b, size=s))])[0], exp[k], (shape, k))
+        ref = o_lg.match(*[f if s else {k_: v for k_, v in f.items() if k_ != "image_size"} for f in (a, b)], w, conf)
+        compare_matches(exp[k], ref, conf["filter_threshold"], 2e-4)
     assert max(len(e["matches"]) for e in exp) > 0
 
 

@@ -1,12 +1,12 @@
 """The matching heads on their own: LightGlue's assignment and per-layer tail (csrc/lg_assign.cuh), the shape-generic LightGlue
-assignment with its host filter (csrc/generic_kernels.cuh, lightglue_generic.cuh) and SuperGlue's Sinkhorn and mutual-max matching
+assignment with its filter (csrc/lgx_assign.cuh) and SuperGlue's Sinkhorn and mutual-max matching
 (csrc/sg_assign.cuh), through the self-test entries that run the production launch helpers on host fp32 inputs.  Every output buffer
 starts as a sentinel and is followed by a tail, and padded score cells hold a finite poison (1e6), so unwritten slots, stray writes and
 reads of padding all show.
 
 Each head turns float scores into discrete decisions, and every decision is a pure fp32 expression of values the kernel returns itself:
   LightGlue  la = ((x - rmax) - rlog) + ((x - cmax) - clog), then + (lz0 + lz1)       (lg_assign.cuh la_value)
-  generic    la = ((s - rlse) + (s - clse)) + (ls0 + ls1)                            (generic_kernels.cuh gx_argmax_kernel)
+  generic    la = ((s - rlse) + (s - clse)) + (ls0 + ls1)                            (generic_kernels.cuh gx_argmax_one)
   SuperGlue  la = ((Z + u) + v) - norm                                               (sg_assign.cuh sg_row_max_kernel)
   stop test  1 - float(counter) / float(n0 + n1) > depth_conf                        (lg_assign.cuh lg_decide_kernel)
 None holds a multiply, so nothing contracts into an FMA and numpy float32 reproduces them exactly.  The statistics (rlog, clog, rlse,
@@ -637,7 +637,8 @@ def test_lg_assign_exact_threshold(st):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", DESIGNS + NONFINITE)
 def test_lgx_assign(st, name):
-    """The shape-generic assignment and host filter on one pair at a time: unequal sizes, padding columns of POISON in sim's rows."""
+    """The shape-generic assignment and device filter (launch_lgx_assign at P = 1) on one pair at a time: unequal sizes, padding columns
+    of POISON in sim's rows, compaction across 1024-row chunks (m = 1025 and 2048)."""
     for m, n in [(1, 2), (33, 31), (255, 1024), (1025, 256), (2048, 1023)]:
         rng = _np_rng("gx", name, m, n)
         s, l0, l1 = design(name, m, n, rng)
