@@ -28,7 +28,7 @@ EXPORTS = [
     "dimb_sg_weight_count", "dimb_sg_create", "dimb_sg_destroy", "dimb_sg_match", "dimb_sg_match_dev", "dimb_fstore_sg_feats_dev",
     "dimb_aliked_create", "dimb_aliked_destroy", "dimb_aliked_extract", "dimb_aliked_extract_dev", "dimb_aliked_debug_read",
     "dimb_fstore_create", "dimb_fstore_destroy", "dimb_fstore_put_dev", "dimb_fstore_put", "dimb_fstore_count", "dimb_fstore_get",
-    "dimb_fstore_feats_dev", "dimb_fstore_block_dev", "dimb_gv_fundamental", "dimb_gv_fundamental_batch_dev", "dimb_gv_verify_dev",
+    "dimb_fstore_feats_dev", "dimb_fstore_block_dev", "dimb_gv_fundamental", "dimb_gv_estimate", "dimb_gv_fundamental_batch_dev", "dimb_gv_verify_dev",
     "dimb_tile_grid", "dimb_tile_cut_dev", "dimb_tile_merge_dev", "dimb_tile_views_dev", "dimb_tile_match_merge_dev",
     "dimb_resize_area_tab", "dimb_resize_area_dev", "dimb_kpts_extent_dev", "dimb_tile_preselect_dev",
     "dimb_resize_area_linear_tab", "dimb_resize_area_linear_dev", "dimb_resize_area_rgb_dev", "dimb_pyr_size", "dimb_pyr_dev", "dimb_fstore_rescale_dev",
@@ -85,7 +85,18 @@ class FeatsDev(C.Structure):
 
 
 class GvConf(C.Structure):
-    _fields_ = [("threshold", C.c_float), ("max_iters", C.c_int), ("min_inliers", C.c_int), ("min_inlier_ratio", C.c_float)]
+    _fields_ = [("threshold", C.c_float), ("max_iters", C.c_int), ("min_inliers", C.c_int), ("min_inlier_ratio", C.c_float),
+                ("estimator", C.c_int), ("confidence", C.c_float)]
+
+
+GV_ESTIMATORS = {"ransac8": 0, "lo-ransac": 1}
+
+
+def gv_estimator(name) -> int:
+    """dimb_gv_conf.estimator of an estimator name in GV_ESTIMATORS; ValueError otherwise."""
+    if name not in GV_ESTIMATORS:
+        raise ValueError(f"unknown geometric verification estimator {name!r}; expected one of {list(GV_ESTIMATORS)}")
+    return GV_ESTIMATORS[name]
 
 
 _lib = None
@@ -161,6 +172,7 @@ def load_library():
     lib.dimb_fstore_feats_dev.argtypes = [vp, ip, C.POINTER(FeatsDev)]
     lib.dimb_fstore_sg_feats_dev.argtypes = [vp, ip, C.POINTER(SgFeatsDev)]
     lib.dimb_gv_fundamental.argtypes = [vp, vp, vp, ip, fp, ip, C.c_uint, vp, vp, C.POINTER(ip)]
+    lib.dimb_gv_estimate.argtypes = [vp, vp, vp, ip, C.POINTER(GvConf), C.c_uint, vp, vp, C.POINTER(ip), C.POINTER(ip)]
     lib.dimb_gv_fundamental_batch_dev.argtypes = [vp, ip, vp, vp, vp, vp, ip, fp, ip, C.c_uint, vp, vp, vp, vp]
     lib.dimb_gv_verify_dev.argtypes = [vp, ip, C.POINTER(FeatsDev), C.POINTER(FeatsDev), vp, vp, ip, C.POINTER(C.c_uint),
                                        C.POINTER(GvConf), vp, vp, vp, vp, vp, vp]
@@ -228,6 +240,8 @@ def load_selftest_library():
         lib.dimb_selftest_lgx_assign.argtypes = [vp, ip, ip, ip] + [vp] * 5 + [fp, ip, fp] + [vp] * 11
         lib.dimb_selftest_sg_sinkhorn.argtypes = [vp, ip, vp, vp, vp, fp, fp, vp, vp, ip, ip, fp, ip, fp] + [vp] * 9
         lib.dimb_gv_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_uint, vp, vp]
+        lib.dimb_gv_lo_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_float, C.c_uint, vp, vp, C.POINTER(ip)]
+        lib.dimb_gv_seven_point_host.argtypes = [vp, vp, vp]
         _selftest = lib
     return _selftest
 
@@ -658,18 +672,34 @@ class Context:
                                                 _ptr(mask), C.byref(cnt)), "dimb_gv_fundamental")
         return (F.reshape(3, 3) if np.any(F) else None), mask[:n].astype(bool)
 
+    def gv_estimate(self, kpts0: np.ndarray, kpts1: np.ndarray, threshold: float = 1.0, max_iters: int = 10000, seed: int = 0,
+                    estimator: str = "ransac8", confidence: float = 0.9999):
+        """Matched keypoints (n,2) each -> (F (3,3) float32 or None, inlier mask bool (n,), hypotheses run) with the named estimator
+        (dimb_gv_estimate; ``confidence`` is read by lo-ransac only)."""
+        k0 = np.ascontiguousarray(kpts0, np.float32)
+        k1 = np.ascontiguousarray(kpts1, np.float32)
+        n = k0.shape[0]
+        F = np.zeros(9, np.float32)
+        mask = np.ones(max(n, 1), np.uint8)
+        cnt, hyp = C.c_int(0), C.c_int(0)
+        conf = GvConf(float(threshold), int(max_iters), 0, 0.0, gv_estimator(estimator), float(confidence))
+        self.check(self.lib.dimb_gv_estimate(self.h, _ptr(k0), _ptr(k1), n, C.byref(conf), int(seed) & 0xffffffff, _ptr(F), _ptr(mask),
+                                             C.byref(cnt), C.byref(hyp)), "dimb_gv_estimate")
+        return (F.reshape(3, 3) if np.any(F) else None), mask[:n].astype(bool), hyp.value
+
     def gv_verify_dev(self, f0: list, f1: list, d_matches, d_n_matches, cap, seeds, threshold=1.0, max_iters=10000, min_inliers=0,
-                      min_inlier_ratio=0.0, d_verified=0, d_n_verified=0, d_F=0, d_mask=0, d_n_inliers=0, stream=0):
+                      min_inlier_ratio=0.0, d_verified=0, d_n_verified=0, d_F=0, d_mask=0, d_n_inliers=0, stream=0, estimator="ransac8",
+                      confidence=0.9999):
         """Geometric verification of P match tables on the device (dimb_gv_verify_dev).  f0/f1: lists of FeatsDev (e.g.
         FeatureStoreDev.feats_dev); d_matches [P][cap][2] int64 / d_n_matches [P] int32 as LightGlueNet.match_dev writes them; seeds:
         one uint32 per pair (geometric_verification.gv_seed).  Outputs are device buffers (ints are device addresses): d_verified
         [P][cap][2] int64, d_n_verified [P] int32, d_F [P][9] float32, d_mask [P][cap] uint8, d_n_inliers [P] int32.  Asynchronous
-        on `stream`."""
+        on `stream`.  estimator: a name in GV_ESTIMATORS; confidence is read by lo-ransac only."""
         P = len(f0)
         a0 = (FeatsDev * P)(*f0)
         a1 = (FeatsDev * P)(*f1)
         sd = (C.c_uint * P)(*[int(s) & 0xffffffff for s in seeds])
-        conf = GvConf(float(threshold), int(max_iters), int(min_inliers), float(min_inlier_ratio))
+        conf = GvConf(float(threshold), int(max_iters), int(min_inliers), float(min_inlier_ratio), gv_estimator(estimator), float(confidence))
         self.check(self.lib.dimb_gv_verify_dev(self.h, P, a0, a1, d_matches, d_n_matches, cap, sd, C.byref(conf), d_verified, d_n_verified,
                                                d_F, d_mask, d_n_inliers, stream), "dimb_gv_verify_dev")
 

@@ -5,8 +5,13 @@
 //
 // Per pair: Hartley normalisation of the matched keypoints; H hypotheses (8 random correspondences each, counter-based RNG ->
 // reproducible), each solved by the normalised 8-point algorithm and scored by its Sampson inlier count over all matches by ONE
-// thread (gv_math.cuh); the best hypothesis is refitted twice by least squares on its inliers (local optimisation) and the final
-// inlier mask is written.  No adaptive stopping: every hypothesis runs in parallel, H = min(max_iters, 8192).
+// thread (gv_math.cuh); the best hypothesis is refitted twice by least squares on its inliers and the final inlier mask is written.
+// Two estimators share that frame:
+//   ransac8 (estimator 0): no adaptive stopping, every hypothesis runs in parallel, H = max(64, min(max_iters, 8192)).
+//   lo-ransac (estimator 1): 7-point hypotheses (up to 3 models each) in waves of kLoWave; after each wave one CTA per pair adopts
+//     the wave's best model if it beats the pair's best and runs local optimisation on it (inner RANSAC on 16-inlier least-squares
+//     fits, each iterated 4 times), then applies confidence stopping.  Up to min(max_iters, 65536) hypotheses; every wave is
+//     enqueued and a pair that has stopped returns at once, so nothing waits for the host.  The finalize step is shared.
 // RANSAC is stochastic in the reference too (pydegensac's own RNG), so parity is statistical: tests compare inlier sets on data
 // with known geometry and against OpenCV on the same matches.  Every reduction runs in a fixed order (integer atomics only), so a
 // pair's result is a function of its matches, its seed and the configuration alone: bitwise reproducible across calls and batches.
@@ -130,9 +135,23 @@ __global__ void gv_hypotheses_kernel(const GvPair* pairs, const float* xy, const
 // rows of the match table in order (ballot + warp prefix + block prefix per 256-row chunk) and the gated count
 constexpr int kFinThreads = 256, kFinWarps = kFinThreads / 32;
 
+// lo-ransac state of one pair (zeroed before the first wave)
+struct GvLo {
+  unsigned long long wave_key;  // best (count << 32 | ~(3 h + root)) of the current wave; 0: no model yet
+  float F[9];                   // the adopted model; its count is best[pair] >> 32
+  int lim;                      // hypotheses the pair runs: min(H, the confidence bound of its best model); 0 before the first wave
+  int run;                      // hypotheses run so far
+  int done;
+};
+constexpr int kLoWave = 1024, kLoMaxIters = 65536, kLoInner = 20, kLoSample = 16, kLoLsq = 4;
+__device__ __forceinline__ int gv_lo_lim(const GvLo& s, int H) { return s.lim ? s.lim : H; }
+
+
+// kLo: the model is the one lo-ransac adopted (lo[pair].F) rather than hypothesis best[pair] re-solved
+template <bool kLo>
 __global__ void __launch_bounds__(kFinThreads)
 gv_finalize_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, const unsigned long long* best, int cap, float thr2,
-                   float* Fout, unsigned char* mask, int* n_inl, GvCompact cmp) {
+                   float* Fout, unsigned char* mask, int* n_inl, GvCompact cmp, const GvLo* lo) {
   const int pi = blockIdx.x, t = threadIdx.x, lane = t & 31, wid = t >> 5;
   const GvPair p = pairs[pi];
   const int n = gv_count(p);
@@ -158,7 +177,9 @@ gv_finalize_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, 
   }
   const gv::Norm n0 = norms[2 * pi], n1 = norms[2 * pi + 1];
   const float* pts = xy + static_cast<size_t>(pi) * cap * 4;
-  if (t == 0) {
+  if (kLo) {
+    if (t < 9) F[t] = lo[pi].F[t];
+  } else if (t == 0) {
     const unsigned h = 0xffffffffu - static_cast<unsigned>(best[pi] & 0xffffffffu);
     int idx[8], id8[8];
     float k0[16], k1[16], f[9];
@@ -259,9 +280,234 @@ gv_finalize_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, 
   }
 }
 
+// ------------------------------------------------------------------ lo-ransac
+// grid (kLoWave / 128, P): hypothesis h = wave * kLoWave + thread of the pair's wave, for h < its limit; 7 points, up to 3 models,
+// each scored over all matches; wave_key = max over (count << 32 | ~(3 h + root)) (ties -> lowest hypothesis, then lowest root)
+__global__ void __launch_bounds__(128)
+gv_lo_hypotheses_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, GvLo* lo, int cap, int wave, int H, float thr2) {
+  const int pi = blockIdx.y, h = wave * kLoWave + blockIdx.x * blockDim.x + threadIdx.x;
+  GvLo& s = lo[pi];
+  if (s.done) return;
+  const GvPair p = pairs[pi];
+  const int n = gv_count(p);
+  if (n < 8 || h >= gv_lo_lim(s, H)) return;
+  const float* pts = xy + static_cast<size_t>(pi) * cap * 4;
+  int idx[7], id7[7];
+  gv::sample7(p.seed, h, n, idx);
+  float k0[14], k1[14];
+  for (int k = 0; k < 7; ++k) {
+    k0[2 * k] = pts[4 * idx[k]], k0[2 * k + 1] = pts[4 * idx[k] + 1], k1[2 * k] = pts[4 * idx[k] + 2], k1[2 * k + 1] = pts[4 * idx[k] + 3];
+    id7[k] = k;
+  }
+  float F[3][9];
+  const int m = gv::seven_point(k0, k1, id7, norms[2 * pi], norms[2 * pi + 1], F);
+  if (m == 0) return;
+  int cnt[3] = {0, 0, 0};
+  const float4* p4 = reinterpret_cast<const float4*>(pts);
+  for (int i = 0; i < n; ++i) {
+    const float4 c = __ldg(p4 + i);
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+      if (r < m) cnt[r] += gv::sampson2(F[r], c.x, c.y, c.z, c.w) < thr2;
+  }
+  unsigned long long key = 0ull;
+  for (int r = 0; r < m; ++r)
+    key = max(key, (static_cast<unsigned long long>(cnt[r]) << 32) | (0xffffffffu - static_cast<unsigned>(3 * h + r)));
+  atomicMax(&s.wave_key, key);
+}
+
+// CTA-wide count of the matches whose Sampson distance to F is below thr2 and, with `normal`, the sum of their normal-matrix rows
+// into Nm (45 upper-triangular entries).  Per-thread partials, warp shuffles, warps summed in order: a fixed order, no float atomics.
+// Every thread gets the count.
+__device__ int gv_lo_sums(const float* Fs, const float* pts, int n, float thr2, gv::Norm n0, gv::Norm n1, bool normal,
+                          float (*part)[45], int* wcnt, float* Nm) {
+  const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
+  float f[9];
+  for (int j = 0; j < 9; ++j) f[j] = Fs[j];
+  float acc[45];
+#pragma unroll
+  for (int k = 0; k < 45; ++k) acc[k] = 0.f;
+  int c = 0;
+  for (int i = t; i < n; i += blockDim.x) {
+    const float x0 = pts[4 * i], y0 = pts[4 * i + 1], x1 = pts[4 * i + 2], y1 = pts[4 * i + 3];
+    if (gv::sampson2(f, x0, y0, x1, y1) < thr2) {
+      ++c;
+      if (normal) {
+        float a[9];
+        gv::normal_row(x0, y0, x1, y1, n0, n1, a);
+        int k = 0;
+#pragma unroll
+        for (int r = 0; r < 9; ++r)
+#pragma unroll
+          for (int q = r; q < 9; ++q) acc[k++] += a[r] * a[q];
+      }
+    }
+  }
+  for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+  if (lane == 0) wcnt[wid] = c;
+  if (normal) {
+#pragma unroll
+    for (int k = 0; k < 45; ++k) {
+      float v = acc[k];
+      for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (lane == 0) part[wid][k] = v;
+    }
+  }
+  __syncthreads();
+  if (normal && t < 45) {
+    float a = 0.f;
+    for (int w = 0; w < kFinWarps; ++w) a += part[w][t];
+    Nm[t] = a;
+  }
+  int total = 0;
+  for (int w = 0; w < kFinWarps; ++w) total += wcnt[w];
+  __syncthreads();  // wcnt / part are rewritten by the next call; Nm is complete
+  return total;
+}
+
+// the indices of the matches within thr2 of F, in order (ballot + warp prefix + block prefix per chunk), into out; returns their number
+__device__ int gv_lo_inliers(const float* Fs, const float* pts, int n, float thr2, int* out, int* wcnt) {
+  const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
+  float f[9];
+  for (int j = 0; j < 9; ++j) f[j] = Fs[j];
+  int total = 0;
+  for (int base = 0; base < n; base += kFinThreads) {
+    const int i = base + t;
+    const bool in = i < n && gv::sampson2(f, pts[4 * i], pts[4 * i + 1], pts[4 * i + 2], pts[4 * i + 3]) < thr2;
+    const unsigned bal = __ballot_sync(0xffffffffu, in);
+    if (lane == 0) wcnt[wid] = __popc(bal);
+    __syncthreads();
+    int off = total + __popc(bal & ((1u << lane) - 1u));
+    for (int w = 0; w < wid; ++w) off += wcnt[w];
+    if (in) out[off] = i;
+    for (int w = 0; w < kFinWarps; ++w) total += wcnt[w];
+    __syncthreads();
+  }
+  return total;
+}
+
+// refit_from_normal on the 45 sums Nm (one thread)
+__device__ bool gv_lo_refit(const float* Nm, gv::Norm n0, gv::Norm n1, float f[9]) {
+  float N9[9][9];
+  int k = 0;
+  for (int r = 0; r < 9; ++r)
+    for (int q = r; q < 9; ++q) N9[r][q] = N9[q][r] = Nm[k++];
+  return gv::refit_from_normal(N9, n0, n1, f);
+}
+
+// one CTA per running pair, after the hypotheses of wave `wave`: adopt the wave's best model if it beats the pair's best, then local
+// optimisation - kLoInner times: the inliers at 2x the threshold (fewer than kLoSample: stop), a least-squares fit of kLoSample of them
+// drawn on the LO stream, kLoLsq least-squares refits on that fit's inliers, the result adopted if it explains more matches.  Then
+// confidence stopping: the pair is done once it has run min(its limit, the hypotheses its best model calls for).  inl: [P][cap] scratch.
+__global__ void __launch_bounds__(kFinThreads)
+gv_lo_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, unsigned long long* best, GvLo* lo, int* inl, int cap, int wave,
+             int H, float thr2, float confidence) {
+  const int pi = blockIdx.x, t = threadIdx.x;
+  GvLo* s = lo + pi;
+  if (s->done) return;
+  const GvPair p = pairs[pi];
+  const int n = gv_count(p), lim = gv_lo_lim(*s, H);
+  if (n < 8) {  // finalize keeps every match; no hypothesis ran
+    if (t == 0) s->done = 1;
+    return;
+  }
+  const gv::Norm n0 = norms[2 * pi], n1 = norms[2 * pi + 1];
+  const float* pts = xy + static_cast<size_t>(pi) * cap * 4;
+  __shared__ float F[9], G[9], Nm[45];
+  __shared__ float part[kFinWarps][45];
+  __shared__ int wcnt[kFinWarps];
+  __shared__ int adopt, ok, cur;
+  if (t == 0) {
+    const unsigned long long key = s->wave_key;
+    s->wave_key = 0ull;
+    cur = static_cast<int>(best[pi] >> 32);
+    adopt = key != 0ull && static_cast<int>(key >> 32) > cur;
+    if (adopt) {  // re-solve the winning hypothesis
+      const unsigned id = 0xffffffffu - static_cast<unsigned>(key & 0xffffffffu);
+      int idx[7], id7[7];
+      float k0[14], k1[14], M[3][9];
+      gv::sample7(p.seed, id / 3, n, idx);
+      for (int k = 0; k < 7; ++k) {
+        k0[2 * k] = pts[4 * idx[k]], k0[2 * k + 1] = pts[4 * idx[k] + 1], k1[2 * k] = pts[4 * idx[k] + 2], k1[2 * k + 1] = pts[4 * idx[k] + 3];
+        id7[k] = k;
+      }
+      gv::seven_point(k0, k1, id7, n0, n1, M);
+      for (int j = 0; j < 9; ++j) F[j] = M[id % 3][j];
+      cur = static_cast<int>(key >> 32);
+    }
+  }
+  __syncthreads();
+  if (adopt) {
+    int* list = inl + static_cast<size_t>(pi) * cap;
+    for (int it = 0; it < kLoInner; ++it) {
+      const int m = gv_lo_inliers(F, pts, n, 4.f * thr2, list, wcnt);
+      if (m < kLoSample) break;
+      if (t == 0) {
+        int pos[kLoSample];
+        gv::lo_sample16(p.seed, wave, it, m, pos);
+        float N9[9][9] = {}, f[9];
+        for (int k = 0; k < kLoSample; ++k) {
+          const int i = list[pos[k]];
+          float a[9];
+          gv::normal_row(pts[4 * i], pts[4 * i + 1], pts[4 * i + 2], pts[4 * i + 3], n0, n1, a);
+          for (int r = 0; r < 9; ++r)
+            for (int q = 0; q < 9; ++q) N9[r][q] += a[r] * a[q];
+        }
+        ok = gv::refit_from_normal(N9, n0, n1, f);
+        if (ok)
+          for (int j = 0; j < 9; ++j) G[j] = f[j];
+      }
+      __syncthreads();
+      if (!ok) continue;
+      for (int r = 0; r < kLoLsq; ++r) {
+        const int c = gv_lo_sums(G, pts, n, thr2, n0, n1, true, part, wcnt, Nm);
+        if (t == 0) {
+          float f[9];
+          ok = c >= 8 && gv_lo_refit(Nm, n0, n1, f);
+          if (ok)
+            for (int j = 0; j < 9; ++j) G[j] = f[j];
+        }
+        __syncthreads();
+        if (!ok) break;
+      }
+      const int c = gv_lo_sums(G, pts, n, thr2, n0, n1, false, part, wcnt, Nm);
+      if (t == 0 && c > cur) {
+        cur = c;
+        for (int j = 0; j < 9; ++j) F[j] = G[j];
+      }
+      __syncthreads();
+    }
+  }
+  if (t == 0) {
+    if (adopt) {
+      best[pi] = static_cast<unsigned long long>(cur) << 32;
+      for (int j = 0; j < 9; ++j) s->F[j] = F[j];
+    }
+    const int run = min(lim, (wave + 1) * kLoWave), need = min(lim, gv::lo_needed(cur, n, confidence, H));
+    s->run = run;
+    s->lim = need;
+    s->done = run >= need;
+  }
+}
+
+// The estimator of a gv_run call: 0 ransac8, 1 lo-ransac (confidence read by lo-ransac only).  lo_slot, lo_slot + 1: lo-ransac's
+// context scratch slots (52 for dimb_gv_estimate, 54 for dimb_gv_verify_dev).  gv_run's d_lo (optional) receives the address of the
+// per-pair lo-ransac state, whose `run` is the hypotheses count.
+struct GvEstimator {
+  int kind, max_iters;
+  float confidence;
+  int lo_slot;
+};
+
+int gv_check_estimator(const dimb_gv_conf& c) {
+  if (c.estimator == 0) return DIMB_OK;
+  if (c.estimator != 1 || !(c.confidence > 0.f && c.confidence < 1.f) || c.max_iters < 1) return DIMB_ERR_ARG;
+  return DIMB_OK;
+}
+
 // slot0 .. slot0 + 3: the context scratch slots of the calling entry (40 for the float32 entries, 48 for dimb_gv_verify_dev)
-int gv_run(dimb_ctx* ctx, cudaStream_t st, const std::vector<GvPair>& hp, int cap, float threshold, int max_iters, float* d_F,
-           unsigned char* d_mask, int* d_ninl, const GvCompact& cmp, int slot0) {
+int gv_run(dimb_ctx* ctx, cudaStream_t st, const std::vector<GvPair>& hp, int cap, float threshold, const GvEstimator& est, float* d_F,
+           unsigned char* d_mask, int* d_ninl, const GvCompact& cmp, int slot0, GvLo** d_lo = nullptr) {
   const int P = static_cast<int>(hp.size());
   GvPair* d_pairs;
   float* d_xy;
@@ -271,15 +517,38 @@ int gv_run(dimb_ctx* ctx, cudaStream_t st, const std::vector<GvPair>& hp, int ca
   DIMB_TRY(dimb_scratch(ctx, slot0 + 1, static_cast<size_t>(P) * cap * 4 * sizeof(float), reinterpret_cast<void**>(&d_xy)));
   DIMB_TRY(dimb_scratch(ctx, slot0 + 2, 2 * P * sizeof(gv::Norm), reinterpret_cast<void**>(&d_norm)));
   DIMB_TRY(dimb_scratch(ctx, slot0 + 3, P * sizeof(unsigned long long), reinterpret_cast<void**>(&d_best)));
+  GvLo* lo = nullptr;
+  int* d_inl = nullptr;
+  if (est.kind == 1) {
+    DIMB_TRY(dimb_scratch(ctx, est.lo_slot, P * sizeof(GvLo), reinterpret_cast<void**>(&lo)));
+    DIMB_TRY(dimb_scratch(ctx, est.lo_slot + 1, static_cast<size_t>(P) * cap * sizeof(int), reinterpret_cast<void**>(&d_inl)));
+    if (d_lo) *d_lo = lo;
+  }
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_pairs, hp.data(), P * sizeof(GvPair), cudaMemcpyHostToDevice, st));
-  const int H = std::max(64, std::min(max_iters, 8192));
   const float thr2 = threshold * threshold;
+  if (est.kind == 1) {
+    const int H = std::min(est.max_iters, kLoMaxIters);
+    ProfScope prof(ctx, st, "gv.lo_ransac");
+    DIMB_CUDA_OK(ctx, cudaMemsetAsync(lo, 0, P * sizeof(GvLo), st));
+    gv_prepare_kernel<<<P, 256, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap);
+    DIMB_LAUNCH_CHECK(ctx);
+    for (int w = 0; w * kLoWave < H; ++w) {
+      gv_lo_hypotheses_kernel<<<dim3(kLoWave / 128, P), 128, 0, st>>>(d_pairs, d_xy, d_norm, lo, cap, w, H, thr2);
+      DIMB_LAUNCH_CHECK(ctx);
+      gv_lo_kernel<<<P, kFinThreads, 0, st>>>(d_pairs, d_xy, d_norm, d_best, lo, d_inl, cap, w, H, thr2, est.confidence);
+      DIMB_LAUNCH_CHECK(ctx);
+    }
+    gv_finalize_kernel<true><<<P, kFinThreads, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap, thr2, d_F, d_mask, d_ninl, cmp, lo);
+    DIMB_LAUNCH_CHECK(ctx);
+    return DIMB_OK;
+  }
+  const int H = std::max(64, std::min(est.max_iters, 8192));
   ProfScope prof(ctx, st, "gv.ransac");
   gv_prepare_kernel<<<P, 256, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap);
   DIMB_LAUNCH_CHECK(ctx);
   gv_hypotheses_kernel<<<dim3(ceil_div(H, 128), P), 128, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap, H, thr2);
   DIMB_LAUNCH_CHECK(ctx);
-  gv_finalize_kernel<<<P, kFinThreads, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap, thr2, d_F, d_mask, d_ninl, cmp);
+  gv_finalize_kernel<false><<<P, kFinThreads, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap, thr2, d_F, d_mask, d_ninl, cmp, nullptr);
   DIMB_LAUNCH_CHECK(ctx);
   return DIMB_OK;
 }
@@ -288,12 +557,16 @@ int gv_run(dimb_ctx* ctx, cudaStream_t st, const std::vector<GvPair>& hp, int ca
 
 extern "C" {
 
-// Host entry: matched keypoints kpts0[i] <-> kpts1[i] (n,2) float32 pixels.  F [9] row-major with x1^T F x0 = 0 (zeros when n < 8 or
-// no model was found - the reference returns F = None and an all-True mask then), mask [n] 0/1, n_inliers.
-int dimb_gv_fundamental(dimb_ctx* ctx, const float* kpts0, const float* kpts1, int n, float threshold, int max_iters, unsigned seed, float* F,
-                        unsigned char* mask, int* n_inliers) {
-  if (!ctx || n < 0 || (n > 0 && (!kpts0 || !kpts1)) || !F || !mask || !n_inliers || threshold <= 0.f) return DIMB_ERR_ARG;
+// Host entry: matched keypoints kpts0[i] <-> kpts1[i] (n,2) float32 pixels, verified with the estimator of conf (its gate fields are
+// not read).  F [9] row-major with x1^T F x0 = 0 (zeros when n < 8 or no model was found - the reference returns F = None and an
+// all-True mask then), mask [n] 0/1, n_inliers, n_hypotheses (optional): the hypotheses that ran.
+int dimb_gv_estimate(dimb_ctx* ctx, const float* kpts0, const float* kpts1, int n, const dimb_gv_conf* conf, unsigned seed, float* F,
+                     unsigned char* mask, int* n_inliers, int* n_hypotheses) {
+  if (!ctx || n < 0 || (n > 0 && (!kpts0 || !kpts1)) || !conf || !F || !mask || !n_inliers || !(conf->threshold > 0.f))
+    return DIMB_ERR_ARG;
+  DIMB_TRY(gv_check_estimator(*conf));
   DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  if (n_hypotheses) *n_hypotheses = 0;
   if (n == 0) {
     for (int i = 0; i < 9; ++i) F[i] = 0.f;
     *n_inliers = 0;
@@ -312,12 +585,23 @@ int dimb_gv_fundamental(dimb_ctx* ctx, const float* kpts0, const float* kpts1, i
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_k1, kpts1, static_cast<size_t>(n) * 2 * sizeof(float), cudaMemcpyHostToDevice, st));
   std::vector<GvPair> hp(1);
   hp[0] = GvPair{d_k0, d_k1, nullptr, nullptr, n, n, seed, {0, 0}, {0, 0}};
-  DIMB_TRY(gv_run(ctx, st, hp, n, threshold, max_iters, d_F, d_mask, d_n, GvCompact{}, 40));
+  GvLo* d_lo = nullptr;
+  DIMB_TRY(gv_run(ctx, st, hp, n, conf->threshold, GvEstimator{conf->estimator, conf->max_iters, conf->confidence, 52}, d_F, d_mask, d_n,
+                  GvCompact{}, 40, &d_lo));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(F, d_F, 9 * sizeof(float), cudaMemcpyDeviceToHost, st));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(n_inliers, d_n, sizeof(int), cudaMemcpyDeviceToHost, st));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(mask, d_mask, n, cudaMemcpyDeviceToHost, st));
+  if (n_hypotheses && d_lo) DIMB_CUDA_OK(ctx, cudaMemcpyAsync(n_hypotheses, &d_lo->run, sizeof(int), cudaMemcpyDeviceToHost, st));
   DIMB_CUDA_OK(ctx, cudaStreamSynchronize(st));
+  if (n_hypotheses && !d_lo && n >= 8) *n_hypotheses = std::max(64, std::min(conf->max_iters, 8192));
   return DIMB_OK;
+}
+
+// ransac8 through dimb_gv_estimate
+int dimb_gv_fundamental(dimb_ctx* ctx, const float* kpts0, const float* kpts1, int n, float threshold, int max_iters, unsigned seed, float* F,
+                        unsigned char* mask, int* n_inliers) {
+  const dimb_gv_conf conf{threshold, max_iters, 0, 0.f, 0, 0.f};
+  return dimb_gv_estimate(ctx, kpts0, kpts1, n, &conf, seed, F, mask, n_inliers, nullptr);
 }
 
 // Batch on device buffers, asynchronous on `stream`: pair p verifies d_matches[p][0..d_n_matches[p]) (the output layout of
@@ -333,7 +617,8 @@ int dimb_gv_fundamental_batch_dev(dimb_ctx* ctx, int P, const float* const* d_kp
   for (int p = 0; p < P; ++p)
     hp[p] = GvPair{d_kpts0[p], d_kpts1[p], reinterpret_cast<const long long*>(d_matches) + static_cast<size_t>(p) * cap * 2, d_n_matches + p, 0, cap,
                    seed + 0x9E37u * static_cast<unsigned>(p), {0, 0}, {0, 0}};
-  return gv_run(ctx, static_cast<cudaStream_t>(stream), hp, cap, threshold, max_iters, d_F, d_mask, d_n_inliers, GvCompact{}, 40);
+  return gv_run(ctx, static_cast<cudaStream_t>(stream), hp, cap, threshold, GvEstimator{0, max_iters, 0.f, 0}, d_F, d_mask, d_n_inliers,
+                GvCompact{}, 40);
 }
 
 // P pairs of an image set, asynchronous on `stream`: keypoints from dimb_feats_dev (feature-store slots or float32 extractor
@@ -346,6 +631,7 @@ int dimb_gv_verify_dev(dimb_ctx* ctx, int P, const dimb_feats_dev* f0, const dim
     return DIMB_ERR_ARG;
   if (!(conf->threshold > 0.f) || conf->min_inliers < 0 || !(conf->min_inlier_ratio >= 0.f && conf->min_inlier_ratio <= 1.f))
     return DIMB_ERR_ARG;
+  DIMB_TRY(gv_check_estimator(*conf));
   for (int p = 0; p < P; ++p)
     if (!f0[p].keypoints || !f1[p].keypoints) return DIMB_ERR_ARG;
   DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
@@ -355,7 +641,8 @@ int dimb_gv_verify_dev(dimb_ctx* ctx, int P, const dimb_feats_dev* f0, const dim
                    d_n_matches + p, 0, cap, seeds[p], {f0[p].f16 ? 1 : 0, f1[p].f16 ? 1 : 0},
                    {f0[p].round_fp16 ? 1 : 0, f1[p].round_fp16 ? 1 : 0}};
   const GvCompact cmp{reinterpret_cast<long long*>(d_verified), d_n_verified, conf->min_inliers, conf->min_inlier_ratio};
-  return gv_run(ctx, static_cast<cudaStream_t>(stream), hp, cap, conf->threshold, conf->max_iters, d_F, d_mask, d_n_inliers, cmp, 48);
+  return gv_run(ctx, static_cast<cudaStream_t>(stream), hp, cap, conf->threshold,
+                GvEstimator{conf->estimator, conf->max_iters, conf->confidence, 54}, d_F, d_mask, d_n_inliers, cmp, 48);
 }
 
 }  // extern "C"

@@ -9,7 +9,8 @@
 //   dimb_selftest_lg_assign / dimb_selftest_lg_tail: the LightGlue assignment and per-layer tail (lg_assign.cuh) through their launch
 //     helpers; dimb_selftest_lgx_assign: the shape-generic LightGlue assignment and filter (lgx_assign.cuh) through its launch helper;
 //     dimb_selftest_sg_sinkhorn: SuperGlue's Sinkhorn and mutual-max matching (sg_assign.cuh);
-//   dimb_gv_host: the RANSAC arithmetic of gv.cu on the host.
+//   dimb_gv_host / dimb_gv_lo_host / dimb_gv_seven_point_host: the RANSAC arithmetic of gv.cu on the host (ransac8, lo-ransac, the
+//     7-point solver).
 #include <algorithm>
 #include <cstring>
 #include <vector>
@@ -693,11 +694,11 @@ extern "C" int dimb_selftest_sp_describe(dimb_ctx* ctx, const int* sel_idx, cons
 }
 
 // ------------------------------------------------------------------ CPU drive of the RANSAC arithmetic of gv.cu (gv_math.cuh)
-// The same host/device functions, run sequentially on the host: lets tests/ check the estimator without a GPU.
+// The same host/device functions, run sequentially on the host: lets tests/ check the estimators without a GPU.  Sums run in a
+// different order than on the device, so results agree statistically, not bitwise.
 #include "gv_math.cuh"
-extern "C" int dimb_gv_host(const float* k0, const float* k1, int n, float threshold, int iters, unsigned seed, float* F, unsigned char* mask) {
-  if (!k0 || !k1 || !F || !mask || n < 8) return DIMB_ERR_ARG;
-  gv::Norm nm[2];
+namespace {
+void gv_host_norms(const float* k0, const float* k1, int n, gv::Norm nm[2]) {
   for (int s = 0; s < 2; ++s) {
     const float* k = s ? k1 : k0;
     double mx = 0, my = 0, d = 0;
@@ -706,22 +707,35 @@ extern "C" int dimb_gv_host(const float* k0, const float* k1, int n, float thres
     for (int i = 0; i < n; ++i) d += sqrt((k[2 * i] - mx) * (k[2 * i] - mx) + (k[2 * i + 1] - my) * (k[2 * i + 1] - my));
     nm[s] = gv::Norm{static_cast<float>(mx), static_cast<float>(my), static_cast<float>(1.41421356 * n / d)};
   }
-  const float thr2 = threshold * threshold;
-  int best = -1;
-  float bf[9] = {0};
-  for (int h = 0; h < iters; ++h) {
-    int idx[8];
-    float f[9];
-    gv::sample8(seed, h, n, idx);
-    if (!gv::eight_point(k0, k1, idx, nm[0], nm[1], f)) continue;
-    int c = 0;
-    for (int i = 0; i < n; ++i) c += gv::sampson2(f, k0[2 * i], k0[2 * i + 1], k1[2 * i], k1[2 * i + 1]) < thr2;
-    if (c > best) {
-      best = c;
-      for (int j = 0; j < 9; ++j) bf[j] = f[j];
+}
+
+// the matches within thr2 of f: their count, and with `ids` their indices in order
+int gv_host_count(const float* f, const float* k0, const float* k1, int n, float thr2, std::vector<int>* ids = nullptr) {
+  int c = 0;
+  if (ids) ids->clear();
+  for (int i = 0; i < n; ++i)
+    if (gv::sampson2(f, k0[2 * i], k0[2 * i + 1], k1[2 * i], k1[2 * i + 1]) < thr2) {
+      ++c;
+      if (ids) ids->push_back(i);
     }
+  return c;
+}
+
+// least-squares fit on the matches `ids` (at least 8)
+bool gv_host_lsq(const std::vector<int>& ids, const float* k0, const float* k1, const gv::Norm nm[2], float f[9]) {
+  if (ids.size() < 8) return false;
+  float N[9][9] = {};
+  for (int i : ids) {
+    float a[9];
+    gv::normal_row(k0[2 * i], k0[2 * i + 1], k1[2 * i], k1[2 * i + 1], nm[0], nm[1], a);
+    for (int p = 0; p < 9; ++p)
+      for (int q = 0; q < 9; ++q) N[p][q] += a[p] * a[q];
   }
-  if (best < 8) return DIMB_ERR_UNSUPPORTED;
+  return gv::refit_from_normal(N, nm[0], nm[1], f);
+}
+
+// the finalize step: two least-squares refits of bf on its inliers (kept unless they lose inliers), then F and the mask
+void gv_host_finish(float bf[9], const float* k0, const float* k1, int n, float thr2, const gv::Norm nm[2], float* F, unsigned char* mask) {
   for (int round = 0; round < 2; ++round) {
     float N[9][9] = {};
     int c = 0;
@@ -744,7 +758,104 @@ extern "C" int dimb_gv_host(const float* k0, const float* k1, int n, float thres
   }
   for (int j = 0; j < 9; ++j) F[j] = bf[j];
   for (int i = 0; i < n; ++i) mask[i] = gv::sampson2(bf, k0[2 * i], k0[2 * i + 1], k1[2 * i], k1[2 * i + 1]) < thr2;
+}
+}  // namespace
+
+extern "C" int dimb_gv_host(const float* k0, const float* k1, int n, float threshold, int iters, unsigned seed, float* F, unsigned char* mask) {
+  if (!k0 || !k1 || !F || !mask || n < 8) return DIMB_ERR_ARG;
+  gv::Norm nm[2];
+  gv_host_norms(k0, k1, n, nm);
+  const float thr2 = threshold * threshold;
+  int best = -1;
+  float bf[9] = {0};
+  for (int h = 0; h < iters; ++h) {
+    int idx[8];
+    float f[9];
+    gv::sample8(seed, h, n, idx);
+    if (!gv::eight_point(k0, k1, idx, nm[0], nm[1], f)) continue;
+    const int c = gv_host_count(f, k0, k1, n, thr2);
+    if (c > best) {
+      best = c;
+      for (int j = 0; j < 9; ++j) bf[j] = f[j];
+    }
+  }
+  if (best < 8) return DIMB_ERR_UNSUPPORTED;
+  gv_host_finish(bf, k0, k1, n, thr2, nm, F, mask);
   return DIMB_OK;
+}
+
+// lo-ransac of gv.cu in wave order on the host: the wave's best hypothesis (highest count, then lowest 3 h + root), its local
+// optimisation when it beats the pair's best, confidence stopping, the finalize step.  n_hyp: the hypotheses that ran.  n < 8 or no
+// model: DIMB_ERR_UNSUPPORTED (the device keeps every match then).
+extern "C" int dimb_gv_lo_host(const float* k0, const float* k1, int n, float threshold, int max_iters, float confidence, unsigned seed,
+                               float* F, unsigned char* mask, int* n_hyp) {
+  if (!k0 || !k1 || !F || !mask || !n_hyp || n < 8 || max_iters < 1 || !(confidence > 0.f && confidence < 1.f)) return DIMB_ERR_ARG;
+  constexpr int W = 1024;
+  gv::Norm nm[2];
+  gv_host_norms(k0, k1, n, nm);
+  const float thr2 = threshold * threshold;
+  const int H = std::min(max_iters, 65536);
+  int best = 0, lim = H, run = 0;
+  float bf[9] = {0};
+  std::vector<int> in;
+  for (int wave = 0; run < lim; ++wave) {
+    int wb = -1;
+    float wf[9] = {0};
+    const int end = std::min(lim, (wave + 1) * W);
+    for (int h = wave * W; h < end; ++h) {
+      int idx[7];
+      float M[3][9];
+      gv::sample7(seed, h, n, idx);
+      const int m = gv::seven_point(k0, k1, idx, nm[0], nm[1], M);
+      for (int r = 0; r < m; ++r) {
+        const int c = gv_host_count(M[r], k0, k1, n, thr2);
+        if (c > wb) {
+          wb = c;
+          for (int j = 0; j < 9; ++j) wf[j] = M[r][j];
+        }
+      }
+    }
+    run = end;
+    if (wb > best) {
+      best = wb;
+      for (int j = 0; j < 9; ++j) bf[j] = wf[j];
+      for (int it = 0; it < 20; ++it) {
+        gv_host_count(bf, k0, k1, n, 4.f * thr2, &in);
+        if (in.size() < 16) break;
+        int pos[16];
+        gv::lo_sample16(seed, wave, it, static_cast<int>(in.size()), pos);
+        std::vector<int> sub(16);
+        for (int k = 0; k < 16; ++k) sub[k] = in[pos[k]];
+        float f[9], g[9];
+        if (!gv_host_lsq(sub, k0, k1, nm, f)) continue;
+        for (int r = 0; r < 4; ++r) {
+          gv_host_count(f, k0, k1, n, thr2, &in);
+          if (!gv_host_lsq(in, k0, k1, nm, g)) break;
+          for (int j = 0; j < 9; ++j) f[j] = g[j];
+        }
+        const int c = gv_host_count(f, k0, k1, n, thr2);
+        if (c > best) {
+          best = c;
+          for (int j = 0; j < 9; ++j) bf[j] = f[j];
+        }
+      }
+    }
+    lim = std::min(lim, gv::lo_needed(best, n, confidence, H));
+  }
+  *n_hyp = run;
+  if (best < 8) return DIMB_ERR_UNSUPPORTED;
+  gv_host_finish(bf, k0, k1, n, thr2, nm, F, mask);
+  return DIMB_OK;
+}
+
+// gv::seven_point on 7 correspondences k0[i] <-> k1[i] (pixels) with the Hartley normalisations of those 7 points: the models in
+// F [3][9], their number returned
+extern "C" int dimb_gv_seven_point_host(const float* k0, const float* k1, float* F) {
+  if (!k0 || !k1 || !F) return DIMB_ERR_ARG;
+  gv::Norm nm[2];
+  gv_host_norms(k0, k1, 7, nm);
+  const int idx[7] = {0, 1, 2, 3, 4, 5, 6};
+  return gv::seven_point(k0, k1, idx, nm[0], nm[1], reinterpret_cast<float(*)[9]>(F));
 }
 
 // ------------------------------------------------------------------ matching heads: LightGlue assignment and tail, SuperGlue Sinkhorn

@@ -3,10 +3,17 @@
 ``geometric_verification(kpts0, kpts1, method, threshold, confidence, max_iters)`` keeps the reference's signature and return
 contract ``(F, inlMask)``: ``F`` a (3,3) fundamental matrix or ``None``, ``inlMask`` a boolean array over the correspondences;
 method NONE returns ``(None, all True)`` (:100-101) and fewer than 8 matches return ``(None, all True)`` (:107-111).  Every other
-method name of the reference (PYDEGENSAC, MAGSAC, RANSAC, the OpenCV USAC family) selects ONE estimator here: seeded 8-point
-RANSAC with Sampson inliers and two least-squares refits (csrc/gv.cu), all hypotheses evaluated in parallel.  ``confidence`` is
-accepted and unused (there is no adaptive stopping: min(max_iters, 8192) hypotheses always run).  Like the reference's
-estimators the result is stochastic in the sense that it depends on the seed; parity is statistical (tests/test_geometry.py).
+method name of the reference (PYDEGENSAC, MAGSAC, RANSAC, the OpenCV USAC family) runs the estimator chosen by ``estimator``
+(csrc/gv.cu), both seeded, with Sampson inliers and two least-squares refits of the final model:
+
+- ``"ransac8"`` (the default): max(64, min(max_iters, 8192)) 8-point hypotheses, all evaluated in parallel; ``confidence`` is
+  accepted and unused (no adaptive stopping).
+- ``"lo-ransac"``: 7-point hypotheses in waves of 1024, local optimisation of each wave's new best model and confidence stopping
+  (``confidence`` in (0, 1)), up to min(max_iters, 65536) hypotheses - the structure of pydegensac and OpenCV's USAC, which keeps
+  the true inliers at outlier ratios where ransac8 loses them.
+
+Like the reference's estimators the result is stochastic in the sense that it depends on the seed; parity is statistical
+(tests/test_geometry.py, tests/test_gv_lo.py).
 For image sets, ``gv_seed(seed, pair_id)`` is the seed of each pair, so that a pair's result does not depend on how the pair list is
 batched or sharded (``sharded.ImageSetMatcher(verification=...)``).
 """
@@ -45,10 +52,12 @@ def gv_seed(seed: int, pair_id: int) -> int:
 
 
 def geometric_verification(kpts0: np.ndarray = None, kpts1: np.ndarray = None, method="pydegensac", threshold: float = 1, confidence: float = 0.9999,
-                           max_iters: int = 10000, quiet: bool = False, device: int = 0, seed: int = 0, **kwargs):
+                           max_iters: int = 10000, quiet: bool = False, device: int = 0, seed: int = 0, estimator: str = "ransac8", **kwargs):
     from . import _native
     name = method_name(method)
+    _native.gv_estimator(estimator)
     n = len(kpts0)
     if name == "NONE" or n < 8:
         return None, np.ones(n, dtype=bool)
-    return _native.Context.get(device).gv_fundamental(kpts0, kpts1, threshold, max_iters, seed)
+    F, mask, _ = _native.Context.get(device).gv_estimate(kpts0, kpts1, threshold, max_iters, seed, estimator, confidence)
+    return F, mask

@@ -199,13 +199,14 @@ def export_verified_to_colmap(store, n_images: int, world: int, pairs, results, 
 def verification_conf(verification) -> dict | None:
     """The ``verification`` argument of ImageSetMatcher with its defaults filled in (None stays None).  Defaults: method
     "pydegensac", threshold 1.0, max_iters 10000, seed 0 (those of geometric_verification), min_inliers_per_pair 15 and
-    min_inlier_ratio_per_pair 0.2 (MatcherBase's general defaults).  ``confidence`` is accepted and unused, as in
-    geometric_verification."""
+    min_inlier_ratio_per_pair 0.2 (MatcherBase's general defaults), estimator "ransac8" and confidence 0.9999 (read by
+    estimator "lo-ransac" only, as in geometric_verification)."""
     if verification is None:
         return None
+    from ._native import gv_estimator
     from .geometric_verification import method_name
     conf = {"method": "pydegensac", "threshold": 1.0, "max_iters": 10000, "seed": 0, "min_inliers_per_pair": 15,
-            "min_inlier_ratio_per_pair": 0.2, "confidence": 0.9999}
+            "min_inlier_ratio_per_pair": 0.2, "confidence": 0.9999, "estimator": "ransac8"}
     unknown = set(verification) - set(conf)
     if unknown:
         raise ValueError(f"unknown verification option(s) {sorted(unknown)}; expected some of {sorted(conf)}")
@@ -213,6 +214,8 @@ def verification_conf(verification) -> dict | None:
     conf["method"] = method_name(conf["method"])
     if not float(conf["threshold"]) > 0 or int(conf["min_inliers_per_pair"]) < 0 or not 0 <= float(conf["min_inlier_ratio_per_pair"]) <= 1:
         raise ValueError("verification needs threshold > 0, min_inliers_per_pair >= 0 and 0 <= min_inlier_ratio_per_pair <= 1")
+    if gv_estimator(conf["estimator"]) == 1 and not (0 < float(conf["confidence"]) < 1 and int(conf["max_iters"]) >= 1):
+        raise ValueError("verification with estimator lo-ransac needs 0 < confidence < 1 and max_iters >= 1")
     return conf
 
 
@@ -1179,7 +1182,8 @@ class ImageSetMatcher:
                 f1 = [self.store.feats_dev(self.slots[j]) for _, j in chunk]
                 self.ctx.gv_verify_dev(f0, f1, m.data_ptr(), nm.data_ptr(), cap, [gv_seed(g["seed"], k) for k in ids], g["threshold"],
                                        g["max_iters"], g["min_inliers_per_pair"], g["min_inlier_ratio_per_pair"], self.v.data_ptr(),
-                                       self.nv.data_ptr(), self.F.data_ptr(), self.mask.data_ptr(), self.ninl.data_ptr(), stream.cuda_stream)
+                                       self.nv.data_ptr(), self.F.data_ptr(), self.mask.data_ptr(), self.ninl.data_ptr(), stream.cuda_stream,
+                                       g["estimator"], g["confidence"])
                 (raw, ver), (F, ninl) = self._read_back([(m, nm, cap), (self.v, self.nv, cap)], (self.F, self.ninl), e - s, stream)
                 for k, (i, (a, b)) in enumerate(zip(ids, chunk)):
                     Fk = F[k].reshape(3, 3).copy() if np.any(F[k]) else None

@@ -226,10 +226,14 @@ int dimb_fstore_block_dev(dimb_fstore* fs, void** d_base, size_t* slot_bytes, in
 
 /* ------------------------------------------------------------------ geometric verification (fundamental-matrix RANSAC)
  * Replaces the estimator inside geometric_verification (utils/geometric_verification.py:45-179: pydegensac.findFundamentalMatrix /
- * cv2.findFundamentalMat), the step after _match_pairs (matchers/matcher_base.py:298-340).  min(max_iters, 8192) 8-point
- * hypotheses per pair in parallel, Sampson inliers (threshold in pixels), two least-squares refits of the best model.  Stochastic
- * like the reference's estimators (seeded, reproducible here): parity is statistical.  F row-major, x1^T F x0 = 0; zeros and an
- * all-ones mask when fewer than 8 matches exist or no model is found (the reference returns F = None, mask all True). */
+ * cv2.findFundamentalMat), the step after _match_pairs (matchers/matcher_base.py:298-340).  Two estimators (dimb_gv_conf.estimator),
+ * both with Sampson inliers (threshold in pixels) and two least-squares refits of the final model:
+ *   ransac8: max(64, min(max_iters, 8192)) 8-point hypotheses per pair in parallel, no adaptive stopping;
+ *   lo-ransac: 7-point hypotheses in waves of 1024, local optimisation of each wave's new best model (inner RANSAC on 16-inlier
+ *     least-squares fits, each iterated 4 times) and confidence stopping, up to min(max_iters, 65536) hypotheses.
+ * Stochastic like the reference's estimators (seeded, reproducible here): parity is statistical.  F row-major, x1^T F x0 = 0; zeros
+ * and an all-ones mask when fewer than 8 matches exist or no model is found (the reference returns F = None, mask all True).
+ * dimb_gv_fundamental is dimb_gv_estimate with ransac8. */
 int dimb_gv_fundamental(dimb_ctx* ctx, const float* kpts0, const float* kpts1, int n, float threshold, int max_iters, unsigned seed, float* F,
                         unsigned char* mask, int* n_inliers);
 /* P pairs on device buffers, asynchronous on `stream`: matches in the output layout of dimb_lg_match_dev / dimb_pipe_* ([P][cap][2]
@@ -241,10 +245,19 @@ int dimb_gv_fundamental_batch_dev(dimb_ctx* ctx, int P, const float* const* d_kp
  * reproducible: a pair's mask, F and count depend on its matches, its seed and the configuration only. */
 typedef struct {
   float threshold;          /* Sampson distance threshold in pixels, > 0 */
-  int max_iters;            /* hypotheses per pair = max(64, min(max_iters, 8192)) */
+  int max_iters;            /* ransac8: hypotheses per pair = max(64, min(max_iters, 8192)); lo-ransac: at most min(max_iters, 65536) */
   int min_inliers;          /* gate: a pair keeps its verified table iff n_inliers >= min_inliers ... */
   float min_inlier_ratio;   /* ... and float(n_inliers) >= min_inlier_ratio * float(n_raw), in [0, 1] (0 / 0: every pair kept) */
+  int estimator;            /* 0: ransac8, 1: lo-ransac (a zero-filled trailing part of the struct means ransac8) */
+  float confidence;         /* lo-ransac only: stop once the best model leaves a chance below 1 - confidence of having missed a
+                               better all-inlier 7-point sample, in (0, 1) */
 } dimb_gv_conf;
+/* One pair on host buffers (n,2) float32 with the estimator of `conf` (its gate fields are not read): F [9], mask [n], n_inliers as
+ * dimb_gv_fundamental; n_hypotheses (may be NULL): the hypotheses that ran (ransac8: its fixed count; 0 when n < 8).  Equal to
+ * dimb_gv_verify_dev on the same points and seed.  DIMB_ERR_ARG, before any CUDA call, for the argument errors of
+ * dimb_gv_fundamental, an unknown estimator, and with lo-ransac confidence outside (0, 1) or max_iters < 1. */
+int dimb_gv_estimate(dimb_ctx* ctx, const float* kpts0, const float* kpts1, int n, const dimb_gv_conf* conf, unsigned seed, float* F,
+                     unsigned char* mask, int* n_inliers, int* n_hypotheses);
 /* P pairs, asynchronous on `stream`, never synchronises (once its scratch has grown to the call's size).  Keypoints come from
  * f0[p] / f1[p], of which only keypoints, f16 and round_fp16 are read: feature-store slots or float32 extractor outputs.
  * d_matches [P][cap][2] int64 + d_n_matches [P] in the layout of dimb_lg_match_dev / dimb_sg_match_dev (n_raw = min(d_n_matches[p],
@@ -252,8 +265,8 @@ typedef struct {
  * d_verified [P][cap][2] int64 = the rows of d_matches whose mask is 1, in their original order; d_n_verified [P] = n_inliers, or 0
  * when the gate rejects the pair; d_F [P][9] (x1^T F x0 = 0, zeros when no model); d_mask [P][cap]; d_n_inliers [P].  Pairs with
  * fewer than 8 raw matches (or no model): mask all ones, F zeros, n_inliers = n_raw, then the gate.  DIMB_ERR_ARG, before any CUDA
- * call, for a NULL ctx / f0 / f1 / seeds / conf / buffer / keypoint pointer, P < 1, cap < 1, threshold <= 0, min_inliers < 0 or
- * min_inlier_ratio outside [0, 1]. */
+ * call, for a NULL ctx / f0 / f1 / seeds / conf / buffer / keypoint pointer, P < 1, cap < 1, threshold <= 0, min_inliers < 0,
+ * min_inlier_ratio outside [0, 1], an unknown estimator, and with lo-ransac confidence outside (0, 1) or max_iters < 1. */
 int dimb_gv_verify_dev(dimb_ctx* ctx, int P, const dimb_feats_dev* f0, const dimb_feats_dev* f1, const int64_t* d_matches,
                        const int* d_n_matches, int cap, const unsigned* seeds, const dimb_gv_conf* conf, int64_t* d_verified,
                        int* d_n_verified, float* d_F, unsigned char* d_mask, int* d_n_inliers, void* stream);
