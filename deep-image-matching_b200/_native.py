@@ -33,6 +33,7 @@ EXPORTS = [
     "dimb_resize_area_tab", "dimb_resize_area_dev", "dimb_kpts_extent_dev", "dimb_tile_preselect_dev",
     "dimb_resize_area_linear_tab", "dimb_resize_area_linear_dev", "dimb_resize_area_rgb_dev", "dimb_pyr_size", "dimb_pyr_dev", "dimb_fstore_rescale_dev",
     "dimb_tile_preselect_pairs_dev", "dimb_rot90_dev", "dimb_fstore_unrotate_dev",
+    "dimb_sift_create", "dimb_sift_destroy", "dimb_sift_extract", "dimb_sift_extract_dev", "dimb_sift_debug_read",
 ]
 
 
@@ -49,6 +50,12 @@ class SpConf(C.Structure):
 class AlikedConf(C.Structure):
     _fields_ = [("max_num_keypoints", C.c_int), ("detection_threshold", C.c_float), ("nms_radius", C.c_int),
                 ("max_height", C.c_int), ("max_width", C.c_int)]
+
+
+class SiftConf(C.Structure):
+    _fields_ = [("n_features", C.c_int), ("n_octave_layers", C.c_int), ("contrast_threshold", C.c_double),
+                ("edge_threshold", C.c_double), ("sigma", C.c_double), ("max_batch", C.c_int), ("max_height", C.c_int),
+                ("max_width", C.c_int)]
 
 
 class SgConf(C.Structure):
@@ -161,6 +168,12 @@ def load_library():
     lib.dimb_aliked_extract.argtypes = [vp, vp, ip, ip, ip, vp, vp, vp, vp, ip]
     lib.dimb_aliked_extract_dev.argtypes = [vp, vp, ip, ip, ip, vp, vp, vp, vp, ip, vp]
     lib.dimb_aliked_debug_read.argtypes = [vp, ip, vp, C.c_size_t]
+    lib.dimb_sift_create.argtypes = [vp, C.POINTER(SiftConf), C.POINTER(vp)]
+    lib.dimb_sift_destroy.argtypes = [vp]
+    lib.dimb_sift_destroy.restype = None
+    lib.dimb_sift_extract.argtypes = [vp, vp, ip, ip, vp, vp, vp, vp, vp, ip]
+    lib.dimb_sift_extract_dev.argtypes = [vp, vp, ip, ip, ip, vp, vp, vp, vp, vp, ip, vp]
+    lib.dimb_sift_debug_read.argtypes = [vp, ip, ip, ip, vp, C.c_size_t]
     lib.dimb_sp_ctx.restype = vp
     lib.dimb_fstore_create.argtypes = [vp, ip, ip, ip, C.POINTER(vp)]
     lib.dimb_fstore_destroy.argtypes = [vp]
@@ -965,6 +978,77 @@ class AlikedNet:
     def __del__(self):
         try:
             self.ctx.lib.dimb_aliked_destroy(self.h)
+        except Exception:
+            pass
+
+
+def sift_octaves(height: int, width: int) -> list:
+    """(h, w) of every octave of a SIFT pyramid, OpenCV's octave -1 (2H x 2W) first: cvRound(log2(min(2H, 2W)) - 2) + 1 octaves,
+    each later one halving (floor) both sides."""
+    n = int(np.rint(np.log(min(2 * height, 2 * width)) / np.log(2.0) - 2)) + 1
+    sizes, h, w = [], 2 * height, 2 * width
+    for o in range(n):
+        if o:
+            h, w = h // 2, w // 2
+        sizes.append((h, w))
+    return sizes
+
+
+class SiftNet:
+    """Handle on dimb_sift: cv2.SIFT_create(n_features, n_octave_layers, contrast_threshold, edge_threshold, sigma)
+    .detectAndCompute on the device, for batches of equally sized gray images."""
+
+    def __init__(self, ctx: Context, n_features=0, n_octave_layers=3, contrast_threshold=0.04, edge_threshold=10.0, sigma=1.6,
+                 max_batch=1, max_height=1024, max_width=1024):
+        self.ctx = ctx
+        self.conf = SiftConf(int(n_features), int(n_octave_layers), float(contrast_threshold), float(edge_threshold), float(sigma),
+                             int(max_batch), int(max_height), int(max_width))
+        h = C.c_void_p()
+        ctx.check(ctx.lib.dimb_sift_create(ctx.h, C.byref(self.conf), C.byref(h)), "dimb_sift_create")
+        self.h = h
+
+    def extract(self, image: np.ndarray, cap: int | None = None) -> dict:
+        """image uint8 (H,W) -> keypoints (N,2), descriptors (128,N) float32 with integral 0..255 values, size / angle / response
+        (N,) and octave (N,) int32 (cv2's packed KeyPoint.octave)."""
+        image = np.ascontiguousarray(image)
+        if image.dtype != np.uint8 or image.ndim != 2:
+            raise ValueError("SiftNet.extract takes a uint8 (H, W) image")
+        H, W = image.shape
+        cap = cap or max(self.conf.n_features, 1) + 64
+        while True:
+            kp = np.zeros((cap, 2), np.float32)
+            de = np.zeros((128, cap), np.float32)
+            fr = np.zeros((cap, 3), np.float32)
+            oc = np.zeros(cap, np.int32)
+            cnt = np.zeros(1, np.int32)
+            rc = self.ctx.lib.dimb_sift_extract(self.h, _ptr(image), H, W, _ptr(kp), _ptr(de), _ptr(fr), _ptr(oc), _ptr(cnt), cap)
+            if rc == ERR_CAPACITY and cnt[0] > cap:
+                cap = int(cnt[0])
+                continue
+            self.ctx.check(rc, "dimb_sift_extract")
+            break
+        n = int(cnt[0])
+        return {"keypoints": kp[:n].copy(), "descriptors": de[:, :n].copy(), "size": fr[:n, 0].copy(), "angle": fr[:n, 1].copy(),
+                "response": fr[:n, 2].copy(), "octave": oc[:n].copy()}
+
+    def extract_dev(self, d_images, B, H, W, d_kpts, d_desc, d_counts, cap, d_frames=0, d_octave=0, stream=0):
+        """Raw device-pointer variant (ints are device addresses, e.g. torch.Tensor.data_ptr())."""
+        self.ctx.check(self.ctx.lib.dimb_sift_extract_dev(self.h, d_images, B, H, W, d_kpts, d_desc, d_frames or None,
+                                                          d_octave or None, d_counts, cap, stream), "dimb_sift_extract_dev")
+
+    def debug_read(self, which: int, image: int, octave: int, level: int, height: int, width: int) -> np.ndarray:
+        """which 0: Gaussian level `level` of `octave`, 1: DoG level; (height, width) are the image's, the shape comes from
+        sift_octaves."""
+        h, w = sift_octaves(height, width)[octave]
+        per = self.conf.n_octave_layers + 3 - which
+        out = np.zeros((h, w), np.float32)
+        self.ctx.check(self.ctx.lib.dimb_sift_debug_read(self.h, which, image, octave * per + level, _ptr(out), out.size),
+                       "dimb_sift_debug_read")
+        return out
+
+    def __del__(self):
+        try:
+            self.ctx.lib.dimb_sift_destroy(self.h)
         except Exception:
             pass
 

@@ -18,7 +18,7 @@ confs = {
         "extractor": {"name": "superpoint", "nms_radius": 3, "keypoint_threshold": 0.0005, "max_keypoints": 2048},
         "matcher": {"name": "kornia_matcher", "match_mode": "smnn", "th": 0.99},
     },
-    "sift+kornia_matcher": {  # config.py:232-244 (the SIFT extractor itself is OpenCV on the CPU: out of scope, its matcher is not)
+    "sift+kornia_matcher": {  # config.py:232-244 (SIFTExtractor: cv2.SIFT's detectAndCompute on the device, csrc/sift.cu)
         "extractor": {"name": "sift", "n_features": 2048, "nOctaveLayers": 3, "contrastThreshold": 0.0004, "edgeThreshold": 10,
                       "sigma": 1.6},
         "matcher": {"name": "kornia_matcher", "match_mode": "smnn", "th": 0.85},

@@ -234,6 +234,23 @@ def kornia_conf(conf) -> dict:
     return out
 
 
+SIFT_TIE_ROOM = 64  # store rows above n_features for the keypoints retainBest keeps at the boundary response
+
+
+def sift_set_conf(sp_conf) -> dict:
+    """SiftNet keyword arguments of a SIFT set's ``sp_conf``: the SIFTExtractor keys (n_features, nOctaveLayers, contrastThreshold,
+    edgeThreshold, sigma; missing ones take SIFTExtractor's defaults), n_features >= 1.  Raises ValueError otherwise."""
+    from .extractors.sift import SIFT_KEYS, SIFTExtractor, sift_conf
+    unknown = set(sp_conf or {}) - set(SIFT_KEYS) - {"name"}
+    if unknown:
+        raise ValueError(f"unknown SIFT option(s) {sorted(unknown)}; expected some of {list(SIFT_KEYS)}")
+    conf = {**{k: SIFTExtractor._default_conf[k] for k in SIFT_KEYS}, **{k: v for k, v in (sp_conf or {}).items() if k != "name"}}
+    out = sift_conf(conf)
+    if out["n_features"] < 1:
+        raise ValueError(f"a SIFT image set needs n_features >= 1 (it sizes the feature store), got {out['n_features']}")
+    return out
+
+
 def lighterglue_conf(conf) -> dict:
     """The ``lg_conf`` of ImageSetMatcher(matcher="lighterglue"), validated like ``kornia_conf``: only ``filter_threshold`` (default 0.1)
     of LighterGlueMatcher's configuration reaches the network (the plugin's ``min_conf``); the network itself is ``LIGHTERGLUE_CONF``
@@ -577,6 +594,13 @@ class ImageSetMatcher:
     is that network), and since ``lg_weights`` is then an input_dim-128 LightGlue, ``preselection_weights`` / ``lowres_weights`` /
     ``upright_weights`` are required for the passes configured, whatever the matcher.
 
+    ``extractor="sift"``: the reference's sift+kornia_matcher pipeline.  Gray images (k, H, W) as for SuperPoint, extracted by
+    ``SiftNet`` (cv2.SIFT's detectAndCompute, ``batch_images`` per call); ``sp_conf`` holds the SIFTExtractor keys (``sift_set_conf``,
+    n_features >= 1), ``sp_weights`` / ``lg_weights`` are not used, D = 128 and the stored scores are ones.  The store holds
+    n_features + ``SIFT_TIE_ROOM`` rows per image, since retainBest keeps every keypoint tied with the n_features-th response;
+    ``exchange`` raises RuntimeError for an image with more (``_check_sift_counts``).  Only ``matcher="kornia_matcher"`` with quality
+    "high" is supported: other matchers, tiling (and tile preselection), pair generation, upright and other qualities raise ValueError.
+
     ``tiling``: None (default) or a dict checked by ``tiling_conf``.  With tiling, ``extract`` takes full-size images, cuts their tiles
     on the device, runs the extractor over tiles (SuperPoint ``batch_images`` tiles per call, network sized for one tile, with
     ``fix_sampling=True`` as the reference's tiling requires) and merges each image's tile features into its slot (store capacity
@@ -649,8 +673,19 @@ class ImageSetMatcher:
         from . import _native
         if matcher not in ("lightglue", "superglue", "kornia_matcher", "lighterglue"):
             raise ValueError(f'matcher must be "lightglue", "superglue", "kornia_matcher" or "lighterglue", got {matcher!r}')
-        if extractor not in ("superpoint", "aliked", None):
-            raise ValueError(f'extractor must be "superpoint", "aliked" or None (given features), got {extractor!r}')
+        if extractor not in ("superpoint", "aliked", "sift", None):
+            raise ValueError(f'extractor must be "superpoint", "aliked", "sift" or None (given features), got {extractor!r}')
+        if extractor == "sift":
+            if matcher != "kornia_matcher":
+                raise ValueError(f'matcher {matcher!r} with extractor="sift" is not supported; SIFT sets match with "kornia_matcher"')
+            for name, val, off in (("tiling (and tile preselection)", tiling, None), ("pair_generation", pair_generation, None),
+                                   ("upright", upright, None)):
+                if val != off:
+                    raise ValueError(f'{name} with extractor="sift" is not supported')
+            if quality_conf(quality) != 0:
+                raise ValueError(f'quality {quality!r} with extractor="sift" is not supported (the reference resizes uint8 images '
+                                 'there); use quality="high"')
+            sp_conf = sift_set_conf(sp_conf)
         if matcher == "lighterglue" and extractor is not None:
             raise ValueError(f"LighterGlue matches XFeat features only, which are given (extractor=None), not extracted by {extractor}")
         given = None
@@ -757,6 +792,8 @@ class ImageSetMatcher:
         self.extractor = extractor
         if given is not None:
             self.cap, self.D = given
+        elif extractor == "sift":
+            self.cap, self.D = sp_conf["n_features"] + SIFT_TIE_ROOM, 128
         else:
             self.cap = int(sp_conf["max_keypoints"]) if extractor == "superpoint" else int(sp_conf.get("max_num_keypoints", 4000))
             self.D = 256 if extractor == "superpoint" else 128
@@ -772,6 +809,8 @@ class ImageSetMatcher:
             self.sp = _native.SuperPointNet(ctx, sp_weights, max_batch=batch_images, max_height=eh, max_width=ew, **sp_conf)
         elif extractor == "aliked":
             self.al = _native.AlikedNet(ctx, sp_weights, max_height=eh, max_width=ew, **sp_conf)
+        elif extractor == "sift":
+            self.sift = _native.SiftNet(ctx, max_batch=batch_images, max_height=eh, max_width=ew, **sp_conf)
         self.matcher = matcher
         if matcher == "superglue":
             self.sg = _native.SuperGlueNet(ctx, lg_weights, max_pairs=batch_pairs, max_kpts=self.cap, **lg_conf)
@@ -787,7 +826,7 @@ class ImageSetMatcher:
         dev = torch.device("cuda", ctx.device)
         # extraction outputs of one batch (float32, library layouts) and match outputs of one pair batch; tiled: the tiles of the
         # max(1, batch_images // T) images of one cut, T the tile count of their size
-        self.C = 1 if extractor == "superpoint" else 3
+        self.C = 3 if extractor == "aliked" else 1
         n_img = {s: batch_images if self.tiling is None else max(1, batch_images // len(grids[s]["origins"])) for s in shapes}
         n_ext = batch_images
         if self.tiling is not None:
@@ -800,6 +839,8 @@ class ImageSetMatcher:
             self.sc = torch.zeros(n_ext, self.cap, device=dev)
             self.de = torch.zeros(n_ext, self.D, self.cap, device=dev)
             self.cnt = torch.zeros(n_ext, dtype=torch.int32, device=dev)
+        if extractor == "sift":  # every image's true keypoint count, checked against the store's capacity by exchange
+            self.sift_counts = torch.zeros(n_images, dtype=torch.int32, device=dev)
         self.m = torch.zeros(batch_pairs, self.cap, 2, dtype=torch.int64, device=dev)
         self.ms = torch.zeros(batch_pairs, self.cap, device=dev)
         self.nm = torch.zeros(batch_pairs, dtype=torch.int32, device=dev)
@@ -927,8 +968,11 @@ class ImageSetMatcher:
         src = self._resize(src, h2, w2, st)
         self._extract_rows(src, h2, w2, st)
         for k, s in enumerate(slots):
-            self.store.put_dev(s, self.kp[k].data_ptr(), self.sc[k].data_ptr(), self.de[k].data_ptr(), self.cap, self.cnt[k:k + 1].data_ptr(),
+            scores = None if self.extractor == "sift" else self.sc[k].data_ptr()  # SIFT has no scores: the store writes ones
+            self.store.put_dev(s, self.kp[k].data_ptr(), scores, self.de[k].data_ptr(), self.cap, self.cnt[k:k + 1].data_ptr(),
                                h2, w2, None, st)
+        if self.extractor == "sift":
+            self.sift_counts[self.torch.tensor(ids, device=self.cnt.device)] = self.cnt[:len(ids)]
         self._rescale(slots, H, W, st)
 
     def _extract_turned(self, d_images, image_ids, st):
@@ -1013,9 +1057,13 @@ class ImageSetMatcher:
 
     def _extract_rows(self, src, h, w, st):
         """The configured extractor on the len(src) h x w images or tiles of `src` into rows [0, len(src)) of kp / sc / de / cnt:
-        SuperPoint in calls of at most batch_images, ALIKED one per call."""
-        step = self.B if self.extractor == "superpoint" else 1
+        SuperPoint and SIFT in calls of at most batch_images, ALIKED one per call."""
+        step = 1 if self.extractor == "aliked" else self.B
         for r in range(0, len(src), step):
+            if self.extractor == "sift":
+                self.sift.extract_dev(src[r].data_ptr(), min(step, len(src) - r), h, w, self.kp[r].data_ptr(), self.de[r].data_ptr(),
+                                      self.cnt[r:].data_ptr(), self.cap, stream=st)
+                continue
             ptrs = (self.kp[r].data_ptr(), self.sc[r].data_ptr(), self.de[r].data_ptr(), self.cnt[r:].data_ptr(), self.cap, st)
             if self.extractor == "superpoint":
                 self.sp.extract_dev(src[r].data_ptr(), min(step, len(src) - r), h, w, *ptrs)
@@ -1047,6 +1095,8 @@ class ImageSetMatcher:
         """The collective of the path: every rank's float16 feature blocks to every rank (NCCL all_gather over NVLink).  With tiling,
         every rank then builds the per-tile views of all images from the merged slots.  With upright the low-resolution sets were
         exchanged by ``upright``."""
+        if self.extractor == "sift":
+            self._check_sift_counts()
         self.exchanged_bytes = all_gather_blocks(self.store_t, self.n, self.dist)
         if self.up is None:
             self.exchanged_bytes += self._exchange_lows((self.pre, self.lowres))
@@ -1059,6 +1109,18 @@ class ImageSetMatcher:
                     ids = images[b0:b0 + step]
                     self.store.tile_views_dev([self.slots[i] for i in ids], T, self.views, [self.view_offsets[i] for i in ids],
                                               self.vmap.data_ptr(), st)
+
+    def _check_sift_counts(self):
+        """A SIFT store holds n_features + SIFT_TIE_ROOM rows per image; retainBest's boundary ties rarely add more than a few.  An
+        image with more keypoints than that (or with more extrema than the extractor's candidate buffers hold, count -1) is an error,
+        raised here before the exchange, never a silent cut."""
+        counts = self.sift_counts.cpu().tolist()
+        bad = [(i, c) for i, c in enumerate(counts) if c < 0 or c > self.cap]
+        if bad:
+            i, c = bad[0]
+            what = ("more extrema than the SIFT candidate buffers hold" if c < 0 else
+                    f"{c} SIFT keypoints, above the store's n_features + {SIFT_TIE_ROOM} = {self.cap} rows")
+            raise RuntimeError(f"image {i}: {what}")
 
     def _exchange_lows(self, lows) -> int:
         """The low-resolution features of every image, for any pair: one all_gather per buffer of each set in `lows` (None skipped; a

@@ -536,6 +536,47 @@ int dimb_sg_match_dev(dimb_sg* sg, int P, const dimb_sg_feats_dev* f0, const dim
 /* The slot as SuperGlue device input: f16 = 1, scores from the slot's score block, size_dev = the slot header's [H,W]. */
 int dimb_fstore_sg_feats_dev(dimb_fstore* fs, int slot, dimb_sg_feats_dev* out);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * SIFT extraction.  Replaces SIFTExtractor._extract (reference extractors/sift.py): cv2.SIFT_create(nfeatures, nOctaveLayers,
+ * contrastThreshold, edgeThreshold, sigma).detectAndCompute(gray_uint8, None) of OpenCV 4.x with enable_precise_upscale = false
+ * (csrc/sift.cu lists the stages).  Results are deterministic: an image gives bitwise the same output on every run and at every
+ * position of a batch.  Output order: removeDuplicatedSorted's (x asc, y asc, size desc, angle asc, response desc, octave desc),
+ * which is cv2's own order unless retainBest cuts; when it cuts, cv2's order is an artefact of std::nth_element and this order
+ * replaces it.  retainBest keeps every keypoint whose response equals the n_features-th largest, so a count may exceed n_features.
+ * Memory: sized at create time for max_batch images of max_height x max_width, about 0.8 GB of float32 pyramid and 0.23 GB of
+ * refined-extremum and keypoint buffers per 2048 x 1536 image at 3 layers.  Profile groups sift.pyr, sift.extrema, sift.ori, sift.select,
+ * sift.desc. */
+typedef struct dimb_sift dimb_sift;
+typedef struct {
+  int n_features;             /* retainBest(n_features); 0 keeps every keypoint */
+  int n_octave_layers;        /* 3 */
+  double contrast_threshold;  /* 0.04 in OpenCV, 0.0004 in the sift+kornia_matcher pipeline */
+  double edge_threshold;      /* 10 */
+  double sigma;               /* 1.6 */
+  int max_batch;              /* workspace sizing: images per call (max_batch * n_octave_layers <= 65535) */
+  int max_height, max_width;  /* workspace sizing, at most 16384 */
+} dimb_sift_conf;
+/* DIMB_ERR_ARG, before any CUDA call, for a NULL pointer or a value outside the ranges above. */
+int dimb_sift_create(dimb_ctx* ctx, const dimb_sift_conf* conf, dimb_sift** out);
+void dimb_sift_destroy(dimb_sift* sift);
+/* One host image, uint8 [H][W].  Out (host): kpts [cap][2] (x, y), desc [128][cap] (integral 0..255 values as float; (D,N) rows of
+ * pitch cap), frames [cap][3] (size, angle, response) and octave [cap] (cv2's packed KeyPoint.octave), both optional (NULL), count.
+ * DIMB_ERR_CAPACITY (count filled) when the image has more than cap keypoints, or (count -1) more extrema than the candidate
+ * buffers hold. */
+int dimb_sift_extract(dimb_sift* sift, const uint8_t* image, int H, int W, float* kpts, float* desc, float* frames, int* octave,
+                      int* count, int cap);
+/* B device float32 images [B][H][W]; each pixel is first converted as convertTo(CV_8U) does (round half to even, saturate to 0..255),
+ * so integral 0..255 images are taken exactly.  Outputs (device) in the layouts of dimb_sp_extract_dev: d_kpts [B][cap][2],
+ * d_desc [B][128][cap], d_counts [B]; d_frames [B][cap][3] and d_octave [B][cap] may be NULL.  d_counts holds the true count (-1 when
+ * the candidate buffers overflowed); only the first cap rows are written and the caller checks the count.  Asynchronous on `stream`.
+ * DIMB_ERR_ARG, before any CUDA call, for a NULL pointer, cap < 1, B outside [1, max_batch] or a size above the workspace. */
+int dimb_sift_extract_dev(dimb_sift* sift, const float* d_images, int B, int H, int W, float* d_kpts, float* d_desc, float* d_frames,
+                          int* d_octave, int* d_counts, int cap, void* stream);
+/* Debug taps of the last call, image `image`: which 0 = Gaussian level, level = octave * (n_octave_layers + 3) + i; which 1 = DoG
+ * level, level = octave * (n_octave_layers + 2) + i.  Octave 0 is OpenCV's octave -1 (2H x 2W), each later octave halves (floor) both
+ * sides; out holds exactly that octave's h * w floats (0..255 scale). */
+int dimb_sift_debug_read(dimb_sift* sift, int which, int image, int level, float* out, size_t n_floats);
+
 #ifdef __cplusplus
 }
 #endif
