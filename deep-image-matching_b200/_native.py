@@ -219,8 +219,9 @@ _selftest = None
 
 def load_selftest_library():
     """libdimb200_selftest.so: the production GEMM template behind a C = A B^T entry, the flash-attention kernels behind an
-    attention entry, keypoint detection (simple_nms, compaction, top-k), the SuperPoint head kernels and the matching heads (LightGlue
-    assignment and tail, SuperGlue Sinkhorn) behind their own entries, and the host drive of the RANSAC arithmetic.
+    attention entry, keypoint detection (simple_nms, compaction, top-k), the SuperPoint head kernels, the matching heads (LightGlue
+    assignment and tail, SuperGlue Sinkhorn) and the SIFT stages (extrema, orientation, selection, descriptors) behind their own
+    entries, and the host drive of the RANSAC arithmetic.
     Test / tool infrastructure - the product library exports none of it.  Its context is its own (dimb_ctx_create of
     THIS library); never mix handles of the two libraries."""
     global _selftest
@@ -252,6 +253,10 @@ def load_selftest_library():
         lib.dimb_selftest_lg_tail.argtypes = [vp, ip, ip, vp, vp, fp, vp, fp] + [vp] * 6 + [ip, fp, fp, fp, ip, ip, ip, fp] + [vp] * 6
         lib.dimb_selftest_lgx_assign.argtypes = [vp, ip, ip, ip] + [vp] * 5 + [fp, ip, fp] + [vp] * 11
         lib.dimb_selftest_sg_sinkhorn.argtypes = [vp, ip, vp, vp, vp, fp, fp, vp, vp, ip, ip, fp, ip, fp] + [vp] * 9
+        lib.dimb_selftest_sift_extrema.argtypes = [vp, vp, ip, ip, ip, vp, vp, fp, fp, fp, ip, fp, vp, vp]
+        lib.dimb_selftest_sift_ori.argtypes = [vp, vp, ip, ip, ip, vp, vp, fp, vp, vp, ip, ip, fp, vp, vp]
+        lib.dimb_selftest_sift_select.argtypes = [vp, vp, vp, ip, ip, ip, ip, fp] + [vp] * 5
+        lib.dimb_selftest_sift_desc.argtypes = [vp, vp, ip, ip, ip] + [vp] * 5 + [ip, ip, fp, vp]
         lib.dimb_gv_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_uint, vp, vp]
         lib.dimb_gv_lo_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_float, C.c_uint, vp, vp, C.POINTER(ip)]
         lib.dimb_gv_seven_point_host.argtypes = [vp, vp, vp]
@@ -295,7 +300,7 @@ DET_TAIL = 1024  # elements past the valid ones in every output buffer of the de
 
 class SelfTest:
     """Context of the self-test library (tests/test_gemm_conv_kernel.py, tests/test_attention_kernel.py, tests/test_detect_kernel.py,
-    tests/test_match_heads.py)."""
+    tests/test_match_heads.py, tests/test_sift_kernels.py)."""
 
     def __init__(self, device: int = 0):
         self.lib = load_selftest_library()
@@ -467,6 +472,63 @@ class SelfTest:
         raw = {k: np.zeros(m + DET_TAIL, t) for k, (t, m) in bufs.items()}
         self.check(fn(self.h, *args, *(_ptr(raw[k]) for k in bufs)), what)
         return {k: raw[k][:m] for k, (_, m) in bufs.items()}, {k: raw[k][m:] for k, (_, m) in bufs.items()}
+
+    @staticmethod
+    def _sift_levels(levels):
+        """levels: per octave an array [n_levels][B][h][w] -> (concatenated float32 levels, B, n_oct, h [n_oct], w [n_oct])."""
+        levels = [np.ascontiguousarray(x, np.float32) for x in levels]
+        h = np.array([x.shape[2] for x in levels], np.int32)
+        w = np.array([x.shape[3] for x in levels], np.int32)
+        return np.concatenate([x.ravel() for x in levels]), levels[0].shape[1], len(levels), h, w
+
+    def sift_extrema(self, dog, L: int, contrast: float, edge: float, sigma: float, ccap: int, sentinel: float = -777.0):
+        """sift.extrema through its launch helper (dimb_selftest_sift_extrema) on DoG levels: per octave [L + 2][B][h][w].  Returns
+        (cand [B][ccap][6] int32 Cand records in atomic order, count [B], {'cand', 'count'} tails)."""
+        lv, B, n_oct, h, w = self._sift_levels(dog)
+        out, tail = self._run(self.lib.dimb_selftest_sift_extrema, "selftest_sift_extrema",
+                              {"cand": (np.int32, B * ccap * 6), "count": (np.int32, B)}, _ptr(lv), B, L, n_oct, _ptr(h), _ptr(w),
+                              float(contrast), float(edge), float(sigma), int(ccap), float(sentinel))
+        return out["cand"].reshape(B, ccap, 6), out["count"], tail
+
+    def sift_ori(self, gauss, L: int, sigma: float, cand: np.ndarray, cand_count, kcap: int, sentinel: float = -777.0):
+        """sift.ori through its launch helper (dimb_selftest_sift_ori) on Gaussian levels (per octave [L + 3][B][h][w]) and Cand records
+        cand [B][ccap][6] int32.  Returns (rec [B][6][kcap] float32, kp_count [B], {'rec', 'kp_count'} tails)."""
+        lv, B, n_oct, h, w = self._sift_levels(gauss)
+        cand = np.ascontiguousarray(cand, np.int32)
+        cc = np.ascontiguousarray(cand_count, np.int32)
+        ccap = cand.shape[1]
+        out, tail = self._run(self.lib.dimb_selftest_sift_ori, "selftest_sift_ori",
+                              {"rec": (np.float32, B * 6 * kcap), "kp_count": (np.int32, B)}, _ptr(lv), B, L, n_oct, _ptr(h), _ptr(w),
+                              float(sigma), _ptr(cand), _ptr(cc), int(ccap), int(kcap), float(sentinel))
+        return out["rec"].reshape(B, 6, kcap), out["kp_count"], tail
+
+    def sift_select(self, rec: np.ndarray, kp_count, n_features: int, cap: int, sentinel: float = -777.0):
+        """sift.select through its launch helper (dimb_selftest_sift_select) on records rec [B][6][kcap].  Returns a dict of sel
+        [B][cap] (record index of each output row), kpts [B][cap][2], frames [B][cap][3], octave [B][cap], counts [B] and
+        '<name>_tail' of each."""
+        rec = np.ascontiguousarray(rec, np.float32)
+        kc = np.ascontiguousarray(kp_count, np.int32)
+        B, _, kcap = rec.shape
+        shapes = {"sel": (np.int32, (B, cap)), "kpts": (np.float32, (B, cap, 2)), "frames": (np.float32, (B, cap, 3)),
+                  "octave": (np.int32, (B, cap)), "counts": (np.int32, (B,))}
+        out, tail = self._run(self.lib.dimb_selftest_sift_select, "selftest_sift_select",
+                              {k: (t, int(np.prod(s))) for k, (t, s) in shapes.items()}, _ptr(rec), _ptr(kc), B, kcap, int(n_features),
+                              int(cap), float(sentinel))
+        res = {k: out[k].reshape(s) for k, (_, s) in shapes.items()}
+        res.update({k + "_tail": v for k, v in tail.items()})
+        return res
+
+    def sift_desc(self, gauss, L: int, rows: np.ndarray, octave: np.ndarray, counts, cap: int, sentinel: float = -777.0):
+        """sift.desc through its launch helper (dimb_selftest_sift_desc) on Gaussian levels (per octave [L + 3][B][h][w]) at output rows
+        rows [B][n][4] (x, y, size, angle), octave [B][n] (output packing), counts [B].  Returns (desc [B][128][cap], tail)."""
+        lv, B, n_oct, h, w = self._sift_levels(gauss)
+        rows = np.ascontiguousarray(rows, np.float32)
+        octave = np.ascontiguousarray(octave, np.int32)
+        cnt = np.ascontiguousarray(counts, np.int32)
+        n = rows.shape[1]
+        out, tail = self._run(self.lib.dimb_selftest_sift_desc, "selftest_sift_desc", {"desc": (np.float32, B * 128 * cap)}, _ptr(lv), B,
+                              L, n_oct, _ptr(h), _ptr(w), _ptr(rows), _ptr(octave), _ptr(cnt), int(n), int(cap), float(sentinel))
+        return out["desc"].reshape(B, 128, cap), tail["desc"]
 
     def lg_assign(self, sim: np.ndarray, nf, n_orig, layer, indf: np.ndarray, z: np.ndarray, th: float, cap: int,
                   sentinel: float = -777.0) -> dict:

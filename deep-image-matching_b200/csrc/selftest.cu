@@ -9,6 +9,8 @@
 //   dimb_selftest_lg_assign / dimb_selftest_lg_tail: the LightGlue assignment and per-layer tail (lg_assign.cuh) through their launch
 //     helpers; dimb_selftest_lgx_assign: the shape-generic LightGlue assignment and filter (lgx_assign.cuh) through its launch helper;
 //     dimb_selftest_sg_sinkhorn: SuperGlue's Sinkhorn and mutual-max matching (sg_assign.cuh);
+//   dimb_selftest_sift_extrema / _ori / _select / _desc: the SIFT extremum refinement, orientation, selection and descriptor kernels
+//     (sift_kernels.cuh) through their launch helpers, on caller-given levels, candidates and records;
 //   dimb_gv_host / dimb_gv_lo_host / dimb_gv_seven_point_host: the RANSAC arithmetic of gv.cu on the host (ransac8, lo-ransac, the
 //     7-point solver).
 #include <algorithm>
@@ -1121,4 +1123,223 @@ extern "C" int dimb_selftest_sg_sinkhorn(dimb_ctx* ctx, int P, const int* m, con
   DIMB_TRY(download(ctx, reinterpret_cast<long long*>(matches), d_m, 2 * nt + kDetTail));
   DIMB_TRY(download(ctx, mscores, d_ms, nt + kDetTail));
   return download(ctx, n_matches, d_nm, P + kDetTail);
+}
+
+#include "sift_kernels.cuh"
+
+namespace {
+// Geo of B images, L layers and n_oct octaves of h[o] x w[o], laid out as sift.cu's make_layout does ([levels][B][h][w] per octave:
+// L + 3 Gaussian levels, then L + 2 DoG levels); false on sizes production cannot hold.  sigma <= 16: the first blur of a larger
+// sigma needs more than the 127 taps sift_run takes, and the orientation kernel's sample disc grows with it.
+bool sift_geo(int B, int L, int n_oct, const int* h, const int* w, float contrast, float edge, float sigma, Geo& g, size_t& total) {
+  if (!h || !w || B < 1 || L < 1 || L > 32 || B * L > 65535 || n_oct < 1 || n_oct > 16) return false;
+  if (!(contrast >= 0.f) || !(edge > 0.f) || !(sigma > 0.f && sigma <= 16.f) || !std::isfinite(edge)) return false;
+  g.B = B, g.L = L, g.n_oct = n_oct, g.contrast = contrast, g.edge = edge, g.sigma = sigma;
+  total = 0;
+  for (int o = 0; o < n_oct; ++o) {
+    if (h[o] < 1 || w[o] < 1 || h[o] > 32768 || w[o] > 32768) return false;
+    g.h[o] = h[o], g.w[o] = w[o];
+    const size_t plane = static_cast<size_t>(h[o]) * w[o] * B;
+    g.gauss[o] = total;
+    total += plane * (L + 3);
+    g.dog[o] = total;
+    total += plane * (L + 2);
+  }
+  return total <= (size_t{1} << 31);
+}
+
+// the production pyramid buffer with one kind of level (is_dog) copied from the caller's concatenated octaves and NaN elsewhere
+int sift_stage(DevTmp& t, const Geo& g, size_t total, const float* levels, bool is_dog, float** d_pyr) {
+  std::vector<float> pyr(total, std::nanf(""));
+  size_t src = 0;
+  for (int o = 0; o < g.n_oct; ++o) {
+    const size_t n = static_cast<size_t>(g.h[o]) * g.w[o] * g.B * (g.L + (is_dog ? 2 : 3));
+    std::copy(levels + src, levels + src + n, pyr.begin() + (is_dog ? g.dog[o] : g.gauss[o]));
+    src += n;
+  }
+  return t.upload(d_pyr, pyr);
+}
+
+// int buffer of n elements starting as 0 (atomic counters) or `fill`, and kDetTail more holding `tail`
+std::vector<int> sift_ibuf(size_t n, int fill, int tail) {
+  std::vector<int> v(n + kDetTail, tail);
+  std::fill(v.begin(), v.begin() + n, fill);
+  return v;
+}
+}  // namespace
+
+// SIFT (sift_kernels.cuh) stage by stage, through the launch helpers sift_run calls, on caller-given levels in the production layout.
+// Levels: for each octave o < n_oct in turn, [levels][B][h[o]][w[o]] (L + 2 DoG levels or L + 3 Gaussian levels); the other kind of
+// level holds NaN.  Outputs start as `sentinel` (int buffers: its bit pattern; counters: 0) and hold kDetTail more elements.
+// Candidates are Cand records as 6 ints: octave << 8 | layer, row << 16 | column, then the float bits of xc, xr, xi, contr.
+
+// sift.extrema at findScaleSpaceExtrema's threshold for contrast and L: cand [B][ccap][6] (image b's first min(count[b], ccap) valid,
+// in atomic order), count [B] (every survivor, stored or not).
+extern "C" int dimb_selftest_sift_extrema(dimb_ctx* ctx, const float* dog, int B, int L, int n_oct, const int* h, const int* w, float contrast,
+                                          float edge, float sigma, int ccap, float sentinel, int* cand, int* count) {
+  Geo g{};
+  size_t total;
+  if (!ctx || !dog || !cand || !count || ccap < 1 || !sift_geo(B, L, n_oct, h, w, contrast, edge, sigma, g, total)) return DIMB_ERR_ARG;
+  if (static_cast<size_t>(B) * ccap * 6 > INT_MAX) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const int isent = sentinel_bits(sentinel);
+  const size_t nc = static_cast<size_t>(B) * ccap * 6;
+  DevTmp t{ctx, {}};
+  float* d_pyr;
+  int *d_cand, *d_count;
+  DIMB_TRY(sift_stage(t, g, total, dog, true, &d_pyr));
+  DIMB_TRY(t.upload(&d_cand, sift_ibuf(nc, isent, isent)));
+  DIMB_TRY(t.upload(&d_count, sift_ibuf(B, 0, isent)));
+  DIMB_TRY(launch_sift_extrema(ctx, 0, d_pyr, g, sift_extrema_thr(contrast, L), reinterpret_cast<Cand*>(d_cand), d_count, ccap));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_sift_extrema"));
+  DIMB_TRY(download(ctx, cand, d_cand, nc + kDetTail));
+  return download(ctx, count, d_count, B + kDetTail);
+}
+
+// sift.ori on Gaussian levels and caller-given candidates cand [B][ccap][6] (image b's first min(cand_count[b], ccap) are read: octave
+// < n_oct, layer 1..L, row < h, column < w, offsets within 1): records rec [B][6][kcap] (x, y, size, angle, response, then the packed
+// octave's bits; image b's first min(kp_count[b], kcap) valid, in atomic order), kp_count [B] (every keypoint, stored or not).
+extern "C" int dimb_selftest_sift_ori(dimb_ctx* ctx, const float* gauss, int B, int L, int n_oct, const int* h, const int* w, float sigma,
+                                      const int* cand, const int* cand_count, int ccap, int kcap, float sentinel, float* rec, int* kp_count) {
+  Geo g{};
+  size_t total;
+  if (!ctx || !gauss || !cand || !cand_count || !rec || !kp_count || ccap < 1 || kcap < 1) return DIMB_ERR_ARG;
+  if (!sift_geo(B, L, n_oct, h, w, 0.f, 1.f, sigma, g, total) || static_cast<size_t>(B) * std::max(ccap, kcap) * 6 > INT_MAX) return DIMB_ERR_ARG;
+  for (int b = 0; b < B; ++b)
+    if (cand_count[b] < 0) return DIMB_ERR_ARG;
+  std::vector<Cand> cv(static_cast<size_t>(B) * ccap);
+  memcpy(cv.data(), cand, cv.size() * sizeof(Cand));
+  for (int b = 0; b < B; ++b) {
+    for (int i = 0; i < std::min(cand_count[b], ccap); ++i) {
+      const Cand& c = cv[static_cast<size_t>(b) * ccap + i];
+      const int o = c.ol >> 8, layer = c.ol & 255, r = c.rc >> 16, col = c.rc & 0xffff;
+      if (o >= n_oct || layer < 1 || layer > L || r >= h[o] || col >= w[o]) return DIMB_ERR_ARG;
+      if (!(std::fabs(c.xc) <= 1.f && std::fabs(c.xr) <= 1.f && std::fabs(c.xi) <= 1.f && std::isfinite(c.contr))) return DIMB_ERR_ARG;
+    }
+  }
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const size_t nr = static_cast<size_t>(B) * kNumFields * kcap;
+  DevTmp t{ctx, {}};
+  float *d_pyr, *d_rec;
+  Cand* d_cand;
+  int *d_cc, *d_kc;
+  DIMB_TRY(sift_stage(t, g, total, gauss, false, &d_pyr));
+  DIMB_TRY(t.upload(&d_cand, cv));
+  DIMB_TRY(t.upload(&d_cc, std::vector<int>(cand_count, cand_count + B)));
+  DIMB_TRY(t.upload(&d_rec, std::vector<float>(nr + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_kc, sift_ibuf(B, 0, sentinel_bits(sentinel))));
+  DIMB_TRY(launch_sift_ori(ctx, 0, d_pyr, g, d_cand, d_cc, ccap, d_rec, d_kc, kcap));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_sift_ori"));
+  DIMB_TRY(download(ctx, rec, d_rec, nr + kDetTail));
+  return download(ctx, kp_count, d_kc, B + kDetTail);
+}
+
+// sift.select on caller-given records rec [B][6][kcap] (sift_ori's layout; x, y, size, angle and response >= 0 in image b's first
+// min(kp_count[b], kcap)); kp_count [B] >= 0, above kcap: the overflow path (count -1).  n_features 0 keeps all.  Outputs: sel_out
+// [B][cap] (the record index of each output row), kpts [B][cap][2], frames [B][cap][3] (size, angle, response), octave [B][cap], counts
+// [B].  The sort and selection scratch starts dirty (0xff bytes), as production leaves it between calls.
+extern "C" int dimb_selftest_sift_select(dimb_ctx* ctx, const float* rec, const int* kp_count, int B, int kcap, int n_features, int cap,
+                                         float sentinel, int* sel_out, float* kpts, float* frames, int* octave, int* counts) {
+  if (!ctx || !rec || !kp_count || !sel_out || !kpts || !frames || !octave || !counts) return DIMB_ERR_ARG;
+  if (B < 1 || B > 65535 || kcap < 1 || n_features < 0 || cap < 1 || static_cast<size_t>(B) * kNumFields * std::max(kcap, cap) > INT_MAX)
+    return DIMB_ERR_ARG;
+  for (int b = 0; b < B; ++b) {
+    if (kp_count[b] < 0) return DIMB_ERR_ARG;
+    for (int f = kFx; f <= kFresp; ++f)
+      for (int i = 0; i < std::min(kp_count[b], kcap); ++i) {
+        const float v = rec[(static_cast<size_t>(b) * kNumFields + f) * kcap + i];
+        if (!(v >= 0.f) || std::signbit(v)) return DIMB_ERR_ARG;
+      }
+  }
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const int isent = sentinel_bits(sentinel);
+  const size_t nr = static_cast<size_t>(B) * kNumFields * kcap, nk = static_cast<size_t>(B) * kcap, no = static_cast<size_t>(B) * cap;
+  const size_t nch = ceil_div(kcap, kChunk), nblk = ceil_div(kcap, kSortTile);
+  DevTmp t{ctx, {}};
+  float *d_rec, *d_kpts, *d_frames;
+  int *d_cc, *d_kc, *d_selo, *d_oct, *d_counts;
+  SiftSelectBufs s;
+  DIMB_TRY(t.upload(&d_rec, std::vector<float>(rec, rec + nr)));
+  DIMB_TRY(t.upload(&d_cc, std::vector<int>(B, 0)));
+  DIMB_TRY(t.upload(&d_kc, std::vector<int>(kp_count, kp_count + B)));
+  DIMB_TRY(t.upload(&d_selo, sift_ibuf(no, isent, isent)));
+  DIMB_TRY(t.upload(&d_kpts, std::vector<float>(no * 2 + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_frames, std::vector<float>(no * 3 + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&d_oct, sift_ibuf(no, isent, isent)));
+  DIMB_TRY(t.upload(&d_counts, sift_ibuf(B, isent, isent)));
+  DIMB_TRY(t.get(&s.n_sorted, B));
+  DIMB_TRY(t.get(&s.n_dedup, B));
+  DIMB_TRY(t.get(&s.ovf, B));
+  DIMB_TRY(t.get(&s.dummy, B));
+  DIMB_TRY(t.get(&s.sel, nk));
+  DIMB_TRY(t.get(&s.chunk, B * nch));
+  DIMB_TRY(t.get(&s.digit_off, B * nblk * 256));
+  DIMB_TRY(t.get(&s.resp, nk));
+  DIMB_TRY(t.get(&s.state, static_cast<size_t>(B) * kTkState));
+  DIMB_TRY(t.get(&s.hist, static_cast<size_t>(B) * 256));
+  DIMB_TRY(t.get(&s.keys0, nk));
+  DIMB_TRY(t.get(&s.keys1, nk));
+  s.sel_out = d_selo;
+  DIMB_CUDA_OK(ctx, cudaMemset(s.sel, 0xff, nk * sizeof(int)));
+  DIMB_CUDA_OK(ctx, cudaMemset(s.resp, 0xff, nk * sizeof(float)));
+  DIMB_CUDA_OK(ctx, cudaMemset(s.chunk, 0xff, B * nch * sizeof(int)));
+  DIMB_CUDA_OK(ctx, cudaMemset(s.digit_off, 0xff, B * nblk * 256 * sizeof(int)));
+  DIMB_CUDA_OK(ctx, cudaMemset(s.state, 0xff, static_cast<size_t>(B) * kTkState * sizeof(unsigned)));
+  DIMB_CUDA_OK(ctx, cudaMemset(s.hist, 0xff, static_cast<size_t>(B) * 256 * sizeof(unsigned)));
+  DIMB_CUDA_OK(ctx, cudaMemset(s.keys0, 0xff, nk * sizeof(unsigned long long)));
+  DIMB_CUDA_OK(ctx, cudaMemset(s.keys1, 0xff, nk * sizeof(unsigned long long)));
+  const SiftOut out{d_kpts, nullptr, d_frames, d_oct, d_counts, cap};
+  DIMB_TRY(launch_sift_select(ctx, 0, B, d_rec, d_cc, d_kc, kcap, kcap, n_features, s, out));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_sift_select"));
+  DIMB_TRY(download(ctx, sel_out, d_selo, no + kDetTail));
+  DIMB_TRY(download(ctx, kpts, d_kpts, no * 2 + kDetTail));
+  DIMB_TRY(download(ctx, frames, d_frames, no * 3 + kDetTail));
+  DIMB_TRY(download(ctx, octave, d_oct, no + kDetTail));
+  return download(ctx, counts, d_counts, B + kDetTail);
+}
+
+// sift.desc on Gaussian levels at caller-given output rows (sift_select's outputs): rows [B][n][4] (x, y, size, angle: finite, |x|,
+// |y| <= 1e6, 0 < size <= 1e4, 0 <= angle <= 360), octave [B][n] (output packing: octave - 1 in the low byte, a level 0..L + 2 of an
+// octave < n_oct), counts [B] (0..n).  The rows go back into records as sift.select read them; desc [B][128][cap] holds image b's
+// first min(counts[b], cap) rows.
+extern "C" int dimb_selftest_sift_desc(dimb_ctx* ctx, const float* gauss, int B, int L, int n_oct, const int* h, const int* w,
+                                       const float* rows, const int* octave, const int* counts, int n, int cap, float sentinel, float* desc) {
+  Geo g{};
+  size_t total;
+  if (!ctx || !gauss || !rows || !octave || !counts || !desc || n < 1 || cap < 1) return DIMB_ERR_ARG;
+  if (!sift_geo(B, L, n_oct, h, w, 0.f, 1.f, 1.f, g, total) || static_cast<size_t>(B) * std::max(n * kNumFields, cap * 128) > INT_MAX)
+    return DIMB_ERR_ARG;
+  std::vector<float> rec(static_cast<size_t>(B) * kNumFields * n, 0.f);
+  std::vector<int> sel(static_cast<size_t>(B) * cap, 0);
+  for (int b = 0; b < B; ++b) {
+    if (counts[b] < 0 || counts[b] > n) return DIMB_ERR_ARG;
+    for (int i = 0; i < counts[b]; ++i) {
+      const float* r = rows + (static_cast<size_t>(b) * n + i) * 4;
+      const int oc = octave[static_cast<size_t>(b) * n + i], o = ((oc & 255) + 1) & 255, layer = (oc >> 8) & 255;
+      if (!(std::fabs(r[0]) <= 1e6f && std::fabs(r[1]) <= 1e6f && r[2] > 0.f && r[2] <= 1e4f && r[3] >= 0.f && r[3] <= 360.f)) return DIMB_ERR_ARG;
+      if (o >= n_oct || layer > L + 2) return DIMB_ERR_ARG;
+      float* rb = rec.data() + static_cast<size_t>(b) * kNumFields * n;
+      rb[kFx * static_cast<size_t>(n) + i] = r[0] * 2.f;
+      rb[kFy * static_cast<size_t>(n) + i] = r[1] * 2.f;
+      rb[kFsize * static_cast<size_t>(n) + i] = r[2] * 2.f;
+      rb[kFangle * static_cast<size_t>(n) + i] = r[3];
+      const int packed = (oc & ~255) | o;
+      memcpy(&rb[kFoct * static_cast<size_t>(n) + i], &packed, sizeof packed);
+      if (i < cap) sel[static_cast<size_t>(b) * cap + i] = i;
+    }
+  }
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const size_t nd = static_cast<size_t>(B) * 128 * cap;
+  DevTmp t{ctx, {}};
+  float *d_pyr, *d_rec, *d_desc;
+  int *d_sel, *d_counts;
+  DIMB_TRY(sift_stage(t, g, total, gauss, false, &d_pyr));
+  DIMB_TRY(t.upload(&d_rec, rec));
+  DIMB_TRY(t.upload(&d_sel, sel));
+  DIMB_TRY(t.upload(&d_counts, std::vector<int>(counts, counts + B)));
+  DIMB_TRY(t.upload(&d_desc, std::vector<float>(nd + kDetTail, sentinel)));
+  const SiftOut out{nullptr, d_desc, nullptr, nullptr, d_counts, cap};
+  DIMB_TRY(launch_sift_desc(ctx, 0, d_pyr, g, d_rec, d_sel, n, out));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_sift_desc"));
+  return download(ctx, desc, d_desc, nd + kDetTail);
 }
