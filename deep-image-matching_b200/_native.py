@@ -233,8 +233,8 @@ _selftest = None
 def load_selftest_library():
     """libdimb200_selftest.so: the production GEMM template behind a C = A B^T entry, the flash-attention kernels behind an
     attention entry, keypoint detection (simple_nms, compaction, top-k), the SuperPoint head kernels, the matching heads (LightGlue
-    assignment and tail, SuperGlue Sinkhorn) and the SIFT stages (extrema, orientation, selection, descriptors) behind their own
-    entries, and the host drive of the RANSAC arithmetic.
+    assignment and tail, SuperGlue Sinkhorn), the SIFT stages (extrema, orientation, selection, descriptors) and the ALIKED stages
+    (convolutions, fusion, DKD, SDDH) behind their own entries, and the host drive of the RANSAC arithmetic.
     Test / tool infrastructure - the product library exports none of it.  Its context is its own (dimb_ctx_create of
     THIS library); never mix handles of the two libraries."""
     global _selftest
@@ -270,6 +270,17 @@ def load_selftest_library():
         lib.dimb_selftest_sift_ori.argtypes = [vp, vp, ip, ip, ip, vp, vp, fp, vp, vp, ip, ip, fp, vp, vp]
         lib.dimb_selftest_sift_select.argtypes = [vp, vp, vp, ip, ip, ip, ip, fp] + [vp] * 5
         lib.dimb_selftest_sift_desc.argtypes = [vp, vp, ip, ip, ip] + [vp] * 5 + [ip, ip, fp, vp]
+        lib.dimb_selftest_aliked_conv_plan.argtypes = [ip, ip, ip, vp]
+        lib.dimb_selftest_aliked_conv3x3.argtypes = [vp, ip, vp, ip, ip, ip, vp, vp, vp, vp, ip, ip, fp, vp, vp]
+        lib.dimb_selftest_aliked_conv1x1.argtypes = [vp, vp, ip, ip, vp, vp, ip, ip, fp, vp]
+        lib.dimb_selftest_aliked_avgpool.argtypes = [vp, vp, ip, ip, ip, ip, fp, vp]
+        lib.dimb_selftest_aliked_pad.argtypes = [vp, vp, ip, ip, ip, fp, vp, vp]
+        lib.dimb_selftest_aliked_crop.argtypes = [vp, vp] + [ip] * 6 + [fp, vp]
+        lib.dimb_selftest_aliked_deform.argtypes = [vp, vp, ip, ip, ip, vp, fp, vp, vp, vp, vp, vp, ip, ip, fp, vp, vp]
+        lib.dimb_selftest_aliked_fuse.argtypes = [vp] * 7 + [ip] * 6 + [fp, vp, vp]
+        lib.dimb_selftest_aliked_dkd.argtypes = [vp, vp, ip, ip, ip, vp, ip, ip, fp, vp, vp, vp]
+        lib.dimb_selftest_aliked_sddh.argtypes = [vp, vp, ip, ip, vp, ip, ip] + [vp] * 7 + [fp, vp, vp, vp]
+        lib.dimb_selftest_aliked_threshold.argtypes = [vp, vp, ip, vp, fp, fp, vp]
         lib.dimb_gv_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_uint, vp, vp]
         lib.dimb_gv_lo_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_float, C.c_uint, vp, vp, C.POINTER(ip)]
         lib.dimb_gv_seven_point_host.argtypes = [vp, vp, vp]
@@ -298,6 +309,16 @@ def conv_mode(cout: int, B: int, H: int, W: int, num_sms: int) -> int:
     return int(out[0])
 
 
+def aliked_conv_plan(H: int, W: int, cout: int) -> int:
+    """The al_conv3x3_kernel instantiation ALIKED's conv3 runs on an H x W map with cout output channels: 1 = <8,1>, 2 = <16,4>, 3 =
+    <8,4> (dimb_selftest_aliked_conv_plan).  Host only."""
+    out = np.zeros(1, np.int32)
+    rc = load_selftest_library().dimb_selftest_aliked_conv_plan(int(H), int(W), int(cout), _ptr(out))
+    if rc != OK:
+        raise DimbError(f"aliked_conv_plan({H}, {W}, {cout}) failed (code {rc})")
+    return int(out[0])
+
+
 def nms_plan(r: int, cut: int = 0):
     """Launch plan (kernel, tile, threads, smem_bytes) of simple_nms at radius r (dimb_selftest_nms_plan): kernel 1 = first cut, 2 =
     bit-mask kernel.  cut 0 = the production choice, 1 = first cut (radii 0..8), 2 = bit-mask kernel (radii 1..5).  Host only."""
@@ -313,7 +334,7 @@ DET_TAIL = 1024  # elements past the valid ones in every output buffer of the de
 
 class SelfTest:
     """Context of the self-test library (tests/test_gemm_conv_kernel.py, tests/test_attention_kernel.py, tests/test_detect_kernel.py,
-    tests/test_match_heads.py, tests/test_sift_kernels.py)."""
+    tests/test_match_heads.py, tests/test_sift_kernels.py, tests/test_aliked_kernels.py)."""
 
     def __init__(self, device: int = 0):
         self.lib = load_selftest_library()
@@ -542,6 +563,123 @@ class SelfTest:
         out, tail = self._run(self.lib.dimb_selftest_sift_desc, "selftest_sift_desc", {"desc": (np.float32, B * 128 * cap)}, _ptr(lv), B,
                               L, n_oct, _ptr(h), _ptr(w), _ptr(rows), _ptr(octave), _ptr(cnt), int(n), int(cap), float(sentinel))
         return out["desc"].reshape(B, 128, cap), tail["desc"]
+
+    @staticmethod
+    def _f32(a):
+        return None if a is None else np.ascontiguousarray(a, np.float32)
+
+    def aliked_conv3x3(self, x, w, alpha=None, beta=None, resid=None, act=0, variant=0, sentinel: float = -777.0):
+        """ALIKED's conv3 through its launch helper (dimb_selftest_aliked_conv3x3): x [cin][H][W], w [cout][cin][3][3], alpha / beta
+        [cout], resid [cout][H][W].  variant 0 = the production rule, 1 / 2 / 3 = <8,1> / <16,4> / <8,4>.  Returns (out [cout][H][W],
+        tail, the instantiation that ran)."""
+        x, w, alpha, beta, resid = (self._f32(a) for a in (x, w, alpha, beta, resid))
+        cin, H, W = x.shape
+        cout = w.shape[0]
+        plan = np.zeros(1, np.int32)
+        out, tail = self._run(lambda h, *p: self.lib.dimb_selftest_aliked_conv3x3(h, int(variant), _ptr(x), cin, H, W, _ptr(w), *p, _ptr(plan)),
+                              "selftest_aliked_conv3x3", {"out": (np.float32, cout * H * W)},
+                              *(None if a is None else _ptr(a) for a in (alpha, beta, resid)), cout, int(act), float(sentinel))
+        return out["out"].reshape(cout, H, W), tail["out"], int(plan[0])
+
+    def aliked_conv1x1(self, x, w, bias=None, act=0, sentinel: float = -777.0):
+        """ALIKED's conv1 (dimb_selftest_aliked_conv1x1): x [cin][P], w [cout][cin], bias [cout] -> (out [cout][P], tail)."""
+        x, w, bias = self._f32(x), self._f32(w), self._f32(bias)
+        cin, P = x.shape
+        cout = w.shape[0]
+        out, tail = self._run(self.lib.dimb_selftest_aliked_conv1x1, "selftest_aliked_conv1x1", {"out": (np.float32, cout * P)}, _ptr(x), cin,
+                              P, _ptr(w), None if bias is None else _ptr(bias), cout, int(act), float(sentinel))
+        return out["out"].reshape(cout, P), tail["out"]
+
+    def aliked_avgpool(self, x, k: int, sentinel: float = -777.0):
+        """al_avgpool_kernel (dimb_selftest_aliked_avgpool): x [C][H][W] -> (out [C][H // k][W // k], tail)."""
+        x = self._f32(x)
+        C_, H, W = x.shape
+        n = C_ * (H // k) * (W // k)
+        out, tail = self._run(self.lib.dimb_selftest_aliked_avgpool, "selftest_aliked_avgpool", {"out": (np.float32, n)}, _ptr(x), C_, H, W,
+                              int(k), float(sentinel))
+        return out["out"].reshape(C_, H // k, W // k), tail["out"]
+
+    def aliked_pad(self, img, sentinel: float = -777.0):
+        """InputPadder + al_pad_kernel (dimb_selftest_aliked_pad): img [H][W] or [H][W][3] 0..255 -> (out [3][Hp][Wp], (Hp, Wp, top,
+        left), the rest of the buffer)."""
+        img = self._f32(img)
+        H, W = img.shape[:2]
+        ch = 1 if img.ndim == 2 else img.shape[2]
+        n = 3 * (H + 31) * (W + 31)
+        raw = np.zeros(n + DET_TAIL, np.float32)
+        geo = np.zeros(4, np.int32)
+        self.check(self.lib.dimb_selftest_aliked_pad(self.h, _ptr(img), H, W, ch, float(sentinel), _ptr(raw), _ptr(geo)), "selftest_aliked_pad")
+        Hp, Wp, top, left = (int(v) for v in geo)
+        return raw[:3 * Hp * Wp].reshape(3, Hp, Wp), (Hp, Wp, top, left), raw[3 * Hp * Wp:]
+
+    def aliked_crop(self, x, top: int, left: int, H: int, W: int, sentinel: float = -777.0):
+        """al_crop_kernel (dimb_selftest_aliked_crop): x [Hp][Wp] -> (out [H][W], tail)."""
+        x = self._f32(x)
+        Hp, Wp = x.shape
+        out, tail = self._run(self.lib.dimb_selftest_aliked_crop, "selftest_aliked_crop", {"out": (np.float32, H * W)}, _ptr(x), Hp, Wp,
+                              int(top), int(left), int(H), int(W), float(sentinel))
+        return out["out"].reshape(H, W), tail["out"]
+
+    def aliked_deform(self, x, w, bn, offs=None, max_off: float = 0.0, offw=None, offb=None, resid=None, act=1, sentinel: float = -777.0):
+        """ALIKED's deformable conv (dimb_selftest_aliked_deform): x [cin][H][W], w [cout][cin][3][3], bn [4][cout] (gamma, beta, mean,
+        var).  Mode A: offs [18][H][W] clamped to +-max_off.  Mode B (offs None): offset_conv offw [18][cin][3][3], offb [18].  Returns
+        (out [cout][H][W], tail, offsets [18][H][W] of mode B or None)."""
+        x, w, bn, offs, offw, offb, resid = (self._f32(a) for a in (x, w, bn, offs, offw, offb, resid))
+        cin, H, W = x.shape
+        cout = w.shape[0]
+        bufs = {"out": (np.float32, cout * H * W), "off": (np.float32, 18 * H * W)}
+        p = lambda a: None if a is None else _ptr(a)
+        out, tail = self._run(self.lib.dimb_selftest_aliked_deform, "selftest_aliked_deform", bufs, _ptr(x), cin, H, W, p(offs),
+                              float(max_off), p(offw), p(offb), _ptr(w), _ptr(bn), p(resid), cout, int(act), float(sentinel))
+        return out["out"].reshape(cout, H, W), tail["out"], None if offs is not None else out["off"].reshape(18, H, W)
+
+    def aliked_fuse(self, x1, l2o, l3o, l4o, l1, s0, top: int, left: int, H: int, W: int, sentinel: float = -777.0):
+        """al_fuse_kernel (dimb_selftest_aliked_fuse): x1 [16][Hp][Wp], lateral outputs l2o / l3o / l4o [32][Hp/f][Wp/f] (f = 2, 8, 32),
+        conv1.weight l1 [32][16], score_head.0.weight s0 [8][128].  Returns (sh0 [8][Hp][Wp], feat [H][W][128], {'sh0', 'feat'} tails)."""
+        x1, l2o, l3o, l4o, l1, s0 = (self._f32(a) for a in (x1, l2o, l3o, l4o, l1, s0))
+        Hp, Wp = x1.shape[1:]
+        out, tail = self._run(self.lib.dimb_selftest_aliked_fuse, "selftest_aliked_fuse",
+                              {"sh0": (np.float32, 8 * Hp * Wp), "feat": (np.float32, H * W * 128)}, _ptr(x1), _ptr(l2o), _ptr(l3o),
+                              _ptr(l4o), _ptr(l1), _ptr(s0), Hp, Wp, int(top), int(left), int(H), int(W), float(sentinel))
+        return out["sh0"].reshape(8, Hp, Wp), out["feat"].reshape(H, W, 128), tail
+
+    def aliked_dkd(self, score, r: int, sel_idx, count: int, cap: int, sentinel: float = -777.0):
+        """al_dkd_refine_kernel (dimb_selftest_aliked_dkd) on score [H][W] at pixels sel_idx.  Returns ({'kxy' [cap][2], 'disp' [cap],
+        'kscore' [cap]}, tails)."""
+        score = self._f32(score)
+        H, W = score.shape
+        idx = np.ascontiguousarray(np.asarray(sel_idx, np.int64).astype(np.int32).reshape(-1))
+        idx = idx if idx.size else np.zeros(1, np.int32)
+        out, tail = self._run(self.lib.dimb_selftest_aliked_dkd, "selftest_aliked_dkd",
+                              {"kxy": (np.float32, 2 * cap), "disp": (np.float32, cap), "kscore": (np.float32, cap)}, _ptr(score), H, W,
+                              int(r), _ptr(idx), int(count), int(cap), float(sentinel))
+        out["kxy"] = out["kxy"].reshape(cap, 2)
+        return out, tail
+
+    def aliked_sddh(self, feat, kxy, count: int, cap: int, w: dict, off=None, sentinel: float = -777.0):
+        """SDDH (dimb_selftest_aliked_sddh) in the context's precision: feat [H][W][128], kxy [n][2] normalised, w the state_dict
+        (desc_head.*), off [n][32] replacing the offsets stage's for the samples.  Returns ({'kpts' [cap][2], 'off' [cap][32], 'desc'
+        [128][cap]}, tails)."""
+        feat = self._f32(feat)
+        H, W = feat.shape[:2]
+        kxy = self._f32(np.asarray(kxy).reshape(-1, 2) if len(kxy) else np.zeros((1, 2)))
+        off = self._f32(off)
+        ws = [self._f32(w["desc_head." + k]) for k in ("offset_conv.0.weight", "offset_conv.0.bias", "offset_conv.2.weight",
+                                                     "offset_conv.2.bias", "sf_conv.weight", "agg_weights")]
+        out, tail = self._run(self.lib.dimb_selftest_aliked_sddh, "selftest_aliked_sddh",
+                              {"kpts": (np.float32, 2 * cap), "off": (np.float32, 32 * cap), "desc": (np.float32, 128 * cap)}, _ptr(feat),
+                              H, W, _ptr(kxy), int(count), int(cap), *(_ptr(a) for a in ws), None if off is None else _ptr(off),
+                              float(sentinel))
+        out["kpts"], out["off"], out["desc"] = out["kpts"].reshape(cap, 2), out["off"].reshape(cap, 32), out["desc"].reshape(128, cap)
+        return out, tail
+
+    def aliked_threshold(self, score, cand_count=None, thr: float = 0.0, sentinel: float = -777.0):
+        """al_threshold_kernel (dimb_selftest_aliked_threshold): score [HW]; cand_count None = mean mode.  Returns (thr, tail)."""
+        score = self._f32(np.asarray(score).reshape(-1))
+        cc = None if cand_count is None else np.array([cand_count], np.int32)
+        out, tail = self._run(self.lib.dimb_selftest_aliked_threshold, "selftest_aliked_threshold", {"thr": (np.float32, 1)}, _ptr(score),
+                              score.size, None if cc is None else _ptr(cc), float(thr), float(sentinel))
+        return out["thr"][0], tail["thr"]
 
     def lg_assign(self, sim: np.ndarray, nf, n_orig, layer, indf: np.ndarray, z: np.ndarray, th: float, cap: int,
                   sentinel: float = -777.0) -> dict:

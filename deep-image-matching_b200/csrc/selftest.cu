@@ -11,6 +11,8 @@
 //     dimb_selftest_sg_sinkhorn: SuperGlue's Sinkhorn and mutual-max matching (sg_assign.cuh);
 //   dimb_selftest_sift_extrema / _ori / _select / _desc: the SIFT extremum refinement, orientation, selection and descriptor kernels
 //     (sift_kernels.cuh) through their launch helpers, on caller-given levels, candidates and records;
+//   dimb_selftest_aliked_conv_plan / _conv3x3 / _conv1x1 / _avgpool / _pad / _crop / _deform / _fuse / _dkd / _sddh / _threshold: the
+//     ALIKED stages (aliked_kernels.cuh) through their launch helpers, on caller-given maps, weights and keypoints;
 //   dimb_gv_host / dimb_gv_lo_host / dimb_gv_seven_point_host: the RANSAC arithmetic of gv.cu on the host (ransac8, lo-ransac, the
 //     7-point solver).
 #include <algorithm>
@@ -1342,4 +1344,311 @@ extern "C" int dimb_selftest_sift_desc(dimb_ctx* ctx, const float* gauss, int B,
   DIMB_TRY(launch_sift_desc(ctx, 0, d_pyr, g, d_rec, d_sel, n, out));
   DIMB_TRY(sync_call(ctx, "dimb_selftest_sift_desc"));
   return download(ctx, desc, d_desc, nd + kDetTail);
+}
+
+#include "aliked_kernels.cuh"
+
+namespace {
+// caller's n floats followed by kDetTail NaN: a read past the logical end turns an output into NaN
+std::vector<float> al_nan_tail(const float* p, size_t n) {
+  std::vector<float> v(n + kDetTail, std::nanf(""));
+  std::copy(p, p + n, v.begin());
+  return v;
+}
+// n + kDetTail floats holding `sentinel`
+std::vector<float> al_sent(size_t n, float sentinel) { return std::vector<float>(n + kDetTail, sentinel); }
+// a staged input, or null when the caller gives none
+int al_up_opt(DevTmp& t, const float* p, size_t n, float** d) {
+  *d = nullptr;
+  return p ? t.upload(d, al_nan_tail(p, n)) : DIMB_OK;
+}
+bool al_sizes_ok(int H, int W, int c) {
+  return H >= 1 && W >= 1 && c >= 1 && H <= 16384 && W <= 16384 && static_cast<size_t>(H) * W * c <= (size_t{1} << 30);
+}
+}  // namespace
+
+// ALIKED (aliked_kernels.cuh) stage by stage, through the launch helpers dimb_aliked_extract_dev calls, on caller-given inputs in the
+// production layout.  Inputs are staged with kDetTail NaN after them; every output buffer holds kDetTail more elements after the valid
+// ones and starts as `sentinel`.  Bad arguments return DIMB_ERR_ARG (DIMB_ERR_UNSUPPORTED: a deformable shape production has no
+// kernel for) before any CUDA call.
+
+// The al_conv3x3_kernel instantiation conv3 picks for an H x W map with cout output channels: out[0] = 1 (<8,1>), 2 (<16,4>) or 3
+// (<8,4>).  Host only.
+extern "C" int dimb_selftest_aliked_conv_plan(int H, int W, int cout, int* out) {
+  if (!out || H < 1 || W < 1 || cout < 1) return DIMB_ERR_ARG;
+  out[0] = al_conv3_plan(H, W, cout);
+  return DIMB_OK;
+}
+
+// conv3: out [cout][H][W] = act(alpha * conv3x3(x [cin][H][W], w [cout][cin][3][3], zero padding 1) + beta (+ resid [cout][H][W])).
+// alpha, beta [cout] and resid may be null; act 0 none, 1 SELU, 2 sigmoid.  variant 0: the production rule (al_conv3_plan), 1..3 that
+// instantiation.  plan[0] (may be null): the instantiation that ran.
+extern "C" int dimb_selftest_aliked_conv3x3(dimb_ctx* ctx, int variant, const float* x, int cin, int H, int W, const float* w,
+                                            const float* alpha, const float* beta, const float* resid, int cout, int act, float sentinel,
+                                            float* out, int* plan) {
+  if (!ctx || !x || !w || !out || variant < 0 || variant > 3 || act < 0 || act > 2 || cin < 1 || cout < 1 || cin > 1024 || cout > 1024 ||
+      !al_sizes_ok(H, W, std::max(cin, cout)))
+    return DIMB_ERR_ARG;
+  const int pl = variant ? variant : al_conv3_plan(H, W, cout);
+  if (plan) plan[0] = pl;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const size_t hw = static_cast<size_t>(H) * W;
+  DevTmp t{ctx, {}};
+  float *d_x, *d_w, *d_a, *d_b, *d_r, *d_o;
+  DIMB_TRY(t.upload(&d_x, al_nan_tail(x, hw * cin)));
+  DIMB_TRY(t.upload(&d_w, al_nan_tail(w, static_cast<size_t>(cout) * cin * 9)));
+  DIMB_TRY(al_up_opt(t, alpha, cout, &d_a));
+  DIMB_TRY(al_up_opt(t, beta, cout, &d_b));
+  DIMB_TRY(al_up_opt(t, resid, hw * cout, &d_r));
+  DIMB_TRY(t.upload(&d_o, al_sent(hw * cout, sentinel)));
+  DIMB_TRY(conv3_as(ctx, 0, pl, d_x, cin, H, W, d_w, d_a, d_b, d_r, d_o, cout, act));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_aliked_conv3x3"));
+  return download(ctx, out, d_o, hw * cout + kDetTail);
+}
+
+// conv1: out [cout][P] = act(w [cout][cin] x [cin][P] + bias [cout] (may be null)); cin <= 512
+extern "C" int dimb_selftest_aliked_conv1x1(dimb_ctx* ctx, const float* x, int cin, int P, const float* w, const float* bias, int cout,
+                                            int act, float sentinel, float* out) {
+  if (!ctx || !x || !w || !out || act < 0 || act > 2 || cin < 1 || cout < 1 || cin > 512 || cout > 1024 || !al_sizes_ok(1, P, std::max(cin, cout)))
+    return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  DevTmp t{ctx, {}};
+  float *d_x, *d_w, *d_b, *d_o;
+  DIMB_TRY(t.upload(&d_x, al_nan_tail(x, static_cast<size_t>(P) * cin)));
+  DIMB_TRY(t.upload(&d_w, al_nan_tail(w, static_cast<size_t>(cout) * cin)));
+  DIMB_TRY(al_up_opt(t, bias, cout, &d_b));
+  DIMB_TRY(t.upload(&d_o, al_sent(static_cast<size_t>(P) * cout, sentinel)));
+  DIMB_TRY(conv1(ctx, 0, d_x, cin, P, d_w, d_b, d_o, cout, act));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_aliked_conv1x1"));
+  return download(ctx, out, d_o, static_cast<size_t>(P) * cout + kDetTail);
+}
+
+// k x k average pooling, stride k: x [C][H][W] -> out [C][H / k][W / k]; 1 <= k <= min(H, W)
+extern "C" int dimb_selftest_aliked_avgpool(dimb_ctx* ctx, const float* x, int C, int H, int W, int k, float sentinel, float* out) {
+  if (!ctx || !x || !out || !al_sizes_ok(H, W, C) || k < 1 || k > H || k > W) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const size_t no = static_cast<size_t>(C) * (H / k) * (W / k);
+  DevTmp t{ctx, {}};
+  float *d_x, *d_o;
+  DIMB_TRY(t.upload(&d_x, al_nan_tail(x, static_cast<size_t>(C) * H * W)));
+  DIMB_TRY(t.upload(&d_o, al_sent(no, sentinel)));
+  DIMB_TRY(launch_al_avgpool(ctx, 0, d_x, C, H, W, k, d_o));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_aliked_avgpool"));
+  return download(ctx, out, d_o, no + kDetTail);
+}
+
+// InputPadder and al_pad_kernel: image [H][W][channels] (channels 1 or 3, 0..255) -> out [3][Hp][Wp]; geo[4] = {Hp, Wp, top, left}.
+// out holds 3 (H + 31) (W + 31) elements and kDetTail more: the padded size is not known to the caller in advance.
+extern "C" int dimb_selftest_aliked_pad(dimb_ctx* ctx, const float* img, int H, int W, int channels, float sentinel, float* out, int* geo) {
+  if (!ctx || !img || !out || !geo || (channels != 1 && channels != 3) || !al_sizes_ok(H, W, 3)) return DIMB_ERR_ARG;
+  int Hp, Wp, top, left;
+  al_input_padder(H, W, Hp, Wp, top, left);
+  geo[0] = Hp, geo[1] = Wp, geo[2] = top, geo[3] = left;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const size_t no = static_cast<size_t>(3) * (H + 31) * (W + 31);
+  DevTmp t{ctx, {}};
+  float *d_i, *d_o;
+  DIMB_TRY(t.upload(&d_i, al_nan_tail(img, static_cast<size_t>(H) * W * channels)));
+  DIMB_TRY(t.upload(&d_o, al_sent(no, sentinel)));
+  DIMB_TRY(launch_al_pad(ctx, 0, d_i, H, W, channels, d_o, Hp, Wp, top, left));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_aliked_pad"));
+  return download(ctx, out, d_o, no + kDetTail);
+}
+
+// al_crop_kernel: one plane [Hp][Wp] -> out [H][W] = rows top.., columns left..
+extern "C" int dimb_selftest_aliked_crop(dimb_ctx* ctx, const float* in, int Hp, int Wp, int top, int left, int H, int W, float sentinel,
+                                         float* out) {
+  if (!ctx || !in || !out || !al_sizes_ok(Hp, Wp, 1) || H < 1 || W < 1 || top < 0 || left < 0 || top + H > Hp || left + W > Wp)
+    return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const size_t no = static_cast<size_t>(H) * W;
+  DevTmp t{ctx, {}};
+  float *d_i, *d_o;
+  DIMB_TRY(t.upload(&d_i, al_nan_tail(in, static_cast<size_t>(Hp) * Wp)));
+  DIMB_TRY(t.upload(&d_o, al_sent(no, sentinel)));
+  DIMB_TRY(launch_al_crop(ctx, 0, d_i, Hp, Wp, top, left, d_o, H, W));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_aliked_crop"));
+  return download(ctx, out, d_o, no + kDetTail);
+}
+
+// Deformable 3x3 conv + eval BatchNorm (+ resid [cout][H][W], may be null) + act on x [cin][H][W]; cin a multiple of 8 up to 128, cout
+// 64 or 128.  w [cout][cin][3][3] (the state_dict layout) and bn [4][cout] (gamma, beta, running mean, running var) go through the
+// transforms dimb_aliked_create applies.  Mode A (offs given): offsets [18][H][W] ((dy, dx) per tap) clamped to +-max_off.  Mode B (offs
+// null): the dcn helper, offsets = offset_conv(x) with offw [18][cin][3][3] and offb [18], max_off = max(H, W) / 4; off_out [18][H][W]
+// (may be null) receives them.  out [cout][H][W].
+extern "C" int dimb_selftest_aliked_deform(dimb_ctx* ctx, const float* x, int cin, int H, int W, const float* offs, float max_off,
+                                           const float* offw, const float* offb, const float* w, const float* bn, const float* resid, int cout,
+                                           int act, float sentinel, float* out, float* off_out) {
+  if (!ctx || !x || !w || !bn || !out || (!offs && (!offw || !offb)) || act < 0 || act > 2 || !al_sizes_ok(H, W, 128) || cin < 1 ||
+      cout < 1 || (offs && !(max_off >= 0.f && std::isfinite(max_off))))
+    return DIMB_ERR_ARG;
+  if (cin % 8 || cin > 128 || (cout != 64 && cout != 128)) return DIMB_ERR_UNSUPPORTED;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const size_t hw = static_cast<size_t>(H) * W;
+  std::vector<float> al, be;
+  al_bn_fold(bn, bn + cout, bn + 2 * cout, bn + 3 * cout, cout, al, be);
+  const std::vector<float> wt = al_dcn_weight(w, cout, cin);
+  DevTmp t{ctx, {}};
+  BnConv c;
+  c.cin = cin, c.cout = cout;
+  float *d_x, *d_off, *d_r, *d_o;
+  DIMB_TRY(t.upload(&d_x, al_nan_tail(x, hw * cin)));
+  DIMB_TRY(t.upload(&c.w, wt));
+  DIMB_TRY(t.upload(&c.alpha, al));
+  DIMB_TRY(t.upload(&c.beta, be));
+  DIMB_TRY(al_up_opt(t, resid, hw * cout, &d_r));
+  DIMB_TRY(t.upload(&d_o, al_sent(hw * cout, sentinel)));
+  if (offs) {
+    DIMB_TRY(t.upload(&d_off, al_nan_tail(offs, hw * 18)));
+    DIMB_TRY(launch_al_deform(ctx, 0, d_x, cin, H, W, d_off, max_off, c, d_r, d_o, act));
+  } else {
+    float *d_ow, *d_ob;
+    DIMB_TRY(t.upload(&d_ow, al_nan_tail(offw, static_cast<size_t>(18) * cin * 9)));
+    DIMB_TRY(t.upload(&d_ob, al_nan_tail(offb, 18)));
+    DIMB_TRY(t.upload(&d_off, al_sent(hw * 18, sentinel)));
+    DIMB_TRY(dcn(ctx, 0, d_x, cin, H, W, d_ow, d_ob, d_off, c, d_r, d_o, act));
+  }
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_aliked_deform"));
+  if (!offs && off_out) DIMB_TRY(download(ctx, off_out, d_off, hw * 18 + kDetTail));
+  return download(ctx, out, d_o, hw * cout + kDetTail);
+}
+
+// al_fuse_kernel on a padded Hp x Wp map (multiples of 32): x1 [16][Hp][Wp] (block 1's output), the lateral outputs l2o [32][Hp/2][Wp/2],
+// l3o [32][Hp/8][Wp/8], l4o [32][Hp/32][Wp/32], l1 = conv1.weight [32][16], s0 = score_head.0.weight [8][128].  Outputs sh0 [8][Hp][Wp]
+// and feat [H][W][128], the crop at (top, left).
+extern "C" int dimb_selftest_aliked_fuse(dimb_ctx* ctx, const float* x1, const float* l2o, const float* l3o, const float* l4o, const float* l1,
+                                         const float* s0, int Hp, int Wp, int top, int left, int H, int W, float sentinel, float* sh0,
+                                         float* feat) {
+  if (!ctx || !x1 || !l2o || !l3o || !l4o || !l1 || !s0 || !sh0 || !feat || !al_sizes_ok(Hp, Wp, 128) || Hp % 32 || Wp % 32 || H < 1 ||
+      W < 1 || top < 0 || left < 0 || top + H > Hp || left + W > Wp)
+    return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const size_t P = static_cast<size_t>(Hp) * Wp, nf = static_cast<size_t>(H) * W * 128;
+  DevTmp t{ctx, {}};
+  float *d_x1, *d_l2, *d_l3, *d_l4, *d_w1, *d_s0, *d_sh, *d_f;
+  DIMB_TRY(t.upload(&d_x1, al_nan_tail(x1, P * 16)));
+  DIMB_TRY(t.upload(&d_l2, al_nan_tail(l2o, P / 4 * 32)));
+  DIMB_TRY(t.upload(&d_l3, al_nan_tail(l3o, P / 64 * 32)));
+  DIMB_TRY(t.upload(&d_l4, al_nan_tail(l4o, P / 1024 * 32)));
+  DIMB_TRY(t.upload(&d_w1, al_nan_tail(l1, 32 * 16)));
+  DIMB_TRY(t.upload(&d_s0, al_nan_tail(s0, 8 * 128)));
+  DIMB_TRY(t.upload(&d_sh, al_sent(P * 8, sentinel)));
+  DIMB_TRY(t.upload(&d_f, al_sent(nf, sentinel)));
+  DIMB_TRY(launch_al_fuse(ctx, 0, d_x1, d_w1, d_l2, d_l3, d_l4, d_s0, Hp, Wp, top, left, H, W, d_sh, d_f));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_aliked_fuse"));
+  DIMB_TRY(download(ctx, sh0, d_sh, P * 8 + kDetTail));
+  return download(ctx, feat, d_f, nf + kDetTail);
+}
+
+// DKD refinement at radius r (1..5) on score [H][W] (H, W >= 2) at the pixels sel_idx [min(count, cap)] (each < H W): kxy [cap][2]
+// normalised, disp [cap], kscore [cap]; entries from min(count, cap) on are not written.
+extern "C" int dimb_selftest_aliked_dkd(dimb_ctx* ctx, const float* score, int H, int W, int r, const int* sel_idx, int count, int cap,
+                                        float sentinel, float* kxy, float* disp, float* kscore) {
+  if (!ctx || !score || !kxy || !disp || !kscore || (count > 0 && !sel_idx) || !al_sizes_ok(H, W, 1) || H < 2 || W < 2 || r < 1 || r > 5 ||
+      count < 0 || cap < 1 || cap > (1 << 24))
+    return DIMB_ERR_ARG;
+  const int n = std::min(count, cap);
+  for (int i = 0; i < n; ++i)
+    if (sel_idx[i] < 0 || sel_idx[i] >= H * W) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  DevTmp t{ctx, {}};
+  float *d_s, *d_kxy, *d_disp, *d_ks;
+  int *d_idx, *d_cnt;
+  std::vector<int> idx(static_cast<size_t>(n) + kDetTail, 0);
+  std::copy(sel_idx, sel_idx + n, idx.begin());
+  DIMB_TRY(t.upload(&d_s, al_nan_tail(score, static_cast<size_t>(H) * W)));
+  DIMB_TRY(t.upload(&d_idx, idx));
+  DIMB_TRY(t.upload(&d_cnt, std::vector<int>{count}));
+  DIMB_TRY(t.upload(&d_kxy, al_sent(static_cast<size_t>(cap) * 2, sentinel)));
+  DIMB_TRY(t.upload(&d_disp, al_sent(cap, sentinel)));
+  DIMB_TRY(t.upload(&d_ks, al_sent(cap, sentinel)));
+  DIMB_TRY(launch_al_dkd(ctx, 0, d_s, H, W, r, d_idx, d_cnt, cap, d_kxy, d_disp, d_ks));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_aliked_dkd"));
+  DIMB_TRY(download(ctx, kxy, d_kxy, static_cast<size_t>(cap) * 2 + kDetTail));
+  DIMB_TRY(download(ctx, disp, d_disp, cap + kDetTail));
+  return download(ctx, kscore, d_ks, cap + kDetTail);
+}
+
+// The SDDH descriptor head in the context's precision on feat [H][W][128] (H, W >= 8) at normalised keypoints kxy [min(count, cap)][2]
+// (within [-1, 1]).  Weights in the state_dict layout: w0 [32][128][3][3], b0 [32], w2 [32][32], b2 [32], sf [128][128], agg
+// [16][128][128].  off_in [min(count, cap)][32] (may be null; finite): offsets (16 x, then 16 y) that replace the offsets stage's for the
+// samples.  Outputs kpts_px [cap][2] and off [cap][32] of the offsets stage, and desc [128][cap].
+extern "C" int dimb_selftest_aliked_sddh(dimb_ctx* ctx, const float* feat, int H, int W, const float* kxy, int count, int cap, const float* w0,
+                                         const float* b0, const float* w2, const float* b2, const float* sf, const float* agg,
+                                         const float* off_in, float sentinel, float* kpts_px, float* off, float* desc) {
+  if (!ctx || !feat || !w0 || !b0 || !w2 || !b2 || !sf || !agg || !kpts_px || !off || !desc || (count > 0 && !kxy) ||
+      !al_sizes_ok(H, W, 128) || H < 8 || W < 8 || count < 0 || cap < 1 || cap > (1 << 20))
+    return DIMB_ERR_ARG;
+  const int n = std::min(count, cap);
+  for (int i = 0; i < 2 * n; ++i)
+    if (!(std::fabs(kxy[i]) <= 1.f)) return DIMB_ERR_ARG;
+  if (off_in)
+    for (int i = 0; i < 32 * n; ++i)
+      if (!std::isfinite(off_in[i])) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const bool exact = ctx->precision == DIMB_PRECISION_EXACT;
+  const size_t rows = static_cast<size_t>(round_up(cap, kTileM)) * 16;
+  DevTmp t{ctx, {}};
+  float *d_feat, *d_kxy, *d_w0T, *d_b0, *d_w2, *d_b2, *d_kp, *d_off, *d_offs, *d_dsc, *d_desc;
+  __half *sfh, *sfl, *agh, *agl, *fsh, *fsl, *f2h, *f2l;
+  int* d_cnt;
+  CUtensorMap m_sf[2], m_ag[2], m_fs[2], m_f2[2];
+  std::vector<__half> h, l;
+  al_split_host(sf, static_cast<size_t>(128) * 128, h, l);
+  DIMB_TRY(t.upload(&sfh, h));
+  DIMB_TRY(t.upload(&sfl, l));
+  const std::vector<float> agt = al_sddh_agg(agg);
+  al_split_host(agt.data(), agt.size(), h, l);
+  DIMB_TRY(t.upload(&agh, h));
+  DIMB_TRY(t.upload(&agl, l));
+  DIMB_TRY(dimb_tmap_2d(ctx, &m_sf[0], sfh, 128, 128, 128, 128));
+  DIMB_TRY(dimb_tmap_2d(ctx, &m_sf[1], sfl, 128, 128, 128, 128));
+  DIMB_TRY(dimb_tmap_2d(ctx, &m_ag[0], agh, 128, 2048, 2048, 128));
+  DIMB_TRY(dimb_tmap_2d(ctx, &m_ag[1], agl, 128, 2048, 2048, 128));
+  DIMB_TRY(t.get(&fsh, rows * 128));
+  DIMB_TRY(t.get(&fsl, rows * 128));
+  DIMB_TRY(t.get(&f2h, rows * 128));
+  DIMB_TRY(t.get(&f2l, rows * 128));
+  DIMB_TRY(dimb_tmap_2d(ctx, &m_fs[0], fsh, rows, 128, 128, kTileM));
+  DIMB_TRY(dimb_tmap_2d(ctx, &m_fs[1], fsl, rows, 128, 128, kTileM));
+  DIMB_TRY(dimb_tmap_2d(ctx, &m_f2[0], f2h, rows / 16, 2048, 2048, kTileM));
+  DIMB_TRY(dimb_tmap_2d(ctx, &m_f2[1], f2l, rows / 16, 2048, 2048, kTileM));
+  DIMB_TRY(t.get(&d_dsc, static_cast<size_t>(round_up(cap, kTileM)) * 128));
+  DIMB_TRY(t.upload(&d_feat, al_nan_tail(feat, static_cast<size_t>(H) * W * 128)));
+  DIMB_TRY(t.upload(&d_kxy, al_nan_tail(kxy, static_cast<size_t>(2) * n)));
+  DIMB_TRY(t.upload(&d_w0T, al_sddh_w0T(w0)));
+  DIMB_TRY(t.upload(&d_b0, al_nan_tail(b0, 32)));
+  DIMB_TRY(t.upload(&d_w2, al_nan_tail(w2, 32 * 32)));
+  DIMB_TRY(t.upload(&d_b2, al_nan_tail(b2, 32)));
+  DIMB_TRY(t.upload(&d_cnt, std::vector<int>{count}));
+  DIMB_TRY(t.upload(&d_kp, al_sent(static_cast<size_t>(cap) * 2, sentinel)));
+  DIMB_TRY(t.upload(&d_off, al_sent(static_cast<size_t>(cap) * 32, sentinel)));
+  DIMB_TRY(t.upload(&d_desc, al_sent(static_cast<size_t>(cap) * 128, sentinel)));
+  d_offs = d_off;
+  if (off_in) DIMB_TRY(t.upload(&d_offs, al_nan_tail(off_in, static_cast<size_t>(32) * n)));
+  DIMB_TRY(launch_al_sddh_offsets(ctx, 0, d_feat, H, W, d_kxy, d_cnt, cap, d_w0T, d_b0, d_w2, d_b2, d_kp, d_off));
+  DIMB_TRY(launch_al_sddh_sample(ctx, 0, d_feat, H, W, d_kxy, d_cnt, cap, d_offs, fsh, exact ? fsl : nullptr));
+  DIMB_TRY(launch_al_sddh_sf_gemm(ctx, 0, m_fs, m_sf, f2h, exact ? f2l : nullptr, d_cnt, cap));
+  DIMB_TRY(launch_al_sddh_agg_gemm(ctx, 0, m_f2, m_ag, d_dsc, d_cnt, cap));
+  DIMB_TRY(launch_al_sddh_norm(ctx, 0, d_dsc, d_cnt, cap, d_desc));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_aliked_sddh"));
+  DIMB_TRY(download(ctx, kpts_px, d_kp, static_cast<size_t>(cap) * 2 + kDetTail));
+  DIMB_TRY(download(ctx, off, d_off, static_cast<size_t>(cap) * 32 + kDetTail));
+  return download(ctx, desc, d_desc, static_cast<size_t>(cap) * 128 + kDetTail);
+}
+
+// al_threshold_kernel on score [HW]: cand_count (may be null: mean mode) points at the candidate count above thr.  thr_out [1].
+extern "C" int dimb_selftest_aliked_threshold(dimb_ctx* ctx, const float* score, int HW, const int* cand_count, float thr, float sentinel,
+                                              float* thr_out) {
+  if (!ctx || !score || !thr_out || HW < 1 || HW > (1 << 28) || (cand_count && *cand_count < 0)) return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  DevTmp t{ctx, {}};
+  float *d_s, *d_o;
+  int* d_c = nullptr;
+  DIMB_TRY(t.upload(&d_s, al_nan_tail(score, HW)));
+  if (cand_count) DIMB_TRY(t.upload(&d_c, std::vector<int>{*cand_count}));
+  DIMB_TRY(t.upload(&d_o, al_sent(1, sentinel)));
+  DIMB_TRY(launch_al_threshold(ctx, 0, d_s, HW, d_c, thr, d_o));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_aliked_threshold"));
+  return download(ctx, thr_out, d_o, 1 + kDetTail);
 }
