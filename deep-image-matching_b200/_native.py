@@ -103,7 +103,7 @@ class GvConf(C.Structure):
                 ("estimator", C.c_int), ("confidence", C.c_float)]
 
 
-GV_ESTIMATORS = {"ransac8": 0, "lo-ransac": 1}
+GV_ESTIMATORS = {"ransac8": 0, "lo-ransac": 1, "degensac": 3}
 
 
 def gv_estimator(name) -> int:
@@ -284,6 +284,10 @@ def load_selftest_library():
         lib.dimb_gv_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_uint, vp, vp]
         lib.dimb_gv_lo_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_float, C.c_uint, vp, vp, C.POINTER(ip)]
         lib.dimb_gv_seven_point_host.argtypes = [vp, vp, vp]
+        lib.dimb_gv_degensac_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_float, C.c_uint, vp, vp, C.POINTER(ip)]
+        lib.dimb_gv_h_from_f3_host.argtypes = [vp, vp, vp, ip, vp, vp]
+        lib.dimb_gv_degenerate_host.argtypes = [vp, vp, vp, ip, vp, C.c_float, vp]
+        lib.dimb_gv_plane_parallax_host.argtypes = [vp, vp, vp, ip, ip, ip, vp]
         _selftest = lib
     return _selftest
 
@@ -901,7 +905,7 @@ class Context:
     def gv_estimate(self, kpts0: np.ndarray, kpts1: np.ndarray, threshold: float = 1.0, max_iters: int = 10000, seed: int = 0,
                     estimator: str = "ransac8", confidence: float = 0.9999):
         """Matched keypoints (n,2) each -> (F (3,3) float32 or None, inlier mask bool (n,), hypotheses run) with the named estimator
-        (dimb_gv_estimate; ``confidence`` is read by lo-ransac only)."""
+        (dimb_gv_estimate; ``confidence`` is read by lo-ransac and degensac only)."""
         k0 = np.ascontiguousarray(kpts0, np.float32)
         k1 = np.ascontiguousarray(kpts1, np.float32)
         n = k0.shape[0]
@@ -920,7 +924,7 @@ class Context:
         FeatureStoreDev.feats_dev); d_matches [P][cap][2] int64 / d_n_matches [P] int32 as LightGlueNet.match_dev writes them; seeds:
         one uint32 per pair (geometric_verification.gv_seed).  Outputs are device buffers (ints are device addresses): d_verified
         [P][cap][2] int64, d_n_verified [P] int32, d_F [P][9] float32, d_mask [P][cap] uint8, d_n_inliers [P] int32.  Asynchronous
-        on `stream`.  estimator: a name in GV_ESTIMATORS; confidence is read by lo-ransac only."""
+        on `stream`.  estimator: a name in GV_ESTIMATORS; confidence is read by lo-ransac and degensac only."""
         P = len(f0)
         a0 = (FeatsDev * P)(*f0)
         a1 = (FeatsDev * P)(*f1)

@@ -12,6 +12,11 @@
 //     the wave's best model if it beats the pair's best and runs local optimisation on it (inner RANSAC on 16-inlier least-squares
 //     fits, each iterated 4 times), then applies confidence stopping.  Up to min(max_iters, 65536) hypotheses; every wave is
 //     enqueued and a pair that has stopped returns at once, so nothing waits for the host.  The finalize step is shared.
+//   degensac (estimator 3; 2 stays refused, as it was before degensac existed): lo-ransac's waves plus DEGENSAC's treatment of
+//     dominant planes (Chum, Werner, Matas, CVPR 2005).  A 7-point model whose sample is dominated by a plane (gv::degenerate7) also
+//     has that plane's H scored; when a wave's best H beats the pair's best H, plane and parallax (gv_pp_kernel) recovers
+//     F = [e']_x H from pairs of the matches off that plane, and the best such F competes with the wave's best model for adoption and
+//     local optimisation.
 // RANSAC is stochastic in the reference too (pydegensac's own RNG), so parity is statistical: tests compare inlier sets on data
 // with known geometry and against OpenCV on the same matches.  Every reduction runs in a fixed order (integer atomics only), so a
 // pair's result is a function of its matches, its seed and the configuration alone: bitwise reproducible across calls and batches.
@@ -145,6 +150,15 @@ struct GvLo {
 };
 constexpr int kLoWave = 1024, kLoMaxIters = 65536, kLoInner = 20, kLoSample = 16, kLoLsq = 4;
 __device__ __forceinline__ int gv_lo_lim(const GvLo& s, int H) { return s.lim ? s.lim : H; }
+
+// degensac state of one pair next to its GvLo (zeroed before the first wave)
+struct GvDeg {
+  unsigned long long wave_hkey;  // best (H count << 32 | ~(3 h + root)) of the current wave's plane-dominated models; 0: none
+  int hbest;                     // the best H count the pair has seen
+  int pp_cnt;                    // Sampson count of the plane-and-parallax model of the current wave, -1: none
+  float F[9];                    // that model
+};
+static_assert(gv::kPpChunk == kFinThreads, "gv_pp_kernel runs one plane-and-parallax draw per thread and chunk");
 
 
 // kLo: the model is the one lo-ransac adopted (lo[pair].F) rather than hypothesis best[pair] re-solved
@@ -282,9 +296,13 @@ gv_finalize_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, 
 
 // ------------------------------------------------------------------ lo-ransac
 // grid (kLoWave / 128, P): hypothesis h = wave * kLoWave + thread of the pair's wave, for h < its limit; 7 points, up to 3 models,
-// each scored over all matches; wave_key = max over (count << 32 | ~(3 h + root)) (ties -> lowest hypothesis, then lowest root)
+// each scored over all matches; wave_key = max over (count << 32 | ~(3 h + root)) (ties -> lowest hypothesis, then lowest root).
+// kDeg (degensac): the first model of the hypothesis that gv::degenerate7 finds dominated by a plane also has that plane's H scored
+// (matches within gv::kDegHFactor * threshold transfer error) into deg[pair].wave_hkey, keyed as wave_key.
+template <bool kDeg>
 __global__ void __launch_bounds__(128)
-gv_lo_hypotheses_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, GvLo* lo, int cap, int wave, int H, float thr2) {
+gv_lo_hypotheses_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, GvLo* lo, int cap, int wave, int H, float thr2,
+                        GvDeg* deg) {
   const int pi = blockIdx.y, h = wave * kLoWave + blockIdx.x * blockDim.x + threadIdx.x;
   GvLo& s = lo[pi];
   if (s.done) return;
@@ -300,20 +318,44 @@ gv_lo_hypotheses_kernel(const GvPair* pairs, const float* xy, const gv::Norm* no
     id7[k] = k;
   }
   float F[3][9];
-  const int m = gv::seven_point(k0, k1, id7, norms[2 * pi], norms[2 * pi + 1], F);
+  float Hp[9];
+  int hr = -1;  // kDeg: the model whose plane H (pixels) is scored
+  int m;
+  if constexpr (kDeg) {
+    const gv::Norm n0 = norms[2 * pi], n1 = norms[2 * pi + 1];
+    float u[7][4];
+    m = gv::seven_point(k0, k1, id7, n0, n1, F);
+    for (int k = 0; k < 7; ++k)
+      u[k][0] = (k0[2 * k] - n0.cx) * n0.s, u[k][1] = (k0[2 * k + 1] - n0.cy) * n0.s, u[k][2] = (k1[2 * k] - n1.cx) * n1.s,
+      u[k][3] = (k1[2 * k + 1] - n1.cy) * n1.s;
+    for (int r = 0; r < m; ++r) {
+      float Fn[9], Hn[9];
+      gv::normalise_f(F[r], n0, n1, Fn);
+      if (gv::degenerate7(Fn, u, gv::deg_t2n(thr2, n1), Hn) < 0) continue;
+      if (gv::h_denormalise(Hn, n0, n1, Hp)) hr = r;
+      break;
+    }
+  } else {
+    m = gv::seven_point(k0, k1, id7, norms[2 * pi], norms[2 * pi + 1], F);
+  }
   if (m == 0) return;
-  int cnt[3] = {0, 0, 0};
+  int cnt[3] = {0, 0, 0}, hc = 0;
   const float4* p4 = reinterpret_cast<const float4*>(pts);
   for (int i = 0; i < n; ++i) {
     const float4 c = __ldg(p4 + i);
 #pragma unroll
     for (int r = 0; r < 3; ++r)
       if (r < m) cnt[r] += gv::sampson2(F[r], c.x, c.y, c.z, c.w) < thr2;
+    if constexpr (kDeg)
+      if (hr >= 0) hc += gv::transfer2(Hp, c.x, c.y, c.z, c.w) < gv::kDegHFactor * gv::kDegHFactor * thr2;
   }
   unsigned long long key = 0ull;
   for (int r = 0; r < m; ++r)
     key = max(key, (static_cast<unsigned long long>(cnt[r]) << 32) | (0xffffffffu - static_cast<unsigned>(3 * h + r)));
   atomicMax(&s.wave_key, key);
+  if constexpr (kDeg)
+    if (hr >= 0)
+      atomicMax(&deg[pi].wave_hkey, (static_cast<unsigned long long>(hc) << 32) | (0xffffffffu - static_cast<unsigned>(3 * h + hr)));
 }
 
 // CTA-wide count of the matches whose Sampson distance to F is below thr2 and, with `normal`, the sum of their normal-matrix rows
@@ -399,9 +441,12 @@ __device__ bool gv_lo_refit(const float* Nm, gv::Norm n0, gv::Norm n1, float f[9
 // optimisation - kLoInner times: the inliers at 2x the threshold (fewer than kLoSample: stop), a least-squares fit of kLoSample of them
 // drawn on the LO stream, kLoLsq least-squares refits on that fit's inliers, the result adopted if it explains more matches.  Then
 // confidence stopping: the pair is done once it has run min(its limit, the hypotheses its best model calls for).  inl: [P][cap] scratch.
+// kDeg (degensac): the wave's plane-and-parallax model (deg[pair]) is adopted instead when it explains at least 8 matches and at least
+// as many as the pair's best and the wave's best model.
+template <bool kDeg>
 __global__ void __launch_bounds__(kFinThreads)
 gv_lo_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, unsigned long long* best, GvLo* lo, int* inl, int cap, int wave,
-             int H, float thr2, float confidence) {
+             int H, float thr2, float confidence, const GvDeg* deg) {
   const int pi = blockIdx.x, t = threadIdx.x;
   GvLo* s = lo + pi;
   if (s->done) return;
@@ -421,8 +466,17 @@ gv_lo_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, unsign
     const unsigned long long key = s->wave_key;
     s->wave_key = 0ull;
     cur = static_cast<int>(best[pi] >> 32);
-    adopt = key != 0ull && static_cast<int>(key >> 32) > cur;
-    if (adopt) {  // re-solve the winning hypothesis
+    bool pp = false;
+    if constexpr (kDeg) {
+      const int pc = deg[pi].pp_cnt;
+      pp = pc >= 8 && pc >= cur && pc >= static_cast<int>(key >> 32);
+      if (pp) {
+        for (int j = 0; j < 9; ++j) F[j] = deg[pi].F[j];
+        cur = pc;
+      }
+    }
+    adopt = pp || (key != 0ull && static_cast<int>(key >> 32) > cur);
+    if (adopt && !pp) {  // re-solve the winning hypothesis
       const unsigned id = 0xffffffffu - static_cast<unsigned>(key & 0xffffffffu);
       int idx[7], id7[7];
       float k0[14], k1[14], M[3][9];
@@ -490,18 +544,135 @@ gv_lo_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, unsign
   }
 }
 
-// The estimator of a gv_run call: 0 ransac8, 1 lo-ransac (confidence read by lo-ransac only).  lo_slot, lo_slot + 1: lo-ransac's
-// context scratch slots (52 for dimb_gv_estimate, 54 for dimb_gv_verify_dev).  gv_run's d_lo (optional) receives the address of the
-// per-pair lo-ransac state, whose `run` is the hypotheses count.
+// ------------------------------------------------------------------ degensac
+// The indices of the matches whose squared transfer error to H (pixels) is not below t2, in order (as gv_lo_inliers); their number.
+__device__ int gv_pp_outside(const float* Hs, const float* pts, int n, float t2, int* out, int* wcnt) {
+  const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
+  float h[9];
+  for (int j = 0; j < 9; ++j) h[j] = Hs[j];
+  int total = 0;
+  for (int base = 0; base < n; base += kFinThreads) {
+    const int i = base + t;
+    const bool off = i < n && !(gv::transfer2(h, pts[4 * i], pts[4 * i + 1], pts[4 * i + 2], pts[4 * i + 3]) < t2);
+    const unsigned bal = __ballot_sync(0xffffffffu, off);
+    if (lane == 0) wcnt[wid] = __popc(bal);
+    __syncthreads();
+    int o = total + __popc(bal & ((1u << lane) - 1u));
+    for (int w = 0; w < wid; ++w) o += wcnt[w];
+    if (off) out[o] = i;
+    for (int w = 0; w < kFinWarps; ++w) total += wcnt[w];
+    __syncthreads();
+  }
+  return total;
+}
+
+// one CTA per running pair, between the hypotheses and gv_lo_kernel of wave `wave`: if the wave's best H beats the pair's best H, plane
+// and parallax on it - the m matches off the plane in order, up to gv::kPpMax draws of two of them (one per thread in chunks of
+// gv::kPpChunk, stream gv::pp_sample2), F = [e']_x H of each scored by its Sampson count over all matches; the best (lowest draw on
+// ties) into deg[pair].  Between chunks, confidence stopping on the off-plane inlier fraction (count - (n - m)) / m of 2-point samples.
+// inl: [P][cap] scratch (gv_lo_kernel reuses it after).
+__global__ void __launch_bounds__(kFinThreads)
+gv_pp_kernel(const GvPair* pairs, const float* xy, const gv::Norm* norms, const GvLo* lo, GvDeg* deg, int* inl, int cap, int wave,
+             float thr2, float confidence) {
+  const int pi = blockIdx.x, t = threadIdx.x;
+  if (lo[pi].done) return;
+  GvDeg* d = deg + pi;
+  const GvPair p = pairs[pi];
+  const int n = gv_count(p);
+  const gv::Norm n0 = norms[2 * pi], n1 = norms[2 * pi + 1];
+  const float* pts = xy + static_cast<size_t>(pi) * cap * 4;
+  __shared__ float Hn[9], Hp[9], Fb[9];
+  __shared__ int wcnt[kFinWarps];
+  __shared__ int go;
+  __shared__ unsigned long long ckey;
+  if (t == 0) {
+    const unsigned long long key = d->wave_hkey;
+    d->wave_hkey = 0ull;
+    d->pp_cnt = -1;
+    go = 0;
+    if (key != 0ull && static_cast<int>(key >> 32) > d->hbest) {  // re-solve the winning model's plane
+      d->hbest = static_cast<int>(key >> 32);
+      const unsigned id = 0xffffffffu - static_cast<unsigned>(key & 0xffffffffu);
+      int idx[7], id7[7];
+      float k0[14], k1[14], M[3][9], Mn[9], u[7][4], h[9];
+      gv::sample7(p.seed, id / 3, n, idx);
+      for (int k = 0; k < 7; ++k) {
+        k0[2 * k] = pts[4 * idx[k]], k0[2 * k + 1] = pts[4 * idx[k] + 1], k1[2 * k] = pts[4 * idx[k] + 2], k1[2 * k + 1] = pts[4 * idx[k] + 3];
+        id7[k] = k;
+        u[k][0] = (k0[2 * k] - n0.cx) * n0.s, u[k][1] = (k0[2 * k + 1] - n0.cy) * n0.s, u[k][2] = (k1[2 * k] - n1.cx) * n1.s,
+        u[k][3] = (k1[2 * k + 1] - n1.cy) * n1.s;
+      }
+      const int m = gv::seven_point(k0, k1, id7, n0, n1, M);
+      const int r = static_cast<int>(id % 3);
+      if (r < m) gv::normalise_f(M[r], n0, n1, Mn);
+      if (r < m && gv::degenerate7(Mn, u, gv::deg_t2n(thr2, n1), h) >= 0) {
+        float g[9];
+        go = gv::h_denormalise(h, n0, n1, g);
+        for (int j = 0; j < 9; ++j) Hn[j] = h[j], Hp[j] = g[j];
+      }
+    }
+  }
+  __syncthreads();
+  if (!go) return;
+  int* list = inl + static_cast<size_t>(pi) * cap;
+  const int m = gv_pp_outside(Hp, pts, n, gv::kDegHFactor * gv::kDegHFactor * thr2, list, wcnt);
+  if (m < 2) return;
+  float h[9];
+  for (int j = 0; j < 9; ++j) h[j] = Hn[j];
+  const float4* p4 = reinterpret_cast<const float4*>(pts);
+  unsigned long long bkey = 0ull;  // best (count << 32 | ~draw) so far; 0: no model
+  int need = gv::kPpMax;
+  for (int base = 0; base < need; base += gv::kPpChunk) {
+    const int dr = base + t;
+    int pos[2];
+    gv::pp_sample2(p.seed, wave, dr, m, pos);
+    float a[4], b[4], fn[9], f[9];
+    for (int s = 0; s < 2; ++s) {
+      const int i = list[pos[s]];
+      float* c = s ? b : a;
+      c[0] = (pts[4 * i] - n0.cx) * n0.s, c[1] = (pts[4 * i + 1] - n0.cy) * n0.s, c[2] = (pts[4 * i + 2] - n1.cx) * n1.s,
+      c[3] = (pts[4 * i + 3] - n1.cy) * n1.s;
+    }
+    unsigned long long key = 0ull;
+    if (gv::plane_parallax(h, a, b, fn) && gv::denormalise(fn, n0, n1, f)) {
+      int c = 0;
+      for (int i = 0; i < n; ++i) {
+        const float4 q = __ldg(p4 + i);
+        c += gv::sampson2(f, q.x, q.y, q.z, q.w) < thr2;
+      }
+      key = (static_cast<unsigned long long>(c) << 32) | (0xffffffffu - static_cast<unsigned>(dr));
+    }
+    if (t == 0) ckey = 0ull;
+    __syncthreads();
+    atomicMax(&ckey, key);
+    __syncthreads();
+    const unsigned long long top = ckey;
+    if (key != 0ull && key == top && top > bkey)
+      for (int j = 0; j < 9; ++j) Fb[j] = f[j];
+    bkey = max(bkey, top);
+    const int bc = bkey ? static_cast<int>(bkey >> 32) : -1;
+    need = gv::ransac_needed<2>(max(0, bc - (n - m)), m, confidence, gv::kPpMax);
+    __syncthreads();  // Fb complete; ckey is reset by the next chunk
+  }
+  if (t == 0 && bkey) {
+    d->pp_cnt = static_cast<int>(bkey >> 32);
+    for (int j = 0; j < 9; ++j) d->F[j] = Fb[j];
+  }
+}
+
+// The estimator of a gv_run call: 0 ransac8, 1 lo-ransac, 3 degensac (confidence read by lo-ransac and degensac only).  lo_slot,
+// lo_slot + 1: the context scratch slots of lo-ransac's state, also used by degensac (52 for dimb_gv_estimate, 54 for
+// dimb_gv_verify_dev); deg_slot: degensac's state (56 / 57).  gv_run's d_lo (optional) receives the address of the per-pair lo-ransac
+// state, whose `run` is the hypotheses count.
 struct GvEstimator {
   int kind, max_iters;
   float confidence;
-  int lo_slot;
+  int lo_slot, deg_slot;
 };
 
 int gv_check_estimator(const dimb_gv_conf& c) {
   if (c.estimator == 0) return DIMB_OK;
-  if (c.estimator != 1 || !(c.confidence > 0.f && c.confidence < 1.f) || c.max_iters < 1) return DIMB_ERR_ARG;
+  if ((c.estimator != 1 && c.estimator != 3) || !(c.confidence > 0.f && c.confidence < 1.f) || c.max_iters < 1) return DIMB_ERR_ARG;
   return DIMB_OK;
 }
 
@@ -518,12 +689,14 @@ int gv_run(dimb_ctx* ctx, cudaStream_t st, const std::vector<GvPair>& hp, int ca
   DIMB_TRY(dimb_scratch(ctx, slot0 + 2, 2 * P * sizeof(gv::Norm), reinterpret_cast<void**>(&d_norm)));
   DIMB_TRY(dimb_scratch(ctx, slot0 + 3, P * sizeof(unsigned long long), reinterpret_cast<void**>(&d_best)));
   GvLo* lo = nullptr;
+  GvDeg* deg = nullptr;
   int* d_inl = nullptr;
-  if (est.kind == 1) {
+  if (est.kind != 0) {
     DIMB_TRY(dimb_scratch(ctx, est.lo_slot, P * sizeof(GvLo), reinterpret_cast<void**>(&lo)));
     DIMB_TRY(dimb_scratch(ctx, est.lo_slot + 1, static_cast<size_t>(P) * cap * sizeof(int), reinterpret_cast<void**>(&d_inl)));
     if (d_lo) *d_lo = lo;
   }
+  if (est.kind == 3) DIMB_TRY(dimb_scratch(ctx, est.deg_slot, P * sizeof(GvDeg), reinterpret_cast<void**>(&deg)));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(d_pairs, hp.data(), P * sizeof(GvPair), cudaMemcpyHostToDevice, st));
   const float thr2 = threshold * threshold;
   if (est.kind == 1) {
@@ -533,9 +706,28 @@ int gv_run(dimb_ctx* ctx, cudaStream_t st, const std::vector<GvPair>& hp, int ca
     gv_prepare_kernel<<<P, 256, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap);
     DIMB_LAUNCH_CHECK(ctx);
     for (int w = 0; w * kLoWave < H; ++w) {
-      gv_lo_hypotheses_kernel<<<dim3(kLoWave / 128, P), 128, 0, st>>>(d_pairs, d_xy, d_norm, lo, cap, w, H, thr2);
+      gv_lo_hypotheses_kernel<false><<<dim3(kLoWave / 128, P), 128, 0, st>>>(d_pairs, d_xy, d_norm, lo, cap, w, H, thr2, nullptr);
       DIMB_LAUNCH_CHECK(ctx);
-      gv_lo_kernel<<<P, kFinThreads, 0, st>>>(d_pairs, d_xy, d_norm, d_best, lo, d_inl, cap, w, H, thr2, est.confidence);
+      gv_lo_kernel<false><<<P, kFinThreads, 0, st>>>(d_pairs, d_xy, d_norm, d_best, lo, d_inl, cap, w, H, thr2, est.confidence, nullptr);
+      DIMB_LAUNCH_CHECK(ctx);
+    }
+    gv_finalize_kernel<true><<<P, kFinThreads, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap, thr2, d_F, d_mask, d_ninl, cmp, lo);
+    DIMB_LAUNCH_CHECK(ctx);
+    return DIMB_OK;
+  }
+  if (est.kind == 3) {
+    const int H = std::min(est.max_iters, kLoMaxIters);
+    ProfScope prof(ctx, st, "gv.degensac");
+    DIMB_CUDA_OK(ctx, cudaMemsetAsync(lo, 0, P * sizeof(GvLo), st));
+    DIMB_CUDA_OK(ctx, cudaMemsetAsync(deg, 0, P * sizeof(GvDeg), st));
+    gv_prepare_kernel<<<P, 256, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap);
+    DIMB_LAUNCH_CHECK(ctx);
+    for (int w = 0; w * kLoWave < H; ++w) {
+      gv_lo_hypotheses_kernel<true><<<dim3(kLoWave / 128, P), 128, 0, st>>>(d_pairs, d_xy, d_norm, lo, cap, w, H, thr2, deg);
+      DIMB_LAUNCH_CHECK(ctx);
+      gv_pp_kernel<<<P, kFinThreads, 0, st>>>(d_pairs, d_xy, d_norm, lo, deg, d_inl, cap, w, thr2, est.confidence);
+      DIMB_LAUNCH_CHECK(ctx);
+      gv_lo_kernel<true><<<P, kFinThreads, 0, st>>>(d_pairs, d_xy, d_norm, d_best, lo, d_inl, cap, w, H, thr2, est.confidence, deg);
       DIMB_LAUNCH_CHECK(ctx);
     }
     gv_finalize_kernel<true><<<P, kFinThreads, 0, st>>>(d_pairs, d_xy, d_norm, d_best, cap, thr2, d_F, d_mask, d_ninl, cmp, lo);
@@ -586,7 +778,7 @@ int dimb_gv_estimate(dimb_ctx* ctx, const float* kpts0, const float* kpts1, int 
   std::vector<GvPair> hp(1);
   hp[0] = GvPair{d_k0, d_k1, nullptr, nullptr, n, n, seed, {0, 0}, {0, 0}};
   GvLo* d_lo = nullptr;
-  DIMB_TRY(gv_run(ctx, st, hp, n, conf->threshold, GvEstimator{conf->estimator, conf->max_iters, conf->confidence, 52}, d_F, d_mask, d_n,
+  DIMB_TRY(gv_run(ctx, st, hp, n, conf->threshold, GvEstimator{conf->estimator, conf->max_iters, conf->confidence, 52, 56}, d_F, d_mask, d_n,
                   GvCompact{}, 40, &d_lo));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(F, d_F, 9 * sizeof(float), cudaMemcpyDeviceToHost, st));
   DIMB_CUDA_OK(ctx, cudaMemcpyAsync(n_inliers, d_n, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -617,7 +809,7 @@ int dimb_gv_fundamental_batch_dev(dimb_ctx* ctx, int P, const float* const* d_kp
   for (int p = 0; p < P; ++p)
     hp[p] = GvPair{d_kpts0[p], d_kpts1[p], reinterpret_cast<const long long*>(d_matches) + static_cast<size_t>(p) * cap * 2, d_n_matches + p, 0, cap,
                    seed + 0x9E37u * static_cast<unsigned>(p), {0, 0}, {0, 0}};
-  return gv_run(ctx, static_cast<cudaStream_t>(stream), hp, cap, threshold, GvEstimator{0, max_iters, 0.f, 0}, d_F, d_mask, d_n_inliers,
+  return gv_run(ctx, static_cast<cudaStream_t>(stream), hp, cap, threshold, GvEstimator{0, max_iters, 0.f, 0, 0}, d_F, d_mask, d_n_inliers,
                 GvCompact{}, 40);
 }
 
@@ -642,7 +834,7 @@ int dimb_gv_verify_dev(dimb_ctx* ctx, int P, const dimb_feats_dev* f0, const dim
                    {f0[p].round_fp16 ? 1 : 0, f1[p].round_fp16 ? 1 : 0}};
   const GvCompact cmp{reinterpret_cast<long long*>(d_verified), d_n_verified, conf->min_inliers, conf->min_inlier_ratio};
   return gv_run(ctx, static_cast<cudaStream_t>(stream), hp, cap, conf->threshold,
-                GvEstimator{conf->estimator, conf->max_iters, conf->confidence, 54}, d_F, d_mask, d_n_inliers, cmp, 48);
+                GvEstimator{conf->estimator, conf->max_iters, conf->confidence, 54, 57}, d_F, d_mask, d_n_inliers, cmp, 48);
 }
 
 }  // extern "C"

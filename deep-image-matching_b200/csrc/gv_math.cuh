@@ -307,17 +307,37 @@ __host__ __device__ inline int seven_point(const float* k0, const float* k1, con
   return out;
 }
 
-// hypotheses LO-RANSAC must run for `confidence` when the best model explains `best` of n matches: ceil(log(1 - confidence) /
-// log(1 - w^7)), w = best / n; 1 when w = 1, `cap` when w^7 is too small to bound it (and never more than cap)
-__host__ __device__ inline int lo_needed(int best, int n, float confidence, int cap) {
+// F (pixels) in the normalised coordinates, Fn = T1^-T F T0^-1 (the inverse of denormalise, up to scale)
+__host__ __device__ inline void normalise_f(const float F[9], Norm n0, Norm n1, float Fn[9]) {
+  const float i0 = 1.f / n0.s, i1 = 1.f / n1.s;
+  float G[9];  // T1^-T F
+  for (int c = 0; c < 3; ++c) {
+    G[c] = i1 * F[c];
+    G[3 + c] = i1 * F[3 + c];
+    G[6 + c] = n1.cx * F[c] + n1.cy * F[3 + c] + F[6 + c];
+  }
+  for (int r = 0; r < 3; ++r) {  // G T0^-1
+    Fn[3 * r] = i0 * G[3 * r];
+    Fn[3 * r + 1] = i0 * G[3 * r + 1];
+    Fn[3 * r + 2] = n0.cx * G[3 * r] + n0.cy * G[3 * r + 1] + G[3 * r + 2];
+  }
+}
+
+// samples of K points a RANSAC must draw for `confidence` when the best model explains `best` of n candidates: ceil(log(1 -
+// confidence) / log(1 - w^K)), w = best / n; 1 when w = 1, `cap` when w^K is too small to bound it (and never more than cap)
+template <int K>
+__host__ __device__ inline int ransac_needed(int best, int n, float confidence, int cap) {
   if (best >= n) return 1;
-  const double w = static_cast<double>(best) / n, p = pow(w, 7.0);
+  const double w = static_cast<double>(best) / n, p = pow(w, static_cast<double>(K));
   if (!(p > 0.0)) return cap;
   const double den = log(1.0 - p);
   if (!(den < 0.0)) return cap;
   const double need = ceil(log(1.0 - static_cast<double>(confidence)) / den);
   return need < static_cast<double>(cap) ? static_cast<int>(need) : cap;
 }
+
+// hypotheses LO-RANSAC must run: 7-point samples
+__host__ __device__ inline int lo_needed(int best, int n, float confidence, int cap) { return ransac_needed<7>(best, n, confidence, cap); }
 
 // positions in [0, m) of the 16 distinct inliers that inner LO iteration `it` after wave `wave` fits: the counter RNG of the pair's
 // seed on stream numbers 2^31 + 32 wave + it, above every hypothesis index (m >= 16)
@@ -381,6 +401,160 @@ __host__ __device__ inline bool refit_from_normal(float N[9][9], Norm n0, Norm n
   for (int i = 0; i < 9; ++i) f[i] = V[i][k];
   rank2(f);
   return denormalise(f, n0, n1, F);
+}
+
+// ------------------------------------------------------------------ DEGENSAC (Chum, Werner, Matas, CVPR 2005)
+// In the Hartley-normalised coordinates of the 7-point solver; a correspondence c is (x, y, x', y').
+
+// H-inlier threshold of degensac: transfer error |x' - H x| below kDegHFactor * threshold, in image-1 pixels, both in the degeneracy
+// test of a sample and when an H is scored over all matches.  The transfer error carries the noise of both images and the error of an
+// H solved from three noisy points, where the Sampson distance of F carries one first-order residual: twice the F threshold keeps the
+// plane's points together without taking in off-plane points of small parallax.
+constexpr float kDegHFactor = 2.f;
+
+// the squared H-inlier threshold in normalised units of image 1, for the squared F threshold thr2 in pixels
+__host__ __device__ inline float deg_t2n(float thr2, Norm n1) { return kDegHFactor * kDegHFactor * thr2 * n1.s * n1.s; }
+
+// squared transfer error |x' - H x|^2 of a correspondence, in the units of x'; 3.4e38 when H x is at infinity
+__host__ __device__ inline float transfer2(const float H[9], float x0, float y0, float x1, float y1) {
+  const float u = H[0] * x0 + H[1] * y0 + H[2], v = H[3] * x0 + H[4] * y0 + H[5], w = H[6] * x0 + H[7] * y0 + H[8];
+  if (w == 0.f) return 3.4e38f;
+  const float iw = 1.f / w, dx = x1 - u * iw, dy = y1 - v * iw;
+  return dx * dx + dy * dy;
+}
+
+__host__ __device__ inline void cross3(const float a[3], const float b[3], float c[3]) {
+  c[0] = a[1] * b[2] - a[2] * b[1], c[1] = a[2] * b[0] - a[0] * b[2], c[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+// G = [e]_x M (3 x 3, row-major)
+__host__ __device__ inline void skew_times(const float e[3], const float M[9], float G[9]) {
+  for (int c = 0; c < 3; ++c) {
+    G[c] = -e[2] * M[3 + c] + e[1] * M[6 + c];
+    G[3 + c] = e[2] * M[c] - e[0] * M[6 + c];
+    G[6 + c] = -e[1] * M[c] + e[0] * M[3 + c];
+  }
+}
+
+// The homography compatible with F (x'^T F x = 0) that maps three correspondences c[0..2] (Hartley & Zisserman, Result 13.6):
+// H = A - e' (M^-1 b)^T with A = [e']_x F, e' the left null vector of F, M the rows x_i^T and
+// b_i = (x'_i x A x_i)^T (x'_i x e') / |x'_i x e'|^2.  False when it is ill-conditioned: F of rank < 2 (no e'), a point x'_i at the
+// epipole, or three (nearly) collinear x_i.
+__host__ __device__ inline bool h_from_f3(const float F[9], const float c[3][4], float H[9]) {
+  float e[3] = {0.f, 0.f, 0.f}, ee = 0.f, ff = 0.f;
+  for (int k = 0; k < 9; ++k) ff += F[k] * F[k];
+  for (int a = 0; a < 2; ++a)  // e' = the longest cross product of two columns of F (F^T e' = 0)
+    for (int b = a + 1; b < 3; ++b) {
+      const float p[3] = {F[a], F[3 + a], F[6 + a]}, q[3] = {F[b], F[3 + b], F[6 + b]};
+      float x[3];
+      cross3(p, q, x);
+      const float s = x[0] * x[0] + x[1] * x[1] + x[2] * x[2];
+      if (s > ee) ee = s, e[0] = x[0], e[1] = x[1], e[2] = x[2];
+    }
+  if (!(ee > 1e-10f * ff * ff)) return false;
+  const float ie = 1.f / sqrtf(ee);
+  for (int k = 0; k < 3; ++k) e[k] *= ie;
+  float A[9];
+  skew_times(e, F, A);
+  float b[3], x[3][3];
+  for (int i = 0; i < 3; ++i) {
+    x[i][0] = c[i][0], x[i][1] = c[i][1], x[i][2] = 1.f;
+    const float xp[3] = {c[i][2], c[i][3], 1.f};
+    const float ax[3] = {A[0] * x[i][0] + A[1] * x[i][1] + A[2], A[3] * x[i][0] + A[4] * x[i][1] + A[5], A[6] * x[i][0] + A[7] * x[i][1] + A[8]};
+    float p[3], q[3];
+    cross3(xp, ax, p);
+    cross3(xp, e, q);
+    const float qq = q[0] * q[0] + q[1] * q[1] + q[2] * q[2];
+    if (!(qq > 1e-10f * (xp[0] * xp[0] + xp[1] * xp[1] + 1.f))) return false;
+    b[i] = (p[0] * q[0] + p[1] * q[1] + p[2] * q[2]) / qq;
+  }
+  // M^-1 = [x1 x x2 | x2 x x0 | x0 x x1] / det M (columns)
+  float adj[3][3];
+  cross3(x[1], x[2], adj[0]);
+  cross3(x[2], x[0], adj[1]);
+  cross3(x[0], x[1], adj[2]);
+  const float det = x[0][0] * adj[0][0] + x[0][1] * adj[0][1] + x[0][2] * adj[0][2];
+  float nx = 1.f;
+  for (int i = 0; i < 3; ++i) nx *= x[i][0] * x[i][0] + x[i][1] * x[i][1] + 1.f;
+  if (!(det * det > 1e-10f * nx)) return false;
+  const float id = 1.f / det;
+  float v[3];
+  for (int k = 0; k < 3; ++k) v[k] = (b[0] * adj[0][k] + b[1] * adj[1][k] + b[2] * adj[2][k]) * id;
+  for (int r = 0; r < 3; ++r)
+    for (int k = 0; k < 3; ++k) H[3 * r + k] = A[3 * r + k] - e[r] * v[k];
+  return true;
+}
+
+// DEGENSAC's degeneracy test of a 7-point model F of the sample u[0..6]: for each of the five triplets {0,1,2}, {3,4,5}, {0,1,6},
+// {3,4,6}, {2,5,6} (every 5 of the 7 points contain one), H from F and the triplet, and the sample points whose squared transfer error
+// is below t2.  Returns the first triplet whose H maps 5 or more of them (the sample is dominated by a plane; its H in H), -1 if none.
+__host__ __device__ inline int degenerate7(const float F[9], const float u[7][4], float t2, float H[9]) {
+  const int tri[5][3] = {{0, 1, 2}, {3, 4, 5}, {0, 1, 6}, {3, 4, 6}, {2, 5, 6}};
+  for (int t = 0; t < 5; ++t) {
+    float c[3][4], G[9];
+    for (int i = 0; i < 3; ++i)
+      for (int k = 0; k < 4; ++k) c[i][k] = u[tri[t][i]][k];
+    if (!h_from_f3(F, c, G)) continue;
+    int on = 0;
+    for (int j = 0; j < 7; ++j) on += transfer2(G, u[j][0], u[j][1], u[j][2], u[j][3]) < t2;
+    if (on >= 5) {
+      for (int k = 0; k < 9; ++k) H[k] = G[k];
+      return t;
+    }
+  }
+  return -1;
+}
+
+// H in pixels from H in normalised coordinates: T1^-1 Hn T0, scaled to unit Frobenius norm; false for a zero matrix
+__host__ __device__ inline bool h_denormalise(const float h[9], Norm n0, Norm n1, float H[9]) {
+  float G[9];  // Hn T0
+  for (int r = 0; r < 3; ++r) {
+    G[3 * r] = h[3 * r] * n0.s;
+    G[3 * r + 1] = h[3 * r + 1] * n0.s;
+    G[3 * r + 2] = h[3 * r + 2] - n0.s * (h[3 * r] * n0.cx + h[3 * r + 1] * n0.cy);
+  }
+  const float is = 1.f / n1.s;
+  for (int c = 0; c < 3; ++c) {
+    H[c] = G[c] * is + n1.cx * G[6 + c];
+    H[3 + c] = G[3 + c] * is + n1.cy * G[6 + c];
+    H[6 + c] = G[6 + c];
+  }
+  float nrm = 0.f;
+  for (int c = 0; c < 9; ++c) nrm += H[c] * H[c];
+  if (!(nrm > 0.f)) return false;
+  nrm = 1.f / sqrtf(nrm);
+  for (int c = 0; c < 9; ++c) H[c] *= nrm;
+  return true;
+}
+
+// Plane and parallax: F = [e']_x H with e' = (H x_a x x'_a) x (H x_b x x'_b), where the parallax lines of two off-plane
+// correspondences a, b meet; rank 2 by construction.  False when the lines (nearly) coincide or vanish (a point on the plane).
+__host__ __device__ inline bool plane_parallax(const float H[9], const float a[4], const float b[4], float F[9]) {
+  float l[2][3];
+  for (int s = 0; s < 2; ++s) {
+    const float* c = s ? b : a;
+    const float hx[3] = {H[0] * c[0] + H[1] * c[1] + H[2], H[3] * c[0] + H[4] * c[1] + H[5], H[6] * c[0] + H[7] * c[1] + H[8]};
+    const float xp[3] = {c[2], c[3], 1.f};
+    cross3(hx, xp, l[s]);
+  }
+  float e[3];
+  cross3(l[0], l[1], e);
+  const float ee = e[0] * e[0] + e[1] * e[1] + e[2] * e[2];
+  const float l0 = l[0][0] * l[0][0] + l[0][1] * l[0][1] + l[0][2] * l[0][2], l1 = l[1][0] * l[1][0] + l[1][1] * l[1][1] + l[1][2] * l[1][2];
+  if (!(ee > 1e-12f * l0 * l1)) return false;
+  const float ie = 1.f / sqrtf(ee);
+  for (int k = 0; k < 3; ++k) e[k] *= ie;
+  skew_times(e, H, F);
+  return true;
+}
+
+// plane-and-parallax draws per step: at most kPpMax, in chunks of kPpChunk with confidence stopping between chunks
+constexpr int kPpMax = 1024, kPpChunk = 256;
+
+// the positions in [0, m) of plane-and-parallax draw d after wave `wave`: the counter RNG of the pair's seed on stream numbers
+// 3 * 2^30 + 2^16 wave + d, above the 7-point (< 2^16) and local-optimisation (2^31 + 32 wave + it) streams (m >= 2, d < 2^16)
+__host__ __device__ inline void pp_sample2(uint32_t seed, int wave, int d, int m, int pos[2]) {
+  sample_distinct<2>(seed, 0xC0000000u + 65536u * static_cast<uint32_t>(wave) + static_cast<uint32_t>(d), m, pos);
 }
 
 }  // namespace gv

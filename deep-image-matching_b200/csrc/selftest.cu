@@ -13,8 +13,9 @@
 //     (sift_kernels.cuh) through their launch helpers, on caller-given levels, candidates and records;
 //   dimb_selftest_aliked_conv_plan / _conv3x3 / _conv1x1 / _avgpool / _pad / _crop / _deform / _fuse / _dkd / _sddh / _threshold: the
 //     ALIKED stages (aliked_kernels.cuh) through their launch helpers, on caller-given maps, weights and keypoints;
-//   dimb_gv_host / dimb_gv_lo_host / dimb_gv_seven_point_host: the RANSAC arithmetic of gv.cu on the host (ransac8, lo-ransac, the
-//     7-point solver).
+//   dimb_gv_host / dimb_gv_lo_host / dimb_gv_degensac_host / dimb_gv_seven_point_host: the RANSAC arithmetic of gv.cu on the host
+//     (ransac8, lo-ransac, degensac, the 7-point solver); dimb_gv_h_from_f3_host / _degenerate_host / _plane_parallax_host: degensac's
+//     H from F and three points, dominant-plane test and plane-and-parallax F.
 #include <algorithm>
 #include <cstring>
 #include <vector>
@@ -763,6 +764,31 @@ void gv_host_finish(float bf[9], const float* k0, const float* k1, int n, float 
   for (int j = 0; j < 9; ++j) F[j] = bf[j];
   for (int i = 0; i < n; ++i) mask[i] = gv::sampson2(bf, k0[2 * i], k0[2 * i + 1], k1[2 * i], k1[2 * i + 1]) < thr2;
 }
+
+// the local optimisation of gv_lo_kernel on the model bf adopted after wave `wave` with count best (both updated)
+void gv_host_lo(float bf[9], int& best, int wave, unsigned seed, const float* k0, const float* k1, int n, float thr2, const gv::Norm nm[2]) {
+  std::vector<int> in;
+  for (int it = 0; it < 20; ++it) {
+    gv_host_count(bf, k0, k1, n, 4.f * thr2, &in);
+    if (in.size() < 16) break;
+    int pos[16];
+    gv::lo_sample16(seed, wave, it, static_cast<int>(in.size()), pos);
+    std::vector<int> sub(16);
+    for (int k = 0; k < 16; ++k) sub[k] = in[pos[k]];
+    float f[9], g[9];
+    if (!gv_host_lsq(sub, k0, k1, nm, f)) continue;
+    for (int r = 0; r < 4; ++r) {
+      gv_host_count(f, k0, k1, n, thr2, &in);
+      if (!gv_host_lsq(in, k0, k1, nm, g)) break;
+      for (int j = 0; j < 9; ++j) f[j] = g[j];
+    }
+    const int c = gv_host_count(f, k0, k1, n, thr2);
+    if (c > best) {
+      best = c;
+      for (int j = 0; j < 9; ++j) bf[j] = f[j];
+    }
+  }
+}
 }  // namespace
 
 extern "C" int dimb_gv_host(const float* k0, const float* k1, int n, float threshold, int iters, unsigned seed, float* F, unsigned char* mask) {
@@ -801,7 +827,6 @@ extern "C" int dimb_gv_lo_host(const float* k0, const float* k1, int n, float th
   const int H = std::min(max_iters, 65536);
   int best = 0, lim = H, run = 0;
   float bf[9] = {0};
-  std::vector<int> in;
   for (int wave = 0; run < lim; ++wave) {
     int wb = -1;
     float wf[9] = {0};
@@ -823,26 +848,7 @@ extern "C" int dimb_gv_lo_host(const float* k0, const float* k1, int n, float th
     if (wb > best) {
       best = wb;
       for (int j = 0; j < 9; ++j) bf[j] = wf[j];
-      for (int it = 0; it < 20; ++it) {
-        gv_host_count(bf, k0, k1, n, 4.f * thr2, &in);
-        if (in.size() < 16) break;
-        int pos[16];
-        gv::lo_sample16(seed, wave, it, static_cast<int>(in.size()), pos);
-        std::vector<int> sub(16);
-        for (int k = 0; k < 16; ++k) sub[k] = in[pos[k]];
-        float f[9], g[9];
-        if (!gv_host_lsq(sub, k0, k1, nm, f)) continue;
-        for (int r = 0; r < 4; ++r) {
-          gv_host_count(f, k0, k1, n, thr2, &in);
-          if (!gv_host_lsq(in, k0, k1, nm, g)) break;
-          for (int j = 0; j < 9; ++j) f[j] = g[j];
-        }
-        const int c = gv_host_count(f, k0, k1, n, thr2);
-        if (c > best) {
-          best = c;
-          for (int j = 0; j < 9; ++j) bf[j] = f[j];
-        }
-      }
+      gv_host_lo(bf, best, wave, seed, k0, k1, n, thr2, nm);
     }
     lim = std::min(lim, gv::lo_needed(best, n, confidence, H));
   }
@@ -850,6 +856,196 @@ extern "C" int dimb_gv_lo_host(const float* k0, const float* k1, int n, float th
   if (best < 8) return DIMB_ERR_UNSUPPORTED;
   gv_host_finish(bf, k0, k1, n, thr2, nm, F, mask);
   return DIMB_OK;
+}
+
+namespace {
+// correspondence i in the normalised coordinates (x, y, x', y')
+void gv_host_unit(const float* k0, const float* k1, int i, const gv::Norm nm[2], float u[4]) {
+  u[0] = (k0[2 * i] - nm[0].cx) * nm[0].s, u[1] = (k0[2 * i + 1] - nm[0].cy) * nm[0].s;
+  u[2] = (k1[2 * i] - nm[1].cx) * nm[1].s, u[3] = (k1[2 * i + 1] - nm[1].cy) * nm[1].s;
+}
+
+// the matches within the squared transfer error t2 (pixels) of H (pixels)
+int gv_host_count_h(const float* H, const float* k0, const float* k1, int n, float t2, std::vector<int>* outside = nullptr) {
+  int c = 0;
+  if (outside) outside->clear();
+  for (int i = 0; i < n; ++i) {
+    const bool in = gv::transfer2(H, k0[2 * i], k0[2 * i + 1], k1[2 * i], k1[2 * i + 1]) < t2;
+    c += in;
+    if (outside && !in) outside->push_back(i);
+  }
+  return c;
+}
+
+// the plane-and-parallax step of gv_pp_kernel after wave `wave`: the matches outside the plane Hn (normalised) in order, up to
+// gv::kPpMax pairs of them drawn in chunks with confidence stopping on the off-plane inlier fraction, F = [e']_x H of each, the best by
+// Sampson count (lowest draw on ties) into pf.  Returns its count, -1 when fewer than 2 matches are off the plane or no draw gave a model.
+int gv_host_pp(const float Hn[9], int wave, unsigned seed, const float* k0, const float* k1, int n, float thr2, const gv::Norm nm[2],
+               float confidence, float pf[9]) {
+  float Hp[9];
+  if (!gv::h_denormalise(Hn, nm[0], nm[1], Hp)) return -1;
+  std::vector<int> off;
+  gv_host_count_h(Hp, k0, k1, n, gv::kDegHFactor * gv::kDegHFactor * thr2, &off);
+  const int m = static_cast<int>(off.size());
+  if (m < 2) return -1;
+  int bc = -1, need = gv::kPpMax;
+  for (int base = 0; base < need; base += gv::kPpChunk) {
+    for (int d = base; d < base + gv::kPpChunk; ++d) {
+      int pos[2];
+      gv::pp_sample2(seed, wave, d, m, pos);
+      float a[4], b[4], f[9], Fp[9];
+      gv_host_unit(k0, k1, off[pos[0]], nm, a);
+      gv_host_unit(k0, k1, off[pos[1]], nm, b);
+      if (!gv::plane_parallax(Hn, a, b, f) || !gv::denormalise(f, nm[0], nm[1], Fp)) continue;
+      const int c = gv_host_count(Fp, k0, k1, n, thr2);
+      if (c > bc) {
+        bc = c;
+        for (int j = 0; j < 9; ++j) pf[j] = Fp[j];
+      }
+    }
+    need = gv::ransac_needed<2>(std::max(0, bc - (n - m)), m, confidence, gv::kPpMax);
+  }
+  return bc;
+}
+}  // namespace
+
+// degensac of gv.cu in wave order on the host: lo-ransac's waves, where a 7-point model that DEGENSAC's test finds dominated by a plane
+// also has its H scored (matches within gv::kDegHFactor * threshold transfer error; the first such model of a hypothesis, highest
+// count then lowest 3 h + root per wave).  When a wave's best H beats the pair's best H, the plane-and-parallax step runs on it, and
+// its F is adopted (and locally optimised) if it explains at least as many matches as the pair's best and the wave's best 7-point
+// model; otherwise the wave's best model is adopted as in lo-ransac.  Confidence stopping and the finalize step as lo-ransac.
+extern "C" int dimb_gv_degensac_host(const float* k0, const float* k1, int n, float threshold, int max_iters, float confidence, unsigned seed,
+                                     float* F, unsigned char* mask, int* n_hyp) {
+  if (!k0 || !k1 || !F || !mask || !n_hyp || n < 8 || max_iters < 1 || !(confidence > 0.f && confidence < 1.f)) return DIMB_ERR_ARG;
+  constexpr int W = 1024;
+  gv::Norm nm[2];
+  gv_host_norms(k0, k1, n, nm);
+  const float thr2 = threshold * threshold, tH2 = gv::kDegHFactor * gv::kDegHFactor * thr2, t2n = gv::deg_t2n(thr2, nm[1]);
+  const int H = std::min(max_iters, 65536);
+  int best = 0, lim = H, run = 0, hbest = 0;
+  float bf[9] = {0};
+  for (int wave = 0; run < lim; ++wave) {
+    int wb = -1, hb = -1;
+    float wf[9] = {0}, wh[9] = {0};
+    const int end = std::min(lim, (wave + 1) * W);
+    for (int h = wave * W; h < end; ++h) {
+      int idx[7];
+      float M[3][9], Mn[3][9], u[7][4];
+      gv::sample7(seed, h, n, idx);
+      const int m = gv::seven_point(k0, k1, idx, nm[0], nm[1], M);
+      for (int r = 0; r < m; ++r) gv::normalise_f(M[r], nm[0], nm[1], Mn[r]);
+      for (int r = 0; r < m; ++r) {
+        const int c = gv_host_count(M[r], k0, k1, n, thr2);
+        if (c > wb) {
+          wb = c;
+          for (int j = 0; j < 9; ++j) wf[j] = M[r][j];
+        }
+      }
+      for (int k = 0; k < 7; ++k) gv_host_unit(k0, k1, idx[k], nm, u[k]);
+      for (int r = 0; r < m; ++r) {
+        float Hn[9], Hp[9];
+        if (gv::degenerate7(Mn[r], u, t2n, Hn) < 0) continue;
+        if (gv::h_denormalise(Hn, nm[0], nm[1], Hp)) {
+          const int c = gv_host_count_h(Hp, k0, k1, n, tH2);
+          if (c > hb) {
+            hb = c;
+            for (int j = 0; j < 9; ++j) wh[j] = Hn[j];
+          }
+        }
+        break;
+      }
+    }
+    run = end;
+    int pc = -1;
+    float pf[9];
+    if (hb > hbest) {
+      hbest = hb;
+      pc = gv_host_pp(wh, wave, seed, k0, k1, n, thr2, nm, confidence, pf);
+    }
+    const float* adopt = nullptr;
+    if (pc >= 8 && pc >= best && pc >= wb) {
+      best = pc;
+      adopt = pf;
+    } else if (wb > best) {
+      best = wb;
+      adopt = wf;
+    }
+    if (adopt) {
+      for (int j = 0; j < 9; ++j) bf[j] = adopt[j];
+      gv_host_lo(bf, best, wave, seed, k0, k1, n, thr2, nm);
+    }
+    lim = std::min(lim, gv::lo_needed(best, n, confidence, H));
+  }
+  *n_hyp = run;
+  if (best < 8) return DIMB_ERR_UNSUPPORTED;
+  gv_host_finish(bf, k0, k1, n, thr2, nm, F, mask);
+  return DIMB_OK;
+}
+
+namespace {
+void gv_mul3(const double a[9], const double b[9], double c[9]) {
+  for (int r = 0; r < 3; ++r)
+    for (int k = 0; k < 3; ++k) c[3 * r + k] = a[3 * r] * b[k] + a[3 * r + 1] * b[3 + k] + a[3 * r + 2] * b[6 + k];
+}
+
+// L X R for 3 x 3 matrices (X float, in double), into out (float)
+void gv_sandwich(const double L[9], const float* X, const double R[9], float out[9]) {
+  double x[9], t[9], o[9];
+  for (int k = 0; k < 9; ++k) x[k] = X[k];
+  gv_mul3(L, x, t);
+  gv_mul3(t, R, o);
+  for (int k = 0; k < 9; ++k) out[k] = static_cast<float>(o[k]);
+}
+
+// a matrix in pixels in the normalised coordinates: F -> T1^-T F T0^-1 (`fundamental`), H -> T1 H T0^-1, T = the Hartley normalisation
+void gv_host_normalise(const float* X, bool fundamental, const gv::Norm nm[2], float out[9]) {
+  const double s0 = nm[0].s, s1 = nm[1].s;
+  const double T0i[9] = {1 / s0, 0, nm[0].cx, 0, 1 / s0, nm[0].cy, 0, 0, 1};
+  const double T1[9] = {s1, 0, -s1 * nm[1].cx, 0, s1, -s1 * nm[1].cy, 0, 0, 1};
+  const double T1it[9] = {1 / s1, 0, 0, 0, 1 / s1, 0, nm[1].cx, nm[1].cy, 1};
+  gv_sandwich(fundamental ? T1it : T1, X, T0i, out);
+}
+}  // namespace
+
+// gv::h_from_f3 on F (pixels) and the correspondences idx[0..2] of k0[i] <-> k1[i] (n of them, which set the Hartley normalisations as
+// in the estimator): H in pixels (unit norm).  Returns 1, or 0 when h_from_f3 rejects the triplet.
+extern "C" int dimb_gv_h_from_f3_host(const float* F, const float* k0, const float* k1, int n, const int* idx, float* H) {
+  if (!F || !k0 || !k1 || !idx || !H || n < 3) return DIMB_ERR_ARG;
+  gv::Norm nm[2];
+  gv_host_norms(k0, k1, n, nm);
+  float Fn[9], c[3][4], Hn[9];
+  gv_host_normalise(F, true, nm, Fn);
+  for (int i = 0; i < 3; ++i) gv_host_unit(k0, k1, idx[i], nm, c[i]);
+  if (!gv::h_from_f3(Fn, c, Hn)) return 0;
+  return gv::h_denormalise(Hn, nm[0], nm[1], H) ? 1 : 0;
+}
+
+// gv::degenerate7 on the 7-point model F (pixels) of the sample idx[0..6] at the estimator's H threshold (gv::kDegHFactor *
+// threshold): the triplet found (0 .. 4; H in pixels, unit norm) or -1.
+extern "C" int dimb_gv_degenerate_host(const float* F, const float* k0, const float* k1, int n, const int* idx, float threshold, float* H) {
+  if (!F || !k0 || !k1 || !idx || !H || n < 7 || !(threshold > 0.f)) return DIMB_ERR_ARG;
+  gv::Norm nm[2];
+  gv_host_norms(k0, k1, n, nm);
+  float Fn[9], u[7][4], Hn[9];
+  gv_host_normalise(F, true, nm, Fn);
+  for (int k = 0; k < 7; ++k) gv_host_unit(k0, k1, idx[k], nm, u[k]);
+  const int t = gv::degenerate7(Fn, u, gv::deg_t2n(threshold * threshold, nm[1]), Hn);
+  if (t >= 0) gv::h_denormalise(Hn, nm[0], nm[1], H);
+  return t;
+}
+
+// gv::plane_parallax on H (pixels) and the correspondences i, j of k0 <-> k1 (n of them, for the normalisations): F in pixels (unit
+// norm).  Returns 1, or 0 when the parallax lines do not define an epipole.
+extern "C" int dimb_gv_plane_parallax_host(const float* H, const float* k0, const float* k1, int n, int i, int j, float* F) {
+  if (!H || !k0 || !k1 || !F || n < 2 || i < 0 || j < 0 || i >= n || j >= n) return DIMB_ERR_ARG;
+  gv::Norm nm[2];
+  gv_host_norms(k0, k1, n, nm);
+  float Hn[9], a[4], b[4], f[9];
+  gv_host_normalise(H, false, nm, Hn);
+  gv_host_unit(k0, k1, i, nm, a);
+  gv_host_unit(k0, k1, j, nm, b);
+  if (!gv::plane_parallax(Hn, a, b, f)) return 0;
+  return gv::denormalise(f, nm[0], nm[1], F) ? 1 : 0;
 }
 
 // gv::seven_point on 7 correspondences k0[i] <-> k1[i] (pixels) with the Hartley normalisations of those 7 points: the models in

@@ -11,9 +11,14 @@ method name of the reference (PYDEGENSAC, MAGSAC, RANSAC, the OpenCV USAC family
 - ``"lo-ransac"``: 7-point hypotheses in waves of 1024, local optimisation of each wave's new best model and confidence stopping
   (``confidence`` in (0, 1)), up to min(max_iters, 65536) hypotheses - the structure of pydegensac and OpenCV's USAC, which keeps
   the true inliers at outlier ratios where ransac8 loses them.
+- ``"degensac"``: lo-ransac's waves plus DEGENSAC's handling of a dominant plane (Chum, Werner, Matas, CVPR 2005), the core of
+  pydegensac: a 7-point sample with 5 or more points on one plane is detected by five H-from-F-and-3-points tests, its plane's H is
+  scored (transfer error below 2 x threshold), and plane and parallax recovers F = [e']_x H from pairs of off-plane matches (up to
+  1024 per step, with confidence stopping).  It keeps the off-plane inliers (the parallax SfM needs) that the other two lose on
+  façades, floors and aerial views of flat ground, at a higher cost per pair on such scenes.
 
 Like the reference's estimators the result is stochastic in the sense that it depends on the seed; parity is statistical
-(tests/test_geometry.py, tests/test_gv_lo.py).
+(tests/test_geometry.py, tests/test_gv_lo.py, tests/test_gv_degensac.py).
 For image sets, ``gv_seed(seed, pair_id)`` is the seed of each pair, so that a pair's result does not depend on how the pair list is
 batched or sharded (``sharded.ImageSetMatcher(verification=...)``).
 """

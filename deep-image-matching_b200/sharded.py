@@ -200,7 +200,7 @@ def verification_conf(verification) -> dict | None:
     """The ``verification`` argument of ImageSetMatcher with its defaults filled in (None stays None).  Defaults: method
     "pydegensac", threshold 1.0, max_iters 10000, seed 0 (those of geometric_verification), min_inliers_per_pair 15 and
     min_inlier_ratio_per_pair 0.2 (MatcherBase's general defaults), estimator "ransac8" and confidence 0.9999 (read by
-    estimator "lo-ransac" only, as in geometric_verification)."""
+    estimators "lo-ransac" and "degensac" only, as in geometric_verification)."""
     if verification is None:
         return None
     from ._native import gv_estimator
@@ -214,8 +214,8 @@ def verification_conf(verification) -> dict | None:
     conf["method"] = method_name(conf["method"])
     if not float(conf["threshold"]) > 0 or int(conf["min_inliers_per_pair"]) < 0 or not 0 <= float(conf["min_inlier_ratio_per_pair"]) <= 1:
         raise ValueError("verification needs threshold > 0, min_inliers_per_pair >= 0 and 0 <= min_inlier_ratio_per_pair <= 1")
-    if gv_estimator(conf["estimator"]) == 1 and not (0 < float(conf["confidence"]) < 1 and int(conf["max_iters"]) >= 1):
-        raise ValueError("verification with estimator lo-ransac needs 0 < confidence < 1 and max_iters >= 1")
+    if gv_estimator(conf["estimator"]) != 0 and not (0 < float(conf["confidence"]) < 1 and int(conf["max_iters"]) >= 1):
+        raise ValueError(f"verification with estimator {conf['estimator']} needs 0 < confidence < 1 and max_iters >= 1")
     return conf
 
 

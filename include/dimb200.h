@@ -226,11 +226,14 @@ int dimb_fstore_block_dev(dimb_fstore* fs, void** d_base, size_t* slot_bytes, in
 
 /* ------------------------------------------------------------------ geometric verification (fundamental-matrix RANSAC)
  * Replaces the estimator inside geometric_verification (utils/geometric_verification.py:45-179: pydegensac.findFundamentalMatrix /
- * cv2.findFundamentalMat), the step after _match_pairs (matchers/matcher_base.py:298-340).  Two estimators (dimb_gv_conf.estimator),
+ * cv2.findFundamentalMat), the step after _match_pairs (matchers/matcher_base.py:298-340).  Three estimators (dimb_gv_conf.estimator),
  * both with Sampson inliers (threshold in pixels) and two least-squares refits of the final model:
  *   ransac8: max(64, min(max_iters, 8192)) 8-point hypotheses per pair in parallel, no adaptive stopping;
  *   lo-ransac: 7-point hypotheses in waves of 1024, local optimisation of each wave's new best model (inner RANSAC on 16-inlier
- *     least-squares fits, each iterated 4 times) and confidence stopping, up to min(max_iters, 65536) hypotheses.
+ *     least-squares fits, each iterated 4 times) and confidence stopping, up to min(max_iters, 65536) hypotheses;
+ *   degensac: lo-ransac plus DEGENSAC's dominant-plane test of each 7-point model (H from F and three points over five triplets,
+ *     5 of 7 sample points within 2 x threshold transfer error) and plane-and-parallax recovery of F = [e']_x H from up to 1024
+ *     pairs of off-plane matches when a wave finds a better plane; n_hypotheses counts the 7-point hypotheses.
  * Stochastic like the reference's estimators (seeded, reproducible here): parity is statistical.  F row-major, x1^T F x0 = 0; zeros
  * and an all-ones mask when fewer than 8 matches exist or no model is found (the reference returns F = None, mask all True).
  * dimb_gv_fundamental is dimb_gv_estimate with ransac8. */
@@ -245,17 +248,19 @@ int dimb_gv_fundamental_batch_dev(dimb_ctx* ctx, int P, const float* const* d_kp
  * reproducible: a pair's mask, F and count depend on its matches, its seed and the configuration only. */
 typedef struct {
   float threshold;          /* Sampson distance threshold in pixels, > 0 */
-  int max_iters;            /* ransac8: hypotheses per pair = max(64, min(max_iters, 8192)); lo-ransac: at most min(max_iters, 65536) */
+  int max_iters;            /* ransac8: hypotheses per pair = max(64, min(max_iters, 8192)); lo-ransac, degensac: at most
+                               min(max_iters, 65536) */
   int min_inliers;          /* gate: a pair keeps its verified table iff n_inliers >= min_inliers ... */
   float min_inlier_ratio;   /* ... and float(n_inliers) >= min_inlier_ratio * float(n_raw), in [0, 1] (0 / 0: every pair kept) */
-  int estimator;            /* 0: ransac8, 1: lo-ransac (a zero-filled trailing part of the struct means ransac8) */
-  float confidence;         /* lo-ransac only: stop once the best model leaves a chance below 1 - confidence of having missed a
+  int estimator;            /* 0: ransac8, 1: lo-ransac, 3: degensac; 2 and every other value are refused (a zero-filled trailing part of the struct means
+                               ransac8) */
+  float confidence;         /* lo-ransac and degensac only: stop once the best model leaves a chance below 1 - confidence of having missed a
                                better all-inlier 7-point sample, in (0, 1) */
 } dimb_gv_conf;
 /* One pair on host buffers (n,2) float32 with the estimator of `conf` (its gate fields are not read): F [9], mask [n], n_inliers as
  * dimb_gv_fundamental; n_hypotheses (may be NULL): the hypotheses that ran (ransac8: its fixed count; 0 when n < 8).  Equal to
  * dimb_gv_verify_dev on the same points and seed.  DIMB_ERR_ARG, before any CUDA call, for the argument errors of
- * dimb_gv_fundamental, an unknown estimator, and with lo-ransac confidence outside (0, 1) or max_iters < 1. */
+ * dimb_gv_fundamental, an unknown estimator, and with lo-ransac or degensac confidence outside (0, 1) or max_iters < 1. */
 int dimb_gv_estimate(dimb_ctx* ctx, const float* kpts0, const float* kpts1, int n, const dimb_gv_conf* conf, unsigned seed, float* F,
                      unsigned char* mask, int* n_inliers, int* n_hypotheses);
 /* P pairs, asynchronous on `stream`, never synchronises (once its scratch has grown to the call's size).  Keypoints come from
@@ -266,7 +271,7 @@ int dimb_gv_estimate(dimb_ctx* ctx, const float* kpts0, const float* kpts1, int 
  * when the gate rejects the pair; d_F [P][9] (x1^T F x0 = 0, zeros when no model); d_mask [P][cap]; d_n_inliers [P].  Pairs with
  * fewer than 8 raw matches (or no model): mask all ones, F zeros, n_inliers = n_raw, then the gate.  DIMB_ERR_ARG, before any CUDA
  * call, for a NULL ctx / f0 / f1 / seeds / conf / buffer / keypoint pointer, P < 1, cap < 1, threshold <= 0, min_inliers < 0,
- * min_inlier_ratio outside [0, 1], an unknown estimator, and with lo-ransac confidence outside (0, 1) or max_iters < 1. */
+ * min_inlier_ratio outside [0, 1], an unknown estimator, and with lo-ransac or degensac confidence outside (0, 1) or max_iters < 1. */
 int dimb_gv_verify_dev(dimb_ctx* ctx, int P, const dimb_feats_dev* f0, const dimb_feats_dev* f1, const int64_t* d_matches,
                        const int* d_n_matches, int cap, const unsigned* seeds, const dimb_gv_conf* conf, int64_t* d_verified,
                        int* d_n_verified, float* d_F, unsigned char* d_mask, int* d_n_inliers, void* stream);
