@@ -233,8 +233,9 @@ _selftest = None
 def load_selftest_library():
     """libdimb200_selftest.so: the production GEMM template behind a C = A B^T entry, the flash-attention kernels behind an
     attention entry, keypoint detection (simple_nms, compaction, top-k), the SuperPoint head kernels, the matching heads (LightGlue
-    assignment and tail, SuperGlue Sinkhorn), the SIFT stages (extrema, orientation, selection, descriptors) and the ALIKED stages
-    (convolutions, fusion, DKD, SDDH) behind their own entries, and the host drive of the RANSAC arithmetic.
+    assignment and tail, SuperGlue Sinkhorn), the SIFT stages (extrema, orientation, selection, descriptors), the ALIKED stages
+    (convolutions, fusion, DKD, SDDH) and the brute-force NN engine (row statistics, mode logic) behind their own entries, and the
+    host drive of the RANSAC arithmetic.
     Test / tool infrastructure - the product library exports none of it.  Its context is its own (dimb_ctx_create of
     THIS library); never mix handles of the two libraries."""
     global _selftest
@@ -281,6 +282,8 @@ def load_selftest_library():
         lib.dimb_selftest_aliked_dkd.argtypes = [vp, vp, ip, ip, ip, vp, ip, ip, fp, vp, vp, vp]
         lib.dimb_selftest_aliked_sddh.argtypes = [vp, vp, ip, ip, vp, ip, ip] + [vp] * 7 + [fp, vp, vp, vp]
         lib.dimb_selftest_aliked_threshold.argtypes = [vp, vp, ip, vp, fp, fp, vp]
+        lib.dimb_selftest_nn_stats.argtypes = [vp, ip, C.POINTER(FeatsDev), C.POINTER(FeatsDev)] + [ip] * 5 + [fp] + [vp] * 5
+        lib.dimb_selftest_nn_select.argtypes = [vp, ip, fp, ip, ip] + [vp] * 4 + [ip, fp] + [vp] * 3
         lib.dimb_gv_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_uint, vp, vp]
         lib.dimb_gv_lo_host.argtypes = [vp, vp, ip, C.c_float, ip, C.c_float, C.c_uint, vp, vp, C.POINTER(ip)]
         lib.dimb_gv_seven_point_host.argtypes = [vp, vp, vp]
@@ -338,7 +341,7 @@ DET_TAIL = 1024  # elements past the valid ones in every output buffer of the de
 
 class SelfTest:
     """Context of the self-test library (tests/test_gemm_conv_kernel.py, tests/test_attention_kernel.py, tests/test_detect_kernel.py,
-    tests/test_match_heads.py, tests/test_sift_kernels.py, tests/test_aliked_kernels.py)."""
+    tests/test_match_heads.py, tests/test_sift_kernels.py, tests/test_aliked_kernels.py, tests/test_nn_kernels.py)."""
 
     def __init__(self, device: int = 0):
         self.lib = load_selftest_library()
@@ -684,6 +687,38 @@ class SelfTest:
         out, tail = self._run(self.lib.dimb_selftest_aliked_threshold, "selftest_aliked_threshold", {"thr": (np.float32, 1)}, _ptr(score),
                               score.size, None if cc is None else _ptr(cc), float(thr), float(sentinel))
         return out["thr"][0], tail["thr"]
+
+    def nn_stats(self, f0: list, f1: list, D: int, mode: str, split: bool, host_counts: bool, sentinel: float = -777.0) -> dict:
+        """The NN engine's row statistics (dimb_selftest_nn_stats): prep, then top-2 GEMM and merge of both directions, on the device
+        sides f0 / f1 (lists of FeatsDev, as nn_match_batch_dev takes them).  split: three MMAs per product, else one; host_counts:
+        the host-count engine of nn_match_dev (one pair, n_cap rows).  Returns n_live [2P], d1 / d2 / i1 [2P][NPp] (side 2p: the
+        forward rows of pair p, side 2p + 1 its backward rows), plan [2][5] (the top-2 GEMM plan of each direction as gemm_plan gives
+        it), NPp, and '<name>_tail' of every buffer."""
+        P = len(f0)
+        NPp = max(-(-max(f.n_cap for f in list(f0) + list(f1)) // 128) * 128, 128)
+        R = 2 * P * NPp
+        bufs = {"n_live": (np.int32, 2 * P), "d1": (np.float32, R), "d2": (np.float32, R), "i1": (np.int32, R), "plan": (np.int32, 10)}
+        out, tail = self._run(self.lib.dimb_selftest_nn_stats, "selftest_nn_stats", bufs, P, (FeatsDev * P)(*f0), (FeatsDev * P)(*f1),
+                              int(D), NN_MODES[mode], int(bool(split)), int(bool(host_counts)), NPp, float(sentinel))
+        res = {k: out[k].reshape(2 * P, NPp) for k in ("d1", "d2", "i1")}
+        res.update(n_live=out["n_live"], plan=out["plan"].reshape(2, 5), NPp=NPp)
+        res.update({k + "_tail": v for k, v in tail.items() if k != "plan"})
+        return res
+
+    def nn_select(self, mode: str, th: float, n_live, d1: np.ndarray, d2: np.ndarray, i1: np.ndarray, cap: int,
+                  sentinel: float = -777.0) -> dict:
+        """nn_select_kernel (dimb_selftest_nn_select) on planted row statistics: n_live [2P], d1 / d2 / i1 [2P][NPp] as nn_stats
+        returns them.  Returns idx [P][cap][2], dist [P][cap], count [P] (the full count) and '<name>_tail' of each."""
+        d1, d2 = np.ascontiguousarray(d1, np.float32), np.ascontiguousarray(d2, np.float32)
+        i1, nl = np.ascontiguousarray(i1, np.int32), np.ascontiguousarray(n_live, np.int32)
+        S, NPp = d1.shape
+        P = S // 2
+        bufs = {"idx": (np.int64, P * cap * 2), "dist": (np.float32, P * cap), "count": (np.int32, P)}
+        out, tail = self._run(self.lib.dimb_selftest_nn_select, "selftest_nn_select", bufs, NN_MODES[mode], float(th), P, NPp, _ptr(nl),
+                              _ptr(d1), _ptr(d2), _ptr(i1), int(cap), float(sentinel))
+        res = {"idx": out["idx"].reshape(P, cap, 2), "dist": out["dist"].reshape(P, cap), "count": out["count"]}
+        res.update({k + "_tail": v for k, v in tail.items()})
+        return res
 
     def lg_assign(self, sim: np.ndarray, nf, n_orig, layer, indf: np.ndarray, z: np.ndarray, th: float, cap: int,
                   sentinel: float = -777.0) -> dict:

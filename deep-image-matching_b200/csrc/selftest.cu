@@ -13,6 +13,8 @@
 //     (sift_kernels.cuh) through their launch helpers, on caller-given levels, candidates and records;
 //   dimb_selftest_aliked_conv_plan / _conv3x3 / _conv1x1 / _avgpool / _pad / _crop / _deform / _fuse / _dkd / _sddh / _threshold: the
 //     ALIKED stages (aliked_kernels.cuh) through their launch helpers, on caller-given maps, weights and keypoints;
+//   dimb_selftest_nn_stats / _select: the brute-force NN engine (nn_kernels.cuh) through the pieces nn_run calls: prep, top-2 GEMM and
+//     merge of both directions on caller-given device sides, and the mode logic and compaction on planted row statistics;
 //   dimb_gv_host / dimb_gv_lo_host / dimb_gv_degensac_host / dimb_gv_seven_point_host: the RANSAC arithmetic of gv.cu on the host
 //     (ransac8, lo-ransac, degensac, the 7-point solver); dimb_gv_h_from_f3_host / _degenerate_host / _plane_parallax_host: degensac's
 //     H from F and three points, dominant-plane test and plane-and-parallax F.
@@ -1847,4 +1849,108 @@ extern "C" int dimb_selftest_aliked_threshold(dimb_ctx* ctx, const float* score,
   DIMB_TRY(launch_al_threshold(ctx, 0, d_s, HW, d_c, thr, d_o));
   DIMB_TRY(sync_call(ctx, "dimb_selftest_aliked_threshold"));
   return download(ctx, thr_out, d_o, 1 + kDetTail);
+}
+
+// ------------------------------------------------------------------ brute-force NN matcher
+#include "nn_kernels.cuh"
+
+namespace {
+// the engine's sides of P pairs as dimb_nn_match_batch_dev resolves them (descriptors, n, n_cap, desc_ld, f16, round_fp16 read); host:
+// n unused, n_cap rows (the host-count entries).  False for a side the entries refuse.
+bool nn_sides(int P, const dimb_feats_dev* f0, const dimb_feats_dev* f1, bool host, std::vector<NNSideIn>& sides, int& max_cap) {
+  sides.resize(2 * P);
+  max_cap = 0;
+  for (int p = 0; p < P; ++p)
+    for (int sd = 0; sd < 2; ++sd) {
+      const dimb_feats_dev& f = sd ? f1[p] : f0[p];
+      if (!f.descriptors || (!host && !f.n) || f.n_cap < 0 || f.desc_layout != 0 || f.desc_ld < 0) return false;
+      sides[2 * p + sd] = NNSideIn{f.descriptors, host ? nullptr : f.n, f.n_cap, f.desc_ld ? f.desc_ld : f.n_cap, f.f16 ? 1 : 0,
+                                   f.round_fp16 ? 1 : 0};
+      max_cap = std::max(max_cap, f.n_cap);
+    }
+  return true;
+}
+}  // namespace
+
+// The NN engine (nn_kernels.cuh) up to its row statistics: prep, then top-2 GEMM and merge in both directions (whatever the mode, which
+// only decides the sides kornia leaves empty), through the pieces nn_run calls.  f0 / f1 [P]: device sides as dimb_nn_match_batch_dev
+// reads them.  host_counts 1 (P = 1): the host-count engine of dimb_nn_match_dev / dimb_nn_match (EpiNNTop2, n_cap rows, n unused;
+// a pair kornia leaves empty is refused, as those entries return before the engine); 0: device counts (EpiNNTop2Batch).  split: 1 / 0 =
+// three / one MMA per product, whatever the context's precision.  NPp: the caller's row pitch of the outputs, which must be the
+// engine's (the largest n_cap rounded up to 128, at least 128).
+// Outputs hold kDetTail more elements and start as `sentinel` (int buffers: its bit pattern): n_live [2P]; d1 / d2 / i1 [2P][NPp], the
+// merged best and second distance and the argbest of side s's row r at s * NPp + r (the rows of side 2p + 1 are the backward
+// direction).  plan[10]: {resb, sa, sb, smem_bytes, grid} of the top-2 GEMM of each direction, as dimb_selftest_gemm_plan gives it for
+// the row tiles and padded columns of the engine's NNShape (what nn_direction launches; the plan is not read back from the launch).
+extern "C" int dimb_selftest_nn_stats(dimb_ctx* ctx, int P, const dimb_feats_dev* f0, const dimb_feats_dev* f1, int D, int mode, int split,
+                                      int host_counts, int NPp, float sentinel, int* n_live, float* d1, float* d2, int* i1, int* plan) {
+  std::vector<NNSideIn> sides;
+  int max_cap = 0;
+  if (!ctx || !f0 || !f1 || !n_live || !d1 || !d2 || !i1 || !plan || P < 1 || D < 1 || mode < 0 || mode > 3 || split < 0 || split > 1 ||
+      host_counts < 0 || host_counts > 1 || (host_counts && P != 1) || !nn_sides(P, f0, f1, host_counts, sides, max_cap))
+    return DIMB_ERR_ARG;
+  const int hn[2] = {sides[0].n_cap, sides[1].n_cap};
+  if (host_counts && nn_trivially_empty(hn[0], hn[1], mode)) return DIMB_ERR_ARG;
+  const NNShape sh = nn_shape(P, max_cap, host_counts ? hn : nullptr);
+  if (NPp != sh.NPp || static_cast<size_t>(2 * P) * NPp > INT_MAX) return DIMB_ERR_ARG;
+  const int const_b = host_counts ? EpiNNTop2::kConstB : EpiNNTop2Batch::kConstB, num_kb = round_up(D, 64) / 64;
+  for (int d = 0; d < 2; ++d)
+    if (dimb_selftest_gemm_plan(0, kNnBN, split, const_b, num_kb, std::max(sh.P * sh.tps[d], 1), sh.npad[d] / kNnBN, ctx->num_sms,
+                                plan + 5 * d) != DIMB_OK)
+      return DIMB_ERR_ARG;
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  NNWork w;
+  DIMB_TRY(nn_workspace(ctx, sh, D, split != 0, &w));
+  // the outputs replace the workspace's statistics buffers, so that rows the engine must not write keep the sentinel
+  const size_t rows = static_cast<size_t>(2 * P) * NPp;
+  const int isent = sentinel_bits(sentinel);
+  DevTmp t{ctx, {}};
+  DIMB_TRY(t.upload(&w.n_live, std::vector<int>(2 * P + kDetTail, isent)));
+  DIMB_TRY(t.upload(&w.d1, std::vector<float>(rows + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&w.d2, std::vector<float>(rows + kDetTail, sentinel)));
+  DIMB_TRY(t.upload(&w.i1, std::vector<int>(rows + kDetTail, isent)));
+  DIMB_CUDA_OK(ctx, cudaMemcpy(w.sides, sides.data(), sides.size() * sizeof(NNSideIn), cudaMemcpyHostToDevice));
+  nn_prep_kernel<<<dim3(sh.NPp / 32, 2 * P), dim3(32, 8)>>>(w.sides, mode, D, w.Dp, sh.NPp, w.hi, w.lo, w.norm, w.n_live, nullptr);
+  DIMB_CUDA_OK(ctx, cudaGetLastError());
+  for (int d = 0; d < 2; ++d)
+    if (sh.tps[d] > 0) DIMB_TRY(nn_direction(ctx, 0, w, sh, d, split != 0));
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_nn_stats"));
+  DIMB_TRY(download(ctx, n_live, w.n_live, 2 * P + kDetTail));
+  DIMB_TRY(download(ctx, d1, w.d1, rows + kDetTail));
+  DIMB_TRY(download(ctx, d2, w.d2, rows + kDetTail));
+  return download(ctx, i1, w.i1, rows + kDetTail);
+}
+
+// nn_select_kernel, as nn_run launches it, on planted row statistics: n_live [2P] (0..NPp), d1 / d2 / i1 [2P][NPp] (side s's row r at
+// s * NPp + r; only live rows are read, and their i1 must lie in [0, NPp)).  th: the ratio threshold of snn / smnn.  Outputs hold
+// kDetTail more elements and start as `sentinel` (idx: (long long) sentinel, count: its bit pattern): idx [P][cap][2], dist [P][cap],
+// count [P] (the full count; only the first cap rows of a pair are written).
+extern "C" int dimb_selftest_nn_select(dimb_ctx* ctx, int mode, float th, int P, int NPp, const int* n_live, const float* d1, const float* d2,
+                                       const int* i1, int cap, float sentinel, int64_t* idx, float* dist, int* count) {
+  if (!ctx || !n_live || !d1 || !d2 || !i1 || !idx || !dist || !count || mode < 0 || mode > 3 || P < 1 || NPp < 1 || cap < 1 ||
+      static_cast<size_t>(2 * P) * NPp > INT_MAX || static_cast<size_t>(P) * cap * 2 > INT_MAX)
+    return DIMB_ERR_ARG;
+  for (int s = 0; s < 2 * P; ++s) {
+    if (n_live[s] < 0 || n_live[s] > NPp) return DIMB_ERR_ARG;
+    for (int r = 0; r < n_live[s]; ++r)
+      if (i1[static_cast<size_t>(s) * NPp + r] < 0 || i1[static_cast<size_t>(s) * NPp + r] >= NPp) return DIMB_ERR_ARG;
+  }
+  DIMB_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  const size_t rows = static_cast<size_t>(2 * P) * NPp, out = static_cast<size_t>(P) * cap;
+  DevTmp t{ctx, {}};
+  int *d_live, *d_i1, *d_count;
+  float *d_d1, *d_d2, *d_dist;
+  long long* d_idx;
+  DIMB_TRY(t.upload(&d_live, std::vector<int>(n_live, n_live + 2 * P)));
+  DIMB_TRY(t.upload(&d_d1, al_nan_tail(d1, rows)));
+  DIMB_TRY(t.upload(&d_d2, al_nan_tail(d2, rows)));
+  DIMB_TRY(t.upload(&d_i1, std::vector<int>(i1, i1 + rows)));
+  DIMB_TRY(t.upload(&d_idx, std::vector<long long>(2 * out + kDetTail, static_cast<long long>(sentinel))));
+  DIMB_TRY(t.upload(&d_dist, al_sent(out, sentinel)));
+  DIMB_TRY(t.upload(&d_count, std::vector<int>(P + kDetTail, sentinel_bits(sentinel))));
+  nn_select_kernel<<<P, 1024>>>(mode, th, d_live, NPp, d_d1, d_d2, d_i1, d_idx, d_dist, d_count, cap);
+  DIMB_TRY(sync_call(ctx, "dimb_selftest_nn_select"));
+  DIMB_TRY(download(ctx, reinterpret_cast<long long*>(idx), d_idx, 2 * out + kDetTail));
+  DIMB_TRY(download(ctx, dist, d_dist, out + kDetTail));
+  return download(ctx, count, d_count, P + kDetTail);
 }

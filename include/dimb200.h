@@ -174,11 +174,13 @@ enum { DIMB_NN_NN = 0, DIMB_NN_MNN = 1, DIMB_NN_SNN = 2, DIMB_NN_SMNN = 3 };
 /* d0: (D,n0) float32 host (FeaturesDict layout), d1: (D,n1); any descriptor size D >= 1 (zero-padded to a multiple of 64 on
  * device, which changes no distance).  Outputs: idx [cap][2] int64 sorted by column 0, dist [cap] (distance for nn/mnn, ratio
  * for snn/smnn), n = number of matches.  Descriptors that are exactly fp16-representable (everything read back from
- * features.h5 is, extractor_base.py:56-99) are detected on device and take the single-MMA path, which is then exact. */
+ * features.h5 is, extractor_base.py:56-99) are detected on device and take the single-MMA path: its products are then exact and
+ * only the fp32 accumulation rounds, so integer descriptors whose squared norms add up to less than 2^24 (ORB's and SIFT's) get
+ * correctly rounded distances and tables that follow kornia's rules exactly, ties included. */
 int dimb_nn_match(dimb_ctx* ctx, const float* d0, int n0, const float* d1, int n1, int D, int mode, float th,
                   int64_t* idx, float* dist, int* n, int cap);
 /* Same on device pointers, asynchronous on `stream`: d_desc0 / d_desc1 are (D,n) arrays of row pitch ld0 / ld1 elements
- * (0 = dense), float32 (desc_f16 = 0) or float16 (desc_f16 = 1: the layout the device feature store keeps, exact single-MMA
+ * (0 = dense), float32 (desc_f16 = 0) or float16 (desc_f16 = 1: the layout the device feature store keeps, single-MMA
  * path); d_idx [cap][2] int64, d_dist [cap], d_n [1] are device buffers.  The sequential-pair workload of
  * pairs_generator.py:22-34 keeps every image's descriptors in HBM and calls this once per pair. */
 int dimb_nn_match_dev(dimb_ctx* ctx, const void* d_desc0, int n0, int ld0, const void* d_desc1, int n1, int ld1, int D, int desc_f16,
@@ -188,7 +190,7 @@ int dimb_nn_match_dev(dimb_ctx* ctx, const void* d_desc0, int n0, int ld0, const
  * d_idx [P][cap][2] int64, d_dist [P][cap] (distance for nn / mnn, ratio for snn / smnn), d_n [P] = the full count (only the first
  * cap rows are written), in the order and with the empty-input rules of dimb_nn_match (kornia's).  round_fp16 = 1 rounds float32
  * descriptors to fp16 first (round to nearest even, the features.h5 cast).  Three MMAs per product (EXACT) only when some side is
- * float32 without round_fp16; fp16 inputs are exact with one.  Results per pair do not depend on the other pairs of the call.
+ * float32 without round_fp16; fp16 inputs need one (exact products).  Results per pair do not depend on the other pairs of the call.
  * dimb_nn_match_dev and dimb_nn_match run this engine with P = 1.  DIMB_ERR_ARG, before any CUDA call, for a NULL ctx / array /
  * output / descriptors / n, P < 1, cap < 1, D < 1, mode outside 0..3, n_cap < 0 or desc_layout != 0.
  * Scratch (context slots, grow-only), NPp = the largest n_cap rounded up to 128, Dp = D rounded up to 64: the fp16 operands
